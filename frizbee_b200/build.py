@@ -13,7 +13,7 @@ SOURCES = ["pack.cu", "prefilter.cu", "sw.cu", "sort.cu", "unicode.cu", "host.cu
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr"]
-# A/B hook (compile-time, the default binary is untouched): extra -D flags from the environment, e.g. FRZ_NVCC_DEFINES="FRZ_SW64_SMEM=1"
+# A/B hook (compile-time, the default binary is untouched): extra -D flags from the environment, e.g. FRZ_NVCC_DEFINES="NAME=1"
 # (force a rebuild: `python frizbee_b200/build.py --force`); `--variant NAME --define D` builds libfrz_cuda_NAME.so beside the default
 FLAGS += ["-D" + d for d in os.environ.get("FRZ_NVCC_DEFINES", "").split()]
 

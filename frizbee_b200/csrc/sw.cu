@@ -33,7 +33,8 @@
 namespace {
 
 using namespace frzsw;
-constexpr int kSw64MinBlocks = kSw64RowsInSmem ? 3 : 2;
+template <int LANES, bool WRAP8>
+constexpr int kSw64MinBlocks = kSw64RowsInSmem<LANES, WRAP8> ? 3 : 2;
 
 struct FrzRankView {
     const uint64_t* tile_out_base;
@@ -146,7 +147,7 @@ __global__ void __launch_bounds__(kSwThreads) k_sw(const FrzCorpusView cv, const
 // kernel.  A work item is 32 consecutive survivors of one class; warps claim items from a device counter, so
 // the load balances itself and the only tail is the last item of each warp.
 //
-// The kernel is issue-bound with two warps per scheduler, so every exposed load latency costs: the loop is
+// The kernel is issue-bound (three warps per scheduler for LANES 64), so every exposed load latency costs: the loop is
 // software-pipelined two items deep.  While item i is being scored, item i+1's window units travel
 // global → shared with cp.async (no registers held) and item i+2's records are in flight.
 constexpr int kSw64Units = 5;  // 16-byte units a <= 64-byte window can straddle
@@ -155,12 +156,12 @@ struct Sw64Stage {
 };
 
 template <int LANES, bool WRAP8, int VAR = 0>
-__global__ void __launch_bounds__(kSwThreads, kSw64MinBlocks) k_sw64(const FrzCorpusView cv, const __grid_constant__ FrzPatternDev pat,
+__global__ void __launch_bounds__(kSwThreads, (kSw64MinBlocks<LANES, WRAP8>)) k_sw64(const FrzCorpusView cv, const __grid_constant__ FrzPatternDev pat,
                                                      const FrzSurvLists lists, unsigned long long surv_cap,
                                                      const FrzRankView rv, FrzCounters* __restrict__ ctr,
                                                      uint32_t index_offset, int reversed, FrzMatchDev* __restrict__ out) {
     __shared__ Sw64Stage stage;
-    __shared__ uint32_t rows_smem[kSw64RowsInSmem ? 2 * 32 * kSwThreads : 1];
+    __shared__ __align__(16) uint32_t rows_smem[kSw64RowsInSmem<LANES, WRAP8> ? 2 * 32 * kSwThreads : 1];
     const uint32_t lane = frz_lane();
     unsigned long long cnt[4];
     uint32_t items_end[4];   // cumulative item counts in processing order CC64, CC56, CC48, CC40
@@ -432,16 +433,14 @@ frz_status launch_sw_lanes(const FrzCorpusView& cv, const FrzPatternDev& pat, ui
                            FrzWorkspace& ws, FrzMatchDev* d_out, cudaStream_t stream) {
     // persistent grids: a multiple of the SM count
     const int blocks = frz_sm_count() * 2;
-    const int blocks64 = frz_sm_count() * kSw64MinBlocks;
     const int rev = reversed ? 1 : 0;
-    if (LANES == 64 && !pat.wrap8) {
-        // VAR 8: the per-column bonus is classified on the packed window bytes (SwCore) rather than per 16-bit lane
-        k_sw64<64, false, 8><<<blocks64, kSwThreads, 0, stream>>>(cv, pat, ws.lists(), ws.survivor_cap, rank_view(ws), ws.counters,
-                                                                  index_offset, rev, d_out);
-    } else if (pat.wrap8)
-        k_sw64<LANES, true><<<blocks64, kSwThreads, 0, stream>>>(cv, pat, ws.lists(), ws.survivor_cap, rank_view(ws), ws.counters, index_offset, rev, d_out);
+    // VAR 8: the per-column bonus is classified on the packed window bytes (SwCore) rather than per 16-bit lane
+    if (pat.wrap8)
+        k_sw64<LANES, true><<<frz_sm_count() * kSw64MinBlocks<LANES, true>, kSwThreads, 0, stream>>>(
+            cv, pat, ws.lists(), ws.survivor_cap, rank_view(ws), ws.counters, index_offset, rev, d_out);
     else
-        k_sw64<LANES, false, 8><<<blocks64, kSwThreads, 0, stream>>>(cv, pat, ws.lists(), ws.survivor_cap, rank_view(ws), ws.counters, index_offset, rev, d_out);
+        k_sw64<LANES, false, 8><<<frz_sm_count() * kSw64MinBlocks<LANES, false>, kSwThreads, 0, stream>>>(
+            cv, pat, ws.lists(), ws.survivor_cap, rank_view(ws), ws.counters, index_offset, rev, d_out);
     // windows of 65..128 bytes only exist when some haystack of the corpus is longer than 64 bytes (recorded at pack time)
     if (cv.max_gunits <= 4) { FRZ_CUDA_TRY(cudaGetLastError()); return FRZ_OK; }
     const size_t smem = SwCore<LANES, 128, false>::smem_bytes;

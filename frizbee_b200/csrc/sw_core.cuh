@@ -51,10 +51,10 @@ inline uint32_t __funnelshift_r(uint32_t lo, uint32_t hi, uint32_t sh) { return 
 namespace frzsw {
 
 constexpr int kSwThreads = 128;
-#ifndef FRZ_SW64_SMEM
-#define FRZ_SW64_SMEM 0
-#endif
-constexpr bool kSw64RowsInSmem = FRZ_SW64_SMEM != 0;  // <= 64-byte windows: haystack/bonus rows in shared memory, 3 blocks per SM
+// The non-wrapping 64-lane kernel for <= 64-byte windows keeps the haystack/bonus rows in shared memory: that brings it
+// to <= 168 registers, i.e. 3 blocks (3 warps per scheduler) per SM.
+template <int LANES, bool WRAP8>
+constexpr bool kSw64RowsInSmem = LANES == 64 && !WRAP8;
 
 FRZ_SW_FN uint32_t splat16(int v) { return ((uint32_t)v & 0xffffu) * 0x00010001u; }
 
@@ -114,6 +114,27 @@ struct RowStore<R, true> {
     FRZ_SW_FN void set(int r, uint32_t x) { base[r * kSwThreads] = x; }
 };
 
+// The haystack lanes and the bonus row of one window, read together by every row of the recurrence.  PAIR: both in
+// shared memory, interleaved per register [r][thread]{h, b}, so that a row reads each register's pair with one LDS.64.
+template <int R, bool SMEM, bool PAIR>
+struct HayRows {
+    RowStore<R, SMEM> h, b;
+    FRZ_SW_FN HayRows(uint32_t* s) : h(s), b(s + R * kSwThreads) {}
+    FRZ_SW_FN uint32_t get_h(int r) const { return h.get(r); }
+    FRZ_SW_FN void set_h(int r, uint32_t x) { h.set(r, x); }
+    FRZ_SW_FN void set_b(int r, uint32_t x) { b.set(r, x); }
+    FRZ_SW_FN uint2 get(int r) const { return make_uint2(h.get(r), b.get(r)); }
+};
+template <int R, bool SMEM>
+struct HayRows<R, SMEM, true> {
+    uint2* base;
+    FRZ_SW_FN HayRows(uint32_t* s) : base(reinterpret_cast<uint2*>(s) + FRZ_SW_TID) {}
+    FRZ_SW_FN uint32_t get_h(int r) const { return base[r * kSwThreads].x; }
+    FRZ_SW_FN void set_h(int r, uint32_t x) { base[r * kSwThreads].x = x; }
+    FRZ_SW_FN void set_b(int r, uint32_t x) { base[r * kSwThreads].y = x; }
+    FRZ_SW_FN uint2 get(int r) const { return base[r * kSwThreads]; }
+};
+
 // VAR bit 3 (8): the per-column bonus is classified on the packed bytes (4 at a time) instead of per 16-bit lane — the
 // default of the non-wrapping 64-lane kernel.  Forms that were tried and removed because they were slower: one-lane
 // shifts as IMAD.HI + IMAD pairs instead of PRMT, the shifted match mask folded into the gap penalty with IMAD.HI, two
@@ -130,18 +151,55 @@ struct SwCore {
     static constexpr int R = CC / 2;       // registers per row
     static constexpr int RL = LANES / 2;   // registers per chunk
     static constexpr int NCH = (CC + LANES - 1) / LANES;
-    static constexpr bool SMEM = COLS > 64 || kSw64RowsInSmem;
+    static constexpr bool SMEM = COLS > 64 || kSw64RowsInSmem<LANES, WRAP8>;
+    static constexpr bool PAIR = COLS <= 64 && SMEM;
     static constexpr size_t smem_bytes = SMEM ? 2 * R * kSwThreads * sizeof(uint32_t) : 0;
+
+    // ---- diagonal + up of needle row i at register r, in place (H[r-1] must still hold row i-1).  up: the needle byte
+    // is an uppercase letter (rare), whose exact-case bonus moves from the non-upper to the upper haystack bytes.
+    static FRZ_SW_FN void diag_up(uint32_t (&H)[R], uint32_t (&M)[R], int r, uint2 hb, const FrzPatternDev& p, int i, bool up_row) {
+        const uint32_t om16 = p.om16[i], tg16 = p.tg16[i];
+        const uint32_t hv = hb.x, Bv = hb.y;
+        if (!WRAP8) {
+            // nm: 0 where the haystack byte matches needle[i] (either case), else 1
+            const uint32_t nm = __vminu2((hv | om16) ^ tg16, 0x00010001u);
+            const uint32_t nmfull = nm * 0xFFFFu;
+            const uint32_t prevs = r > 0 ? __byte_perm(H[r - 1], H[r], 0x5432) : __byte_perm(0u, H[0], 0x5432);
+            uint32_t Dv = Bv;
+            if (up_row) {
+                const uint32_t t = __vadd2(hv, splat16(-'A')), d = __vadd2(hv, splat16(-('Z' + 1)));
+                const uint32_t up = __byte_perm(d & ~t, 0, 0x3311);
+                Dv = __vadd2(Dv, sel(up, p.k_case, splat16(-p.case_bonus)));
+            }
+            // no ReLU here: max(H + upd, diag, 0) below clamps anyway, and VIADDMNMX has no zero operand, so the ReLU
+            // form costs a register holding zero (or a PRMT rematerialising one per use)
+            const uint32_t diag = __vadd2(prevs, sel(nmfull, p.k_neg_mis, Dv));
+            const uint32_t upd = p.k_up_open + M[r] * (uint32_t)p.gap_open_x;   // M[r] still row i-1
+            H[r] = addmax_relu(H[r], upd, diag);
+            M[r] = nm;
+        } else {
+            const bool folded = p.om[i] != 0;  // case-insensitive letter: exact-case mask differs from match mask
+            const uint32_t mmn = eqmask16((hv | om16) ^ tg16);
+            const uint32_t prevs = r > 0 ? __byte_perm(H[r - 1], H[r], 0x5432) : __byte_perm(0u, H[0], 0x5432);
+            const uint32_t ex = folded ? eqmask16(hv ^ p.c16[i]) : mmn;
+            uint32_t d = __vadd2(prevs, mmn & Bv) & 0x00FF00FFu;        // wrapping u8 add
+            d = addmax_relu(d, p.k_neg_mis, 0u);                         // saturating sub
+            const uint32_t diag = __vadd2(d, ex & p.k_case) & 0x00FF00FFu;  // wrapping u8 add
+            const uint32_t upd = sel(M[r], p.k_up_open, p.k_up_plain);       // M[r] still row i-1
+            H[r] = addmax_relu(H[r], upd, diag);
+            M[r] = mmn;
+        }
+    }
 
     // hw: CC/4 words of window bytes, zero beyond W
     static FRZ_SW_FN uint32_t run(const uint32_t (&hw)[CC / 4], int W, const FrzPatternDev& p, bool include_prefix,
                                    uint32_t* smem) {
-        RowStore<R, SMEM> h16s(smem), Bs(smem + R * kSwThreads);
+        HayRows<R, SMEM, PAIR> rows(smem);
         // expand bytes to one per 16-bit lane
 #pragma unroll
         for (int i = 0; i < CC / 4; i++) {
-            h16s.set(2 * i, __byte_perm(hw[i], 0, 0x4140));
-            h16s.set(2 * i + 1, __byte_perm(hw[i], 0, 0x4342));
+            rows.set_h(2 * i, __byte_perm(hw[i], 0, 0x4140));
+            rows.set_h(2 * i + 1, __byte_perm(hw[i], 0, 0x4342));
         }
         // ---- per-column bonus (ascii.rs:64-101) ----
         if ((VAR & 8) && !WRAP8) {
@@ -173,7 +231,7 @@ struct SwCore {
                     uint32_t bonus = __vadd2(__vadd2(del_m & delb, cap_m & capb), base2);
                     if (k == 0 && h == 0 && include_prefix) bonus = __vadd2(bonus, (uint32_t)p.prefix_bonus & 0xffffu);
                     bonus = __vadd2(bonus, ~up_m & p.k_case);
-                    Bs.set(2 * k + h, bonus);
+                    rows.set_b(2 * k + h, bonus);
                 }
             }
         } else {
@@ -181,7 +239,7 @@ struct SwCore {
             uint32_t prev_lower = 0, prev_delim = 0;  // masks of the previous register
 #pragma unroll
             for (int r = 0; r < R; r++) {
-                const uint32_t b = h16s.get(r);
+                const uint32_t b = rows.get_h(r);
                 // range tests on lanes in 0..255:  lo <= b <= hi  ⇔  (b-lo) >= 0 && (b-hi-1) < 0
                 auto in_range = [&](int lo, int hi) {
                     uint32_t t = __vadd2(b, splat16(-lo));
@@ -205,16 +263,11 @@ struct SwCore {
                 // ⇔ match && !upper(hay) (a lowercase letter matches {c, C}; a non-letter matches only itself),
                 // so a matched cell's whole diagonal increment is D and the row needs no exact-case mask.
                 if (!WRAP8) bonus = __vadd2(__vadd2(bonus, p.k_neg_mis), ~upper & p.k_case);
-                Bs.set(r, bonus);
+                rows.set_b(r, bonus);
                 prev_lower = lower;
                 prev_delim = delim;
             }
         }
-        // ---- constants ----
-        const uint32_t neg_mis = p.k_neg_mis;
-        const uint32_t up_plain = p.k_up_plain;
-        const uint32_t up_open = p.k_up_open;
-        (void)up_open;
         uint32_t H[R], M[R];
 #pragma unroll
         for (int r = 0; r < R; r++) { H[r] = 0; M[r] = WRAP8 ? 0u : 0x00010001u; }  // row 0: no matches
@@ -225,39 +278,17 @@ struct SwCore {
         // "penalty = base - mask * gap_open" is one IMAD, and lane shifts use IMAD / IMAD.HI too.
         const uint32_t gopx = (uint32_t)p.gap_open_x;
         for (int i = 0; i < p.n; i++) {
-            const uint32_t om16 = p.om16[i], tg16 = p.tg16[i], c16 = p.c16[i];
-            const bool folded = p.om[i] != 0;  // case-insensitive letter: exact-case mask differs from match mask
             const bool upper_row = (uint32_t)(p.c[i] - 'A') <= 25u;  // exact case ⇔ match && upper(hay)
-            // ---- diagonal + up, in place, high register first (H[r-1] must still hold row i-1) ----
-#pragma unroll
-            for (int r = R - 1; r >= 0; r--) {
-                const uint32_t hv = h16s.get(r), Bv = Bs.get(r);
-                if (!WRAP8) {
-                    // nm: 0 where the haystack byte matches needle[i] (either case), else 1
-                    const uint32_t nm = __vminu2((hv | om16) ^ tg16, 0x00010001u);
-                    const uint32_t nmfull = nm * 0xFFFFu;
-                    const uint32_t prevs = r > 0 ? __byte_perm(H[r - 1], H[r], 0x5432) : __byte_perm(0u, H[0], 0x5432);
-                    uint32_t Dv = Bv;
-                    if (upper_row) {  // rare: move the exact-case bonus from the non-upper to the upper haystack bytes
-                        const uint32_t t = __vadd2(hv, splat16(-'A')), d = __vadd2(hv, splat16(-('Z' + 1)));
-                        const uint32_t up = __byte_perm(d & ~t, 0, 0x3311);
-                        Dv = __vadd2(Dv, sel(up, p.k_case, splat16(-p.case_bonus)));
-                    }
-                    const uint32_t diag = addmax_relu(prevs, sel(nmfull, neg_mis, Dv), 0u);
-                    const uint32_t upd = up_open + M[r] * gopx;                      // M[r] still row i-1
-                    H[r] = addmax_relu(H[r], upd, diag);
-                    M[r] = nm;
-                } else {
-                    const uint32_t mmn = eqmask16((hv | om16) ^ tg16);
-                    const uint32_t prevs = r > 0 ? __byte_perm(H[r - 1], H[r], 0x5432) : __byte_perm(0u, H[0], 0x5432);
-                    const uint32_t ex = folded ? eqmask16(hv ^ c16) : mmn;
-                    uint32_t d = __vadd2(prevs, mmn & Bv) & 0x00FF00FFu;        // wrapping u8 add
-                    d = addmax_relu(d, neg_mis, 0u);                             // saturating sub
-                    const uint32_t diag = __vadd2(d, ex & p.k_case) & 0x00FF00FFu;  // wrapping u8 add
-                    const uint32_t upd = sel(M[r], up_open, up_plain);               // M[r] still row i-1
-                    H[r] = addmax_relu(H[r], upd, diag);
-                    M[r] = mmn;
-                }
+            // ---- diagonal + up, in place, high register first.  <= 64 columns: one branch per row picks one of two
+            // bodies, so the common one has no per-register test (the 128-column variant keeps the test: two bodies
+            // make it spill).  The unroll count is explicit because a plain `#pragma unroll` leaves the rare copy
+            // rolled, which puts H[] in local memory.
+            if (COLS <= 64 && !WRAP8 && upper_row) {
+#pragma unroll R
+                for (int r = R - 1; r >= 0; r--) diag_up(H, M, r, rows.get(r), p, i, true);
+            } else {
+#pragma unroll R
+                for (int r = R - 1; r >= 0; r--) diag_up(H, M, r, rows.get(r), p, i, COLS > 64 && !WRAP8 && upper_row);
             }
             // ---- horizontal gap propagation, chunk by chunk (ascii_gap.rs gap_step!) ----
 #pragma unroll
