@@ -29,6 +29,7 @@
 
 #include "frz_host.h"
 #include "sw_core.cuh"
+#include "sw_generic.cuh"
 
 namespace {
 
@@ -107,7 +108,7 @@ __device__ __forceinline__ uint32_t score_window(const FrzPatternDev& pat, const
 }
 
 // Same, loading the units straight from the packed corpus.
-template <int LANES, int COLS, bool WRAP8, int CC>
+template <int LANES, int COLS, bool WRAP8, int CC, int VAR = 0>
 __device__ __forceinline__ uint32_t score_survivor(const FrzCorpusView& cv, const FrzPatternDev& pat, const FrzSurvivor& rec,
                                                    const FrzRankView& rv, const FrzCounters* __restrict__ ctr, uint32_t index_offset,
                                                    int reversed, FrzMatchDev* __restrict__ out, uint32_t* sw_smem) {
@@ -121,12 +122,12 @@ __device__ __forceinline__ uint32_t score_survivor(const FrzCorpusView& cv, cons
         u[k] = make_uint4(0, 0, 0, 0);
         if (k < nu) u[k] = __ldg(base + k);
     }
-    return score_window<LANES, COLS, WRAP8, CC>(pat, rec, wr, u, rv, ctr, index_offset, reversed, out, sw_smem);
+    return score_window<LANES, COLS, WRAP8, CC, VAR>(pat, rec, wr, u, rv, ctr, index_offset, reversed, out, sw_smem);
 }
 
 // Windows of 65..128 bytes: one window per thread, score rows in shared memory, survivors strided over a
 // persistent grid.
-template <int LANES, int COLS, bool WRAP8>
+template <int LANES, int COLS, bool WRAP8, int VAR = 0>
 __global__ void __launch_bounds__(kSwThreads) k_sw(const FrzCorpusView cv, const __grid_constant__ FrzPatternDev pat,
                                                    const FrzSurvivor* __restrict__ surv, unsigned long long surv_cap, int cls,
                                                    const FrzRankView rv, FrzCounters* __restrict__ ctr,
@@ -137,7 +138,7 @@ __global__ void __launch_bounds__(kSwThreads) k_sw(const FrzCorpusView cv, const
     for (unsigned long long j = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; j < count;
          j += (unsigned long long)gridDim.x * blockDim.x) {
         const FrzSurvivor rec = surv[j];
-        local_max = max(local_max, score_survivor<LANES, COLS, WRAP8, COLS>(cv, pat, rec, rv, ctr, index_offset, reversed, out, sw_smem));
+        local_max = max(local_max, score_survivor<LANES, COLS, WRAP8, COLS, VAR>(cv, pat, rec, rv, ctr, index_offset, reversed, out, sw_smem));
     }
     local_max = __reduce_max_sync(0xffffffffu, local_max);
     if (frz_lane() == 0 && local_max) atomicMax(&ctr->max_score, local_max);
@@ -267,67 +268,23 @@ __global__ void __launch_bounds__(kSwThreads, (kSw64MinBlocks<LANES, WRAP8>)) k_
     if (lane == 0 && local_max) atomicMax(&ctr->max_score, local_max);
 }
 
-// ---- generic fallback: windows of 129..1024 bytes (row-major, local-memory rows) and the
-// ---- greedy scorer for windows > 1024 (src/smith_waterman/greedy.rs:7-91).  One window per thread.
-constexpr int kGenCols = FRZ_SW_MAX_WINDOW + 64;
-
+// ---- generic fallback: windows of 129..1024 bytes (row-major, local-memory rows) and the greedy scorer for
+// ---- windows > 1024 (sw_generic.cuh).  One window per thread.
 __device__ __forceinline__ uint32_t hay_byte(const uint4* base, uint32_t i) {
     return (reinterpret_cast<const uint32_t*>(base)[i >> 2] >> ((i & 3) * 8)) & 0xff;
 }
-
-__device__ int greedy_score(const uint4* base, uint32_t start, int W, const FrzPatternDev& p, bool include_prefix) {
-    const int n = p.n;
-    if (n > W) return -1;
-    auto sat_add = [](uint32_t a, uint32_t b) { uint32_t r = a + b; return r > 0xffffu ? 0xffffu : r; };
-    auto sat_sub = [](uint32_t a, uint32_t b) { return a > b ? a - b : 0u; };
-    uint32_t score = 0;
-    int hi = 0;
-    bool delim_enabled = false, prev_lower = false, prev_delim = false;
-    for (int ni = 0; ni < n; ni++) {
-        const int hstart = hi;
-        bool matched = false;
-        while (hi <= W - n + ni) {
-            const uint32_t hc = hay_byte(base, start + hi);
-            const bool is_digit = hc - '0' <= 9u, is_upper = hc - 'A' <= 25u, is_lower = hc - 'a' <= 25u;
-            const bool is_delim = hc < 128 && !(is_lower || is_upper || is_digit);
-            if (!is_delim) delim_enabled = true;
-            if (p.c[ni] != hc && p.flip[ni] != hc) {
-                prev_delim = delim_enabled && is_delim;
-                prev_lower = is_lower;
-                hi++;
-                continue;
-            }
-            score = sat_add(score, p.raw_match);
-            if (hi != hstart && ni != 0) {
-                uint32_t gl = (uint32_t)(hi - hstart);
-                gl = gl > 0 ? gl - 1 : 0;
-                if (gl > 0xffffu) gl = 0xffffu;
-                uint32_t mul = (uint32_t)p.raw_gap_extend * gl;
-                if (mul > 0xffffu) mul = 0xffffu;
-                score = sat_sub(score, sat_add(p.raw_gap_open, mul));
-            }
-            if (p.c[ni] == hc) score = sat_add(score, p.raw_case);
-            if (is_upper && prev_lower) score = sat_add(score, p.raw_cap);
-            if (include_prefix && hi == 0) score = sat_add(score, p.raw_prefix);
-            if (prev_delim && !is_delim) score = sat_add(score, p.raw_delim);
-            prev_delim = delim_enabled && is_delim;
-            prev_lower = is_lower;
-            hi++;
-            matched = true;
-            break;
-        }
-        if (!matched) return -1;
-    }
-    return (int)score;
-}
+// byte i of the window that starts at byte `start` of the haystack at `base`
+struct GenericHay {
+    const uint4* base;
+    uint32_t start;
+    __device__ __forceinline__ uint32_t operator()(int i) const { return hay_byte(base, start + i); }
+};
 
 __global__ void __launch_bounds__(64) k_sw_generic(const FrzCorpusView cv, const __grid_constant__ FrzPatternDev pat,
                                                    const FrzSurvivor* __restrict__ surv, unsigned long long surv_cap, int cls,
                                                    const FrzRankView rv, FrzCounters* __restrict__ ctr,
                                                    uint32_t index_offset, int reversed, FrzMatchDev* __restrict__ out) {
     const unsigned long long count = min(ctr->class_count[cls], surv_cap);
-    const int L = pat.sw_lanes;
-    const uint32_t lane_mask = pat.score_bits == 8 ? 0xffu : 0xffffu;  // real element width
     uint32_t local_max = 0;
     for (unsigned long long j = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; j < count;
          j += (unsigned long long)gridDim.x * blockDim.x) {
@@ -338,68 +295,13 @@ __global__ void __launch_bounds__(64) k_sw_generic(const FrzCorpusView cv, const
         const int W = (int)(end - start);
         const uint4* base = frz_unit_ptr(cv, rec.tile, slot, 0);
         const bool include_prefix = start == 0;
+        const GenericHay hay{base, start};
         uint32_t score;
         if (W > FRZ_SW_MAX_WINDOW) {
-            int g = greedy_score(base, start, W, pat, include_prefix);
+            int g = greedy_score(hay, W, pat, include_prefix);
             score = g < 0 ? 0u : (uint32_t)g;
         } else {
-            // literal row-major restatement with true element-width arithmetic
-            uint16_t Hp[kGenCols], Hc[kGenCols], bon[kGenCols];
-            uint8_t Mp[kGenCols], Mc[kGenCols], hb[kGenCols];
-            const int nch = (W + L - 1) / L, cols = nch * L;
-            bool pl = false, pd = false;
-            for (int c = 0; c < cols; c++) {
-                uint32_t b = c < W ? hay_byte(base, start + c) : 0;
-                hb[c] = (uint8_t)b;
-                bool up = b - 'A' <= 25u, lo = b - 'a' <= 25u, dg = b - '0' <= 9u;
-                bool dl = !(up || lo || dg || b > 127);
-                // wrapping adds in the element width (ascii.rs:98-101)
-                uint32_t bo = 0;
-                if (pd && !dl) bo = (bo + pat.delim_bonus) & lane_mask;
-                if (up && pl) bo = (bo + pat.cap_bonus) & lane_mask;
-                if (c == 0 && include_prefix) bo = (bo + pat.prefix_bonus) & lane_mask;
-                bo = (bo + pat.match_x) & lane_mask;
-                bon[c] = (uint16_t)bo;
-                Hp[c] = 0; Mp[c] = 0;
-                pl = lo; pd = dl;
-            }
-            auto bonus_at = [&](int c) -> uint32_t { return bon[c]; };
-            for (int i = 0; i < pat.n; i++) {
-                for (int c = 0; c < cols; c++) {
-                    uint32_t b = hb[c];
-                    bool e = b == pat.c[i], f = b == pat.flip[i];
-                    bool m = e || f;
-                    uint32_t dg = c > 0 ? Hp[c - 1] : 0;
-                    if (m) dg = (dg + bonus_at(c)) & lane_mask;
-                    dg = dg > (uint32_t)pat.mismatch ? dg - pat.mismatch : 0;
-                    if (e) dg = (dg + pat.case_bonus) & lane_mask;
-                    uint32_t upv = Hp[c];
-                    upv = upv > (uint32_t)pat.gap_extend ? upv - pat.gap_extend : 0;
-                    if (Mp[c]) upv = upv > (uint32_t)pat.gap_open_x ? upv - pat.gap_open_x : 0;
-                    Hc[c] = (uint16_t)max(dg, upv);
-                    Mc[c] = m;
-                }
-                for (int ch = 0; ch < nch; ch++) {
-                    const int lo = ch * L;
-                    uint32_t gex = pat.gap_extend;
-                    for (int s = 1; s < L; s <<= 1) {
-                        for (int c = lo + L - 1; c >= lo; c--) {
-                            int src = c - s;
-                            if (src < 0) continue;
-                            if (src < lo && src < lo - L) continue;  // only the adjacent chunk feeds in
-                            uint32_t pen = (gex + (Mc[src] ? (uint32_t)pat.gap_open_x : 0u)) & lane_mask;
-                            uint32_t v = Hc[src];
-                            v = v > pen ? v - pen : 0;
-                            if (v > Hc[c]) Hc[c] = (uint16_t)v;
-                        }
-                        gex = (gex + gex) & lane_mask;
-                    }
-                }
-                for (int c = 0; c < cols; c++) { Hp[c] = Hc[c]; Mp[c] = Mc[c]; }
-            }
-            uint32_t mx = 0;
-            for (int c = 0; c < cols; c++) mx = max(mx, (uint32_t)Hp[c]);
-            score = mx;
+            score = generic_score(hay, W, pat, include_prefix);
         }
         bool exact = false;
         if (start == 0 && full_end && W == pat.n) {
@@ -434,9 +336,14 @@ frz_status launch_sw_lanes(const FrzCorpusView& cv, const FrzPatternDev& pat, ui
     // persistent grids: a multiple of the SM count
     const int blocks = frz_sm_count() * 2;
     const int rev = reversed ? 1 : 0;
-    // VAR 8: the per-column bonus is classified on the packed window bytes (SwCore) rather than per 16-bit lane
+    // VAR 8: the per-column bonus is classified on the packed window bytes (SwCore) rather than per 16-bit lane.
+    // kSwVarLanePen: gap_extend == 0 < gap_open_x, whose penalties the default IMAD form gets wrong (SwCore).
+    const bool lane_pen = !pat.wrap8 && pat.gap_extend == 0 && pat.gap_open_x > 0;
     if (pat.wrap8)
         k_sw64<LANES, true><<<frz_sm_count() * kSw64MinBlocks<LANES, true>, kSwThreads, 0, stream>>>(
+            cv, pat, ws.lists(), ws.survivor_cap, rank_view(ws), ws.counters, index_offset, rev, d_out);
+    else if (lane_pen)
+        k_sw64<LANES, false, 8 | kSwVarLanePen><<<frz_sm_count() * kSw64MinBlocks<LANES, false>, kSwThreads, 0, stream>>>(
             cv, pat, ws.lists(), ws.survivor_cap, rank_view(ws), ws.counters, index_offset, rev, d_out);
     else
         k_sw64<LANES, false, 8><<<frz_sm_count() * kSw64MinBlocks<LANES, false>, kSwThreads, 0, stream>>>(
@@ -449,11 +356,16 @@ frz_status launch_sw_lanes(const FrzCorpusView& cv, const FrzPatternDev& pat, ui
     if (!attr_set) {
         FRZ_CUDA_TRY(cudaFuncSetAttribute(k_sw<LANES, 128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         FRZ_CUDA_TRY(cudaFuncSetAttribute(k_sw<LANES, 128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        FRZ_CUDA_TRY(cudaFuncSetAttribute(k_sw<LANES, 128, false, kSwVarLanePen>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr_set = true;
     }
     if (pat.wrap8)
         k_sw<LANES, 128, true><<<blocks, kSwThreads, smem, stream>>>(cv, pat, ws.survivors[FRZ_C_COLS128], ws.survivor_cap, FRZ_C_COLS128,
                                                                     rank_view(ws), ws.counters, index_offset, rev, d_out);
+    else if (lane_pen)
+        k_sw<LANES, 128, false, kSwVarLanePen><<<blocks, kSwThreads, smem, stream>>>(cv, pat, ws.survivors[FRZ_C_COLS128], ws.survivor_cap,
+                                                                                  FRZ_C_COLS128, rank_view(ws), ws.counters, index_offset,
+                                                                                  rev, d_out);
     else
         k_sw<LANES, 128, false><<<blocks, kSwThreads, smem, stream>>>(cv, pat, ws.survivors[FRZ_C_COLS128], ws.survivor_cap, FRZ_C_COLS128,
                                                                      rank_view(ws), ws.counters, index_offset, rev, d_out);

@@ -55,6 +55,8 @@ constexpr int kSwThreads = 128;
 // to <= 168 registers, i.e. 3 blocks (3 warps per scheduler) per SM.
 template <int LANES, bool WRAP8>
 constexpr bool kSw64RowsInSmem = LANES == 64 && !WRAP8;
+// SwCore VAR bit: per-lane gap penalties, for scorings with gap_extend == 0 < gap_open_x (see SwCore)
+constexpr int kSwVarLanePen = 16;
 
 FRZ_SW_FN uint32_t splat16(int v) { return ((uint32_t)v & 0xffffu) * 0x00010001u; }
 
@@ -140,6 +142,12 @@ struct HayRows<R, SMEM, true> {
 // shifts as IMAD.HI + IMAD pairs instead of PRMT, the shifted match mask folded into the gap penalty with IMAD.HI, two
 // column classes instead of four.
 //
+// VAR bit 4 (kSwVarLanePen): the gap penalties are formed per 16-bit lane with a select on the full match mask, as
+// WRAP8 does.  The default form `base + mask * gap_open_x` is one 32-bit IMAD over both lanes of a register, which is
+// exact only while the low lane's sum stays below 0x10000.  It does for gap_extend >= 1, but with gap_extend == 0 and
+// gap_open_x > 0 the low lane of a non-matching column sums to exactly 0x10000, and the carry takes one point off the
+// high lane's penalty.  frz_launch_sw (sw.cu) selects this variant for exactly that scoring.
+//
 // CC (<= COLS, multiple of 8) is the number of columns actually evaluated.  Cells never depend on cells to
 // their right, and a cell in column >= W + needle_len can only hold a value that decayed from a cell to its
 // left in the same row (it is past the reach of the diagonal/up chains that start inside the window, and zero
@@ -174,7 +182,8 @@ struct SwCore {
             // no ReLU here: max(H + upd, diag, 0) below clamps anyway, and VIADDMNMX has no zero operand, so the ReLU
             // form costs a register holding zero (or a PRMT rematerialising one per use)
             const uint32_t diag = __vadd2(prevs, sel(nmfull, p.k_neg_mis, Dv));
-            const uint32_t upd = p.k_up_open + M[r] * (uint32_t)p.gap_open_x;   // M[r] still row i-1
+            const uint32_t upd = (VAR & kSwVarLanePen) ? sel(M[r] * 0xFFFFu, p.k_up_plain, p.k_up_open)
+                                                       : p.k_up_open + M[r] * (uint32_t)p.gap_open_x;   // M[r] still row i-1
             H[r] = addmax_relu(H[r], upd, diag);
             M[r] = nm;
         } else {
@@ -313,7 +322,9 @@ struct SwCore {
                             sh = H[src];
                             smm = M[src];
                         }
-                        const uint32_t pen = WRAP8 ? sel(smm, penB, penA) : penB + smm * gopx;
+                        const uint32_t pen = WRAP8                    ? sel(smm, penB, penA)
+                                             : (VAR & kSwVarLanePen) ? sel(smm * 0xFFFFu, penA, penB)
+                                                                     : penB + smm * gopx;
                         H[r] = addmax_relu(sh, pen, H[r]);
                     }
                 }

@@ -30,14 +30,18 @@ uint32_t run_one(const FrzPatternDev& pat, const uint8_t* window, int W, int sta
     return score;
 }
 
+// VAR bit of SwCore's per-lane gap penalties (sw_core.cuh: kSwVarLanePen)
+constexpr int kLanePen = 16;
+
 template <int LANES, bool WRAP8, int VAR>
 int dispatch_cc(const FrzPatternDev& pat, const uint8_t* w, int W, int startlo, bool pre, int cols, int cc, int* eq) {
     if (cols == 128) {
+        constexpr int V = VAR & kLanePen;   // the 128-column kernel classifies the bonus per lane
         switch (cc) {   // column-limited forms of the 128-column variant (groundwork, DESIGN.md §8 item 6)
-            case 80: return (int)run_one<LANES, 128, WRAP8, 0, 80>(pat, w, W, startlo, pre, eq);
-            case 96: return (int)run_one<LANES, 128, WRAP8, 0, 96>(pat, w, W, startlo, pre, eq);
-            case 112: return (int)run_one<LANES, 128, WRAP8, 0, 112>(pat, w, W, startlo, pre, eq);
-            default: return (int)run_one<LANES, 128, WRAP8, 0, 128>(pat, w, W, startlo, pre, eq);
+            case 80: return (int)run_one<LANES, 128, WRAP8, V, 80>(pat, w, W, startlo, pre, eq);
+            case 96: return (int)run_one<LANES, 128, WRAP8, V, 96>(pat, w, W, startlo, pre, eq);
+            case 112: return (int)run_one<LANES, 128, WRAP8, V, 112>(pat, w, W, startlo, pre, eq);
+            default: return (int)run_one<LANES, 128, WRAP8, V, 128>(pat, w, W, startlo, pre, eq);
         }
     }
     switch (cc) {
@@ -54,6 +58,8 @@ int dispatch(const FrzPatternDev& pat, const uint8_t* w, int W, int startlo, boo
     {
         switch (var) {
             case 8: return dispatch_cc<LANES, false, 8>(pat, w, W, startlo, pre, cols, cc, eq);
+            case kLanePen: return dispatch_cc<LANES, false, kLanePen>(pat, w, W, startlo, pre, cols, cc, eq);
+            case 8 | kLanePen: return dispatch_cc<LANES, false, 8 | kLanePen>(pat, w, W, startlo, pre, cols, cc, eq);
         }
     }
     return dispatch_cc<LANES, false, 0>(pat, w, W, startlo, pre, cols, cc, eq);
@@ -62,6 +68,15 @@ int dispatch(const FrzPatternDev& pat, const uint8_t* w, int W, int startlo, boo
 
 extern "C" {
 size_t h_pattern_size() { return sizeof(FrzPatternDev); }
+// the pattern fields that pick the SwCore instantiation: wrap8, col_classes, and whether frz_launch_sw (sw.cu) takes the
+// per-lane gap penalty variant (gap_extend == 0 < gap_open_x, no WRAP8)
+void h_pattern_flags(const void* pat_bytes, int* wrap8, int* col_classes, int* lane_pen) {
+    FrzPatternDev pat;
+    memcpy(&pat, pat_bytes, sizeof pat);
+    *wrap8 = pat.wrap8;
+    *col_classes = pat.col_classes;
+    *lane_pen = !pat.wrap8 && pat.gap_extend == 0 && pat.gap_open_x > 0;
+}
 // score of SwCore<lanes, cols, wrap8, var, cc> on window[0..W) staged at byte offset `startlo` of its first unit
 int h_swcore(const void* pat_bytes, const uint8_t* window, int W, int startlo, int include_prefix, int lanes, int cols, int cc,
              int wrap8, int var, int* exact_eq) {

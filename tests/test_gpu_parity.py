@@ -10,6 +10,7 @@ from frizbee_b200 import synth
 from frizbee_b200.types import (CaseMatching, Config, Match, Matching, Pattern, Scoring, SortStrategy,
                                 UnicodeMatching)
 from oracle import pyoracle as O
+from scorings import edge_cases, scorings
 
 pytestmark = pytest.mark.gpu
 
@@ -161,6 +162,65 @@ def test_custom_scoring_configs():
         for needle in ("ab", "aB_b", "BBBB"):
             for k in (0, 1, None):
                 gpu_vs_oracle(needle, data, off, Config(max_typos=k, scoring=sc, emulate_lanes=32))
+
+
+SWEEP_NEEDLES = ("a_B", "ab0/", "abAB_-ab01ab")
+SWEEP_SCORINGS = scorings(seed=5150, count=len(edge_cases(12)) + 3, max_needle=max(map(len, SWEEP_NEEDLES)))
+
+
+def class_sweep_list(rng, per_class=250):
+    """Haystacks whose whole-haystack windows fall into every Smith-Waterman work class: <= 40, 41-48, 49-56, 57-64
+    (the column classes of k_sw64), 65-128 (k_sw), 129-1024 (k_sw_generic) and > 1024 bytes (the greedy scorer)."""
+    spans = [(0, 40), (41, 48), (49, 56), (57, 64), (65, 128), (129, 1024), (1025, 1600)]
+    counts = [per_class] * 5 + [per_class // 3, 12]
+    pool = b"abAB_/-ab01"
+    return [bytes(rng.choice(pool) for _ in range(rng.randint(lo, hi)))
+            for (lo, hi), c in zip(spans, counts) for _ in range(c)]
+
+
+@pytest.mark.parametrize("lanes", [16, 32, 64])
+def test_scoring_sweep(lanes):
+    """Generated scorings (tests/scorings.py, with its edge cases: gap_extend = 0 < gap_open, gap_open < gap_extend,
+    constants >= 256, both sides of score_fits_in_u8, WRAP8 through the scoring, the signed 16-bit bounds) through every
+    SW kernel the lane width reaches (k_sw64 in its column classes, WRAP8 and u16 forms, k_sw, k_sw_generic and the
+    greedy scorer), typo modes 0, 1 and None."""
+    rng = random.Random(11 + lanes)
+    data, off = from_list(class_sweep_list(rng))
+    corpus = F.Corpus.from_arrow(data, off)
+    for sc in SWEEP_SCORINGS:
+        for needle in SWEEP_NEEDLES:
+            for k in (0, 1, None):
+                gpu_vs_oracle(needle, data, off, Config(max_typos=k, scoring=sc, emulate_lanes=lanes), corpus)
+    corpus.close()
+
+
+def test_sort_strategies_across_score_bounds():
+    """The counting sort picks its digit bins from the host's score bound: a scoring whose bound is <= 255 (one pass)
+    and one whose bound is > 1023 (two passes), under every sort strategy."""
+    rng = random.Random(12)
+    data, off = from_list(class_sweep_list(rng, per_class=150))
+    corpus = F.Corpus.from_arrow(data, off)
+    low, high = Scoring(), Scoring(match_score=300, mismatch_penalty=10, gap_open_penalty=20, gap_extend_penalty=0)
+    assert O.score_fits_in_u8(2, low) and not O.score_fits_in_u8(4, high)
+    for sort in SortStrategy:
+        for needle, sc in (("ab", low), ("ab0/", high)):
+            got = gpu_vs_oracle(needle, data, off, Config(sort=sort, max_typos=1, scoring=sc), corpus)
+            assert len(got) > 100
+            if sc is high:
+                assert got["score"].max() > 1023
+    corpus.close()
+
+
+def test_multi_pattern_per_atom_scoring():
+    """One query whose atoms carry different Pattern.scoring values (one with gap_extend = 0 < gap_open)."""
+    rng = random.Random(13)
+    data, off = from_list(class_sweep_list(rng, per_class=150))
+    pats = [Pattern("ab", scoring=Scoring(gap_open_penalty=7, gap_extend_penalty=0)),
+            Pattern("B_a", scoring=Scoring(match_score=40, delimiter_bonus=0, gap_open_penalty=1, gap_extend_penalty=3)),
+            Pattern("01")]
+    for k in (0, 1, None):
+        for lanes in (16, 32, 64):
+            gpu_vs_oracle(pats, data, off, Config(max_typos=k, emulate_lanes=lanes))
 
 
 def test_sort_strategies_and_radix_sort():

@@ -2,7 +2,8 @@
 check) is compiled here for the CPU — same source, scalar stand-ins for the CUDA SIMD-in-register intrinsics — and run
 against the oracle with the pattern constants of the real library (frz_matcher_debug_pattern).  Covers what a GPU is
 otherwise needed for: every emulated lane width, the column-limited classes (CC 40/48/56/64), the 128-column variant,
-the u8 wrap emulation and the shift-placement variants."""
+the u8 wrap emulation and the shift-placement variants, across the scorings of tests/scorings.py.  k_sw_generic's scorers
+(sw_generic.cuh) are built the same way from tests/harness/sw_generic_harness.cpp."""
 import ctypes as C
 import os
 import random
@@ -14,6 +15,7 @@ import pytest
 import frizbee_b200 as F
 from frizbee_b200.types import CaseMatching, Config, Scoring
 from oracle import pyoracle as O
+from scorings import scorings
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SRC = os.path.join(ROOT, "tests", "harness", "sw_harness.cpp")
@@ -32,6 +34,7 @@ def H():
     L.h_pattern_size.restype = C.c_size_t
     L.h_swcore.argtypes = [C.c_void_p, C.c_char_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                            C.POINTER(C.c_int)]
+    L.h_pattern_flags.argtypes = [C.c_void_p] + [C.POINTER(C.c_int)] * 3
     return L
 
 
@@ -128,6 +131,185 @@ def test_swcore_u8_wrap_emulation(H):
             eq = C.c_int()
             got = H.h_swcore(pat, win, len(win), 3, int(pre), 64, 64, 64, 1, 0, C.byref(eq))
             assert got == want, (win, pre, got, want)
+
+
+# ---------------------------------------------------------------- the scorers across the scoring space (tests/scorings.py)
+MAX_NEEDLE = 24
+SCORINGS = scorings(seed=424242, count=44, max_needle=MAX_NEEDLE)
+SWEEP_POOLS = POOLS + [b"aBcD-_Xy", b"fooBAR/._", b"aA\x00b"]
+HAY_HIGH = b"\x80\xc3\xa9\xff\x00"
+
+
+def needle_for(rng, sc, lanes):
+    """A needle whose reference backend runs `lanes` wide for scoring `sc`, with the emulate_lanes and score family
+    that select it, or None when no such needle is drawn (LANES 8 is u16 only, LANES 64 u8 only)."""
+    for _ in range(8):
+        pool = rng.choice(SWEEP_POOLS)
+        needle = rand_bytes(rng, pool, rng.choice([rng.randint(1, 6), rng.randint(1, MAX_NEEDLE), MAX_NEEDLE]))
+        bits = 8 if O.score_fits_in_u8(len(needle), sc) else 16
+        em = lanes if bits == 8 else 2 * lanes
+        if em in (16, 32, 64):
+            return needle, pool, bits, em
+    return None
+
+
+def case_for(rng, needle):
+    casing = rng.choice([CaseMatching.Ignore, CaseMatching.Respect, CaseMatching.Smart])
+    cs = casing == CaseMatching.Respect or (casing == CaseMatching.Smart and any(65 <= b <= 90 for b in needle))
+    return casing, cs
+
+
+def sweep_window(rng, needle, pool, W):
+    r = rng.random()
+    if r < 0.08 and len(needle) == W:
+        return needle
+    if r < 0.12 and len(needle) == W:
+        return needle.swapcase()
+    extra = rng.choice([b"", b"x", HAY_HIGH])
+    return rand_bytes(rng, pool + extra, W)
+
+
+def pattern_flags(H, pat):
+    wrap8, col_classes, lane_pen = C.c_int(), C.c_int(), C.c_int()
+    H.h_pattern_flags(pat, C.byref(wrap8), C.byref(col_classes), C.byref(lane_pen))
+    return bool(wrap8.value), bool(col_classes.value), bool(lane_pen.value)
+
+
+@pytest.mark.parametrize("lanes", [8, 16, 32, 64])
+def test_swcore_scoring_sweep(H, lanes):
+    """SwCore with the constants of generated scorings (tests/scorings.py: zeros, gap_extend = 0 < gap_open,
+    gap_open < gap_extend, constants >= 256, both sides of score_fits_in_u8, WRAP8 through the scoring, the signed 16-bit
+    bounds) vs the oracle at the same LANES and score family.  Each window is scored by the instantiation the kernels
+    launch for it (column class as prefilter.cu: sw_class_of, WRAP8, the per-lane penalty variant) and by every wider
+    column class, with both bonus forms (VAR 0 / 8); all three case modes, needles with NUL and uppercase letters,
+    haystack bytes >= 0x80 and NUL, every startlo, prefix bonus on and off, and the exact-window check."""
+    rng = random.Random(31000 + lanes)
+    F.lib().frz_matcher_debug_pattern.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]
+    checked, seen = 0, set()
+    for trial in range(400):
+        sc = SCORINGS[trial % len(SCORINGS)]
+        drawn = needle_for(rng, sc, lanes)
+        if drawn is None:
+            continue
+        needle, pool, bits, em = drawn
+        casing, cs = case_for(rng, needle)
+        pat, info = device_pattern(H, needle, Config(max_typos=None, emulate_lanes=em, casing=casing, scoring=sc))
+        assert (info["lanes"], info["score_bits"]) == (lanes, bits)
+        wrap8, col_classes, lane_pen = pattern_flags(H, pat)
+        assert col_classes == (not wrap8 and 0 not in needle)
+        seen.add((bits, wrap8, lane_pen, cs))
+        for _ in range(5):
+            W = rng.choice([len(needle), rng.randint(1, 64), rng.randint(1, 64), rng.randint(65, 128)])
+            W = max(1, min(W, 128))
+            win = sweep_window(rng, needle, pool, W)
+            pre = rng.random() < 0.5
+            want = O.sw_score(needle, win, sc, cs, pre, lanes, bits)
+            if W <= 64:
+                cols = 64
+                if col_classes:
+                    need = min(W + len(needle), (W + lanes - 1) // lanes * lanes)
+                    cls_cc = next(cc for cc in (40, 48, 56, 64) if need <= cc)
+                    ccs = [cc for cc in (40, 48, 56, 64) if cc >= cls_cc]
+                else:
+                    ccs = [64]
+            else:
+                cols = 128
+                need = min(W + len(needle), (W + lanes - 1) // lanes * lanes)
+                ccs = [128] + ([cc for cc in (80, 96, 112) if cc >= need and cc >= W] if col_classes else [])
+            for cc in ccs:
+                for var in ((0,) if wrap8 else (0, 8)):
+                    v = var | (16 if lane_pen else 0)
+                    eq = C.c_int()
+                    startlo = rng.randint(0, 15)
+                    got = H.h_swcore(pat, win, W, startlo, int(pre), lanes, cols, cc, int(wrap8), v, C.byref(eq))
+                    assert got == want, (needle, win, sc, cs, pre, lanes, bits, cols, cc, v, startlo, got, want)
+                    assert bool(eq.value) == (win == needle)
+                    checked += 1
+    assert checked > 2500, checked
+    # the sweep reached the variants that matter at this width
+    assert any(lp for _, _, lp, _ in seen) and any(cs for *_, cs in seen)
+    if lanes != 8:
+        assert any(w for _, w, _, _ in seen)
+    assert {b for b, *_ in seen} == ({16} if lanes == 8 else {8} if lanes == 64 else {8, 16})
+
+
+# ---------------------------------------------------------------- k_sw_generic's scorers (sw_generic.cuh)
+G_SRC = os.path.join(ROOT, "tests", "harness", "sw_generic_harness.cpp")
+G_LIB = os.path.join(ROOT, "tests", "harness", "libsw_generic_harness.so")
+G_DEPS = [G_SRC] + [os.path.join(ROOT, "frizbee_b200", "csrc", f) for f in ("sw_generic.cuh", "sw_core.cuh", "frz_device.cuh")]
+
+
+@pytest.fixture(scope="module")
+def G():
+    if not os.path.isdir(CUDA_INC):
+        pytest.skip("CUDA headers not found")
+    if not os.path.exists(G_LIB) or any(os.path.getmtime(d) > os.path.getmtime(G_LIB) for d in G_DEPS):
+        subprocess.run(["g++", "-O2", "-std=c++17", "-I" + CUDA_INC, "-fPIC", "-shared", "-o", G_LIB, G_SRC], check=True)
+    L = C.CDLL(G_LIB)
+    L.h_pattern_size.restype = C.c_size_t
+    L.h_sw_generic.argtypes = [C.c_void_p, C.c_char_p, C.c_int, C.c_int]
+    L.h_greedy.argtypes = [C.c_void_p, C.c_char_p, C.c_int, C.c_int]
+    return L
+
+
+@pytest.mark.parametrize("lanes", [8, 16, 32, 64])
+def test_generic_scorer_across_scorings(H, G, lanes):
+    """generic_score (k_sw_generic, windows of 129..1024 bytes: true u8 / u16 element arithmetic) vs the oracle's
+    score_haystack at the same LANES and family, over the scoring sweep."""
+    assert G.h_pattern_size() == H.h_pattern_size()
+    rng = random.Random(33000 + lanes)
+    F.lib().frz_matcher_debug_pattern.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]
+    checked, families = 0, set()
+    for trial in range(3 * len(SCORINGS)):
+        sc = SCORINGS[trial % len(SCORINGS)]
+        drawn = needle_for(rng, sc, lanes)
+        if drawn is None:
+            continue
+        needle, pool, bits, em = drawn
+        casing, cs = case_for(rng, needle)
+        pat, info = device_pattern(H, needle, Config(max_typos=None, emulate_lanes=em, casing=casing, scoring=sc))
+        assert (info["lanes"], info["score_bits"]) == (lanes, bits)
+        families.add(bits)
+        for W in (rng.choice([129, 130, 1023, 1024]), rng.randint(129, 1024)):
+            win = rand_bytes(rng, pool + rng.choice([b"", b"x-", HAY_HIGH]), W)
+            pre = rng.random() < 0.5
+            want = O.sw_score(needle, win, sc, cs, pre, lanes, bits)
+            got = G.h_sw_generic(pat, win, W, int(pre))
+            assert got == want, (needle, win, sc, cs, pre, lanes, bits, got, want)
+            checked += 1
+    assert checked > 60, checked
+    assert families == ({16} if lanes == 8 else {8} if lanes == 64 else {8, 16})
+
+
+def test_greedy_scorer_across_scorings(H, G):
+    """greedy_score (k_sw_generic, windows over 1024 bytes) vs the oracle's match_greedy, over the scoring sweep: windows
+    that hold the needle's bytes spread out (gaps of every length, either case) and windows that miss one of them."""
+    rng = random.Random(34000)
+    F.lib().frz_matcher_debug_pattern.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]
+    matched = missed = 0
+    for trial in range(4 * len(SCORINGS)):
+        sc = SCORINGS[trial % len(SCORINGS)]
+        pool = rng.choice(SWEEP_POOLS)
+        needle = rand_bytes(rng, pool, rng.randint(1, MAX_NEEDLE))
+        casing, cs = case_for(rng, needle)
+        pat, _ = device_pattern(H, needle, Config(max_typos=None, casing=casing, scoring=sc))
+        W = rng.randint(1025, 3000)
+        filler = rand_bytes(rng, b"xyz_-/ 019QW" + HAY_HIGH, W)
+        if rng.random() < 0.8:   # plant the needle at sorted random positions, some bytes case-flipped
+            pos = sorted(rng.sample(range(W), len(needle)))
+            win = bytearray(filler)
+            for p, b in zip(pos, needle):
+                win[p] = b ^ 0x20 if (chr(b).isalpha() and rng.random() < 0.3) else b
+            win = bytes(win)
+        else:
+            win = filler
+        pre = rng.random() < 0.5
+        want = O.match_greedy(needle, win, sc, cs, pre)
+        got = G.h_greedy(pat, win, W, int(pre))
+        assert got == (-1 if want is None else want), (needle, sc, cs, pre, got, want)
+        matched += want is not None
+        missed += want is None
+    assert matched > 40 and missed > 10, (matched, missed)
 
 
 # ---------------------------------------------------------------- occurrence-mask prefilter windows (prefilter_masks.cuh)

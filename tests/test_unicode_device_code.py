@@ -12,6 +12,7 @@ import pytest
 
 from frizbee_b200.types import Scoring
 from oracle import pyoracle as O
+from scorings import scorings
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SRC = os.path.join(ROOT, "tests", "harness", "unicode_harness.cpp")
@@ -44,6 +45,7 @@ def scoring9(s: Scoring):
 
 
 POOLS = ["aéAÉ_다", "abé✓😀", "éÉeE-/x", "нНaя_Я", "ab"]
+SCORINGS = scorings(seed=7700, count=30, max_needle=20)   # needles of up to 5 scalars
 
 
 def rand_str(rng, pool, n):
@@ -120,11 +122,9 @@ def test_prefilter_equals_oracle(H, lanes):
 @pytest.mark.parametrize("lanes,bits", [(8, 16), (16, 16), (32, 16), (16, 8), (32, 8), (64, 8)])
 def test_sw_score_equals_oracle(H, lanes, bits):
     rng = random.Random(77 + lanes + bits)
-    scorings = [Scoring(), Scoring(gap_open_penalty=2, gap_extend_penalty=2, delimiter_bonus=7),
-                Scoring(match_score=5, mismatch_penalty=1, matching_case_bonus=0, prefix_bonus=3)]
     for trial in range(2500):
         pool = rng.choice(POOLS)
-        sc = rng.choice(scorings)
+        sc = SCORINGS[trial % len(SCORINGS)]
         needle = rand_str(rng, pool, rng.randint(1, 5))
         if bits == 8 and not O.score_fits_in_u8(len(needle.encode()), sc):
             continue
