@@ -107,6 +107,16 @@ typedef frz_status (*FrzChunkFn)(void* ctx, uint32_t t0, uint32_t t1, bool last)
 frz_status frz_ingest_host(FrzIngest& ing, const uint8_t* h_bytes, const void* h_offsets, int offset_width, uint64_t n,
                            cudaStream_t stream, FrzCorpusStorage* out, FrzChunkFn after_chunk = nullptr, void* ctx = nullptr);
 
+// Score histogram that the scoring kernels (sw.cu) accumulate as they emit, for the single-pass score sort (sort.cu):
+// counts[d * stride + s] = matches with score digit d whose index-ordered position lies in segment s = pos >> kFrzSortSegShift.
+// counts == nullptr: no histogram is wanted.
+constexpr int kFrzSortSegShift = 11;   // 2048-element segments
+struct FrzScoreHist {
+    uint32_t* counts = nullptr;
+    uint32_t stride = 0;   // words per digit row: segments of the largest possible list, rounded up to a multiple of 4
+    uint32_t mask = 0;     // bins - 1
+};
+
 // Per-matcher device workspace (grown on demand, reused across calls).
 struct FrzWorkspace {
     int device = -1;
@@ -126,6 +136,10 @@ struct FrzWorkspace {
     uint64_t match_cap = 0;
     uint32_t* sort_hist = nullptr;          // [256 * n_sort_blocks]
     uint64_t sort_hist_cap = 0;
+    uint32_t* fused_hist = nullptr;         // FrzScoreHist counts, then the per-segment prefix rows the sort's scan writes
+    uint64_t fused_hist_cap = 0;            // in words
+    uint64_t fused_clean_words = 0;         // leading words of fused_hist known to be zero (the scan re-zeroes what it reads)
+    bool fused_hist_dirty = false;          // counts were handed to the scoring kernels, their scan was not enqueued yet
     void* cand_list = nullptr;              // k_sig_scan → k_window candidate records (16 bytes each)
     uint64_t cand_cap = 0;                  // in records
     uint32_t* retain_cnt = nullptr;         // multi-pattern stable compaction scratch
@@ -163,8 +177,10 @@ frz_status frz_launch_prefilter_list(const FrzCorpusView& cv, const FrzPatternDe
                                      FrzLaunchStats* st);
 frz_status frz_launch_tile_scan(const FrzCorpusView& cv, FrzWorkspace& ws, cudaStream_t stream, FrzLaunchStats* st,
                                 unsigned long long* carry = nullptr);
+// hist.counts != nullptr: every emitted match also counts itself into `hist` (see FrzScoreHist)
 frz_status frz_launch_sw(const FrzCorpusView& cv, const FrzPatternDev& pat, uint32_t index_offset, bool reversed,
-                         FrzWorkspace& ws, FrzMatchDev* d_out, cudaStream_t stream, FrzLaunchStats* st);
+                         FrzWorkspace& ws, FrzMatchDev* d_out, cudaStream_t stream, FrzLaunchStats* st,
+                         const FrzScoreHist& hist = FrzScoreHist());
 // stable sort by descending score; the element count is read from device memory (*n_ptr).
 // d_tmp is only used when score_bound >= 1024 (two 8-bit passes); result always lands in d_out.
 frz_status frz_launch_sort_by_score_dev(const FrzMatchDev* d_in, FrzMatchDev* d_tmp, FrzMatchDev* d_out,
@@ -174,6 +190,12 @@ size_t frz_sort_hist_words();
 frz_status frz_sort_hist_alloc(uint32_t** out);
 const uint32_t* frz_sort_digit_base(const FrzWorkspace& ws);
 int frz_sort_single_pass_bins(uint32_t score_bound);   // bins of the single-pass sort for this bound, 0 = two passes
+// The fused single-pass sort: the scoring kernels build the histogram (frz_launch_sw with `hist`), so the sort is a scan
+// and a block-per-segment scatter.  prepare: sizes and zeroes the histogram for lists of up to n_cap matches whose scores
+// are below score_bound (< 1024).  The sort reads the count at *n_ptr and leaves the histogram zeroed for the next call.
+frz_status frz_sort_fused_prepare(FrzWorkspace& ws, uint64_t n_cap, uint32_t score_bound, cudaStream_t stream, FrzScoreHist* out);
+frz_status frz_launch_sort_fused(const FrzMatchDev* d_in, FrzMatchDev* d_out, const unsigned long long* n_ptr, const FrzScoreHist& hist,
+                                 FrzWorkspace& ws, cudaStream_t stream, FrzLaunchStats* st);
 
 // k-way merge of per-shard runs (host.cu) with caller-owned scratch — one per concurrent user (parallel.cu: one per rank)
 #define FRZ_MERGE_MAX_RUNS 64

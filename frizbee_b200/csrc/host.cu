@@ -600,6 +600,7 @@ void FrzWorkspace::release() {
     sort_hist = nullptr; cand_list = nullptr;
     cudaFree(retain_cnt); cudaFree(retain_base); cudaFree(retain_keep); retain_cnt = nullptr; retain_base = nullptr; retain_keep = nullptr; retain_cap = 0;
     cudaFree(unicode_scratch); unicode_scratch = nullptr; unicode_scratch_cap = 0;
+    cudaFree(fused_hist); fused_hist = nullptr; fused_hist_cap = fused_clean_words = 0; fused_hist_dirty = false;
     survivor_cap = match_cap = sort_hist_cap = cand_cap = 0; tiles_cap = 0; device = -1;
 }
 
@@ -925,7 +926,8 @@ uint64_t initial_survivor_cap(const FrzCorpusStorage& cs, const FrzPatternDev& d
 // d_out (reversed order if `reversed`); the count is left in ws.counters->total (device).
 frz_status run_pattern(frz_matcher* m, const FrzCorpusStorage& cs, const Compiled& c, const uint32_t* cand_bitmap,
                        uint32_t index_offset, bool reversed, FrzMatchDev* d_out, cudaStream_t stream, FrzLaunchStats* st,
-                       bool record_events, const FrzMatchDev* cand_list = nullptr, uint64_t n_cand = 0) {
+                       bool record_events, const FrzMatchDev* cand_list = nullptr, uint64_t n_cand = 0,
+                       const FrzScoreHist& hist = FrzScoreHist()) {
     FrzWorkspace& ws = m->ws;
     const FrzCorpusView cv = cs.view();
     uint64_t cap = std::max(ws.survivor_cap, initial_survivor_cap(cs, c.dev));
@@ -949,9 +951,9 @@ frz_status run_pattern(frz_matcher* m, const FrzCorpusStorage& cs, const Compile
         // the unicode kernel has already scored its survivors: they travel as literal-style records (score, exact)
         FrzPatternDev emit = c.dev;
         emit.typo_mode = FRZ_T_LITERAL;
-        FRZ_TRY(frz_launch_sw(cv, emit, index_offset, reversed, ws, d_out, stream, st));
+        FRZ_TRY(frz_launch_sw(cv, emit, index_offset, reversed, ws, d_out, stream, st, hist));
     } else {
-        FRZ_TRY(frz_launch_sw(cv, c.dev, index_offset, reversed, ws, d_out, stream, st));
+        FRZ_TRY(frz_launch_sw(cv, c.dev, index_offset, reversed, ws, d_out, stream, st, hist));
     }
     if (record_events) { cudaEventRecord(ws.ev[2], stream); ws.ev_rec[2] = true; }
     return FRZ_OK;
@@ -973,10 +975,12 @@ int grid_for(uint64_t n, int block) {
 }
 
 // match_list_into over all compiled patterns → index-ordered device list; returns pointer + leaves the
-// count in ws.counters->total.  `final_reversed` asks for the list in descending index order.
+// count in ws.counters->total.  `final_reversed` asks for the list in descending index order.  `score_hist` (optional):
+// the caller will sort the list by score; where the scoring kernels emit the list directly and one sort pass will do,
+// they also build the sort's histogram, returned there (score_hist->counts stays nullptr otherwise).
 frz_status match_into_device(frz_matcher* m, const FrzCorpusStorage& cs, uint32_t index_offset, bool final_reversed,
                              FrzMatchDev** d_result, uint32_t* score_bound, cudaStream_t stream, FrzLaunchStats* st,
-                             FrzMatchDev* prefer_out = nullptr) {
+                             FrzMatchDev* prefer_out = nullptr, FrzScoreHist* score_hist = nullptr) {
     FrzWorkspace& ws = m->ws;
     if ((uint64_t)cs.n + index_offset > 0xFFFFFFFFull)
         return frz_fail(FRZ_ERR_TOO_MANY_ITEMS, "too many items in haystack, will overflow the u32 index: %llu > %u (index offset: %u)",
@@ -999,7 +1003,12 @@ frz_status match_into_device(frz_matcher* m, const FrzCorpusStorage& cs, uint32_
     if (pats.size() == 1 && !pats[0].negated) {  // CompiledPatterns::Single
         FRZ_TRY(ensure_workspace(m, cs, initial_survivor_cap(cs, pats[0].dev)));
         FrzMatchDev* dst = prefer_out ? prefer_out : ws.matches_a;
-        FRZ_TRY(run_pattern(m, cs, pats[0], nullptr, index_offset, final_reversed, dst, stream, st, true));
+        FrzScoreHist hist;
+        if (score_hist && frz_sort_single_pass_bins(pats[0].score_bound) > 0) {
+            FRZ_TRY(frz_sort_fused_prepare(ws, cs.n, pats[0].score_bound, stream, &hist));
+            *score_hist = hist;
+        }
+        FRZ_TRY(run_pattern(m, cs, pats[0], nullptr, index_offset, final_reversed, dst, stream, st, true, nullptr, 0, hist));
         *d_result = dst;
         *score_bound = pats[0].score_bound;
         return FRZ_OK;
@@ -1099,7 +1108,9 @@ frz_status match_list_device(frz_matcher* m, const FrzCorpusStorage& cs, uint32_
     m->last_sort_bins = 0;
     FrzMatchDev* d_list = nullptr;
     uint32_t bound = 0;
-    FRZ_TRY(match_into_device(m, cs, index_offset, reversed, &d_list, &bound, stream, st, will_sort ? nullptr : final_out));
+    FrzScoreHist hist;
+    FRZ_TRY(match_into_device(m, cs, index_offset, reversed, &d_list, &bound, stream, st, will_sort ? nullptr : final_out,
+                              will_sort ? &hist : nullptr));
     // `!self.patterns.is_empty() && sort.is_by_score()` (src/matcher/mod.rs:218)
     if (will_sort) {
         FrzMatchDev* other = final_out ? final_out : (d_list == ws.matches_a ? ws.matches_b : ws.matches_a);
@@ -1110,7 +1121,8 @@ frz_status match_list_device(frz_matcher* m, const FrzCorpusStorage& cs, uint32_
             FRZ_TRY(ensure_multi_buffers(m, cs.n));
             tmp = m->multi_a;
         }
-        FRZ_TRY(frz_launch_sort_by_score_dev(d_list, tmp, other, &ws.counters->total, bound, ws, stream, st));
+        if (hist.counts) FRZ_TRY(frz_launch_sort_fused(d_list, other, &ws.counters->total, hist, ws, stream, st));
+        else FRZ_TRY(frz_launch_sort_by_score_dev(d_list, tmp, other, &ws.counters->total, bound, ws, stream, st));
         m->last_sort_bins = frz_sort_single_pass_bins(bound);
         d_list = other;
     } else if (final_out && d_list != final_out) {

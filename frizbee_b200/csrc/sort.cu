@@ -11,10 +11,16 @@
 //   k_sort_scatter  each virtual warp re-walks its segment IN ORDER, 32 elements at a time;
 //                   __match_any_sync gives the in-warp stable rank, a per-warp counter array the rest
 //
+// The fused single-pass sort (frz_sort_fused_prepare / frz_launch_sort_fused) has no histogram kernel: the scoring kernels
+// count every match they emit into FrzScoreHist (per score digit, per 2048-element segment of its index-ordered position),
+// k_sort_scan_rows scans that histogram (and re-zeroes it), and k_sort_scatter_seg places one segment per block.
+//
 // The element count lives in device memory (it is produced by the previous stage), so the whole
 // match_list pipeline runs without a host round trip until the final copy-out.
 #include "frz_device.cuh"
 #include "frz_host.h"
+
+#include <algorithm>
 
 namespace {
 
@@ -64,38 +70,57 @@ __global__ void __launch_bounds__(kSortWarps * 32) k_sort_hist(const FrzMatchDev
     for (int d = lane; d < bins; d += 32) hist[(size_t)d * kV + v] = cnt[d];
 }
 
-// hist[d][v] → exclusive prefix over v (in place), one warp per digit row; totals[d] = row sum.  The LAST block to
-// finish (device counter, self-resetting) then turns the row totals into digit_base[d] = #elements with digit > d
-// (descending exclusive prefix over the digits) — one launch instead of two.
-__global__ void __launch_bounds__(256) k_sort_scan_rows(uint32_t* __restrict__ hist, int bins, uint32_t* __restrict__ totals,
-                                                        uint32_t* __restrict__ digit_base, unsigned int* __restrict__ done_counter) {
+// hist[d][v] → exclusive prefix over v into pref[d][v], one warp per digit row; totals[d] = row sum.  A row holds `stride`
+// words of which the first `count` are used: count = kV for k_sort_hist's segments, or (n_ptr) the number of
+// 2^kFrzSortSegShift-element segments of the list, read at run time.  ZERO: the words read are zeroed again (the fused
+// histogram is left clean for the next call).  A lane owns 4 * U contiguous entries of a 128 * U-entry chunk; U = kV / 128
+// covers k_sort_hist's rows in one chunk with all loads in flight.  The LAST block to finish (device counter,
+// self-resetting) then turns the row totals into digit_base[d] = #elements with digit > d (descending exclusive prefix over
+// the digits) — one launch instead of two.
+template <int U, bool ZERO>
+__global__ void __launch_bounds__(256) k_sort_scan_rows(uint32_t* __restrict__ hist, uint32_t* __restrict__ pref, uint32_t stride,
+                                                        const unsigned long long* __restrict__ n_ptr, int bins,
+                                                        uint32_t* __restrict__ totals, uint32_t* __restrict__ digit_base,
+                                                        unsigned int* __restrict__ done_counter) {
     __shared__ bool is_last;
     __shared__ uint32_t wsum[8];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int d = blockIdx.x * 8 + warp;
     if (d < bins) {
-        constexpr int PER = kV / 32;  // contiguous entries per lane
-        uint4* row = reinterpret_cast<uint4*>(hist + (size_t)d * kV + lane * PER);
-        uint4 v[PER / 4];
-        uint32_t s = 0;
+        const uint32_t count = n_ptr ? (uint32_t)((*n_ptr + (1ull << kFrzSortSegShift) - 1) >> kFrzSortSegShift) : (uint32_t)kV;
+        uint4* row = reinterpret_cast<uint4*>(hist + (size_t)d * stride);
+        uint4* prow = reinterpret_cast<uint4*>(pref + (size_t)d * stride);
+        uint32_t carry = 0;
+        for (uint32_t c0 = 0; c0 < count; c0 += 128 * U) {
+            const uint32_t q0 = (c0 >> 2) + lane * U;   // this lane's first uint4 of the chunk
+            uint4 v[U];
+            uint32_t s = 0;
 #pragma unroll
-        for (int k = 0; k < PER / 4; k++) { v[k] = row[k]; s += v[k].x + v[k].y + v[k].z + v[k].w; }
-        uint32_t x = s;
-        for (int o = 1; o < 32; o <<= 1) {
-            uint32_t y = __shfl_up_sync(0xffffffffu, x, o);
-            if (lane >= o) x += y;
-        }
-        uint32_t run = x - s;
+            for (int k = 0; k < U; k++) {
+                v[k] = make_uint4(0, 0, 0, 0);
+                if ((q0 + k) * 4 < count) v[k] = row[q0 + k];
+                s += v[k].x + v[k].y + v[k].z + v[k].w;
+            }
+            uint32_t x = s;
+            for (int o = 1; o < 32; o <<= 1) {
+                uint32_t y = __shfl_up_sync(0xffffffffu, x, o);
+                if (lane >= o) x += y;
+            }
+            uint32_t run = carry + x - s;
 #pragma unroll
-        for (int k = 0; k < PER / 4; k++) {
-            uint4 o4;
-            o4.x = run; run += v[k].x;
-            o4.y = run; run += v[k].y;
-            o4.z = run; run += v[k].z;
-            o4.w = run; run += v[k].w;
-            row[k] = o4;
+            for (int k = 0; k < U; k++) {
+                if ((q0 + k) * 4 >= count) break;
+                uint4 o4;
+                o4.x = run; run += v[k].x;
+                o4.y = run; run += v[k].y;
+                o4.z = run; run += v[k].z;
+                o4.w = run; run += v[k].w;
+                prow[q0 + k] = o4;
+                if (ZERO) row[q0 + k] = make_uint4(0, 0, 0, 0);
+            }
+            carry += __shfl_sync(0xffffffffu, x, 31);
         }
-        if (lane == 31) totals[d] = x;
+        if (lane == 0) totals[d] = carry;
     }
     __threadfence();
     __syncthreads();
@@ -172,6 +197,71 @@ __global__ void __launch_bounds__(kSortWarps * 32) k_sort_scatter(const FrzMatch
     }
 }
 
+// The fused single-pass scatter: one block per 2^kFrzSortSegShift-element segment of the list (a persistent grid strides over
+// the segments).  Warp w owns the segment's w-th run of kSegRounds * 32 elements and loads all of it at once (coalesced, every
+// load in flight).  It ranks its run stably, 32 elements per round: __match_any_sync gives the rank inside the round, and the
+// round's leader of each digit adds the round's count to the warp's digit counter in shared memory, whose old value it
+// broadcasts.  A per-digit exclusive prefix over the warps, plus digit_base[d] + pref[d][segment] (the scoring kernels'
+// histogram, scanned), then gives every element its final position: (score desc, index asc) exactly.
+constexpr int kSegThreads = 256;
+constexpr int kSegWarps = kSegThreads / 32;
+constexpr int kSegRounds = (1 << kFrzSortSegShift) / kSegThreads;   // elements per lane
+static_assert(kSegRounds * kSegThreads == (1 << kFrzSortSegShift), "a segment is a whole number of block-wide rounds");
+
+__global__ void __launch_bounds__(kSegThreads) k_sort_scatter_seg(const FrzMatchDev* __restrict__ in, FrzMatchDev* __restrict__ out,
+                                                                  const unsigned long long* __restrict__ n_ptr, int bins,
+                                                                  const uint32_t* __restrict__ pref, uint32_t stride,
+                                                                  const uint32_t* __restrict__ digit_base) {
+    extern __shared__ uint32_t sm[];   // [kSegWarps][bins]: per-warp digit counters, then each warp's output base per digit
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    uint32_t* cnt = sm + warp * bins;
+    const unsigned long long n = *n_ptr;
+    const uint32_t nseg = (uint32_t)((n + (1ull << kFrzSortSegShift) - 1) >> kFrzSortSegShift);
+    const uint32_t mask = (uint32_t)bins - 1;
+    const uint32_t lt = (1u << lane) - 1;
+    for (uint32_t seg = blockIdx.x; seg < nseg; seg += gridDim.x) {
+        for (int d = threadIdx.x; d < kSegWarps * bins; d += kSegThreads) sm[d] = 0;
+        const unsigned long long first = ((unsigned long long)seg << kFrzSortSegShift) + warp * (kSegRounds * 32) + lane;
+        FrzMatchDev m[kSegRounds];
+#pragma unroll
+        for (int r = 0; r < kSegRounds; r++) {
+            m[r].index = 0; m[r].score = 0; m[r].exact = 0; m[r].pad = 0;
+            if (first + r * 32 < n) m[r] = in[first + r * 32];
+        }
+        __syncthreads();
+        uint32_t rank[kSegRounds];
+#pragma unroll
+        for (int r = 0; r < kSegRounds; r++) {
+            const bool valid = first + r * 32 < n;
+            const uint32_t d = valid ? (uint32_t)m[r].score & mask : (uint32_t)bins + lane;   // sentinel: matches nobody
+            const uint32_t peers = __match_any_sync(0xffffffffu, d);
+            const int leader = __ffs(peers) - 1;
+            uint32_t old = 0;
+            if (valid && lane == leader) old = atomicAdd(&cnt[d], (uint32_t)__popc(peers));
+            rank[r] = __shfl_sync(0xffffffffu, old, leader) + __popc(peers & lt);
+        }
+        __syncthreads();
+        // per digit: exclusive prefix over the warps, offset by where the digit's run of this segment starts in the output
+        for (int d = threadIdx.x; d < bins; d += kSegThreads) {
+            uint32_t tot = 0;
+#pragma unroll
+            for (int w = 0; w < kSegWarps; w++) tot += sm[w * bins + d];
+            uint32_t run = tot ? digit_base[d] + pref[(size_t)d * stride + seg] : 0u;
+#pragma unroll
+            for (int w = 0; w < kSegWarps; w++) {
+                const uint32_t c = sm[w * bins + d];
+                sm[w * bins + d] = run;
+                run += c;
+            }
+        }
+        __syncthreads();
+#pragma unroll
+        for (int r = 0; r < kSegRounds; r++)
+            if (first + r * 32 < n) out[cnt[(uint32_t)m[r].score & mask] + rank[r]] = m[r];
+        __syncthreads();   // the counters are reset for the next segment
+    }
+}
+
 }  // namespace
 
 // n_ptr: device pointer to the element count.  score_bound: host-known upper bound of any score.
@@ -184,7 +274,8 @@ frz_status frz_launch_sort_by_score_dev(const FrzMatchDev* d_in, FrzMatchDev* d_
         uint32_t* totals = ws.sort_hist + (size_t)kMaxBins * kV;
         uint32_t* digit_base = totals + kMaxBins;
         unsigned int* done_counter = reinterpret_cast<unsigned int*>(digit_base + kMaxBins);   // zeroed at allocation, self-resetting
-        k_sort_scan_rows<<<(bins + 7) / 8, 256, 0, stream>>>(ws.sort_hist, bins, totals, digit_base, done_counter);
+        k_sort_scan_rows<kV / 128, false><<<(bins + 7) / 8, 256, 0, stream>>>(ws.sort_hist, ws.sort_hist, kV, nullptr, bins, totals,
+                                                                               digit_base, done_counter);
         if (ws.arm_table_ev && ws.table_ev) {   // digit_base is final: the multi-GPU layer publishes it while the scatter runs
             FRZ_CUDA_TRY(cudaEventRecord(ws.table_ev, stream));
             ws.table_ev_recorded = true;
@@ -215,3 +306,50 @@ frz_status frz_sort_hist_alloc(uint32_t** out) {
 // the multi-GPU slice exchange needs (parallel.cu) — so nobody has to binary-search the sorted run for it.
 const uint32_t* frz_sort_digit_base(const FrzWorkspace& ws) { return ws.sort_hist ? ws.sort_hist + (size_t)kMaxBins * kV + kMaxBins : nullptr; }
 int frz_sort_single_pass_bins(uint32_t score_bound) { return score_bound < 256 ? 256 : score_bound < 512 ? 512 : score_bound < 1024 ? 1024 : 0; }
+
+// fused_hist holds the counts ([bins][stride]) and then the scan's prefix rows (same shape).  The counts are zero between
+// calls (the scan re-zeroes every word the scoring kernels can have touched), so only growth, a new layout reaching past
+// the words known to be zero, or a call that stopped between scoring and scan costs a memset.
+frz_status frz_sort_fused_prepare(FrzWorkspace& ws, uint64_t n_cap, uint32_t score_bound, cudaStream_t stream, FrzScoreHist* out) {
+    const int bins = frz_sort_single_pass_bins(score_bound);
+    if (bins == 0) return frz_fail(FRZ_ERR_INVALID_ARG, "fused sort needs a score bound below 1024 (got %u)", score_bound);
+    const uint64_t segs = (n_cap + (1ull << kFrzSortSegShift) - 1) >> kFrzSortSegShift;
+    const uint64_t stride = std::max<uint64_t>((segs + 3) & ~3ull, 4);
+    const uint64_t words = (uint64_t)bins * stride;
+    if (ws.fused_hist_cap < 2 * words) {
+        cudaFree(ws.fused_hist);
+        ws.fused_hist = nullptr; ws.fused_hist_cap = 0; ws.fused_clean_words = 0;
+        FRZ_CUDA_TRY(cudaMalloc(&ws.fused_hist, 2 * words * sizeof(uint32_t)));
+        ws.fused_hist_cap = 2 * words;
+    }
+    if (ws.fused_hist_dirty || ws.fused_clean_words < words)
+        FRZ_CUDA_TRY(cudaMemsetAsync(ws.fused_hist, 0, words * sizeof(uint32_t), stream));
+    ws.fused_clean_words = words;   // the prefix rows are written right behind the counts
+    ws.fused_hist_dirty = true;
+    out->counts = ws.fused_hist;
+    out->stride = (uint32_t)stride;
+    out->mask = (uint32_t)bins - 1;
+    return FRZ_OK;
+}
+
+frz_status frz_launch_sort_fused(const FrzMatchDev* d_in, FrzMatchDev* d_out, const unsigned long long* n_ptr, const FrzScoreHist& h,
+                                 FrzWorkspace& ws, cudaStream_t stream, FrzLaunchStats* st) {
+    const int bins = (int)h.mask + 1;
+    uint32_t* pref = h.counts + (size_t)bins * h.stride;
+    uint32_t* totals = ws.sort_hist + (size_t)kMaxBins * kV;
+    uint32_t* digit_base = totals + kMaxBins;
+    unsigned int* done_counter = reinterpret_cast<unsigned int*>(digit_base + kMaxBins);
+    k_sort_scan_rows<4, true><<<(bins + 7) / 8, 256, 0, stream>>>(h.counts, pref, h.stride, n_ptr, bins, totals, digit_base, done_counter);
+    FRZ_CUDA_TRY(cudaGetLastError());
+    ws.fused_hist_dirty = false;
+    if (ws.arm_table_ev && ws.table_ev) {   // digit_base is final: the multi-GPU layer publishes it while the scatter runs
+        FRZ_CUDA_TRY(cudaEventRecord(ws.table_ev, stream));
+        ws.table_ev_recorded = true;
+    }
+    const size_t smem = (size_t)kSegWarps * bins * sizeof(uint32_t);
+    const int grid = (int)std::max<uint32_t>(1, std::min<uint32_t>(h.stride, (uint32_t)frz_sm_count() * 4));
+    k_sort_scatter_seg<<<grid, kSegThreads, smem, stream>>>(d_in, d_out, n_ptr, bins, pref, h.stride, digit_base);
+    FRZ_CUDA_TRY(cudaGetLastError());
+    if (st) st->launches += 2;
+    return FRZ_OK;
+}

@@ -76,7 +76,7 @@ __device__ __forceinline__ uint64_t match_position(const FrzSurvivor& rec, bool 
     return pos;
 }
 __device__ __forceinline__ void store_match(const FrzSurvivor& rec, uint64_t pos, uint32_t score, bool exact, uint32_t index_offset,
-                                            FrzMatchDev* __restrict__ out) {
+                                            FrzMatchDev* __restrict__ out, const FrzScoreHist& hist) {
     const uint32_t li = (rec.slot_rank >> 10) & 0x3ff;
     FrzMatchDev m;
     m.index = index_offset + rec.tile * FRZ_TILE + li;
@@ -84,11 +84,12 @@ __device__ __forceinline__ void store_match(const FrzSurvivor& rec, uint64_t pos
     m.exact = exact ? 1 : 0;
     m.pad = 0;
     out[pos] = m;
+    if (hist.counts) atomicAdd(&hist.counts[(size_t)(score & hist.mask) * hist.stride + (pos >> kFrzSortSegShift)], 1u);
 }
 __device__ __forceinline__ void emit_match(const FrzSurvivor& rec, uint32_t score, bool exact, uint32_t index_offset,
                                            bool reversed, const FrzRankView& rv,
-                                           const FrzCounters* __restrict__ ctr, FrzMatchDev* __restrict__ out) {
-    store_match(rec, match_position(rec, reversed, rv, ctr), score, exact, index_offset, out);
+                                           const FrzCounters* __restrict__ ctr, FrzMatchDev* __restrict__ out, const FrzScoreHist& hist) {
+    store_match(rec, match_position(rec, reversed, rv, ctr), score, exact, index_offset, out, hist);
 }
 
 // One survivor whose window units are in registers: score it, write the Match at its index-ordered position.
@@ -96,14 +97,14 @@ template <int LANES, int COLS, bool WRAP8, int CC, int VAR = 0>
 __device__ __forceinline__ uint32_t score_window(const FrzPatternDev& pat, const FrzSurvivor& rec, const WindowRec& wr,
                                                  const uint4 (&u)[(CC + 15) / 16 + 1], const FrzRankView& rv,
                                                  const FrzCounters* __restrict__ ctr, uint32_t index_offset, int reversed,
-                                                 FrzMatchDev* __restrict__ out, uint32_t* sw_smem) {
+                                                 FrzMatchDev* __restrict__ out, const FrzScoreHist& hist, uint32_t* sw_smem) {
     const uint64_t pos = match_position(rec, reversed != 0, rv, ctr);   // loads overlap the DP
     uint32_t hw[CC / 4];
     window_from_units<CC>(u, wr.startlo, wr.W, hw);
     uint32_t score = SwCore<LANES, COLS, WRAP8, VAR, CC>::run(hw, wr.W, pat, wr.start0, sw_smem);
     bool exact = wr.start0 && wr.full_end && window_equals_needle(hw, wr.W, pat);
     if (exact) score = (score + pat.exact_bonus) & 0xffffu;
-    store_match(rec, pos, score, exact, index_offset, out);
+    store_match(rec, pos, score, exact, index_offset, out, hist);
     return score;
 }
 
@@ -111,7 +112,8 @@ __device__ __forceinline__ uint32_t score_window(const FrzPatternDev& pat, const
 template <int LANES, int COLS, bool WRAP8, int CC, int VAR = 0>
 __device__ __forceinline__ uint32_t score_survivor(const FrzCorpusView& cv, const FrzPatternDev& pat, const FrzSurvivor& rec,
                                                    const FrzRankView& rv, const FrzCounters* __restrict__ ctr, uint32_t index_offset,
-                                                   int reversed, FrzMatchDev* __restrict__ out, uint32_t* sw_smem) {
+                                                   int reversed, FrzMatchDev* __restrict__ out, const FrzScoreHist& hist,
+                                                   uint32_t* sw_smem) {
     constexpr int NU = (CC + 15) / 16 + 1;
     const WindowRec wr = decode_window(rec);
     const int nu = window_units(wr);
@@ -122,7 +124,7 @@ __device__ __forceinline__ uint32_t score_survivor(const FrzCorpusView& cv, cons
         u[k] = make_uint4(0, 0, 0, 0);
         if (k < nu) u[k] = __ldg(base + k);
     }
-    return score_window<LANES, COLS, WRAP8, CC, VAR>(pat, rec, wr, u, rv, ctr, index_offset, reversed, out, sw_smem);
+    return score_window<LANES, COLS, WRAP8, CC, VAR>(pat, rec, wr, u, rv, ctr, index_offset, reversed, out, hist, sw_smem);
 }
 
 // Windows of 65..128 bytes: one window per thread, score rows in shared memory, survivors strided over a
@@ -131,14 +133,15 @@ template <int LANES, int COLS, bool WRAP8, int VAR = 0>
 __global__ void __launch_bounds__(kSwThreads) k_sw(const FrzCorpusView cv, const __grid_constant__ FrzPatternDev pat,
                                                    const FrzSurvivor* __restrict__ surv, unsigned long long surv_cap, int cls,
                                                    const FrzRankView rv, FrzCounters* __restrict__ ctr,
-                                                   uint32_t index_offset, int reversed, FrzMatchDev* __restrict__ out) {
+                                                   uint32_t index_offset, int reversed, FrzMatchDev* __restrict__ out,
+                                                   const FrzScoreHist hist) {
     extern __shared__ __align__(16) uint32_t sw_smem[];
     const unsigned long long count = min(ctr->class_count[cls], surv_cap);
     uint32_t local_max = 0;
     for (unsigned long long j = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; j < count;
          j += (unsigned long long)gridDim.x * blockDim.x) {
         const FrzSurvivor rec = surv[j];
-        local_max = max(local_max, score_survivor<LANES, COLS, WRAP8, COLS, VAR>(cv, pat, rec, rv, ctr, index_offset, reversed, out, sw_smem));
+        local_max = max(local_max, score_survivor<LANES, COLS, WRAP8, COLS, VAR>(cv, pat, rec, rv, ctr, index_offset, reversed, out, hist, sw_smem));
     }
     local_max = __reduce_max_sync(0xffffffffu, local_max);
     if (frz_lane() == 0 && local_max) atomicMax(&ctr->max_score, local_max);
@@ -160,7 +163,8 @@ template <int LANES, bool WRAP8, int VAR = 0>
 __global__ void __launch_bounds__(kSwThreads, (kSw64MinBlocks<LANES, WRAP8>)) k_sw64(const FrzCorpusView cv, const __grid_constant__ FrzPatternDev pat,
                                                      const FrzSurvLists lists, unsigned long long surv_cap,
                                                      const FrzRankView rv, FrzCounters* __restrict__ ctr,
-                                                     uint32_t index_offset, int reversed, FrzMatchDev* __restrict__ out) {
+                                                     uint32_t index_offset, int reversed, FrzMatchDev* __restrict__ out,
+                                                   const FrzScoreHist hist) {
     __shared__ Sw64Stage stage;
     __shared__ __align__(16) uint32_t rows_smem[kSw64RowsInSmem<LANES, WRAP8> ? 2 * 32 * kSwThreads : 1];
     const uint32_t lane = frz_lane();
@@ -248,15 +252,15 @@ __global__ void __launch_bounds__(kSwThreads, (kSw64MinBlocks<LANES, WRAP8>)) k_
             const int k = class_of(item0);
             uint32_t sc;
             if (k == 0) {
-                sc = score_window<LANES, 64, WRAP8, 64, VAR>(pat, rec0, wr, u, rv, ctr, index_offset, reversed, out, rows_smem);
+                sc = score_window<LANES, 64, WRAP8, 64, VAR>(pat, rec0, wr, u, rv, ctr, index_offset, reversed, out, hist, rows_smem);
             } else if (k == 1) {
-                sc = score_window<LANES, 64, WRAP8, 56, VAR>(pat, rec0, wr, u, rv, ctr, index_offset, reversed, out, rows_smem);
+                sc = score_window<LANES, 64, WRAP8, 56, VAR>(pat, rec0, wr, u, rv, ctr, index_offset, reversed, out, hist, rows_smem);
             } else if (k == 2) {
                 const uint4 (&u4)[4] = reinterpret_cast<const uint4 (&)[4]>(u);
-                sc = score_window<LANES, 64, WRAP8, 48, VAR>(pat, rec0, wr, u4, rv, ctr, index_offset, reversed, out, rows_smem);
+                sc = score_window<LANES, 64, WRAP8, 48, VAR>(pat, rec0, wr, u4, rv, ctr, index_offset, reversed, out, hist, rows_smem);
             } else {
                 const uint4 (&u4)[4] = reinterpret_cast<const uint4 (&)[4]>(u);
-                sc = score_window<LANES, 64, WRAP8, 40, VAR>(pat, rec0, wr, u4, rv, ctr, index_offset, reversed, out, rows_smem);
+                sc = score_window<LANES, 64, WRAP8, 40, VAR>(pat, rec0, wr, u4, rv, ctr, index_offset, reversed, out, hist, rows_smem);
             }
             local_max = max(local_max, sc);
         }
@@ -283,7 +287,8 @@ struct GenericHay {
 __global__ void __launch_bounds__(64) k_sw_generic(const FrzCorpusView cv, const __grid_constant__ FrzPatternDev pat,
                                                    const FrzSurvivor* __restrict__ surv, unsigned long long surv_cap, int cls,
                                                    const FrzRankView rv, FrzCounters* __restrict__ ctr,
-                                                   uint32_t index_offset, int reversed, FrzMatchDev* __restrict__ out) {
+                                                   uint32_t index_offset, int reversed, FrzMatchDev* __restrict__ out,
+                                                   const FrzScoreHist hist) {
     const unsigned long long count = min(ctr->class_count[cls], surv_cap);
     uint32_t local_max = 0;
     for (unsigned long long j = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; j < count;
@@ -309,7 +314,7 @@ __global__ void __launch_bounds__(64) k_sw_generic(const FrzCorpusView cv, const
             for (int k = 0; k < pat.n; k++) exact = exact && hay_byte(base, k) == pat.c[k];
         }
         if (exact) score = (score + pat.exact_bonus) & 0xffffu;
-        emit_match(rec, score, exact, index_offset, reversed != 0, rv, ctr, out);
+        emit_match(rec, score, exact, index_offset, reversed != 0, rv, ctr, out, hist);
         local_max = max(local_max, score);
     }
     if (local_max) atomicMax(&ctr->max_score, local_max);
@@ -318,13 +323,14 @@ __global__ void __launch_bounds__(64) k_sw_generic(const FrzCorpusView cv, const
 // literal patterns: the prefilter stage already produced (score, exact); just place the match
 __global__ void __launch_bounds__(256) k_emit_literal(const FrzSurvivor* __restrict__ surv, unsigned long long surv_cap,
                                                       const FrzRankView rv, FrzCounters* __restrict__ ctr,
-                                                      uint32_t index_offset, int reversed, FrzMatchDev* __restrict__ out) {
+                                                      uint32_t index_offset, int reversed, FrzMatchDev* __restrict__ out,
+                                                   const FrzScoreHist hist) {
     const unsigned long long count = min(ctr->class_count[FRZ_C_COLS64], surv_cap);
     uint32_t local_max = 0;
     for (unsigned long long j = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; j < count;
          j += (unsigned long long)gridDim.x * blockDim.x) {
         const FrzSurvivor rec = surv[j];
-        emit_match(rec, rec.start, rec.end != 0, index_offset, reversed != 0, rv, ctr, out);
+        emit_match(rec, rec.start, rec.end != 0, index_offset, reversed != 0, rv, ctr, out, hist);
         local_max = max(local_max, rec.start);
     }
     if (local_max) atomicMax(&ctr->max_score, local_max);
@@ -332,7 +338,7 @@ __global__ void __launch_bounds__(256) k_emit_literal(const FrzSurvivor* __restr
 
 template <int LANES>
 frz_status launch_sw_lanes(const FrzCorpusView& cv, const FrzPatternDev& pat, uint32_t index_offset, bool reversed,
-                           FrzWorkspace& ws, FrzMatchDev* d_out, cudaStream_t stream) {
+                           FrzWorkspace& ws, FrzMatchDev* d_out, const FrzScoreHist& hist, cudaStream_t stream) {
     // persistent grids: a multiple of the SM count
     const int blocks = frz_sm_count() * 2;
     const int rev = reversed ? 1 : 0;
@@ -341,13 +347,13 @@ frz_status launch_sw_lanes(const FrzCorpusView& cv, const FrzPatternDev& pat, ui
     const bool lane_pen = !pat.wrap8 && pat.gap_extend == 0 && pat.gap_open_x > 0;
     if (pat.wrap8)
         k_sw64<LANES, true><<<frz_sm_count() * kSw64MinBlocks<LANES, true>, kSwThreads, 0, stream>>>(
-            cv, pat, ws.lists(), ws.survivor_cap, rank_view(ws), ws.counters, index_offset, rev, d_out);
+            cv, pat, ws.lists(), ws.survivor_cap, rank_view(ws), ws.counters, index_offset, rev, d_out, hist);
     else if (lane_pen)
         k_sw64<LANES, false, 8 | kSwVarLanePen><<<frz_sm_count() * kSw64MinBlocks<LANES, false>, kSwThreads, 0, stream>>>(
-            cv, pat, ws.lists(), ws.survivor_cap, rank_view(ws), ws.counters, index_offset, rev, d_out);
+            cv, pat, ws.lists(), ws.survivor_cap, rank_view(ws), ws.counters, index_offset, rev, d_out, hist);
     else
         k_sw64<LANES, false, 8><<<frz_sm_count() * kSw64MinBlocks<LANES, false>, kSwThreads, 0, stream>>>(
-            cv, pat, ws.lists(), ws.survivor_cap, rank_view(ws), ws.counters, index_offset, rev, d_out);
+            cv, pat, ws.lists(), ws.survivor_cap, rank_view(ws), ws.counters, index_offset, rev, d_out, hist);
     // windows of 65..128 bytes only exist when some haystack of the corpus is longer than 64 bytes (recorded at pack time)
     if (cv.max_gunits <= 4) { FRZ_CUDA_TRY(cudaGetLastError()); return FRZ_OK; }
     const size_t smem = SwCore<LANES, 128, false>::smem_bytes;
@@ -361,14 +367,14 @@ frz_status launch_sw_lanes(const FrzCorpusView& cv, const FrzPatternDev& pat, ui
     }
     if (pat.wrap8)
         k_sw<LANES, 128, true><<<blocks, kSwThreads, smem, stream>>>(cv, pat, ws.survivors[FRZ_C_COLS128], ws.survivor_cap, FRZ_C_COLS128,
-                                                                    rank_view(ws), ws.counters, index_offset, rev, d_out);
+                                                                    rank_view(ws), ws.counters, index_offset, rev, d_out, hist);
     else if (lane_pen)
         k_sw<LANES, 128, false, kSwVarLanePen><<<blocks, kSwThreads, smem, stream>>>(cv, pat, ws.survivors[FRZ_C_COLS128], ws.survivor_cap,
                                                                                   FRZ_C_COLS128, rank_view(ws), ws.counters, index_offset,
-                                                                                  rev, d_out);
+                                                                                  rev, d_out, hist);
     else
         k_sw<LANES, 128, false><<<blocks, kSwThreads, smem, stream>>>(cv, pat, ws.survivors[FRZ_C_COLS128], ws.survivor_cap, FRZ_C_COLS128,
-                                                                     rank_view(ws), ws.counters, index_offset, rev, d_out);
+                                                                     rank_view(ws), ws.counters, index_offset, rev, d_out, hist);
     FRZ_CUDA_TRY(cudaGetLastError());
     return FRZ_OK;
 }
@@ -376,25 +382,25 @@ frz_status launch_sw_lanes(const FrzCorpusView& cv, const FrzPatternDev& pat, ui
 }  // namespace
 
 frz_status frz_launch_sw(const FrzCorpusView& cv, const FrzPatternDev& pat, uint32_t index_offset, bool reversed,
-                         FrzWorkspace& ws, FrzMatchDev* d_out, cudaStream_t stream, FrzLaunchStats* st) {
+                         FrzWorkspace& ws, FrzMatchDev* d_out, cudaStream_t stream, FrzLaunchStats* st, const FrzScoreHist& hist) {
     if (cv.n_tiles == 0) return FRZ_OK;
     if (pat.typo_mode == FRZ_T_LITERAL) {
         k_emit_literal<<<frz_sm_count() * 4, 256, 0, stream>>>(ws.survivors[FRZ_C_COLS64], ws.survivor_cap, rank_view(ws), ws.counters,
-                                                           index_offset, reversed ? 1 : 0, d_out);
+                                                           index_offset, reversed ? 1 : 0, d_out, hist);
         FRZ_CUDA_TRY(cudaGetLastError());
         if (st) st->launches++;
         return FRZ_OK;
     }
     switch (pat.sw_lanes) {
-        case 64: FRZ_TRY(launch_sw_lanes<64>(cv, pat, index_offset, reversed, ws, d_out, stream)); break;
-        case 32: FRZ_TRY(launch_sw_lanes<32>(cv, pat, index_offset, reversed, ws, d_out, stream)); break;
-        case 16: FRZ_TRY(launch_sw_lanes<16>(cv, pat, index_offset, reversed, ws, d_out, stream)); break;
-        case 8: FRZ_TRY(launch_sw_lanes<8>(cv, pat, index_offset, reversed, ws, d_out, stream)); break;
+        case 64: FRZ_TRY(launch_sw_lanes<64>(cv, pat, index_offset, reversed, ws, d_out, hist, stream)); break;
+        case 32: FRZ_TRY(launch_sw_lanes<32>(cv, pat, index_offset, reversed, ws, d_out, hist, stream)); break;
+        case 16: FRZ_TRY(launch_sw_lanes<16>(cv, pat, index_offset, reversed, ws, d_out, hist, stream)); break;
+        case 8: FRZ_TRY(launch_sw_lanes<8>(cv, pat, index_offset, reversed, ws, d_out, hist, stream)); break;
         default: return frz_fail(FRZ_ERR_INVALID_ARG, "unsupported lane count %d", pat.sw_lanes);
     }
     if (cv.max_gunits > 8) {   // windows > 128 bytes need a haystack > 128 bytes
         k_sw_generic<<<frz_sm_count() * 2, 64, 0, stream>>>(cv, pat, ws.survivors[FRZ_C_GENERIC], ws.survivor_cap, FRZ_C_GENERIC, rank_view(ws),
-                                                        ws.counters, index_offset, reversed ? 1 : 0, d_out);
+                                                        ws.counters, index_offset, reversed ? 1 : 0, d_out, hist);
     }
     FRZ_CUDA_TRY(cudaGetLastError());
     if (st) st->launches += 1 + (cv.max_gunits > 4 ? 1 : 0) + (cv.max_gunits > 8 ? 1 : 0);
