@@ -483,16 +483,16 @@ __device__ __forceinline__ void emit_commit(const Emit& e, const FrzSurvLists& l
 }
 
 // ================================================================================================================
-// Stage 1a  k_sig_scan — the streaming half.  Lane per FOUR consecutive haystacks: one 16-byte load of their lengths and
+// k_sig_scan — the streaming signature scan alone: the unicode path's first stage (k_scan_window scans the same way on
+// the byte path).  Lane per FOUR consecutive haystacks: one 16-byte load of their lengths and
 // two 16-byte loads of their byte-class signatures (written at pack time, pack.cu: k_pack_sig) decide "can this
 // haystack hold the needle up to the typo budget?" (two POPCs each).  The haystack bytes themselves are never touched
 // here: a rejected haystack costs 12 bytes of HBM traffic instead of len + 8.  Survivors of the test become 16-byte
 // candidate records {tile << 10 | slot, len << 10 | index-in-tile, address of unit 0}: the group descriptor is resolved
-// here (four contiguous 16-byte descriptors per trip, L2-resident), so stage 1b starts its unit loads straight from the
+// here (four contiguous 16-byte descriptors per trip, L2-resident), so the consumer starts its unit loads straight from the
 // record.  Warp-autonomous: a per-warp ring in shared memory collects candidates, every 32 are flushed with ONE atomic
 // and one coalesced 512-byte store.  Small (about 40 registers): 12 blocks per SM keep enough bytes in flight to stream
-// at HBM speed — in the fused kernel the same loop spent most of its stalls waiting on its own loads behind
-// the 76-register window code.
+// at HBM speed.
 constexpr int kScanThreads = 128;
 constexpr int kScanWarps = kScanThreads / 32;
 constexpr int kScanRing = 256;   // entries per warp: up to 31 left over + up to 128 new per trip
@@ -686,98 +686,147 @@ __global__ void __launch_bounds__(kScanThreads, TMA ? 6 : 10) k_sig_scan(const F
 }
 
 // ================================================================================================================
-// Stage 1b  k_window — the exact reference window (process_candidate) on the candidates, lane per candidate.
-// Work items are 32 consecutive candidate records, claimed from a device counter.  The loop is software-pipelined two
-// items deep: while item i is in the mask builders / state machine, item i+1's haystack units travel global → shared
-// with cp.async (the record carries the unit address: no dependent descriptor load) and item i+2's records are in
-// flight — the scattered unit loads are what phase B of the fused kernel stalled on.
-constexpr int kWinThreads = 128;
-constexpr int kWinWarps = kWinThreads / 32;
+// Stage 1 of the whole-corpus byte path  k_scan_window — the signature scan of k_sig_scan<true> and the exact reference
+// window (process_candidate) in one persistent kernel.  The scan keeps HBM busy and leaves the ALUs idle, the window
+// machine the other way round; in one kernel an SM's warps do both at once, and the candidates never leave the SM.
+// Each warp:
+//   - walks its statically strided 128-slot chunks like k_sig_scan<true> (TMA stages, per-warp mbarriers) and appends the
+//     records of the haystacks that pass the length gate and the signature test to its shared-memory ring;
+//   - after each chunk, takes every 32 records in the ring as a BATCH (lane per candidate): their haystack units travel
+//     global → shared with cp.async while the warp scans on, and the batch is windowed and emitted when the next one is
+//     taken (or at the end).  The chunk's TMA refill is issued before any batch runs, so the warp's DRAM requests stay
+//     in flight (bulk copies hold no registers) while it runs the state machine.
+// Haystacks of more than four units (staged == false) are read by the mask builders straight from the corpus.
+constexpr int kFusedStages = 2;   // TMA stages per warp: two keep four blocks per SM within the shared memory
 struct WinStage {
     uint4 units[32][5];   // [lane][unit]: the lane's four units contiguous like in the packed corpus; the fifth pads the row
                           // to 80 bytes, which makes the warp's 16-byte accesses bank-conflict-free (rows of 64 would be 4-way)
 };
-struct WinSmem {
-    uint2 occ[kMaxDistinct][32];
-    WinStage stage[2];
-    uint4 rec[3][32];     // candidate records of items k, k+1, k+2 (ring), also filled by cp.async
+struct __align__(16) ScanWinSmem {   // one warp's part of the dynamic shared memory
+    CandRec ring[kScanRing];         // at most 31 left over + 128 new records between two batch takes
+    ScanStage stage[kFusedStages];
+    WinStage win;
+    uint64_t bar[kFusedStages];
 };
+// The kWarps ScanWinSmem are followed by one occurrence table per warp (OccTable's layout) of `occ_rows` rows: only the
+// rows the mask builders touch, n_distinct (+ n for the single-chunk forms' position masks).
 
 template <int MODE>
-__global__ void __launch_bounds__(kWinThreads, 4) k_window(const FrzCorpusView cv, const __grid_constant__ FrzPatternDev pat,
-                                                           const CandRec* __restrict__ cand, unsigned long long cand_cap,
-                                                           const FrzSurvLists lists, unsigned long long surv_cap,
-                                                           uint32_t* __restrict__ surv_bitmap, FrzCounters* __restrict__ ctr,
-                                                           uint32_t flags) {
+__global__ void __launch_bounds__(kThreads, 4) k_scan_window(const FrzCorpusView cv, const __grid_constant__ FrzPatternDev pat,
+                                                             int use_sig, int occ_rows, const FrzSurvLists lists,
+                                                             unsigned long long surv_cap, uint32_t* __restrict__ surv_bitmap,
+                                                             FrzCounters* __restrict__ ctr, uint32_t flags) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const uint32_t lane = frz_lane(), warp = threadIdx.x >> 5;
-    WinSmem& sm = reinterpret_cast<WinSmem*>(smem_raw)[warp];
+    ScanWinSmem& sm = reinterpret_cast<ScanWinSmem*>(smem_raw)[warp];
+    uint2 (*occ)[32] = reinterpret_cast<uint2 (*)[32]>(smem_raw + sizeof(ScanWinSmem) * kWarps) + (size_t)warp * occ_rows;
     __shared__ uint8_t cid_s[FRZ_MAX_NEEDLE];
     if (threadIdx.x < FRZ_MAX_NEEDLE) cid_s[threadIdx.x] = pat.cid[threadIdx.x];
+    if (lane == 0)
+        for (int i = 0; i < kFusedStages; i++) mbar_init(&sm.bar[i], 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     __syncthreads();
-    const unsigned long long n_cand = min(ctr->cand_count, cand_cap);
-    const uint32_t n_items = (uint32_t)((n_cand + 31) >> 5);
     const bool staged = cv.max_gunits <= 4;   // every haystack fits the four staged units
     const bool single = (MODE == FRZ_T_0 || MODE == FRZ_T_1) && (flags & 1u) && single_chunk_ok(pat, cv.max_gunits);
-
-    // Work items are strided statically over the warps of the grid (their cost is uniform), so the item sequence of a warp
-    // is known ahead: item k's units AND item k+1's records were requested with cp.async one iteration earlier (records
-    // fetched into registers were sunk by ptxas to their first use, where the warp stalled on them).
-    //   group G_k (committed in iteration k) = { units of item k+1 , records of item k+2 }
-    const uint32_t n_warps = gridDim.x * kWinWarps;
-    const uint32_t item0 = blockIdx.x * kWinWarps + warp;
-    auto fetch_rec = [&](uint32_t k) {   // records of this warp's k-th item → ring slot k % 3
-        const uint32_t item = item0 + k * n_warps;
-        const unsigned long long j = (unsigned long long)item * 32 + lane;
-        uint4* dst = &sm.rec[k % 3][lane];
-        if (item < n_items && j < n_cand) __pipeline_memcpy_async(dst, reinterpret_cast<const uint4*>(cand) + j, 16);
-        else *dst = make_uint4(0xFFFFFFFFu, 0u, 0u, 0u);
-    };
-    auto unit0_of = [](const uint4& r) { return ((unsigned long long)r.w << 32) | r.z; };
-    auto fetch_units = [&](const uint4& r, int st) {
-        if (staged && r.x != 0xFFFFFFFFu) {
-            const int units = ((int)(r.y >> FRZ_TILE_SHIFT) + 15) >> 4;
-            const uint4* base = cv.data + unit0_of(r);
-#pragma unroll
-            for (int k = 0; k < 4; k++)
-                if (k < units) __pipeline_memcpy_async(&sm.stage[st].units[lane][k], base + k, 16);
+    const uint32_t n_warps = gridDim.x * kWarps;
+    const uint32_t total_chunks = cv.n_tiles * (FRZ_TILE / 128);   // 128 slots (4 groups) per chunk
+    const uint32_t tx_bytes = (uint32_t)(sizeof(uint32_t) * 128 + sizeof(FrzGroupDesc) * 4) + (use_sig ? (uint32_t)sizeof(uint2) * 128 : 0u);
+    uint32_t req = blockIdx.x * kWarps + warp;   // next chunk to REQUEST
+    auto issue = [&](int st) {
+        if (req < total_chunks && lane == 0) {
+            const uint64_t slot0 = (uint64_t)req * 128;
+            mbar_expect_tx(&sm.bar[st], tx_bytes);
+            bulk_g2s(sm.stage[st].meta, cv.slot_meta + slot0, (uint32_t)sizeof(uint32_t) * 128, &sm.bar[st]);
+            if (use_sig) bulk_g2s(sm.stage[st].sig, cv.slot_sig + slot0, (uint32_t)sizeof(uint2) * 128, &sm.bar[st]);
+            bulk_g2s(sm.stage[st].desc, cv.groups + (size_t)req * 4, (uint32_t)sizeof(FrzGroupDesc) * 4, &sm.bar[st]);
         }
+        req += n_warps;
     };
-    fetch_rec(0);
-    fetch_rec(1);
-    __pipeline_commit();
-    __pipeline_wait_prior(0);
-    __syncwarp();
-    fetch_units(sm.rec[0][lane], 0);
-    __pipeline_commit();
+    uint4* ring = reinterpret_cast<uint4*>(sm.ring);
+    uint32_t head = 0, count = 0;
+    // the batch whose units are in flight: this lane's candidate record (x == 0xFFFFFFFF: none)
+    uint4 batch = make_uint4(0xFFFFFFFFu, 0u, 0u, 0u);
+    bool batch_pending = false;
     Emit pending;
     pending.ok = false; pending.cls = 0; pending.peers = 0; pending.base_raw = 0;
     pending.rec.tile = 0; pending.rec.slot_rank = 0; pending.rec.start = 0; pending.rec.end = 0;
-    for (uint32_t k = 0; item0 + k * n_warps < n_items; k++) {
-        __pipeline_wait_prior(0);                        // G_{k-1}: this item's units and the next item's records
+    auto run_batch = [&]() {
+        __pipeline_wait_prior(0);
         __syncwarp();
-        const uint4 rec0 = sm.rec[k % 3][lane];
-        fetch_units(sm.rec[(k + 1) % 3][lane], (k + 1) & 1);
-        fetch_rec(k + 2);
-        __pipeline_commit();                             // G_k flies while item k is processed
-        const int st = k & 1;
-        const bool active = rec0.x != 0xFFFFFFFFu;
+        const bool active = batch.x != 0xFFFFFFFFu;
         Cand cd;
-        cd.tile = rec0.x >> FRZ_TILE_SHIFT;
-        cd.slot = rec0.x & (FRZ_TILE - 1);
-        cd.li = rec0.y & (FRZ_TILE - 1);
-        cd.len = (int)(rec0.y >> FRZ_TILE_SHIFT);
-        cd.base = cv.data + unit0_of(rec0);
-        cd.units = staged ? &sm.stage[st].units[lane][0] : cd.base;
+        cd.tile = batch.x >> FRZ_TILE_SHIFT;
+        cd.slot = batch.x & (FRZ_TILE - 1);
+        cd.li = batch.y & (FRZ_TILE - 1);
+        cd.len = (int)(batch.y >> FRZ_TILE_SHIFT);
+        cd.base = cv.data + (((unsigned long long)batch.w << 32) | batch.z);
+        cd.units = staged ? &sm.win.units[lane][0] : cd.base;
         Emit cur;
-        process_candidate<MODE>(cv, pat, cid_s, sm.occ, cd, active, surv_bitmap, &cur, single);
-        emit_commit(pending, lists, surv_cap, ctr);      // the previous item's list space has arrived by now
+        process_candidate<MODE>(cv, pat, cid_s, occ, cd, active, surv_bitmap, &cur, single);
+        emit_commit(pending, lists, surv_cap, ctr);      // the previous batch's list space has arrived by now
         emit_request(cur, ctr);
         pending = cur;
         __syncwarp();
+    };
+    // the n (<= 32) oldest ring records become the next batch; the previous batch runs first (one unit stage)
+    auto take_batch = [&](uint32_t n) {
+        if (batch_pending) run_batch();
+        batch = lane < n ? ring[(head + lane) & (kScanRing - 1)] : make_uint4(0xFFFFFFFFu, 0u, 0u, 0u);
+        head = (head + n) & (kScanRing - 1);
+        count -= n;
+        if (staged && batch.x != 0xFFFFFFFFu) {
+            const int units = ((int)(batch.y >> FRZ_TILE_SHIFT) + 15) >> 4;
+            const uint4* base = cv.data + (((unsigned long long)batch.w << 32) | batch.z);
+#pragma unroll
+            for (int k = 0; k < 4; k++)
+                if (k < units) __pipeline_memcpy_async(&sm.win.units[lane][k], base + k, 16);
+        }
+        __pipeline_commit();
+        batch_pending = true;
+    };
+    // length gate + signature test of one slot; passing lanes append their record to the ring
+    auto test_slot = [&](uint32_t m, uint32_t p1, uint32_t p2, uint32_t slot_global, unsigned long long unit0) {
+        bool pass = m != FRZ_INVALID_SLOT && (int)(m >> FRZ_TILE_SHIFT) >= pat.min_hay_len;
+        if (use_sig) pass = pass && frz_sig_pass(pat.sig_need1, pat.sig_need2, pat.sig_k, p1, p2);
+        const uint32_t ballot = __ballot_sync(0xffffffffu, pass);
+        if (pass)
+            ring[(head + count + __popc(ballot & ((1u << lane) - 1))) & (kScanRing - 1)] =
+                make_uint4(slot_global, m, (uint32_t)unit0, (uint32_t)(unit0 >> 32));
+        count += __popc(ballot);
+    };
+    uint32_t cur = req;
+#pragma unroll
+    for (int i = 0; i < kFusedStages; i++) issue(i);
+    int st = 0;
+    uint32_t parity = 0;
+    while (cur < total_chunks) {
+        mbar_wait(&sm.bar[st], parity);
+        const uint4 meta = reinterpret_cast<const uint4*>(sm.stage[st].meta)[lane];
+        uint4 sig0 = make_uint4(0u, 0u, 0u, 0u), sig1 = sig0;
+        if (use_sig) {
+            sig0 = reinterpret_cast<const uint4*>(sm.stage[st].sig)[2 * lane];
+            sig1 = reinterpret_cast<const uint4*>(sm.stage[st].sig)[2 * lane + 1];
+        }
+        const unsigned long long grp_off = sm.stage[st].desc[lane >> 3].abs_off;
+        const uint32_t gunits = sm.stage[st].desc[lane >> 3].gunits;
+        __syncwarp();
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic reads of the stage before its async refill
+        issue(st);
+        // lane L owns slots 4L .. 4L+3 of the chunk, all in group L / 8
+        const uint32_t slot_g = cur * 128 + lane * 4;                   // == tile << 10 | slot of this lane's first slot
+        const unsigned long long unit0 = grp_off + (unsigned long long)((lane * 4) & 31) * gunits;   // slot-major group
+        test_slot(meta.x, sig0.x, sig0.y, slot_g, unit0);
+        test_slot(meta.y, sig0.z, sig0.w, slot_g + 1, unit0 + gunits);
+        test_slot(meta.z, sig1.x, sig1.y, slot_g + 2, unit0 + 2 * gunits);
+        test_slot(meta.w, sig1.z, sig1.w, slot_g + 3, unit0 + 3 * gunits);
+        __syncwarp();
+        while (count >= 32) take_batch(32);
+        cur += n_warps;
+        if (++st == kFusedStages) { st = 0; parity ^= 1; }
     }
+    if (count) take_batch(count);   // partial batch: lanes >= count are inactive
+    if (batch_pending) run_batch();
     emit_commit(pending, lists, surv_cap, ctr);
-    __pipeline_wait_prior(0);
 }
 
 // Candidate-list mode (multi-pattern, src/matcher/multi.rs:108-120): the extra patterns are evaluated only
@@ -836,15 +885,26 @@ __global__ void __launch_bounds__(256) k_tile_rank(const uint32_t* __restrict__ 
 
 // exclusive scan of tile_count → tile_out_base; total → counters.total.  One block; every thread owns a CONTIGUOUS run
 // of ceil(n / 1024) tiles, so the block makes one pass (two for > 1 M tiles) instead of n / 1024 barrier rounds.
+// Up to kTileScanSmem tiles the counts go through shared memory: loaded and stored coalesced, the per-thread runs walk
+// shared memory (a run walked in global memory is a chain of dependent loads per thread).  Larger corpora walk the
+// global arrays.
 // `carry` (optional): the scan starts at *carry and leaves the new total there too — streamed calls (host.cu:
 // frz_match_shard_streamed) run the pipeline over consecutive tile ranges and append each range's matches to the same list.
+constexpr uint32_t kTileScanSmem = 12224;   // with warp_sum, 48 KB of static shared memory; the sum of the counts (<= 1024 per tile) fits 32 bits
 __global__ void __launch_bounds__(1024) k_tile_scan(const uint32_t* __restrict__ tile_count, uint64_t* __restrict__ out,
                                                     uint32_t n, FrzCounters* __restrict__ ctr, unsigned long long* carry) {
     __shared__ uint64_t warp_sum[32];
+    __shared__ uint32_t cnt_s[kTileScanSmem];
+    const bool in_smem = n <= kTileScanSmem;
+    if (in_smem) {
+        for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) cnt_s[i] = tile_count[i];
+        __syncthreads();
+    }
+    const uint32_t* cnt = in_smem ? cnt_s : tile_count;
     const uint32_t per = (n + blockDim.x - 1) / blockDim.x;
     const uint32_t lo = min(threadIdx.x * per, n), hi = min(lo + per, n);
     uint64_t sum = 0;
-    for (uint32_t i = lo; i < hi; i++) sum += tile_count[i];
+    for (uint32_t i = lo; i < hi; i++) sum += cnt[i];
     uint64_t x = sum;
     for (int d = 1; d < 32; d <<= 1) {
         uint64_t y = __shfl_up_sync(0xffffffffu, x, d);
@@ -864,9 +924,21 @@ __global__ void __launch_bounds__(1024) k_tile_scan(const uint32_t* __restrict__
     const uint64_t start = carry ? *carry : 0ull;
     __syncthreads();                                        // everybody has read the carry before the last thread replaces it
     uint64_t run = start + warp_sum[threadIdx.x >> 5] + x - sum;   // exclusive prefix of this thread's run
-    for (uint32_t i = lo; i < hi; i++) {
-        out[i] = run;
-        run += tile_count[i];
+    if (in_smem) {   // exclusive prefixes (without the carry) in place, then one coalesced pass
+        uint32_t r = (uint32_t)(run - start);
+        for (uint32_t i = lo; i < hi; i++) {
+            const uint32_t c = cnt_s[i];
+            cnt_s[i] = r;
+            r += c;
+        }
+        run = start + r;
+        __syncthreads();
+        for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) out[i] = start + cnt_s[i];
+    } else {
+        for (uint32_t i = lo; i < hi; i++) {
+            out[i] = run;
+            run += tile_count[i];
+        }
     }
     if (threadIdx.x == blockDim.x - 1) {   // the last thread's run ends at n (empty runs carry the total)
         ctr->total = run;
@@ -965,8 +1037,8 @@ frz_status frz_launch_prefilter_list(const FrzCorpusView& cv, const FrzPatternDe
     return FRZ_OK;
 }
 
-// Stage 1a alone: the streaming signature scan over the whole corpus → candidate records in ws.cand_list, their number in
-// ws.counters->cand_count.  Shared by the byte path (k_window consumes the records) and the unicode path (k_unicode does).
+// The streaming signature scan alone over the whole corpus → candidate records in ws.cand_list, their number in
+// ws.counters->cand_count, for the unicode path (k_unicode consumes the records).
 frz_status frz_launch_sig_scan(const FrzCorpusView& cv, const FrzPatternDev& pat, FrzWorkspace& ws, cudaStream_t stream, FrzLaunchStats* st) {
     if (cv.n_tiles == 0) return FRZ_OK;
     const int sms = frz_sm_count();
@@ -1000,8 +1072,8 @@ frz_status frz_launch_sig_scan(const FrzCorpusView& cv, const FrzPatternDev& pat
     return FRZ_OK;
 }
 
-// Stage 1 of match_list over the whole corpus: k_sig_scan (streaming signature test → candidate records) and
-// k_window (exact windows of the candidates → survivor records + per-tile survivor bitmap).
+// Stage 1 of match_list over the whole corpus: k_scan_window (length gate + signature test + exact windows → survivor
+// records + per-tile survivor bitmap).
 frz_status frz_launch_prefilter(const FrzCorpusView& cv, const FrzPatternDev& pat, FrzWorkspace& ws, cudaStream_t stream,
                                 FrzLaunchStats* st) {
     if (cv.n_tiles == 0) return FRZ_OK;
@@ -1010,26 +1082,23 @@ frz_status frz_launch_prefilter(const FrzCorpusView& cv, const FrzPatternDev& pa
     static int single_knob = -1;   // A/B knob: FRZ_PF_SINGLE=0 keeps the general (multi-chunk) mask forms
     if (single_knob < 0) { const char* e = getenv("FRZ_PF_SINGLE"); single_knob = e ? atoi(e) : 1; }
     const uint32_t pf_flags = single_knob ? 1u : 0u;
-    CandRec* cand = reinterpret_cast<CandRec*>(ws.cand_list);
-    FRZ_TRY(frz_launch_sig_scan(cv, pat, ws, stream, st));   // 1a
-    const size_t smem = sizeof(WinSmem) * kWinWarps;
+    const int use_sig = pat.typo_mode != FRZ_T_NONE && pat.sig_on;
+    const int occ_rows = pat.n_distinct ? std::min(kMaxDistinct, pat.n_distinct + pat.n) : 0;
+    const size_t smem = (sizeof(ScanWinSmem) + sizeof(uint2) * 32 * occ_rows) * kWarps;
+    const size_t smem_max = (sizeof(ScanWinSmem) + sizeof(OccTable)) * kWarps;
+    const uint32_t total_chunks = cv.n_tiles * (FRZ_TILE / 128);
 #define FRZ_PF_LAUNCH(MODE)                                                                                              \
     do {                                                                                                                 \
-        static int bps_dev[64] = {};                                                                                     \
-        int& bps = bps_dev[frz_current_device() & 63];                                                                   \
+        static int bps_dev[64][kMaxDistinct + 1] = {};   /* blocks per SM by device and occurrence-table rows */         \
+        int& bps = bps_dev[frz_current_device() & 63][occ_rows];                                                         \
         if (!bps) {                                                                                                      \
-            FRZ_CUDA_TRY(cudaFuncSetAttribute(k_window<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));  \
-            FRZ_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_window<MODE>, kWinThreads, smem));        \
-            static int knob = -1;   /* experiment knob: FRZ_PF_BLOCKS caps the resident blocks per SM */                 \
-            if (knob < 0) { const char* e = getenv("FRZ_PF_BLOCKS"); knob = e ? atoi(e) : 0; }                           \
-            /* on an H100 (400 W) capping at 3, 4, 5 or not at all moved the stage by less than its run-to-run spread */ \
-            /* (193-207 us per 10 M haystacks), so the cap stays at 5 */                                                 \
-            if (knob > 0) bps = std::min(bps, knob);                                                                     \
-            else if (bps > 5) bps = 5;                                                                                   \
+            FRZ_CUDA_TRY(cudaFuncSetAttribute(k_scan_window<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max)); \
+            FRZ_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_scan_window<MODE>, kThreads, smem));      \
             if (bps < 1) bps = 1;                                                                                        \
         }                                                                                                                \
-        k_window<MODE><<<sms * bps, kWinThreads, smem, stream>>>(cv, pat, cand, ws.cand_cap, ws.lists(), ws.survivor_cap, \
-                                                                 ws.surv_bitmap, ws.counters, pf_flags);                 \
+        const uint32_t grid = std::max<uint32_t>(1, std::min<uint32_t>((uint32_t)(sms * bps), (total_chunks + kWarps - 1) / kWarps)); \
+        k_scan_window<MODE><<<grid, kThreads, smem, stream>>>(cv, pat, use_sig, occ_rows, ws.lists(), ws.survivor_cap,   \
+                                                              ws.surv_bitmap, ws.counters, pf_flags);                    \
     } while (0)
     switch (pat.typo_mode) {
         case FRZ_T_0: FRZ_PF_LAUNCH(FRZ_T_0); break;

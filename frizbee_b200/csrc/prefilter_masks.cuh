@@ -59,7 +59,7 @@ FRZ_PF_FN uint32_t zero_flags(uint32_t x) {
 
 // occ[d][lane] = occurrence mask of distinct class d over bytes [64*blk, 64*blk+64) of the lane's haystack.
 // `base` points at unit 0 of the lane's haystack, unit k at base + k — in the packed corpus, or in the lane's row of
-// the shared-memory stage k_window fills with cp.async (same layout).  `units` = ceil(len / 16) bounds the reads.
+// the shared-memory stage k_scan_window fills with cp.async (same layout).  `units` = ceil(len / 16) bounds the reads.
 FRZ_PF_FN void build_block_masks(const uint4* base, int units, int blk, const FrzPatternDev& pat,
                                                   uint2 (*occ)[32], uint32_t lane) {
     uint32_t w[16];
