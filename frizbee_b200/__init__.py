@@ -87,6 +87,7 @@ def lib():
     L.frz_matcher_backend_info.argtypes = [vp, sz] + [C.POINTER(C.c_int)] * 4
     L.frz_matcher_last_timings.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(u64)]
     L.frz_match_list.argtypes = [vp, vp, vp, u64, C.POINTER(u64)]
+    L.frz_match_list_top.argtypes = [vp, vp, u64, vp, C.POINTER(u64), C.POINTER(u64)]
     L.frz_match_list_into.argtypes = [vp, vp, u32, vp, u64, C.POINTER(u64)]
     L.frz_match_list_host.argtypes = [vp, vp, vp, u64, C.c_int, vp, u64, C.POINTER(u64)]
     L.frz_match_list_host_arrow.argtypes = [vp, vp, vp, C.c_int, u64, C.c_int, vp, u64, C.POINTER(u64)]
@@ -306,6 +307,23 @@ class Matcher:
 
     def match_list(self, haystacks, device: int = 0) -> List[Match]:
         return _to_matches(self.match_list_array(haystacks, device))
+
+    def match_list_top_array(self, haystacks, k: int, device: int = 0, out: Optional[np.ndarray] = None) -> Tuple[np.ndarray, int]:
+        """Matcher::match_list truncated to its first k rows (frz_match_list_top): (array of min(k, total) matches, total).
+        `out` (optional) needs room for min(k, len(corpus)) matches: no more rows can match."""
+        corpus, owned = self._corpus(haystacks, device)
+        try:
+            need = min(int(k), corpus.n)
+            if out is None:
+                out = np.empty(max(1, need), dtype=MATCH_DTYPE)
+            elif len(out) < need:
+                raise ValueError(f"out holds {len(out)} matches; a top-{k} call on {corpus.n} haystacks needs {need}")
+            n, total = C.c_uint64(), C.c_uint64()
+            _check(lib().frz_match_list_top(self._h, corpus._h, int(k), out.ctypes.data, C.byref(n), C.byref(total)))
+            return out[: n.value], total.value
+        finally:
+            if owned:
+                corpus.close()
 
     def match_list_into_array(self, haystacks, index_offset: int = 0, device: int = 0) -> np.ndarray:
         """Specialized::match_list / Matcher::match_list_into: index order, unsorted."""

@@ -181,11 +181,14 @@ frz_status frz_launch_tile_scan(const FrzCorpusView& cv, FrzWorkspace& ws, cudaS
 frz_status frz_launch_sw(const FrzCorpusView& cv, const FrzPatternDev& pat, uint32_t index_offset, bool reversed,
                          FrzWorkspace& ws, FrzMatchDev* d_out, cudaStream_t stream, FrzLaunchStats* st,
                          const FrzScoreHist& hist = FrzScoreHist());
+// "no limit" for the sorts' `limit` argument: every position of a list is below it (lists hold at most 2^32 - 1 matches)
+constexpr uint32_t kFrzNoLimit = 0xFFFFFFFFu;
 // stable sort by descending score; the element count is read from device memory (*n_ptr).
 // d_tmp is only used when score_bound >= 1024 (two 8-bit passes); result always lands in d_out.
+// limit: only the sorted positions below it are stored (top-K calls); kFrzNoLimit sorts the whole list.
 frz_status frz_launch_sort_by_score_dev(const FrzMatchDev* d_in, FrzMatchDev* d_tmp, FrzMatchDev* d_out,
                                         const unsigned long long* n_ptr, uint32_t score_bound, FrzWorkspace& ws,
-                                        cudaStream_t stream, FrzLaunchStats* st);
+                                        cudaStream_t stream, FrzLaunchStats* st, uint32_t limit = kFrzNoLimit);
 size_t frz_sort_hist_words();
 frz_status frz_sort_hist_alloc(uint32_t** out);
 const uint32_t* frz_sort_digit_base(const FrzWorkspace& ws);
@@ -195,7 +198,7 @@ int frz_sort_single_pass_bins(uint32_t score_bound);   // bins of the single-pas
 // are below score_bound (< 1024).  The sort reads the count at *n_ptr and leaves the histogram zeroed for the next call.
 frz_status frz_sort_fused_prepare(FrzWorkspace& ws, uint64_t n_cap, uint32_t score_bound, cudaStream_t stream, FrzScoreHist* out);
 frz_status frz_launch_sort_fused(const FrzMatchDev* d_in, FrzMatchDev* d_out, const unsigned long long* n_ptr, const FrzScoreHist& hist,
-                                 FrzWorkspace& ws, cudaStream_t stream, FrzLaunchStats* st);
+                                 FrzWorkspace& ws, cudaStream_t stream, FrzLaunchStats* st, uint32_t limit = kFrzNoLimit);
 
 // k-way merge of per-shard runs (host.cu) with caller-owned scratch — one per concurrent user (parallel.cu: one per rank)
 #define FRZ_MERGE_MAX_RUNS 64
@@ -223,6 +226,9 @@ cudaEvent_t frz_matcher_table_event(const frz_matcher* m);
 // host Arrow buffers → the matcher's reusable packed corpus (the ingest half of frz_match_list_host_arrow)
 frz_status frz_matcher_ingest_e2e(frz_matcher* m, const uint8_t* bytes, const void* offsets, int offset_width, uint64_t n, int device,
                                   const frz_corpus** out);
+// frz_match_shard_device that writes only the first `limit` elements of the run (top-K calls; *d_count is the full count)
+frz_status frz_match_shard_device_top(frz_matcher* m, const frz_corpus* shard, uint32_t index_offset, frz_match* d_out, uint64_t cap,
+                                      uint64_t* d_count, void* stream, uint32_t limit);
 // frz_matcher_ingest_e2e + frz_match_shard_device in one pass: the match pipeline runs over consecutive tile ranges as their
 // H2D chunks land (prefilter → scan with carry → scoring append to one list), only the sort waits for the last chunk.
 frz_status frz_match_shard_streamed(frz_matcher* m, const uint8_t* bytes, const void* offsets, int offset_width, uint64_t n, int device,

@@ -1091,15 +1091,19 @@ frz_status match_into_device(frz_matcher* m, const FrzCorpusStorage& cs, uint32_
 }
 
 // Matcher::match_list on device: into (+reverse) (+stable score sort).  Result pointer + device count.
-__global__ void k_copy_n(const FrzMatchDev* __restrict__ in, FrzMatchDev* __restrict__ out, const unsigned long long* n_ptr) {
-    const unsigned long long n = *n_ptr;
+__global__ void k_copy_n(const FrzMatchDev* __restrict__ in, FrzMatchDev* __restrict__ out, const unsigned long long* n_ptr,
+                         uint32_t limit) {
+    const unsigned long long n = min(*n_ptr, (unsigned long long)limit);
     for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (unsigned long long)gridDim.x * blockDim.x)
         out[i] = in[i];
 }
 
-// `final_out` (optional, device, >= corpus length): where the final list must land
+// `final_out` (optional, device, >= corpus length): where the final list must land.  `limit` (top-K calls): only the first
+// `limit` positions of the final list are written (the sort's last scatter and the final copy drop the rest); the count in
+// ws.counters->total stays the full match count.
 frz_status match_list_device(frz_matcher* m, const FrzCorpusStorage& cs, uint32_t index_offset, uint8_t sort,
-                             FrzMatchDev** d_result, cudaStream_t stream, FrzLaunchStats* st, FrzMatchDev* final_out = nullptr) {
+                             FrzMatchDev** d_result, cudaStream_t stream, FrzLaunchStats* st, FrzMatchDev* final_out = nullptr,
+                             uint32_t limit = kFrzNoLimit) {
     FrzWorkspace& ws = m->ws;
     const bool reversed = sort == FRZ_SORT_INDEX_DESC || sort == FRZ_SORT_SCORE_THEN_INDEX_DESC;
     const bool by_score = sort == FRZ_SORT_SCORE_THEN_INDEX_ASC || sort == FRZ_SORT_SCORE_THEN_INDEX_DESC;
@@ -1121,12 +1125,12 @@ frz_status match_list_device(frz_matcher* m, const FrzCorpusStorage& cs, uint32_
             FRZ_TRY(ensure_multi_buffers(m, cs.n));
             tmp = m->multi_a;
         }
-        if (hist.counts) FRZ_TRY(frz_launch_sort_fused(d_list, other, &ws.counters->total, hist, ws, stream, st));
-        else FRZ_TRY(frz_launch_sort_by_score_dev(d_list, tmp, other, &ws.counters->total, bound, ws, stream, st));
+        if (hist.counts) FRZ_TRY(frz_launch_sort_fused(d_list, other, &ws.counters->total, hist, ws, stream, st, limit));
+        else FRZ_TRY(frz_launch_sort_by_score_dev(d_list, tmp, other, &ws.counters->total, bound, ws, stream, st, limit));
         m->last_sort_bins = frz_sort_single_pass_bins(bound);
         d_list = other;
     } else if (final_out && d_list != final_out) {
-        k_copy_n<<<grid_for(cs.n, 256), 256, 0, stream>>>(d_list, final_out, &ws.counters->total);
+        k_copy_n<<<grid_for(std::min<uint64_t>(cs.n, limit), 256), 256, 0, stream>>>(d_list, final_out, &ws.counters->total, limit);
         st->launches++;
         d_list = final_out;
     }
@@ -1165,6 +1169,21 @@ frz_status copy_out(frz_matcher* m, FrzMatchDev* d_list, frz_match* out, uint64_
     return FRZ_OK;
 }
 
+// top-K: the first min(k, total) matches → host; never a capacity error
+frz_status copy_out_top(frz_matcher* m, FrzMatchDev* d_list, uint64_t k, frz_match* out, uint64_t* n_out, uint64_t* n_total,
+                        cudaStream_t stream) {
+    FRZ_TRY(read_counters(m, stream));
+    const uint64_t total = m->ws.h_counters->total;
+    const uint64_t n = std::min(k, total);
+    if (n_out) *n_out = n;
+    if (n_total) *n_total = total;
+    if (n) {
+        FRZ_CUDA_TRY(cudaMemcpyAsync(out, d_list, n * sizeof(frz_match), cudaMemcpyDeviceToHost, stream));
+        FRZ_CUDA_TRY(cudaStreamSynchronize(stream));
+    }
+    return FRZ_OK;
+}
+
 }  // namespace
 
 extern "C" frz_status frz_match_list(frz_matcher* m, const frz_corpus* corpus, frz_match* out, uint64_t cap, uint64_t* n_out) {
@@ -1177,6 +1196,28 @@ extern "C" frz_status frz_match_list(frz_matcher* m, const frz_corpus* corpus, f
     for (int attempt = 0; attempt < 2; attempt++) {
         s = match_list_device(m, corpus->st, 0, m->config.sort, &d_list, stream, &st);
         if (s == FRZ_OK) s = copy_out(m, d_list, out, cap, n_out, stream);
+        if (s != kRetryOverflow) break;
+        FRZ_TRY(ensure_workspace(m, corpus->st, std::max<uint64_t>(corpus->st.n, 1)));  // worst-case lists, then once more
+    }
+    if (s == kRetryOverflow) s = frz_fail(FRZ_ERR_CUDA, "survivor list overflow persisted");
+    collect_timings(m, st);
+    return s;
+}
+
+// Matcher::match_list followed by truncation to the first k rows: the same pipeline with a limit on the final scatter and copy
+extern "C" frz_status frz_match_list_top(frz_matcher* m, const frz_corpus* corpus, uint64_t k, frz_match* out, uint64_t* n_out,
+                                         uint64_t* n_total) {
+    if (!m || !corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    if (!out && k > 0) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
+    FRZ_TRY(ensure_device(corpus->st.device));
+    cudaStream_t stream = nullptr;
+    FrzLaunchStats st;
+    FrzMatchDev* d_list = nullptr;
+    const uint32_t limit = (uint32_t)std::min<uint64_t>(k, kFrzNoLimit);   // a list never holds more than 2^32 - 1 matches
+    frz_status s = FRZ_OK;
+    for (int attempt = 0; attempt < 2; attempt++) {
+        s = match_list_device(m, corpus->st, 0, m->config.sort, &d_list, stream, &st, nullptr, limit);
+        if (s == FRZ_OK) s = copy_out_top(m, d_list, k, out, n_out, n_total, stream);
         if (s != kRetryOverflow) break;
         FRZ_TRY(ensure_workspace(m, corpus->st, std::max<uint64_t>(corpus->st.n, 1)));  // worst-case lists, then once more
     }
@@ -1336,6 +1377,12 @@ extern "C" frz_status frz_match_indices(frz_matcher* m, const frz_corpus* corpus
 
 extern "C" frz_status frz_match_shard_device(frz_matcher* m, const frz_corpus* shard, uint32_t index_offset, frz_match* d_out,
                                              uint64_t cap, uint64_t* d_count, void* stream_) {
+    return frz_match_shard_device_top(m, shard, index_offset, d_out, cap, d_count, stream_, kFrzNoLimit);
+}
+
+// frz_match_shard_device whose run holds only its first `limit` elements (the count is still the full match count)
+frz_status frz_match_shard_device_top(frz_matcher* m, const frz_corpus* shard, uint32_t index_offset, frz_match* d_out, uint64_t cap,
+                                      uint64_t* d_count, void* stream_, uint32_t limit) {
     if (!m || !shard || !d_out || !d_count) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
     FRZ_TRY(ensure_device(shard->st.device));
     cudaStream_t stream = (cudaStream_t)stream_;
@@ -1350,7 +1397,8 @@ extern "C" frz_status frz_match_shard_device(frz_matcher* m, const frz_corpus* s
     m->count_published = false;
     m->ws.arm_table_ev = true;
     m->ws.table_ev_recorded = false;
-    const frz_status ms = match_list_device(m, shard->st, index_offset, m->config.sort, &d_list, stream, &st, reinterpret_cast<FrzMatchDev*>(d_out));
+    const frz_status ms = match_list_device(m, shard->st, index_offset, m->config.sort, &d_list, stream, &st, reinterpret_cast<FrzMatchDev*>(d_out),
+                                            limit);
     m->early_count_dst = nullptr;
     m->ws.arm_table_ev = false;
     FRZ_TRY(ms);

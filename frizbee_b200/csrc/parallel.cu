@@ -26,6 +26,11 @@
 // "my slice has landed" flags that end a host-out step.  In the multi-process form the block (and the output
 // buffer) is a memfd segment that every rank maps and pins.
 //
+// Top-K calls (frz_match_list_parallel*_top) keep only the first K' = min(k, total) positions of the merged list: a run keeps its
+// order in the merge, so nothing past a run's own first k can land there — every GPU sorts only its run's first k, the slice
+// boundaries become lo[p] = K' * p / G, k_place walks the first min(k, n_q) elements and drops positions >= K', the slice
+// exchange sends only ranges inside [0, K'), and the all-gather moves each run's first min(k, n_q) elements.
+//
 // NCCL is resolved with dlopen at the first multi-GPU use: the library itself has no NCCL link dependency, a
 // process that already carries PyTorch's libnccl.so.2 shares it, and single-GPU users never need it.
 #include <dlfcn.h>
@@ -206,7 +211,7 @@ static_assert(sizeof(PlaceHeader) <= kPlaceHeaderBytes, "place header");
 struct PlaceMeta {
     unsigned char* peer[kMaxWorld];             // every rank's place buffer (header + slice elements) as mapped on THIS device
     unsigned long long lo[kMaxWorld + 1];       // slice boundaries in the merged list
-    unsigned long long total;
+    unsigned long long total;                   // positions kept: the merged list's length, or K' of a top-K call
     int world, rank, bins, parity;
 };
 // DIRECT form (template, opt-in with FRZ_PARALLEL_EXCHANGE=direct): the destination is the caller's HOST buffer itself (pinned +
@@ -226,7 +231,8 @@ __global__ void __launch_bounds__(256) k_place(const FrzMatchDev* __restrict__ r
         for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (unsigned long long)gridDim.x * blockDim.x) {
             const FrzMatchDev m = run[i];
             const uint32_t s = bins > 1 ? min((uint32_t)m.score, (uint32_t)bins - 1) : 0u;
-            host_out[pos0[s] + (i - gt[s])] = m;
+            const unsigned long long x = pos0[s] + (i - gt[s]);
+            if (x < meta.total) host_out[x] = m;
         }
         return;   // kernel completion + the stream-ordered "landed" flag make the stores visible to the host
     }
@@ -238,6 +244,7 @@ __global__ void __launch_bounds__(256) k_place(const FrzMatchDev* __restrict__ r
         const FrzMatchDev m = run[i];
         const uint32_t s = bins > 1 ? min((uint32_t)m.score, (uint32_t)bins - 1) : 0u;
         const unsigned long long x = pos0[s] + (i - gt[s]);
+        if (x >= total) continue;   // beyond the first K' of a top-K call
         int p = (int)min((unsigned long long)(world - 1), x * (unsigned long long)world / total);   // lo[p] = floor(total * p / world): at most one off
         while (p > 0 && x < lo_s[p]) p--;
         while (p + 1 < world && x >= lo_s[p + 1]) p++;
@@ -804,6 +811,7 @@ struct StepResult {
     frz_status status = FRZ_OK;
     std::string error;
     uint64_t total = 0;
+    uint64_t kept = 0;      // min(limit, total): the length of the list the call returns
     const FrzMatchDev* d_merged = nullptr;
 };
 
@@ -817,9 +825,10 @@ struct HostShard {
 
 // Everything one GPU does for one match_list_parallel call.  `seq` is the step number shared by all ranks.
 // `want_slices`: the caller only needs the list in host memory (no device copy of the whole merged list): slice exchange allowed.
-// Exactly one of `shard` (resident packed corpus) and `hs` (host buffers) is given.
+// Exactly one of `shard` (resident packed corpus) and `hs` (host buffers) is given.  `limit` (top-K calls, resident shards only):
+// only the first K' = min(limit, total) positions of the merged list are produced; UINT64_MAX for the whole list.
 frz_status rank_step(frz_comm* c, RankCtx& r, frz_matcher* m, const frz_corpus* shard, const HostShard* hs, uint32_t index_offset, uint64_t seq,
-                     frz_match* out_host, uint64_t cap, bool want_host, bool want_slices, StepResult* res) {
+                     frz_match* out_host, uint64_t cap, bool want_host, bool want_slices, uint64_t limit, StepResult* res) {
     FRZ_TRY(set_device(r.device));
     cudaStream_t main = nullptr;   // the device's legacy default stream: ordered with the caller's own default-stream work
     const int world = c->world;
@@ -847,8 +856,8 @@ frz_status rank_step(frz_comm* c, RankCtx& r, frz_matcher* m, const frz_corpus* 
         FRZ_TRY(frz_match_shard_streamed(r.clone, hs->bytes, hs->offsets, hs->offset_width, hs->n, r.device, index_offset,
                                          reinterpret_cast<frz_match*>(r.run), r.run_cap, reinterpret_cast<uint64_t*>(r.d_count), main));
     else
-        FRZ_TRY(frz_match_shard_device(r.clone, shard, index_offset, reinterpret_cast<frz_match*>(r.run), r.run_cap,
-                                       reinterpret_cast<uint64_t*>(r.d_count), main));
+        FRZ_TRY(frz_match_shard_device_top(r.clone, shard, index_offset, reinterpret_cast<frz_match*>(r.run), r.run_cap,
+                                           reinterpret_cast<uint64_t*>(r.d_count), main, (uint32_t)std::min<uint64_t>(limit, kFrzNoLimit)));
     FRZ_TRY(frz_matcher_wait_count(r.clone, r.side));
     k_publish<<<1, 1, 0, r.side>>>(reinterpret_cast<volatile unsigned long long*>(r.ctrl_dev + kCtrlCount + parity * kMaxWorld + r.rank),
                                    r.d_count, seq);
@@ -857,9 +866,17 @@ frz_status rank_step(frz_comm* c, RankCtx& r, frz_matcher* m, const frz_corpus* 
     // ---- the Vec lengths of all workers (k_merge.rs:96-104): polled from the shared block while the GPU scores
     uint64_t counts[kMaxWorld];
     FRZ_TRY(wait_slots(c->ctrl_host + kCtrlCount + parity * kMaxWorld, world, seq, counts, "match count"));
-    uint64_t stride = 1, total = 0;
-    for (int k = 0; k < world; k++) { stride = std::max(stride, counts[k]); total += counts[k]; }
+    // kept[q]: the part of run q the merge can need — its first min(limit, n_q) elements (all of them for a full call)
+    uint64_t kept[kMaxWorld], stride = 1, total = 0, kept_total = 0;
+    for (int k = 0; k < world; k++) {
+        kept[k] = std::min(counts[k], limit);
+        stride = std::max(stride, kept[k]);
+        total += counts[k];
+        kept_total += kept[k];
+    }
+    const uint64_t kp = std::min(total, limit);   // K': positions of the merged list this call produces
     res->total = total;
+    res->kept = kp;
     const bool collective = world > 1 || c->force_nccl;
     const FrzMatchDev* d_final = r.run;
     uint64_t d_final_first = 0;   // merged position of d_final[0] (non-zero in the slice form)
@@ -876,12 +893,12 @@ frz_status rank_step(frz_comm* c, RankCtx& r, frz_matcher* m, const frz_corpus* 
     int bins = 1;
     const uint32_t* d_table = nullptr;
     if (by_score) d_table = frz_matcher_last_sort_table(r.clone, &bins);
-    const bool slice_form = want_host && want_slices && world > 1 && r.nccl && c->slice_exchange && (!by_score || bins > 0) && total > 0 &&
+    const bool slice_form = want_host && want_slices && world > 1 && r.nccl && c->slice_exchange && (!by_score || bins > 0) && kp > 0 &&
                             total <= 0xFFFFFFFFull;
     if (slice_form) {
-        if (total > cap) {
+        if (kp > cap) {
             FRZ_CUDA_TRY(cudaStreamSynchronize(main));
-            return frz_fail(FRZ_ERR_CAPACITY, "output capacity %llu < %llu matches", (unsigned long long)cap, (unsigned long long)total);
+            return frz_fail(FRZ_ERR_CAPACITY, "output capacity %llu < %llu matches", (unsigned long long)cap, (unsigned long long)kp);
         }
         if (!out_host) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
         // direct form: the caller's buffer mapped on every GPU?  Else the slice buffers of the P2P placement (collective,
@@ -889,7 +906,7 @@ frz_status rank_step(frz_comm* c, RankCtx& r, frz_matcher* m, const frz_corpus* 
         FrzMatchDev* direct_out = nullptr;
         FRZ_TRY(negotiate_direct(c, r, out_host, cap, &direct_out));
         bool place_ready = direct_out != nullptr;
-        if (!direct_out) FRZ_TRY(ensure_place_buffers(c, r, total / (uint64_t)world + 2, &place_ready));
+        if (!direct_out) FRZ_TRY(ensure_place_buffers(c, r, kp / (uint64_t)world + 2, &place_ready));
         // 1. my table → shared block (after the local pipeline on the main stream), everybody's tables ← shared block
         volatile uint32_t* tab_host = c->tables_host + ((size_t)parity * world) * kTableBins;
         if (by_score) {
@@ -908,7 +925,7 @@ frz_status rank_step(frz_comm* c, RankCtx& r, frz_matcher* m, const frz_corpus* 
         // 2. merged positions: pos0[q][s] = everything scoring higher than s in any run + the score-s blocks of the runs
         //    that precede q in merge order; A[q][p] = how many elements of run q lie before slice boundary lo_p
         uint64_t lo_p[kMaxWorld + 1];
-        for (int p2 = 0; p2 <= world; p2++) lo_p[p2] = total * (uint64_t)p2 / (uint64_t)world;
+        for (int p2 = 0; p2 <= world; p2++) lo_p[p2] = kp * (uint64_t)p2 / (uint64_t)world;
       if (place_ready) {
         // ---- P2P PLACEMENT: only MY run's rows of pos0 / gt are needed; k_place stores every element of my run at its merged
         // position inside the owning rank's slice buffer (peer memory over NVLink) and ends when all peers have done the same
@@ -930,15 +947,15 @@ frz_status rank_step(frz_comm* c, RankCtx& r, frz_matcher* m, const frz_corpus* 
         memset(&meta, 0, sizeof meta);
         for (int q = 0; q < world; q++) meta.peer[q] = r.peer_raw[q];
         for (int p2 = 0; p2 <= world; p2++) meta.lo[p2] = lo_p[p2];
-        meta.total = total; meta.world = world; meta.rank = r.rank; meta.bins = bins; meta.parity = parity;
-        const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((counts[r.rank] + 255) / 256, (uint64_t)frz_sm_count() * 4));
+        meta.total = kp; meta.world = world; meta.rank = r.rank; meta.bins = bins; meta.parity = parity;
+        const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((kept[r.rank] + 255) / 256, (uint64_t)frz_sm_count() * 4));
         if (direct_out) {
-            k_place<true><<<grid, 256, 0, main>>>(r.run, counts[r.rank], meta, reinterpret_cast<const unsigned long long*>(r.d_pos0),
+            k_place<true><<<grid, 256, 0, main>>>(r.run, kept[r.rank], meta, reinterpret_cast<const unsigned long long*>(r.d_pos0),
                                                   reinterpret_cast<const uint32_t*>(r.d_pos0 + bins), seq, 0ull, nullptr, direct_out);
             FRZ_CUDA_TRY(cudaGetLastError());
             direct_done = true;   // my part of the list is already on its way to the host buffer: no slice copy
         } else {
-            k_place<false><<<grid, 256, 0, main>>>(r.run, counts[r.rank], meta, reinterpret_cast<const unsigned long long*>(r.d_pos0),
+            k_place<false><<<grid, 256, 0, main>>>(r.run, kept[r.rank], meta, reinterpret_cast<const unsigned long long*>(r.d_pos0),
                                                    reinterpret_cast<const uint32_t*>(r.d_pos0 + bins), seq,
                                                    (unsigned long long)(poll_timeout_s() * 1e9),
                                                    reinterpret_cast<volatile unsigned long long*>(r.ctrl_dev + kCtrlPlaceErr + r.rank), nullptr);
@@ -1023,7 +1040,7 @@ frz_status rank_step(frz_comm* c, RankCtx& r, frz_matcher* m, const frz_corpus* 
             // empty): the all-gather reads `stride` elements from every rank, so move the run into a buffer that long
             FrzMatchDev* bigger = nullptr;
             FRZ_CUDA_TRY(cudaMalloc(&bigger, stride * sizeof(FrzMatchDev)));
-            FRZ_CUDA_TRY(cudaMemcpyAsync(bigger, r.run, counts[r.rank] * sizeof(FrzMatchDev), cudaMemcpyDeviceToDevice, main));
+            FRZ_CUDA_TRY(cudaMemcpyAsync(bigger, r.run, kept[r.rank] * sizeof(FrzMatchDev), cudaMemcpyDeviceToDevice, main));
             FRZ_CUDA_TRY(cudaStreamSynchronize(main));
             cudaFree(r.run);
             r.run = bigger;
@@ -1036,9 +1053,9 @@ frz_status rank_step(frz_comm* c, RankCtx& r, frz_matcher* m, const frz_corpus* 
             FRZ_CUDA_TRY(cudaMalloc(&r.gathered, want * sizeof(FrzMatchDev)));
             r.gathered_cap = want;
         }
-        if (r.merged_cap < total) {
+        if (r.merged_cap < kept_total) {
             cudaFree(r.merged); r.merged = nullptr; r.merged_cap = 0;
-            const uint64_t want = total + total / 4 + 1024;
+            const uint64_t want = kept_total + kept_total / 4 + 1024;
             FRZ_CUDA_TRY(cudaMalloc(&r.merged, want * sizeof(FrzMatchDev)));
             r.merged_cap = want;
         }
@@ -1048,20 +1065,20 @@ frz_status rank_step(frz_comm* c, RankCtx& r, frz_matcher* m, const frz_corpus* 
         } else {   // world 1 without a communicator (local form + force flag): the gather of one run is a copy
             FRZ_CUDA_TRY(cudaMemcpyAsync(r.gathered, r.run, stride * sizeof(FrzMatchDev), cudaMemcpyDeviceToDevice, main));
         }
-        // ---- k_merge_matches_by on this GPU
-        FRZ_TRY(frz_merge_runs_ex(r.merge, r.gathered, stride, counts, world, frz_matcher_sort(m), frz_matcher_score_bound(m), r.merged, main));
+        // ---- k_merge_matches_by on this GPU (of the runs' kept prefixes: the merged list's first K' are the same)
+        FRZ_TRY(frz_merge_runs_ex(r.merge, r.gathered, stride, kept, world, frz_matcher_sort(m), frz_matcher_score_bound(m), r.merged, main));
         d_final = r.merged;
     }
     res->d_merged = slice_form ? nullptr : d_final;
     FRZ_CUDA_TRY(cudaEventRecord(r.ev[2], main));
     if (want_host) {
-        if (total > cap) {   // every rank sees the same counts, so every rank takes this exit: no collective is left unbalanced
+        if (kp > cap) {   // every rank sees the same counts, so every rank takes this exit: no collective is left unbalanced
             FRZ_CUDA_TRY(cudaStreamSynchronize(main));
-            return frz_fail(FRZ_ERR_CAPACITY, "output capacity %llu < %llu matches", (unsigned long long)cap, (unsigned long long)total);
+            return frz_fail(FRZ_ERR_CAPACITY, "output capacity %llu < %llu matches", (unsigned long long)cap, (unsigned long long)kp);
         }
-        if (total && !out_host) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
+        if (kp && !out_host) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
         // this rank's slice of the merged list → host (all ranks hold the whole list: the copy uses every PCIe link)
-        const uint64_t lo = total * (uint64_t)r.rank / (uint64_t)world, hi = total * (uint64_t)(r.rank + 1) / (uint64_t)world;
+        const uint64_t lo = kp * (uint64_t)r.rank / (uint64_t)world, hi = kp * (uint64_t)(r.rank + 1) / (uint64_t)world;
         if (hi > lo && !direct_done)
             FRZ_CUDA_TRY(cudaMemcpyAsync(out_host + lo, d_final + (lo - d_final_first), (hi - lo) * sizeof(FrzMatchDev), cudaMemcpyDeviceToHost, main));
     }
@@ -1082,8 +1099,8 @@ frz_status rank_step(frz_comm* c, RankCtx& r, frz_matcher* m, const frz_corpus* 
 }
 
 void run_job(frz_comm* c, RankCtx& r, frz_matcher* m, const frz_corpus* shard, uint32_t offset, uint64_t seq, frz_match* out,
-             uint64_t cap, bool want_host, StepResult* res) {
-    res->status = rank_step(c, r, m, shard, nullptr, offset, seq, out, cap, want_host, true, res);
+             uint64_t cap, bool want_host, uint64_t limit, StepResult* res) {
+    res->status = rank_step(c, r, m, shard, nullptr, offset, seq, out, cap, want_host, true, limit, res);
     if (res->status != FRZ_OK) res->error = frz_last_error();
 }
 
@@ -1232,8 +1249,10 @@ extern "C" frz_status frz_corpus_create_sharded(const uint8_t* bytes, const void
     return FRZ_OK;
 }
 
-extern "C" frz_status frz_match_list_parallel(frz_matcher* m, const frz_corpus* const* shards, int n_shards, frz_comm* c, frz_match* out,
-                                              uint64_t cap, uint64_t* n_out) {
+namespace {
+// the local form of frz_match_list_parallel{,_top}: *n_out = the length of the returned list, *n_total = all matches
+frz_status match_list_parallel_local(frz_matcher* m, const frz_corpus* const* shards, int n_shards, frz_comm* c, frz_match* out, uint64_t cap,
+                                     uint64_t limit, uint64_t* n_out, uint64_t* n_total) {
     if (!m || !c || !shards) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
     if (!c->local_form) return frz_fail(FRZ_ERR_INVALID_ARG, "multi-process communicator: call frz_match_list_parallel_rank on every rank");
     if (n_shards != c->world) return frz_fail(FRZ_ERR_INVALID_ARG, "%d shards for a communicator of %d GPUs", n_shards, c->world);
@@ -1248,17 +1267,19 @@ extern "C" frz_status frz_match_list_parallel(frz_matcher* m, const frz_corpus* 
     if (total_items > 0xFFFFFFFFull)
         return frz_fail(FRZ_ERR_TOO_MANY_ITEMS, "too many items in haystack, will overflow the u32 index: %llu > %u (index offset: 0)",
                         (unsigned long long)total_items, 0xFFFFFFFFu);
+    // a top-K call never writes more than min(k, haystacks) rows: that is the buffer the direct placement has to map
+    if (limit != UINT64_MAX) cap = std::min(cap, total_items);
     const uint64_t seq = ++c->seq;
     std::vector<StepResult> res(c->world);
     if (c->world == 1) {
-        run_job(c, c->ranks[0], m, shards[0], 0, seq, out, cap, true, &res[0]);
+        run_job(c, c->ranks[0], m, shards[0], 0, seq, out, cap, true, limit, &res[0]);
     } else {
         for (int g = 0; g < c->world; g++) {
             Worker* w = c->workers[g].get();
             {
                 std::lock_guard<std::mutex> lk(w->mu);
-                w->job = [c, g, m, shards, &offs, seq, out, cap, &res] {
-                    run_job(c, c->ranks[g], m, shards[g], (uint32_t)offs[g], seq, out, cap, true, &res[g]);
+                w->job = [c, g, m, shards, &offs, seq, out, cap, limit, &res] {
+                    run_job(c, c->ranks[g], m, shards[g], (uint32_t)offs[g], seq, out, cap, true, limit, &res[g]);
                 };
                 w->done = false;
                 w->has_job = true;
@@ -1271,10 +1292,24 @@ extern "C" frz_status frz_match_list_parallel(frz_matcher* m, const frz_corpus* 
             w->cv.wait(lk, [&] { return w->done; });
         }
     }
-    if (n_out) *n_out = res[0].total;
+    if (n_out) *n_out = limit == UINT64_MAX ? res[0].total : res[0].kept;
+    if (n_total) *n_total = res[0].total;
     for (int g = 0; g < c->world; g++)
         if (res[g].status != FRZ_OK) return frz_fail(res[g].status, "GPU %d: %s", c->ranks[g].device, res[g].error.c_str());
     return FRZ_OK;
+}
+}  // namespace
+
+extern "C" frz_status frz_match_list_parallel(frz_matcher* m, const frz_corpus* const* shards, int n_shards, frz_comm* c, frz_match* out,
+                                              uint64_t cap, uint64_t* n_out) {
+    return match_list_parallel_local(m, shards, n_shards, c, out, cap, UINT64_MAX, n_out, nullptr);
+}
+
+// match_list_parallel followed by truncation to the first k rows; `out` has room for min(k, haystacks over all shards) matches
+extern "C" frz_status frz_match_list_parallel_top(frz_matcher* m, const frz_corpus* const* shards, int n_shards, frz_comm* c, uint64_t k,
+                                                  frz_match* out, uint64_t* n_out, uint64_t* n_total) {
+    if (!out && k > 0) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
+    return match_list_parallel_local(m, shards, n_shards, c, out, k, k, n_out, n_total);
 }
 
 extern "C" frz_status frz_match_list_parallel_rank(frz_matcher* m, const frz_corpus* shard, uint32_t index_offset, frz_comm* c, frz_match* out,
@@ -1288,8 +1323,26 @@ extern "C" frz_status frz_match_list_parallel_rank(frz_matcher* m, const frz_cor
     const uint64_t seq = ++c->seq;
     StepResult res;
     const bool want_host = out != nullptr || cap != 0;
-    const frz_status s = rank_step(c, c->ranks[0], m, shard, nullptr, index_offset, seq, out, cap, want_host, d_out == nullptr, &res);
+    const frz_status s = rank_step(c, c->ranks[0], m, shard, nullptr, index_offset, seq, out, cap, want_host, d_out == nullptr, UINT64_MAX, &res);
     if (n_out) *n_out = res.total;
+    if (d_out) *d_out = reinterpret_cast<const frz_match*>(res.d_merged);
+    return s;
+}
+
+// one rank of match_list_parallel followed by truncation to the first k rows; `out`: the shared segment (room for k), or NULL
+extern "C" frz_status frz_match_list_parallel_rank_top(frz_matcher* m, const frz_corpus* shard, uint32_t index_offset, frz_comm* c, uint64_t k,
+                                                       frz_match* out, uint64_t* n_out, uint64_t* n_total, const frz_match** d_out) {
+    if (!m || !c || !shard) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    if (c->local_form && c->world != 1) return frz_fail(FRZ_ERR_INVALID_ARG, "local communicator: call frz_match_list_parallel_top");
+    if ((uint64_t)index_offset + frz_corpus_len(shard) > 0xFFFFFFFFull)
+        return frz_fail(FRZ_ERR_TOO_MANY_ITEMS, "too many items in haystack, will overflow the u32 index: %llu > %u (index offset: %u)",
+                        (unsigned long long)index_offset + frz_corpus_len(shard), 0xFFFFFFFFu, index_offset);
+    std::lock_guard<std::mutex> lock(c->mu);
+    const uint64_t seq = ++c->seq;
+    StepResult res;
+    const frz_status s = rank_step(c, c->ranks[0], m, shard, nullptr, index_offset, seq, out, out ? k : 0, out != nullptr, d_out == nullptr, k, &res);
+    if (n_out) *n_out = res.kept;
+    if (n_total) *n_total = res.total;
     if (d_out) *d_out = reinterpret_cast<const frz_match*>(res.d_merged);
     return s;
 }
@@ -1316,7 +1369,7 @@ extern "C" frz_status frz_match_list_parallel_rank_host(frz_matcher* m, const ui
     const HostShard hs{bytes, offsets, offset_width, n};
     const uint64_t seq = ++c->seq;
     StepResult res;
-    const frz_status s = rank_step(c, r, m, nullptr, &hs, index_offset, seq, out, cap, true, true, &res);
+    const frz_status s = rank_step(c, r, m, nullptr, &hs, index_offset, seq, out, cap, true, true, UINT64_MAX, &res);
     if (n_out) *n_out = res.total;
     return s;
 }

@@ -17,6 +17,10 @@
 //
 // The element count lives in device memory (it is produced by the previous stage), so the whole
 // match_list pipeline runs without a host round trip until the final copy-out.
+//
+// Top-K calls (frz_match_list_top): the final scatter of every sort takes a limit and stores only the positions below it —
+// every element's final position is known before its store, so the first `limit` elements of the sorted list are exactly
+// the ones written.  Full sorts pass kFrzNoLimit.
 #include "frz_device.cuh"
 #include "frz_host.h"
 
@@ -164,7 +168,7 @@ __global__ void __launch_bounds__(256) k_sort_scan_rows(uint32_t* __restrict__ h
 __global__ void __launch_bounds__(kSortWarps * 32) k_sort_scatter(const FrzMatchDev* __restrict__ in, FrzMatchDev* __restrict__ out,
                                                                   const unsigned long long* __restrict__ n_ptr, int shift, int bins,
                                                                   const uint32_t* __restrict__ hist,
-                                                                  const uint32_t* __restrict__ digit_base) {
+                                                                  const uint32_t* __restrict__ digit_base, uint32_t limit) {
     extern __shared__ uint32_t sm[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     uint32_t* cnt = sm + warp * bins;
@@ -193,7 +197,7 @@ __global__ void __launch_bounds__(kSortWarps * 32) k_sort_scatter(const FrzMatch
         __syncwarp();
         if (valid && rank == 0) cnt[d] += __popc(peers);
         __syncwarp();
-        if (valid) out[pos] = m;
+        if (valid && pos < limit) out[pos] = m;
     }
 }
 
@@ -211,7 +215,7 @@ static_assert(kSegRounds * kSegThreads == (1 << kFrzSortSegShift), "a segment is
 __global__ void __launch_bounds__(kSegThreads) k_sort_scatter_seg(const FrzMatchDev* __restrict__ in, FrzMatchDev* __restrict__ out,
                                                                   const unsigned long long* __restrict__ n_ptr, int bins,
                                                                   const uint32_t* __restrict__ pref, uint32_t stride,
-                                                                  const uint32_t* __restrict__ digit_base) {
+                                                                  const uint32_t* __restrict__ digit_base, uint32_t limit) {
     extern __shared__ uint32_t sm[];   // [kSegWarps][bins]: per-warp digit counters, then each warp's output base per digit
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     uint32_t* cnt = sm + warp * bins;
@@ -257,7 +261,10 @@ __global__ void __launch_bounds__(kSegThreads) k_sort_scatter_seg(const FrzMatch
         __syncthreads();
 #pragma unroll
         for (int r = 0; r < kSegRounds; r++)
-            if (first + r * 32 < n) out[cnt[(uint32_t)m[r].score & mask] + rank[r]] = m[r];
+            if (first + r * 32 < n) {
+                const uint32_t pos = cnt[(uint32_t)m[r].score & mask] + rank[r];
+                if (pos < limit) out[pos] = m[r];
+            }
         __syncthreads();   // the counters are reset for the next segment
     }
 }
@@ -267,8 +274,8 @@ __global__ void __launch_bounds__(kSegThreads) k_sort_scatter_seg(const FrzMatch
 // n_ptr: device pointer to the element count.  score_bound: host-known upper bound of any score.
 frz_status frz_launch_sort_by_score_dev(const FrzMatchDev* d_in, FrzMatchDev* d_tmp, FrzMatchDev* d_out,
                                         const unsigned long long* n_ptr, uint32_t score_bound, FrzWorkspace& ws,
-                                        cudaStream_t stream, FrzLaunchStats* st) {
-    auto pass = [&](const FrzMatchDev* src, FrzMatchDev* dst, int shift, int bins) -> frz_status {
+                                        cudaStream_t stream, FrzLaunchStats* st, uint32_t limit) {
+    auto pass = [&](const FrzMatchDev* src, FrzMatchDev* dst, int shift, int bins, uint32_t keep) -> frz_status {
         const size_t smem = (size_t)kSortWarps * bins * sizeof(uint32_t);
         k_sort_hist<<<kSortBlocks, kSortWarps * 32, smem, stream>>>(src, n_ptr, shift, bins, ws.sort_hist);
         uint32_t* totals = ws.sort_hist + (size_t)kMaxBins * kV;
@@ -280,17 +287,17 @@ frz_status frz_launch_sort_by_score_dev(const FrzMatchDev* d_in, FrzMatchDev* d_
             FRZ_CUDA_TRY(cudaEventRecord(ws.table_ev, stream));
             ws.table_ev_recorded = true;
         }
-        k_sort_scatter<<<kSortBlocks, kSortWarps * 32, smem, stream>>>(src, dst, n_ptr, shift, bins, ws.sort_hist, digit_base);
+        k_sort_scatter<<<kSortBlocks, kSortWarps * 32, smem, stream>>>(src, dst, n_ptr, shift, bins, ws.sort_hist, digit_base, keep);
         FRZ_CUDA_TRY(cudaGetLastError());
         if (st) st->launches += 3;
         return FRZ_OK;
     };
-    if (score_bound < 256) return pass(d_in, d_out, 0, 256);
-    if (score_bound < 512) return pass(d_in, d_out, 0, 512);
-    if (score_bound < 1024) return pass(d_in, d_out, 0, 1024);
-    // the reference's two 8-bit LSD passes (src/sort.rs:8-39)
-    FRZ_TRY(pass(d_in, d_tmp, 0, 256));
-    return pass(d_tmp, d_out, 8, 256);
+    if (score_bound < 256) return pass(d_in, d_out, 0, 256, limit);
+    if (score_bound < 512) return pass(d_in, d_out, 0, 512, limit);
+    if (score_bound < 1024) return pass(d_in, d_out, 0, 1024, limit);
+    // the reference's two 8-bit LSD passes (src/sort.rs:8-39); only the second one knows final positions
+    FRZ_TRY(pass(d_in, d_tmp, 0, 256, kFrzNoLimit));
+    return pass(d_tmp, d_out, 8, 256, limit);
 }
 
 size_t frz_sort_hist_words() { return (size_t)kMaxBins * kV + 2 * kMaxBins + 4; }   // + the pass-completion counter (must start at zero)
@@ -333,7 +340,7 @@ frz_status frz_sort_fused_prepare(FrzWorkspace& ws, uint64_t n_cap, uint32_t sco
 }
 
 frz_status frz_launch_sort_fused(const FrzMatchDev* d_in, FrzMatchDev* d_out, const unsigned long long* n_ptr, const FrzScoreHist& h,
-                                 FrzWorkspace& ws, cudaStream_t stream, FrzLaunchStats* st) {
+                                 FrzWorkspace& ws, cudaStream_t stream, FrzLaunchStats* st, uint32_t limit) {
     const int bins = (int)h.mask + 1;
     uint32_t* pref = h.counts + (size_t)bins * h.stride;
     uint32_t* totals = ws.sort_hist + (size_t)kMaxBins * kV;
@@ -348,7 +355,7 @@ frz_status frz_launch_sort_fused(const FrzMatchDev* d_in, FrzMatchDev* d_out, co
     }
     const size_t smem = (size_t)kSegWarps * bins * sizeof(uint32_t);
     const int grid = (int)std::max<uint32_t>(1, std::min<uint32_t>(h.stride, (uint32_t)frz_sm_count() * 4));
-    k_sort_scatter_seg<<<grid, kSegThreads, smem, stream>>>(d_in, d_out, n_ptr, bins, pref, h.stride, digit_base);
+    k_sort_scatter_seg<<<grid, kSegThreads, smem, stream>>>(d_in, d_out, n_ptr, bins, pref, h.stride, digit_base, limit);
     FRZ_CUDA_TRY(cudaGetLastError());
     if (st) st->launches += 2;
     return FRZ_OK;

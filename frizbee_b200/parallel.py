@@ -9,6 +9,7 @@ every GPU, every GPU copying its slice of the merged list to the host buffer.  T
   Comm.from_torch_distributed(device)      one rank per process (torchrun); torch.distributed only ships the 128-byte id
   comm.match_list_parallel(matcher, shards)            frz_match_list_parallel
   comm.match_list_parallel_rank(matcher, shard, off)   frz_match_list_parallel_rank
+  comm.match_list_parallel_top / _rank_top             the same, truncated to the first k rows (frz_match_list_parallel*_top)
 
 The numpy helpers at the bottom (shard_bounds, merge_runs_host, all_gather_runs, match_list_parallel_host) are the
 host-side SPECIFICATION of the shard/merge logic; the world-size-2 gloo tests (tests/test_parallel_gloo.py) run them on
@@ -47,6 +48,8 @@ def _bind(L):
     L.frz_corpus_create_sharded.argtypes = [vp, vp, C.c_int, u64, vp, C.POINTER(vp)]
     L.frz_match_list_parallel.argtypes = [vp, C.POINTER(vp), C.c_int, vp, vp, u64, C.POINTER(u64)]
     L.frz_match_list_parallel_rank.argtypes = [vp, vp, u32, vp, vp, u64, C.POINTER(u64), C.POINTER(vp)]
+    L.frz_match_list_parallel_top.argtypes = [vp, C.POINTER(vp), C.c_int, vp, u64, vp, C.POINTER(u64), C.POINTER(u64)]
+    L.frz_match_list_parallel_rank_top.argtypes = [vp, vp, u32, vp, u64, vp, C.POINTER(u64), C.POINTER(u64), C.POINTER(vp)]
     L.frz_match_list_parallel_rank_host.argtypes = [vp, vp, vp, C.c_int, u64, u32, vp, vp, u64, C.POINTER(u64)]
     L.frz_comm_last_timings.argtypes = [vp, C.c_int, C.POINTER(C.c_float), C.POINTER(vp)]
     L.frz_matcher_clone.argtypes = [vp, C.POINTER(vp)]
@@ -162,6 +165,34 @@ class Comm:
                                                    C.byref(d) if want_device else None))
         return n.value, d.value or 0
 
+    def match_list_parallel_top(self, matcher: Matcher, shards: Sequence[Corpus], k: int,
+                                out: Optional[np.ndarray] = None) -> Tuple[np.ndarray, int]:
+        """frz_match_list_parallel_top: the first min(k, total) rows of match_list_parallel.  Returns (rows, total).  `out`
+        (optional) needs room for min(k, haystacks over all shards) matches: no more rows can match."""
+        need = min(int(k), sum(len(s) for s in shards))
+        if out is None:
+            out = np.empty(max(need, 1), dtype=MATCH_DTYPE)
+        elif len(out) < need:
+            raise ValueError(f"out holds {len(out)} matches; a top-{k} call on these shards needs {need}")
+        hs = (C.c_void_p * len(shards))(*[s._h for s in shards])
+        n, total = C.c_uint64(), C.c_uint64()
+        _check(plib().frz_match_list_parallel_top(matcher._h, hs, len(shards), self._h, int(k), out.ctypes.data, C.byref(n), C.byref(total)))
+        return out[: n.value], total.value
+
+    def match_list_parallel_rank_top(self, matcher: Matcher, shard: Corpus, index_offset: int, k: int,
+                                     out: Optional[np.ndarray] = None, want_device: Optional[bool] = None) -> Tuple[int, int, int]:
+        """frz_match_list_parallel_rank_top, collective: the first min(k, total) rows land in the shared `out` (room for k,
+        from host_alloc_matches) unless it is None.  Returns (min(k, total), total, device pointer of the merged list or 0)."""
+        if want_device is None:
+            want_device = out is None
+        if out is not None and len(out) < k:   # (a rank does not know the other shards' lengths: the buffer holds k rows)
+            raise ValueError(f"out holds {len(out)} matches; a top-{k} call needs room for {k}")
+        n, total, d = C.c_uint64(), C.c_uint64(), C.c_void_p()
+        _check(plib().frz_match_list_parallel_rank_top(matcher._h, shard._h, index_offset, self._h, int(k),
+                                                       out.ctypes.data if out is not None else None, C.byref(n), C.byref(total),
+                                                       C.byref(d) if want_device else None))
+        return n.value, total.value, d.value or 0
+
     def match_list_parallel_rank_host(self, matcher: Matcher, data: np.ndarray, offsets: np.ndarray, index_offset: int,
                                       out: np.ndarray) -> int:
         """End to end on one rank: this rank's shard arrives as HOST Arrow buffers (streamed H2D + pack), then the parallel
@@ -222,19 +253,24 @@ def merge_runs_host(runs: List[np.ndarray], sort: SortStrategy) -> np.ndarray:
     return cat[order]
 
 
-def placement_host(runs: List[np.ndarray], sort: SortStrategy, bins: int = 1024) -> List[np.ndarray]:
+def placement_host(runs: List[np.ndarray], sort: SortStrategy, bins: int = 1024, limit: Optional[int] = None) -> List[np.ndarray]:
     """Host specification of the P2P placement (csrc/parallel.cu: k_place + the position arithmetic of rank_step): from every
     run's per-score table gt[q][s] (how many elements of run q score higher than s) each rank derives, for ITS run only,
     pos0[s] — the merged position of the first element of its score-s block = everything scoring higher in any run + the
     score-s blocks of the runs that precede it in merge order — and stores element i (score s) at merged position
     pos0[s] + (i - gt[s]), i.e. into slice p = the rank with lo[p] <= position < lo[p + 1], lo[p] = total * p // world.
-    Returns the world slices; their concatenation is the k-way merge (tests/test_parallel_gloo.py)."""
+    Returns the world slices; their concatenation is the k-way merge (tests/test_parallel_gloo.py).
+
+    `limit` (top-K calls): only the first K' = min(limit, total) merged positions are produced — lo[p] = K' * p // world, each
+    rank walks only the first min(limit, n_q) elements of its run (a run keeps its order in the merge, so nothing after them
+    can land before K') and drops positions >= K'.  The concatenation is then the k-way merge's first K' rows."""
     world = len(runs)
     counts = [len(r) for r in runs]
     total = sum(counts)
-    lo = [total * p // world for p in range(world + 1)]
+    keep = total if limit is None else min(int(limit), total)
+    lo = [keep * p // world for p in range(world + 1)]
     slices = [np.zeros(lo[p + 1] - lo[p], dtype=MATCH_DTYPE) for p in range(world)]
-    if total == 0:
+    if keep == 0:
         return slices
     by_score = sort.is_by_score()
     nb = bins if by_score else 1
@@ -255,9 +291,11 @@ def placement_host(runs: List[np.ndarray], sort: SortStrategy, bins: int = 1024)
                     break
                 acc += int(ge[q][s] - gt[q][s])
             pos0[s] = acc
+        r = r if limit is None else r[:limit]
         i = np.arange(len(r), dtype=np.int64)
         s_of = np.minimum(r["score"].astype(np.int64), nb - 1) if by_score else np.zeros(len(r), dtype=np.int64)
         x = pos0[s_of] + (i - gt[me][s_of])
+        r, x = r[x < keep], x[x < keep]
         p_of = np.searchsorted(np.asarray(lo[1:], dtype=np.int64), x, side="right")
         for p in range(world):
             sel = p_of == p

@@ -9,6 +9,7 @@
  *   trait Specialized::match_list            src/matcher/algo.rs:14-22
  *   Matcher::{new,from_patterns,from_query}  src/matcher/mod.rs:90-136
  *   Matcher::match_list                      src/matcher/mod.rs:212-222
+ *     (and, truncated to its first k rows, frz_match_list_top / frz_match_list_parallel*_top)
  *   Matcher::match_list_parallel             src/matcher/parallel.rs:18-89
  *   Pattern::{parse,parse_query}             src/pattern.rs:100-222
  *   radix_sort_matches                       src/sort.rs:6-40
@@ -208,6 +209,16 @@ FRZ_API size_t frz_matcher_num_patterns(const frz_matcher* m); /* compiled (non-
 FRZ_API frz_status frz_match_list(frz_matcher* m, const frz_corpus* corpus,
                           frz_match* out, uint64_t cap, uint64_t* n_out);
 
+/* Matcher::match_list (src/matcher/mod.rs:212-222) followed by truncation to its first k rows — the rows a UI shows.
+ * The reference has no such method.  Bit-identical to frz_match_list(m, corpus)[0 : min(k, total)] under
+ * m->config.sort, for every sort strategy.  `out` is HOST memory with room for `k` matches (room for
+ * min(k, frz_corpus_len(corpus)) suffices: no more rows can match); *n_out = min(k, total) and
+ * *n_total = total (the full match count; n_total may be NULL).  k = 0 counts and copies nothing.  Never returns
+ * FRZ_ERR_CAPACITY; a NULL `out` with k > 0 is FRZ_ERR_INVALID_ARG.  The score sort stores only the first k positions
+ * and only min(k, total) matches cross PCIe. */
+FRZ_API frz_status frz_match_list_top(frz_matcher* m, const frz_corpus* corpus, uint64_t k,
+                              frz_match* out, uint64_t* n_out, uint64_t* n_total);
+
 /* Specialized::match_list / Matcher::match_list_into (src/matcher/algo.rs:17-22,
  * src/matcher/mod.rs:373-392): matches appended in input (index-ascending) order,
  * indices offset by `index_offset`, no sort. */
@@ -286,6 +297,21 @@ FRZ_API frz_status frz_match_list_parallel_rank(frz_matcher* m, const frz_corpus
 FRZ_API frz_status frz_match_list_parallel_rank_host(frz_matcher* m, const uint8_t* bytes, const void* offsets, int offset_width,
                                              uint64_t n, uint32_t index_offset, frz_comm* c, frz_match* out, uint64_t cap,
                                              uint64_t* n_out);
+/* Matcher::match_list_parallel (src/matcher/parallel.rs:18-89) followed by truncation to its first k rows (the reference
+ * has no such method), local form: bit-identical to frz_match_list_parallel(...)[0 : min(k, total)].  Same arguments as
+ * frz_match_list_parallel, with `k` in place of `cap`: `out` is host memory with room for `k` matches (room for min(k, the
+ * haystacks of all shards) suffices: no more rows can match).  *n_out = min(k, total),
+ * *n_total = total (may be NULL); k = 0 is valid; never FRZ_ERR_CAPACITY; NULL `out` with k > 0 is FRZ_ERR_INVALID_ARG.
+ * Every GPU sorts only its run's first k and the exchange moves only what lands in the first min(k, total) positions. */
+FRZ_API frz_status frz_match_list_parallel_top(frz_matcher* m, const frz_corpus* const* shards, int n_shards, frz_comm* c,
+                                       uint64_t k, frz_match* out, uint64_t* n_out, uint64_t* n_total);
+/* The same for one rank of the multi-process form (collective, like frz_match_list_parallel_rank): `out` is the
+ * frz_comm_host_alloc buffer with room for k matches (on return the first min(k, total) rows are there), or NULL to skip
+ * the host copy.  *n_out = min(k, total), *n_total = total (may be NULL).  *d_out (optional) receives this rank's device
+ * copy of the merged list, whose first min(k, total) entries are the result, valid until the next call on `c`. */
+FRZ_API frz_status frz_match_list_parallel_rank_top(frz_matcher* m, const frz_corpus* shard, uint32_t index_offset, frz_comm* c,
+                                            uint64_t k, frz_match* out, uint64_t* n_out, uint64_t* n_total,
+                                            const frz_match** d_out);
 /* How host-out calls move the matches on this communicator: 3 = direct placement (every GPU stores its matches at their
  * merged positions straight into the caller's pinned + mapped host buffer — frz_comm_host_alloc memory — over its own
  * PCIe link; a buffer that is not mapped on every GPU uses form 2 for that call), 2 = P2P placement (into the peers' slice
