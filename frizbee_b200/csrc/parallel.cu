@@ -13,12 +13,12 @@
 //
 // Host-out calls (the caller wants the list in host memory, the bench's `value`) do better than gather-then-merge:
 // every rank's per-score table crosses the shared host block, after which every rank KNOWS the merged position of each
-// of its matches, and ONE kernel (k_place) stores them straight to where they belong — into the caller's pinned + mapped
-// HOST buffer itself (direct form: zero-copy stores over each GPU's own PCIe link, no peer traffic and no separate
-// device→host copy at all), or, when the buffer is not mapped, into the peer GPUs' slice buffers over NVLink (P2P stores
-// into cudaIpc-mapped / peer-enabled memory, then every GPU copies its slice out) — the k-way merge and the exchange are
-// the same pass, no NCCL kernel, no receive buffer, no second scatter.  The all-gather form remains for device-out calls
-// and as the fallback (FRZ_PARALLEL_EXCHANGE=direct|p2p|slices|allgather).
+// of its matches, and ONE kernel (k_place) stores them straight to where they belong — into the peer GPUs' slice buffers
+// over NVLink (P2P stores into cudaIpc-mapped / peer-enabled memory, then every GPU copies its slice out) — the k-way merge
+// and the exchange are the same pass, no NCCL kernel, no receive buffer, no second scatter.  When peer memory cannot be
+// mapped the slice exchange (grouped ncclSend/ncclRecv) takes its place; FRZ_PARALLEL_EXCHANGE=slices selects it on any
+// machine, so that it can be tested.  The all-gather form serves device-out calls and host-out calls without per-score
+// tables (a score bound that needs the two-pass sort).
 //
 // The only per-step collective is that all-gather.  The match counts (the `Vec` lengths the k-merge reads) are
 // published by each GPU into a small pinned host block shared by all ranks — a 1-thread kernel right after the tile
@@ -40,7 +40,6 @@
 #include <sched.h>
 #include <sys/mman.h>
 #include <sys/stat.h>
-#include <sys/syscall.h>
 #include <time.h>
 #include <unistd.h>
 
@@ -214,28 +213,13 @@ struct PlaceMeta {
     unsigned long long total;                   // positions kept: the merged list's length, or K' of a top-K call
     int world, rank, bins, parity;
 };
-// DIRECT form (template, opt-in with FRZ_PARALLEL_EXCHANGE=direct): the destination is the caller's HOST buffer itself (pinned +
-// mapped, zero-copy stores over this GPU's own PCIe link): element i goes to host_out[pos0[s] + (i - gt[s])].  No peer
-// memory, no flags, no separate device→host copy, and no rank waits for another rank's run before its own bytes move.
-// SM-issued posted writes to host memory are slower than the copy engine's slice copy, so it is not the default.
-template <bool DIRECT>
 __global__ void __launch_bounds__(256) k_place(const FrzMatchDev* __restrict__ run, unsigned long long n, const __grid_constant__ PlaceMeta meta,
                                                const unsigned long long* __restrict__ pos0, const uint32_t* __restrict__ gt,
-                                               unsigned long long seq, unsigned long long timeout_ns, volatile unsigned long long* err_slot,
-                                               FrzMatchDev* __restrict__ host_out) {
+                                               unsigned long long seq, unsigned long long timeout_ns, volatile unsigned long long* err_slot) {
     __shared__ unsigned long long lo_s[kMaxWorld + 1];
     __shared__ FrzMatchDev* dst_s[kMaxWorld];
     __shared__ int last_s;
     const int world = meta.world, bins = meta.bins;
-    if constexpr (DIRECT) {
-        for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (unsigned long long)gridDim.x * blockDim.x) {
-            const FrzMatchDev m = run[i];
-            const uint32_t s = bins > 1 ? min((uint32_t)m.score, (uint32_t)bins - 1) : 0u;
-            const unsigned long long x = pos0[s] + (i - gt[s]);
-            if (x < meta.total) host_out[x] = m;
-        }
-        return;   // kernel completion + the stream-ordered "landed" flag make the stores visible to the host
-    }
     for (int i = threadIdx.x; i <= meta.world; i += blockDim.x) lo_s[i] = meta.lo[i];
     for (int i = threadIdx.x; i < meta.world; i += blockDim.x) dst_s[i] = reinterpret_cast<FrzMatchDev*>(meta.peer[i] + kPlaceHeaderBytes);
     __syncthreads();
@@ -335,9 +319,6 @@ struct RankCtx {
     uint64_t place_cap = 0;                 // elements
     unsigned char* peer_raw[kMaxWorld] = {};
     bool peer_ipc[kMaxWorld] = {};          // opened with cudaIpcOpenMemHandle (multi-process form)
-    const void* direct_for = nullptr;       // host `out` pointer (and capacity) the direct form was last negotiated for
-    uint64_t direct_cap = 0;
-    FrzMatchDev* direct_dev = nullptr;      // its device-side address (nullptr: not mapped on some rank → peer / NCCL forms)
     uint32_t* table_dev = nullptr;          // device-side address of the shared table block
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
     bool ev_valid = false;
@@ -365,11 +346,8 @@ struct frz_comm {
     volatile uint64_t* ctrl_host = nullptr;
     HostBlock tables;             // [parity][rank][kTableBins] uint32: every rank's score table of the current step
     volatile uint32_t* tables_host = nullptr;
-    bool slice_exchange = true;   // FRZ_PARALLEL_EXCHANGE=allgather forces the all-gather form for host-out calls too
     bool p2p_exchange = true;     // host-out calls place matches straight into the peers' slice buffers (k_place); cleared by
-                                  // FRZ_PARALLEL_EXCHANGE=slices|allgather, or when peer access / cudaIpc is unavailable
-    bool direct_exchange = true;  // host-out calls store matches straight into the caller's mapped host buffer (k_place<DIRECT>);
-                                  // needs `out` to be pinned + mapped on every rank (frz_comm_host_alloc memory is)
+                                  // FRZ_PARALLEL_EXCHANGE=slices, or when peer access / cudaIpc is unavailable
     // local form: rendezvous of the worker threads (allgather_words)
     std::mutex tb_mu;
     std::condition_variable tb_cv;
@@ -478,31 +456,6 @@ frz_status allgather_words(frz_comm* c, RankCtx& r, const uint64_t* mine, int n_
     return FRZ_OK;
 }
 
-// Direct form: is the caller's `out` buffer addressable from every rank's GPU?  Negotiated once per buffer (collective: the
-// ranks make the same calls with the same shared buffer, so they reach this together); any rank that cannot map it turns
-// the form off for that buffer on all ranks.
-frz_status negotiate_direct(frz_comm* c, RankCtx& r, const frz_match* out_host, uint64_t cap, FrzMatchDev** dev) {
-    *dev = nullptr;
-    if (!c->direct_exchange || !out_host) return FRZ_OK;
-    if (r.direct_for == out_host && r.direct_cap == cap) { *dev = r.direct_dev; return FRZ_OK; }
-    void* dp = nullptr;
-    uint64_t ok = cudaHostGetDevicePointer(&dp, const_cast<frz_match*>(out_host), 0) == cudaSuccess && dp ? 1 : 0;
-    if (ok && cap) {   // the whole buffer, not just its first page
-        void* dp2 = nullptr;
-        ok = cudaHostGetDevicePointer(&dp2, const_cast<frz_match*>(out_host + (cap - 1)), 0) == cudaSuccess &&
-             dp2 == static_cast<void*>(static_cast<FrzMatchDev*>(dp) + (cap - 1)) ? 1 : 0;
-    }
-    if (!ok) cudaGetLastError();
-    uint64_t all[kMaxWorld];
-    FRZ_TRY(allgather_words(c, r, &ok, 1, all));
-    for (int q = 0; q < c->world; q++) ok = ok && all[q] == 1;
-    r.direct_for = out_host;
-    r.direct_cap = cap;
-    r.direct_dev = ok ? static_cast<FrzMatchDev*>(dp) : nullptr;
-    *dev = r.direct_dev;
-    return FRZ_OK;
-}
-
 // Slice buffers of the P2P placement: every rank owns `header + cap elements`, every other rank maps it (local form: peer
 // access between the devices of one process; multi-process form: cudaIpc handles exchanged over the communicator).
 // Grow-only and COLLECTIVE: `need` is derived from the step's total match count, which every rank knows, so all ranks
@@ -567,8 +520,9 @@ frz_status ensure_place_buffers(frz_comm* c, RankCtx& r, uint64_t need, bool* re
 
 // ---- NUMA placement of the shared host buffer ------------------------------------------------------------------
 // All G GPUs copy their slices into the buffer at the same moment: G copy engines' worth of inbound DMA writes.  With every page on
-// one memory node that node's DRAM write bandwidth and the socket interconnect are the limit.  The first-touch placement below
-// only lines up with the slices when the list fills the buffer.  See numa_policy().
+// one memory node that node's DRAM write bandwidth and the socket interconnect are the limit.  So rank r first-touches the r-th
+// part of the buffer from a CPU of its GPU's node (first_touch_near); that lines up with the slices exactly only when the list
+// fills the buffer, since slices are fractions of the USED part.
 int gpu_numa_node(int device) {
     char bus[32] = {0};
     if (cudaDeviceGetPCIBusId(bus, sizeof bus, device) != cudaSuccess) { cudaGetLastError(); return -1; }
@@ -600,72 +554,19 @@ bool node_cpus(int node, cpu_set_t* set) {   // parses /sys/devices/system/node/
     fclose(f);
     return n > 0;
 }
-// Page placement policy of the shared host buffers (FRZ_HOST_NUMA):
-//   touch (default)  rank r first-touches the r-th part of the buffer from a CPU of its GPU's node (exact only when the list
-//                    fills the buffer: slices are fractions of the USED part)
-//   interleave       pages alternate over the memory nodes (mbind MPOL_INTERLEAVE before the first touch): every GPU's slice
-//                    is half local, half remote, wherever the slice boundaries of a step fall
-//   none             wherever the kernel puts them
-// FRZ_PARALLEL_DEBUG=1 prints where the pages are.
-enum { kNumaInterleave = 0, kNumaTouch = 1, kNumaNone = 2 };
-int numa_policy() {
-    static int p = -1;
-    if (p < 0) {
-        const char* e = getenv("FRZ_HOST_NUMA");
-        p = !e ? kNumaTouch : strcmp(e, "interleave") == 0 ? kNumaInterleave : strcmp(e, "none") == 0 ? kNumaNone : kNumaTouch;
-    }
-    return p;
-}
-bool numa_debug() { static int d = -1; if (d < 0) { const char* e = getenv("FRZ_PARALLEL_DEBUG"); d = e && atoi(e) ? 1 : 0; } return d == 1; }
-// nodes that have memory: /sys/devices/system/node/has_memory ("0-1"); 0 when unknown
-unsigned long memory_node_mask() {
-    FILE* f = fopen("/sys/devices/system/node/has_memory", "r");
-    if (!f) f = fopen("/sys/devices/system/node/online", "r");
-    if (!f) return 0;
-    unsigned long mask = 0;
-    int a = 0, b = 0;
-    for (;;) {
-        if (fscanf(f, "%d", &a) != 1) break;
-        b = a;
-        int ch = fgetc(f);
-        if (ch == '-') { if (fscanf(f, "%d", &b) != 1) break; ch = fgetc(f); }
-        for (int n = a; n <= b && n < (int)(8 * sizeof mask); n++) mask |= 1ul << n;
-        if (ch != ',') break;
-    }
-    fclose(f);
-    return mask;
-}
-// mbind(MPOL_INTERLEAVE) over the memory nodes; raw syscall (no libnuma in the image).  false = unavailable (one node, no permission)
-bool interleave_pages(void* ptr, uint64_t bytes) {
-    const unsigned long mask = memory_node_mask();
-    if (__builtin_popcountl(mask) < 2) return false;
-    constexpr int kMpolInterleave = 3;
-    return syscall(SYS_mbind, ptr, (unsigned long)bytes, kMpolInterleave, &mask, (unsigned long)(8 * sizeof mask + 1), 0u) == 0;
-}
-// node of the page holding `addr` (move_pages with a null target = query), -1 when unknown
-int page_node(void* addr) {
-    void* page = reinterpret_cast<void*>(reinterpret_cast<uintptr_t>(addr) & ~4095ull);
-    int status = -1;
-    if (syscall(SYS_move_pages, 0, 1ul, &page, nullptr, &status, 0) != 0) return -1;
-    return status;
-}
 // touches [lo, hi) of `ptr` (one byte per page, value preserved as zero) from a CPU near `device`, then restores the affinity
-void first_touch_near(int device, unsigned char* ptr, uint64_t lo, uint64_t hi, bool pin_near) {
+void first_touch_near(int device, unsigned char* ptr, uint64_t lo, uint64_t hi) {
     cpu_set_t old_set, near_set;
     const bool have_old = sched_getaffinity(0, sizeof old_set, &old_set) == 0;
     const int node = gpu_numa_node(device);
     bool moved = false;
-    if (pin_near && have_old && node >= 0 && node_cpus(node, &near_set)) {
+    if (have_old && node >= 0 && node_cpus(node, &near_set)) {
         cpu_set_t both;
         CPU_AND(&both, &near_set, &old_set);   // stay inside whatever the launcher allowed
         if (CPU_COUNT(&both) > 0) moved = sched_setaffinity(0, sizeof both, &both) == 0;
     }
     for (uint64_t off = lo & ~4095ull; off < hi; off += 4096) ptr[off] = 0;
     if (moved) sched_setaffinity(0, sizeof old_set, &old_set);
-    if (numa_debug() && hi > lo)
-        fprintf(stderr, "[frz numa] device %d: sysfs node %d, affinity %s, policy %d; pages of [%llu, %llu): first on node %d, middle %d, last %d\n",
-                device, node, moved ? "moved" : "unchanged", numa_policy(), (unsigned long long)lo, (unsigned long long)hi,
-                page_node(ptr + lo), page_node(ptr + (lo + hi) / 2), page_node(ptr + hi - 1));
 }
 
 frz_status host_block_alloc(frz_comm* c, uint64_t bytes, HostBlock* out) {
@@ -678,10 +579,8 @@ frz_status host_block_alloc(frz_comm* c, uint64_t bytes, HostBlock* out) {
         b.ptr = mmap(nullptr, bytes, PROT_READ | PROT_WRITE, MAP_PRIVATE | MAP_ANONYMOUS, -1, 0);
         if (b.ptr == MAP_FAILED) return frz_fail(FRZ_ERR_OOM, "cannot map %llu bytes of host memory", (unsigned long long)bytes);
         const int world = c->world;
-        const bool inter = numa_policy() == kNumaInterleave && interleave_pages(b.ptr, bytes);
         for (int g = 0; g < world; g++)
-            first_touch_near(c->ranks[g].device, static_cast<unsigned char*>(b.ptr), bytes * (uint64_t)g / world, bytes * (uint64_t)(g + 1) / world,
-                             !inter && numa_policy() == kNumaTouch);
+            first_touch_near(c->ranks[g].device, static_cast<unsigned char*>(b.ptr), bytes * (uint64_t)g / world, bytes * (uint64_t)(g + 1) / world);
         FRZ_TRY(set_device(c->ranks[0].device));
         if (cudaHostRegister(b.ptr, bytes, cudaHostRegisterPortable | cudaHostRegisterMapped) != cudaSuccess) {
             cudaGetLastError();
@@ -712,13 +611,10 @@ frz_status host_block_alloc(frz_comm* c, uint64_t bytes, HostBlock* out) {
         b.ptr = mmap(nullptr, bytes, PROT_READ | PROT_WRITE, MAP_SHARED, b.fd, 0);
         if (b.ptr == MAP_FAILED) { b.ptr = nullptr; ok = 0; }
     }
-    // page placement (numa_policy above): the policy is set on every rank's mapping, every rank touches ITS part of the
-    // segment (shared-memory pages follow the policy of the mapping that faults them in), everybody waits, then everybody pins
-    if (ok) {
-        const bool inter = numa_policy() == kNumaInterleave && interleave_pages(b.ptr, bytes);
+    // page placement: every rank touches ITS part of the segment from a CPU near its GPU, everybody waits, then everybody pins
+    if (ok)
         first_touch_near(c->ranks[0].device, static_cast<unsigned char*>(b.ptr), bytes * (uint64_t)c->rank / c->world,
-                         bytes * (uint64_t)(c->rank + 1) / c->world, !inter && numa_policy() == kNumaTouch);
-    }
+                         bytes * (uint64_t)(c->rank + 1) / c->world);
     std::vector<uint64_t> oks(c->world);
     FRZ_TRY(exchange_words(c, &ok, 1, oks.data()));
     if (ok) {
@@ -740,17 +636,21 @@ frz_status host_block_alloc(frz_comm* c, uint64_t bytes, HostBlock* out) {
     return FRZ_OK;
 }
 
-frz_status comm_finish_setup(frz_comm* c) {
+// test hook: FRZ_PARALLEL_EXCHANGE=slices behaves as if peer memory could not be mapped (the NCCL slice exchange).  Read
+// before anything is set up, so that any other value fails communicator creation at once, on every rank.
+frz_status exchange_slices_requested(bool* slices) {
+    const char* e = getenv("FRZ_PARALLEL_EXCHANGE");
+    *slices = e && strcmp(e, "slices") == 0;
+    if (e && *e && !*slices)
+        return frz_fail(FRZ_ERR_INVALID_ARG, "FRZ_PARALLEL_EXCHANGE=%s: the only accepted value is 'slices' (unset: P2P placement)", e);
+    return FRZ_OK;
+}
+
+frz_status comm_finish_setup(frz_comm* c, bool slices) {
     { const char* e = getenv("FRZ_PARALLEL_FORCE_NCCL"); c->force_nccl = e && atoi(e) != 0; }
+    c->p2p_exchange = !slices && c->world > 1;
     FRZ_TRY(host_block_alloc(c, kCtrlBytes, &c->ctrl));
     c->ctrl_host = reinterpret_cast<volatile uint64_t*>(c->ctrl.ptr);
-    {   // host-out exchange: p2p (default) → slices (NCCL send/recv) → allgather
-        const char* e = getenv("FRZ_PARALLEL_EXCHANGE");
-        c->slice_exchange = !(e && strcmp(e, "allgather") == 0);
-        c->p2p_exchange = c->slice_exchange && !(e && strcmp(e, "slices") == 0) && c->world > 1;
-        // direct form: opt-in; the SMs' zero-copy stores to host memory are slower than the copy engine's slice copy
-        c->direct_exchange = c->slice_exchange && c->world > 1 && e && strcmp(e, "direct") == 0;
-    }
     if (c->p2p_exchange && c->local_form) {   // one process: plain peer access between every pair of devices
         for (RankCtx& a : c->ranks) {
             FRZ_TRY(set_device(a.device));
@@ -881,7 +781,6 @@ frz_status rank_step(frz_comm* c, RankCtx& r, frz_matcher* m, const frz_corpus* 
     const FrzMatchDev* d_final = r.run;
     uint64_t d_final_first = 0;   // merged position of d_final[0] (non-zero in the slice form)
     bool placed = false;          // the P2P placement ran this step
-    bool direct_done = false;     // the direct form ran: this rank's matches went straight into the host buffer
     // ---- host-out calls: SLICE EXCHANGE.  A rank copies only its slice [lo, hi) of the merged list to the host, and the
     // elements of run q that land in that slice are ONE contiguous range of run q (a run's elements keep their order in the
     // merged list).  With every rank's per-score table (published like the counts) each rank computes those ranges on the
@@ -893,7 +792,7 @@ frz_status rank_step(frz_comm* c, RankCtx& r, frz_matcher* m, const frz_corpus* 
     int bins = 1;
     const uint32_t* d_table = nullptr;
     if (by_score) d_table = frz_matcher_last_sort_table(r.clone, &bins);
-    const bool slice_form = want_host && want_slices && world > 1 && r.nccl && c->slice_exchange && (!by_score || bins > 0) && kp > 0 &&
+    const bool slice_form = want_host && want_slices && world > 1 && r.nccl && (!by_score || bins > 0) && kp > 0 &&
                             total <= 0xFFFFFFFFull;
     if (slice_form) {
         if (kp > cap) {
@@ -901,12 +800,9 @@ frz_status rank_step(frz_comm* c, RankCtx& r, frz_matcher* m, const frz_corpus* 
             return frz_fail(FRZ_ERR_CAPACITY, "output capacity %llu < %llu matches", (unsigned long long)cap, (unsigned long long)kp);
         }
         if (!out_host) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
-        // direct form: the caller's buffer mapped on every GPU?  Else the slice buffers of the P2P placement (collective,
-        // grow-only), else the NCCL slice exchange
-        FrzMatchDev* direct_out = nullptr;
-        FRZ_TRY(negotiate_direct(c, r, out_host, cap, &direct_out));
-        bool place_ready = direct_out != nullptr;
-        if (!direct_out) FRZ_TRY(ensure_place_buffers(c, r, kp / (uint64_t)world + 2, &place_ready));
+        // the slice buffers of the P2P placement (collective, grow-only), else the NCCL slice exchange
+        bool place_ready = false;
+        FRZ_TRY(ensure_place_buffers(c, r, kp / (uint64_t)world + 2, &place_ready));
         // 1. my table → shared block (after the local pipeline on the main stream), everybody's tables ← shared block
         volatile uint32_t* tab_host = c->tables_host + ((size_t)parity * world) * kTableBins;
         if (by_score) {
@@ -949,21 +845,13 @@ frz_status rank_step(frz_comm* c, RankCtx& r, frz_matcher* m, const frz_corpus* 
         for (int p2 = 0; p2 <= world; p2++) meta.lo[p2] = lo_p[p2];
         meta.total = kp; meta.world = world; meta.rank = r.rank; meta.bins = bins; meta.parity = parity;
         const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((kept[r.rank] + 255) / 256, (uint64_t)frz_sm_count() * 4));
-        if (direct_out) {
-            k_place<true><<<grid, 256, 0, main>>>(r.run, kept[r.rank], meta, reinterpret_cast<const unsigned long long*>(r.d_pos0),
-                                                  reinterpret_cast<const uint32_t*>(r.d_pos0 + bins), seq, 0ull, nullptr, direct_out);
-            FRZ_CUDA_TRY(cudaGetLastError());
-            direct_done = true;   // my part of the list is already on its way to the host buffer: no slice copy
-        } else {
-            k_place<false><<<grid, 256, 0, main>>>(r.run, kept[r.rank], meta, reinterpret_cast<const unsigned long long*>(r.d_pos0),
-                                                   reinterpret_cast<const uint32_t*>(r.d_pos0 + bins), seq,
-                                                   (unsigned long long)(poll_timeout_s() * 1e9),
-                                                   reinterpret_cast<volatile unsigned long long*>(r.ctrl_dev + kCtrlPlaceErr + r.rank), nullptr);
-            FRZ_CUDA_TRY(cudaGetLastError());
-            placed = true;
-            d_final = reinterpret_cast<const FrzMatchDev*>(r.place_raw + kPlaceHeaderBytes);
-            d_final_first = lo_p[r.rank];
-        }
+        k_place<<<grid, 256, 0, main>>>(r.run, kept[r.rank], meta, reinterpret_cast<const unsigned long long*>(r.d_pos0),
+                                         reinterpret_cast<const uint32_t*>(r.d_pos0 + bins), seq, (unsigned long long)(poll_timeout_s() * 1e9),
+                                         reinterpret_cast<volatile unsigned long long*>(r.ctrl_dev + kCtrlPlaceErr + r.rank));
+        FRZ_CUDA_TRY(cudaGetLastError());
+        placed = true;
+        d_final = reinterpret_cast<const FrzMatchDev*>(r.place_raw + kPlaceHeaderBytes);
+        d_final_first = lo_p[r.rank];
       } else {
         static thread_local std::vector<uint64_t> A;
         A.assign((size_t)world * (world + 1), 0);
@@ -1079,7 +967,7 @@ frz_status rank_step(frz_comm* c, RankCtx& r, frz_matcher* m, const frz_corpus* 
         if (kp && !out_host) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
         // this rank's slice of the merged list → host (all ranks hold the whole list: the copy uses every PCIe link)
         const uint64_t lo = kp * (uint64_t)r.rank / (uint64_t)world, hi = kp * (uint64_t)(r.rank + 1) / (uint64_t)world;
-        if (hi > lo && !direct_done)
+        if (hi > lo)
             FRZ_CUDA_TRY(cudaMemcpyAsync(out_host + lo, d_final + (lo - d_final_first), (hi - lo) * sizeof(FrzMatchDev), cudaMemcpyDeviceToHost, main));
     }
     FRZ_CUDA_TRY(cudaEventRecord(r.ev[3], main));
@@ -1136,6 +1024,8 @@ extern "C" frz_status frz_comm_create_local(int n_gpus, const int* devices, frz_
     if (!out) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
     if (n_gpus <= 0) return frz_fail(FRZ_ERR_THREADS_ZERO, "threads must be positive");   // parallel.rs:24
     if (n_gpus > kMaxWorld) return frz_fail(FRZ_ERR_INVALID_ARG, "at most %d GPUs per communicator", kMaxWorld);
+    bool slices = false;
+    FRZ_TRY(exchange_slices_requested(&slices));
     std::unique_ptr<frz_comm, void (*)(frz_comm*)> c(new frz_comm(), frz_comm_destroy);
     c->world = n_gpus;
     c->local_form = true;
@@ -1155,7 +1045,7 @@ extern "C" frz_status frz_comm_create_local(int n_gpus, const int* devices, frz_
         FRZ_NCCL_TRY(nccl_api().CommInitAll(comms.data(), n_gpus, devs.data()));
         for (int g = 0; g < n_gpus; g++) c->ranks[g].nccl = comms[g];
     }
-    FRZ_TRY(comm_finish_setup(c.get()));
+    FRZ_TRY(comm_finish_setup(c.get(), slices));
     if (n_gpus > 1) {
         for (int g = 0; g < n_gpus; g++) {
             c->workers.emplace_back(new Worker());
@@ -1171,6 +1061,8 @@ extern "C" frz_status frz_comm_create_rank(const uint8_t id[FRZ_UNIQUE_ID_BYTES]
     if (!out || !id) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
     if (world <= 0) return frz_fail(FRZ_ERR_THREADS_ZERO, "threads must be positive");
     if (world > kMaxWorld || rank < 0 || rank >= world) return frz_fail(FRZ_ERR_INVALID_ARG, "bad world/rank %d/%d", rank, world);
+    bool slices = false;
+    FRZ_TRY(exchange_slices_requested(&slices));
     FRZ_TRY(nccl_ready());
     std::unique_ptr<frz_comm, void (*)(frz_comm*)> c(new frz_comm(), frz_comm_destroy);
     c->world = world;
@@ -1183,7 +1075,7 @@ extern "C" frz_status frz_comm_create_rank(const uint8_t id[FRZ_UNIQUE_ID_BYTES]
     ncclUniqueId u;
     memcpy(&u, id, sizeof u);
     FRZ_NCCL_TRY(nccl_api().CommInitRank(&c->ranks[0].nccl, world, u, rank));
-    FRZ_TRY(comm_finish_setup(c.get()));
+    FRZ_TRY(comm_finish_setup(c.get(), slices));
     *out = c.release();
     return FRZ_OK;
 }
@@ -1193,7 +1085,7 @@ extern "C" int frz_comm_rank(const frz_comm* c) { return c ? c->rank : -1; }
 extern "C" int frz_comm_device(const frz_comm* c, int i) { return (c && i >= 0 && i < (int)c->ranks.size()) ? c->ranks[i].device : -1; }
 
 extern "C" int frz_comm_exchange_mode(const frz_comm* c) {
-    return !c ? -1 : (c->direct_exchange && c->world > 1) ? 3 : (c->p2p_exchange && c->world > 1) ? 2 : c->slice_exchange ? 1 : 0;
+    return !c ? -1 : (c->p2p_exchange && c->world > 1) ? 2 : 1;
 }
 
 extern "C" frz_status frz_comm_host_alloc(frz_comm* c, uint64_t bytes, void** out) {
@@ -1209,7 +1101,7 @@ extern "C" frz_status frz_comm_host_free(frz_comm* c, void* p) {
     if (!c || !p) return FRZ_OK;
     for (size_t i = 0; i < c->blocks.size(); i++)
         if (c->blocks[i].ptr == p) {
-            for (RankCtx& r : c->ranks) { cudaSetDevice(r.device); cudaDeviceSynchronize(); r.direct_for = nullptr; r.direct_dev = nullptr; }
+            for (RankCtx& r : c->ranks) { cudaSetDevice(r.device); cudaDeviceSynchronize(); }
             host_block_release(c->blocks[i]);
             c->blocks.erase(c->blocks.begin() + (long)i);
             return FRZ_OK;
@@ -1267,8 +1159,6 @@ frz_status match_list_parallel_local(frz_matcher* m, const frz_corpus* const* sh
     if (total_items > 0xFFFFFFFFull)
         return frz_fail(FRZ_ERR_TOO_MANY_ITEMS, "too many items in haystack, will overflow the u32 index: %llu > %u (index offset: 0)",
                         (unsigned long long)total_items, 0xFFFFFFFFu);
-    // a top-K call never writes more than min(k, haystacks) rows: that is the buffer the direct placement has to map
-    if (limit != UINT64_MAX) cap = std::min(cap, total_items);
     const uint64_t seq = ++c->seq;
     std::vector<StepResult> res(c->world);
     if (c->world == 1) {

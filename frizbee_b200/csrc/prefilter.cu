@@ -506,8 +506,8 @@ struct __align__(16) CandRec {
 // ---- TMA staging (cp.async.bulk, 1-D) of the phase-A arrays ---------------------------------------------------------
 // The metadata, signature and group-descriptor arrays are contiguous, so a warp's next 128-slot chunk is three bulk
 // copies (512 + 1024 + 64 bytes) that complete on the warp's OWN mbarrier: warp-autonomous, no block barrier, and the
-// bytes in flight hold no registers (the register-prefetch form, kept below as the A/B partner, pays 14 registers per
-// chunk in flight and ptxas sinks such loads towards their use).  Three stages per warp.
+// bytes in flight hold no registers (a register prefetch pays 14 registers per chunk in flight, and ptxas sinks such loads
+// towards their use).  Three stages per warp.
 constexpr int kScanStages = 3;
 struct __align__(16) ScanStage {
     uint32_t meta[128];
@@ -540,10 +540,9 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
         : "memory");
 }
 
-template <bool TMA>
-__global__ void __launch_bounds__(kScanThreads, TMA ? 6 : 10) k_sig_scan(const FrzCorpusView cv, int use_sig, uint32_t need1, uint32_t need2,
-                                                                         int sig_k, int min_len, CandRec* __restrict__ cand,
-                                                                         unsigned long long cand_cap, FrzCounters* __restrict__ ctr) {
+__global__ void __launch_bounds__(kScanThreads, 6) k_sig_scan(const FrzCorpusView cv, int use_sig, uint32_t need1, uint32_t need2,
+                                                              int sig_k, int min_len, CandRec* __restrict__ cand,
+                                                              unsigned long long cand_cap, FrzCounters* __restrict__ ctr) {
     extern __shared__ __align__(16) unsigned char scan_smem[];
     const uint32_t lane = frz_lane(), warp = threadIdx.x >> 5;
     CandRec* ring = reinterpret_cast<CandRec*>(scan_smem) + (size_t)warp * kScanRing;
@@ -595,102 +594,57 @@ __global__ void __launch_bounds__(kScanThreads, TMA ? 6 : 10) k_sig_scan(const F
         while (count >= 32) flush_request(32);
         __syncwarp();
     };
-    if constexpr (TMA) {
-        ScanStage* stages = reinterpret_cast<ScanStage*>(scan_smem + sizeof(CandRec) * kScanRing * kScanWarps) + warp * kScanStages;
-        uint64_t* bars = reinterpret_cast<uint64_t*>(scan_smem + (sizeof(CandRec) * kScanRing + sizeof(ScanStage) * kScanStages) * kScanWarps) +
-                         warp * kScanStages;
-        if (lane == 0)
-            for (int i = 0; i < kScanStages; i++) mbar_init(&bars[i], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        __syncwarp();
-        const uint32_t tx_bytes = (uint32_t)(sizeof(uint32_t) * 128 + sizeof(FrzGroupDesc) * 4) + (use_sig ? (uint32_t)sizeof(uint2) * 128 : 0u);
-        uint32_t req = blockIdx.x * kScanWarps + warp;   // next chunk to REQUEST
-        auto issue = [&](int st) {
-            if (req < total_chunks && lane == 0) {
-                const uint64_t slot0 = (uint64_t)req * 128;
-                mbar_expect_tx(&bars[st], tx_bytes);
-                bulk_g2s(stages[st].meta, cv.slot_meta + slot0, (uint32_t)sizeof(uint32_t) * 128, &bars[st]);
-                if (use_sig) bulk_g2s(stages[st].sig, cv.slot_sig + slot0, (uint32_t)sizeof(uint2) * 128, &bars[st]);
-                bulk_g2s(stages[st].desc, cv.groups + (size_t)req * 4, (uint32_t)sizeof(FrzGroupDesc) * 4, &bars[st]);
-            }
-            req += n_warps;
-        };
-        uint32_t cur = req;
+    ScanStage* stages = reinterpret_cast<ScanStage*>(scan_smem + sizeof(CandRec) * kScanRing * kScanWarps) + warp * kScanStages;
+    uint64_t* bars = reinterpret_cast<uint64_t*>(scan_smem + (sizeof(CandRec) * kScanRing + sizeof(ScanStage) * kScanStages) * kScanWarps) +
+                     warp * kScanStages;
+    if (lane == 0)
+        for (int i = 0; i < kScanStages; i++) mbar_init(&bars[i], 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    __syncwarp();
+    const uint32_t tx_bytes = (uint32_t)(sizeof(uint32_t) * 128 + sizeof(FrzGroupDesc) * 4) + (use_sig ? (uint32_t)sizeof(uint2) * 128 : 0u);
+    uint32_t req = blockIdx.x * kScanWarps + warp;   // next chunk to REQUEST
+    auto issue = [&](int st) {
+        if (req < total_chunks && lane == 0) {
+            const uint64_t slot0 = (uint64_t)req * 128;
+            mbar_expect_tx(&bars[st], tx_bytes);
+            bulk_g2s(stages[st].meta, cv.slot_meta + slot0, (uint32_t)sizeof(uint32_t) * 128, &bars[st]);
+            if (use_sig) bulk_g2s(stages[st].sig, cv.slot_sig + slot0, (uint32_t)sizeof(uint2) * 128, &bars[st]);
+            bulk_g2s(stages[st].desc, cv.groups + (size_t)req * 4, (uint32_t)sizeof(FrzGroupDesc) * 4, &bars[st]);
+        }
+        req += n_warps;
+    };
+    uint32_t cur = req;
 #pragma unroll
-        for (int i = 0; i < kScanStages; i++) issue(i);
-        int st = 0;
-        uint32_t parity = 0;
-        while (cur < total_chunks) {
-            mbar_wait(&bars[st], parity);
-            const uint4 meta = reinterpret_cast<const uint4*>(stages[st].meta)[lane];
-            uint4 sig0 = make_uint4(0u, 0u, 0u, 0u), sig1 = sig0;
-            if (use_sig) {
-                sig0 = reinterpret_cast<const uint4*>(stages[st].sig)[2 * lane];
-                sig1 = reinterpret_cast<const uint4*>(stages[st].sig)[2 * lane + 1];
-            }
-            const unsigned long long grp_off = stages[st].desc[lane >> 3].abs_off;
-            const uint32_t grp_units = stages[st].desc[lane >> 3].gunits;
-            __syncwarp();
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic reads of the stage before its async refill
-            issue(st);
-            process(cur, meta, sig0, sig1, grp_off, grp_units);
-            cur += n_warps;
-            if (++st == kScanStages) { st = 0; parity ^= 1; }
+    for (int i = 0; i < kScanStages; i++) issue(i);
+    int st = 0;
+    uint32_t parity = 0;
+    while (cur < total_chunks) {
+        mbar_wait(&bars[st], parity);
+        const uint4 meta = reinterpret_cast<const uint4*>(stages[st].meta)[lane];
+        uint4 sig0 = make_uint4(0u, 0u, 0u, 0u), sig1 = sig0;
+        if (use_sig) {
+            sig0 = reinterpret_cast<const uint4*>(stages[st].sig)[2 * lane];
+            sig1 = reinterpret_cast<const uint4*>(stages[st].sig)[2 * lane + 1];
         }
-    } else {
-        // register prefetch: two chunk buffers ping-pong, the other buffer's loads are in flight while one is tested
-        struct Chunk {
-            uint4 meta;
-            uint4 sig0, sig1;
-            unsigned long long abs_off;   // lanes 0-3: first unit of the chunk's group `lane`
-            uint32_t gunits;              // lanes 0-3: units per slot of that group
-            uint32_t idx;
-        };
-        uint32_t next = blockIdx.x * kScanWarps + warp;
-        auto load_chunk = [&](Chunk& c) {
-            c.idx = next < total_chunks ? next : 0xFFFFFFFFu;
-            c.meta = make_uint4(FRZ_INVALID_SLOT, FRZ_INVALID_SLOT, FRZ_INVALID_SLOT, FRZ_INVALID_SLOT);
-            c.sig0 = c.sig1 = make_uint4(0u, 0u, 0u, 0u);
-            c.abs_off = 0;
-            c.gunits = 0;
-            if (next < total_chunks) {
-                const uint64_t slot0 = (uint64_t)next * 128 + lane * 4;
-                c.meta = __ldg(reinterpret_cast<const uint4*>(cv.slot_meta + slot0));
-                if (use_sig) {
-                    const uint4* sp = reinterpret_cast<const uint4*>(cv.slot_sig + slot0);
-                    c.sig0 = __ldg(sp);
-                    c.sig1 = __ldg(sp + 1);
-                }
-                if (lane < 4) {   // four contiguous 16-byte descriptors, L2-resident
-                    const FrzGroupDesc gd = cv.groups[next * 4 + lane];
-                    c.abs_off = gd.abs_off;
-                    c.gunits = gd.gunits;
-                }
-            }
-            next += n_warps;
-        };
-        Chunk ca, cb;
-        load_chunk(ca);
-        load_chunk(cb);
-        for (;;) {
-            if (ca.idx == 0xFFFFFFFFu) break;
-            process(ca.idx, ca.meta, ca.sig0, ca.sig1, __shfl_sync(0xffffffffu, ca.abs_off, lane >> 3), __shfl_sync(0xffffffffu, ca.gunits, lane >> 3));
-            load_chunk(ca);
-            if (cb.idx == 0xFFFFFFFFu) break;
-            process(cb.idx, cb.meta, cb.sig0, cb.sig1, __shfl_sync(0xffffffffu, cb.abs_off, lane >> 3), __shfl_sync(0xffffffffu, cb.gunits, lane >> 3));
-            load_chunk(cb);
-        }
+        const unsigned long long grp_off = stages[st].desc[lane >> 3].abs_off;
+        const uint32_t grp_units = stages[st].desc[lane >> 3].gunits;
+        __syncwarp();
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic reads of the stage before its async refill
+        issue(st);
+        process(cur, meta, sig0, sig1, grp_off, grp_units);
+        cur += n_warps;
+        if (++st == kScanStages) { st = 0; parity ^= 1; }
     }
     flush_commit();
     if (count) { flush_request(count); flush_commit(); }
 }
 
 // ================================================================================================================
-// Stage 1 of the whole-corpus byte path  k_scan_window — the signature scan of k_sig_scan<true> and the exact reference
+// Stage 1 of the whole-corpus byte path  k_scan_window — the signature scan of k_sig_scan and the exact reference
 // window (process_candidate) in one persistent kernel.  The scan keeps HBM busy and leaves the ALUs idle, the window
 // machine the other way round; in one kernel an SM's warps do both at once, and the candidates never leave the SM.
 // Each warp:
-//   - walks its statically strided 128-slot chunks like k_sig_scan<true> (TMA stages, per-warp mbarriers) and appends the
+//   - walks its statically strided 128-slot chunks like k_sig_scan (TMA stages, per-warp mbarriers) and appends the
 //     records of the haystacks that pass the length gate and the signature test to its shared-memory ring;
 //   - after each chunk, takes every 32 records in the ring as a BATCH (lane per candidate): their haystack units travel
 //     global → shared with cp.async while the warp scans on, and the batch is windowed and emitted when the next one is
@@ -715,7 +669,7 @@ template <int MODE>
 __global__ void __launch_bounds__(kThreads, 4) k_scan_window(const FrzCorpusView cv, const __grid_constant__ FrzPatternDev pat,
                                                              int use_sig, int occ_rows, const FrzSurvLists lists,
                                                              unsigned long long surv_cap, uint32_t* __restrict__ surv_bitmap,
-                                                             FrzCounters* __restrict__ ctr, uint32_t flags) {
+                                                             FrzCounters* __restrict__ ctr) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const uint32_t lane = frz_lane(), warp = threadIdx.x >> 5;
     ScanWinSmem& sm = reinterpret_cast<ScanWinSmem*>(smem_raw)[warp];
@@ -727,7 +681,10 @@ __global__ void __launch_bounds__(kThreads, 4) k_scan_window(const FrzCorpusView
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     __syncthreads();
     const bool staged = cv.max_gunits <= 4;   // every haystack fits the four staged units
-    const bool single = (MODE == FRZ_T_0 || MODE == FRZ_T_1) && (flags & 1u) && single_chunk_ok(pat, cv.max_gunits);
+    // (single_chunk_ok implies occ_rows > 0.  Testing that kernel argument first keeps the FRZ_T_0 / FRZ_T_1 code that
+    // CUDA 12.9's ptxas schedules best: when the first test is on max_gunits, the prefilter stage of the max_typos=1
+    // benchmark measured about 4% slower on an H100 SXM at 400 W.)
+    const bool single = (MODE == FRZ_T_0 || MODE == FRZ_T_1) && occ_rows > 0 && single_chunk_ok(pat, cv.max_gunits);
     const uint32_t n_warps = gridDim.x * kWarps;
     const uint32_t total_chunks = cv.n_tiles * (FRZ_TILE / 128);   // 128 slots (4 groups) per chunk
     const uint32_t tx_bytes = (uint32_t)(sizeof(uint32_t) * 128 + sizeof(FrzGroupDesc) * 4) + (use_sig ? (uint32_t)sizeof(uint2) * 128 : 0u);
@@ -1044,28 +1001,19 @@ frz_status frz_launch_sig_scan(const FrzCorpusView& cv, const FrzPatternDev& pat
     const int sms = frz_sm_count();
     CandRec* cand = reinterpret_cast<CandRec*>(ws.cand_list);
     {   // persistent warps, as many blocks as fit
-        static int tma_knob = -1;   // A/B knob: FRZ_PF_TMA=0 selects the register-prefetch form of the phase-A loads
-        if (tma_knob < 0) { const char* e = getenv("FRZ_PF_TMA"); tma_knob = e ? atoi(e) : 1; }
         const uint32_t total_chunks = cv.n_tiles * (FRZ_TILE / 128);
         const int use_sig = pat.typo_mode != FRZ_T_NONE && pat.sig_on;
-        const size_t ring_bytes = sizeof(CandRec) * kScanRing * kScanWarps;
-        const size_t smem_tma = ring_bytes + (sizeof(ScanStage) * kScanStages + sizeof(uint64_t) * kScanStages) * kScanWarps;
-#define FRZ_SCAN_LAUNCH(TMA, SMEM)                                                                                       \
-        do {                                                                                                             \
-            static int bps_dev[64] = {};                                                                                 \
-            int& bps = bps_dev[frz_current_device() & 63];                                                               \
-            if (!bps) {                                                                                                  \
-                FRZ_CUDA_TRY(cudaFuncSetAttribute(k_sig_scan<TMA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(SMEM))); \
-                FRZ_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_sig_scan<TMA>, kScanThreads, (SMEM))); \
-                if (bps < 1) bps = 1;                                                                                    \
-            }                                                                                                            \
-            const uint32_t grid = std::max<uint32_t>(1, std::min<uint32_t>((uint32_t)(sms * bps), (total_chunks + kScanWarps - 1) / kScanWarps)); \
-            k_sig_scan<TMA><<<grid, kScanThreads, (SMEM), stream>>>(cv, use_sig, pat.sig_need1, pat.sig_need2, pat.sig_k,  \
-                                                                   pat.min_hay_len, cand, ws.cand_cap, ws.counters);     \
-        } while (0)
-        if (tma_knob) FRZ_SCAN_LAUNCH(true, smem_tma);
-        else FRZ_SCAN_LAUNCH(false, ring_bytes);
-#undef FRZ_SCAN_LAUNCH
+        const size_t smem = (sizeof(CandRec) * kScanRing + sizeof(ScanStage) * kScanStages + sizeof(uint64_t) * kScanStages) * kScanWarps;
+        static int bps_dev[64] = {};
+        int& bps = bps_dev[frz_current_device() & 63];
+        if (!bps) {
+            FRZ_CUDA_TRY(cudaFuncSetAttribute(k_sig_scan, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            FRZ_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_sig_scan, kScanThreads, smem));
+            if (bps < 1) bps = 1;
+        }
+        const uint32_t grid = std::max<uint32_t>(1, std::min<uint32_t>((uint32_t)(sms * bps), (total_chunks + kScanWarps - 1) / kScanWarps));
+        k_sig_scan<<<grid, kScanThreads, smem, stream>>>(cv, use_sig, pat.sig_need1, pat.sig_need2, pat.sig_k, pat.min_hay_len, cand,
+                                                         ws.cand_cap, ws.counters);
     }
     FRZ_CUDA_TRY(cudaGetLastError());
     if (st) st->launches++;
@@ -1079,9 +1027,6 @@ frz_status frz_launch_prefilter(const FrzCorpusView& cv, const FrzPatternDev& pa
     if (cv.n_tiles == 0) return FRZ_OK;
     const int sms = frz_sm_count();
     FRZ_CUDA_TRY(cudaMemsetAsync(ws.surv_bitmap, 0, (size_t)cv.n_tiles * 32 * sizeof(uint32_t), stream));
-    static int single_knob = -1;   // A/B knob: FRZ_PF_SINGLE=0 keeps the general (multi-chunk) mask forms
-    if (single_knob < 0) { const char* e = getenv("FRZ_PF_SINGLE"); single_knob = e ? atoi(e) : 1; }
-    const uint32_t pf_flags = single_knob ? 1u : 0u;
     const int use_sig = pat.typo_mode != FRZ_T_NONE && pat.sig_on;
     const int occ_rows = pat.n_distinct ? std::min(kMaxDistinct, pat.n_distinct + pat.n) : 0;
     const size_t smem = (sizeof(ScanWinSmem) + sizeof(uint2) * 32 * occ_rows) * kWarps;
@@ -1098,7 +1043,7 @@ frz_status frz_launch_prefilter(const FrzCorpusView& cv, const FrzPatternDev& pa
         }                                                                                                                \
         const uint32_t grid = std::max<uint32_t>(1, std::min<uint32_t>((uint32_t)(sms * bps), (total_chunks + kWarps - 1) / kWarps)); \
         k_scan_window<MODE><<<grid, kThreads, smem, stream>>>(cv, pat, use_sig, occ_rows, ws.lists(), ws.survivor_cap,   \
-                                                              ws.surv_bitmap, ws.counters, pf_flags);                    \
+                                                              ws.surv_bitmap, ws.counters);                              \
     } while (0)
     switch (pat.typo_mode) {
         case FRZ_T_0: FRZ_PF_LAUNCH(FRZ_T_0); break;

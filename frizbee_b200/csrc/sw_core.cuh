@@ -212,9 +212,9 @@ struct SwCore {
         }
         // ---- per-column bonus (ascii.rs:64-101) ----
         if ((VAR & 8) && !WRAP8) {
-            // VAR bit 3 (experiment, DESIGN.md §8): classify the haystack bytes four at a time on the PACKED words (the
-            // flag of a byte is bit 7 of its position) and expand only the three masks the bonus needs.  Same values as
-            // the per-lane form below, about 40% fewer instructions and a smaller body.
+            // VAR bit 3 (set by every k_sw64 launch without wrap8): classify the haystack bytes four at a time on the
+            // PACKED words (the flag of a byte is bit 7 of its position) and expand only the three masks the bonus needs.
+            // Same values as the per-lane form below, about 40% fewer instructions and a smaller body.
             const uint32_t capb = p.k_cap, delb = p.k_delim;
             const uint32_t base2 = __vadd2(p.k_base, p.k_neg_mis);
             uint32_t prev_lo = 0, prev_dl = 0;   // flags of the previous word (byte 3 feeds byte 0 of this one)

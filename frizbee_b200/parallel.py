@@ -119,7 +119,8 @@ class Comm:
         _check(plib().frz_comm_barrier(self._h))
 
     def exchange_mode(self) -> int:
-        """3 = direct placement into the mapped host buffer, 2 = P2P placement, 1 = NCCL slice exchange, 0 = all-gather."""
+        """How host-out calls exchange matches: 2 = P2P placement, 1 = NCCL slice exchange (FRZ_PARALLEL_EXCHANGE=slices,
+        one GPU, or peer memory that cannot be mapped)."""
         return int(plib().frz_comm_exchange_mode(self._h))
 
     def p2p_active(self) -> bool:

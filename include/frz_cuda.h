@@ -312,14 +312,13 @@ FRZ_API frz_status frz_match_list_parallel_top(frz_matcher* m, const frz_corpus*
 FRZ_API frz_status frz_match_list_parallel_rank_top(frz_matcher* m, const frz_corpus* shard, uint32_t index_offset, frz_comm* c,
                                             uint64_t k, frz_match* out, uint64_t* n_out, uint64_t* n_total,
                                             const frz_match** d_out);
-/* How host-out calls move the matches on this communicator: 3 = direct placement (every GPU stores its matches at their
- * merged positions straight into the caller's pinned + mapped host buffer — frz_comm_host_alloc memory — over its own
- * PCIe link; a buffer that is not mapped on every GPU uses form 2 for that call), 2 = P2P placement (into the peers' slice
- * buffers over NVLink — peer access in the local form, cudaIpc in the multi-process form — then every GPU copies its slice
- * out), 1 = NCCL slice exchange (grouped ncclSend/ncclRecv), 0 = ncclAllGather of whole runs + merge.  Chosen at creation
- * (FRZ_PARALLEL_EXCHANGE=direct|p2p|slices|allgather, default p2p — the copy engine moves a slice to host memory faster than
- * SM-issued stores do); 2 is downgraded to 1 by the first
- * call when peer memory cannot be mapped.  Device-out calls always use the all-gather. */
+/* How host-out calls move the matches on this communicator: 2 = P2P placement (every GPU stores its matches at their
+ * merged positions in the peers' slice buffers over NVLink — peer access in the local form, cudaIpc in the multi-process
+ * form — then every GPU copies its slice out), 1 = NCCL slice exchange (grouped ncclSend/ncclRecv); -1 for a NULL
+ * communicator.  2 on more than one GPU; the first call downgrades it to 1 when peer memory cannot be mapped, and
+ * FRZ_PARALLEL_EXCHANGE=slices (a test hook) starts at 1.  Any other non-empty value of that variable makes
+ * frz_comm_create_local / frz_comm_create_rank fail with FRZ_ERR_INVALID_ARG.  Device-out calls, and host-out calls whose
+ * score bound needs the two-pass sort, use ncclAllGather of whole runs + merge. */
 FRZ_API int frz_comm_exchange_mode(const frz_comm* c);
 
 /* Device timings (ms) of the last parallel call on local rank `local_index`: [0] local pipeline (prefilter, scoring,

@@ -2,8 +2,9 @@
 C ABI (frz_comm_create_rank + frz_match_list_parallel_rank: NCCL all-gather + device merge + per-rank slice copy into
 the shared host buffer) and checks on rank 0 that the result equals the single-GPU match_list (parallel == sequential,
 src/matcher/parallel.rs:104-130) — for every sort strategy, for shard sizes that do not divide evenly, for a
-match-everything query (another rank's run longer than the last rank's whole shard) and for lists shorter than the
-number of ranks (empty shards)."""
+match-everything query (another rank's run longer than the last rank's whole shard), for a score bound that needs the
+two-pass sort and for lists shorter than the number of ranks (empty shards).  With FRZ_PARALLEL_EXCHANGE set to a value
+other than `slices`, it checks instead that every rank's communicator creation refuses it."""
 import os
 import sys
 
@@ -53,10 +54,40 @@ def run_case(comm, rank, world, local, needle, cfg, data, off, label):
     return ok
 
 
+def refused_exchange(local):
+    """FRZ_PARALLEL_EXCHANGE set to anything but `slices` (or nothing): this rank's communicator creation must fail with
+    FRZ_ERR_INVALID_ARG.  Returns None when the variable is unset or `slices`, else whether the creation was refused."""
+    value = os.environ.get("FRZ_PARALLEL_EXCHANGE", "")
+    if value in ("", "slices"):
+        return None
+    try:
+        parallel.Comm.from_torch_distributed(local).close()
+        refused = False
+    except F.FrizbeeError as e:
+        refused = e.status_name == "FRZ_ERR_INVALID_ARG"
+    print(f"FRZ_PARALLEL_EXCHANGE={value}: communicator refused with FRZ_ERR_INVALID_ARG: {refused}", flush=True)
+    return refused
+
+
+def finish(local, ok, comm=None):
+    """Every rank learns whether all ranks passed; exits with 1 if one did not."""
+    flag = torch.tensor([0 if ok else 1], device=torch.device("cuda", local))
+    dist.all_reduce(flag)
+    if comm is not None:
+        comm.close()
+    dist.barrier()
+    dist.destroy_process_group()
+    if int(flag.item()) != 0:
+        sys.exit(1)
+
+
 def main():
     rank, world, local = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"]), int(os.environ["LOCAL_RANK"])
     torch.cuda.set_device(local)
     dist.init_process_group("nccl", device_id=torch.device("cuda", local))
+    refused = refused_exchange(local)
+    if refused is not None:
+        return finish(local, refused)
     comm = parallel.Comm.from_torch_distributed(local)
     assert comm.world == world and comm.rank == rank
     n = 400_003
@@ -70,6 +101,11 @@ def main():
     d2, o2 = synth.generate("deadbeef", n2, 24, 32, seed=9)
     for sort in (SortStrategy.ScoreThenIndexAsc, SortStrategy.IndexDesc):
         ok = run_case(comm, rank, world, local, "deadbeef", Config(max_typos=None, sort=sort), d2, o2, f"all-match sort={sort.name} n={n2}") and ok
+    # a score bound >= 1024 sorts in two passes, which publish no per-score table: host-out calls take the all-gather + merge
+    long_needle = "abcdefghijklmnopqrstuvwxyzabcdefghijklmnopqrstuvwxyzabcdefgh"   # 60 bytes
+    d5, o5 = synth.generate(long_needle, 20_001, 80, 128, seed=2, p_full=0.5)
+    for sort in (SortStrategy.ScoreThenIndexAsc, SortStrategy.ScoreThenIndexDesc):
+        ok = run_case(comm, rank, world, local, long_needle, Config(max_typos=None, sort=sort), d5, o5, f"two-pass bound sort={sort.name}") and ok
     # fewer haystacks than ranks (empty shards), and the empty list
     for n3 in (1, 0):
         d3, o3 = synth.generate("deadbeef", n3, 24, 32, seed=3, p_full=1.0, p_partial=0.0)
@@ -91,14 +127,7 @@ def main():
     comm.barrier()
     comm.host_free(out)
     shard.close(); mq.close()
-    ok = ok and m_ok
-    flag = torch.tensor([0 if ok else 1], device=torch.device("cuda", local))
-    dist.all_reduce(flag)
-    comm.close()
-    dist.barrier()
-    dist.destroy_process_group()
-    if int(flag.item()) != 0:
-        sys.exit(1)
+    finish(local, ok and m_ok, comm)
 
 
 if __name__ == "__main__":

@@ -12,6 +12,11 @@ import pytest
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+LONG_NEEDLE = "abcdefghijklmnopqrstuvwxyzabcdefghijklmnopqrstuvwxyzabcdefgh"   # 60 bytes: score bound >= 1024
+# FRZ_PARALLEL_EXCHANGE of the 2-GPU tests: unset (the default P2P placement), `slices` (the NCCL slice exchange), and
+# two values that named removed forms, which communicator creation must refuse
+EXCHANGES = [pytest.param(None, id="p2p"), "slices", "direct", "allgather"]
+REFUSED = ("direct", "allgather")
 
 
 def _gpus():
@@ -125,7 +130,7 @@ def test_sort_scratch_regrows_for_a_larger_corpus():
     from frizbee_b200 import synth
     from frizbee_b200.types import Config
     from oracle import pyoracle as O
-    needle = "abcdefghijklmnopqrstuvwxyzabcdefghijklmnopqrstuvwxyzabcdefgh"   # 60 bytes: score bound >= 1024
+    needle = LONG_NEEDLE
     cfg = Config(max_typos=None)
     m = F.Matcher(needle, cfg)
     assert m.score_bound() >= 1024
@@ -153,19 +158,57 @@ def test_c_client_on_the_gpu(tmp_path):
     assert f"match_list_parallel over {n} GPU(s)" in r.stdout and "parallel == sequential: yes" in r.stdout
 
 
-@pytest.mark.parametrize("exchange", ["direct", "p2p", "slices", "allgather"])
+@pytest.mark.parametrize("value", ["direct", "allgather"])
+def test_exchange_variable_accepts_only_slices(value, monkeypatch):
+    """FRZ_PARALLEL_EXCHANGE is a test hook with one value, `slices`: any other value fails communicator creation, in the
+    local and in the multi-process form, instead of silently running the default exchange."""
+    import frizbee_b200 as F
+    from frizbee_b200 import parallel
+    from frizbee_b200.types import Config
+    unique_id = parallel.Comm.unique_id()
+    monkeypatch.setenv("FRZ_PARALLEL_EXCHANGE", value)
+    for create in (lambda: parallel.Comm.local(1), lambda: parallel.Comm.from_rank(unique_id, 1, 0, 0)):
+        with pytest.raises(F.FrizbeeError) as e:
+            create()
+        assert e.value.status_name == "FRZ_ERR_INVALID_ARG" and "FRZ_PARALLEL_EXCHANGE" in str(e.value)
+    monkeypatch.setenv("FRZ_PARALLEL_EXCHANGE", "slices")
+    comm = parallel.Comm.local(1)
+    assert comm.exchange_mode() == 1
+    hs = _haystacks_4101()
+    d, o = F.pack_host(hs)
+    shards = comm.shard_arrow(d, o)
+    m = F.Matcher("foo", Config())
+    assert [int(x) for x in comm.match_list_parallel(m, shards)["index"]] == [x.index for x in m.match_list(hs)]
+    m.close()
+    for s in shards:
+        s.close()
+    comm.close()
+
+
+@pytest.mark.parametrize("exchange", EXCHANGES)
 def test_local_form_two_gpus(exchange, monkeypatch):
-    """Single process, two GPUs (frz_comm_create_local: ncclCommInitAll + one worker thread per GPU), with all four forms of
-    the exchange step: direct placement into the mapped host buffer (k_place<DIRECT>), P2P placement (k_place: every GPU stores its matches at their merged positions in the peers' slice
-    buffers over NVLink), the slice exchange (grouped ncclSend/ncclRecv of exactly what each rank copies out) and the
-    all-gather of whole runs."""
+    """Single process, two GPUs (frz_comm_create_local: ncclCommInitAll + one worker thread per GPU), with both forms of
+    the host-out exchange step: P2P placement (k_place: every GPU stores its matches at their merged positions in the
+    peers' slice buffers over NVLink) and the slice exchange (grouped ncclSend/ncclRecv of exactly what each rank copies
+    out).  A score bound >= 1024 sorts in two passes, which publish no per-score table: those host-out calls take the
+    all-gather of whole runs + merge, like every device-out call.  `direct` and `allgather` named removed forms: a
+    two-GPU communicator must refuse them."""
     if _gpus() < 2:
         pytest.skip("needs >= 2 GPUs")
     import frizbee_b200 as F
     from frizbee_b200 import parallel, synth
     from frizbee_b200.types import Config, SortStrategy
-    monkeypatch.setenv("FRZ_PARALLEL_EXCHANGE", exchange)
+    if exchange is None:
+        monkeypatch.delenv("FRZ_PARALLEL_EXCHANGE", raising=False)
+    else:
+        monkeypatch.setenv("FRZ_PARALLEL_EXCHANGE", exchange)
+    if exchange in REFUSED:
+        with pytest.raises(F.FrizbeeError) as e:
+            parallel.Comm.local(2)
+        assert e.value.status_name == "FRZ_ERR_INVALID_ARG"
+        return
     comm = parallel.Comm.local(2)
+    assert comm.exchange_mode() == (1 if exchange == "slices" else 2)
     data, off = synth.generate("deadbeef", 300_001, 48, 64, seed=33)
     shards = comm.shard_arrow(data, off)
     whole = F.Corpus.from_arrow(data, off)
@@ -182,20 +225,36 @@ def test_local_form_two_gpus(exchange, monkeypatch):
     s2 = comm.shard_arrow(d2, o2)
     m = F.Matcher("foo", Config())
     assert [int(x) for x in comm.match_list_parallel(m, s2)["index"]] == [x.index for x in m.match_list(hs)]
+    m.close()
+    d3, o3 = synth.generate(LONG_NEEDLE, 20_001, 80, 128, seed=2, p_full=0.5)
+    s3 = comm.shard_arrow(d3, o3)
+    w3 = F.Corpus.from_arrow(d3, o3)
+    for sort in (SortStrategy.ScoreThenIndexAsc, SortStrategy.ScoreThenIndexDesc):
+        m = F.Matcher(LONG_NEEDLE, Config(max_typos=None, sort=sort))
+        assert m.score_bound() >= 1024
+        got = comm.match_list_parallel(m, s3, out)
+        want = m.match_list_array(w3)
+        assert len(got) == len(want) and np.array_equal(np.array(got), want), ("two-pass bound", sort)
+        m.close()
     comm.host_free(out)
-    for s in shards + s2:
+    for s in shards + s2 + s3:
         s.close()
-    whole.close(); comm.close()
+    whole.close(); w3.close(); comm.close()
 
 
-@pytest.mark.parametrize("exchange", ["direct", "p2p", "slices", "allgather"])
+@pytest.mark.parametrize("exchange", EXCHANGES)
 def test_match_list_parallel_two_gpus_torchrun(exchange):
-    """One rank per GPU under torchrun (the bench's launch mode): tests/_multi_gpu_worker.py, with all four forms of the
-    exchange step for the host-out calls (device-only calls always all-gather; p2p maps the peers' slice buffers with cudaIpc)."""
+    """One rank per GPU under torchrun (the bench's launch mode): tests/_multi_gpu_worker.py, with both forms of the
+    exchange step for the host-out calls (P2P placement maps the peers' slice buffers with cudaIpc; device-only calls and
+    the worker's two-pass score bound query take the all-gather).  Under `direct` and `allgather` every rank's
+    frz_comm_create_rank must refuse the value."""
     if _gpus() < 2:
         pytest.skip("needs >= 2 GPUs")
     world = 2
-    env = dict(os.environ, FRZ_PARALLEL_TIMEOUT_S="60", FRZ_PARALLEL_EXCHANGE=exchange)
+    env = dict(os.environ, FRZ_PARALLEL_TIMEOUT_S="60")
+    env.pop("FRZ_PARALLEL_EXCHANGE", None)
+    if exchange:
+        env["FRZ_PARALLEL_EXCHANGE"] = exchange
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", str(world), "--master-addr", "127.0.0.1",
            "--master-port", "29533", os.path.join(ROOT, "tests", "_multi_gpu_worker.py")]
     r = subprocess.run(cmd, capture_output=True, text=True, timeout=900, env=env)
@@ -203,3 +262,5 @@ def test_match_list_parallel_two_gpus_torchrun(exchange):
     sys.stderr.write(r.stderr[-4000:])
     assert r.returncode == 0
     assert "False" not in r.stdout and "differs" not in r.stdout
+    if exchange in REFUSED:
+        assert r.stdout.count("communicator refused with FRZ_ERR_INVALID_ARG: True") == world

@@ -15,6 +15,11 @@ from frizbee_b200.types import Config, Matching, Pattern, Scoring, SortStrategy
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SEG = 2048   # elements per segment of the fused scatter (kFrzSortSegShift in frz_host.h)
+LONG_NEEDLE = "abcdefghijklmnopqrstuvwxyzabcdefghijklmnopqrstuvwxyzabcdefgh"   # 60 bytes: score bound >= 1024
+# FRZ_PARALLEL_EXCHANGE of the 2-GPU tests: unset (the default P2P placement), `slices` (the NCCL slice exchange), and
+# two values that named removed forms, which communicator creation must refuse
+EXCHANGES = [pytest.param(None, id="p2p"), "slices", "direct", "allgather"]
+REFUSED = ("direct", "allgather")
 
 
 def _gpus():
@@ -207,12 +212,23 @@ def test_parallel_top_world1(force_nccl, monkeypatch):
     whole.close(); comm.close()
 
 
-@pytest.mark.parametrize("exchange", ["direct", "p2p", "slices", "allgather"])
+@pytest.mark.parametrize("exchange", EXCHANGES)
 def test_parallel_top_two_gpus_local(exchange, monkeypatch):
+    """Both host-out exchange forms; a score bound >= 1024 (two-pass sort, no per-score table) takes the all-gather + merge.
+    `direct` and `allgather` named removed forms: a two-GPU communicator must refuse them."""
     if _gpus() < 2:
         pytest.skip("needs >= 2 GPUs")
-    monkeypatch.setenv("FRZ_PARALLEL_EXCHANGE", exchange)
+    if exchange is None:
+        monkeypatch.delenv("FRZ_PARALLEL_EXCHANGE", raising=False)
+    else:
+        monkeypatch.setenv("FRZ_PARALLEL_EXCHANGE", exchange)
+    if exchange in REFUSED:
+        with pytest.raises(F.FrizbeeError) as e:
+            parallel.Comm.local(2)
+        assert e.value.status_name == "FRZ_ERR_INVALID_ARG"
+        return
     comm = parallel.Comm.local(2)
+    assert comm.exchange_mode() == (1 if exchange == "slices" else 2)
     data, off = synth.generate("deadbeef", 300_001, 48, 64, seed=33)
     shards = comm.shard_arrow(data, off)
     out = comm.host_alloc_matches(300_001)
@@ -224,17 +240,31 @@ def test_parallel_top_two_gpus_local(exchange, monkeypatch):
                 top, total = comm.match_list_parallel_top(m, shards, k, out)
                 assert total == len(full) and np.array_equal(np.array(top), full[:k]), (exchange, sort, k_typos, k)
             m.close()
+    d2, o2 = synth.generate(LONG_NEEDLE, 20_001, 80, 128, seed=2, p_full=0.5)
+    s2 = comm.shard_arrow(d2, o2)
+    w2 = F.Corpus.from_arrow(d2, o2)
+    for sort in (SortStrategy.ScoreThenIndexAsc, SortStrategy.ScoreThenIndexDesc):
+        m = F.Matcher(LONG_NEEDLE, Config(max_typos=None, sort=sort))
+        assert m.score_bound() >= 1024
+        full = m.match_list_array(w2).copy()
+        for k in edge_ks(len(full)) + [len(full) // 2 + 1]:
+            top, total = comm.match_list_parallel_top(m, s2, k, out)
+            assert total == len(full) and np.array_equal(np.array(top), full[:k]), (exchange, "two-pass bound", sort, k)
+        m.close()
     comm.host_free(out)
-    for s in shards:
+    for s in shards + s2:
         s.close()
-    comm.close()
+    w2.close(); comm.close()
 
 
-@pytest.mark.parametrize("exchange", ["direct", "p2p", "slices", "allgather"])
+@pytest.mark.parametrize("exchange", EXCHANGES)
 def test_parallel_top_two_gpus_torchrun(exchange):
     if _gpus() < 2:
         pytest.skip("needs >= 2 GPUs")
-    env = dict(os.environ, FRZ_PARALLEL_TIMEOUT_S="60", FRZ_PARALLEL_EXCHANGE=exchange)
+    env = dict(os.environ, FRZ_PARALLEL_TIMEOUT_S="60")
+    env.pop("FRZ_PARALLEL_EXCHANGE", None)
+    if exchange:
+        env["FRZ_PARALLEL_EXCHANGE"] = exchange
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node", "2", "--master-addr", "127.0.0.1",
            "--master-port", "29541", os.path.join(ROOT, "tests", "_top_multi_gpu_worker.py")]
     r = subprocess.run(cmd, capture_output=True, text=True, timeout=900, env=env)
@@ -242,6 +272,8 @@ def test_parallel_top_two_gpus_torchrun(exchange):
     sys.stderr.write(r.stderr[-4000:])
     assert r.returncode == 0
     assert "False" not in r.stdout and "differs" not in r.stdout
+    if exchange in REFUSED:
+        assert r.stdout.count("communicator refused with FRZ_ERR_INVALID_ARG: True") == 2
 
 
 def test_parallel_rank_top_world1():
