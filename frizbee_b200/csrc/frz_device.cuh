@@ -24,8 +24,18 @@
 #define FRZ_UNIT 16            // bytes per unit
 #define FRZ_MAX_HAY_LEN ((1u << 22) - 1)  // slot meta keeps len in 22 bits
 #define FRZ_INVALID_SLOT 0xFFFFFFFFu      // slot meta of an unused slot (last tile)
-#define FRZ_MAX_NEEDLE 64      // needle bytes handled by the kernels (longer → FRZ_ERR_UNSUPPORTED)
+#define FRZ_MAX_NEEDLE 64      // needle bytes whose per-position data lives in FrzPatternDev (the constant bank)
+#define FRZ_LONG_NEEDLE 1024   // longest byte-path needle: 65..1024 bytes read FrzNeedleTab (longer → FRZ_ERR_UNSUPPORTED)
 #define FRZ_SW_MAX_WINDOW 1024 // src/smith_waterman/algo/mod.rs:18 (MAX_HAYSTACK_LEN)
+
+// Per-position data of a needle of FRZ_MAX_NEEDLE + 1 .. FRZ_LONG_NEEDLE bytes (the byte path's case_needle pairs and word
+// probes, as in FrzPatternDev).  Device-resident, owned by the matcher; the long-needle kernels stage it in shared memory.
+struct __align__(16) FrzNeedleTab {
+    uint8_t c[FRZ_LONG_NEEDLE];
+    uint8_t flip[FRZ_LONG_NEEDLE];
+    uint8_t om[FRZ_LONG_NEEDLE];
+    uint8_t tg[FRZ_LONG_NEEDLE];
+};
 
 struct __align__(16) FrzGroupDesc {
     uint64_t abs_off;   // first unit of the group, in 16-byte units from the start of the packed data
@@ -103,6 +113,9 @@ struct FrzPatternDev {
     uint32_t sig_need1, sig_need2;      // byte classes the needle holds at least once / at least twice
     // untruncated scoring for the literal matcher / greedy fallback (u16 arithmetic)
     int32_t raw_match, raw_mismatch, raw_gap_open, raw_gap_extend, raw_prefix, raw_cap, raw_case, raw_delim;
+    // (n > FRZ_MAX_NEEDLE: the arrays above hold the first FRZ_MAX_NEEDLE positions; the long-needle kernels take the
+    // whole FrzNeedleTab as a kernel argument of their own, so that this struct, and with it the constant-bank offsets of
+    // every argument of the short-needle kernels, keeps its size)
 };
 
 // Byte class of the signature index (32 classes).  ASCII letters fold case (a needle byte and its case flip share a

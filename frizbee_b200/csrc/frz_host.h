@@ -161,8 +161,9 @@ struct FrzLaunchStats {
     uint64_t launches = 0;
 };
 
+// ntab: the needle's FrzNeedleTab (device) when pat.n > FRZ_MAX_NEEDLE, else unused
 frz_status frz_launch_prefilter(const FrzCorpusView& cv, const FrzPatternDev& pat, FrzWorkspace& ws, cudaStream_t stream,
-                                FrzLaunchStats* st);
+                                FrzLaunchStats* st, const FrzNeedleTab* ntab = nullptr);
 frz_status frz_launch_sig_scan(const FrzCorpusView& cv, const FrzPatternDev& pat, FrzWorkspace& ws, cudaStream_t stream,
                                FrzLaunchStats* st);
 frz_status frz_launch_unicode(const FrzCorpusView& cv, const FrzPatternDev& pat, const FrzUNeedle& un, const FrzUScoring& usc,
@@ -174,13 +175,13 @@ frz_status frz_launch_match_indices(const FrzCorpusView& cv, const FrzPatternDev
                                     cudaStream_t stream);
 frz_status frz_launch_prefilter_list(const FrzCorpusView& cv, const FrzPatternDev& pat, const FrzMatchDev* cand,
                                      uint64_t n_cand, uint32_t index_offset, FrzWorkspace& ws, cudaStream_t stream,
-                                     FrzLaunchStats* st);
+                                     FrzLaunchStats* st, const FrzNeedleTab* ntab = nullptr);
 frz_status frz_launch_tile_scan(const FrzCorpusView& cv, FrzWorkspace& ws, cudaStream_t stream, FrzLaunchStats* st,
                                 unsigned long long* carry = nullptr);
 // hist.counts != nullptr: every emitted match also counts itself into `hist` (see FrzScoreHist)
 frz_status frz_launch_sw(const FrzCorpusView& cv, const FrzPatternDev& pat, uint32_t index_offset, bool reversed,
                          FrzWorkspace& ws, FrzMatchDev* d_out, cudaStream_t stream, FrzLaunchStats* st,
-                         const FrzScoreHist& hist = FrzScoreHist());
+                         const FrzScoreHist& hist = FrzScoreHist(), const FrzNeedleTab* ntab = nullptr);
 // "no limit" for the sorts' `limit` argument: every position of a list is below it (lists hold at most 2^32 - 1 matches)
 constexpr uint32_t kFrzNoLimit = 0xFFFFFFFFu;
 // stable sort by descending score; the element count is read from device memory (*n_ptr).

@@ -376,6 +376,9 @@ struct Compiled {
     FrzUNeedle un;             // case_needle_unicode (valid when `unicode`)
     FrzUScoring usc;
     uint32_t score_bound = 0;  // host-side upper bound of any score this pattern can emit
+    // needle of more than FRZ_MAX_NEEDLE bytes: its per-position data (host copy), uploaded per device by pattern_for_launch
+    std::shared_ptr<const FrzNeedleTab> tab;
+    bool is_long() const { return dev.n > FRZ_MAX_NEEDLE; }
 };
 
 // Matcher::compile + get_backend (src/matcher/mod.rs:193-205, 448-498) → device pattern
@@ -403,7 +406,10 @@ frz_status compile_pattern(const OwnedPattern& src, const frz_config& mcfg, bool
     if (casing == FRZ_CASE_IGNORE) case_sensitive = false;
     else if (casing == FRZ_CASE_RESPECT) case_sensitive = true;
     else case_sensitive = frz_needle_has_uppercase(nd, n);
-    if (n > FRZ_MAX_NEEDLE) return frz_fail(FRZ_ERR_UNSUPPORTED, "needle of %zu bytes exceeds the GPU kernels' limit of %d", n, FRZ_MAX_NEEDLE);
+    if (n > FRZ_LONG_NEEDLE) return frz_fail(FRZ_ERR_UNSUPPORTED, "needle of %zu bytes exceeds the GPU kernels' limit of %d", n, FRZ_LONG_NEEDLE);
+    if (n > FRZ_MAX_NEEDLE && needs_unicode)
+        return frz_fail(FRZ_ERR_UNSUPPORTED, "needle of %zu bytes takes the unicode path, whose kernels handle up to %d bytes", n,
+                        FRZ_MAX_NEEDLE);
 
     Compiled c;
     FrzPatternDev& d = c.dev;
@@ -414,10 +420,11 @@ frz_status compile_pattern(const OwnedPattern& src, const frz_config& mcfg, bool
     if (needs_unicode) {
         if (!frz_build_uneedle(nd, n, case_sensitive, &c.un)) return frz_fail(FRZ_ERR_INVALID_ARG, "the needle is not valid UTF-8");
     } else {
-        // byte path: only the byte-level case_needle pairs are used (frz_match_indices); the needle may be any bytes
+        // byte path: only the byte-level case_needle pairs are used (frz_match_indices, which refuses long needles); the
+        // needle may be any bytes
         memset(&c.un, 0, sizeof c.un);
         c.un.nbytes = (int32_t)n;
-        for (size_t i = 0; i < n; i++) {
+        for (size_t i = 0; i < n && i < FRZ_MAX_NEEDLE; i++) {
             const uint8_t ch = nd[i];
             c.un.c[i] = ch;
             c.un.f[i] = ch;
@@ -427,17 +434,24 @@ frz_status compile_pattern(const OwnedPattern& src, const frz_config& mcfg, bool
     d.n = (int)n;
     d.matching = matching;
     d.case_sensitive = case_sensitive;
+    FrzNeedleTab tab;   // per-position data; FrzPatternDev keeps its first FRZ_MAX_NEEDLE positions
+    memset(&tab, 0, sizeof tab);
     for (size_t i = 0; i < n; i++) {  // case_needle (src/prefilter/mod.rs:49-65)
         uint8_t ch = nd[i], fl;
         if (case_sensitive) fl = ch;
         else if (ch >= 'a' && ch <= 'z') fl = (uint8_t)(ch - 32);
         else if (ch >= 'A' && ch <= 'Z') fl = (uint8_t)(ch + 32);
         else fl = ch;
-        d.c[i] = ch; d.flip[i] = fl;
-        d.om[i] = fl != ch ? 0x20 : 0;
-        d.tg[i] = fl != ch ? (uint8_t)(ch | 0x20) : ch;
+        tab.c[i] = ch; tab.flip[i] = fl;
+        tab.om[i] = fl != ch ? 0x20 : 0;
+        tab.tg[i] = fl != ch ? (uint8_t)(ch | 0x20) : ch;
     }
-    {   // distinct (om, tg) classes
+    const size_t n_short = std::min<size_t>(n, FRZ_MAX_NEEDLE);
+    memcpy(d.c, tab.c, n_short); memcpy(d.flip, tab.flip, n_short); memcpy(d.om, tab.om, n_short); memcpy(d.tg, tab.tg, n_short);
+    if (n > FRZ_MAX_NEEDLE) c.tab = std::make_shared<const FrzNeedleTab>(tab);
+    // distinct (om, tg) classes for the occurrence-mask prefilter.  A long needle takes the scanning forms (n_distinct 0):
+    // over 64 bytes of ordinary text seldom stay within 16 classes.
+    if (n <= FRZ_MAX_NEEDLE) {
         int nd = 0;
         bool ok = true;
         for (size_t i = 0; i < n && ok; i++) {
@@ -475,7 +489,7 @@ frz_status compile_pattern(const OwnedPattern& src, const frz_config& mcfg, bool
             // every byte, an ASCII scalar is matched by the same letter in either case, which the classes fold)
             uint32_t cnt[32] = {0};
             for (size_t i = 0; i < n; i++)
-                if (!needs_unicode || d.c[i] < 0x80) cnt[frz_sig_bucket(d.c[i])]++;
+                if (!needs_unicode || nd[i] < 0x80) cnt[frz_sig_bucket(nd[i])]++;
             for (int b2 = 0; b2 < 32; b2++) {
                 if (cnt[b2] >= 1) d.sig_need1 |= 1u << b2;
                 if (cnt[b2] >= 2) d.sig_need2 |= 1u << b2;
@@ -534,7 +548,7 @@ frz_status compile_pattern(const OwnedPattern& src, const frz_config& mcfg, bool
         d.k_up_plain = sp(-d.gap_extend);
         d.k_up_open = sp(-(d.gap_extend + d.gap_open_x));
         d.k_case = sp(d.case_bonus); d.k_cap = sp(d.cap_bonus); d.k_delim = sp(d.delim_bonus); d.k_base = sp(d.match_x);
-        for (size_t i = 0; i < n; i++) { d.om16[i] = sp(d.om[i]); d.tg16[i] = sp(d.tg[i]); d.c16[i] = sp(d.c[i]); }
+        for (size_t i = 0; i < n_short; i++) { d.om16[i] = sp(d.om[i]); d.tg16[i] = sp(d.tg[i]); d.c16[i] = sp(d.c[i]); }
     }
     // the kernels keep cells in signed 16-bit lanes: every intermediate must stay below 2^15
     const uint64_t cell_bound = (uint64_t)n * ((uint64_t)sc.match_score + maxb + sc.matching_case_bonus) + sc.prefix_bonus +
@@ -545,7 +559,7 @@ frz_status compile_pattern(const OwnedPattern& src, const frz_config& mcfg, bool
     d.wrap8 = use_u8 && cell_bound > 255;  // cannot prove "no u8 add ever wraps" → emulate the wrap
     {   // column-limited SW classes need: padding bytes (0) never match, and plain (non-wrapping) arithmetic
         bool has_nul = false;
-        for (int i = 0; i < d.n; i++) has_nul = has_nul || d.c[i] == 0;
+        for (size_t i = 0; i < n; i++) has_nul = has_nul || nd[i] == 0;
         d.col_classes = (!d.wrap8 && !has_nul) ? 1 : 0;
     }
     if (max_typos < 0) d.typo_mode = FRZ_T_NONE;
@@ -565,7 +579,7 @@ frz_status compile_pattern(const OwnedPattern& src, const frz_config& mcfg, bool
         // literal branch above), which keeps the sum a lower bound.
         uint32_t cnt[32] = {0};
         for (size_t i = 0; i < n; i++)
-            if (!needs_unicode || d.c[i] < 0x80) cnt[frz_sig_bucket(d.c[i])]++;
+            if (!needs_unicode || nd[i] < 0x80) cnt[frz_sig_bucket(nd[i])]++;
         d.sig_need1 = d.sig_need2 = 0;
         for (int b2 = 0; b2 < 32; b2++) {
             if (cnt[b2] >= 1) d.sig_need1 |= 1u << b2;
@@ -625,7 +639,12 @@ struct frz_matcher {
     bool timings_pending = false;
     uint64_t epoch = 0;                    // identity of the compiled patterns (clones made for another epoch are stale)
     int last_sort_bins = 0;                // bins of the single-pass score sort of the last call (0: none / two passes)
+    // the long needles' FrzNeedleTab, in pattern order, on ntab_device for the patterns of ntab_epoch
+    FrzNeedleTab* ntab = nullptr;
+    int ntab_device = -1;
+    uint64_t ntab_epoch = 0;
     ~frz_matcher() {
+        if (ntab) { cudaSetDevice(ntab_device); cudaFree(ntab); }
         if (ws.device >= 0) { cudaSetDevice(ws.device); cudaFree(multi_a); cudaFree(multi_b); if (count_ev) cudaEventDestroy(count_ev); }
         if (e2e_ingest.d_bytes || e2e_ingest.copy_stream || e2e_corpus.st.data) {
             cudaSetDevice(e2e_corpus.st.device);
@@ -922,6 +941,38 @@ uint64_t initial_survivor_cap(const FrzCorpusStorage& cs, const FrzPatternDev& d
     return std::min<uint64_t>(std::max<uint64_t>(cs.n / 4, 1 << 16), std::max<uint64_t>(cs.n, 1));
 }
 
+// A long needle's FrzNeedleTab on the workspace's device, uploaded once per compiled pattern set (build_patterns starts a
+// new epoch) and device; nullptr for other needles.
+frz_status needle_table(frz_matcher* m, const Compiled& c, const FrzNeedleTab** out) {
+    *out = nullptr;
+    if (!c.is_long()) return FRZ_OK;
+    if (m->ntab_device != m->ws.device || m->ntab_epoch != m->epoch) {
+        if (m->ntab) {
+            cudaSetDevice(m->ntab_device);
+            cudaFree(m->ntab);
+            m->ntab = nullptr;
+            FRZ_CUDA_TRY(cudaSetDevice(m->ws.device));
+        }
+        m->ntab_device = -1;
+        size_t k = 0;
+        for (const Compiled& p : m->compiled) k += p.is_long() ? 1 : 0;
+        FRZ_CUDA_TRY(cudaMalloc(&m->ntab, k * sizeof(FrzNeedleTab)));
+        m->ntab_device = m->ws.device;   // (freed by the destructor or the next upload even when a copy below fails)
+        m->ntab_epoch = 0;
+        k = 0;
+        for (const Compiled& p : m->compiled)
+            if (p.is_long()) FRZ_CUDA_TRY(cudaMemcpy(m->ntab + k++, p.tab.get(), sizeof(FrzNeedleTab), cudaMemcpyHostToDevice));
+        m->ntab_epoch = m->epoch;
+    }
+    size_t k = 0;
+    for (const Compiled& p : m->compiled) {
+        if (&p == &c) break;
+        k += p.is_long() ? 1 : 0;
+    }
+    *out = m->ntab + k;
+    return FRZ_OK;
+}
+
 // One pattern over the corpus (optionally restricted to a candidate bitmap) → index-ordered matches in
 // d_out (reversed order if `reversed`); the count is left in ws.counters->total (device).
 frz_status run_pattern(frz_matcher* m, const FrzCorpusStorage& cs, const Compiled& c, const uint32_t* cand_bitmap,
@@ -932,11 +983,13 @@ frz_status run_pattern(frz_matcher* m, const FrzCorpusStorage& cs, const Compile
     const FrzCorpusView cv = cs.view();
     uint64_t cap = std::max(ws.survivor_cap, initial_survivor_cap(cs, c.dev));
     FRZ_TRY(ensure_workspace(m, cs, cap));
+    const FrzNeedleTab* ntab = nullptr;
+    FRZ_TRY(needle_table(m, c, &ntab));
     FRZ_CUDA_TRY(cudaMemsetAsync(ws.counters, 0, sizeof(FrzCounters), stream));
     if (record_events) { cudaEventRecord(ws.ev[0], stream); ws.ev_rec[0] = true; }
     if (c.unicode) FRZ_TRY(frz_launch_unicode(cv, c.dev, c.un, c.usc, cand_list, n_cand, index_offset, ws, stream, st));
-    else if (cand_list) FRZ_TRY(frz_launch_prefilter_list(cv, c.dev, cand_list, n_cand, index_offset, ws, stream, st));
-    else FRZ_TRY(frz_launch_prefilter(cv, c.dev, ws, stream, st));
+    else if (cand_list) FRZ_TRY(frz_launch_prefilter_list(cv, c.dev, cand_list, n_cand, index_offset, ws, stream, st, ntab));
+    else FRZ_TRY(frz_launch_prefilter(cv, c.dev, ws, stream, st, ntab));
     FRZ_TRY(frz_launch_tile_scan(cv, ws, stream, st));
     if (record_events) { cudaEventRecord(ws.ev[1], stream); ws.ev_rec[1] = true; }
     if (m->early_count_dst && !cand_list && !cand_bitmap && m->compiled.size() == 1) {
@@ -953,7 +1006,7 @@ frz_status run_pattern(frz_matcher* m, const FrzCorpusStorage& cs, const Compile
         emit.typo_mode = FRZ_T_LITERAL;
         FRZ_TRY(frz_launch_sw(cv, emit, index_offset, reversed, ws, d_out, stream, st, hist));
     } else {
-        FRZ_TRY(frz_launch_sw(cv, c.dev, index_offset, reversed, ws, d_out, stream, st, hist));
+        FRZ_TRY(frz_launch_sw(cv, c.dev, index_offset, reversed, ws, d_out, stream, st, hist, ntab));
     }
     if (record_events) { cudaEventRecord(ws.ev[2], stream); ws.ev_rec[2] = true; }
     return FRZ_OK;
@@ -1336,6 +1389,9 @@ extern "C" frz_status frz_match_indices(frz_matcher* m, const frz_corpus* corpus
     if (!m || !corpus || (n && (!which || !out_matches || !out_indices || !out_counts)) || stride == 0)
         return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
     if (m->compiled.empty()) return frz_fail(FRZ_ERR_INVALID_ARG, "the matcher has no pattern");
+    for (const Compiled& c : m->compiled)   // the indices kernel keeps per-needle-byte state in arrays of FRZ_MAX_NEEDLE
+        if (c.is_long())
+            return frz_fail(FRZ_ERR_UNSUPPORTED, "match_indices handles needles of up to %d bytes (this one has %d)", FRZ_MAX_NEEDLE, c.dev.n);
     if (n == 0) return FRZ_OK;
     FRZ_TRY(ensure_device(corpus->st.device));
     if (m->compiled.size() == 1 && !m->compiled[0].negated)   // CompiledPatterns::Single
@@ -1432,6 +1488,7 @@ struct StreamedCtx {
     const Compiled* c;
     uint32_t index_offset;
     FrzMatchDev* dst;       // index-ordered matches (pre-sort)
+    const FrzNeedleTab* ntab;   // the needle table of a long needle (uploaded before the ingest starts), else nullptr
     cudaStream_t stream;
     FrzLaunchStats* st;
     uint32_t pending_t0;    // first tile not yet matched
@@ -1452,7 +1509,7 @@ frz_status streamed_range(StreamedCtx& x, uint32_t t0, uint32_t t1, bool last) {
     cv.n_tiles = t1 - t0;
     const uint32_t off = x.index_offset + t0 * FRZ_TILE;
     FRZ_CUDA_TRY(cudaMemsetAsync(ws.counters, 0, sizeof(FrzCounters), x.stream));
-    FRZ_TRY(frz_launch_prefilter(cv, x.c->dev, ws, x.stream, x.st));
+    FRZ_TRY(frz_launch_prefilter(cv, x.c->dev, ws, x.stream, x.st, x.ntab));
     FRZ_TRY(frz_launch_tile_scan(cv, ws, x.stream, x.st, ws.stream_total));
     if (last) {
         cudaEventRecord(ws.ev[1], x.stream); ws.ev_rec[1] = true;
@@ -1462,7 +1519,7 @@ frz_status streamed_range(StreamedCtx& x, uint32_t t0, uint32_t t1, bool last) {
             m->count_published = true;
         }
     }
-    FRZ_TRY(frz_launch_sw(cv, x.c->dev, off, false, ws, x.dst, x.stream, x.st));
+    FRZ_TRY(frz_launch_sw(cv, x.c->dev, off, false, ws, x.dst, x.stream, x.st, FrzScoreHist(), x.ntab));
     return FRZ_OK;
 }
 frz_status streamed_after_chunk(void* ctx, uint32_t t0, uint32_t t1, bool last) {
@@ -1535,6 +1592,7 @@ frz_status match_streamed_impl(frz_matcher* m, const uint8_t* bytes, const void*
     ws.table_ev_recorded = false;
     StreamedCtx x;
     x.m = m; x.c = &pat; x.index_offset = index_offset; x.dst = will_sort ? ws.matches_a : final_out; x.stream = stream; x.st = &st;
+    FRZ_TRY(needle_table(m, pat, &x.ntab));   // a synchronous upload, so before the first H2D chunk
     x.pending_t0 = 0; x.chunks_pending = 0;
     x.group = 4;   // a range per four H2D chunks (about 1/8 of the list): the tail after the last chunk is one range + the sort
     const frz_status ms = [&]() -> frz_status {

@@ -23,6 +23,7 @@
 #include "frz_device.cuh"
 #include <cuda_pipeline.h>
 #include <algorithm>
+#include <type_traits>
 
 #include "frz_host.h"
 #include "indices_path.cuh"
@@ -82,15 +83,43 @@ __device__ __forceinline__ int find_last2(const A& a, uint32_t om1, uint32_t tg1
     }
 }
 
+// The needle as the prefilter forms below read it (template parameter P): FrzPatternDev itself for needles of up to
+// FRZ_MAX_NEEDLE bytes (per-position data in the constant bank), LongPat for longer ones (per-position data staged from
+// FrzNeedleTab into shared memory, scalars from the pattern).  The forms use the same member names on both.
+struct LongPat {
+    const uint8_t *c, *flip, *om, *tg;   // shared memory
+    int n, pf_lanes, sw_lanes, max_typos, matching, col_classes, n_distinct;
+    uint32_t raw_match, raw_case, raw_prefix, raw_cap, raw_delim, exact_bonus;
+};
+// the block's copy of the table (first 4 * n bytes of `tab_s`); call before the block's first barrier
+__device__ __forceinline__ LongPat stage_long_pat(const FrzPatternDev& p, const FrzNeedleTab* __restrict__ ntab, uint8_t* tab_s) {
+    const int n = p.n;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        tab_s[i] = ntab->c[i];
+        tab_s[n + i] = ntab->flip[i];
+        tab_s[2 * n + i] = ntab->om[i];
+        tab_s[3 * n + i] = ntab->tg[i];
+    }
+    LongPat l;
+    l.c = tab_s; l.flip = tab_s + n; l.om = tab_s + 2 * n; l.tg = tab_s + 3 * n;
+    l.n = n; l.pf_lanes = p.pf_lanes; l.sw_lanes = p.sw_lanes; l.max_typos = p.max_typos; l.matching = p.matching;
+    l.col_classes = p.col_classes; l.n_distinct = 0;
+    l.raw_match = p.raw_match; l.raw_case = p.raw_case; l.raw_prefix = p.raw_prefix; l.raw_cap = p.raw_cap;
+    l.raw_delim = p.raw_delim; l.exact_bonus = p.exact_bonus;
+    return l;
+}
+constexpr size_t kLongPatSmem = 4 * FRZ_LONG_NEEDLE;
+
 struct Probe {
     uint32_t om, tg;
 };
-__device__ __forceinline__ Probe probe_of(const FrzPatternDev& p, int i) { return Probe{splat4(p.om[i]), splat4(p.tg[i])}; }
+template <class P>
+__device__ __forceinline__ Probe probe_of(const P& p, int i) { return Probe{splat4(p.om[i]), splat4(p.tg[i])}; }
 
 // ---- Prefilter::match_haystack (0 typos): closed form of src/prefilter/algo/ascii.rs:6-54 ----
 // start = first occurrence of needle[0]; greedy in-order scan; end = 1 + last occurrence of needle[n-1]
-template <class A>
-__device__ bool window_k0(const A& a, const FrzPatternDev& p, int len, int* ostart, int* oend) {
+template <class A, class P>
+__device__ bool window_k0(const A& a, const P& p, int len, int* ostart, int* oend) {
     if (len == 0) return false;
     int pos = 0, start = 0, q = 0;
     for (int i = 0; i < p.n; i++) {
@@ -108,8 +137,8 @@ __device__ bool window_k0(const A& a, const FrzPatternDev& p, int len, int* osta
 
 // find_end_pos_with_typos (src/prefilter/algo/ascii_typos.rs:375-397): 1 + last occurrence of any of
 // the last (k+1) needle bytes, else len.  Chunk-independent.
-template <class A>
-__device__ int end_pos_with_typos(const A& a, const FrzPatternDev& p, int len, int k) {
+template <class A, class P>
+__device__ int end_pos_with_typos(const A& a, const P& p, int len, int k) {
     int best = -1;
     int first = p.n - 1 - k;
     for (int i = first; i < p.n; i += 2) {
@@ -124,8 +153,8 @@ __device__ int end_pos_with_typos(const A& a, const FrzPatternDev& p, int len, i
 // ---- match_haystack_1_typo (src/prefilter/algo/ascii_typos.rs:15-110), chunk-emulating ----
 // Both paths' chunk masks are always suffixes [pos, chunk_end) of the chunk, so a path is the pair
 // (needle index, position) and `first_path_chunk_mask > second_path_chunk_mask` ⇔ pf < ps.
-template <class A>
-__device__ bool window_k1(const A& a, const FrzPatternDev& p, int len, int* ostart, int* oend) {
+template <class A, class P>
+__device__ bool window_k1(const A& a, const P& p, int len, int* ostart, int* oend) {
     const int n = p.n;
     if (n <= 1) { *ostart = 0; *oend = len; return true; }
     if (len == 0) return false;
@@ -173,8 +202,8 @@ found:
 // ---- match_haystack_many_typos_impl (ascii_typos.rs:254-360); also used for k == 2 ----
 // NOTE the 2-typo specialisation (ascii_typos.rs:113-251) advances each path on its OWN first hit,
 // the N-typo version advances all paths on the single lowest hit; they are distinct algorithms.
-template <class A>
-__device__ bool window_k2(const A& a, const FrzPatternDev& p, int len, int* ostart, int* oend) {
+template <class A, class P>
+__device__ bool window_k2(const A& a, const P& p, int len, int* ostart, int* oend) {
     const int n = p.n;
     if (n <= 2) { *ostart = 0; *oend = len; return true; }
     if (len == 0) return false;
@@ -218,8 +247,8 @@ found:
 
 constexpr int kMaxPaths = 16;  // FRZ_T_MANY supports max_typos <= 15 on the GPU path
 
-template <class A>
-__device__ bool window_many(const A& a, const FrzPatternDev& p, int len, int* ostart, int* oend) {
+template <class A, class P>
+__device__ bool window_many(const A& a, const P& p, int len, int* ostart, int* oend) {
     const int n = p.n, k = p.max_typos;
     if (n <= k) { *ostart = 0; *oend = len; return true; }
     if (len == 0) return false;
@@ -273,16 +302,16 @@ __device__ __forceinline__ bool lit_is_delim(uint32_t b) {
 template <class A>
 __device__ __forceinline__ uint32_t byte_at(const A& a, int i) { return (a.word(i >> 2) >> ((i & 3) * 8)) & 0xff; }
 
-template <class A>
-__device__ bool lit_matches_at(const A& a, const FrzPatternDev& p, int pos) {
+template <class A, class P>
+__device__ bool lit_matches_at(const A& a, const P& p, int pos) {
     for (int k = 0; k < p.n; k++) {
         uint32_t b = byte_at(a, pos + k);
         if (b != p.c[k] && b != p.flip[k]) return false;
     }
     return true;
 }
-template <class A>
-__device__ uint32_t lit_score_at(const A& a, const FrzPatternDev& p, int len, int pos) {
+template <class A, class P>
+__device__ uint32_t lit_score_at(const A& a, const P& p, int len, int pos) {
     uint32_t score = 0;
     uint32_t prev = pos > 0 ? byte_at(a, pos - 1) : 0;
     for (int k = 0; k < p.n; k++) {
@@ -302,8 +331,8 @@ __device__ uint32_t lit_score_at(const A& a, const FrzPatternDev& p, int len, in
     return score & 0xffff;
 }
 // returns true on match; *opos, *oscore
-template <class A>
-__device__ bool lit_find(const A& a, const FrzPatternDev& p, int len, int* opos, uint32_t* oscore) {
+template <class A, class P>
+__device__ bool lit_find(const A& a, const P& p, int len, int* opos, uint32_t* oscore) {
     const int n = p.n;
     if (len < n) return false;
     switch (p.matching) {
@@ -340,7 +369,8 @@ struct OccTable {
     uint2 occ[kMaxDistinct][32];             // per-lane occurrence masks of the distinct needle byte classes
 };
 
-__device__ __forceinline__ int sw_class_of(int window, const FrzPatternDev& pat) {
+template <class P>
+__device__ __forceinline__ int sw_class_of(int window, const P& pat) {
     if (window > 128) return FRZ_C_GENERIC;
     if (window > 64) return FRZ_C_COLS128;
     if (!pat.col_classes) return FRZ_C_COLS64;
@@ -382,8 +412,8 @@ struct Emit {
     bool ok;
 };
 
-template <int MODE>
-__device__ __forceinline__ void process_candidate(const FrzCorpusView& cv, const FrzPatternDev& pat, const uint8_t* __restrict__ cid_s,
+template <int MODE, class P>
+__device__ __forceinline__ void process_candidate(const FrzCorpusView& cv, const P& pat, const uint8_t* __restrict__ cid_s,
                                                   uint2 (*occ)[32], const Cand& cd, bool active,
                                                   uint32_t* __restrict__ surv_bitmap, Emit* out, bool single_chunk = false) {
     bool ok = false;
@@ -397,6 +427,7 @@ __device__ __forceinline__ void process_candidate(const FrzCorpusView& cv, const
     // warp-wide occurrence-mask windows (uniform code) for the 0- and 1-typo modes
     bool flat_done = false, flat_ok = false;
     int flat_start = 0, flat_end = 0;
+    if constexpr (std::is_same<P, FrzPatternDev>::value) {   // (long needles take the scanning forms)
     if ((MODE == FRZ_T_0 || MODE == FRZ_T_1) && pat.n_distinct > 0) {
         if (single_chunk) {   // warp-uniform: corpus of <= 64-byte haystacks at the 64-lane width (prefilter_masks.cuh)
             if (MODE == FRZ_T_0) flat_ok = masks_k0_single(units, pat, occ, len, active, &flat_start, &flat_end);
@@ -413,6 +444,7 @@ __device__ __forceinline__ void process_candidate(const FrzCorpusView& cv, const
         if (MODE == FRZ_T_2) flat_ok = masks_paths<3>(units, pat, cid_s, occ, len, active, &flat_start, &flat_end);
         else flat_ok = masks_many(units, pat, cid_s, occ, len, active, &flat_start, &flat_end);
         flat_done = true;
+    }
     }
     if (active) {
         const uint32_t li = cd.li;
@@ -665,17 +697,28 @@ struct __align__(16) ScanWinSmem {   // one warp's part of the dynamic shared me
 // The kWarps ScanWinSmem are followed by one occurrence table per warp (OccTable's layout) of `occ_rows` rows: only the
 // rows the mask builders touch, n_distinct (+ n for the single-chunk forms' position masks).
 
-template <int MODE>
-__global__ void __launch_bounds__(kThreads, 4) k_scan_window(const FrzCorpusView cv, const __grid_constant__ FrzPatternDev pat,
-                                                             int use_sig, int occ_rows, const FrzSurvLists lists,
-                                                             unsigned long long surv_cap, uint32_t* __restrict__ surv_bitmap,
-                                                             FrzCounters* __restrict__ ctr) {
+// The needle as process_candidate reads it: the pattern itself, or (LONG) the block's staged copy of its FrzNeedleTab.
+template <bool LONG>
+__device__ __forceinline__ std::conditional_t<LONG, LongPat, const FrzPatternDev&> needle_view(const FrzPatternDev& p, const FrzNeedleTab* ntab,
+                                                                                                  uint8_t* tab_s) {
+    if constexpr (LONG) return stage_long_pat(p, ntab, tab_s);
+    else return p;
+}
+
+// k_scan_window (needles of up to FRZ_MAX_NEEDLE bytes) and k_scan_window_long (longer needles: the dynamic shared memory
+// holds the needle table after the warps' parts, where the occurrence tables would be — a long needle has none).
+template <int MODE, bool LONG>
+__device__ __forceinline__ void scan_window(const FrzCorpusView& cv, const FrzPatternDev& pat, int use_sig, int occ_rows,
+                                            const FrzSurvLists& lists, unsigned long long surv_cap,
+                                            uint32_t* __restrict__ surv_bitmap, FrzCounters* __restrict__ ctr,
+                                            const FrzNeedleTab* ntab) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const uint32_t lane = frz_lane(), warp = threadIdx.x >> 5;
     ScanWinSmem& sm = reinterpret_cast<ScanWinSmem*>(smem_raw)[warp];
     uint2 (*occ)[32] = reinterpret_cast<uint2 (*)[32]>(smem_raw + sizeof(ScanWinSmem) * kWarps) + (size_t)warp * occ_rows;
     __shared__ uint8_t cid_s[FRZ_MAX_NEEDLE];
     if (threadIdx.x < FRZ_MAX_NEEDLE) cid_s[threadIdx.x] = pat.cid[threadIdx.x];
+    const auto& pv = needle_view<LONG>(pat, ntab, smem_raw + sizeof(ScanWinSmem) * kWarps);
     if (lane == 0)
         for (int i = 0; i < kFusedStages; i++) mbar_init(&sm.bar[i], 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -719,7 +762,7 @@ __global__ void __launch_bounds__(kThreads, 4) k_scan_window(const FrzCorpusView
         cd.base = cv.data + (((unsigned long long)batch.w << 32) | batch.z);
         cd.units = staged ? &sm.win.units[lane][0] : cd.base;
         Emit cur;
-        process_candidate<MODE>(cv, pat, cid_s, occ, cd, active, surv_bitmap, &cur, single);
+        process_candidate<MODE>(cv, pv, cid_s, occ, cd, active, surv_bitmap, &cur, single);
         emit_commit(pending, lists, surv_cap, ctr);      // the previous batch's list space has arrived by now
         emit_request(cur, ctr);
         pending = cur;
@@ -785,6 +828,20 @@ __global__ void __launch_bounds__(kThreads, 4) k_scan_window(const FrzCorpusView
     if (batch_pending) run_batch();
     emit_commit(pending, lists, surv_cap, ctr);
 }
+template <int MODE>
+__global__ void __launch_bounds__(kThreads, 4) k_scan_window(const FrzCorpusView cv, const __grid_constant__ FrzPatternDev pat,
+                                                             int use_sig, int occ_rows, const FrzSurvLists lists,
+                                                             unsigned long long surv_cap, uint32_t* __restrict__ surv_bitmap,
+                                                             FrzCounters* __restrict__ ctr) {
+    scan_window<MODE, false>(cv, pat, use_sig, occ_rows, lists, surv_cap, surv_bitmap, ctr, nullptr);
+}
+template <int MODE>
+__global__ void __launch_bounds__(kThreads, 4) k_scan_window_long(const FrzCorpusView cv, const __grid_constant__ FrzPatternDev pat,
+                                                                  int use_sig, int occ_rows, const FrzSurvLists lists,
+                                                                  unsigned long long surv_cap, uint32_t* __restrict__ surv_bitmap,
+                                                                  FrzCounters* __restrict__ ctr, const FrzNeedleTab* ntab) {
+    scan_window<MODE, true>(cv, pat, use_sig, occ_rows, lists, surv_cap, surv_bitmap, ctr, ntab);
+}
 
 // Candidate-list mode (multi-pattern, src/matcher/multi.rs:108-120): the extra patterns are evaluated only
 // on the haystacks that survived the previous patterns.  The list is already compact, so each warp takes 32
@@ -818,6 +875,40 @@ __global__ void __launch_bounds__(kThreads) k_prefilter_list(const FrzCorpusView
         __syncwarp();
         Emit e;
         process_candidate<MODE>(cv, pat, cid_s, occ, cd, active, surv_bitmap, &e);
+        emit_request(e, ctr);
+        emit_commit(e, lists, surv_cap, ctr);
+        __syncwarp();
+    }
+}
+// The same for a long needle: the scanning forms over the block's staged copy of its table (no occurrence tables).
+template <int MODE>
+__global__ void __launch_bounds__(kThreads) k_prefilter_list_long(const FrzCorpusView cv, const __grid_constant__ FrzPatternDev pat,
+                                                                  const FrzMatchDev* __restrict__ cand, unsigned long long n_cand,
+                                                                  uint32_t index_offset,
+                                                                  const FrzSurvLists lists, unsigned long long surv_cap,
+                                                                  uint32_t* __restrict__ surv_bitmap, FrzCounters* __restrict__ ctr,
+                                                                  const FrzNeedleTab* __restrict__ ntab) {
+    __shared__ __align__(16) uint8_t tab_s[kLongPatSmem];
+    const uint32_t lane = frz_lane(), warp = threadIdx.x >> 5;
+    const LongPat lp = stage_long_pat(pat, ntab, tab_s);
+    __syncthreads();
+    const unsigned long long n_warps = (unsigned long long)gridDim.x * kWarps;
+    for (unsigned long long base = ((unsigned long long)blockIdx.x * kWarps + warp) * 32; base < n_cand; base += n_warps * 32) {
+        const unsigned long long i = base + lane;
+        bool active = i < n_cand;
+        Cand cd;
+        cd.tile = 0; cd.slot = 0; cd.li = 0; cd.len = 0; cd.base = nullptr; cd.units = nullptr;
+        if (active) {
+            const uint32_t idx = cand[i].index - index_offset;
+            const uint32_t tile = idx >> FRZ_TILE_SHIFT, li = idx & (FRZ_TILE - 1);
+            const uint32_t slot = cv.slot_of[(uint64_t)tile * FRZ_TILE + li];
+            const uint32_t len = cv.slot_meta[(uint64_t)tile * FRZ_TILE + slot] >> FRZ_TILE_SHIFT;
+            active = (int)len >= pat.min_hay_len;
+            cd = resolve_cand(cv, tile, slot, (int)len);
+        }
+        __syncwarp();
+        Emit e;
+        process_candidate<MODE>(cv, lp, nullptr, nullptr, cd, active, surv_bitmap, &e);
         emit_request(e, ctr);
         emit_commit(e, lists, surv_cap, ctr);
         __syncwarp();
@@ -970,15 +1061,23 @@ __global__ void __launch_bounds__(128) k_match_indices(const FrzCorpusView cv, c
 
 frz_status frz_launch_prefilter_list(const FrzCorpusView& cv, const FrzPatternDev& pat, const FrzMatchDev* cand,
                                      uint64_t n_cand, uint32_t index_offset, FrzWorkspace& ws, cudaStream_t stream,
-                                     FrzLaunchStats* st) {
+                                     FrzLaunchStats* st, const FrzNeedleTab* ntab) {
     if (cv.n_tiles == 0) return FRZ_OK;
-    const size_t smem = sizeof(OccTable) * kWarps;
+    const bool is_long = pat.n > FRZ_MAX_NEEDLE;
+    const size_t smem = is_long ? 0 : sizeof(OccTable) * kWarps;
     FRZ_CUDA_TRY(cudaMemsetAsync(ws.surv_bitmap, 0, (size_t)cv.n_tiles * 32 * sizeof(uint32_t), stream));
     if (n_cand == 0) return FRZ_OK;
     const uint32_t grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)frz_sm_count() * 4, (n_cand + kThreads - 1) / kThreads));
-#define FRZ_PFL_LAUNCH(MODE)                                                                                     \
-    k_prefilter_list<MODE><<<grid, kThreads, smem, stream>>>(cv, pat, cand, n_cand, index_offset, ws.lists(),    \
-                                                             ws.survivor_cap, ws.surv_bitmap, ws.counters)
+#define FRZ_PFL_LAUNCH(MODE)                                                                                          \
+    do {                                                                                                              \
+        if (is_long) {                                                                                                \
+            k_prefilter_list_long<MODE><<<grid, kThreads, smem, stream>>>(cv, pat, cand, n_cand, index_offset, ws.lists(), \
+                                                                          ws.survivor_cap, ws.surv_bitmap, ws.counters, ntab); \
+        } else {                                                                                                      \
+            k_prefilter_list<MODE><<<grid, kThreads, smem, stream>>>(cv, pat, cand, n_cand, index_offset, ws.lists(), \
+                                                                     ws.survivor_cap, ws.surv_bitmap, ws.counters);   \
+        }                                                                                                             \
+    } while (0)
     switch (pat.typo_mode) {
         case FRZ_T_0: FRZ_PFL_LAUNCH(FRZ_T_0); break;
         case FRZ_T_1: FRZ_PFL_LAUNCH(FRZ_T_1); break;
@@ -1023,15 +1122,44 @@ frz_status frz_launch_sig_scan(const FrzCorpusView& cv, const FrzPatternDev& pat
 // Stage 1 of match_list over the whole corpus: k_scan_window (length gate + signature test + exact windows → survivor
 // records + per-tile survivor bitmap).
 frz_status frz_launch_prefilter(const FrzCorpusView& cv, const FrzPatternDev& pat, FrzWorkspace& ws, cudaStream_t stream,
-                                FrzLaunchStats* st) {
+                                FrzLaunchStats* st, const FrzNeedleTab* ntab) {
     if (cv.n_tiles == 0) return FRZ_OK;
     const int sms = frz_sm_count();
     FRZ_CUDA_TRY(cudaMemsetAsync(ws.surv_bitmap, 0, (size_t)cv.n_tiles * 32 * sizeof(uint32_t), stream));
     const int use_sig = pat.typo_mode != FRZ_T_NONE && pat.sig_on;
     const int occ_rows = pat.n_distinct ? std::min(kMaxDistinct, pat.n_distinct + pat.n) : 0;
+    const uint32_t total_chunks = cv.n_tiles * (FRZ_TILE / 128);
+    if (pat.n > FRZ_MAX_NEEDLE) {   // long needle (n_distinct 0: no occurrence tables), the table after the warps' parts
+        const size_t smem = sizeof(ScanWinSmem) * kWarps + kLongPatSmem;
+#define FRZ_PF_LAUNCH_LONG(MODE)                                                                                          \
+    do {                                                                                                                 \
+        static int bps_dev[64] = {};                                                                                     \
+        int& bps = bps_dev[frz_current_device() & 63];                                                                   \
+        if (!bps) {                                                                                                      \
+            FRZ_CUDA_TRY(cudaFuncSetAttribute(k_scan_window_long<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+            FRZ_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_scan_window_long<MODE>, kThreads, smem)); \
+            if (bps < 1) bps = 1;                                                                                        \
+        }                                                                                                                \
+        const uint32_t grid = std::max<uint32_t>(1, std::min<uint32_t>((uint32_t)(sms * bps), (total_chunks + kWarps - 1) / kWarps)); \
+        k_scan_window_long<MODE><<<grid, kThreads, smem, stream>>>(cv, pat, use_sig, 0, ws.lists(), ws.survivor_cap,     \
+                                                                   ws.surv_bitmap, ws.counters, ntab);                   \
+    } while (0)
+        switch (pat.typo_mode) {
+            case FRZ_T_0: FRZ_PF_LAUNCH_LONG(FRZ_T_0); break;
+            case FRZ_T_1: FRZ_PF_LAUNCH_LONG(FRZ_T_1); break;
+            case FRZ_T_2: FRZ_PF_LAUNCH_LONG(FRZ_T_2); break;
+            case FRZ_T_MANY: FRZ_PF_LAUNCH_LONG(FRZ_T_MANY); break;
+            case FRZ_T_NONE: FRZ_PF_LAUNCH_LONG(FRZ_T_NONE); break;
+            case FRZ_T_LITERAL: FRZ_PF_LAUNCH_LONG(FRZ_T_LITERAL); break;
+            default: return frz_fail(FRZ_ERR_INVALID_ARG, "bad typo mode %d", pat.typo_mode);
+        }
+#undef FRZ_PF_LAUNCH_LONG
+        FRZ_CUDA_TRY(cudaGetLastError());
+        if (st) st->launches++;
+        return FRZ_OK;
+    }
     const size_t smem = (sizeof(ScanWinSmem) + sizeof(uint2) * 32 * occ_rows) * kWarps;
     const size_t smem_max = (sizeof(ScanWinSmem) + sizeof(OccTable)) * kWarps;
-    const uint32_t total_chunks = cv.n_tiles * (FRZ_TILE / 128);
 #define FRZ_PF_LAUNCH(MODE)                                                                                              \
     do {                                                                                                                 \
         static int bps_dev[64][kMaxDistinct + 1] = {};   /* blocks per SM by device and occurrence-table rows */         \

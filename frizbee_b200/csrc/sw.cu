@@ -30,6 +30,7 @@
 #include "frz_host.h"
 #include "sw_core.cuh"
 #include "sw_generic.cuh"
+#include "sw_wave.cuh"
 
 namespace {
 
@@ -336,6 +337,218 @@ __global__ void __launch_bounds__(256) k_emit_literal(const FrzSurvivor* __restr
     if (local_max) atomicMax(&ctr->max_score, local_max);
 }
 
+// ---- needles of FRZ_MAX_NEEDLE + 1 .. FRZ_LONG_NEEDLE bytes, over all six survivor lists.  Two kernels split the windows:
+// ----   k_sw_long         one warp per window (sw_wave.cuh): every window of up to FRZ_SW_MAX_WINDOW bytes of a u16-family
+// ----                     needle
+// ----   k_sw_long_thread  one window per thread: windows over FRZ_SW_MAX_WINDOW bytes (greedy_score, as the reference) and
+// ----                     every window of a u8-family needle (generic_score: 8-bit elements, lanes up to 64)
+// The per-thread generic_score was measured for the u16 windows too and is about three times slower than the wavefront
+// at every window length of the long-needle benchmark, short windows included (DESIGN.md §4.8).
+constexpr int kLongWarps = 4;
+
+// the needle as greedy_score and generic_score read it: bytes and case flips in shared memory, the rest from the pattern
+struct LongNeedle {
+    const uint8_t *c, *flip;
+    int n, sw_lanes, score_bits;
+    int32_t gap_extend, gap_open_x, match_x, mismatch, case_bonus, cap_bonus, delim_bonus, prefix_bonus;
+    uint32_t raw_match, raw_gap_open, raw_gap_extend, raw_case, raw_cap, raw_prefix, raw_delim;
+};
+__device__ __forceinline__ LongNeedle long_needle(const FrzPatternDev& p, const uint8_t* c_s, const uint8_t* f_s) {
+    return LongNeedle{c_s, f_s, p.n, p.sw_lanes, p.score_bits, p.gap_extend, p.gap_open_x, p.match_x, p.mismatch, p.case_bonus,
+                      p.cap_bonus, p.delim_bonus, p.prefix_bonus, (uint32_t)p.raw_match, (uint32_t)p.raw_gap_open,
+                      (uint32_t)p.raw_gap_extend, (uint32_t)p.raw_case, (uint32_t)p.raw_cap, (uint32_t)p.raw_prefix,
+                      (uint32_t)p.raw_delim};
+}
+struct ByteHay {
+    const uint8_t* p;
+    __host__ __device__ __forceinline__ uint32_t operator()(int i) const { return p[i]; }
+};
+
+// the six survivor lists as one sequence of items
+struct LongItems {
+    unsigned long long ends[FRZ_N_CLASSES];   // cumulative survivor counts
+    __device__ __forceinline__ unsigned long long total() const { return ends[FRZ_N_CLASSES - 1]; }
+};
+__device__ __forceinline__ LongItems long_items(const FrzCounters* __restrict__ ctr, unsigned long long surv_cap) {
+    LongItems it;
+    unsigned long long acc = 0;
+#pragma unroll
+    for (int c = 0; c < FRZ_N_CLASSES; c++) {
+        acc += min(ctr->class_count[c], surv_cap);
+        it.ends[c] = acc;
+    }
+    return it;
+}
+// one survivor of either record layout, decoded
+struct LongWindow {
+    FrzSurvivor rec;
+    const uint8_t* base;   // byte 0 of the window
+    int W;
+    bool pre, full_end;
+};
+__device__ __forceinline__ LongWindow long_window(const FrzCorpusView& cv, const FrzSurvLists& lists, const LongItems& it,
+                                                  unsigned long long item) {
+    int cls = 0;
+    while (item >= it.ends[cls]) cls++;
+    LongWindow w;
+    w.rec = lists.p[cls][item - (cls ? it.ends[cls - 1] : 0ull)];
+    if (cls < FRZ_C_GENERIC) {   // window-class layout
+        const WindowRec wr = decode_window(w.rec);
+        w.base = reinterpret_cast<const uint8_t*>(cv.data + wr.addr) + wr.startlo;
+        w.W = wr.W;
+        w.pre = wr.start0;
+        w.full_end = wr.full_end;
+    } else {
+        const uint32_t start = w.rec.start, end = w.rec.end & 0x7fffffffu;
+        w.base = reinterpret_cast<const uint8_t*>(frz_unit_ptr(cv, w.rec.tile, w.rec.slot_rank & 0x3ff, 0)) + start;
+        w.W = (int)(end - start);
+        w.pre = start == 0;
+        w.full_end = (w.rec.end >> 31) != 0;
+    }
+    return w;
+}
+// k_sw_long's windows; the rest are k_sw_long_thread's
+__device__ __forceinline__ bool wave_window(const FrzPatternDev& p, int W) {
+    return p.score_bits == 16 && W <= FRZ_SW_MAX_WINDOW;
+}
+
+__global__ void __launch_bounds__(64) k_sw_long_thread(const FrzCorpusView cv, const __grid_constant__ FrzPatternDev pat,
+                                                       const FrzNeedleTab* __restrict__ ntab, const FrzSurvLists lists,
+                                                       unsigned long long surv_cap, const FrzRankView rv,
+                                                       FrzCounters* __restrict__ ctr, uint32_t index_offset, int reversed,
+                                                       FrzMatchDev* __restrict__ out, const FrzScoreHist hist) {
+    __shared__ uint8_t c_s[FRZ_LONG_NEEDLE], f_s[FRZ_LONG_NEEDLE];
+    const int n = pat.n;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) { c_s[i] = ntab->c[i]; f_s[i] = ntab->flip[i]; }
+    __syncthreads();
+    const LongNeedle nv = long_needle(pat, c_s, f_s);
+    const LongItems it = long_items(ctr, surv_cap);
+    uint32_t local_max = 0;
+    for (unsigned long long j = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; j < it.total();
+         j += (unsigned long long)gridDim.x * blockDim.x) {
+        const LongWindow w = long_window(cv, lists, it, j);
+        if (wave_window(pat, w.W)) continue;
+        uint32_t score;
+        if (w.W > FRZ_SW_MAX_WINDOW) {
+            const int g = greedy_score(ByteHay{w.base}, w.W, nv, w.pre);
+            score = g < 0 ? 0u : (uint32_t)g;
+        } else {
+            score = generic_score(ByteHay{w.base}, w.W, nv, w.pre);
+        }
+        bool exact = w.pre && w.full_end && w.W == n;
+        for (int k = 0; exact && k < n; k++) exact = w.base[k] == c_s[k];
+        if (exact) score = (score + pat.exact_bonus) & 0xffffu;
+        emit_match(w.rec, score, exact, index_offset, reversed != 0, rv, ctr, out, hist);
+        local_max = max(local_max, score);
+    }
+    if (local_max) atomicMax(&ctr->max_score, local_max);
+}
+
+// per warp: the window bytes, then (LANES < 32: windows of more than 32 chunks) one WaveLeft per needle row that carries
+// the last chunk of a pass over to the first chunk of the next
+template <int L>
+size_t long_warp_smem(int n) {
+    const size_t b = FRZ_SW_MAX_WINDOW + (L < 32 ? (size_t)n * sizeof(frzwave::WaveLeft<L>) : 0);
+    return (b + 15) & ~(size_t)15;
+}
+
+// Score of the window hay_s[0, W) (this warp's shared memory): lane j scores chunk p0 + j of each pass of 32 chunks.
+template <int L>
+__device__ __forceinline__ uint32_t wave_warp(const uint8_t* hay_s, int W, const uint8_t* c_s, const uint8_t* f_s, int n,
+                                              bool include_prefix, const frzwave::WaveConst& k, frzwave::WaveLeft<L>* store) {
+    using namespace frzwave;
+    const int lane = (int)frz_lane();
+    const int nch = (W + L - 1) / L;
+    uint32_t best = 0;
+    WaveLane<L> s;
+    for (int p0 = 0; p0 < nch; p0 += 32) {
+        const int lanes = min(32, nch - p0);
+        const bool has_next = p0 + 32 < nch;
+        lane_load<L>(s, ByteHay{hay_s}, p0 + lane, W, include_prefix, k);
+        for (int t = 0; t < n + lanes - 1; t++) {
+            const WaveLeft<L> mine = lane_out<L>(s);   // the row this lane finished at step t - 1
+            WaveLeft<L> left;
+#pragma unroll
+            for (int q = 0; q < L / 4; q++) left.hp[q] = __shfl_up_sync(0xffffffffu, mine.hp[q], 1);
+            left.m = __shfl_up_sync(0xffffffffu, mine.m, 1);
+            left.diag = __shfl_up_sync(0xffffffffu, mine.diag, 1);
+            const int i = t - lane;
+            const bool live = lane < lanes && i >= 0 && i < n;
+            if (lane == 0) left = (p0 > 0 && live) ? store[i] : wave_left_zero<L>();
+            if (live) {
+                lane_row<L>(s, left, c_s[i], f_s[i], k);
+                if (lane == 31 && has_next) store[i] = lane_out<L>(s);
+            }
+            __syncwarp();
+        }
+        if (lane < lanes) best = max(best, lane_max<L>(s));
+    }
+    return __reduce_max_sync(0xffffffffu, best);
+}
+
+template <int L>
+__global__ void __launch_bounds__(kLongWarps * 32) k_sw_long(const FrzCorpusView cv, const __grid_constant__ FrzPatternDev pat,
+                                                            const FrzNeedleTab* __restrict__ ntab, const FrzSurvLists lists,
+                                                            unsigned long long surv_cap, const FrzRankView rv,
+                                                            FrzCounters* __restrict__ ctr, uint32_t index_offset, int reversed,
+                                                            FrzMatchDev* __restrict__ out, const FrzScoreHist hist,
+                                                            uint32_t warp_smem) {
+    using namespace frzwave;
+    extern __shared__ __align__(16) uint8_t long_smem[];
+    uint8_t* c_s = long_smem;
+    uint8_t* f_s = long_smem + FRZ_LONG_NEEDLE;
+    const int n = pat.n;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) { c_s[i] = ntab->c[i]; f_s[i] = ntab->flip[i]; }
+    __syncthreads();
+    const uint32_t lane = frz_lane(), warp = threadIdx.x >> 5;
+    uint8_t* hay_s = long_smem + 2 * FRZ_LONG_NEEDLE + (size_t)warp * warp_smem;
+    WaveLeft<L>* store = reinterpret_cast<WaveLeft<L>*>(hay_s + FRZ_SW_MAX_WINDOW);
+    const WaveConst k = wave_const(pat);
+    const LongItems it = long_items(ctr, surv_cap);
+    uint32_t local_max = 0;
+    for (;;) {   // a window per claim: window lengths vary by three orders of magnitude
+        uint32_t item = 0;
+        if (lane == 0) item = atomicAdd(&ctr->sw_next, 1u);
+        item = __shfl_sync(0xffffffffu, item, 0);
+        if (item >= it.total()) break;
+        const LongWindow w = long_window(cv, lists, it, item);
+        if (!wave_window(pat, w.W)) continue;   // k_sw_long_thread's
+        for (int c = (int)lane; c < w.W; c += 32) hay_s[c] = w.base[c];
+        __syncwarp();
+        uint32_t score = wave_warp<L>(hay_s, w.W, c_s, f_s, n, w.pre, k, store);
+        bool exact = false;
+        if (w.pre && w.full_end && w.W == n) {
+            bool eq = true;
+            for (int c = (int)lane; c < w.W; c += 32) eq = eq && hay_s[c] == c_s[c];
+            exact = __all_sync(0xffffffffu, eq);
+        }
+        if (exact) score = (score + pat.exact_bonus) & 0xffffu;
+        if (lane == 0) emit_match(w.rec, score, exact, index_offset, reversed != 0, rv, ctr, out, hist);
+        local_max = max(local_max, score);
+        __syncwarp();   // every lane is done with hay_s before the next window overwrites it
+    }
+    if (lane == 0 && local_max) atomicMax(&ctr->max_score, local_max);
+}
+
+template <int L>
+frz_status launch_sw_long(const FrzCorpusView& cv, const FrzPatternDev& pat, const FrzNeedleTab* ntab, uint32_t index_offset,
+                          bool reversed, FrzWorkspace& ws, FrzMatchDev* d_out, const FrzScoreHist& hist, cudaStream_t stream) {
+    const size_t warp_smem = long_warp_smem<L>(pat.n);
+    const size_t smem = 2 * FRZ_LONG_NEEDLE + kLongWarps * warp_smem;
+    static bool attr_set_dev[64] = {};
+    bool& attr_set = attr_set_dev[frz_current_device() & 63];
+    if (!attr_set) {
+        const size_t smem_max = 2 * FRZ_LONG_NEEDLE + kLongWarps * long_warp_smem<L>(FRZ_LONG_NEEDLE);
+        FRZ_CUDA_TRY(cudaFuncSetAttribute(k_sw_long<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max));
+        attr_set = true;
+    }
+    k_sw_long<L><<<frz_sm_count() * 4, kLongWarps * 32, smem, stream>>>(cv, pat, ntab, ws.lists(), ws.survivor_cap, rank_view(ws),
+                                                                         ws.counters, index_offset, reversed ? 1 : 0, d_out, hist,
+                                                                         (uint32_t)warp_smem);
+    FRZ_CUDA_TRY(cudaGetLastError());
+    return FRZ_OK;
+}
+
 template <int LANES>
 frz_status launch_sw_lanes(const FrzCorpusView& cv, const FrzPatternDev& pat, uint32_t index_offset, bool reversed,
                            FrzWorkspace& ws, FrzMatchDev* d_out, const FrzScoreHist& hist, cudaStream_t stream) {
@@ -382,12 +595,32 @@ frz_status launch_sw_lanes(const FrzCorpusView& cv, const FrzPatternDev& pat, ui
 }  // namespace
 
 frz_status frz_launch_sw(const FrzCorpusView& cv, const FrzPatternDev& pat, uint32_t index_offset, bool reversed,
-                         FrzWorkspace& ws, FrzMatchDev* d_out, cudaStream_t stream, FrzLaunchStats* st, const FrzScoreHist& hist) {
+                         FrzWorkspace& ws, FrzMatchDev* d_out, cudaStream_t stream, FrzLaunchStats* st, const FrzScoreHist& hist,
+                         const FrzNeedleTab* ntab) {
     if (cv.n_tiles == 0) return FRZ_OK;
     if (pat.typo_mode == FRZ_T_LITERAL) {
         k_emit_literal<<<frz_sm_count() * 4, 256, 0, stream>>>(ws.survivors[FRZ_C_COLS64], ws.survivor_cap, rank_view(ws), ws.counters,
                                                            index_offset, reversed ? 1 : 0, d_out, hist);
         FRZ_CUDA_TRY(cudaGetLastError());
+        if (st) st->launches++;
+        return FRZ_OK;
+    }
+    if (pat.n > FRZ_MAX_NEEDLE) {
+        // per thread: the u8 family, and windows over FRZ_SW_MAX_WINDOW bytes (which need a longer haystack)
+        if (pat.score_bits != 16 || cv.max_gunits * FRZ_UNIT > FRZ_SW_MAX_WINDOW) {
+            k_sw_long_thread<<<frz_sm_count() * 8, 64, 0, stream>>>(cv, pat, ntab, ws.lists(), ws.survivor_cap, rank_view(ws),
+                                                                     ws.counters, index_offset, reversed ? 1 : 0, d_out, hist);
+            FRZ_CUDA_TRY(cudaGetLastError());
+            if (st) st->launches++;
+        }
+        if (pat.score_bits != 16) return FRZ_OK;
+        // the wavefront: the u16 family, 8, 16 or 32 lanes
+        switch (pat.sw_lanes) {
+            case 32: FRZ_TRY(launch_sw_long<32>(cv, pat, ntab, index_offset, reversed, ws, d_out, hist, stream)); break;
+            case 16: FRZ_TRY(launch_sw_long<16>(cv, pat, ntab, index_offset, reversed, ws, d_out, hist, stream)); break;
+            case 8: FRZ_TRY(launch_sw_long<8>(cv, pat, ntab, index_offset, reversed, ws, d_out, hist, stream)); break;
+            default: return frz_fail(FRZ_ERR_INVALID_ARG, "unsupported lane count %d for a long needle", pat.sw_lanes);
+        }
         if (st) st->launches++;
         return FRZ_OK;
     }

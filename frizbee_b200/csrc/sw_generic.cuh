@@ -18,8 +18,9 @@ constexpr int kGenCols = FRZ_SW_MAX_WINDOW + 64;
 #define FRZ_SW_GREEDY_FN inline
 #endif
 
-template <class Hay>
-FRZ_SW_GREEDY_FN int greedy_score(const Hay& hay, int W, const FrzPatternDev& p, bool include_prefix) {
+// P: FrzPatternDev, or any needle view with its n, c, flip and raw_* members (k_sw_long's WaveNeedle)
+template <class Hay, class P>
+FRZ_SW_GREEDY_FN int greedy_score(const Hay& hay, int W, const P& p, bool include_prefix) {
     const int n = p.n;
     if (n > W) return -1;
     auto sat_add = [](uint32_t a, uint32_t b) { uint32_t r = a + b; return r > 0xffffu ? 0xffffu : r; };
@@ -67,8 +68,9 @@ FRZ_SW_GREEDY_FN int greedy_score(const Hay& hay, int W, const FrzPatternDev& p,
 
 // Score of a window of W <= FRZ_SW_MAX_WINDOW bytes: a literal row-major restatement of the reference with true
 // element-width arithmetic (u8 or u16 lanes, pat.sw_lanes wide chunks).
-template <class Hay>
-FRZ_SW_FN uint32_t generic_score(const Hay& hay, int W, const FrzPatternDev& pat, bool include_prefix) {
+// P: FrzPatternDev, or a needle view with the same members (k_sw_long_thread's LongNeedle)
+template <class Hay, class P>
+FRZ_SW_FN uint32_t generic_score(const Hay& hay, int W, const P& pat, bool include_prefix) {
     const int L = pat.sw_lanes;
     const uint32_t lane_mask = pat.score_bits == 8 ? 0xffu : 0xffffu;  // real element width
     uint16_t Hp[kGenCols], Hc[kGenCols], bon[kGenCols];

@@ -52,7 +52,9 @@ typedef enum frz_status {
     FRZ_ERR_CAPACITY = 6,
     FRZ_ERR_CUDA = 7,
     FRZ_ERR_NO_DEVICE = 8,
-    /* feature of the reference not built on the GPU path yet (never a silent CPU fallback) */
+    /* feature of the reference not built on the GPU path yet (never a silent CPU fallback): needles over 1024 bytes,
+     * needles over 64 bytes on the unicode path or in frz_match_indices, max_typos > 15 below
+     * the needle length (DESIGN.md §7) */
     FRZ_ERR_UNSUPPORTED = 9,
     FRZ_ERR_OOM = 10,
     /* NCCL missing / failed, or a peer rank did not answer (multi-GPU entry points only) */
