@@ -28,7 +28,7 @@ def _stale(target: str, deps) -> bool:
 def build(force: bool = False, verbose: bool = False, variant: str = "", defines=()) -> str:
     """variant/defines: an A/B build (`libfrz_cuda_<variant>.so`, own object directory) with extra -D flags; load it with
     FRZ_LIB=<path> (frizbee_b200.lib_path).  The default build is untouched."""
-    headers = [os.path.join(CSRC, h) for h in ("frz_device.cuh", "frz_host.h", "unicode_path.cuh", "unicode_needle.h", "unicode_case.inc", "indices_path.cuh", "sw_core.cuh", "sw_generic.cuh", "sw_wave.cuh", "prefilter_masks.cuh")] + \
+    headers = [os.path.join(CSRC, h) for h in ("frz_device.cuh", "frz_host.h", "unicode_path.cuh", "unicode_needle.h", "unicode_case.inc", "indices_path.cuh", "sw_core.cuh", "sw_generic.cuh", "sw_wave.cuh", "prefilter_masks.cuh", "prefilter_scan.cuh")] + \
               [os.path.join(HERE, "..", "include", "frz_cuda.h")]
     objdir = os.path.join(HERE, "build" + ("_" + variant if variant else ""))
     out = OUT if not variant else os.path.join(HERE, f"libfrz_cuda_{variant}.so")

@@ -41,6 +41,13 @@ int h_masks_window(const void* pat_bytes, const uint8_t* hay, int len, int mode,
     return ok ? 1 : 0;
 }
 
+// the pattern's distinct byte classes (0: more than 16, the kernels take the scanning forms)
+int h_n_distinct(const void* pat_bytes) {
+    FrzPatternDev pat;
+    memcpy(&pat, pat_bytes, sizeof pat);
+    return pat.n_distinct;
+}
+
 // Phase A of k_prefilter: the signature of the haystack (pack.cu: k_pack_sig uses the same frz_sig_add) against the
 // needle's class requirements (host.cu: compile_pattern).  Returns 1 = candidate, 0 = rejected without reading the bytes.
 int h_sig_pass(const void* pat_bytes, const uint8_t* hay, int len) {

@@ -13,7 +13,8 @@ import numpy as np
 import pytest
 
 import frizbee_b200 as F
-from frizbee_b200.types import CaseMatching, Config, Scoring
+from frizbee_b200.types import CaseMatching, Config, Matching, Scoring, UnicodeMatching
+from needles import case_pairs, case_sensitive, n_distinct, plant
 from oracle import pyoracle as O
 from scorings import scorings
 
@@ -55,34 +56,53 @@ POOLS = [b"abAB_/-ab01", b"ab", b"abcdefghijklmnopqrstuvwxyzABCDEFGHIJKLMNOPQRST
 HAY_EXTRA = b"\xc3\xa9\x00"   # haystacks may hold any bytes (multi-byte scalars, NUL)
 
 
+# a scoring whose whole score range fits in u8 for needles of up to 64 bytes (and far longer): keeps them in the u8 family
+SINGLE_PASS = Scoring(match_score=1, mismatch_penalty=0, gap_open_penalty=1, gap_extend_penalty=0, prefix_bonus=0,
+                      capitalization_bonus=0, matching_case_bonus=0, exact_match_bonus=0, delimiter_bonus=0)
+
+
 @pytest.mark.parametrize("lanes", [16, 32, 64])
 def test_swcore_column_classes_equal_oracle(H, lanes):
     """SwCore<LANES, 64, no-wrap, VAR, CC>: the class the prefilter would choose and every wider one give the oracle's score."""
-    rng = random.Random(5000 + lanes)
+    column_classes_vs_oracle(H, lanes, long_u8=False)
+
+
+@pytest.mark.parametrize("lanes", [16, 32, 64])
+def test_swcore_column_classes_long_u8_needles(H, lanes):
+    """The same for needles of up to 64 bytes: at the default scoring a u8 needle has at most 13 bytes, SINGLE_PASS keeps
+    longer ones in u8, where the needle is longer than the window and W + n passes every class boundary."""
+    column_classes_vs_oracle(H, lanes, long_u8=True)
+
+
+def column_classes_vs_oracle(H, lanes, long_u8):
+    rng = random.Random(5000 + lanes + 100 * long_u8)
     F.lib().frz_matcher_debug_pattern.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]
+    sc = SINGLE_PASS if long_u8 else Scoring()
     checked = 0
-    for trial in range(700):
+    for trial in range(400 if long_u8 else 700):
         pool = rng.choice(POOLS)
-        n = rng.randint(1, 11)
+        n = rng.choice([rng.randint(1, 64), rng.randint(30, 64)]) if long_u8 else rng.randint(1, 11)
         needle = rand_bytes(rng, pool, n)
         if 0 in needle:
             continue
         cs = rng.random() < 0.3
-        cfg = Config(max_typos=None, emulate_lanes=lanes, casing=CaseMatching.Respect if cs else CaseMatching.Ignore)
+        cfg = Config(max_typos=None, emulate_lanes=lanes, casing=CaseMatching.Respect if cs else CaseMatching.Ignore, scoring=sc)
         pat, info = device_pattern(H, needle, cfg)
         assert info["score_bits"] == 8 and info["lanes"] == lanes
+        wrap8, col_classes, lane_pen = pattern_flags(H, pat)
+        assert (wrap8, col_classes, lane_pen) == (False, True, long_u8)   # SINGLE_PASS: gap_extend 0 < gap_open
         for _ in range(6):
             W = rng.randint(1, 64)
             win = rand_bytes(rng, pool + (HAY_EXTRA if rng.random() < 0.3 else b""), W)
             pre = rng.random() < 0.5
-            want = O.sw_score(needle, win, Scoring(), cs, pre, lanes, 8)
+            want = O.sw_score(needle, win, sc, cs, pre, lanes, 8)
             chunk_cols = (W + lanes - 1) // lanes * lanes
             need = min(W + n, chunk_cols)
             for cc in (40, 48, 56, 64):
                 if cc < need or cc < W:
                     continue
                 eq = C.c_int()
-                var = rng.choice([0, 8])
+                var = rng.choice([0, 8]) | (16 if lane_pen else 0)   # the per-lane gap penalty form, as sw.cu launches it
                 got = H.h_swcore(pat, win, W, rng.randint(0, 15), int(pre), lanes, 64, cc, 0, var, C.byref(eq))
                 assert got == want, (needle, win, cs, pre, lanes, cc, var, got, want)
                 assert bool(eq.value) == (win == needle)
@@ -97,13 +117,13 @@ def test_swcore_128_columns_and_u16_family(H, lanes, bits):
     emulate = {(8, 16): 16, (16, 16): 32, (32, 16): 64, (16, 8): 16, (64, 8): 64}[(lanes, bits)]
     for trial in range(150):
         pool = rng.choice(POOLS)
-        n = rng.randint(14, 24) if bits == 16 else rng.randint(1, 10)
+        n = rng.choice([rng.randint(14, 64), rng.randint(40, 64)]) if bits == 16 else rng.randint(1, 10)
         needle = rand_bytes(rng, pool, n)
         cfg = Config(max_typos=None, emulate_lanes=emulate, casing=CaseMatching.Ignore)
         pat, info = device_pattern(H, needle, cfg)
         assert (info["lanes"], info["score_bits"]) == (lanes, bits)
         for _ in range(3):
-            W = rng.randint(1, 128)
+            W = rng.choice([rng.randint(1, n), rng.randint(n, 128), rng.randint(1, 64)])
             win = rand_bytes(rng, pool + (HAY_EXTRA if rng.random() < 0.3 else b""), W)
             pre = rng.random() < 0.5
             want = O.sw_score(needle, win, Scoring(), False, pre, lanes, bits)
@@ -326,7 +346,41 @@ def PF():
         subprocess.run(["g++", "-O1", "-std=c++17", "-I" + CUDA_INC, "-fPIC", "-shared", "-o", PF_LIB, PF_SRC], check=True)
     L = C.CDLL(PF_LIB)
     L.h_masks_window.argtypes = [C.c_void_p, C.c_char_p, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
+    L.h_n_distinct.argtypes = [C.c_void_p]
     return L
+
+
+# needles with few byte classes (the occurrence-mask forms take needles of up to 64 bytes with <= 16 classes)
+MASK_POOLS = [b"ab", b"aAbBcC", b"abAB_/-01", b"aAbB_zZ9"]
+
+
+def mask_needle(rng, pool, n_max=64):
+    return rand_bytes(rng, pool, rng.choice([rng.randint(1, 12), rng.randint(1, n_max), rng.randint(13, n_max)]))
+
+
+def mask_haystack(rng, needle, pool, ln, k):
+    """`ln` bytes of the pool, about half of them holding the needle with 0..k+1 of its bytes deleted"""
+    filler = pool + (HAY_EXTRA if rng.random() < 0.2 else b"x")
+    if ln and rng.random() < 0.5:
+        return plant(rng, needle, ln, filler, drops=rng.randint(0, k + 1), spread=rng.random() < 0.4)
+    return rand_bytes(rng, filler, ln)
+
+
+def test_n_distinct_helper_equals_compile_pattern(H, PF):
+    """tests/needles.py: n_distinct (used by the GPU tests to tell which prefilter form a needle takes) equals the
+    FrzPatternDev.n_distinct host.cu: compile_pattern writes, on both sides of 16 classes and of 64 bytes."""
+    rng = random.Random(8800)
+    F.lib().frz_matcher_debug_pattern.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]
+    seen = set()
+    for trial in range(600):
+        pool = rng.choice(MASK_POOLS + POOLS + [b"abcdefghijklmnopq", b"aA\x00zZ"])
+        needle = rand_bytes(rng, pool, rng.choice([rng.randint(1, 20), rng.randint(1, 64), rng.randint(60, 70)]))
+        casing = rng.choice([CaseMatching.Ignore, CaseMatching.Respect, CaseMatching.Smart])
+        pat, _ = device_pattern(H, needle, Config(max_typos=1, casing=casing, unicode=UnicodeMatching.Ignore))
+        want = PF.h_n_distinct(pat)
+        assert n_distinct(needle, case_sensitive(needle, casing)) == want, (needle, casing, want)
+        seen.add((want == 0, len(needle) > 64))
+    assert seen == {(False, False), (True, False), (True, True)}
 
 
 @pytest.mark.parametrize("lanes", [16, 32, 64])
@@ -336,17 +390,19 @@ def test_mask_prefilter_windows_equal_oracle(H, PF, lanes, k):
     Prefilter::match_haystack / match_haystack_1_typo, on haystacks of up to 200 bytes (several 64-byte blocks)."""
     rng = random.Random(8000 + lanes + k)
     F.lib().frz_matcher_debug_pattern.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]
-    checked = matched = 0
+    checked = matched = long_needles = 0
     for trial in range(500):
-        pool = rng.choice(POOLS)
-        needle = rand_bytes(rng, pool, rng.randint(1, 12))
+        pool = rng.choice(MASK_POOLS)
+        needle = mask_needle(rng, pool)
+        long_needles += len(needle) > 24
         cs = rng.random() < 0.3
         cfg = Config(max_typos=k, emulate_lanes=lanes, casing=CaseMatching.Respect if cs else CaseMatching.Ignore)
         pat, info = device_pattern(H, needle, cfg)
         assert info["prefilter_lanes"] == lanes
+        assert PF.h_n_distinct(pat) == n_distinct(needle, cs) > 0
         for _ in range(12):
             ln = rng.choice([0, 1, 2, 7, 15, 16, 17, 31, 33, 50, 63, 64, 65, 100, 128, 129, 200])
-            hay = rand_bytes(rng, pool + (HAY_EXTRA if rng.random() < 0.2 else b"x"), ln)
+            hay = mask_haystack(rng, needle, pool, ln, k)
             s, e = C.c_int(), C.c_int()
             got = PF.h_masks_window(pat, hay, len(hay), k, C.byref(s), C.byref(e))
             assert got >= 0
@@ -356,36 +412,45 @@ def test_mask_prefilter_windows_equal_oracle(H, PF, lanes, k):
                 assert (s.value, e.value) == (want[1], want[2]), (needle, hay, k, lanes, cs, want, s.value, e.value)
                 matched += 1
             checked += 1
-    assert checked > 5000 and matched > 500
+    assert checked > 5000 and matched > 1000 and long_needles > 150
 
 
 @pytest.mark.parametrize("k", [0, 1])
 def test_single_chunk_mask_forms_equal_oracle(H, PF, k):
     """masks_k0_single / masks_k1_single (corpora of <= 64-byte haystacks at the 64-lane width: one block, one chunk,
-    per-position masks) vs the oracle's Prefilter::match_haystack / match_haystack_1_typo."""
+    per-position masks) vs the oracle's Prefilter::match_haystack / match_haystack_1_typo.  Needles of up to 64 bytes: the
+    single-chunk forms take those with n_distinct + n <= 16, the others are refused (the kernel runs masks_k0 / masks_k1,
+    checked here too)."""
     rng = random.Random(9100 + k)
     F.lib().frz_matcher_debug_pattern.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]
-    checked = matched = 0
+    checked = matched = refused = 0
     for trial in range(900):
-        pool = rng.choice(POOLS)
-        needle = rand_bytes(rng, pool, rng.randint(1, 11))
+        pool = rng.choice(POOLS if rng.random() < 0.5 else MASK_POOLS)
+        needle = rand_bytes(rng, pool, rng.randint(1, 11) if rng.random() < 0.6 else rng.randint(1, 64))
         cs = rng.random() < 0.3
         cfg = Config(max_typos=k, emulate_lanes=64, casing=CaseMatching.Respect if cs else CaseMatching.Ignore)
         pat, info = device_pattern(H, needle, cfg)
+        nd = n_distinct(needle, cs)
+        if nd == 0:
+            continue
         for _ in range(12):
             ln = rng.choice([0, 1, 2, 3, 7, 15, 16, 17, 31, 32, 33, 47, 48, 50, 63, 64])
-            hay = rand_bytes(rng, pool + (HAY_EXTRA if rng.random() < 0.2 else b"x"), ln)
+            hay = mask_haystack(rng, needle, pool, ln, k)
             s, e = C.c_int(), C.c_int()
             got = PF.h_masks_window(pat, hay, len(hay), 100 + k, C.byref(s), C.byref(e))
-            if got == -2:
-                continue   # needle too long for the position table: the kernel takes the general form
+            if got == -2:   # n_distinct + n > 16: the kernel takes the general form
+                assert nd + len(needle) > 16
+                refused += 1
+                got = PF.h_masks_window(pat, hay, len(hay), k, C.byref(s), C.byref(e))
+            else:
+                assert nd + len(needle) <= 16
             want = O.prefilter(needle, hay, k, 64, cs)
             assert bool(got) == want[0], (needle, hay, k, cs, want)
             if want[0]:
                 assert (s.value, e.value) == (want[1], want[2]), (needle, hay, k, cs, want, s.value, e.value)
                 matched += 1
             checked += 1
-    assert checked > 6000 and matched > 800
+    assert checked > 6000 and matched > 1500 and 1000 < refused < checked - 1000
 
 
 @pytest.mark.parametrize("lanes", [16, 32, 64])
@@ -492,23 +557,30 @@ def test_signature_test_is_a_necessary_condition_for_unicode_needles(H, PF, lane
 
 
 @pytest.mark.parametrize("lanes", [16, 32, 64])
-@pytest.mark.parametrize("k", [1, 2, 3, 5])
+@pytest.mark.parametrize("k", [1, 2, 3, 4, 5, 7, 10, 15])
 def test_mask_prefilter_groundwork_2_and_n_typos(H, PF, lanes, k):
-    """masks_paths<NP> / masks_many (prefilter_masks.cuh, not yet wired into the kernels) vs match_haystack_1_typo /
-    _2_typos / _many_typos of the reference (src/prefilter/algo/ascii_typos.rs)."""
+    """masks_paths<NP> / masks_many (prefilter_masks.cuh; k_scan_window and k_prefilter_list run them at k = 2 and k >= 3
+    for needles with <= 16 byte classes, prefilter.cu: process_candidate) vs match_haystack_1_typo / _2_typos /
+    _many_typos of the reference (src/prefilter/algo/ascii_typos.rs).  Needles of up to 64 bytes, n = k + 1 and n <= k
+    among them; haystacks that hold the needle with 0..k+1 bytes deleted."""
     rng = random.Random(9000 + lanes + k)
     F.lib().frz_matcher_debug_pattern.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]
     mode = {1: 12, 2: 2}.get(k, 3)
     checked = matched = 0
-    for trial in range(300):
-        pool = rng.choice(POOLS)
-        needle = rand_bytes(rng, pool, rng.randint(1, 12))
+    lengths = set()
+    for trial in range(200):
+        pool = rng.choice(MASK_POOLS[:3])
+        r = trial % 8
+        needle = rand_bytes(rng, pool, k + 1 if r == 0 else rng.randint(1, k) if r == 1 else
+                            rng.randint(1, 64) if r < 5 else rng.randint(33, 64))
+        lengths.add(len(needle) - k)
         cs = rng.random() < 0.3
         cfg = Config(max_typos=k, emulate_lanes=lanes, casing=CaseMatching.Respect if cs else CaseMatching.Ignore)
         pat, info = device_pattern(H, needle, cfg)
+        assert PF.h_n_distinct(pat) == n_distinct(needle, cs) > 0
         for _ in range(12):
             ln = rng.choice([0, 1, 2, 7, 15, 16, 17, 31, 33, 50, 63, 64, 65, 100, 128, 129, 200])
-            hay = rand_bytes(rng, pool + (HAY_EXTRA if rng.random() < 0.2 else b"x"), ln)
+            hay = mask_haystack(rng, needle, pool, ln, k)
             s, e = C.c_int(), C.c_int()
             got = PF.h_masks_window(pat, hay, len(hay), mode, C.byref(s), C.byref(e))
             want = O.prefilter(needle, hay, k, lanes, cs)
@@ -517,7 +589,8 @@ def test_mask_prefilter_groundwork_2_and_n_typos(H, PF, lanes, k):
                 assert (s.value, e.value) == (want[1], want[2]), (needle, hay, k, lanes, cs, want, s.value, e.value)
                 matched += 1
             checked += 1
-    assert checked > 3000 and matched > 300
+    assert checked == 2400 and matched > checked // 3, (checked, matched)
+    assert 1 in lengths and min(lengths) <= 0 and max(lengths) >= 64 - k - 8
 
 
 @pytest.mark.parametrize("lanes", [16, 32, 64])
@@ -546,3 +619,151 @@ def test_swcore_128_column_classes_groundwork(H, lanes):
                 assert got == want, (needle, win, pre, lanes, cc, got, want)
                 checked += 1
     assert checked > 500
+
+
+# ---------------------------------------------------------------- scanning prefilter forms and the literal matcher (prefilter_scan.cuh)
+PS_SRC = os.path.join(ROOT, "tests", "harness", "pf_scan_harness.cpp")
+PS_LIB = os.path.join(ROOT, "tests", "harness", "libpf_scan_harness.so")
+PS_DEPS = [PS_SRC] + [os.path.join(ROOT, "frizbee_b200", "csrc", f) for f in ("prefilter_scan.cuh", "prefilter_masks.cuh", "frz_device.cuh")]
+
+
+@pytest.fixture(scope="module")
+def PS():
+    if not os.path.isdir(CUDA_INC):
+        pytest.skip("CUDA headers not found")
+    if not os.path.exists(PS_LIB) or any(os.path.getmtime(d) > os.path.getmtime(PS_LIB) for d in PS_DEPS):
+        subprocess.run(["g++", "-O2", "-std=c++17", "-I" + CUDA_INC, "-fPIC", "-shared", "-o", PS_LIB, PS_SRC], check=True)
+    L = C.CDLL(PS_LIB)
+    ip = C.POINTER(C.c_int)
+    L.h_scan_window.argtypes = [C.c_void_p, C.c_char_p, C.c_int, ip, ip]
+    L.h_scan_window_long.argtypes = [C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_int, ip, ip]
+    L.h_lit_find.argtypes = [C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_int, ip, C.POINTER(C.c_uint32)]
+    L.h_pattern_probes.argtypes = [C.c_void_p, C.c_char_p, C.c_char_p]
+    return L
+
+
+SCAN_POOLS = [b"abcdefghijklmnopqrstuvwxyzABCDEFGHIJKLMNOPQRSTUVWXYZ0123456789_-/. ", b"abcdefghijklmnopqrs",
+              b"aAbBcC", b"abAB_/-01", b"ab\x00-Zz"]
+SCAN_LENS = [0, 1, 2, 3, 4, 5, 7, 15, 16, 17, 31, 32, 33, 63, 64, 65, 100, 128, 129, 255, 256, 511, 1024, 1025, 2600]
+
+
+def scan_case(rng, n):
+    """a needle of n bytes (few or many byte classes, NUL among them), its case mode and typo budget"""
+    pool = rng.choice(SCAN_POOLS)
+    needle = rand_bytes(rng, pool, n)
+    casing = rng.choice([CaseMatching.Ignore, CaseMatching.Respect, CaseMatching.Smart])
+    k = rng.choice(list(range(16)) + [n, n + rng.randint(1, 5)])
+    return needle, pool, casing, case_sensitive(needle, casing), k
+
+
+def scan_haystack(rng, needle, pool, k):
+    ln = rng.choice(SCAN_LENS)
+    filler = pool + rng.choice([b"", b"xyz", HAY_EXTRA, b"\x80\xff\x00"])
+    if ln >= 1 and rng.random() < 0.55:
+        return plant(rng, needle, ln, filler, drops=rng.randint(0, k + 1), spread=rng.random() < 0.4, flip_p=0.15)
+    return rand_bytes(rng, filler, ln)
+
+
+def check_window(got, s, e, want, ctx):
+    assert got >= 0, ctx
+    assert bool(got) == want[0], (ctx, want)
+    if want[0]:
+        assert (s.value, e.value) == (want[1], want[2]), (ctx, want, s.value, e.value)
+
+
+@pytest.mark.parametrize("lanes", [16, 32, 64])
+def test_scan_forms_equal_oracle(H, PS, lanes):
+    """window_k0 / _k1 / _k2 / _many on FrzPatternDev (the form the pattern's typo mode selects, as k_match_indices and,
+    for needles of more than 16 byte classes, k_scan_window / k_prefilter_list run it) vs Prefilter::match_haystack* of
+    the reference, window bounds included: needles of 1..64 bytes on both sides of 16 classes, k in 0..15 and >= n, all
+    three case modes, haystacks of 0..2600 bytes with NUL and bytes >= 0x80."""
+    rng = random.Random(15000 + lanes)
+    F.lib().frz_matcher_debug_pattern.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]
+    checked = matched = 0
+    forms, budgets = set(), set()
+    for trial in range(1500):
+        n = rng.choice([rng.randint(1, 16), rng.randint(1, 64), rng.randint(40, 64)])
+        needle, pool, casing, cs, k = scan_case(rng, n)
+        pat, info = device_pattern(H, needle, Config(max_typos=k, emulate_lanes=lanes, casing=casing,
+                                                     unicode=UnicodeMatching.Ignore))
+        assert info["prefilter_lanes"] == lanes
+        forms.add(n_distinct(needle, cs) > 0)
+        budgets.add(min(k, 16) if k < n else "all")
+        for _ in range(8):
+            hay = scan_haystack(rng, needle, pool, k)
+            s, e = C.c_int(), C.c_int()
+            got = PS.h_scan_window(pat, hay, len(hay), C.byref(s), C.byref(e))
+            want = O.prefilter(needle, hay, k, lanes, cs)
+            check_window(got, s, e, want, (needle, hay, k, lanes, cs))
+            matched += want[0]
+            checked += 1
+    assert forms == {True, False} and budgets >= set(range(16)) | {"all"}, (forms, budgets)
+    assert checked == 12000 and checked // 4 < matched < checked - checked // 4, matched
+
+
+@pytest.mark.parametrize("lanes", [16, 32, 64])
+def test_scan_forms_long_needles_equal_oracle(H, PS, lanes):
+    """The same forms on LongPat (k_scan_window_long / k_prefilter_list_long: needles of 65..1024 bytes, per-position data
+    from the needle table) vs the oracle.  The needle table is built from the case_needle pairs with host.cu's probes,
+    checked against the pattern's own probes over its first 64 positions."""
+    rng = random.Random(16000 + lanes)
+    F.lib().frz_matcher_debug_pattern.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]
+    checked = matched = 0
+    om, tg = C.create_string_buffer(64), C.create_string_buffer(64)
+    for trial in range(300):
+        n = rng.choice([65, rng.randint(65, 200), rng.randint(65, 1024), 1024])
+        needle, pool, casing, cs, k = scan_case(rng, n)
+        pat, info = device_pattern(H, needle, Config(max_typos=k, emulate_lanes=lanes, casing=casing,
+                                                     unicode=UnicodeMatching.Ignore))
+        c, flip = case_pairs(needle, cs)
+        PS.h_pattern_probes(pat, om, tg)
+        assert [(om.raw[i], tg.raw[i]) for i in range(64)] == [
+            (0x20, x | 0x20) if f != x else (0, x) for x, f in zip(c[:64], flip[:64])]
+        for _ in range(6):
+            hay = scan_haystack(rng, needle, pool, k)
+            s, e = C.c_int(), C.c_int()
+            got = PS.h_scan_window_long(pat, c, flip, hay, len(hay), C.byref(s), C.byref(e))
+            want = O.prefilter(needle, hay, k, lanes, cs)
+            check_window(got, s, e, want, (n, hay, k, lanes, cs))
+            matched += want[0]
+            checked += 1
+    assert checked == 1800 and matched > 200 and checked - matched > 500, matched
+
+
+def test_literal_matcher_equals_oracle(H, PS):
+    """lit_find (the literal modes of the byte path, on FrzPatternDev and on LongPat) vs the oracle's match_list in the
+    same mode: match, score and exact flag, for needles of 1..1024 bytes and both case modes."""
+    rng = random.Random(17000)
+    F.lib().frz_matcher_debug_pattern.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]
+    found = missed = longs = 0
+    for trial in range(1000):
+        n = rng.choice([rng.randint(1, 8), rng.randint(1, 64), rng.randint(60, 70), rng.randint(65, 1024)])
+        pool = rng.choice(SCAN_POOLS)
+        needle = rand_bytes(rng, pool, n)
+        mode = [Matching.Exact, Matching.Prefix, Matching.Suffix, Matching.Substring][trial % 4]
+        casing = rng.choice([CaseMatching.Ignore, CaseMatching.Respect])
+        cs = casing == CaseMatching.Respect
+        cfg = Config(matching=mode, casing=casing, unicode=UnicodeMatching.Ignore)
+        pat, _ = device_pattern(H, needle, cfg)
+        c, flip = case_pairs(needle, cs)
+        longs += n > 64
+        for _ in range(4):
+            mid = bytes((b ^ 0x20) if (not cs and chr(b).isalpha() and b < 0x80 and rng.random() < 0.3) else b for b in needle)
+            if rng.random() < 0.2 and n > 1:
+                i = rng.randrange(n)
+                mid = mid[:i] + b"#" + mid[i + 1:]
+            pre = rand_bytes(rng, pool + b"_ ", rng.choice([0, 0, 1, 3, 40]))
+            post = rand_bytes(rng, pool + b"_ ", rng.choice([0, 0, 1, 3, 40]))
+            hay = rng.choice([mid, pre + mid, mid + post, pre + mid + post, pre + mid + post + mid])
+            data, off = O.pack([hay])
+            want = O.match_list_packed([needle], cfg, data, off)
+            pos, score = C.c_int(), C.c_uint32()
+            got = PS.h_lit_find(pat, c if n > 64 else None, flip if n > 64 else None, hay, len(hay), C.byref(pos), C.byref(score))
+            assert got == len(want), (needle, hay, mode, cs)
+            if got:
+                exact = pos.value == 0 and n == len(hay)
+                assert (score.value, exact) == (int(want["score"][0]), bool(want["exact"][0])), (needle, hay, mode, cs)
+                found += 1
+            else:
+                missed += 1
+    assert found > 1400 and missed > 400 and longs > 200, (found, missed, longs)
