@@ -77,6 +77,7 @@ def lib():
     L.frz_corpus_device.argtypes = [vp]
     L.frz_corpus_destroy.argtypes = [vp]
     L.frz_corpus_destroy.restype = None
+    L.frz_corpus_debug_image.argtypes = [vp] * 7 + [C.POINTER(u64)]
     L.frz_matcher_create.argtypes = [vp, sz, C.POINTER(CConfig), C.POINTER(vp)]
     L.frz_matcher_from_query.argtypes = [u8p, sz, C.POINTER(CConfig), C.POINTER(vp)]
     L.frz_matcher_set_config.argtypes = [vp, C.POINTER(CConfig)]

@@ -22,7 +22,9 @@
 #define FRZ_GROUP 32           // slots per group (= warp)
 #define FRZ_GROUPS_PER_TILE (FRZ_TILE / FRZ_GROUP)
 #define FRZ_UNIT 16            // bytes per unit
-#define FRZ_MAX_HAY_LEN ((1u << 22) - 1)  // slot meta keeps len in 22 bits
+// Longest haystack, in bytes (4 MiB - 2).  Slot meta keeps len in 22 bits; a length of (1 << 22) - 1 at local index 1023
+// would encode as 0xFFFFFFFF, the unused-slot sentinel below, so the longest length stops one short of the field's maximum.
+#define FRZ_MAX_HAY_LEN ((1u << 22) - 2)
 #define FRZ_INVALID_SLOT 0xFFFFFFFFu      // slot meta of an unused slot (last tile)
 #define FRZ_MAX_NEEDLE 64      // needle bytes whose per-position data lives in FrzPatternDev (the constant bank)
 #define FRZ_LONG_NEEDLE 1024   // longest byte-path needle: 65..1024 bytes read FrzNeedleTab (longer → FRZ_ERR_UNSUPPORTED)

@@ -234,6 +234,9 @@ extern "C" frz_status frz_corpus_create_device(const uint8_t* d_bytes, const uin
     auto c = std::make_unique<frz_corpus>();
     c->st.device = device;
     frz_status s = frz_pack_corpus_device(d_bytes, d_offsets, 8, n, total_bytes, (cudaStream_t)stream, &c->st);
+    // the corpus is complete on return: matches run on other streams, and the caller may free the inputs
+    if (s == FRZ_OK && cudaStreamSynchronize((cudaStream_t)stream) != cudaSuccess)
+        s = frz_fail(FRZ_ERR_CUDA, "pack failed: %s", cudaGetErrorString(cudaGetLastError()));
     if (s != FRZ_OK) { c->st.release(); return s; }
     *out = c.release();
     return FRZ_OK;
@@ -296,6 +299,33 @@ extern "C" uint64_t frz_corpus_device_bytes(const frz_corpus* c) {
     return (s.total_units + 1) * 16 + (uint64_t)s.n_tiles * (8 + FRZ_GROUPS_PER_TILE * 16 + FRZ_TILE * (6 + 8));
 }
 extern "C" int frz_corpus_device(const frz_corpus* c) { return c ? c->st.device : -1; }
+
+// Test aid: the packed image (frz_device.cuh), so that tests can check the layout against a restatement of DESIGN.md §3.
+extern "C" frz_status frz_corpus_debug_image(const frz_corpus* c, void* tile_base, void* groups, void* slot_meta, void* slot_of,
+                                             void* slot_sig, void* units, uint64_t sizes[6]) {
+    if (!c || !sizes) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    const FrzCorpusStorage& s = c->st;
+    const uint64_t slots = (uint64_t)s.n_tiles * FRZ_TILE;
+    const uint64_t need[6] = {(uint64_t)s.n_tiles * sizeof(uint64_t), (uint64_t)s.n_tiles * FRZ_GROUPS_PER_TILE * sizeof(FrzGroupDesc),
+                              slots * sizeof(uint32_t), slots * sizeof(uint16_t), slots * sizeof(uint2), s.total_units * sizeof(uint4)};
+    const void* src[6] = {s.tile_base, s.groups, s.slot_meta, s.slot_of, s.slot_sig, s.data};
+    void* dst[6] = {tile_base, groups, slot_meta, slot_of, slot_sig, units};
+    int given = 0;
+    for (void* d : dst) given += d != nullptr;
+    if (given == 0) {   // size query
+        memcpy(sizes, need, sizeof need);
+        return FRZ_OK;
+    }
+    if (given != 6) return frz_fail(FRZ_ERR_INVALID_ARG, "pass all six buffers, or none for a size query");
+    for (int i = 0; i < 6; i++)
+        if (sizes[i] != need[i])
+            return frz_fail(FRZ_ERR_INVALID_ARG, "buffer %d holds %llu bytes, the image needs %llu", i, (unsigned long long)sizes[i],
+                            (unsigned long long)need[i]);
+    FRZ_TRY(ensure_device(s.device));
+    for (int i = 0; i < 6; i++)
+        if (need[i]) FRZ_CUDA_TRY(cudaMemcpy(dst[i], src[i], need[i], cudaMemcpyDeviceToHost));
+    return FRZ_OK;
+}
 extern "C" void frz_corpus_destroy(frz_corpus* c) {
     if (!c) return;
     cudaSetDevice(c->st.device);

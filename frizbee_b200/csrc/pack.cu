@@ -289,6 +289,8 @@ __global__ void k_rebase_offsets(const OffT* __restrict__ in, uint64_t n_new, co
 //   pack_copy      tiles [t0, t1) from the staged bytes into the slot-major layout
 namespace {
 
+constexpr const char* kHayTooLong = "haystack longer than %u bytes";
+
 frz_status pack_reserve(FrzCorpusStorage* out, uint32_t n_tiles, uint32_t keep_tiles, cudaStream_t stream) {
     if (out->cap_tiles >= n_tiles) return FRZ_OK;
     const uint32_t want = keep_tiles ? std::max<uint32_t>(n_tiles, out->cap_tiles + out->cap_tiles / 2) : n_tiles;
@@ -331,7 +333,7 @@ frz_status pack_plan(FrzCorpusStorage* out, const OffT* d_offsets, uint64_t n, u
     uint64_t h[2] = {0, 0};
     FRZ_CUDA_TRY(cudaMemcpyAsync(h, d_total, 16, cudaMemcpyDeviceToHost, stream));
     FRZ_CUDA_TRY(cudaStreamSynchronize(stream));
-    if ((unsigned int)(h[1] & 0xffffffffu)) return frz_fail(FRZ_ERR_UNSUPPORTED, "haystack longer than 4 MiB");
+    if ((unsigned int)(h[1] & 0xffffffffu)) return frz_fail(FRZ_ERR_UNSUPPORTED, kHayTooLong, FRZ_MAX_HAY_LEN);
     out->total_units = h[0];
     out->max_gunits = std::max<uint32_t>(tile0 ? out->max_gunits : 0u, (uint32_t)(h[1] >> 32));
     if (out->cap_units < out->total_units + 1) {
@@ -364,17 +366,27 @@ frz_status pack_copy(FrzCorpusStorage* out, const uint8_t* d_bytes, const OffT* 
     return FRZ_OK;
 }
 
+// `d_bytes` is the value buffer the offsets index (haystack i = d_bytes[d_offsets[i], d_offsets[i + 1])), and
+// total_bytes = d_offsets[n] - d_offsets[0]; the first and last offsets are read back to check it.
 template <typename OffT>
 frz_status pack_device_t(const uint8_t* d_bytes, const OffT* d_offsets, uint64_t n, uint64_t total_bytes, cudaStream_t stream,
                          FrzCorpusStorage* out) {
     const uint32_t n_tiles = (uint32_t)((n + FRZ_TILE - 1) / FRZ_TILE);
+    if (n_tiles == 0) { out->n = 0; out->n_tiles = 0; out->total_bytes = 0; out->total_units = 0; return FRZ_OK; }
+    OffT ends[2] = {0, 0};
+    FRZ_CUDA_TRY(cudaMemcpyAsync(&ends[0], d_offsets, sizeof(OffT), cudaMemcpyDeviceToHost, stream));
+    FRZ_CUDA_TRY(cudaMemcpyAsync(&ends[1], d_offsets + n, sizeof(OffT), cudaMemcpyDeviceToHost, stream));
+    FRZ_CUDA_TRY(cudaStreamSynchronize(stream));
+    const uint64_t off0 = (uint64_t)ends[0];
+    if ((uint64_t)ends[1] < off0 || (uint64_t)ends[1] - off0 != total_bytes)
+        return frz_fail(FRZ_ERR_INVALID_ARG, "total_bytes %llu != d_offsets[n] - d_offsets[0] = %llu - %llu", (unsigned long long)total_bytes,
+                        (unsigned long long)ends[1], (unsigned long long)off0);
     out->n = n;
     out->n_tiles = n_tiles;
     out->total_bytes = total_bytes;
-    if (n_tiles == 0) { out->total_units = 0; return FRZ_OK; }
     FRZ_TRY(pack_reserve(out, n_tiles, 0, stream));
     FRZ_TRY(pack_plan<OffT>(out, d_offsets, n, 0, 0, 0, false, stream));
-    return pack_copy<OffT>(out, d_bytes, d_offsets, 0, 0, 0, total_bytes, 0, n_tiles, stream);
+    return pack_copy<OffT>(out, d_bytes + off0, d_offsets, 0, 0, off0, total_bytes, 0, n_tiles, stream);
 }
 
 // Streamed ingest: offsets first, then the value bytes in tile-aligned chunks on a copy stream; the plan runs
@@ -432,6 +444,11 @@ frz_status append_host_t(FrzIngest& ing, const uint8_t* h_bytes, const OffT* h_o
     const uint64_t n_old = st->n;
     const uint64_t n = n_old + n_new;
     if (n > 0xFFFFFFFFull) return frz_fail(FRZ_ERR_TOO_MANY_ITEMS, "too many items in haystack: %llu", (unsigned long long)n);
+    // a refused append must leave the corpus as it was, so the lengths are checked here, before anything below
+    // replaces the metadata of the old tail tile (pack_plan would find them only after that)
+    for (uint64_t i = 0; i < n_new; i++)
+        if ((uint64_t)h_offsets[i + 1] - (uint64_t)h_offsets[i] > FRZ_MAX_HAY_LEN)
+            return frz_fail(FRZ_ERR_UNSUPPORTED, kHayTooLong, FRZ_MAX_HAY_LEN);
     const uint32_t t_last = (uint32_t)(n_old / FRZ_TILE), cnt = (uint32_t)(n_old % FRZ_TILE);
     const uint64_t idx0 = (uint64_t)t_last * FRZ_TILE;
     const uint64_t off0 = (uint64_t)h_offsets[0];

@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define FRZ_ABI_VERSION 2
+#define FRZ_ABI_VERSION 3
 #if defined(__GNUC__)
 #define FRZ_API __attribute__((visibility("default")))
 #else
@@ -174,9 +174,16 @@ FRZ_API frz_status frz_corpus_append(frz_corpus* c, const uint8_t* bytes, const 
 /* same, from a pointer array + lengths (the layout a Rust `&[&str]` has) */
 FRZ_API frz_status frz_corpus_create_ptrs(const uint8_t* const* ptrs, const uint32_t* lens, uint64_t n,
                                   int device, frz_corpus** out);
-/* same, but `d_bytes`/`d_offsets` are already device pointers on `device` */
+/* same, but `d_bytes`/`d_offsets` are already device pointers on `device`.  As in Arrow, haystack i is
+ * d_bytes[d_offsets[i], d_offsets[i+1]): a slice may start at d_offsets[0] != 0, and d_bytes may have any alignment.
+ * total_bytes must equal d_offsets[n] - d_offsets[0] (the sum of the lengths, frz_corpus_total_bytes), else
+ * FRZ_ERR_INVALID_ARG.  The work runs on `stream` (a cudaStream_t, NULL = the legacy default stream), so that stream must
+ * be ordered after whatever wrote the buffers.  Blocking: the corpus is complete when the call returns, and the caller
+ * may then reuse or free d_bytes/d_offsets. */
 FRZ_API frz_status frz_corpus_create_device(const uint8_t* d_bytes, const uint64_t* d_offsets, uint64_t n,
                                     uint64_t total_bytes, int device, void* stream, frz_corpus** out);
+/* Every constructor, frz_corpus_append and the end-to-end calls refuse a haystack longer than 4194302 bytes (4 MiB - 2)
+ * with FRZ_ERR_UNSUPPORTED; a refused append leaves the corpus as it was. */
 FRZ_API uint64_t frz_corpus_len(const frz_corpus* c);
 FRZ_API uint64_t frz_corpus_total_bytes(const frz_corpus* c);   /* sum of haystack lengths */
 FRZ_API uint64_t frz_corpus_device_bytes(const frz_corpus* c);  /* HBM footprint of the packed form */
@@ -354,6 +361,14 @@ FRZ_API uint32_t frz_matcher_score_bound(const frz_matcher* m);
 /* Test aid: copies the compiled device pattern (frizbee_b200/csrc/frz_device.cuh: FrzPatternDev) of pattern i; out_size
  * must equal its size.  Lets host builds of the kernel cores run with exactly the constants the GPU receives. */
 FRZ_API frz_status frz_matcher_debug_pattern(const frz_matcher* m, size_t i, void* out, size_t out_size);
+
+/* Test aid: copies the packed image of a corpus (frizbee_b200/csrc/frz_device.cuh, DESIGN.md §3) to host buffers, in
+ * this order: tile_base (u64 per tile), groups (FrzGroupDesc, 16 bytes per group), slot_meta (u32 per slot), slot_of
+ * (u16 per slot), slot_sig (2 x u32 per slot) and the packed units [0, total units) (16 bytes each).  With all six
+ * buffers NULL, writes their sizes in bytes to sizes[0..5]; otherwise all six are needed and sizes[i] must equal those
+ * sizes exactly.  Lets tests check the layout that every constructor and frz_corpus_append produce. */
+FRZ_API frz_status frz_corpus_debug_image(const frz_corpus* c, void* tile_base, void* groups, void* slot_meta, void* slot_of,
+                                  void* slot_sig, void* units, uint64_t sizes[6]);
 
 /* radix_sort_matches (src/sort.rs:6-40): stable, descending score; `matches` is host memory. */
 FRZ_API frz_status frz_radix_sort_matches(frz_match* matches, uint64_t n, int device);

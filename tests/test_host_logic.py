@@ -20,7 +20,19 @@ def test_library_exports_every_declared_symbol():
     lib = ctypes.CDLL(F.lib_path())
     missing = [n for n in sorted(names) if not hasattr(lib, n)]
     assert not missing, missing
-    assert F.lib().frz_abi_version() == 2
+    assert F.lib().frz_abi_version() == 3
+
+
+def test_corpus_debug_image_argument_checks():
+    """frz_corpus_debug_image (a test aid) refuses a null corpus or a null size array before it touches a device; the
+    size and buffer checks on a real corpus are in tests/test_gpu_ingest.py."""
+    L = F.lib()
+    sizes = (ctypes.c_uint64 * 6)()
+    bufs = [ctypes.create_string_buffer(16) for _ in range(6)]
+    assert L.frz_corpus_debug_image(None, *[None] * 6, sizes) == 1   # FRZ_ERR_INVALID_ARG
+    assert L.frz_corpus_debug_image(None, *[ctypes.addressof(b) for b in bufs], sizes) == 1
+    assert L.frz_corpus_debug_image(None, *[None] * 6, None) == 1
+    assert b"null" in L.frz_last_error()
 
 
 def test_parse_atom_reference_vectors():
