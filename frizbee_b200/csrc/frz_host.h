@@ -3,6 +3,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <atomic>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -37,63 +39,133 @@ inline int frz_sm_count() {
         if (_s != FRZ_OK) return _s;          \
     } while (0)
 
+// ------------------------------------------------------------------------------------------ owners
+// The only place the library frees CUDA memory, events and streams.  Every buffer, event and stream is held by one of
+// these move-only types, so error paths and device switches release what they own without a hand-written list.
+
+// Bytes held by all device FrzDevArrays (frz_debug_device_bytes).
+inline std::atomic<uint64_t> g_frz_device_bytes{0};
+
+// A grow-only array of T on one device (Pinned: in page-locked host memory).  It remembers the device it was allocated on
+// and frees the block there; an empty array makes no CUDA call, so host-only users never touch the runtime.
+template <typename T, bool Pinned = false>
+class FrzDevArray {
+public:
+    FrzDevArray() = default;
+    FrzDevArray(FrzDevArray&& o) noexcept : p_(o.p_), cap_(o.cap_), dev_(o.dev_) { o.p_ = nullptr; o.cap_ = 0; }
+    FrzDevArray& operator=(FrzDevArray&& o) noexcept {
+        if (this != &o) {
+            reset();
+            p_ = o.p_; cap_ = o.cap_; dev_ = o.dev_;
+            o.p_ = nullptr; o.cap_ = 0;
+        }
+        return *this;
+    }
+    FrzDevArray(const FrzDevArray&) = delete;
+    FrzDevArray& operator=(const FrzDevArray&) = delete;
+    ~FrzDevArray() { reset(); }
+
+    T* get() const { return p_; }
+    uint64_t cap() const { return cap_; }   // in elements
+    int device() const { return dev_; }
+    // cap() >= need afterwards.  Growing frees the old block first (its contents are dropped, so the peak stays one block)
+    // and then allocates `want` (>= need) elements on the current device.
+    frz_status reserve(uint64_t need, uint64_t want) {
+        if (cap_ >= need) return FRZ_OK;
+        reset();
+        void* p = nullptr;
+        FRZ_CUDA_TRY(Pinned ? cudaMallocHost(&p, want * sizeof(T)) : cudaMalloc(&p, want * sizeof(T)));
+        cudaGetDevice(&dev_);
+        p_ = static_cast<T*>(p);
+        cap_ = want;
+        if (!Pinned) g_frz_device_bytes += cap_ * sizeof(T);
+        return FRZ_OK;
+    }
+    frz_status reserve(uint64_t n) { return reserve(n, n); }
+    // frees the block on its own device; the calling thread's current device is left as it was
+    void reset() {
+        if (!p_) return;
+        int cur = dev_;
+        cudaGetDevice(&cur);
+        if (cur != dev_) cudaSetDevice(dev_);
+        if (Pinned) cudaFreeHost(p_);
+        else { cudaFree(p_); g_frz_device_bytes -= cap_ * sizeof(T); }
+        if (cur != dev_) cudaSetDevice(cur);
+        p_ = nullptr;
+        cap_ = 0;
+    }
+
+private:
+    T* p_ = nullptr;
+    uint64_t cap_ = 0;
+    int dev_ = -1;
+};
+template <typename T>
+using FrzPinnedArray = FrzDevArray<T, true>;
+
+struct FrzEventDeleter { void operator()(cudaEvent_t e) const { cudaEventDestroy(e); } };
+struct FrzStreamDeleter { void operator()(cudaStream_t s) const { cudaStreamDestroy(s); } };
+using FrzEvent = std::unique_ptr<CUevent_st, FrzEventDeleter>;
+using FrzStream = std::unique_ptr<CUstream_st, FrzStreamDeleter>;
+inline frz_status frz_event_create(FrzEvent& out, unsigned flags) {
+    cudaEvent_t e = nullptr;
+    FRZ_CUDA_TRY(cudaEventCreateWithFlags(&e, flags));
+    out.reset(e);
+    return FRZ_OK;
+}
+inline frz_status frz_stream_create(FrzStream& out, unsigned flags) {
+    cudaStream_t s = nullptr;
+    FRZ_CUDA_TRY(cudaStreamCreateWithFlags(&s, flags));
+    out.reset(s);
+    return FRZ_OK;
+}
+
 // Owned device buffers of a packed corpus.
 struct FrzCorpusStorage {
-    uint4* data = nullptr;
-    uint64_t* tile_base = nullptr;
-    FrzGroupDesc* groups = nullptr;
-    uint32_t* slot_meta = nullptr;
-    uint16_t* slot_of = nullptr;
-    uint2* slot_sig = nullptr;
+    // grow-only, reused by the end-to-end path (no cudaMalloc/cudaFree per call); tile_base.cap() is the tile capacity
+    FrzDevArray<uint4> data;
+    FrzDevArray<uint64_t> tile_base;
+    FrzDevArray<FrzGroupDesc> groups;
+    FrzDevArray<uint32_t> slot_meta;
+    FrzDevArray<uint16_t> slot_of;
+    FrzDevArray<uint2> slot_sig;
+    FrzDevArray<uint64_t> scratch_tile_units;  // [tile capacity] + 2 words (total, error)
     uint64_t n = 0;
     uint32_t n_tiles = 0;
     uint64_t total_units = 0;
     uint64_t total_bytes = 0;
     uint32_t max_gunits = 0;   // longest haystack of the corpus in 16-byte units
     int device = 0;
-    // capacities (grow-only reuse by the end-to-end path: no cudaMalloc/cudaFree per call)
-    uint32_t cap_tiles = 0;
-    uint64_t cap_units = 0;
-    uint64_t* scratch_tile_units = nullptr;  // [cap_tiles] + 2 words (total, error)
 
     FrzCorpusView view() const {
         FrzCorpusView v;
-        v.data = data;
-        v.tile_base = tile_base;
-        v.groups = groups;
-        v.slot_meta = slot_meta;
-        v.slot_of = slot_of;
-        v.slot_sig = slot_sig;
+        v.data = data.get();
+        v.tile_base = tile_base.get();
+        v.groups = groups.get();
+        v.slot_meta = slot_meta.get();
+        v.slot_of = slot_of.get();
+        v.slot_sig = slot_sig.get();
         v.n = n;
         v.n_tiles = n_tiles;
         v.max_gunits = max_gunits;
         return v;
     }
-    void release() {
-        cudaFree(data); cudaFree(tile_base); cudaFree(groups); cudaFree(slot_meta); cudaFree(slot_of); cudaFree(slot_sig); cudaFree(scratch_tile_units);
-        data = nullptr; tile_base = nullptr; groups = nullptr; slot_meta = nullptr; slot_of = nullptr; slot_sig = nullptr; scratch_tile_units = nullptr;
-        cap_tiles = 0; cap_units = 0;
-    }
-};
-
-struct FrzIngest;
-struct frz_corpus {
-    FrzCorpusStorage st;
-    FrzIngest* ingest = nullptr;   // created by the first frz_corpus_append, kept for the next ones
 };
 
 // Staging arena + copy stream of the streamed ingest (pack.cu): grow-only, reused across calls.
 struct FrzIngest {
     static constexpr int kMaxChunks = 32;
     static constexpr uint64_t kMinChunkBytes = 8ull << 20;
-    uint8_t* d_bytes = nullptr;
-    uint64_t bytes_cap = 0;
-    void* d_offsets = nullptr;
-    uint64_t offsets_cap = 0;             // bytes
-    cudaStream_t copy_stream = nullptr;   // non-blocking: overlaps the (legacy default) compute stream
-    cudaEvent_t ev[kMaxChunks + 1] = {};  // [c] chunk c landed; [kMaxChunks] offsets landed / arena free
+    FrzDevArray<uint8_t> d_bytes;
+    FrzDevArray<uint8_t> d_offsets;
+    FrzStream copy_stream;            // non-blocking: overlaps the (legacy default) compute stream
+    FrzEvent ev[kMaxChunks + 1];      // [c] chunk c landed; [kMaxChunks] offsets landed / arena free
     frz_status reserve(uint64_t bytes, uint64_t offset_bytes);
-    void release();
+};
+
+struct frz_corpus {
+    FrzCorpusStorage st;
+    std::unique_ptr<FrzIngest> ingest;   // created by the first frz_corpus_append, kept for the next ones
 };
 
 // pack.cu
@@ -117,43 +189,43 @@ struct FrzScoreHist {
     uint32_t mask = 0;     // bins - 1
 };
 
-// Per-matcher device workspace (grown on demand, reused across calls).
-struct FrzWorkspace {
-    int device = -1;
-    FrzCounters* counters = nullptr;        // device
-    FrzCounters* h_counters = nullptr;      // pinned host mirror
-    unsigned long long* stream_total = nullptr;   // device: running match count of a streamed call (tile-scan carry)
-    FrzSurvivor* survivors[FRZ_N_CLASSES] = {};
-    FrzSurvLists lists() const { FrzSurvLists l; for (int c = 0; c < FRZ_N_CLASSES; c++) l.p[c] = survivors[c]; return l; }
-    uint64_t survivor_cap = 0;              // per class
-    uint32_t* surv_bitmap = nullptr;        // [n_tiles * 32] survivor bits by index-within-tile
-    uint16_t* word_prefix = nullptr;        // [n_tiles * 32] exclusive popcount prefix of surv_bitmap words
-    uint32_t* tile_count = nullptr;         // [n_tiles] matches per tile
-    uint64_t* tile_out_base = nullptr;      // [n_tiles] exclusive scan of tile_count
-    uint32_t tiles_cap = 0;
-    FrzMatchDev* matches_a = nullptr;       // index-ordered matches
-    FrzMatchDev* matches_b = nullptr;       // sort ping-pong / final
-    uint64_t match_cap = 0;
-    uint32_t* sort_hist = nullptr;          // [256 * n_sort_blocks]
-    uint64_t sort_hist_cap = 0;
-    uint32_t* fused_hist = nullptr;         // FrzScoreHist counts, then the per-segment prefix rows the sort's scan writes
-    uint64_t fused_hist_cap = 0;            // in words
-    uint64_t fused_clean_words = 0;         // leading words of fused_hist known to be zero (the scan re-zeroes what it reads)
-    bool fused_hist_dirty = false;          // counts were handed to the scoring kernels, their scan was not enqueued yet
-    void* cand_list = nullptr;              // k_sig_scan → k_window candidate records (16 bytes each)
-    uint64_t cand_cap = 0;                  // in records
-    uint32_t* retain_cnt = nullptr;         // multi-pattern stable compaction scratch
-    uint64_t* retain_base = nullptr;
-    uint8_t* retain_keep = nullptr;
-    uint64_t retain_cap = 0;
-    uint16_t* unicode_scratch = nullptr;    // unicode.cu: per-thread row state of the per-scalar Smith-Waterman
-    uint64_t unicode_scratch_cap = 0;       // in uint16 elements
-    cudaEvent_t table_ev = nullptr;         // recorded right after the sort's scan kernel: the per-score table is final there,
+// Scratch of the score sorts (sort.cu), one per concurrent user.
+struct FrzSortScratch {
+    FrzDevArray<uint32_t> hist;             // frz_sort_hist_alloc: per-segment digit counts, totals, digit_base, pass counter
+    FrzDevArray<uint32_t> fused;            // FrzScoreHist counts, then the per-segment prefix rows the sort's scan writes
+    uint64_t fused_clean_words = 0;         // leading words of `fused` known to be zero (the scan re-zeroes what it reads)
+    bool fused_dirty = false;               // counts were handed to the scoring kernels, their scan was not enqueued yet
+    FrzEvent table_ev;                      // recorded right after the sort's scan kernel: the per-score table is final there,
     bool arm_table_ev = false;              //   one kernel (the scatter) before the run itself (shard calls arm it)
     bool table_ev_recorded = false;
-    cudaEvent_t ev[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-    bool ev_rec[6] = {false, false, false, false, false, false};  // recorded during the current call
-    void release();
+};
+
+// Per-matcher device workspace (grown on demand, reused across calls).  Everything in it lives on `device`; moving to
+// another device is a move-assignment from a fresh workspace.
+struct FrzWorkspace {
+    int device = -1;
+    FrzDevArray<FrzCounters> counters;
+    FrzPinnedArray<FrzCounters> h_counters;          // host mirror
+    FrzDevArray<unsigned long long> stream_total;    // [0] running match count of a streamed call (tile-scan carry), [1] spare count slot
+    FrzDevArray<FrzSurvivor> survivors[FRZ_N_CLASSES];
+    FrzSurvLists lists() const { FrzSurvLists l; for (int c = 0; c < FRZ_N_CLASSES; c++) l.p[c] = survivors[c].get(); return l; }
+    uint64_t survivor_cap() const { return survivors[0].cap(); }   // per class
+    FrzDevArray<uint32_t> surv_bitmap;      // [n_tiles * 32] survivor bits by index-within-tile
+    FrzDevArray<uint16_t> word_prefix;      // [n_tiles * 32] exclusive popcount prefix of surv_bitmap words
+    FrzDevArray<uint32_t> tile_count;       // [n_tiles] matches per tile
+    FrzDevArray<uint64_t> tile_out_base;    // [n_tiles] exclusive scan of tile_count
+    FrzDevArray<FrzMatchDev> matches_a;     // index-ordered matches
+    FrzDevArray<FrzMatchDev> matches_b;     // sort ping-pong / final
+    FrzDevArray<FrzMatchDev> multi_a;       // multi-pattern candidate ping-pong / two-pass sort scratch
+    FrzDevArray<FrzMatchDev> multi_b;
+    FrzSortScratch sort;
+    FrzDevArray<uint4> cand_list;           // k_sig_scan → k_window candidate records (16 bytes each)
+    FrzDevArray<uint32_t> retain_cnt;       // multi-pattern stable compaction scratch
+    FrzDevArray<uint64_t> retain_base;
+    FrzDevArray<uint8_t> retain_keep;
+    FrzDevArray<uint16_t> unicode_scratch;  // unicode.cu: per-thread row state of the per-scalar Smith-Waterman
+    FrzEvent ev[4];                         // call start, scan done, scoring done, call end
+    bool ev_rec[4] = {false, false, false, false};  // recorded during the current call
 };
 
 // kernels (prefilter.cu / sw.cu / sort.cu) — all asynchronous on `stream`
@@ -188,30 +260,26 @@ constexpr uint32_t kFrzNoLimit = 0xFFFFFFFFu;
 // d_tmp is only used when score_bound >= 1024 (two 8-bit passes); result always lands in d_out.
 // limit: only the sorted positions below it are stored (top-K calls); kFrzNoLimit sorts the whole list.
 frz_status frz_launch_sort_by_score_dev(const FrzMatchDev* d_in, FrzMatchDev* d_tmp, FrzMatchDev* d_out,
-                                        const unsigned long long* n_ptr, uint32_t score_bound, FrzWorkspace& ws,
+                                        const unsigned long long* n_ptr, uint32_t score_bound, FrzSortScratch& ss,
                                         cudaStream_t stream, FrzLaunchStats* st, uint32_t limit = kFrzNoLimit);
-size_t frz_sort_hist_words();
-frz_status frz_sort_hist_alloc(uint32_t** out);
-const uint32_t* frz_sort_digit_base(const FrzWorkspace& ws);
+frz_status frz_sort_hist_alloc(FrzDevArray<uint32_t>& out);
+const uint32_t* frz_sort_digit_base(const FrzSortScratch& ss);
 int frz_sort_single_pass_bins(uint32_t score_bound);   // bins of the single-pass sort for this bound, 0 = two passes
 // The fused single-pass sort: the scoring kernels build the histogram (frz_launch_sw with `hist`), so the sort is a scan
 // and a block-per-segment scatter.  prepare: sizes and zeroes the histogram for lists of up to n_cap matches whose scores
 // are below score_bound (< 1024).  The sort reads the count at *n_ptr and leaves the histogram zeroed for the next call.
-frz_status frz_sort_fused_prepare(FrzWorkspace& ws, uint64_t n_cap, uint32_t score_bound, cudaStream_t stream, FrzScoreHist* out);
+frz_status frz_sort_fused_prepare(FrzSortScratch& ss, uint64_t n_cap, uint32_t score_bound, cudaStream_t stream, FrzScoreHist* out);
 frz_status frz_launch_sort_fused(const FrzMatchDev* d_in, FrzMatchDev* d_out, const unsigned long long* n_ptr, const FrzScoreHist& hist,
-                                 FrzWorkspace& ws, cudaStream_t stream, FrzLaunchStats* st, uint32_t limit = kFrzNoLimit);
+                                 FrzSortScratch& ss, cudaStream_t stream, FrzLaunchStats* st, uint32_t limit = kFrzNoLimit);
 
 // k-way merge of per-shard runs (host.cu) with caller-owned scratch — one per concurrent user (parallel.cu: one per rank)
 #define FRZ_MERGE_MAX_RUNS 64
 struct FrzMergeScratch {
-    uint32_t* hist = nullptr;      // sort scratch of the concatenate-and-sort fallback
-    uint32_t* tables = nullptr;    // gt / pos0 tables of the scatter merge
-    FrzMatchDev* cat = nullptr;
-    FrzMatchDev* tmp = nullptr;
-    unsigned long long* d_total = nullptr;
-    uint64_t cap = 0;
-    int device = -1;
-    void release();
+    FrzSortScratch sort;                      // of the concatenate-and-sort fallback
+    FrzDevArray<uint32_t> tables;             // gt / pos0 tables of the scatter merge
+    FrzDevArray<FrzMatchDev> cat;
+    FrzDevArray<FrzMatchDev> tmp;
+    FrzDevArray<unsigned long long> d_total;
 };
 frz_status frz_merge_runs_ex(FrzMergeScratch& ms, const FrzMatchDev* runs, uint64_t run_stride, const uint64_t* run_counts_host,
                              int n_runs, uint8_t sort, uint32_t score_bound, FrzMatchDev* d_out, cudaStream_t stream);

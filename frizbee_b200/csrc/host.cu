@@ -237,7 +237,7 @@ extern "C" frz_status frz_corpus_create_device(const uint8_t* d_bytes, const uin
     // the corpus is complete on return: matches run on other streams, and the caller may free the inputs
     if (s == FRZ_OK && cudaStreamSynchronize((cudaStream_t)stream) != cudaSuccess)
         s = frz_fail(FRZ_ERR_CUDA, "pack failed: %s", cudaGetErrorString(cudaGetLastError()));
-    if (s != FRZ_OK) { c->st.release(); return s; }
+    if (s != FRZ_OK) return s;
     *out = c.release();
     return FRZ_OK;
 }
@@ -256,8 +256,7 @@ extern "C" frz_status frz_corpus_create_arrow(const uint8_t* bytes, const void* 
     frz_status s = frz_ingest_host(ing, bytes, offsets, offset_width, n, stream, &c->st);
     if (s == FRZ_OK && cudaStreamSynchronize(stream) != cudaSuccess)
         s = frz_fail(FRZ_ERR_CUDA, "pack failed: %s", cudaGetErrorString(cudaGetLastError()));
-    ing.release();
-    if (s != FRZ_OK) { c->st.release(); return s; }
+    if (s != FRZ_OK) return s;
     *out = c.release();
     return FRZ_OK;
 }
@@ -273,7 +272,7 @@ extern "C" frz_status frz_corpus_append(frz_corpus* c, const uint8_t* bytes, con
     if (offset_width != 4 && offset_width != 8) return frz_fail(FRZ_ERR_INVALID_ARG, "offset_width must be 4 or 8");
     if (n_new == 0) return FRZ_OK;
     FRZ_TRY(ensure_device(c->st.device));
-    if (!c->ingest) c->ingest = new FrzIngest();
+    if (!c->ingest) c->ingest = std::make_unique<FrzIngest>();
     cudaStream_t stream = nullptr;
     FRZ_TRY(frz_append_host(*c->ingest, bytes, offsets, offset_width, n_new, stream, &c->st));
     FRZ_CUDA_TRY(cudaStreamSynchronize(stream));
@@ -308,7 +307,7 @@ extern "C" frz_status frz_corpus_debug_image(const frz_corpus* c, void* tile_bas
     const uint64_t slots = (uint64_t)s.n_tiles * FRZ_TILE;
     const uint64_t need[6] = {(uint64_t)s.n_tiles * sizeof(uint64_t), (uint64_t)s.n_tiles * FRZ_GROUPS_PER_TILE * sizeof(FrzGroupDesc),
                               slots * sizeof(uint32_t), slots * sizeof(uint16_t), slots * sizeof(uint2), s.total_units * sizeof(uint4)};
-    const void* src[6] = {s.tile_base, s.groups, s.slot_meta, s.slot_of, s.slot_sig, s.data};
+    const void* src[6] = {s.tile_base.get(), s.groups.get(), s.slot_meta.get(), s.slot_of.get(), s.slot_sig.get(), s.data.get()};
     void* dst[6] = {tile_base, groups, slot_meta, slot_of, slot_sig, units};
     int given = 0;
     for (void* d : dst) given += d != nullptr;
@@ -326,13 +325,7 @@ extern "C" frz_status frz_corpus_debug_image(const frz_corpus* c, void* tile_bas
         if (need[i]) FRZ_CUDA_TRY(cudaMemcpy(dst[i], src[i], need[i], cudaMemcpyDeviceToHost));
     return FRZ_OK;
 }
-extern "C" void frz_corpus_destroy(frz_corpus* c) {
-    if (!c) return;
-    cudaSetDevice(c->st.device);
-    c->st.release();
-    if (c->ingest) { c->ingest->release(); delete c->ingest; }
-    delete c;
-}
+extern "C" void frz_corpus_destroy(frz_corpus* c) { delete c; }
 
 // --------------------------------------------------------------------------------- matcher
 
@@ -629,25 +622,6 @@ frz_status compile_pattern(const OwnedPattern& src, const frz_config& mcfg, bool
 
 }  // namespace
 
-void FrzWorkspace::release() {
-    if (device >= 0) cudaSetDevice(device);
-    cudaFree(counters);
-    cudaFree(stream_total); stream_total = nullptr;
-    if (h_counters) cudaFreeHost(h_counters);
-    for (auto& s : survivors) { cudaFree(s); s = nullptr; }
-    cudaFree(surv_bitmap); cudaFree(word_prefix); surv_bitmap = nullptr; word_prefix = nullptr;
-    cudaFree(tile_count); cudaFree(tile_out_base); cudaFree(matches_a); cudaFree(matches_b); cudaFree(sort_hist); cudaFree(cand_list);
-    for (auto& e : ev) { if (e) cudaEventDestroy(e); e = nullptr; }
-    if (table_ev) cudaEventDestroy(table_ev);
-    table_ev = nullptr;
-    counters = nullptr; h_counters = nullptr; tile_count = nullptr; tile_out_base = nullptr; matches_a = matches_b = nullptr;
-    sort_hist = nullptr; cand_list = nullptr;
-    cudaFree(retain_cnt); cudaFree(retain_base); cudaFree(retain_keep); retain_cnt = nullptr; retain_base = nullptr; retain_keep = nullptr; retain_cap = 0;
-    cudaFree(unicode_scratch); unicode_scratch = nullptr; unicode_scratch_cap = 0;
-    cudaFree(fused_hist); fused_hist = nullptr; fused_hist_cap = fused_clean_words = 0; fused_hist_dirty = false;
-    survivor_cap = match_cap = sort_hist_cap = cand_cap = 0; tiles_cap = 0; device = -1;
-}
-
 struct frz_matcher {
     frz_config config;
     std::vector<OwnedPattern> raw;
@@ -656,33 +630,19 @@ struct frz_matcher {
     // end-to-end (host in / host out) staging arena, grow-only: raw Arrow buffers + a reusable packed corpus
     FrzIngest e2e_ingest;     // staging arena + copy stream of frz_match_list_host*
     frz_corpus e2e_corpus;
-    FrzMatchDev* multi_a = nullptr;   // multi-pattern candidate ping-pong
-    FrzMatchDev* multi_b = nullptr;
-    uint64_t multi_cap = 0;
     float last_ms[4] = {0, 0, 0, 0};
     uint64_t last_launches = 0;
     // shard path: the match count is known after the tile scan, long before the scores; it is published there so
     // that the count exchange of match_list_parallel overlaps the Smith-Waterman and sort kernels
     uint64_t* early_count_dst = nullptr;   // device destination of the count (set for the duration of a shard call)
-    cudaEvent_t count_ev = nullptr;        // recorded once the count is in early_count_dst
+    FrzEvent count_ev;                     // recorded once the count is in early_count_dst
     bool count_published = false;
     bool timings_pending = false;
     uint64_t epoch = 0;                    // identity of the compiled patterns (clones made for another epoch are stale)
     int last_sort_bins = 0;                // bins of the single-pass score sort of the last call (0: none / two passes)
-    // the long needles' FrzNeedleTab, in pattern order, on ntab_device for the patterns of ntab_epoch
-    FrzNeedleTab* ntab = nullptr;
-    int ntab_device = -1;
+    // the long needles' FrzNeedleTab, in pattern order, for the patterns of ntab_epoch
+    FrzDevArray<FrzNeedleTab> ntab;
     uint64_t ntab_epoch = 0;
-    ~frz_matcher() {
-        if (ntab) { cudaSetDevice(ntab_device); cudaFree(ntab); }
-        if (ws.device >= 0) { cudaSetDevice(ws.device); cudaFree(multi_a); cudaFree(multi_b); if (count_ev) cudaEventDestroy(count_ev); }
-        if (e2e_ingest.d_bytes || e2e_ingest.copy_stream || e2e_corpus.st.data) {
-            cudaSetDevice(e2e_corpus.st.device);
-            e2e_ingest.release();
-            e2e_corpus.st.release();
-        }
-        ws.release();
-    }
 };
 
 namespace {
@@ -773,10 +733,12 @@ extern "C" frz_status frz_matcher_clone(const frz_matcher* src, frz_matcher** ou
 }
 uint64_t frz_matcher_epoch(const frz_matcher* m) { return m ? m->epoch : 0; }
 uint8_t frz_matcher_sort(const frz_matcher* m) { return m ? m->config.sort : 0; }
-cudaEvent_t frz_matcher_table_event(const frz_matcher* m) { return (m && m->last_sort_bins && m->ws.table_ev_recorded) ? m->ws.table_ev : nullptr; }
+cudaEvent_t frz_matcher_table_event(const frz_matcher* m) {
+    return (m && m->last_sort_bins && m->ws.sort.table_ev_recorded) ? m->ws.sort.table_ev.get() : nullptr;
+}
 const uint32_t* frz_matcher_last_sort_table(const frz_matcher* m, int* bins) {
     if (bins) *bins = m ? m->last_sort_bins : 0;
-    return (m && m->last_sort_bins) ? frz_sort_digit_base(m->ws) : nullptr;
+    return (m && m->last_sort_bins) ? frz_sort_digit_base(m->ws.sort) : nullptr;
 }
 
 extern "C" void frz_matcher_destroy(frz_matcher* m) { delete m; }
@@ -796,7 +758,7 @@ extern "C" frz_status frz_matcher_last_timings(const frz_matcher* mc, float* ms4
     if (!m) return frz_fail(FRZ_ERR_INVALID_ARG, "null matcher");
     if (m->timings_pending && m->ws.device >= 0) {
         cudaSetDevice(m->ws.device);
-        cudaEventSynchronize(m->ws.ev[3]);
+        cudaEventSynchronize(m->ws.ev[3].get());
         FrzLaunchStats st;
         st.launches = m->last_launches;
         collect_timings(m, st);
@@ -910,60 +872,34 @@ __global__ void __launch_bounds__(1024) k_scan_blocks(const uint32_t* cnt, uint6
 
 frz_status ensure_workspace(frz_matcher* m, const FrzCorpusStorage& cs, uint64_t survivor_cap) {
     FrzWorkspace& ws = m->ws;
-    if (ws.device != cs.device) {
-        if (ws.device >= 0) { cudaSetDevice(ws.device); cudaFree(m->multi_a); cudaFree(m->multi_b); m->multi_a = m->multi_b = nullptr; m->multi_cap = 0; }
-        ws.release();
+    if (ws.device != cs.device) {   // all or nothing: a failed set-up leaves an empty workspace, redone by the next call
+        ws = FrzWorkspace();         // the old device's buffers go first
         FRZ_CUDA_TRY(cudaSetDevice(cs.device));
-        ws.device = cs.device;
-        FRZ_CUDA_TRY(cudaMalloc(&ws.counters, sizeof(FrzCounters)));
-        FRZ_CUDA_TRY(cudaMalloc(&ws.stream_total, 2 * sizeof(unsigned long long)));   // [0] tile-scan carry, [1] spare count slot
-        FRZ_CUDA_TRY(cudaMallocHost(&ws.h_counters, sizeof(FrzCounters)));
-        for (auto& e : ws.ev) FRZ_CUDA_TRY(cudaEventCreate(&e));
-        FRZ_CUDA_TRY(cudaEventCreateWithFlags(&ws.table_ev, cudaEventDisableTiming));
-        FRZ_TRY(frz_sort_hist_alloc(&ws.sort_hist));
-        ws.sort_hist_cap = frz_sort_hist_words();
+        FrzWorkspace fresh;
+        fresh.device = cs.device;
+        FRZ_TRY(fresh.counters.reserve(1));
+        FRZ_TRY(fresh.stream_total.reserve(2));
+        FRZ_TRY(fresh.h_counters.reserve(1));
+        for (auto& e : fresh.ev) FRZ_TRY(frz_event_create(e, cudaEventDefault));
+        FRZ_TRY(frz_event_create(fresh.sort.table_ev, cudaEventDisableTiming));
+        FRZ_TRY(frz_sort_hist_alloc(fresh.sort.hist));
+        ws = std::move(fresh);
     }
-    if (ws.tiles_cap < cs.n_tiles) {
-        cudaFree(ws.tile_count); cudaFree(ws.tile_out_base); cudaFree(ws.surv_bitmap); cudaFree(ws.word_prefix);
-        ws.tile_count = nullptr; ws.tile_out_base = nullptr; ws.surv_bitmap = nullptr; ws.word_prefix = nullptr; ws.tiles_cap = 0;
-        FRZ_CUDA_TRY(cudaMalloc(&ws.surv_bitmap, (size_t)cs.n_tiles * 32 * sizeof(uint32_t)));
-        FRZ_CUDA_TRY(cudaMalloc(&ws.word_prefix, (size_t)cs.n_tiles * 32 * sizeof(uint16_t)));
-        FRZ_CUDA_TRY(cudaMalloc(&ws.tile_count, (size_t)cs.n_tiles * sizeof(uint32_t)));
-        FRZ_CUDA_TRY(cudaMalloc(&ws.tile_out_base, (size_t)cs.n_tiles * sizeof(uint64_t)));
-        ws.tiles_cap = cs.n_tiles;
-    }
-    if (ws.survivor_cap < survivor_cap) {
-        for (auto& s : ws.survivors) { cudaFree(s); s = nullptr; }
-        ws.survivor_cap = 0;
-        for (auto& s : ws.survivors) FRZ_CUDA_TRY(cudaMalloc(&s, (size_t)survivor_cap * sizeof(FrzSurvivor)));
-        ws.survivor_cap = survivor_cap;
-    }
-    if (ws.cand_cap < std::max<uint64_t>(cs.n, 1)) {   // worst case: every haystack passes the signature test
-        cudaFree(ws.cand_list); ws.cand_list = nullptr; ws.cand_cap = 0;
-        const uint64_t want = std::max<uint64_t>(cs.n, 1);
-        FRZ_CUDA_TRY(cudaMalloc(&ws.cand_list, (size_t)want * 16));
-        ws.cand_cap = want;
-    }
-    if (ws.match_cap < cs.n) {
-        cudaFree(ws.matches_a); cudaFree(ws.matches_b);
-        ws.matches_a = ws.matches_b = nullptr; ws.match_cap = 0;
-        FRZ_CUDA_TRY(cudaMalloc(&ws.matches_a, (size_t)std::max<uint64_t>(cs.n, 1) * sizeof(FrzMatchDev)));
-        FRZ_CUDA_TRY(cudaMalloc(&ws.matches_b, (size_t)std::max<uint64_t>(cs.n, 1) * sizeof(FrzMatchDev)));
-        ws.match_cap = cs.n;
-    }
+    FRZ_TRY(ws.surv_bitmap.reserve((size_t)cs.n_tiles * 32));
+    FRZ_TRY(ws.word_prefix.reserve((size_t)cs.n_tiles * 32));
+    FRZ_TRY(ws.tile_count.reserve(cs.n_tiles));
+    FRZ_TRY(ws.tile_out_base.reserve(cs.n_tiles));
+    for (auto& s : ws.survivors) FRZ_TRY(s.reserve(survivor_cap));
+    FRZ_TRY(ws.cand_list.reserve(std::max<uint64_t>(cs.n, 1)));   // worst case: every haystack passes the signature test
+    FRZ_TRY(ws.matches_a.reserve(cs.n, std::max<uint64_t>(cs.n, 1)));
+    FRZ_TRY(ws.matches_b.reserve(cs.n, std::max<uint64_t>(cs.n, 1)));
     return FRZ_OK;
 }
 
 // multi-pattern candidate ping-pong / two-pass sort scratch: grow-only, always >= n entries after this call
 frz_status ensure_multi_buffers(frz_matcher* m, uint64_t n) {
-    if (m->multi_a && m->multi_b && m->multi_cap >= std::max<uint64_t>(n, 1)) return FRZ_OK;
-    cudaFree(m->multi_a); cudaFree(m->multi_b);
-    m->multi_a = m->multi_b = nullptr; m->multi_cap = 0;
-    const uint64_t want = std::max<uint64_t>(n, 1);
-    FRZ_CUDA_TRY(cudaMalloc(&m->multi_a, (size_t)want * sizeof(FrzMatchDev)));
-    FRZ_CUDA_TRY(cudaMalloc(&m->multi_b, (size_t)want * sizeof(FrzMatchDev)));
-    m->multi_cap = want;
-    return FRZ_OK;
+    FRZ_TRY(m->ws.multi_a.reserve(std::max<uint64_t>(n, 1)));
+    return m->ws.multi_b.reserve(std::max<uint64_t>(n, 1));
 }
 
 uint64_t initial_survivor_cap(const FrzCorpusStorage& cs, const FrzPatternDev& d) {
@@ -976,22 +912,15 @@ uint64_t initial_survivor_cap(const FrzCorpusStorage& cs, const FrzPatternDev& d
 frz_status needle_table(frz_matcher* m, const Compiled& c, const FrzNeedleTab** out) {
     *out = nullptr;
     if (!c.is_long()) return FRZ_OK;
-    if (m->ntab_device != m->ws.device || m->ntab_epoch != m->epoch) {
-        if (m->ntab) {
-            cudaSetDevice(m->ntab_device);
-            cudaFree(m->ntab);
-            m->ntab = nullptr;
-            FRZ_CUDA_TRY(cudaSetDevice(m->ws.device));
-        }
-        m->ntab_device = -1;
+    if (!m->ntab.get() || m->ntab.device() != m->ws.device || m->ntab_epoch != m->epoch) {
+        m->ntab.reset();
+        m->ntab_epoch = 0;
         size_t k = 0;
         for (const Compiled& p : m->compiled) k += p.is_long() ? 1 : 0;
-        FRZ_CUDA_TRY(cudaMalloc(&m->ntab, k * sizeof(FrzNeedleTab)));
-        m->ntab_device = m->ws.device;   // (freed by the destructor or the next upload even when a copy below fails)
-        m->ntab_epoch = 0;
+        FRZ_TRY(m->ntab.reserve(k));
         k = 0;
         for (const Compiled& p : m->compiled)
-            if (p.is_long()) FRZ_CUDA_TRY(cudaMemcpy(m->ntab + k++, p.tab.get(), sizeof(FrzNeedleTab), cudaMemcpyHostToDevice));
+            if (p.is_long()) FRZ_CUDA_TRY(cudaMemcpy(m->ntab.get() + k++, p.tab.get(), sizeof(FrzNeedleTab), cudaMemcpyHostToDevice));
         m->ntab_epoch = m->epoch;
     }
     size_t k = 0;
@@ -999,7 +928,7 @@ frz_status needle_table(frz_matcher* m, const Compiled& c, const FrzNeedleTab** 
         if (&p == &c) break;
         k += p.is_long() ? 1 : 0;
     }
-    *out = m->ntab + k;
+    *out = m->ntab.get() + k;
     return FRZ_OK;
 }
 
@@ -1011,21 +940,21 @@ frz_status run_pattern(frz_matcher* m, const FrzCorpusStorage& cs, const Compile
                        const FrzScoreHist& hist = FrzScoreHist()) {
     FrzWorkspace& ws = m->ws;
     const FrzCorpusView cv = cs.view();
-    uint64_t cap = std::max(ws.survivor_cap, initial_survivor_cap(cs, c.dev));
+    uint64_t cap = std::max(ws.survivor_cap(), initial_survivor_cap(cs, c.dev));
     FRZ_TRY(ensure_workspace(m, cs, cap));
     const FrzNeedleTab* ntab = nullptr;
     FRZ_TRY(needle_table(m, c, &ntab));
-    FRZ_CUDA_TRY(cudaMemsetAsync(ws.counters, 0, sizeof(FrzCounters), stream));
-    if (record_events) { cudaEventRecord(ws.ev[0], stream); ws.ev_rec[0] = true; }
+    FRZ_CUDA_TRY(cudaMemsetAsync(ws.counters.get(), 0, sizeof(FrzCounters), stream));
+    if (record_events) { cudaEventRecord(ws.ev[0].get(), stream); ws.ev_rec[0] = true; }
     if (c.unicode) FRZ_TRY(frz_launch_unicode(cv, c.dev, c.un, c.usc, cand_list, n_cand, index_offset, ws, stream, st));
     else if (cand_list) FRZ_TRY(frz_launch_prefilter_list(cv, c.dev, cand_list, n_cand, index_offset, ws, stream, st, ntab));
     else FRZ_TRY(frz_launch_prefilter(cv, c.dev, ws, stream, st, ntab));
     FRZ_TRY(frz_launch_tile_scan(cv, ws, stream, st));
-    if (record_events) { cudaEventRecord(ws.ev[1], stream); ws.ev_rec[1] = true; }
+    if (record_events) { cudaEventRecord(ws.ev[1].get(), stream); ws.ev_rec[1] = true; }
     if (m->early_count_dst && !cand_list && !cand_bitmap && m->compiled.size() == 1) {
         // single pattern: every survivor becomes exactly one match, so the scan total is the final count
-        FRZ_CUDA_TRY(cudaMemcpyAsync(m->early_count_dst, &ws.counters->total, sizeof(uint64_t), cudaMemcpyDeviceToDevice, stream));
-        FRZ_CUDA_TRY(cudaEventRecord(m->count_ev, stream));
+        FRZ_CUDA_TRY(cudaMemcpyAsync(m->early_count_dst, &ws.counters.get()->total, sizeof(uint64_t), cudaMemcpyDeviceToDevice, stream));
+        FRZ_CUDA_TRY(cudaEventRecord(m->count_ev.get(), stream));
         m->count_published = true;
     }
     // A survivor-list overflow (lists are sized by a heuristic unless the pattern can match everything)
@@ -1038,7 +967,7 @@ frz_status run_pattern(frz_matcher* m, const FrzCorpusStorage& cs, const Compile
     } else {
         FRZ_TRY(frz_launch_sw(cv, c.dev, index_offset, reversed, ws, d_out, stream, st, hist, ntab));
     }
-    if (record_events) { cudaEventRecord(ws.ev[2], stream); ws.ev_rec[2] = true; }
+    if (record_events) { cudaEventRecord(ws.ev[2].get(), stream); ws.ev_rec[2] = true; }
     return FRZ_OK;
 }
 
@@ -1046,9 +975,9 @@ constexpr frz_status kRetryOverflow = (frz_status)100;
 
 frz_status read_counters(frz_matcher* m, cudaStream_t stream) {
     FrzWorkspace& ws = m->ws;
-    FRZ_CUDA_TRY(cudaMemcpyAsync(ws.h_counters, ws.counters, sizeof(FrzCounters), cudaMemcpyDeviceToHost, stream));
+    FRZ_CUDA_TRY(cudaMemcpyAsync(ws.h_counters.get(), ws.counters.get(), sizeof(FrzCounters), cudaMemcpyDeviceToHost, stream));
     FRZ_CUDA_TRY(cudaStreamSynchronize(stream));
-    if (ws.h_counters->error & FRZ_DEVERR_SURVIVOR_OVERFLOW) return kRetryOverflow;
+    if (ws.h_counters.get()->error & FRZ_DEVERR_SURVIVOR_OVERFLOW) return kRetryOverflow;
     return FRZ_OK;
 }
 
@@ -1072,23 +1001,23 @@ frz_status match_into_device(frz_matcher* m, const FrzCorpusStorage& cs, uint32_
     *score_bound = 0;
     if (pats.empty()) {  // CompiledPatterns::Empty (src/matcher/mod.rs:380-383)
         FRZ_TRY(ensure_workspace(m, cs, 1));
-        FRZ_CUDA_TRY(cudaMemsetAsync(ws.counters, 0, sizeof(FrzCounters), stream));
-        k_fill_all<<<grid_for(cs.n, 256), 256, 0, stream>>>(ws.matches_a, cs.n, index_offset, ws.counters);
+        FRZ_CUDA_TRY(cudaMemsetAsync(ws.counters.get(), 0, sizeof(FrzCounters), stream));
+        k_fill_all<<<grid_for(cs.n, 256), 256, 0, stream>>>(ws.matches_a.get(), cs.n, index_offset, ws.counters.get());
         st->launches++;
         if (final_reversed) {
-            k_reverse<<<grid_for(cs.n, 256), 256, 0, stream>>>(ws.matches_a, ws.matches_b, &ws.counters->total);
+            k_reverse<<<grid_for(cs.n, 256), 256, 0, stream>>>(ws.matches_a.get(), ws.matches_b.get(), &ws.counters.get()->total);
             st->launches++;
-            *d_result = ws.matches_b;
-        } else *d_result = ws.matches_a;
+            *d_result = ws.matches_b.get();
+        } else *d_result = ws.matches_a.get();
         FRZ_CUDA_TRY(cudaGetLastError());
         return FRZ_OK;
     }
     if (pats.size() == 1 && !pats[0].negated) {  // CompiledPatterns::Single
         FRZ_TRY(ensure_workspace(m, cs, initial_survivor_cap(cs, pats[0].dev)));
-        FrzMatchDev* dst = prefer_out ? prefer_out : ws.matches_a;
+        FrzMatchDev* dst = prefer_out ? prefer_out : ws.matches_a.get();
         FrzScoreHist hist;
         if (score_hist && frz_sort_single_pass_bins(pats[0].score_bound) > 0) {
-            FRZ_TRY(frz_sort_fused_prepare(ws, cs.n, pats[0].score_bound, stream, &hist));
+            FRZ_TRY(frz_sort_fused_prepare(ws.sort, cs.n, pats[0].score_bound, stream, &hist));
             *score_hist = hist;
         }
         FRZ_TRY(run_pattern(m, cs, pats[0], nullptr, index_offset, final_reversed, dst, stream, st, true, nullptr, 0, hist));
@@ -1101,55 +1030,52 @@ frz_status match_into_device(frz_matcher* m, const FrzCorpusStorage& cs, uint32_
     FRZ_TRY(ensure_multi_buffers(m, cs.n));
     int base = -1;
     for (size_t i = 0; i < pats.size(); i++) if (!pats[i].negated) { base = (int)i; break; }
-    FrzMatchDev* cand = m->multi_a;
-    FrzMatchDev* spare = m->multi_b;
+    FrzMatchDev* cand = ws.multi_a.get();
+    FrzMatchDev* spare = ws.multi_b.get();
     uint64_t nc = 0;
     uint64_t bound = 0;
     if (base >= 0) {
         FRZ_TRY(run_pattern(m, cs, pats[base], nullptr, index_offset, false, cand, stream, st, true));
         FRZ_TRY(read_counters(m, stream));
-        nc = ws.h_counters->total;
+        nc = ws.h_counters.get()->total;
         bound = pats[base].score_bound;
     } else {
-        FRZ_CUDA_TRY(cudaMemsetAsync(ws.counters, 0, sizeof(FrzCounters), stream));
-        k_fill_all<<<grid_for(cs.n, 256), 256, 0, stream>>>(cand, cs.n, index_offset, ws.counters);
+        FRZ_CUDA_TRY(cudaMemsetAsync(ws.counters.get(), 0, sizeof(FrzCounters), stream));
+        k_fill_all<<<grid_for(cs.n, 256), 256, 0, stream>>>(cand, cs.n, index_offset, ws.counters.get());
         st->launches++;
         nc = cs.n;
     }
-    if (ws.retain_cap < cs.n) {
-        cudaFree(ws.retain_cnt); cudaFree(ws.retain_base); cudaFree(ws.retain_keep);
-        ws.retain_cnt = nullptr; ws.retain_base = nullptr; ws.retain_keep = nullptr; ws.retain_cap = 0;
+    if (ws.retain_keep.cap() < cs.n) {
         const uint32_t nb_max = (uint32_t)((cs.n + kCompactBlock - 1) / kCompactBlock) + 1;
-        FRZ_CUDA_TRY(cudaMalloc(&ws.retain_cnt, nb_max * sizeof(uint32_t)));
-        FRZ_CUDA_TRY(cudaMalloc(&ws.retain_base, nb_max * sizeof(uint64_t)));
-        FRZ_CUDA_TRY(cudaMalloc(&ws.retain_keep, std::max<uint64_t>(cs.n, 1)));
-        ws.retain_cap = cs.n;
+        FRZ_TRY(ws.retain_cnt.reserve(nb_max));
+        FRZ_TRY(ws.retain_base.reserve(nb_max));
+        FRZ_TRY(ws.retain_keep.reserve(cs.n));
     }
-    uint32_t* d_block_cnt = ws.retain_cnt;
-    uint64_t* d_block_base = ws.retain_base;
-    uint8_t* d_keep = ws.retain_keep;
+    uint32_t* d_block_cnt = ws.retain_cnt.get();
+    uint64_t* d_block_base = ws.retain_base.get();
+    uint8_t* d_keep = ws.retain_keep.get();
     frz_status status = FRZ_OK;
     for (size_t pi = 0; pi < pats.size() && status == FRZ_OK; pi++) {
         if ((int)pi == base || nc == 0) continue;
         status = [&]() -> frz_status {
             // evaluate the pattern on the surviving candidates only; hits land in ws.matches_a, index-ordered,
             // with real indices
-            FRZ_TRY(run_pattern(m, cs, pats[pi], nullptr, index_offset, false, ws.matches_a, stream, st, false, cand, nc));
+            FRZ_TRY(run_pattern(m, cs, pats[pi], nullptr, index_offset, false, ws.matches_a.get(), stream, st, false, cand, nc));
             FRZ_TRY(read_counters(m, stream));
-            const uint64_t nh = ws.h_counters->total;
+            const uint64_t nh = ws.h_counters.get()->total;
             if (pats[pi].negated) {
                 const uint32_t nb = (uint32_t)((nc + kCompactBlock - 1) / kCompactBlock);
-                k_retain_count<<<nb, kCompactBlock, 0, stream>>>(cand, nc, ws.matches_a, nh, d_block_cnt, d_keep);
-                k_scan_blocks<<<1, 1024, 0, stream>>>(d_block_cnt, d_block_base, nb, ws.counters);
+                k_retain_count<<<nb, kCompactBlock, 0, stream>>>(cand, nc, ws.matches_a.get(), nh, d_block_cnt, d_keep);
+                k_scan_blocks<<<1, 1024, 0, stream>>>(d_block_cnt, d_block_base, nb, ws.counters.get());
                 k_retain_scatter<<<nb, kCompactBlock, 0, stream>>>(cand, nc, d_keep, d_block_base, spare);
                 st->launches += 3;
                 FRZ_TRY(read_counters(m, stream));
-                nc = ws.h_counters->total;
+                nc = ws.h_counters.get()->total;
                 std::swap(cand, spare);
             } else {
-                k_combine_hits<<<grid_for(nh, 256), 256, 0, stream>>>(cand, nc, ws.matches_a, nh);
+                k_combine_hits<<<grid_for(nh, 256), 256, 0, stream>>>(cand, nc, ws.matches_a.get(), nh);
                 st->launches++;
-                FRZ_CUDA_TRY(cudaMemcpyAsync(spare, ws.matches_a, nh * sizeof(FrzMatchDev), cudaMemcpyDeviceToDevice, stream));
+                FRZ_CUDA_TRY(cudaMemcpyAsync(spare, ws.matches_a.get(), nh * sizeof(FrzMatchDev), cudaMemcpyDeviceToDevice, stream));
                 std::swap(cand, spare);
                 nc = nh;
                 bound += pats[pi].score_bound;
@@ -1159,16 +1085,16 @@ frz_status match_into_device(frz_matcher* m, const FrzCorpusStorage& cs, uint32_
     }
     FRZ_TRY(status);
     // publish: count → counters.total, list → matches_a (reversed if asked)
-    ws.h_counters->total = nc;
-    FRZ_CUDA_TRY(cudaMemcpyAsync(&ws.counters->total, &ws.h_counters->total, sizeof(unsigned long long), cudaMemcpyHostToDevice, stream));
+    ws.h_counters.get()->total = nc;
+    FRZ_CUDA_TRY(cudaMemcpyAsync(&ws.counters.get()->total, &ws.h_counters.get()->total, sizeof(unsigned long long), cudaMemcpyHostToDevice, stream));
     if (final_reversed) {
-        k_reverse<<<grid_for(nc, 256), 256, 0, stream>>>(cand, ws.matches_a, &ws.counters->total);
+        k_reverse<<<grid_for(nc, 256), 256, 0, stream>>>(cand, ws.matches_a.get(), &ws.counters.get()->total);
         st->launches++;
     } else {
-        FRZ_CUDA_TRY(cudaMemcpyAsync(ws.matches_a, cand, nc * sizeof(FrzMatchDev), cudaMemcpyDeviceToDevice, stream));
+        FRZ_CUDA_TRY(cudaMemcpyAsync(ws.matches_a.get(), cand, nc * sizeof(FrzMatchDev), cudaMemcpyDeviceToDevice, stream));
     }
     FRZ_CUDA_TRY(cudaGetLastError());
-    *d_result = ws.matches_a;
+    *d_result = ws.matches_a.get();
     *score_bound = (uint32_t)std::min<uint64_t>(bound, 0xFFFF);
     return FRZ_OK;
 }
@@ -1200,24 +1126,24 @@ frz_status match_list_device(frz_matcher* m, const FrzCorpusStorage& cs, uint32_
                               will_sort ? &hist : nullptr));
     // `!self.patterns.is_empty() && sort.is_by_score()` (src/matcher/mod.rs:218)
     if (will_sort) {
-        FrzMatchDev* other = final_out ? final_out : (d_list == ws.matches_a ? ws.matches_b : ws.matches_a);
+        FrzMatchDev* other = final_out ? final_out : (d_list == ws.matches_a.get() ? ws.matches_b.get() : ws.matches_a.get());
         // two-pass sort (score bound >= 1024) needs a scratch list of the corpus size: the multi-pattern ping-pong
         // buffer is free at this point (d_list is never multi_a); grow it whenever THIS corpus is larger
         FrzMatchDev* tmp = nullptr;
         if (bound >= 1024) {
             FRZ_TRY(ensure_multi_buffers(m, cs.n));
-            tmp = m->multi_a;
+            tmp = ws.multi_a.get();
         }
-        if (hist.counts) FRZ_TRY(frz_launch_sort_fused(d_list, other, &ws.counters->total, hist, ws, stream, st, limit));
-        else FRZ_TRY(frz_launch_sort_by_score_dev(d_list, tmp, other, &ws.counters->total, bound, ws, stream, st, limit));
+        if (hist.counts) FRZ_TRY(frz_launch_sort_fused(d_list, other, &ws.counters.get()->total, hist, ws.sort, stream, st, limit));
+        else FRZ_TRY(frz_launch_sort_by_score_dev(d_list, tmp, other, &ws.counters.get()->total, bound, ws.sort, stream, st, limit));
         m->last_sort_bins = frz_sort_single_pass_bins(bound);
         d_list = other;
     } else if (final_out && d_list != final_out) {
-        k_copy_n<<<grid_for(std::min<uint64_t>(cs.n, limit), 256), 256, 0, stream>>>(d_list, final_out, &ws.counters->total, limit);
+        k_copy_n<<<grid_for(std::min<uint64_t>(cs.n, limit), 256), 256, 0, stream>>>(d_list, final_out, &ws.counters.get()->total, limit);
         st->launches++;
         d_list = final_out;
     }
-    cudaEventRecord(ws.ev[3], stream);
+    cudaEventRecord(ws.ev[3].get(), stream);
     ws.ev_rec[3] = true;
     *d_result = d_list;
     return FRZ_OK;
@@ -1228,10 +1154,10 @@ void collect_timings(frz_matcher* m, const FrzLaunchStats& st) {
     FrzWorkspace& ws = m->ws;
     float a = 0, b = 0, c = 0, t = 0;
     const bool* r = ws.ev_rec;
-    if (r[0] && r[1] && cudaEventElapsedTime(&a, ws.ev[0], ws.ev[1]) != cudaSuccess) a = 0;
-    if (r[1] && r[2] && cudaEventElapsedTime(&b, ws.ev[1], ws.ev[2]) != cudaSuccess) b = 0;
-    if (r[2] && r[3] && cudaEventElapsedTime(&c, ws.ev[2], ws.ev[3]) != cudaSuccess) c = 0;
-    if (r[0] && r[3] && cudaEventElapsedTime(&t, ws.ev[0], ws.ev[3]) != cudaSuccess) t = 0;
+    if (r[0] && r[1] && cudaEventElapsedTime(&a, ws.ev[0].get(), ws.ev[1].get()) != cudaSuccess) a = 0;
+    if (r[1] && r[2] && cudaEventElapsedTime(&b, ws.ev[1].get(), ws.ev[2].get()) != cudaSuccess) b = 0;
+    if (r[2] && r[3] && cudaEventElapsedTime(&c, ws.ev[2].get(), ws.ev[3].get()) != cudaSuccess) c = 0;
+    if (r[0] && r[3] && cudaEventElapsedTime(&t, ws.ev[0].get(), ws.ev[3].get()) != cudaSuccess) t = 0;
     cudaGetLastError();
     m->last_ms[0] = a; m->last_ms[1] = b; m->last_ms[2] = c; m->last_ms[3] = t;
     m->last_launches = st.launches;
@@ -1240,7 +1166,7 @@ namespace {
 
 frz_status copy_out(frz_matcher* m, FrzMatchDev* d_list, frz_match* out, uint64_t cap, uint64_t* n_out, cudaStream_t stream) {
     FRZ_TRY(read_counters(m, stream));
-    const uint64_t n = m->ws.h_counters->total;
+    const uint64_t n = m->ws.h_counters.get()->total;
     if (n_out) *n_out = n;
     if (n > cap) return frz_fail(FRZ_ERR_CAPACITY, "output capacity %llu < %llu matches", (unsigned long long)cap, (unsigned long long)n);
     if (n) {
@@ -1256,7 +1182,7 @@ frz_status copy_out(frz_matcher* m, FrzMatchDev* d_list, frz_match* out, uint64_
 frz_status copy_out_top(frz_matcher* m, FrzMatchDev* d_list, uint64_t k, frz_match* out, uint64_t* n_out, uint64_t* n_total,
                         cudaStream_t stream) {
     FRZ_TRY(read_counters(m, stream));
-    const uint64_t total = m->ws.h_counters->total;
+    const uint64_t total = m->ws.h_counters.get()->total;
     const uint64_t n = std::min(k, total);
     if (n_out) *n_out = n;
     if (n_total) *n_total = total;
@@ -1354,6 +1280,18 @@ extern "C" frz_status frz_match_list_host_arrow(frz_matcher* m, const uint8_t* b
     return frz_match_list(m, c, out, cap, n_out);
 }
 
+namespace {
+// The matcher's end-to-end staging arena and packed corpus, for `device`: emptied first when they live on another device.
+frz_corpus& e2e_corpus_on(frz_matcher* m, int device) {
+    if (m->e2e_corpus.st.device != device) {
+        m->e2e_ingest = FrzIngest();
+        m->e2e_corpus.st = FrzCorpusStorage();
+        m->e2e_corpus.st.device = device;
+    }
+    return m->e2e_corpus;
+}
+}  // namespace
+
 // The ingest half of the end-to-end call: host Arrow buffers → the matcher's reusable packed corpus (grow-only staging
 // arena, streamed H2D overlapped with the pack kernels; asynchronous on the legacy default stream).
 frz_status frz_matcher_ingest_e2e(frz_matcher* m, const uint8_t* bytes, const void* offsets, int offset_width, uint64_t n, int device,
@@ -1363,14 +1301,7 @@ frz_status frz_matcher_ingest_e2e(frz_matcher* m, const uint8_t* bytes, const vo
     if (n > 0xFFFFFFFFull) return frz_fail(FRZ_ERR_TOO_MANY_ITEMS, "too many items in haystack: %llu", (unsigned long long)n);
     FRZ_TRY(ensure_device(device));
     cudaStream_t stream = nullptr;
-    frz_corpus& c = m->e2e_corpus;
-    if (c.st.device != device && (m->e2e_ingest.d_bytes || m->e2e_ingest.copy_stream || c.st.data)) {  // arena lives on another device
-        cudaSetDevice(c.st.device);
-        m->e2e_ingest.release();
-        c.st.release();
-        FRZ_CUDA_TRY(cudaSetDevice(device));
-    }
-    c.st.device = device;
+    frz_corpus& c = e2e_corpus_on(m, device);
     FRZ_TRY(frz_ingest_host(m->e2e_ingest, bytes, offsets, offset_width, n, stream, &c.st));
     *out = &c;
     return FRZ_OK;
@@ -1390,27 +1321,23 @@ frz_status match_indices_one(const Compiled& c, const frz_corpus* corpus, const 
     const uint32_t threads = (uint32_t)std::min<uint64_t>(n, 1024);
     const int rows = c.unicode ? c.un.n : c.un.nbytes;
     const uint64_t sstride = c.literal ? 1 : (uint64_t)frzi::indices_scratch_elems(rows, c.dev.sw_lanes);
-    uint32_t *d_which = nullptr, *d_idx = nullptr, *d_cnt = nullptr;
-    FrzMatchDev* d_m = nullptr;
-    uint16_t* d_scratch = nullptr;
-    frz_status st = [&]() -> frz_status {
-        FRZ_CUDA_TRY(cudaMalloc(&d_which, n * sizeof(uint32_t)));
-        FRZ_CUDA_TRY(cudaMalloc(&d_idx, n * (uint64_t)stride * sizeof(uint32_t)));
-        FRZ_CUDA_TRY(cudaMalloc(&d_cnt, n * sizeof(uint32_t)));
-        FRZ_CUDA_TRY(cudaMalloc(&d_m, n * sizeof(FrzMatchDev)));
-        FRZ_CUDA_TRY(cudaMalloc(&d_scratch, (uint64_t)threads * sstride * sizeof(uint16_t)));
-        FRZ_CUDA_TRY(cudaMemcpyAsync(d_which, which, n * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
-        FRZ_CUDA_TRY(cudaMemsetAsync(d_m, 0, n * sizeof(FrzMatchDev), stream));
-        FRZ_TRY(frz_launch_match_indices(corpus->st.view(), c.dev, c.un, c.usc, c.unicode, d_which, n, d_m, d_idx, stride, d_cnt,
-                                         d_scratch, sstride, threads, stream));
-        FRZ_CUDA_TRY(cudaMemcpyAsync(out_matches, d_m, n * sizeof(FrzMatchDev), cudaMemcpyDeviceToHost, stream));
-        FRZ_CUDA_TRY(cudaMemcpyAsync(out_indices, d_idx, n * (uint64_t)stride * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
-        FRZ_CUDA_TRY(cudaMemcpyAsync(out_counts, d_cnt, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
-        FRZ_CUDA_TRY(cudaStreamSynchronize(stream));
-        return FRZ_OK;
-    }();
-    cudaFree(d_which); cudaFree(d_idx); cudaFree(d_cnt); cudaFree(d_m); cudaFree(d_scratch);
-    return st;
+    FrzDevArray<uint32_t> d_which, d_idx, d_cnt;
+    FrzDevArray<FrzMatchDev> d_m;
+    FrzDevArray<uint16_t> d_scratch;
+    FRZ_TRY(d_which.reserve(n));
+    FRZ_TRY(d_idx.reserve(n * (uint64_t)stride));
+    FRZ_TRY(d_cnt.reserve(n));
+    FRZ_TRY(d_m.reserve(n));
+    FRZ_TRY(d_scratch.reserve((uint64_t)threads * sstride));
+    FRZ_CUDA_TRY(cudaMemcpyAsync(d_which.get(), which, n * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
+    FRZ_CUDA_TRY(cudaMemsetAsync(d_m.get(), 0, n * sizeof(FrzMatchDev), stream));
+    FRZ_TRY(frz_launch_match_indices(corpus->st.view(), c.dev, c.un, c.usc, c.unicode, d_which.get(), n, d_m.get(), d_idx.get(), stride,
+                                     d_cnt.get(), d_scratch.get(), sstride, threads, stream));
+    FRZ_CUDA_TRY(cudaMemcpyAsync(out_matches, d_m.get(), n * sizeof(FrzMatchDev), cudaMemcpyDeviceToHost, stream));
+    FRZ_CUDA_TRY(cudaMemcpyAsync(out_indices, d_idx.get(), n * (uint64_t)stride * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
+    FRZ_CUDA_TRY(cudaMemcpyAsync(out_counts, d_cnt.get(), n * sizeof(uint32_t), cudaMemcpyDeviceToHost, stream));
+    FRZ_CUDA_TRY(cudaStreamSynchronize(stream));
+    return FRZ_OK;
 }
 }  // namespace
 
@@ -1478,19 +1405,19 @@ frz_status frz_match_shard_device_top(frz_matcher* m, const frz_corpus* shard, u
     FRZ_TRY(ensure_workspace(m, shard->st, std::max<uint64_t>(shard->st.n, 1)));
     // the run can never exceed the shard size; the caller sizes d_out as >= shard length
     if (cap < shard->st.n) return frz_fail(FRZ_ERR_CAPACITY, "d_out must hold the whole shard (%llu)", (unsigned long long)shard->st.n);
-    if (!m->count_ev) FRZ_CUDA_TRY(cudaEventCreateWithFlags(&m->count_ev, cudaEventDisableTiming));
+    if (!m->count_ev) FRZ_TRY(frz_event_create(m->count_ev, cudaEventDisableTiming));
     m->early_count_dst = d_count;
     m->count_published = false;
-    m->ws.arm_table_ev = true;
-    m->ws.table_ev_recorded = false;
+    m->ws.sort.arm_table_ev = true;
+    m->ws.sort.table_ev_recorded = false;
     const frz_status ms = match_list_device(m, shard->st, index_offset, m->config.sort, &d_list, stream, &st, reinterpret_cast<FrzMatchDev*>(d_out),
                                             limit);
     m->early_count_dst = nullptr;
-    m->ws.arm_table_ev = false;
+    m->ws.sort.arm_table_ev = false;
     FRZ_TRY(ms);
     if (!m->count_published) {   // multi-pattern / empty pattern: the count exists only at the end
-        FRZ_CUDA_TRY(cudaMemcpyAsync(d_count, &m->ws.counters->total, sizeof(uint64_t), cudaMemcpyDeviceToDevice, stream));
-        FRZ_CUDA_TRY(cudaEventRecord(m->count_ev, stream));
+        FRZ_CUDA_TRY(cudaMemcpyAsync(d_count, &m->ws.counters.get()->total, sizeof(uint64_t), cudaMemcpyDeviceToDevice, stream));
+        FRZ_CUDA_TRY(cudaEventRecord(m->count_ev.get(), stream));
     }
     m->last_launches = st.launches;
     m->timings_pending = true;   // events were recorded; frz_matcher_last_timings reads them once the stream is idle
@@ -1502,7 +1429,7 @@ frz_status frz_match_shard_device_top(frz_matcher* m, const frz_corpus* shard, u
 extern "C" frz_status frz_matcher_wait_count(frz_matcher* m, void* stream) {
     if (!m) return frz_fail(FRZ_ERR_INVALID_ARG, "null matcher");
     if (!m->count_ev) return frz_fail(FRZ_ERR_INVALID_ARG, "no shard call has been made on this matcher");
-    FRZ_CUDA_TRY(cudaStreamWaitEvent((cudaStream_t)stream, m->count_ev, 0));
+    FRZ_CUDA_TRY(cudaStreamWaitEvent((cudaStream_t)stream, m->count_ev.get(), 0));
     return FRZ_OK;
 }
 
@@ -1538,14 +1465,14 @@ frz_status streamed_range(StreamedCtx& x, uint32_t t0, uint32_t t1, bool last) {
     cv.n = std::min<uint64_t>(cs.n, (uint64_t)t1 * FRZ_TILE) - (uint64_t)t0 * FRZ_TILE;
     cv.n_tiles = t1 - t0;
     const uint32_t off = x.index_offset + t0 * FRZ_TILE;
-    FRZ_CUDA_TRY(cudaMemsetAsync(ws.counters, 0, sizeof(FrzCounters), x.stream));
+    FRZ_CUDA_TRY(cudaMemsetAsync(ws.counters.get(), 0, sizeof(FrzCounters), x.stream));
     FRZ_TRY(frz_launch_prefilter(cv, x.c->dev, ws, x.stream, x.st, x.ntab));
-    FRZ_TRY(frz_launch_tile_scan(cv, ws, x.stream, x.st, ws.stream_total));
+    FRZ_TRY(frz_launch_tile_scan(cv, ws, x.stream, x.st, ws.stream_total.get()));
     if (last) {
-        cudaEventRecord(ws.ev[1], x.stream); ws.ev_rec[1] = true;
+        cudaEventRecord(ws.ev[1].get(), x.stream); ws.ev_rec[1] = true;
         if (m->early_count_dst) {   // the running count is final: publish it before the last range is scored
-            FRZ_CUDA_TRY(cudaMemcpyAsync(m->early_count_dst, &ws.counters->total, sizeof(uint64_t), cudaMemcpyDeviceToDevice, x.stream));
-            FRZ_CUDA_TRY(cudaEventRecord(m->count_ev, x.stream));
+            FRZ_CUDA_TRY(cudaMemcpyAsync(m->early_count_dst, &ws.counters.get()->total, sizeof(uint64_t), cudaMemcpyDeviceToDevice, x.stream));
+            FRZ_CUDA_TRY(cudaEventRecord(m->count_ev.get(), x.stream));
             m->count_published = true;
         }
     }
@@ -1595,56 +1522,49 @@ frz_status match_streamed_impl(frz_matcher* m, const uint8_t* bytes, const void*
                                uint32_t index_offset, FrzMatchDev* d_out, uint64_t* d_count, cudaStream_t stream, FrzMatchDev** d_result) {
     const uint8_t sort = m->config.sort;
     FRZ_TRY(ensure_device(device));
-    frz_corpus& c = m->e2e_corpus;
-    if (c.st.device != device && (m->e2e_ingest.d_bytes || m->e2e_ingest.copy_stream || c.st.data)) {  // arena lives on another device
-        cudaSetDevice(c.st.device);
-        m->e2e_ingest.release();
-        c.st.release();
-        FRZ_CUDA_TRY(cudaSetDevice(device));
-    }
-    c.st.device = device;
+    frz_corpus& c = e2e_corpus_on(m, device);
     c.st.n = n;
     c.st.n_tiles = (uint32_t)((n + FRZ_TILE - 1) / FRZ_TILE);
     FrzWorkspace& ws = m->ws;
     FRZ_TRY(ensure_workspace(m, c.st, std::max<uint64_t>(n, 1)));   // nobody reads the overflow flag back: worst-case lists
-    if (!m->count_ev) FRZ_CUDA_TRY(cudaEventCreateWithFlags(&m->count_ev, cudaEventDisableTiming));
+    if (!m->count_ev) FRZ_TRY(frz_event_create(m->count_ev, cudaEventDisableTiming));
     const Compiled& pat = m->compiled[0];
     const bool will_sort = sort == FRZ_SORT_SCORE_THEN_INDEX_ASC;
-    FrzMatchDev* final_out = d_out ? d_out : ws.matches_b;
-    if (!d_count) d_count = reinterpret_cast<uint64_t*>(ws.stream_total + 1);
+    FrzMatchDev* final_out = d_out ? d_out : ws.matches_b.get();
+    if (!d_count) d_count = reinterpret_cast<uint64_t*>(ws.stream_total.get() + 1);
     if (d_result) *d_result = final_out;
     FrzLaunchStats st;
     for (bool& f : ws.ev_rec) f = false;
     m->last_sort_bins = 0;
     m->early_count_dst = d_count;
     m->count_published = false;
-    ws.arm_table_ev = true;
-    ws.table_ev_recorded = false;
+    ws.sort.arm_table_ev = true;
+    ws.sort.table_ev_recorded = false;
     StreamedCtx x;
-    x.m = m; x.c = &pat; x.index_offset = index_offset; x.dst = will_sort ? ws.matches_a : final_out; x.stream = stream; x.st = &st;
+    x.m = m; x.c = &pat; x.index_offset = index_offset; x.dst = will_sort ? ws.matches_a.get() : final_out; x.stream = stream; x.st = &st;
     FRZ_TRY(needle_table(m, pat, &x.ntab));   // a synchronous upload, so before the first H2D chunk
     x.pending_t0 = 0; x.chunks_pending = 0;
     x.group = 4;   // a range per four H2D chunks (about 1/8 of the list): the tail after the last chunk is one range + the sort
     const frz_status ms = [&]() -> frz_status {
-        FRZ_CUDA_TRY(cudaMemsetAsync(ws.stream_total, 0, sizeof(unsigned long long), stream));
-        cudaEventRecord(ws.ev[0], stream); ws.ev_rec[0] = true;
+        FRZ_CUDA_TRY(cudaMemsetAsync(ws.stream_total.get(), 0, sizeof(unsigned long long), stream));
+        cudaEventRecord(ws.ev[0].get(), stream); ws.ev_rec[0] = true;
         FRZ_TRY(frz_ingest_host(m->e2e_ingest, bytes, offsets, offset_width, n, stream, &c.st, streamed_after_chunk, &x));
-        cudaEventRecord(ws.ev[2], stream); ws.ev_rec[2] = true;
+        cudaEventRecord(ws.ev[2].get(), stream); ws.ev_rec[2] = true;
         if (will_sort) {
             FrzMatchDev* tmp = nullptr;
-            if (pat.score_bound >= 1024) { FRZ_TRY(ensure_multi_buffers(m, n)); tmp = m->multi_a; }
-            FRZ_TRY(frz_launch_sort_by_score_dev(ws.matches_a, tmp, final_out, &ws.counters->total, pat.score_bound, ws, stream, &st));
+            if (pat.score_bound >= 1024) { FRZ_TRY(ensure_multi_buffers(m, n)); tmp = ws.multi_a.get(); }
+            FRZ_TRY(frz_launch_sort_by_score_dev(ws.matches_a.get(), tmp, final_out, &ws.counters.get()->total, pat.score_bound, ws.sort, stream, &st));
             m->last_sort_bins = frz_sort_single_pass_bins(pat.score_bound);
         }
-        cudaEventRecord(ws.ev[3], stream); ws.ev_rec[3] = true;
+        cudaEventRecord(ws.ev[3].get(), stream); ws.ev_rec[3] = true;
         return FRZ_OK;
     }();
     m->early_count_dst = nullptr;
-    ws.arm_table_ev = false;
+    ws.sort.arm_table_ev = false;
     FRZ_TRY(ms);
     if (!m->count_published) {   // (cannot happen with >= 1 chunk; kept for symmetry with frz_match_shard_device)
-        FRZ_CUDA_TRY(cudaMemcpyAsync(d_count, &ws.counters->total, sizeof(uint64_t), cudaMemcpyDeviceToDevice, stream));
-        FRZ_CUDA_TRY(cudaEventRecord(m->count_ev, stream));
+        FRZ_CUDA_TRY(cudaMemcpyAsync(d_count, &ws.counters.get()->total, sizeof(uint64_t), cudaMemcpyDeviceToDevice, stream));
+        FRZ_CUDA_TRY(cudaEventRecord(m->count_ev.get(), stream));
     }
     m->last_launches = st.launches;
     m->timings_pending = true;
@@ -1742,17 +1662,13 @@ extern "C" frz_status frz_matcher_debug_pattern(const frz_matcher* m, size_t i, 
     return FRZ_OK;
 }
 
+extern "C" uint64_t frz_debug_device_bytes(void) { return g_frz_device_bytes.load(); }
+
 extern "C" uint32_t frz_matcher_score_bound(const frz_matcher* m) {
     if (!m) return 0;
     uint64_t b = 0;
     for (const auto& c : m->compiled) if (!c.negated) b += c.score_bound;
     return (uint32_t)std::min<uint64_t>(b, 0xFFFF);
-}
-
-void FrzMergeScratch::release() {
-    if (device >= 0) cudaSetDevice(device);
-    cudaFree(hist); cudaFree(tables); cudaFree(cat); cudaFree(tmp); cudaFree(d_total);
-    hist = tables = nullptr; cat = tmp = nullptr; d_total = nullptr; cap = 0; device = -1;
 }
 
 // k_merge_matches_by on `stream` with caller-owned scratch (one per concurrent user; grow-only).
@@ -1772,20 +1688,19 @@ frz_status frz_merge_runs_ex(FrzMergeScratch& ms, const FrzMatchDev* runs, uint6
         total += run_counts_host[src_run];
     }
     meta.total = total;
-    if (ms.device < 0) {
-        int dev = 0;
-        FRZ_CUDA_TRY(cudaGetDevice(&dev));
-        FRZ_TRY(frz_sort_hist_alloc(&ms.hist));
-        FRZ_CUDA_TRY(cudaMalloc(&ms.tables, (size_t)2 * FRZ_MERGE_MAX_RUNS * kMergeMaxBins * sizeof(uint32_t)));
-        FRZ_CUDA_TRY(cudaMalloc(&ms.d_total, sizeof(unsigned long long)));
-        ms.device = dev;
+    if (!ms.d_total.get()) {   // first use, all or nothing: a failed set-up leaves the scratch empty
+        FrzMergeScratch fresh;
+        FRZ_TRY(frz_sort_hist_alloc(fresh.sort.hist));
+        FRZ_TRY(fresh.tables.reserve((size_t)2 * FRZ_MERGE_MAX_RUNS * kMergeMaxBins));
+        FRZ_TRY(fresh.d_total.reserve(1));
+        ms = std::move(fresh);
     }
     const int bins = (int)std::min<uint32_t>(score_bound, 0xFFFFu) + 1;
     if (total == 0) return FRZ_OK;
     if (by_score && bins <= kMergeMaxBins && total <= 0xFFFFFFFFull) {
         // score-sorted runs: boundaries by binary search, one scatter pass (no concatenation, no re-sort)
-        uint32_t* gt = ms.tables;
-        uint32_t* pos0 = ms.tables + (size_t)FRZ_MERGE_MAX_RUNS * kMergeMaxBins;
+        uint32_t* gt = ms.tables.get();
+        uint32_t* pos0 = gt + (size_t)FRZ_MERGE_MAX_RUNS * kMergeMaxBins;
         k_merge_bounds<<<(n_runs * bins + 255) / 256, 256, 0, stream>>>(runs, run_stride, meta, n_runs, bins, gt);
         k_merge_bases<<<(bins + 127) / 128, 128, 0, stream>>>(gt, meta, n_runs, bins, reversed ? 1 : 0, pos0);
         uint64_t longest = 0;
@@ -1795,21 +1710,14 @@ frz_status frz_merge_runs_ex(FrzMergeScratch& ms, const FrzMatchDev* runs, uint6
         FRZ_CUDA_TRY(cudaGetLastError());
         return FRZ_OK;  // asynchronous on `stream`
     }
-    if (by_score && ms.cap < total) {
-        cudaFree(ms.cat); cudaFree(ms.tmp); ms.cat = ms.tmp = nullptr; ms.cap = 0;
-        const uint64_t want = total + total / 4 + 1024;
-        FRZ_CUDA_TRY(cudaMalloc(&ms.cat, want * sizeof(FrzMatchDev)));
-        FRZ_CUDA_TRY(cudaMalloc(&ms.tmp, want * sizeof(FrzMatchDev)));
-        ms.cap = want;
-    }
-    FrzMatchDev* dst = by_score ? ms.cat : d_out;
-    k_gather_runs<<<grid_for(total / std::max(n_runs, 1) + 1, 256), 256, 0, stream>>>(runs, run_stride, meta, n_runs, reversed ? 1 : 0, dst,
-                                                                                     ms.d_total);
     if (by_score) {
-        FrzWorkspace ws;  // only the sort scratch is used
-        ws.sort_hist = ms.hist;
-        FRZ_TRY(frz_launch_sort_by_score_dev(ms.cat, ms.tmp, d_out, ms.d_total, score_bound, ws, stream, nullptr));
+        FRZ_TRY(ms.cat.reserve(total, total + total / 4 + 1024));
+        FRZ_TRY(ms.tmp.reserve(total, total + total / 4 + 1024));
     }
+    FrzMatchDev* dst = by_score ? ms.cat.get() : d_out;
+    k_gather_runs<<<grid_for(total / std::max(n_runs, 1) + 1, 256), 256, 0, stream>>>(runs, run_stride, meta, n_runs, reversed ? 1 : 0, dst,
+                                                                                     ms.d_total.get());
+    if (by_score) FRZ_TRY(frz_launch_sort_by_score_dev(ms.cat.get(), ms.tmp.get(), d_out, ms.d_total.get(), score_bound, ms.sort, stream, nullptr));
     FRZ_CUDA_TRY(cudaGetLastError());
     return FRZ_OK;  // asynchronous on `stream`
 }
@@ -1820,8 +1728,9 @@ extern "C" frz_status frz_merge_runs_device(const frz_match* d_runs, uint64_t ru
     FRZ_TRY(ensure_device(device));
     if (device >= 64) return frz_fail(FRZ_ERR_INVALID_ARG, "device index too large");
     // grow-only per-device scratch (tables only: the run metadata travels as kernel parameters).  Calls for one device
-    // must be stream-ordered with each other, as documented in the header.
-    static FrzMergeScratch scratch[64];
+    // must be stream-ordered with each other, as documented in the header.  Never destroyed: its destructors would run
+    // at process exit, when the CUDA runtime may already be gone.
+    static FrzMergeScratch* const scratch = new FrzMergeScratch[64];
     static std::mutex mu;
     std::lock_guard<std::mutex> lock(mu);
     return frz_merge_runs_ex(scratch[device], reinterpret_cast<const FrzMatchDev*>(d_runs), run_stride, run_counts_host, n_runs, sort,
@@ -1832,24 +1741,20 @@ extern "C" frz_status frz_radix_sort_matches(frz_match* matches, uint64_t n, int
     if (n == 0) return FRZ_OK;
     if (!matches) return frz_fail(FRZ_ERR_INVALID_ARG, "null matches");
     FRZ_TRY(ensure_device(device));
-    FrzMatchDev *d_a = nullptr, *d_b = nullptr, *d_c = nullptr;
-    unsigned long long* d_n = nullptr;
-    FrzWorkspace ws;
+    FrzDevArray<FrzMatchDev> d_a, d_b, d_c;
+    FrzDevArray<unsigned long long> d_n;
+    FrzSortScratch ss;
     cudaStream_t stream = nullptr;
-    frz_status s = [&]() -> frz_status {
-        FRZ_CUDA_TRY(cudaMalloc(&d_a, n * sizeof(FrzMatchDev)));
-        FRZ_CUDA_TRY(cudaMalloc(&d_b, n * sizeof(FrzMatchDev)));
-        FRZ_CUDA_TRY(cudaMalloc(&d_c, n * sizeof(FrzMatchDev)));
-        FRZ_CUDA_TRY(cudaMalloc(&d_n, sizeof(unsigned long long)));
-        FRZ_TRY(frz_sort_hist_alloc(&ws.sort_hist));
-        unsigned long long hn = n;
-        FRZ_CUDA_TRY(cudaMemcpyAsync(d_n, &hn, sizeof hn, cudaMemcpyHostToDevice, stream));
-        FRZ_CUDA_TRY(cudaMemcpyAsync(d_a, matches, n * sizeof(FrzMatchDev), cudaMemcpyHostToDevice, stream));
-        FRZ_TRY(frz_launch_sort_by_score_dev(d_a, d_b, d_c, d_n, 0xFFFF, ws, stream, nullptr));
-        FRZ_CUDA_TRY(cudaMemcpyAsync(matches, d_c, n * sizeof(FrzMatchDev), cudaMemcpyDeviceToHost, stream));
-        FRZ_CUDA_TRY(cudaStreamSynchronize(stream));
-        return FRZ_OK;
-    }();
-    cudaFree(d_a); cudaFree(d_b); cudaFree(d_c); cudaFree(d_n); cudaFree(ws.sort_hist);
-    return s;
+    FRZ_TRY(d_a.reserve(n));
+    FRZ_TRY(d_b.reserve(n));
+    FRZ_TRY(d_c.reserve(n));
+    FRZ_TRY(d_n.reserve(1));
+    FRZ_TRY(frz_sort_hist_alloc(ss.hist));
+    unsigned long long hn = n;
+    FRZ_CUDA_TRY(cudaMemcpyAsync(d_n.get(), &hn, sizeof hn, cudaMemcpyHostToDevice, stream));
+    FRZ_CUDA_TRY(cudaMemcpyAsync(d_a.get(), matches, n * sizeof(FrzMatchDev), cudaMemcpyHostToDevice, stream));
+    FRZ_TRY(frz_launch_sort_by_score_dev(d_a.get(), d_b.get(), d_c.get(), d_n.get(), 0xFFFF, ss, stream, nullptr));
+    FRZ_CUDA_TRY(cudaMemcpyAsync(matches, d_c.get(), n * sizeof(FrzMatchDev), cudaMemcpyDeviceToHost, stream));
+    FRZ_CUDA_TRY(cudaStreamSynchronize(stream));
+    return FRZ_OK;
 }

@@ -292,29 +292,30 @@ namespace {
 constexpr const char* kHayTooLong = "haystack longer than %u bytes";
 
 frz_status pack_reserve(FrzCorpusStorage* out, uint32_t n_tiles, uint32_t keep_tiles, cudaStream_t stream) {
-    if (out->cap_tiles >= n_tiles) return FRZ_OK;
-    const uint32_t want = keep_tiles ? std::max<uint32_t>(n_tiles, out->cap_tiles + out->cap_tiles / 2) : n_tiles;
+    const uint64_t cap = out->tile_base.cap();
+    if (cap >= n_tiles) return FRZ_OK;
+    const uint32_t want = keep_tiles ? std::max<uint32_t>(n_tiles, (uint32_t)(cap + cap / 2)) : n_tiles;
     const size_t slots = (size_t)want * FRZ_TILE;
-    uint32_t* slot_meta = nullptr; uint16_t* slot_of = nullptr; FrzGroupDesc* groups = nullptr;
-    uint64_t* tile_base = nullptr; uint64_t* scratch = nullptr; uint2* slot_sig = nullptr;
-    FRZ_CUDA_TRY(cudaMalloc(&slot_meta, slots * sizeof(uint32_t)));
-    FRZ_CUDA_TRY(cudaMalloc(&slot_of, slots * sizeof(uint16_t)));
-    FRZ_CUDA_TRY(cudaMalloc(&slot_sig, slots * sizeof(uint2)));
-    FRZ_CUDA_TRY(cudaMalloc(&groups, (size_t)want * FRZ_GROUPS_PER_TILE * sizeof(FrzGroupDesc)));
-    FRZ_CUDA_TRY(cudaMalloc(&tile_base, (size_t)want * sizeof(uint64_t)));
-    FRZ_CUDA_TRY(cudaMalloc(&scratch, ((size_t)want + 2) * sizeof(uint64_t)));
-    if (keep_tiles) {  // append: carry the existing tiles' metadata over
+    // new arrays next to the old ones, so that an append can carry the existing tiles' metadata over
+    FrzDevArray<uint32_t> slot_meta; FrzDevArray<uint16_t> slot_of; FrzDevArray<uint2> slot_sig; FrzDevArray<FrzGroupDesc> groups;
+    FrzDevArray<uint64_t> tile_base, scratch;
+    FRZ_TRY(slot_meta.reserve(slots));
+    FRZ_TRY(slot_of.reserve(slots));
+    FRZ_TRY(slot_sig.reserve(slots));
+    FRZ_TRY(groups.reserve((size_t)want * FRZ_GROUPS_PER_TILE));
+    FRZ_TRY(tile_base.reserve(want));
+    FRZ_TRY(scratch.reserve((size_t)want + 2));
+    if (keep_tiles) {
         const size_t ks = (size_t)keep_tiles * FRZ_TILE;
-        FRZ_CUDA_TRY(cudaMemcpyAsync(slot_meta, out->slot_meta, ks * sizeof(uint32_t), cudaMemcpyDeviceToDevice, stream));
-        FRZ_CUDA_TRY(cudaMemcpyAsync(slot_of, out->slot_of, ks * sizeof(uint16_t), cudaMemcpyDeviceToDevice, stream));
-        FRZ_CUDA_TRY(cudaMemcpyAsync(slot_sig, out->slot_sig, ks * sizeof(uint2), cudaMemcpyDeviceToDevice, stream));
-        FRZ_CUDA_TRY(cudaMemcpyAsync(groups, out->groups, (size_t)keep_tiles * FRZ_GROUPS_PER_TILE * sizeof(FrzGroupDesc), cudaMemcpyDeviceToDevice, stream));
-        FRZ_CUDA_TRY(cudaMemcpyAsync(tile_base, out->tile_base, (size_t)keep_tiles * sizeof(uint64_t), cudaMemcpyDeviceToDevice, stream));
+        FRZ_CUDA_TRY(cudaMemcpyAsync(slot_meta.get(), out->slot_meta.get(), ks * sizeof(uint32_t), cudaMemcpyDeviceToDevice, stream));
+        FRZ_CUDA_TRY(cudaMemcpyAsync(slot_of.get(), out->slot_of.get(), ks * sizeof(uint16_t), cudaMemcpyDeviceToDevice, stream));
+        FRZ_CUDA_TRY(cudaMemcpyAsync(slot_sig.get(), out->slot_sig.get(), ks * sizeof(uint2), cudaMemcpyDeviceToDevice, stream));
+        FRZ_CUDA_TRY(cudaMemcpyAsync(groups.get(), out->groups.get(), (size_t)keep_tiles * FRZ_GROUPS_PER_TILE * sizeof(FrzGroupDesc), cudaMemcpyDeviceToDevice, stream));
+        FRZ_CUDA_TRY(cudaMemcpyAsync(tile_base.get(), out->tile_base.get(), (size_t)keep_tiles * sizeof(uint64_t), cudaMemcpyDeviceToDevice, stream));
         FRZ_CUDA_TRY(cudaStreamSynchronize(stream));
     }
-    cudaFree(out->slot_meta); cudaFree(out->slot_of); cudaFree(out->slot_sig); cudaFree(out->groups); cudaFree(out->tile_base); cudaFree(out->scratch_tile_units);
-    out->slot_meta = slot_meta; out->slot_of = slot_of; out->slot_sig = slot_sig; out->groups = groups; out->tile_base = tile_base; out->scratch_tile_units = scratch;
-    out->cap_tiles = want;
+    out->slot_meta = std::move(slot_meta); out->slot_of = std::move(slot_of); out->slot_sig = std::move(slot_sig);
+    out->groups = std::move(groups); out->tile_base = std::move(tile_base); out->scratch_tile_units = std::move(scratch);
     return FRZ_OK;
 }
 
@@ -323,30 +324,27 @@ template <typename OffT>
 frz_status pack_plan(FrzCorpusStorage* out, const OffT* d_offsets, uint64_t n, uint32_t tile0, uint64_t idx0, uint64_t carry_in,
                      bool keep_data, cudaStream_t stream) {
     const uint32_t n_tiles = out->n_tiles;
-    uint64_t* d_tile_units = out->scratch_tile_units;
-    uint64_t* d_total = d_tile_units + out->cap_tiles;
+    uint64_t* d_tile_units = out->scratch_tile_units.get();
+    uint64_t* d_total = d_tile_units + out->tile_base.cap();
     unsigned int* d_err = reinterpret_cast<unsigned int*>(d_total + 1);
     FRZ_CUDA_TRY(cudaMemsetAsync(d_total, 0, 16, stream));
-    k_pack_plan<OffT><<<n_tiles - tile0, 256, 0, stream>>>(d_offsets, n, tile0, idx0, out->slot_meta, out->slot_of, out->groups,
-                                                          d_tile_units, d_err);
-    k_scan_u64<<<1, 1024, 0, stream>>>(d_tile_units + tile0, out->tile_base + tile0, n_tiles - tile0, carry_in, d_total);
+    k_pack_plan<OffT><<<n_tiles - tile0, 256, 0, stream>>>(d_offsets, n, tile0, idx0, out->slot_meta.get(), out->slot_of.get(),
+                                                          out->groups.get(), d_tile_units, d_err);
+    k_scan_u64<<<1, 1024, 0, stream>>>(d_tile_units + tile0, out->tile_base.get() + tile0, n_tiles - tile0, carry_in, d_total);
     uint64_t h[2] = {0, 0};
     FRZ_CUDA_TRY(cudaMemcpyAsync(h, d_total, 16, cudaMemcpyDeviceToHost, stream));
     FRZ_CUDA_TRY(cudaStreamSynchronize(stream));
     if ((unsigned int)(h[1] & 0xffffffffu)) return frz_fail(FRZ_ERR_UNSUPPORTED, kHayTooLong, FRZ_MAX_HAY_LEN);
     out->total_units = h[0];
     out->max_gunits = std::max<uint32_t>(tile0 ? out->max_gunits : 0u, (uint32_t)(h[1] >> 32));
-    if (out->cap_units < out->total_units + 1) {
-        const uint64_t want = out->total_units + out->total_units / (keep_data ? 2 : 16) + 1024;
-        uint4* data = nullptr;
-        FRZ_CUDA_TRY(cudaMalloc(&data, (size_t)want * sizeof(uint4)));
+    if (out->data.cap() < out->total_units + 1) {
+        FrzDevArray<uint4> data;
+        FRZ_TRY(data.reserve(out->total_units + out->total_units / (keep_data ? 2 : 16) + 1024));
         if (keep_data && carry_in) {
-            FRZ_CUDA_TRY(cudaMemcpyAsync(data, out->data, (size_t)carry_in * sizeof(uint4), cudaMemcpyDeviceToDevice, stream));
+            FRZ_CUDA_TRY(cudaMemcpyAsync(data.get(), out->data.get(), (size_t)carry_in * sizeof(uint4), cudaMemcpyDeviceToDevice, stream));
             FRZ_CUDA_TRY(cudaStreamSynchronize(stream));
         }
-        cudaFree(out->data);
-        out->data = data;
-        out->cap_units = want;
+        out->data = std::move(data);
     }
     return FRZ_OK;
 }
@@ -356,12 +354,12 @@ frz_status pack_copy(FrzCorpusStorage* out, const uint8_t* d_bytes, const OffT* 
                      uint64_t off0, uint64_t total_bytes, uint32_t t0, uint32_t t1, cudaStream_t stream) {
     if (t1 <= t0) return FRZ_OK;
     (void)tile0;
-    k_pack_copy<OffT><<<t1 - t0, 256, 0, stream>>>(d_bytes, d_offsets, t0, idx0, off0, total_bytes, out->slot_meta, out->groups,
-                                                  out->tile_base, out->data);
+    k_pack_copy<OffT><<<t1 - t0, 256, 0, stream>>>(d_bytes, d_offsets, t0, idx0, off0, total_bytes, out->slot_meta.get(),
+                                                  out->groups.get(), out->tile_base.get(), out->data.get());
     // signature index of the same tiles, from the bytes just interleaved (L2-resident for a streamed chunk)
     const uint32_t g0 = t0 * FRZ_GROUPS_PER_TILE, g1 = t1 * FRZ_GROUPS_PER_TILE;
     const uint32_t sig_blocks = std::min<uint32_t>((g1 - g0 + 7) / 8, frz_sm_count() * 8);
-    k_pack_sig<<<sig_blocks, 256, 0, stream>>>(out->data, out->groups, out->slot_meta, g0, g1, out->slot_sig);
+    k_pack_sig<<<sig_blocks, 256, 0, stream>>>(out->data.get(), out->groups.get(), out->slot_meta.get(), g0, g1, out->slot_sig.get());
     FRZ_CUDA_TRY(cudaGetLastError());
     return FRZ_OK;
 }
@@ -403,12 +401,14 @@ frz_status ingest_host_t(FrzIngest& ing, const uint8_t* h_bytes, const OffT* h_o
     if (n_tiles == 0) { out->total_units = 0; return FRZ_OK; }
     FRZ_TRY(ing.reserve(total, (n + 1) * sizeof(OffT)));
     FRZ_TRY(pack_reserve(out, n_tiles, 0, stream));
-    OffT* d_off = reinterpret_cast<OffT*>(ing.d_offsets);
+    OffT* d_off = reinterpret_cast<OffT*>(ing.d_offsets.get());
+    cudaStream_t copy = ing.copy_stream.get();
+    cudaEvent_t arena_ev = ing.ev[FrzIngest::kMaxChunks].get();
     // everything already queued on `stream` (a previous call's kernels reading the arena) must finish first
-    FRZ_CUDA_TRY(cudaEventRecord(ing.ev[FrzIngest::kMaxChunks], stream));
-    FRZ_CUDA_TRY(cudaStreamWaitEvent(ing.copy_stream, ing.ev[FrzIngest::kMaxChunks], 0));
-    FRZ_CUDA_TRY(cudaMemcpyAsync(d_off, h_offsets, (n + 1) * sizeof(OffT), cudaMemcpyHostToDevice, ing.copy_stream));
-    FRZ_CUDA_TRY(cudaEventRecord(ing.ev[FrzIngest::kMaxChunks], ing.copy_stream));
+    FRZ_CUDA_TRY(cudaEventRecord(arena_ev, stream));
+    FRZ_CUDA_TRY(cudaStreamWaitEvent(copy, arena_ev, 0));
+    FRZ_CUDA_TRY(cudaMemcpyAsync(d_off, h_offsets, (n + 1) * sizeof(OffT), cudaMemcpyHostToDevice, copy));
+    FRZ_CUDA_TRY(cudaEventRecord(arena_ev, copy));
     // chunk plan: tile-aligned, about equal byte counts, at least kMinChunk bytes each
     int n_chunks = (int)std::min<uint64_t>(FrzIngest::kMaxChunks, std::max<uint64_t>(1, total / FrzIngest::kMinChunkBytes));
     n_chunks = (int)std::min<uint64_t>(n_chunks, n_tiles);
@@ -421,14 +421,14 @@ frz_status ingest_host_t(FrzIngest& ing, const uint8_t* h_bytes, const OffT* h_o
     for (int c = 0; c < n_chunks; c++) {
         const uint64_t i0 = std::min<uint64_t>((uint64_t)bounds[c] * FRZ_TILE, n), i1 = std::min<uint64_t>((uint64_t)bounds[c + 1] * FRZ_TILE, n);
         const uint64_t b0 = (uint64_t)h_offsets[i0] - off0, b1 = (uint64_t)h_offsets[i1] - off0;
-        if (b1 > b0) FRZ_CUDA_TRY(cudaMemcpyAsync(ing.d_bytes + b0, h_bytes + off0 + b0, b1 - b0, cudaMemcpyHostToDevice, ing.copy_stream));
-        FRZ_CUDA_TRY(cudaEventRecord(ing.ev[c], ing.copy_stream));
+        if (b1 > b0) FRZ_CUDA_TRY(cudaMemcpyAsync(ing.d_bytes.get() + b0, h_bytes + off0 + b0, b1 - b0, cudaMemcpyHostToDevice, copy));
+        FRZ_CUDA_TRY(cudaEventRecord(ing.ev[c].get(), copy));
     }
-    FRZ_CUDA_TRY(cudaStreamWaitEvent(stream, ing.ev[FrzIngest::kMaxChunks], 0));
+    FRZ_CUDA_TRY(cudaStreamWaitEvent(stream, arena_ev, 0));
     FRZ_TRY(pack_plan<OffT>(out, d_off, n, 0, 0, 0, false, stream));   // waits for the plan only; the byte chunks keep flowing
     for (int c = 0; c < n_chunks; c++) {
-        FRZ_CUDA_TRY(cudaStreamWaitEvent(stream, ing.ev[c], 0));
-        FRZ_TRY(pack_copy<OffT>(out, ing.d_bytes, d_off, 0, 0, off0, total, bounds[c], bounds[c + 1], stream));
+        FRZ_CUDA_TRY(cudaStreamWaitEvent(stream, ing.ev[c].get(), 0));
+        FRZ_TRY(pack_copy<OffT>(out, ing.d_bytes.get(), d_off, 0, 0, off0, total, bounds[c], bounds[c + 1], stream));
         if (after_chunk) FRZ_TRY(after_chunk(ctx, bounds[c], bounds[c + 1], c == n_chunks - 1));
     }
     return FRZ_OK;
@@ -457,12 +457,12 @@ frz_status append_host_t(FrzIngest& ing, const uint8_t* h_bytes, const OffT* h_o
     // staging layout in ing.d_offsets: [tail_info: 2 u64][staged offsets: cnt + n_new + 1 u64][raw new offsets]
     const uint64_t staged_words = 2 + (uint64_t)cnt + n_new + 1;
     FRZ_TRY(ing.reserve(0, staged_words * 8 + (n_new + 1) * sizeof(OffT) + 16));
-    uint64_t* d_info = reinterpret_cast<uint64_t*>(ing.d_offsets);
+    uint64_t* d_info = reinterpret_cast<uint64_t*>(ing.d_offsets.get());
     uint64_t* d_staged = d_info + 2;
     OffT* d_raw = reinterpret_cast<OffT*>(d_staged + cnt + n_new + 1);
     uint64_t info[2] = {0, st->total_units};
     if (cnt) {
-        k_tail_offsets<<<1, 1024, 0, stream>>>(st->slot_meta, st->slot_of, st->tile_base, t_last, cnt, d_staged, d_info);
+        k_tail_offsets<<<1, 1024, 0, stream>>>(st->slot_meta.get(), st->slot_of.get(), st->tile_base.get(), t_last, cnt, d_staged, d_info);
         FRZ_CUDA_TRY(cudaMemcpyAsync(info, d_info, 16, cudaMemcpyDeviceToHost, stream));
         FRZ_CUDA_TRY(cudaStreamSynchronize(stream));
     } else {
@@ -470,8 +470,10 @@ frz_status append_host_t(FrzIngest& ing, const uint8_t* h_bytes, const OffT* h_o
     }
     const uint64_t tail_bytes = info[0], carry_in = info[1];
     FRZ_TRY(ing.reserve(tail_bytes + new_bytes, 0));
-    if (cnt) k_tail_bytes<<<32, 256, 0, stream>>>(st->data, st->groups, st->slot_meta, st->slot_of, t_last, cnt, d_staged, ing.d_bytes);
-    if (new_bytes) FRZ_CUDA_TRY(cudaMemcpyAsync(ing.d_bytes + tail_bytes, h_bytes + off0, new_bytes, cudaMemcpyHostToDevice, stream));
+    if (cnt)
+        k_tail_bytes<<<32, 256, 0, stream>>>(st->data.get(), st->groups.get(), st->slot_meta.get(), st->slot_of.get(), t_last, cnt, d_staged,
+                                             ing.d_bytes.get());
+    if (new_bytes) FRZ_CUDA_TRY(cudaMemcpyAsync(ing.d_bytes.get() + tail_bytes, h_bytes + off0, new_bytes, cudaMemcpyHostToDevice, stream));
     FRZ_CUDA_TRY(cudaMemcpyAsync(d_raw, h_offsets, (n_new + 1) * sizeof(OffT), cudaMemcpyHostToDevice, stream));
     k_rebase_offsets<OffT><<<256, 256, 0, stream>>>(d_raw, n_new, d_info, d_staged + cnt);
     FRZ_CUDA_TRY(cudaGetLastError());
@@ -480,39 +482,19 @@ frz_status append_host_t(FrzIngest& ing, const uint8_t* h_bytes, const OffT* h_o
     st->n_tiles = n_tiles;
     st->total_bytes += new_bytes;
     FRZ_TRY(pack_plan<uint64_t>(st, d_staged, n, t_last, idx0, carry_in, true, stream));
-    return pack_copy<uint64_t>(st, ing.d_bytes, d_staged, t_last, idx0, 0, tail_bytes + new_bytes, t_last, n_tiles, stream);
+    return pack_copy<uint64_t>(st, ing.d_bytes.get(), d_staged, t_last, idx0, 0, tail_bytes + new_bytes, t_last, n_tiles, stream);
 }
 
 }  // namespace
 
 frz_status FrzIngest::reserve(uint64_t bytes, uint64_t offset_bytes) {
-    if (!copy_stream) {
-        FRZ_CUDA_TRY(cudaStreamCreateWithFlags(&copy_stream, cudaStreamNonBlocking));
-        for (auto& e : ev) FRZ_CUDA_TRY(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    if (!ev[kMaxChunks]) {   // created last: a failed set-up is redone by the next call
+        FRZ_TRY(frz_stream_create(copy_stream, cudaStreamNonBlocking));
+        for (auto& e : ev) FRZ_TRY(frz_event_create(e, cudaEventDisableTiming));
     }
-    if (bytes_cap < bytes + 16) {
-        cudaFree(d_bytes); d_bytes = nullptr; bytes_cap = 0;
-        const uint64_t want = bytes + bytes / 16 + 4096;
-        FRZ_CUDA_TRY(cudaMalloc(&d_bytes, want));
-        bytes_cap = want;
-    }
-    if (offsets_cap < offset_bytes) {
-        cudaFree(d_offsets); d_offsets = nullptr; offsets_cap = 0;
-        const uint64_t want = offset_bytes + offset_bytes / 16 + 4096;
-        FRZ_CUDA_TRY(cudaMalloc(&d_offsets, want));
-        offsets_cap = want;
-    }
+    FRZ_TRY(d_bytes.reserve(bytes + 16, bytes + bytes / 16 + 4096));
+    FRZ_TRY(d_offsets.reserve(offset_bytes, offset_bytes + offset_bytes / 16 + 4096));
     return FRZ_OK;
-}
-
-void FrzIngest::release() {
-    cudaFree(d_bytes); cudaFree(d_offsets);
-    d_bytes = nullptr; d_offsets = nullptr; bytes_cap = offsets_cap = 0;
-    if (copy_stream) {
-        cudaStreamDestroy(copy_stream);
-        copy_stream = nullptr;
-        for (auto& e : ev) { cudaEventDestroy(e); e = nullptr; }
-    }
 }
 
 // Builds the packed corpus from device-resident Arrow buffers (64- or 32-bit offsets).  Asynchronous on

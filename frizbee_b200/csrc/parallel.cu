@@ -296,31 +296,28 @@ struct RankCtx {
     int rank = 0;        // global rank
     int device = 0;
     ncclComm_t nccl = nullptr;
-    cudaStream_t side = nullptr;           // non-blocking: publishes the count while the main stream scores
+    FrzStream side;                        // non-blocking: publishes the count while the main stream scores
     frz_matcher* clone = nullptr;
     uint64_t clone_epoch = 0;
-    FrzMatchDev* run = nullptr;            // this rank's locally ordered run
-    uint64_t run_cap = 0;
-    unsigned long long* d_count = nullptr;
-    FrzMatchDev* gathered = nullptr;
-    uint64_t gathered_cap = 0;
-    FrzMatchDev* merged = nullptr;
-    uint64_t merged_cap = 0;
+    FrzDevArray<FrzMatchDev> run;          // this rank's locally ordered run
+    FrzDevArray<unsigned long long> d_count;
+    FrzDevArray<FrzMatchDev> gathered;
+    FrzDevArray<FrzMatchDev> merged;
     FrzMergeScratch merge;
     // slice exchange (host-out calls): pieces received from every run, device copies of the gt / pos0 tables, pinned staging
-    FrzMatchDev* recv = nullptr;
-    uint64_t recv_cap = 0;
-    uint32_t* d_gt = nullptr;               // (d_pos0 and d_gt are one allocation, h_pos0 and h_gt one pinned staging block:
-    unsigned long long* d_pos0 = nullptr;   //  the tables travel in ONE host→device copy)
+    FrzDevArray<FrzMatchDev> recv;
+    // [world * kTableBins] u64 pos0, then as many u32 gt (d_gt, h_gt): the tables travel in ONE host→device copy
+    FrzDevArray<unsigned long long> d_pos0;
+    FrzPinnedArray<unsigned long long> h_pos0;
+    uint32_t* d_gt = nullptr;
     uint32_t* h_gt = nullptr;
-    unsigned long long* h_pos0 = nullptr;
     // P2P placement (host-out calls): my slice buffer (header + elements), exported to the peers; theirs mapped here
-    unsigned char* place_raw = nullptr;
+    FrzDevArray<unsigned char> place_raw;
     uint64_t place_cap = 0;                 // elements
     unsigned char* peer_raw[kMaxWorld] = {};
     bool peer_ipc[kMaxWorld] = {};          // opened with cudaIpcOpenMemHandle (multi-process form)
     uint32_t* table_dev = nullptr;          // device-side address of the shared table block
-    cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
+    FrzEvent ev[4];
     bool ev_valid = false;
     uint64_t* ctrl_dev = nullptr;          // device-side address of the shared control block
 };
@@ -376,6 +373,7 @@ frz_status set_device(int device) {
     return FRZ_OK;
 }
 
+// what the rank's owners do not free themselves: its matcher clone, its peers' mappings and its NCCL communicator
 void rank_release(RankCtx& r) {
     cudaSetDevice(r.device);
     if (r.clone) frz_matcher_destroy(r.clone);
@@ -384,25 +382,16 @@ void rank_release(RankCtx& r) {
         if (r.peer_ipc[q] && r.peer_raw[q]) cudaIpcCloseMemHandle(r.peer_raw[q]);
         r.peer_raw[q] = nullptr; r.peer_ipc[q] = false;
     }
-    cudaFree(r.place_raw); r.place_raw = nullptr; r.place_cap = 0;
-    cudaFree(r.run); cudaFree(r.d_count); cudaFree(r.gathered); cudaFree(r.merged); cudaFree(r.recv); cudaFree(r.d_pos0);
-    if (r.h_pos0) cudaFreeHost(r.h_pos0);
-    r.run = nullptr; r.d_count = nullptr; r.gathered = nullptr; r.merged = nullptr; r.recv = nullptr; r.d_gt = nullptr; r.d_pos0 = nullptr;
-    r.h_gt = nullptr; r.h_pos0 = nullptr;
-    r.merge.release();
-    for (auto& e : r.ev) { if (e) cudaEventDestroy(e); e = nullptr; }
-    if (r.side) cudaStreamDestroy(r.side);
-    r.side = nullptr;
     if (r.nccl) nccl_api().CommDestroy(r.nccl);
     r.nccl = nullptr;
 }
 
 frz_status rank_init(RankCtx& r) {
     FRZ_TRY(set_device(r.device));
-    FRZ_CUDA_TRY(cudaStreamCreateWithFlags(&r.side, cudaStreamNonBlocking));
-    FRZ_CUDA_TRY(cudaMalloc(&r.d_count, 2 * sizeof(unsigned long long)));
-    FRZ_CUDA_TRY(cudaMemset(r.d_count, 0, 2 * sizeof(unsigned long long)));
-    for (auto& e : r.ev) FRZ_CUDA_TRY(cudaEventCreate(&e));
+    FRZ_TRY(frz_stream_create(r.side, cudaStreamNonBlocking));
+    FRZ_TRY(r.d_count.reserve(2));
+    FRZ_CUDA_TRY(cudaMemset(r.d_count.get(), 0, 2 * sizeof(unsigned long long)));
+    for (auto& e : r.ev) FRZ_TRY(frz_event_create(e, cudaEventDefault));
     return FRZ_OK;
 }
 
@@ -419,18 +408,14 @@ void host_block_release(HostBlock& b) {
 frz_status exchange_words(frz_comm* c, const uint64_t* mine, int n_words, uint64_t* all /* [world * n_words] */) {
     RankCtx& r = c->ranks[0];
     FRZ_TRY(set_device(r.device));
-    unsigned long long *d_in = nullptr, *d_out = nullptr;
-    frz_status st = [&]() -> frz_status {
-        FRZ_CUDA_TRY(cudaMalloc(&d_in, n_words * sizeof(uint64_t)));
-        FRZ_CUDA_TRY(cudaMalloc(&d_out, (size_t)c->world * n_words * sizeof(uint64_t)));
-        FRZ_CUDA_TRY(cudaMemcpyAsync(d_in, mine, n_words * sizeof(uint64_t), cudaMemcpyHostToDevice, r.side));
-        FRZ_NCCL_TRY(nccl_api().AllGather(d_in, d_out, (size_t)n_words, ncclUint64, r.nccl, r.side));
-        FRZ_CUDA_TRY(cudaMemcpyAsync(all, d_out, (size_t)c->world * n_words * sizeof(uint64_t), cudaMemcpyDeviceToHost, r.side));
-        FRZ_CUDA_TRY(cudaStreamSynchronize(r.side));
-        return FRZ_OK;
-    }();
-    cudaFree(d_in); cudaFree(d_out);
-    return st;
+    FrzDevArray<unsigned long long> d_in, d_out;
+    FRZ_TRY(d_in.reserve(n_words));
+    FRZ_TRY(d_out.reserve((size_t)c->world * n_words));
+    FRZ_CUDA_TRY(cudaMemcpyAsync(d_in.get(), mine, n_words * sizeof(uint64_t), cudaMemcpyHostToDevice, r.side.get()));
+    FRZ_NCCL_TRY(nccl_api().AllGather(d_in.get(), d_out.get(), (size_t)n_words, ncclUint64, r.nccl, r.side.get()));
+    FRZ_CUDA_TRY(cudaMemcpyAsync(all, d_out.get(), (size_t)c->world * n_words * sizeof(uint64_t), cudaMemcpyDeviceToHost, r.side.get()));
+    FRZ_CUDA_TRY(cudaStreamSynchronize(r.side.get()));
+    return FRZ_OK;
 }
 
 // every rank contributes n_words (<= 16) host words and receives everybody's: NCCL in the multi-process form, a
@@ -473,24 +458,25 @@ frz_status ensure_place_buffers(frz_comm* c, RankCtx& r, uint64_t need, bool* re
     uint64_t w[10], all[kMaxWorld * 10];
     memset(w, 0, sizeof w);
     FRZ_TRY(allgather_words(c, r, w, 1, all));   // everybody has dropped its mappings: the owners may free
-    cudaFree(r.place_raw); r.place_raw = nullptr; r.place_cap = 0;
+    r.place_raw.reset();
+    r.place_cap = 0;
     const uint64_t want = need + need / 4 + 4096;
-    bool ok = cudaMalloc(&r.place_raw, kPlaceHeaderBytes + want * sizeof(FrzMatchDev)) == cudaSuccess &&
-              cudaMemset(r.place_raw, 0, kPlaceHeaderBytes) == cudaSuccess;
+    bool ok = r.place_raw.reserve(kPlaceHeaderBytes + want * sizeof(FrzMatchDev)) == FRZ_OK &&
+              cudaMemset(r.place_raw.get(), 0, kPlaceHeaderBytes) == cudaSuccess;
     static_assert(sizeof(cudaIpcMemHandle_t) == 64, "cudaIpcMemHandle_t size");
     if (ok && !c->local_form) {
         cudaIpcMemHandle_t h;
-        ok = cudaIpcGetMemHandle(&h, r.place_raw) == cudaSuccess;
+        ok = cudaIpcGetMemHandle(&h, r.place_raw.get()) == cudaSuccess;
         if (ok) memcpy(&w[2], &h, sizeof h);
     }
     if (!ok) cudaGetLastError();
     w[0] = ok ? 1 : 0;
-    w[1] = (uint64_t)reinterpret_cast<uintptr_t>(r.place_raw);
+    w[1] = (uint64_t)reinterpret_cast<uintptr_t>(r.place_raw.get());
     FRZ_TRY(allgather_words(c, r, w, 10, all));
     for (int q = 0; q < world; q++) ok = ok && all[(size_t)q * 10] == 1;
     if (ok) {
         for (int q = 0; q < world && ok; q++) {
-            if (q == r.rank) { r.peer_raw[q] = r.place_raw; continue; }
+            if (q == r.rank) { r.peer_raw[q] = r.place_raw.get(); continue; }
             if (c->local_form) { r.peer_raw[q] = reinterpret_cast<unsigned char*>((uintptr_t)all[(size_t)q * 10 + 1]); continue; }
             cudaIpcMemHandle_t h;
             memcpy(&h, &all[(size_t)q * 10 + 2], sizeof h);
@@ -509,7 +495,8 @@ frz_status ensure_place_buffers(frz_comm* c, RankCtx& r, uint64_t need, bool* re
             if (r.peer_ipc[q] && r.peer_raw[q]) cudaIpcCloseMemHandle(r.peer_raw[q]);
             r.peer_raw[q] = nullptr; r.peer_ipc[q] = false;
         }
-        cudaFree(r.place_raw); r.place_raw = nullptr; r.place_cap = 0;
+        r.place_raw.reset();
+        r.place_cap = 0;
         if (&r == &c->ranks[0]) c->p2p_exchange = false;   // one writer; the other workers read it at their next call
         return FRZ_OK;
     }
@@ -677,10 +664,10 @@ frz_status comm_finish_setup(frz_comm* c, bool slices) {
             FRZ_CUDA_TRY(cudaHostGetDevicePointer(&dp, c->tables.ptr, 0));
             r.table_dev = reinterpret_cast<uint32_t*>(dp);
             const size_t entries = (size_t)c->world * kTableBins;
-            FRZ_CUDA_TRY(cudaMalloc(&r.d_pos0, entries * (sizeof(unsigned long long) + sizeof(uint32_t))));
-            r.d_gt = reinterpret_cast<uint32_t*>(r.d_pos0 + entries);
-            FRZ_CUDA_TRY(cudaMallocHost(&r.h_pos0, entries * (sizeof(unsigned long long) + sizeof(uint32_t))));
-            r.h_gt = reinterpret_cast<uint32_t*>(r.h_pos0 + entries);
+            FRZ_TRY(r.d_pos0.reserve(entries + entries / 2));   // entries u64 + entries u32 (entries is even)
+            r.d_gt = reinterpret_cast<uint32_t*>(r.d_pos0.get() + entries);
+            FRZ_TRY(r.h_pos0.reserve(entries + entries / 2));
+            r.h_gt = reinterpret_cast<uint32_t*>(r.h_pos0.get() + entries);
         }
     }
     return FRZ_OK;
@@ -744,25 +731,20 @@ frz_status rank_step(frz_comm* c, RankCtx& r, frz_matcher* m, const frz_corpus* 
         r.clone_epoch = frz_matcher_epoch(m);
     }
     const uint64_t n_local = hs ? hs->n : frz_corpus_len(shard);
-    if (r.run_cap < std::max<uint64_t>(n_local, 1)) {
-        cudaFree(r.run); r.run = nullptr; r.run_cap = 0;
-        const uint64_t want = std::max<uint64_t>(n_local, 1);
-        FRZ_CUDA_TRY(cudaMalloc(&r.run, want * sizeof(FrzMatchDev)));
-        r.run_cap = want;
-    }
-    FRZ_CUDA_TRY(cudaEventRecord(r.ev[0], main));
+    FRZ_TRY(r.run.reserve(std::max<uint64_t>(n_local, 1)));
+    FRZ_CUDA_TRY(cudaEventRecord(r.ev[0].get(), main));
     // ---- local pipeline (asynchronous): prefilter → count published → scoring → local order
     if (hs)
         FRZ_TRY(frz_match_shard_streamed(r.clone, hs->bytes, hs->offsets, hs->offset_width, hs->n, r.device, index_offset,
-                                         reinterpret_cast<frz_match*>(r.run), r.run_cap, reinterpret_cast<uint64_t*>(r.d_count), main));
+                                         reinterpret_cast<frz_match*>(r.run.get()), r.run.cap(), reinterpret_cast<uint64_t*>(r.d_count.get()), main));
     else
-        FRZ_TRY(frz_match_shard_device_top(r.clone, shard, index_offset, reinterpret_cast<frz_match*>(r.run), r.run_cap,
-                                           reinterpret_cast<uint64_t*>(r.d_count), main, (uint32_t)std::min<uint64_t>(limit, kFrzNoLimit)));
-    FRZ_TRY(frz_matcher_wait_count(r.clone, r.side));
-    k_publish<<<1, 1, 0, r.side>>>(reinterpret_cast<volatile unsigned long long*>(r.ctrl_dev + kCtrlCount + parity * kMaxWorld + r.rank),
-                                   r.d_count, seq);
+        FRZ_TRY(frz_match_shard_device_top(r.clone, shard, index_offset, reinterpret_cast<frz_match*>(r.run.get()), r.run.cap(),
+                                           reinterpret_cast<uint64_t*>(r.d_count.get()), main, (uint32_t)std::min<uint64_t>(limit, kFrzNoLimit)));
+    FRZ_TRY(frz_matcher_wait_count(r.clone, r.side.get()));
+    k_publish<<<1, 1, 0, r.side.get()>>>(reinterpret_cast<volatile unsigned long long*>(r.ctrl_dev + kCtrlCount + parity * kMaxWorld + r.rank),
+                                         r.d_count.get(), seq);
     FRZ_CUDA_TRY(cudaGetLastError());
-    FRZ_CUDA_TRY(cudaEventRecord(r.ev[1], main));
+    FRZ_CUDA_TRY(cudaEventRecord(r.ev[1].get(), main));
     // ---- the Vec lengths of all workers (k_merge.rs:96-104): polled from the shared block while the GPU scores
     uint64_t counts[kMaxWorld];
     FRZ_TRY(wait_slots(c->ctrl_host + kCtrlCount + parity * kMaxWorld, world, seq, counts, "match count"));
@@ -778,7 +760,7 @@ frz_status rank_step(frz_comm* c, RankCtx& r, frz_matcher* m, const frz_corpus* 
     res->total = total;
     res->kept = kp;
     const bool collective = world > 1 || c->force_nccl;
-    const FrzMatchDev* d_final = r.run;
+    const FrzMatchDev* d_final = r.run.get();
     uint64_t d_final_first = 0;   // merged position of d_final[0] (non-zero in the slice form)
     bool placed = false;          // the P2P placement ran this step
     // ---- host-out calls: SLICE EXCHANGE.  A rank copies only its slice [lo, hi) of the merged list to the host, and the
@@ -810,8 +792,8 @@ frz_status rank_step(frz_comm* c, RankCtx& r, frz_matcher* m, const frz_corpus* 
             // stream at that point, so the tables cross the host block — and the host prepares the exchange — while the scatter runs
             cudaStream_t pub = main;
             if (cudaEvent_t tev = frz_matcher_table_event(r.clone)) {
-                FRZ_CUDA_TRY(cudaStreamWaitEvent(r.side, tev, 0));
-                pub = r.side;
+                FRZ_CUDA_TRY(cudaStreamWaitEvent(r.side.get(), tev, 0));
+                pub = r.side.get();
             }
             k_publish_table<<<1, 256, 0, pub>>>(r.table_dev + ((size_t)parity * world + r.rank) * kTableBins, d_table, bins,
                                                 reinterpret_cast<volatile unsigned long long*>(r.ctrl_dev + kCtrlTable + parity * kMaxWorld + r.rank), seq);
@@ -826,7 +808,7 @@ frz_status rank_step(frz_comm* c, RankCtx& r, frz_matcher* m, const frz_corpus* 
         // ---- P2P PLACEMENT: only MY run's rows of pos0 / gt are needed; k_place stores every element of my run at its merged
         // position inside the owning rank's slice buffer (peer memory over NVLink) and ends when all peers have done the same
         auto gt_at = [&](int q, int sc) -> uint64_t { return by_score ? (uint64_t)tab_host[(size_t)q * kTableBins + sc] : 0ull; };
-        uint64_t* hp = reinterpret_cast<uint64_t*>(r.h_pos0);
+        uint64_t* hp = reinterpret_cast<uint64_t*>(r.h_pos0.get());
         uint32_t* hg = reinterpret_cast<uint32_t*>(hp + bins);
         for (int sc = bins - 1; sc >= 0; sc--) {
             uint64_t acc = 0;
@@ -838,19 +820,18 @@ frz_status rank_step(frz_comm* c, RankCtx& r, frz_matcher* m, const frz_corpus* 
                 acc += (sc == 0 ? counts[q] : gt_at(q, sc - 1)) - gtq;
             }
         }
-        FRZ_CUDA_TRY(cudaMemcpyAsync(r.d_pos0, r.h_pos0, (size_t)bins * (sizeof(uint64_t) + sizeof(uint32_t)), cudaMemcpyHostToDevice, main));
+        FRZ_CUDA_TRY(cudaMemcpyAsync(r.d_pos0.get(), r.h_pos0.get(), (size_t)bins * (sizeof(uint64_t) + sizeof(uint32_t)), cudaMemcpyHostToDevice, main));
         PlaceMeta meta;
         memset(&meta, 0, sizeof meta);
         for (int q = 0; q < world; q++) meta.peer[q] = r.peer_raw[q];
         for (int p2 = 0; p2 <= world; p2++) meta.lo[p2] = lo_p[p2];
         meta.total = kp; meta.world = world; meta.rank = r.rank; meta.bins = bins; meta.parity = parity;
         const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((kept[r.rank] + 255) / 256, (uint64_t)frz_sm_count() * 4));
-        k_place<<<grid, 256, 0, main>>>(r.run, kept[r.rank], meta, reinterpret_cast<const unsigned long long*>(r.d_pos0),
-                                         reinterpret_cast<const uint32_t*>(r.d_pos0 + bins), seq, (unsigned long long)(poll_timeout_s() * 1e9),
+        k_place<<<grid, 256, 0, main>>>(r.run.get(), kept[r.rank], meta, r.d_pos0.get(), reinterpret_cast<const uint32_t*>(r.d_pos0.get() + bins), seq, (unsigned long long)(poll_timeout_s() * 1e9),
                                          reinterpret_cast<volatile unsigned long long*>(r.ctrl_dev + kCtrlPlaceErr + r.rank));
         FRZ_CUDA_TRY(cudaGetLastError());
         placed = true;
-        d_final = reinterpret_cast<const FrzMatchDev*>(r.place_raw + kPlaceHeaderBytes);
+        d_final = reinterpret_cast<const FrzMatchDev*>(r.place_raw.get() + kPlaceHeaderBytes);
         d_final_first = lo_p[r.rank];
       } else {
         static thread_local std::vector<uint64_t> A;
@@ -865,7 +846,7 @@ frz_status rank_step(frz_comm* c, RankCtx& r, frz_matcher* m, const frz_corpus* 
                 const uint64_t gtq = gt_of(q, sc);
                 const uint64_t ge = sc == 0 ? counts[q] : gt_of(q, sc - 1);
                 const uint64_t size = ge - gtq;
-                r.h_pos0[(size_t)q * bins + sc] = acc;
+                r.h_pos0.get()[(size_t)q * bins + sc] = acc;
                 r.h_gt[(size_t)q * bins + sc] = (uint32_t)gtq;
                 if (size) {
                     for (int p2 = 0; p2 <= world; p2++) {
@@ -879,18 +860,8 @@ frz_status rank_step(frz_comm* c, RankCtx& r, frz_matcher* m, const frz_corpus* 
         // 3. ONE grouped exchange: to every rank p the part of my run it needs, from every run q the part I need
         const uint64_t lo = lo_p[r.rank], hi = lo_p[r.rank + 1];
         const uint64_t mine = hi - lo;
-        if (r.recv_cap < std::max<uint64_t>(mine, 1)) {
-            cudaFree(r.recv); r.recv = nullptr; r.recv_cap = 0;
-            const uint64_t want = mine + mine / 4 + 1024;
-            FRZ_CUDA_TRY(cudaMalloc(&r.recv, want * sizeof(FrzMatchDev)));
-            r.recv_cap = want;
-        }
-        if (r.merged_cap < std::max<uint64_t>(mine, 1)) {
-            cudaFree(r.merged); r.merged = nullptr; r.merged_cap = 0;
-            const uint64_t want = mine + mine / 4 + 1024;
-            FRZ_CUDA_TRY(cudaMalloc(&r.merged, want * sizeof(FrzMatchDev)));
-            r.merged_cap = want;
-        }
+        FRZ_TRY(r.recv.reserve(std::max<uint64_t>(mine, 1), mine + mine / 4 + 1024));
+        FRZ_TRY(r.merged.reserve(std::max<uint64_t>(mine, 1), mine + mine / 4 + 1024));
         SliceMeta meta;
         memset(&meta, 0, sizeof meta);
         meta.lo = lo;
@@ -903,62 +874,51 @@ frz_status rank_step(frz_comm* c, RankCtx& r, frz_matcher* m, const frz_corpus* 
         }
         if (off != mine) return frz_fail(FRZ_ERR_NCCL, "slice exchange: the ranks' score tables are inconsistent (%llu != %llu)",
                                          (unsigned long long)off, (unsigned long long)mine);
-        FRZ_CUDA_TRY(cudaMemcpyAsync(r.d_pos0, r.h_pos0, (size_t)world * kTableBins * (sizeof(unsigned long long) + sizeof(uint32_t)),
+        FRZ_CUDA_TRY(cudaMemcpyAsync(r.d_pos0.get(), r.h_pos0.get(), (size_t)world * kTableBins * (sizeof(unsigned long long) + sizeof(uint32_t)),
                                      cudaMemcpyHostToDevice, main));   // pos0 and gt in one copy (fixed layout, <= 96 KB)
         FRZ_NCCL_TRY(nccl_api().GroupStart());
         for (int p2 = 0; p2 < world; p2++) {
             const uint64_t a = A[(size_t)r.rank * (world + 1) + p2], b = A[(size_t)r.rank * (world + 1) + p2 + 1];
-            if (b > a) FRZ_NCCL_TRY(nccl_api().Send(r.run + a, (size_t)(b - a), ncclUint64, p2, r.nccl, main));
+            if (b > a) FRZ_NCCL_TRY(nccl_api().Send(r.run.get() + a, (size_t)(b - a), ncclUint64, p2, r.nccl, main));
         }
         for (int q = 0; q < world; q++)
-            if (meta.n[q]) FRZ_NCCL_TRY(nccl_api().Recv(r.recv + meta.off[q], (size_t)meta.n[q], ncclUint64, q, r.nccl, main));
+            if (meta.n[q]) FRZ_NCCL_TRY(nccl_api().Recv(r.recv.get() + meta.off[q], (size_t)meta.n[q], ncclUint64, q, r.nccl, main));
         FRZ_NCCL_TRY(nccl_api().GroupEnd());
         // 4. my slice of the k-way merge
         if (mine) {
             const dim3 grid((unsigned)std::max<uint64_t>(1, std::min<uint64_t>((longest + 255) / 256, frz_sm_count() * 4 / world + 1)), (unsigned)world);
-            k_slice_scatter<<<grid, 256, 0, main>>>(r.recv, meta, r.d_gt, r.d_pos0, bins, r.merged);
+            k_slice_scatter<<<grid, 256, 0, main>>>(r.recv.get(), meta, r.d_gt, r.d_pos0.get(), bins, r.merged.get());
             FRZ_CUDA_TRY(cudaGetLastError());
         }
-        d_final = r.merged;
+        d_final = r.merged.get();
         d_final_first = lo;
       }
     } else if (collective) {
-        if (r.run_cap < stride) {
+        if (r.run.cap() < stride) {
             // another rank's run is longer than this rank's whole shard (ceil partitioning leaves the last shard short, or
             // empty): the all-gather reads `stride` elements from every rank, so move the run into a buffer that long
-            FrzMatchDev* bigger = nullptr;
-            FRZ_CUDA_TRY(cudaMalloc(&bigger, stride * sizeof(FrzMatchDev)));
-            FRZ_CUDA_TRY(cudaMemcpyAsync(bigger, r.run, kept[r.rank] * sizeof(FrzMatchDev), cudaMemcpyDeviceToDevice, main));
+            FrzDevArray<FrzMatchDev> bigger;
+            FRZ_TRY(bigger.reserve(stride));
+            FRZ_CUDA_TRY(cudaMemcpyAsync(bigger.get(), r.run.get(), kept[r.rank] * sizeof(FrzMatchDev), cudaMemcpyDeviceToDevice, main));
             FRZ_CUDA_TRY(cudaStreamSynchronize(main));
-            cudaFree(r.run);
-            r.run = bigger;
-            r.run_cap = stride;
+            r.run = std::move(bigger);
         }
         const uint64_t need = (uint64_t)world * stride;
-        if (r.gathered_cap < need) {
-            cudaFree(r.gathered); r.gathered = nullptr; r.gathered_cap = 0;
-            const uint64_t want = need + need / 4 + 1024;
-            FRZ_CUDA_TRY(cudaMalloc(&r.gathered, want * sizeof(FrzMatchDev)));
-            r.gathered_cap = want;
-        }
-        if (r.merged_cap < kept_total) {
-            cudaFree(r.merged); r.merged = nullptr; r.merged_cap = 0;
-            const uint64_t want = kept_total + kept_total / 4 + 1024;
-            FRZ_CUDA_TRY(cudaMalloc(&r.merged, want * sizeof(FrzMatchDev)));
-            r.merged_cap = want;
-        }
+        FRZ_TRY(r.gathered.reserve(need, need + need / 4 + 1024));
+        FRZ_TRY(r.merged.reserve(kept_total, kept_total + kept_total / 4 + 1024));
         // ---- THE collective: one all-gather of the per-shard (score, index) runs over NVLink
         if (r.nccl) {
-            FRZ_NCCL_TRY(nccl_api().AllGather(r.run, r.gathered, (size_t)stride, ncclUint64, r.nccl, main));
+            FRZ_NCCL_TRY(nccl_api().AllGather(r.run.get(), r.gathered.get(), (size_t)stride, ncclUint64, r.nccl, main));
         } else {   // world 1 without a communicator (local form + force flag): the gather of one run is a copy
-            FRZ_CUDA_TRY(cudaMemcpyAsync(r.gathered, r.run, stride * sizeof(FrzMatchDev), cudaMemcpyDeviceToDevice, main));
+            FRZ_CUDA_TRY(cudaMemcpyAsync(r.gathered.get(), r.run.get(), stride * sizeof(FrzMatchDev), cudaMemcpyDeviceToDevice, main));
         }
         // ---- k_merge_matches_by on this GPU (of the runs' kept prefixes: the merged list's first K' are the same)
-        FRZ_TRY(frz_merge_runs_ex(r.merge, r.gathered, stride, kept, world, frz_matcher_sort(m), frz_matcher_score_bound(m), r.merged, main));
-        d_final = r.merged;
+        FRZ_TRY(frz_merge_runs_ex(r.merge, r.gathered.get(), stride, kept, world, frz_matcher_sort(m), frz_matcher_score_bound(m),
+                                  r.merged.get(), main));
+        d_final = r.merged.get();
     }
     res->d_merged = slice_form ? nullptr : d_final;
-    FRZ_CUDA_TRY(cudaEventRecord(r.ev[2], main));
+    FRZ_CUDA_TRY(cudaEventRecord(r.ev[2].get(), main));
     if (want_host) {
         if (kp > cap) {   // every rank sees the same counts, so every rank takes this exit: no collective is left unbalanced
             FRZ_CUDA_TRY(cudaStreamSynchronize(main));
@@ -970,7 +930,7 @@ frz_status rank_step(frz_comm* c, RankCtx& r, frz_matcher* m, const frz_corpus* 
         if (hi > lo)
             FRZ_CUDA_TRY(cudaMemcpyAsync(out_host + lo, d_final + (lo - d_final_first), (hi - lo) * sizeof(FrzMatchDev), cudaMemcpyDeviceToHost, main));
     }
-    FRZ_CUDA_TRY(cudaEventRecord(r.ev[3], main));
+    FRZ_CUDA_TRY(cudaEventRecord(r.ev[3].get(), main));
     r.ev_valid = true;
     if (want_host && !c->local_form && world > 1) {
         // "my slice has landed", stream-ordered after the copy; the call returns once every rank has said so
@@ -1272,11 +1232,11 @@ extern "C" frz_status frz_comm_last_timings(frz_comm* c, int local_index, float*
         ms4[0] = ms4[1] = ms4[2] = ms4[3] = 0;
         if (r.ev_valid) {
             FRZ_TRY(set_device(r.device));
-            FRZ_CUDA_TRY(cudaEventSynchronize(r.ev[3]));
-            cudaEventElapsedTime(&ms4[0], r.ev[0], r.ev[1]);
-            cudaEventElapsedTime(&ms4[1], r.ev[1], r.ev[2]);
-            cudaEventElapsedTime(&ms4[2], r.ev[2], r.ev[3]);
-            cudaEventElapsedTime(&ms4[3], r.ev[0], r.ev[3]);
+            FRZ_CUDA_TRY(cudaEventSynchronize(r.ev[3].get()));
+            cudaEventElapsedTime(&ms4[0], r.ev[0].get(), r.ev[1].get());
+            cudaEventElapsedTime(&ms4[1], r.ev[1].get(), r.ev[2].get());
+            cudaEventElapsedTime(&ms4[2], r.ev[2].get(), r.ev[3].get());
+            cudaEventElapsedTime(&ms4[3], r.ev[0].get(), r.ev[3].get());
             cudaGetLastError();
         }
     }

@@ -764,17 +764,17 @@ frz_status frz_launch_prefilter_list(const FrzCorpusView& cv, const FrzPatternDe
     if (cv.n_tiles == 0) return FRZ_OK;
     const bool is_long = pat.n > FRZ_MAX_NEEDLE;
     const size_t smem = is_long ? 0 : sizeof(OccTable) * kWarps;
-    FRZ_CUDA_TRY(cudaMemsetAsync(ws.surv_bitmap, 0, (size_t)cv.n_tiles * 32 * sizeof(uint32_t), stream));
+    FRZ_CUDA_TRY(cudaMemsetAsync(ws.surv_bitmap.get(), 0, (size_t)cv.n_tiles * 32 * sizeof(uint32_t), stream));
     if (n_cand == 0) return FRZ_OK;
     const uint32_t grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)frz_sm_count() * 4, (n_cand + kThreads - 1) / kThreads));
 #define FRZ_PFL_LAUNCH(MODE)                                                                                          \
     do {                                                                                                              \
         if (is_long) {                                                                                                \
             k_prefilter_list_long<MODE><<<grid, kThreads, smem, stream>>>(cv, pat, cand, n_cand, index_offset, ws.lists(), \
-                                                                          ws.survivor_cap, ws.surv_bitmap, ws.counters, ntab); \
+                                                                          ws.survivor_cap(), ws.surv_bitmap.get(), ws.counters.get(), ntab); \
         } else {                                                                                                      \
             k_prefilter_list<MODE><<<grid, kThreads, smem, stream>>>(cv, pat, cand, n_cand, index_offset, ws.lists(), \
-                                                                     ws.survivor_cap, ws.surv_bitmap, ws.counters);   \
+                                                                     ws.survivor_cap(), ws.surv_bitmap.get(), ws.counters.get());   \
         }                                                                                                             \
     } while (0)
     switch (pat.typo_mode) {
@@ -797,7 +797,7 @@ frz_status frz_launch_prefilter_list(const FrzCorpusView& cv, const FrzPatternDe
 frz_status frz_launch_sig_scan(const FrzCorpusView& cv, const FrzPatternDev& pat, FrzWorkspace& ws, cudaStream_t stream, FrzLaunchStats* st) {
     if (cv.n_tiles == 0) return FRZ_OK;
     const int sms = frz_sm_count();
-    CandRec* cand = reinterpret_cast<CandRec*>(ws.cand_list);
+    CandRec* cand = reinterpret_cast<CandRec*>(ws.cand_list.get());
     {   // persistent warps, as many blocks as fit
         const uint32_t total_chunks = cv.n_tiles * (FRZ_TILE / 128);
         const int use_sig = pat.typo_mode != FRZ_T_NONE && pat.sig_on;
@@ -811,7 +811,7 @@ frz_status frz_launch_sig_scan(const FrzCorpusView& cv, const FrzPatternDev& pat
         }
         const uint32_t grid = std::max<uint32_t>(1, std::min<uint32_t>((uint32_t)(sms * bps), (total_chunks + kScanWarps - 1) / kScanWarps));
         k_sig_scan<<<grid, kScanThreads, smem, stream>>>(cv, use_sig, pat.sig_need1, pat.sig_need2, pat.sig_k, pat.min_hay_len, cand,
-                                                         ws.cand_cap, ws.counters);
+                                                         ws.cand_list.cap(), ws.counters.get());
     }
     FRZ_CUDA_TRY(cudaGetLastError());
     if (st) st->launches++;
@@ -824,7 +824,7 @@ frz_status frz_launch_prefilter(const FrzCorpusView& cv, const FrzPatternDev& pa
                                 FrzLaunchStats* st, const FrzNeedleTab* ntab) {
     if (cv.n_tiles == 0) return FRZ_OK;
     const int sms = frz_sm_count();
-    FRZ_CUDA_TRY(cudaMemsetAsync(ws.surv_bitmap, 0, (size_t)cv.n_tiles * 32 * sizeof(uint32_t), stream));
+    FRZ_CUDA_TRY(cudaMemsetAsync(ws.surv_bitmap.get(), 0, (size_t)cv.n_tiles * 32 * sizeof(uint32_t), stream));
     const int use_sig = pat.typo_mode != FRZ_T_NONE && pat.sig_on;
     const int occ_rows = pat.n_distinct ? std::min(kMaxDistinct, pat.n_distinct + pat.n) : 0;
     const uint32_t total_chunks = cv.n_tiles * (FRZ_TILE / 128);
@@ -840,8 +840,8 @@ frz_status frz_launch_prefilter(const FrzCorpusView& cv, const FrzPatternDev& pa
             if (bps < 1) bps = 1;                                                                                        \
         }                                                                                                                \
         const uint32_t grid = std::max<uint32_t>(1, std::min<uint32_t>((uint32_t)(sms * bps), (total_chunks + kWarps - 1) / kWarps)); \
-        k_scan_window_long<MODE><<<grid, kThreads, smem, stream>>>(cv, pat, use_sig, 0, ws.lists(), ws.survivor_cap,     \
-                                                                   ws.surv_bitmap, ws.counters, ntab);                   \
+        k_scan_window_long<MODE><<<grid, kThreads, smem, stream>>>(cv, pat, use_sig, 0, ws.lists(), ws.survivor_cap(),     \
+                                                                   ws.surv_bitmap.get(), ws.counters.get(), ntab);                   \
     } while (0)
         switch (pat.typo_mode) {
             case FRZ_T_0: FRZ_PF_LAUNCH_LONG(FRZ_T_0); break;
@@ -869,8 +869,8 @@ frz_status frz_launch_prefilter(const FrzCorpusView& cv, const FrzPatternDev& pa
             if (bps < 1) bps = 1;                                                                                        \
         }                                                                                                                \
         const uint32_t grid = std::max<uint32_t>(1, std::min<uint32_t>((uint32_t)(sms * bps), (total_chunks + kWarps - 1) / kWarps)); \
-        k_scan_window<MODE><<<grid, kThreads, smem, stream>>>(cv, pat, use_sig, occ_rows, ws.lists(), ws.survivor_cap,   \
-                                                              ws.surv_bitmap, ws.counters);                              \
+        k_scan_window<MODE><<<grid, kThreads, smem, stream>>>(cv, pat, use_sig, occ_rows, ws.lists(), ws.survivor_cap(),   \
+                                                              ws.surv_bitmap.get(), ws.counters.get());                              \
     } while (0)
     switch (pat.typo_mode) {
         case FRZ_T_0: FRZ_PF_LAUNCH(FRZ_T_0); break;
@@ -890,10 +890,10 @@ frz_status frz_launch_prefilter(const FrzCorpusView& cv, const FrzPatternDev& pa
 frz_status frz_launch_tile_scan(const FrzCorpusView& cv, FrzWorkspace& ws, cudaStream_t stream, FrzLaunchStats* st,
                                 unsigned long long* carry) {
     if (cv.n_tiles) {
-        k_tile_rank<<<(cv.n_tiles * 32 + 255) / 256, 256, 0, stream>>>(ws.surv_bitmap, ws.word_prefix, ws.tile_count, cv.n_tiles);
+        k_tile_rank<<<(cv.n_tiles * 32 + 255) / 256, 256, 0, stream>>>(ws.surv_bitmap.get(), ws.word_prefix.get(), ws.tile_count.get(), cv.n_tiles);
         if (st) st->launches++;
     }
-    k_tile_scan<<<1, 1024, 0, stream>>>(ws.tile_count, ws.tile_out_base, cv.n_tiles, ws.counters, carry);
+    k_tile_scan<<<1, 1024, 0, stream>>>(ws.tile_count.get(), ws.tile_out_base.get(), cv.n_tiles, ws.counters.get(), carry);
     FRZ_CUDA_TRY(cudaGetLastError());
     if (st) st->launches++;
     return FRZ_OK;

@@ -273,21 +273,22 @@ __global__ void __launch_bounds__(kSegThreads) k_sort_scatter_seg(const FrzMatch
 
 // n_ptr: device pointer to the element count.  score_bound: host-known upper bound of any score.
 frz_status frz_launch_sort_by_score_dev(const FrzMatchDev* d_in, FrzMatchDev* d_tmp, FrzMatchDev* d_out,
-                                        const unsigned long long* n_ptr, uint32_t score_bound, FrzWorkspace& ws,
+                                        const unsigned long long* n_ptr, uint32_t score_bound, FrzSortScratch& ss,
                                         cudaStream_t stream, FrzLaunchStats* st, uint32_t limit) {
+    uint32_t* const hist = ss.hist.get();
     auto pass = [&](const FrzMatchDev* src, FrzMatchDev* dst, int shift, int bins, uint32_t keep) -> frz_status {
         const size_t smem = (size_t)kSortWarps * bins * sizeof(uint32_t);
-        k_sort_hist<<<kSortBlocks, kSortWarps * 32, smem, stream>>>(src, n_ptr, shift, bins, ws.sort_hist);
-        uint32_t* totals = ws.sort_hist + (size_t)kMaxBins * kV;
+        k_sort_hist<<<kSortBlocks, kSortWarps * 32, smem, stream>>>(src, n_ptr, shift, bins, hist);
+        uint32_t* totals = hist + (size_t)kMaxBins * kV;
         uint32_t* digit_base = totals + kMaxBins;
         unsigned int* done_counter = reinterpret_cast<unsigned int*>(digit_base + kMaxBins);   // zeroed at allocation, self-resetting
-        k_sort_scan_rows<kV / 128, false><<<(bins + 7) / 8, 256, 0, stream>>>(ws.sort_hist, ws.sort_hist, kV, nullptr, bins, totals,
+        k_sort_scan_rows<kV / 128, false><<<(bins + 7) / 8, 256, 0, stream>>>(hist, hist, kV, nullptr, bins, totals,
                                                                                digit_base, done_counter);
-        if (ws.arm_table_ev && ws.table_ev) {   // digit_base is final: the multi-GPU layer publishes it while the scatter runs
-            FRZ_CUDA_TRY(cudaEventRecord(ws.table_ev, stream));
-            ws.table_ev_recorded = true;
+        if (ss.arm_table_ev && ss.table_ev) {   // digit_base is final: the multi-GPU layer publishes it while the scatter runs
+            FRZ_CUDA_TRY(cudaEventRecord(ss.table_ev.get(), stream));
+            ss.table_ev_recorded = true;
         }
-        k_sort_scatter<<<kSortBlocks, kSortWarps * 32, smem, stream>>>(src, dst, n_ptr, shift, bins, ws.sort_hist, digit_base, keep);
+        k_sort_scatter<<<kSortBlocks, kSortWarps * 32, smem, stream>>>(src, dst, n_ptr, shift, bins, hist, digit_base, keep);
         FRZ_CUDA_TRY(cudaGetLastError());
         if (st) st->launches += 3;
         return FRZ_OK;
@@ -300,58 +301,56 @@ frz_status frz_launch_sort_by_score_dev(const FrzMatchDev* d_in, FrzMatchDev* d_
     return pass(d_tmp, d_out, 8, 256, limit);
 }
 
-size_t frz_sort_hist_words() { return (size_t)kMaxBins * kV + 2 * kMaxBins + 4; }   // + the pass-completion counter (must start at zero)
-// allocates the sort scratch on the current device (the completion counter of k_sort_scan_rows starts at zero)
-frz_status frz_sort_hist_alloc(uint32_t** out) {
-    FRZ_CUDA_TRY(cudaMalloc(out, frz_sort_hist_words() * sizeof(uint32_t)));
-    FRZ_CUDA_TRY(cudaMemset(*out + (size_t)kMaxBins * kV + 2 * kMaxBins, 0, 4 * sizeof(uint32_t)));
+// allocates the sort scratch on the current device: counts, totals, digit_base + the pass-completion counter of
+// k_sort_scan_rows, which must start at zero
+frz_status frz_sort_hist_alloc(FrzDevArray<uint32_t>& out) {
+    FRZ_TRY(out.reserve((size_t)kMaxBins * kV + 2 * kMaxBins + 4));
+    FRZ_CUDA_TRY(cudaMemset(out.get() + (size_t)kMaxBins * kV + 2 * kMaxBins, 0, 4 * sizeof(uint32_t)));
     return FRZ_OK;
 }
 
-// digit_base[d] of the LAST pass run on this workspace = number of elements whose digit is greater than d.  After a
+// digit_base[d] of the LAST pass run with this scratch = number of elements whose digit is greater than d.  After a
 // single-pass sort (score bound < 1024) that is, per score s, how many matches of the run score higher than s — the table
 // the multi-GPU slice exchange needs (parallel.cu) — so nobody has to binary-search the sorted run for it.
-const uint32_t* frz_sort_digit_base(const FrzWorkspace& ws) { return ws.sort_hist ? ws.sort_hist + (size_t)kMaxBins * kV + kMaxBins : nullptr; }
+const uint32_t* frz_sort_digit_base(const FrzSortScratch& ss) { return ss.hist.get() ? ss.hist.get() + (size_t)kMaxBins * kV + kMaxBins : nullptr; }
 int frz_sort_single_pass_bins(uint32_t score_bound) { return score_bound < 256 ? 256 : score_bound < 512 ? 512 : score_bound < 1024 ? 1024 : 0; }
 
-// fused_hist holds the counts ([bins][stride]) and then the scan's prefix rows (same shape).  The counts are zero between
+// ss.fused holds the counts ([bins][stride]) and then the scan's prefix rows (same shape).  The counts are zero between
 // calls (the scan re-zeroes every word the scoring kernels can have touched), so only growth, a new layout reaching past
 // the words known to be zero, or a call that stopped between scoring and scan costs a memset.
-frz_status frz_sort_fused_prepare(FrzWorkspace& ws, uint64_t n_cap, uint32_t score_bound, cudaStream_t stream, FrzScoreHist* out) {
+frz_status frz_sort_fused_prepare(FrzSortScratch& ss, uint64_t n_cap, uint32_t score_bound, cudaStream_t stream, FrzScoreHist* out) {
     const int bins = frz_sort_single_pass_bins(score_bound);
     if (bins == 0) return frz_fail(FRZ_ERR_INVALID_ARG, "fused sort needs a score bound below 1024 (got %u)", score_bound);
     const uint64_t segs = (n_cap + (1ull << kFrzSortSegShift) - 1) >> kFrzSortSegShift;
     const uint64_t stride = std::max<uint64_t>((segs + 3) & ~3ull, 4);
     const uint64_t words = (uint64_t)bins * stride;
-    if (ws.fused_hist_cap < 2 * words) {
-        cudaFree(ws.fused_hist);
-        ws.fused_hist = nullptr; ws.fused_hist_cap = 0; ws.fused_clean_words = 0;
-        FRZ_CUDA_TRY(cudaMalloc(&ws.fused_hist, 2 * words * sizeof(uint32_t)));
-        ws.fused_hist_cap = 2 * words;
+    if (ss.fused.cap() < 2 * words) {
+        ss.fused_clean_words = 0;
+        FRZ_TRY(ss.fused.reserve(2 * words));
     }
-    if (ws.fused_hist_dirty || ws.fused_clean_words < words)
-        FRZ_CUDA_TRY(cudaMemsetAsync(ws.fused_hist, 0, words * sizeof(uint32_t), stream));
-    ws.fused_clean_words = words;   // the prefix rows are written right behind the counts
-    ws.fused_hist_dirty = true;
-    out->counts = ws.fused_hist;
+    if (ss.fused_dirty || ss.fused_clean_words < words)
+        FRZ_CUDA_TRY(cudaMemsetAsync(ss.fused.get(), 0, words * sizeof(uint32_t), stream));
+    ss.fused_clean_words = words;   // the prefix rows are written right behind the counts
+    ss.fused_dirty = true;
+    out->counts = ss.fused.get();
     out->stride = (uint32_t)stride;
     out->mask = (uint32_t)bins - 1;
     return FRZ_OK;
 }
 
 frz_status frz_launch_sort_fused(const FrzMatchDev* d_in, FrzMatchDev* d_out, const unsigned long long* n_ptr, const FrzScoreHist& h,
-                                 FrzWorkspace& ws, cudaStream_t stream, FrzLaunchStats* st, uint32_t limit) {
+                                 FrzSortScratch& ss, cudaStream_t stream, FrzLaunchStats* st, uint32_t limit) {
     const int bins = (int)h.mask + 1;
     uint32_t* pref = h.counts + (size_t)bins * h.stride;
-    uint32_t* totals = ws.sort_hist + (size_t)kMaxBins * kV;
+    uint32_t* totals = ss.hist.get() + (size_t)kMaxBins * kV;
     uint32_t* digit_base = totals + kMaxBins;
     unsigned int* done_counter = reinterpret_cast<unsigned int*>(digit_base + kMaxBins);
     k_sort_scan_rows<4, true><<<(bins + 7) / 8, 256, 0, stream>>>(h.counts, pref, h.stride, n_ptr, bins, totals, digit_base, done_counter);
     FRZ_CUDA_TRY(cudaGetLastError());
-    ws.fused_hist_dirty = false;
-    if (ws.arm_table_ev && ws.table_ev) {   // digit_base is final: the multi-GPU layer publishes it while the scatter runs
-        FRZ_CUDA_TRY(cudaEventRecord(ws.table_ev, stream));
-        ws.table_ev_recorded = true;
+    ss.fused_dirty = false;
+    if (ss.arm_table_ev && ss.table_ev) {   // digit_base is final: the multi-GPU layer publishes it while the scatter runs
+        FRZ_CUDA_TRY(cudaEventRecord(ss.table_ev.get(), stream));
+        ss.table_ev_recorded = true;
     }
     const size_t smem = (size_t)kSegWarps * bins * sizeof(uint32_t);
     const int grid = (int)std::max<uint32_t>(1, std::min<uint32_t>(h.stride, (uint32_t)frz_sm_count() * 4));

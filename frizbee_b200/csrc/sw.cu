@@ -43,7 +43,7 @@ struct FrzRankView {
     const uint32_t* surv_bitmap;
     const uint16_t* word_prefix;
 };
-FrzRankView rank_view(const FrzWorkspace& ws) { return FrzRankView{ws.tile_out_base, ws.surv_bitmap, ws.word_prefix}; }
+FrzRankView rank_view(const FrzWorkspace& ws) { return FrzRankView{ws.tile_out_base.get(), ws.surv_bitmap.get(), ws.word_prefix.get()}; }
 
 
 // decoded window record (FrzSurvivor, window-class layout)
@@ -542,8 +542,8 @@ frz_status launch_sw_long(const FrzCorpusView& cv, const FrzPatternDev& pat, con
         FRZ_CUDA_TRY(cudaFuncSetAttribute(k_sw_long<L>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max));
         attr_set = true;
     }
-    k_sw_long<L><<<frz_sm_count() * 4, kLongWarps * 32, smem, stream>>>(cv, pat, ntab, ws.lists(), ws.survivor_cap, rank_view(ws),
-                                                                         ws.counters, index_offset, reversed ? 1 : 0, d_out, hist,
+    k_sw_long<L><<<frz_sm_count() * 4, kLongWarps * 32, smem, stream>>>(cv, pat, ntab, ws.lists(), ws.survivor_cap(), rank_view(ws),
+                                                                         ws.counters.get(), index_offset, reversed ? 1 : 0, d_out, hist,
                                                                          (uint32_t)warp_smem);
     FRZ_CUDA_TRY(cudaGetLastError());
     return FRZ_OK;
@@ -560,13 +560,13 @@ frz_status launch_sw_lanes(const FrzCorpusView& cv, const FrzPatternDev& pat, ui
     const bool lane_pen = !pat.wrap8 && pat.gap_extend == 0 && pat.gap_open_x > 0;
     if (pat.wrap8)
         k_sw64<LANES, true><<<frz_sm_count() * kSw64MinBlocks<LANES, true>, kSwThreads, 0, stream>>>(
-            cv, pat, ws.lists(), ws.survivor_cap, rank_view(ws), ws.counters, index_offset, rev, d_out, hist);
+            cv, pat, ws.lists(), ws.survivor_cap(), rank_view(ws), ws.counters.get(), index_offset, rev, d_out, hist);
     else if (lane_pen)
         k_sw64<LANES, false, 8 | kSwVarLanePen><<<frz_sm_count() * kSw64MinBlocks<LANES, false>, kSwThreads, 0, stream>>>(
-            cv, pat, ws.lists(), ws.survivor_cap, rank_view(ws), ws.counters, index_offset, rev, d_out, hist);
+            cv, pat, ws.lists(), ws.survivor_cap(), rank_view(ws), ws.counters.get(), index_offset, rev, d_out, hist);
     else
         k_sw64<LANES, false, 8><<<frz_sm_count() * kSw64MinBlocks<LANES, false>, kSwThreads, 0, stream>>>(
-            cv, pat, ws.lists(), ws.survivor_cap, rank_view(ws), ws.counters, index_offset, rev, d_out, hist);
+            cv, pat, ws.lists(), ws.survivor_cap(), rank_view(ws), ws.counters.get(), index_offset, rev, d_out, hist);
     // windows of 65..128 bytes only exist when some haystack of the corpus is longer than 64 bytes (recorded at pack time)
     if (cv.max_gunits <= 4) { FRZ_CUDA_TRY(cudaGetLastError()); return FRZ_OK; }
     const size_t smem = SwCore<LANES, 128, false>::smem_bytes;
@@ -579,15 +579,15 @@ frz_status launch_sw_lanes(const FrzCorpusView& cv, const FrzPatternDev& pat, ui
         attr_set = true;
     }
     if (pat.wrap8)
-        k_sw<LANES, 128, true><<<blocks, kSwThreads, smem, stream>>>(cv, pat, ws.survivors[FRZ_C_COLS128], ws.survivor_cap, FRZ_C_COLS128,
-                                                                    rank_view(ws), ws.counters, index_offset, rev, d_out, hist);
+        k_sw<LANES, 128, true><<<blocks, kSwThreads, smem, stream>>>(cv, pat, ws.survivors[FRZ_C_COLS128].get(), ws.survivor_cap(), FRZ_C_COLS128,
+                                                                    rank_view(ws), ws.counters.get(), index_offset, rev, d_out, hist);
     else if (lane_pen)
-        k_sw<LANES, 128, false, kSwVarLanePen><<<blocks, kSwThreads, smem, stream>>>(cv, pat, ws.survivors[FRZ_C_COLS128], ws.survivor_cap,
-                                                                                  FRZ_C_COLS128, rank_view(ws), ws.counters, index_offset,
+        k_sw<LANES, 128, false, kSwVarLanePen><<<blocks, kSwThreads, smem, stream>>>(cv, pat, ws.survivors[FRZ_C_COLS128].get(), ws.survivor_cap(),
+                                                                                  FRZ_C_COLS128, rank_view(ws), ws.counters.get(), index_offset,
                                                                                   rev, d_out, hist);
     else
-        k_sw<LANES, 128, false><<<blocks, kSwThreads, smem, stream>>>(cv, pat, ws.survivors[FRZ_C_COLS128], ws.survivor_cap, FRZ_C_COLS128,
-                                                                     rank_view(ws), ws.counters, index_offset, rev, d_out, hist);
+        k_sw<LANES, 128, false><<<blocks, kSwThreads, smem, stream>>>(cv, pat, ws.survivors[FRZ_C_COLS128].get(), ws.survivor_cap(), FRZ_C_COLS128,
+                                                                     rank_view(ws), ws.counters.get(), index_offset, rev, d_out, hist);
     FRZ_CUDA_TRY(cudaGetLastError());
     return FRZ_OK;
 }
@@ -599,7 +599,7 @@ frz_status frz_launch_sw(const FrzCorpusView& cv, const FrzPatternDev& pat, uint
                          const FrzNeedleTab* ntab) {
     if (cv.n_tiles == 0) return FRZ_OK;
     if (pat.typo_mode == FRZ_T_LITERAL) {
-        k_emit_literal<<<frz_sm_count() * 4, 256, 0, stream>>>(ws.survivors[FRZ_C_COLS64], ws.survivor_cap, rank_view(ws), ws.counters,
+        k_emit_literal<<<frz_sm_count() * 4, 256, 0, stream>>>(ws.survivors[FRZ_C_COLS64].get(), ws.survivor_cap(), rank_view(ws), ws.counters.get(),
                                                            index_offset, reversed ? 1 : 0, d_out, hist);
         FRZ_CUDA_TRY(cudaGetLastError());
         if (st) st->launches++;
@@ -608,8 +608,8 @@ frz_status frz_launch_sw(const FrzCorpusView& cv, const FrzPatternDev& pat, uint
     if (pat.n > FRZ_MAX_NEEDLE) {
         // per thread: the u8 family, and windows over FRZ_SW_MAX_WINDOW bytes (which need a longer haystack)
         if (pat.score_bits != 16 || cv.max_gunits * FRZ_UNIT > FRZ_SW_MAX_WINDOW) {
-            k_sw_long_thread<<<frz_sm_count() * 8, 64, 0, stream>>>(cv, pat, ntab, ws.lists(), ws.survivor_cap, rank_view(ws),
-                                                                     ws.counters, index_offset, reversed ? 1 : 0, d_out, hist);
+            k_sw_long_thread<<<frz_sm_count() * 8, 64, 0, stream>>>(cv, pat, ntab, ws.lists(), ws.survivor_cap(), rank_view(ws),
+                                                                     ws.counters.get(), index_offset, reversed ? 1 : 0, d_out, hist);
             FRZ_CUDA_TRY(cudaGetLastError());
             if (st) st->launches++;
         }
@@ -632,8 +632,8 @@ frz_status frz_launch_sw(const FrzCorpusView& cv, const FrzPatternDev& pat, uint
         default: return frz_fail(FRZ_ERR_INVALID_ARG, "unsupported lane count %d", pat.sw_lanes);
     }
     if (cv.max_gunits > 8) {   // windows > 128 bytes need a haystack > 128 bytes
-        k_sw_generic<<<frz_sm_count() * 2, 64, 0, stream>>>(cv, pat, ws.survivors[FRZ_C_GENERIC], ws.survivor_cap, FRZ_C_GENERIC, rank_view(ws),
-                                                        ws.counters, index_offset, reversed ? 1 : 0, d_out, hist);
+        k_sw_generic<<<frz_sm_count() * 2, 64, 0, stream>>>(cv, pat, ws.survivors[FRZ_C_GENERIC].get(), ws.survivor_cap(), FRZ_C_GENERIC, rank_view(ws),
+                                                        ws.counters.get(), index_offset, reversed ? 1 : 0, d_out, hist);
     }
     FRZ_CUDA_TRY(cudaGetLastError());
     if (st) st->launches += 1 + (cv.max_gunits > 4 ? 1 : 0) + (cv.max_gunits > 8 ? 1 : 0);

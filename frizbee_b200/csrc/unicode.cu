@@ -95,7 +95,7 @@ frz_status frz_launch_unicode(const FrzCorpusView& cv, const FrzPatternDev& pat,
                               const FrzMatchDev* cand, uint64_t n_cand, uint32_t index_offset, FrzWorkspace& ws,
                               cudaStream_t stream, FrzLaunchStats* st) {
     if (cv.n_tiles == 0) return FRZ_OK;
-    FRZ_CUDA_TRY(cudaMemsetAsync(ws.surv_bitmap, 0, (size_t)cv.n_tiles * 32 * sizeof(uint32_t), stream));
+    FRZ_CUDA_TRY(cudaMemsetAsync(ws.surv_bitmap.get(), 0, (size_t)cv.n_tiles * 32 * sizeof(uint32_t), stream));
     if (cand && n_cand == 0) return FRZ_OK;
     if (!cand) FRZ_TRY(frz_launch_sig_scan(cv, pat, ws, stream, st));   // length gate + signature test → candidate records
     const int sms = frz_sm_count();
@@ -104,14 +104,10 @@ frz_status frz_launch_unicode(const FrzCorpusView& cv, const FrzPatternDev& pat,
     // per-thread Smith-Waterman row state: previous-chunk rows + pending-gap-open vectors of every needle scalar
     const uint32_t stride = 2u * (uint32_t)(un.n + 1) * (uint32_t)pat.sw_lanes;
     const uint64_t need = (uint64_t)grid * kUThreads * stride;
-    if (ws.unicode_scratch_cap < need) {
-        cudaFree(ws.unicode_scratch); ws.unicode_scratch = nullptr; ws.unicode_scratch_cap = 0;
-        FRZ_CUDA_TRY(cudaMalloc(&ws.unicode_scratch, need * sizeof(uint16_t)));
-        ws.unicode_scratch_cap = need;
-    }
-    k_unicode<<<grid, kUThreads, 0, stream>>>(cv, pat, un, usc, cand, n_cand, reinterpret_cast<const uint4*>(ws.cand_list), ws.cand_cap,
-                                              index_offset, ws.lists(), ws.survivor_cap,
-                                              ws.surv_bitmap, ws.counters, ws.unicode_scratch, stride);
+    FRZ_TRY(ws.unicode_scratch.reserve(need));
+    k_unicode<<<grid, kUThreads, 0, stream>>>(cv, pat, un, usc, cand, n_cand, ws.cand_list.get(), ws.cand_list.cap(),
+                                              index_offset, ws.lists(), ws.survivor_cap(),
+                                              ws.surv_bitmap.get(), ws.counters.get(), ws.unicode_scratch.get(), stride);
     FRZ_CUDA_TRY(cudaGetLastError());
     if (st) st->launches++;
     return FRZ_OK;

@@ -370,6 +370,10 @@ FRZ_API frz_status frz_matcher_debug_pattern(const frz_matcher* m, size_t i, voi
 FRZ_API frz_status frz_corpus_debug_image(const frz_corpus* c, void* tile_base, void* groups, void* slot_meta, void* slot_of,
                                   void* slot_sig, void* units, uint64_t sizes[6]);
 
+/* Test aid: bytes of device memory the library holds right now, over every device (corpora, matchers, communicators
+ * and internal scratch).  Lets tests check that repeated calls and destroyed objects leave nothing behind. */
+FRZ_API uint64_t frz_debug_device_bytes(void);
+
 /* radix_sort_matches (src/sort.rs:6-40): stable, descending score; `matches` is host memory. */
 FRZ_API frz_status frz_radix_sort_matches(frz_match* matches, uint64_t n, int device);
 
