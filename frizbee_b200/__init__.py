@@ -69,6 +69,8 @@ def lib():
     L.frz_corpus_create.argtypes = [vp, vp, u64, C.c_int, C.POINTER(vp)]
     L.frz_corpus_create_arrow.argtypes = [vp, vp, C.c_int, u64, C.c_int, C.POINTER(vp)]
     L.frz_corpus_append.argtypes = [vp, vp, vp, C.c_int, u64]
+    L.frz_corpus_remove.argtypes = [vp, vp, u64]
+    L.frz_corpus_replace.argtypes = [vp, vp, u64, vp, vp, C.c_int]
     L.frz_corpus_create_ptrs.argtypes = [vp, vp, u64, C.c_int, C.POINTER(vp)]
     L.frz_corpus_create_device.argtypes = [vp, vp, u64, u64, C.c_int, vp, C.POINTER(vp)]
     for fn in (L.frz_corpus_len, L.frz_corpus_total_bytes, L.frz_corpus_device_bytes):
@@ -209,6 +211,28 @@ class Corpus:
     def append_list(self, haystacks: Sequence) -> "Corpus":
         data, offsets = pack_host(haystacks)
         return self.append(data, offsets)
+
+    def remove(self, which) -> "Corpus":
+        """Haystacks `which` stop matching; indices do not move (len(self) is unchanged).  Duplicates are allowed."""
+        which = np.ascontiguousarray(which, dtype=np.uint32)
+        _check(lib().frz_corpus_remove(self._h, which.ctypes.data if which.size else None, len(which)))
+        return self
+
+    def replace(self, which, data: np.ndarray, offsets: np.ndarray) -> "Corpus":
+        """Haystack which[j] becomes data[offsets[j], offsets[j + 1]) (Arrow value bytes + offsets); a removed one comes
+        back.  Only the tiles holding `which` are re-packed."""
+        which = np.ascontiguousarray(which, dtype=np.uint32)
+        data = np.ascontiguousarray(data, dtype=np.uint8)
+        offsets, width = _arrow_offsets(offsets)
+        if len(offsets) != len(which) + 1:
+            raise ValueError(f"{len(which)} indices need {len(which) + 1} offsets, got {len(offsets)}")
+        _check(lib().frz_corpus_replace(self._h, which.ctypes.data if which.size else None, len(which),
+                                        data.ctypes.data if data.size else None, offsets.ctypes.data, width))
+        return self
+
+    def replace_list(self, which, haystacks: Sequence) -> "Corpus":
+        data, offsets = pack_host(haystacks)
+        return self.replace(which, data, offsets)
 
     def __len__(self):
         return self.n

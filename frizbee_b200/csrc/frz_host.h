@@ -45,6 +45,8 @@ inline int frz_sm_count() {
 
 // Bytes held by all device FrzDevArrays (frz_debug_device_bytes).
 inline std::atomic<uint64_t> g_frz_device_bytes{0};
+// Their high-water mark since the last frz_debug_device_bytes_peak(reset != 0).
+inline std::atomic<uint64_t> g_frz_device_bytes_peak{0};
 
 // A grow-only array of T on one device (Pinned: in page-locked host memory).  It remembers the device it was allocated on
 // and frees the block there; an empty array makes no CUDA call, so host-only users never touch the runtime.
@@ -78,7 +80,11 @@ public:
         cudaGetDevice(&dev_);
         p_ = static_cast<T*>(p);
         cap_ = want;
-        if (!Pinned) g_frz_device_bytes += cap_ * sizeof(T);
+        if (!Pinned) {
+            const uint64_t now = g_frz_device_bytes += cap_ * sizeof(T);
+            uint64_t peak = g_frz_device_bytes_peak.load();
+            while (now > peak && !g_frz_device_bytes_peak.compare_exchange_weak(peak, now)) {}
+        }
         return FRZ_OK;
     }
     frz_status reserve(uint64_t n) { return reserve(n, n); }
@@ -132,9 +138,11 @@ struct FrzCorpusStorage {
     FrzDevArray<uint64_t> scratch_tile_units;  // [tile capacity] + 2 words (total, error)
     uint64_t n = 0;
     uint32_t n_tiles = 0;
-    uint64_t total_units = 0;
-    uint64_t total_bytes = 0;
-    uint32_t max_gunits = 0;   // longest haystack of the corpus in 16-byte units
+    uint64_t total_units = 0;  // end of the arena: units [0, total_units) are written
+    uint64_t total_bytes = 0;  // sum of the live haystacks' lengths
+    uint32_t max_gunits = 0;   // longest haystack of the corpus in 16-byte units (never below the truth)
+    uint64_t n_removed = 0;    // haystacks whose slot is FRZ_INVALID_SLOT (frz_corpus_remove); matching filters only when > 0
+    uint64_t dead_units = 0;   // arena units no tile points at any more (left behind by re-packed tiles)
     int device = 0;
 
     FrzCorpusView view() const {
@@ -165,7 +173,10 @@ struct FrzIngest {
 
 struct frz_corpus {
     FrzCorpusStorage st;
-    std::unique_ptr<FrzIngest> ingest;   // created by the first frz_corpus_append, kept for the next ones
+    std::unique_ptr<FrzIngest> ingest;   // created by the first frz_corpus_append / _remove / _replace, kept for the next ones
+    // metadata of the tiles a frz_corpus_replace re-packs (grow-only; a replace releases it, and the ingest staging, once
+    // they pass 64 MiB)
+    std::unique_ptr<FrzCorpusStorage> edit_tiles;
 };
 
 // pack.cu
@@ -173,6 +184,10 @@ frz_status frz_pack_corpus_device(const uint8_t* d_bytes, const void* d_offsets,
                                   cudaStream_t stream, FrzCorpusStorage* out);
 frz_status frz_append_host(FrzIngest& ing, const uint8_t* h_bytes, const void* h_offsets, int offset_width, uint64_t n_new,
                            cudaStream_t stream, FrzCorpusStorage* st);
+// In-place edits (the arguments are checked by the callers in host.cu, before anything changes).  Synchronous.
+frz_status frz_remove_host(FrzIngest& ing, const uint32_t* which, uint64_t n, cudaStream_t stream, FrzCorpusStorage* st);
+frz_status frz_replace_host(FrzIngest& ing, FrzCorpusStorage& scratch, const uint32_t* which, uint64_t n, const uint8_t* h_bytes,
+                            const void* h_offsets, int offset_width, cudaStream_t stream, FrzCorpusStorage* st);
 // `after_chunk` (optional) is called on the host right after the pack kernels of tiles [t0, t1) have been enqueued on
 // `stream` (chunks arrive in tile order; `last` marks the final one): the caller may enqueue work on those tiles at once.
 typedef frz_status (*FrzChunkFn)(void* ctx, uint32_t t0, uint32_t t1, bool last);

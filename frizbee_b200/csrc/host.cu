@@ -279,6 +279,67 @@ extern "C" frz_status frz_corpus_append(frz_corpus* c, const uint8_t* bytes, con
     return FRZ_OK;
 }
 
+// In-place edits.  Every check runs on the host before anything changes, so a refused call leaves the corpus as it was.
+static frz_status check_indices(const frz_corpus* c, const uint32_t* which, uint64_t n) {
+    for (uint64_t j = 0; j < n; j++)
+        if (which[j] >= c->st.n)
+            return frz_fail(FRZ_ERR_INVALID_ARG, "index %u out of range (the corpus has %llu haystacks)", which[j],
+                            (unsigned long long)c->st.n);
+    return FRZ_OK;
+}
+
+extern "C" frz_status frz_corpus_remove(frz_corpus* c, const uint32_t* which, uint64_t n) {
+    if (!c || (n && !which)) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    if (n == 0) return FRZ_OK;
+    FRZ_TRY(check_indices(c, which, n));
+    FRZ_TRY(ensure_device(c->st.device));
+    if (!c->ingest) c->ingest = std::make_unique<FrzIngest>();
+    return frz_remove_host(*c->ingest, which, n, nullptr, &c->st);
+}
+
+template <typename OffT>
+static frz_status check_replacement_lengths(const OffT* off, uint64_t n) {
+    for (uint64_t j = 0; j < n; j++) {
+        if (off[j + 1] < off[j]) return frz_fail(FRZ_ERR_INVALID_ARG, "offsets decrease at %llu", (unsigned long long)j);
+        if ((uint64_t)off[j + 1] - (uint64_t)off[j] > FRZ_MAX_HAY_LEN)
+            return frz_fail(FRZ_ERR_UNSUPPORTED, "haystack longer than %u bytes", FRZ_MAX_HAY_LEN);
+    }
+    return FRZ_OK;
+}
+
+extern "C" frz_status frz_corpus_replace(frz_corpus* c, const uint32_t* which, uint64_t n, const uint8_t* bytes, const void* offsets,
+                                         int offset_width) {
+    if (!c || (n && (!which || !offsets))) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    if (offset_width != 4 && offset_width != 8) return frz_fail(FRZ_ERR_INVALID_ARG, "offset_width must be 4 or 8");
+    if (n == 0) return FRZ_OK;
+    FRZ_TRY(check_indices(c, which, n));
+    std::vector<uint32_t> sorted(which, which + n);
+    std::sort(sorted.begin(), sorted.end());
+    for (uint64_t j = 1; j < n; j++)
+        if (sorted[j] == sorted[j - 1]) return frz_fail(FRZ_ERR_INVALID_ARG, "index %u is replaced twice", sorted[j]);
+    if (offset_width == 4) FRZ_TRY(check_replacement_lengths(static_cast<const uint32_t*>(offsets), n));
+    else FRZ_TRY(check_replacement_lengths(static_cast<const uint64_t*>(offsets), n));
+    const uint64_t r_bytes = offset_width == 4 ? (uint64_t)(static_cast<const uint32_t*>(offsets)[n] - static_cast<const uint32_t*>(offsets)[0])
+                                               : static_cast<const uint64_t*>(offsets)[n] - static_cast<const uint64_t*>(offsets)[0];
+    if (r_bytes && !bytes) return frz_fail(FRZ_ERR_INVALID_ARG, "null bytes");
+    FRZ_TRY(ensure_device(c->st.device));
+    if (!c->ingest) c->ingest = std::make_unique<FrzIngest>();
+    if (!c->edit_tiles) c->edit_tiles = std::make_unique<FrzCorpusStorage>();
+    const frz_status s = frz_replace_host(*c->ingest, *c->edit_tiles, which, n, bytes, offsets, offset_width, nullptr, &c->st);
+    // The staging of a replace (the touched tiles' raw bytes and metadata) is kept for the next edit while it is small; a
+    // large one, up to a second copy of the list when every tile was touched, is given back at once.
+    constexpr uint64_t kKeepStaging = 64ull << 20;
+    FrzIngest& ing = *c->ingest;
+    if (ing.d_bytes.cap() + ing.d_offsets.cap() > kKeepStaging) {
+        ing.d_bytes.reset();
+        ing.d_offsets.reset();
+    }
+    const FrzCorpusStorage& et = *c->edit_tiles;
+    const uint64_t et_bytes = et.tile_base.cap() * (8 + FRZ_GROUPS_PER_TILE * sizeof(FrzGroupDesc) + FRZ_TILE * (4 + 2 + 8) + 8);
+    if (et_bytes > kKeepStaging) c->edit_tiles.reset();
+    return s;
+}
+
 extern "C" frz_status frz_corpus_create_ptrs(const uint8_t* const* ptrs, const uint32_t* lens, uint64_t n, int device,
                                              frz_corpus** out) {
     if (!out || (n && (!ptrs || !lens))) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
@@ -869,6 +930,23 @@ __global__ void __launch_bounds__(1024) k_scan_blocks(const uint32_t* cnt, uint6
     }
     if (threadIdx.x == 0) ctr->total = carry;
 }
+// keep[i] = haystack i was not removed (its slot metadata is not FRZ_INVALID_SLOT), with per-block counts as k_retain_count
+// writes them: the retain compaction then drops removed rows from a k_fill_all list
+__global__ void __launch_bounds__(kCompactBlock) k_live_keep(const uint32_t* __restrict__ slot_meta, const uint16_t* __restrict__ slot_of,
+                                                             uint64_t n, uint32_t* block_count, uint8_t* keep) {
+    __shared__ uint32_t wc[32];
+    const uint64_t i = (uint64_t)blockIdx.x * kCompactBlock + threadIdx.x;
+    const bool k = i < n && slot_meta[(i & ~(uint64_t)(FRZ_TILE - 1)) + slot_of[i]] != FRZ_INVALID_SLOT;
+    if (i < n) keep[i] = k;
+    const uint32_t b = __ballot_sync(0xffffffffu, k);
+    if ((threadIdx.x & 31) == 0) wc[threadIdx.x >> 5] = __popc(b);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        uint32_t s = 0;
+        for (int w = 0; w < 32; w++) s += wc[w];
+        block_count[blockIdx.x] = s;
+    }
+}
 
 frz_status ensure_workspace(frz_matcher* m, const FrzCorpusStorage& cs, uint64_t survivor_cap) {
     FrzWorkspace& ws = m->ws;
@@ -900,6 +978,16 @@ frz_status ensure_workspace(frz_matcher* m, const FrzCorpusStorage& cs, uint64_t
 frz_status ensure_multi_buffers(frz_matcher* m, uint64_t n) {
     FRZ_TRY(m->ws.multi_a.reserve(std::max<uint64_t>(n, 1)));
     return m->ws.multi_b.reserve(std::max<uint64_t>(n, 1));
+}
+
+// stable-compaction scratch (k_retain_count / k_live_keep → k_scan_blocks → k_retain_scatter) for lists of up to n entries
+frz_status ensure_retain_buffers(frz_matcher* m, uint64_t n) {
+    FrzWorkspace& ws = m->ws;
+    if (ws.retain_keep.cap() >= n) return FRZ_OK;
+    const uint32_t nb_max = (uint32_t)((n + kCompactBlock - 1) / kCompactBlock) + 1;
+    FRZ_TRY(ws.retain_cnt.reserve(nb_max));
+    FRZ_TRY(ws.retain_base.reserve(nb_max));
+    return ws.retain_keep.reserve(n);
 }
 
 uint64_t initial_survivor_cap(const FrzCorpusStorage& cs, const FrzPatternDev& d) {
@@ -986,6 +1074,25 @@ int grid_for(uint64_t n, int block) {
     return (int)std::max<uint64_t>(1, std::min<uint64_t>(g, (uint64_t)frz_sm_count() * 16));
 }
 
+// Every index of the corpus, ascending, into `out` (count in ws.counters->total): the list of the empty matcher and the
+// start of an all-negated one.  A corpus with removed haystacks fills `tmp` and keeps only the live indices.
+frz_status fill_all(frz_matcher* m, const FrzCorpusStorage& cs, uint32_t index_offset, FrzMatchDev* out, FrzMatchDev* tmp,
+                    cudaStream_t stream, FrzLaunchStats* st) {
+    FrzWorkspace& ws = m->ws;
+    k_fill_all<<<grid_for(cs.n, 256), 256, 0, stream>>>(cs.n_removed ? tmp : out, cs.n, index_offset, ws.counters.get());
+    st->launches++;
+    if (cs.n_removed) {
+        FRZ_TRY(ensure_retain_buffers(m, cs.n));
+        const uint32_t nb = (uint32_t)((cs.n + kCompactBlock - 1) / kCompactBlock);
+        k_live_keep<<<nb, kCompactBlock, 0, stream>>>(cs.slot_meta.get(), cs.slot_of.get(), cs.n, ws.retain_cnt.get(), ws.retain_keep.get());
+        k_scan_blocks<<<1, 1024, 0, stream>>>(ws.retain_cnt.get(), ws.retain_base.get(), nb, ws.counters.get());
+        k_retain_scatter<<<nb, kCompactBlock, 0, stream>>>(tmp, cs.n, ws.retain_keep.get(), ws.retain_base.get(), out);
+        st->launches += 3;
+    }
+    FRZ_CUDA_TRY(cudaGetLastError());
+    return FRZ_OK;
+}
+
 // match_list_into over all compiled patterns → index-ordered device list; returns pointer + leaves the
 // count in ws.counters->total.  `final_reversed` asks for the list in descending index order.  `score_hist` (optional):
 // the caller will sort the list by score; where the scoring kernels emit the list directly and one sort pass will do,
@@ -1002,8 +1109,7 @@ frz_status match_into_device(frz_matcher* m, const FrzCorpusStorage& cs, uint32_
     if (pats.empty()) {  // CompiledPatterns::Empty (src/matcher/mod.rs:380-383)
         FRZ_TRY(ensure_workspace(m, cs, 1));
         FRZ_CUDA_TRY(cudaMemsetAsync(ws.counters.get(), 0, sizeof(FrzCounters), stream));
-        k_fill_all<<<grid_for(cs.n, 256), 256, 0, stream>>>(ws.matches_a.get(), cs.n, index_offset, ws.counters.get());
-        st->launches++;
+        FRZ_TRY(fill_all(m, cs, index_offset, ws.matches_a.get(), ws.matches_b.get(), stream, st));
         if (final_reversed) {
             k_reverse<<<grid_for(cs.n, 256), 256, 0, stream>>>(ws.matches_a.get(), ws.matches_b.get(), &ws.counters.get()->total);
             st->launches++;
@@ -1041,16 +1147,10 @@ frz_status match_into_device(frz_matcher* m, const FrzCorpusStorage& cs, uint32_
         bound = pats[base].score_bound;
     } else {
         FRZ_CUDA_TRY(cudaMemsetAsync(ws.counters.get(), 0, sizeof(FrzCounters), stream));
-        k_fill_all<<<grid_for(cs.n, 256), 256, 0, stream>>>(cand, cs.n, index_offset, ws.counters.get());
-        st->launches++;
-        nc = cs.n;
+        FRZ_TRY(fill_all(m, cs, index_offset, cand, spare, stream, st));
+        nc = cs.n - cs.n_removed;
     }
-    if (ws.retain_keep.cap() < cs.n) {
-        const uint32_t nb_max = (uint32_t)((cs.n + kCompactBlock - 1) / kCompactBlock) + 1;
-        FRZ_TRY(ws.retain_cnt.reserve(nb_max));
-        FRZ_TRY(ws.retain_base.reserve(nb_max));
-        FRZ_TRY(ws.retain_keep.reserve(cs.n));
-    }
+    FRZ_TRY(ensure_retain_buffers(m, cs.n));
     uint32_t* d_block_cnt = ws.retain_cnt.get();
     uint64_t* d_block_base = ws.retain_base.get();
     uint8_t* d_keep = ws.retain_keep.get();
@@ -1339,6 +1439,30 @@ frz_status match_indices_one(const Compiled& c, const frz_corpus* corpus, const 
     FRZ_CUDA_TRY(cudaStreamSynchronize(stream));
     return FRZ_OK;
 }
+
+__global__ void k_rows_removed(const uint32_t* __restrict__ slot_meta, const uint16_t* __restrict__ slot_of, const uint32_t* __restrict__ which,
+                               uint64_t n, uint64_t corpus_n, uint8_t* __restrict__ removed) {
+    for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) {
+        const uint64_t idx = which[j];
+        removed[j] = idx < corpus_n && slot_meta[(idx & ~(uint64_t)(FRZ_TILE - 1)) + slot_of[idx]] == FRZ_INVALID_SLOT;
+    }
+}
+
+// removed[j] = haystack which[j] was removed (frz_corpus_remove)
+frz_status rows_removed(const frz_corpus* corpus, const uint32_t* which, uint64_t n, uint8_t* removed) {
+    cudaStream_t stream = nullptr;
+    FrzDevArray<uint32_t> d_which;
+    FrzDevArray<uint8_t> d_removed;
+    FRZ_TRY(d_which.reserve(n));
+    FRZ_TRY(d_removed.reserve(n));
+    FRZ_CUDA_TRY(cudaMemcpyAsync(d_which.get(), which, n * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
+    k_rows_removed<<<grid_for(n, 256), 256, 0, stream>>>(corpus->st.slot_meta.get(), corpus->st.slot_of.get(), d_which.get(), n, corpus->st.n,
+                                                      d_removed.get());
+    FRZ_CUDA_TRY(cudaGetLastError());
+    FRZ_CUDA_TRY(cudaMemcpyAsync(removed, d_removed.get(), n, cudaMemcpyDeviceToHost, stream));
+    FRZ_CUDA_TRY(cudaStreamSynchronize(stream));
+    return FRZ_OK;
+}
 }  // namespace
 
 extern "C" frz_status frz_match_indices(frz_matcher* m, const frz_corpus* corpus, const uint32_t* which, uint64_t n,
@@ -1362,6 +1486,11 @@ extern "C" frz_status frz_match_indices(frz_matcher* m, const frz_corpus* corpus
     std::vector<uint32_t> pi((size_t)n * istride), pc(n);
     std::vector<std::vector<uint32_t>> pooled(n);
     std::vector<uint8_t> alive(n, 1);
+    if (corpus->st.n_removed) {   // an all-negated matcher would keep a removed row: none of its atoms can hit it
+        std::vector<uint8_t> removed(n);
+        FRZ_TRY(rows_removed(corpus, which, n, removed.data()));
+        for (uint64_t j = 0; j < n; j++) alive[j] = !removed[j];
+    }
     for (uint64_t j = 0; j < n; j++) out_matches[j] = frz_match{which[j], 0, 0, 0};
     for (const Compiled& c : m->compiled) {
         FRZ_TRY(match_indices_one(c, corpus, which, n, pm.data(), pi.data(), istride, pc.data()));
@@ -1663,6 +1792,10 @@ extern "C" frz_status frz_matcher_debug_pattern(const frz_matcher* m, size_t i, 
 }
 
 extern "C" uint64_t frz_debug_device_bytes(void) { return g_frz_device_bytes.load(); }
+extern "C" uint64_t frz_debug_device_bytes_peak(int reset) {
+    if (reset) g_frz_device_bytes_peak.store(g_frz_device_bytes.load());
+    return g_frz_device_bytes_peak.load();
+}
 
 extern "C" uint32_t frz_matcher_score_bound(const frz_matcher* m) {
     if (!m) return 0;

@@ -7,6 +7,7 @@
 #include "frz_host.h"
 
 #include <algorithm>
+#include <vector>
 
 namespace {
 
@@ -222,15 +223,55 @@ __global__ void __launch_bounds__(256) k_pack_sig(const uint4* __restrict__ data
 
 }  // namespace
 
-// ---- append support: the partial last tile is turned back into raw (bytes, offsets) so that it can be
-// re-bucketed together with the appended haystacks.  One block; thread i owns haystack idx0 + i.
-__global__ void __launch_bounds__(1024) k_tail_offsets(const uint32_t* __restrict__ slot_meta, const uint16_t* __restrict__ slot_of,
-                                                       const uint64_t* __restrict__ tile_base, uint32_t tile, uint32_t cnt,
-                                                       uint64_t* __restrict__ out_offsets, uint64_t* __restrict__ out_info) {
+// ---- unpack: packed tiles turned back into raw (bytes, offsets), so that they can be re-bucketed — the partial last tile
+// with the haystacks an append adds behind it, or any list of tiles whose haystacks a replace changes.  Staged haystack
+// s = b * 1024 + i is local index i of tiles[b]; the last listed tile holds `last_cnt` haystacks, the others 1024.  A
+// replaced haystack (repl[s] = its position in the replacement list) is staged with its new bytes; a removed one that is
+// not replaced is staged empty and flagged in `dead`, so that the re-packed tile keeps it removed.
+constexpr uint32_t kNoRepl = 0xFFFFFFFFu;
+// words of the unpack's info block (device, zeroed by the caller)
+enum : int { kInfoOldBytes = 0,   // live bytes the replaced haystacks had
+             kInfoRevived = 1,    // replaced haystacks that had been removed
+             kInfoOldUnits = 2,   // units the listed tiles occupied
+             kInfoTileBase = 3,   // first and one-past-last unit of the (single) listed tile: the append's tail rule
+             kInfoTileEnd = 4,
+             kInfoStaged = 5,     // staged bytes
+             kInfoWords = 8 };
+
+// One block per listed tile: lengths → local exclusive offsets (staged_off[s]) and the tile's byte count (tile_sum[b]).
+__global__ void __launch_bounds__(1024) k_unpack_offsets(const uint32_t* __restrict__ slot_meta, const uint16_t* __restrict__ slot_of,
+                                                         const FrzGroupDesc* __restrict__ groups, const uint64_t* __restrict__ tile_base,
+                                                         const uint32_t* __restrict__ tiles, uint32_t n_list, uint32_t last_cnt,
+                                                         const uint32_t* __restrict__ repl, const uint64_t* __restrict__ r_off,
+                                                         uint64_t* __restrict__ out_offsets, uint64_t* __restrict__ tile_sum,
+                                                         uint8_t* __restrict__ dead, unsigned long long* __restrict__ info) {
     __shared__ uint64_t wsum[32];
-    const uint32_t i = threadIdx.x, lane = i & 31, warp = i >> 5;
+    const uint32_t i = threadIdx.x, lane = i & 31, warp = i >> 5, b = blockIdx.x;
+    const uint64_t tile = tiles[b];
+    const uint32_t cnt = b == n_list - 1 ? last_cnt : FRZ_TILE;
+    const uint64_t s = (uint64_t)b * FRZ_TILE + i;
     uint64_t len = 0;
-    if (i < cnt) len = slot_meta[(uint64_t)tile * FRZ_TILE + slot_of[(uint64_t)tile * FRZ_TILE + i]] >> FRZ_TILE_SHIFT;
+    if (i < cnt) {
+        const uint32_t meta = slot_meta[tile * FRZ_TILE + slot_of[tile * FRZ_TILE + i]];
+        const uint32_t r = repl ? repl[s] : kNoRepl;
+        if (r != kNoRepl) {
+            len = r_off[r + 1] - r_off[r];
+            if (meta != FRZ_INVALID_SLOT) atomicAdd(info + kInfoOldBytes, (unsigned long long)(meta >> FRZ_TILE_SHIFT));
+            else atomicAdd(info + kInfoRevived, 1ull);
+        } else if (meta != FRZ_INVALID_SLOT) {
+            len = meta >> FRZ_TILE_SHIFT;
+        }
+        dead[s] = r == kNoRepl && meta == FRZ_INVALID_SLOT;
+    }
+    if (i == 0) {
+        const FrzGroupDesc last = groups[tile * FRZ_GROUPS_PER_TILE + FRZ_GROUPS_PER_TILE - 1];
+        const uint64_t units = (uint64_t)last.unit_off + (uint64_t)last.gunits * FRZ_GROUP;
+        atomicAdd(info + kInfoOldUnits, (unsigned long long)units);
+        if (n_list == 1) {
+            info[kInfoTileBase] = tile_base[tile];
+            info[kInfoTileEnd] = tile_base[tile] + units;
+        }
+    }
     uint64_t x = len;
     for (int d = 1; d < 32; d <<= 1) {
         uint64_t y = __shfl_up_sync(0xffffffffu, x, d);
@@ -248,35 +289,130 @@ __global__ void __launch_bounds__(1024) k_tail_offsets(const uint32_t* __restric
     }
     __syncthreads();
     const uint64_t incl = wsum[warp] + x;
-    if (i < cnt) out_offsets[i] = incl - len;
-    if (i == FRZ_TILE - 1) {
-        out_offsets[cnt] = incl;       // lanes >= cnt add 0: incl of the last thread is the total
-        out_info[0] = incl;            // tail bytes
-        out_info[1] = tile_base[tile]; // first unit of the tail tile
+    if (i < cnt) out_offsets[s] = incl - len;
+    if (i == FRZ_TILE - 1) tile_sum[b] = incl;   // lanes >= cnt add 0: incl of the last thread is the tile's total
+}
+
+// One warp per staged haystack: its offset becomes global (tile_sum holds the tiles' exclusive scan by now) and its bytes
+// are copied from the packed tile, or from the uploaded replacement bytes r_bytes[r_off[r], r_off[r + 1]).
+__global__ void __launch_bounds__(256) k_unpack_bytes(const uint4* __restrict__ data, const FrzGroupDesc* __restrict__ groups,
+                                                      const uint32_t* __restrict__ slot_meta, const uint16_t* __restrict__ slot_of,
+                                                      const uint32_t* __restrict__ tiles, uint64_t staged_n,
+                                                      const uint32_t* __restrict__ repl, const uint64_t* __restrict__ r_off,
+                                                      const uint8_t* __restrict__ r_bytes, const uint8_t* __restrict__ dead,
+                                                      const uint64_t* __restrict__ tile_sum, uint64_t* __restrict__ offsets,
+                                                      uint8_t* __restrict__ out_bytes) {
+    // lanes stride over the haystack's bytes
+    const uint64_t warp = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const uint32_t lane = threadIdx.x & 31;
+    const uint64_t n_warps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
+    for (uint64_t s = warp; s < staged_n; s += n_warps) {
+        const uint64_t tile = tiles[s >> FRZ_TILE_SHIFT];
+        const uint32_t i = (uint32_t)(s & (FRZ_TILE - 1));
+        const uint64_t at = tile_sum[s >> FRZ_TILE_SHIFT] + offsets[s];
+        __syncwarp();
+        if (lane == 0) offsets[s] = at;
+        uint8_t* dst = out_bytes + at;
+        const uint32_t r = repl ? repl[s] : kNoRepl;
+        if (r != kNoRepl) {
+            const uint64_t b0 = r_off[r], len = r_off[r + 1] - b0;
+            for (uint64_t b = lane; b < len; b += 32) dst[b] = r_bytes[b0 + b];
+        } else if (!dead[s]) {
+            const uint32_t slot = slot_of[tile * FRZ_TILE + i];
+            const uint32_t len = slot_meta[tile * FRZ_TILE + slot] >> FRZ_TILE_SHIFT;
+            const FrzGroupDesc gd = groups[tile * FRZ_GROUPS_PER_TILE + (slot >> 5)];
+            const uint8_t* base = reinterpret_cast<const uint8_t*>(data + frz_slot_unit0(gd, slot & 31));
+            for (uint32_t b = lane; b < len; b += 32) dst[b] = base[b];
+        }
     }
 }
 
-__global__ void __launch_bounds__(256) k_tail_bytes(const uint4* __restrict__ data, const FrzGroupDesc* __restrict__ groups,
-                                                    const uint32_t* __restrict__ slot_meta, const uint16_t* __restrict__ slot_of,
-                                                    uint32_t tile, uint32_t cnt, const uint64_t* __restrict__ offsets,
-                                                    uint8_t* __restrict__ out_bytes) {
-    // one warp per haystack, lanes stride over its bytes
-    const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
-    const uint32_t n_warps = (gridDim.x * blockDim.x) >> 5;
-    for (uint32_t i = warp; i < cnt; i += n_warps) {
-        const uint32_t slot = slot_of[(uint64_t)tile * FRZ_TILE + i];
-        const uint32_t len = slot_meta[(uint64_t)tile * FRZ_TILE + slot] >> FRZ_TILE_SHIFT;
-        const FrzGroupDesc gd = groups[tile * FRZ_GROUPS_PER_TILE + (slot >> 5)];
-        const uint8_t* base = reinterpret_cast<const uint8_t*>(data + frz_slot_unit0(gd, slot & 31));
-        uint8_t* dst = out_bytes + offsets[i];
-        for (uint32_t b = lane; b < len; b += 32) dst[b] = base[b];
+// repl[slot_pos[j]] = j: where replacement j lands among the staged haystacks
+__global__ void k_mark_repl(const uint32_t* __restrict__ slot_pos, uint64_t n, uint32_t* __restrict__ repl) {
+    for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x)
+        repl[slot_pos[j]] = (uint32_t)j;
+}
+
+// After the re-pack: a staged haystack flagged dead is removed again (it was packed as an empty haystack).
+__global__ void k_mark_dead(const uint8_t* __restrict__ dead, uint64_t staged_n, const uint32_t* __restrict__ tiles,
+                            const uint16_t* __restrict__ slot_of, uint32_t* __restrict__ slot_meta) {
+    for (uint64_t s = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; s < staged_n; s += (uint64_t)gridDim.x * blockDim.x) {
+        if (!dead[s]) continue;
+        const uint64_t tile = tiles[s >> FRZ_TILE_SHIFT];
+        slot_meta[tile * FRZ_TILE + slot_of[tile * FRZ_TILE + (s & (FRZ_TILE - 1))]] = FRZ_INVALID_SLOT;
     }
+}
+
+// One block per re-packed tile: its metadata, planned as tile b of a scratch corpus, replaces that of tiles[b].
+__global__ void __launch_bounds__(256) k_scatter_tiles(const uint32_t* __restrict__ tiles, const uint64_t* __restrict__ s_tile_base,
+                                                       const FrzGroupDesc* __restrict__ s_groups, const uint32_t* __restrict__ s_meta,
+                                                       const uint16_t* __restrict__ s_of, const uint2* __restrict__ s_sig,
+                                                       uint64_t* __restrict__ tile_base, FrzGroupDesc* __restrict__ groups,
+                                                       uint32_t* __restrict__ slot_meta, uint16_t* __restrict__ slot_of,
+                                                       uint2* __restrict__ slot_sig) {
+    const uint64_t b = blockIdx.x, t = tiles[b];
+    if (threadIdx.x == 0) tile_base[t] = s_tile_base[b];
+    if (threadIdx.x < FRZ_GROUPS_PER_TILE)
+        groups[t * FRZ_GROUPS_PER_TILE + threadIdx.x] = s_groups[b * FRZ_GROUPS_PER_TILE + threadIdx.x];
+    for (uint32_t i = threadIdx.x; i < FRZ_TILE; i += blockDim.x) {
+        slot_meta[t * FRZ_TILE + i] = s_meta[b * FRZ_TILE + i];
+        slot_of[t * FRZ_TILE + i] = s_of[b * FRZ_TILE + i];
+        slot_sig[t * FRZ_TILE + i] = s_sig[b * FRZ_TILE + i];
+    }
+}
+
+// Removal: the slot's metadata becomes FRZ_INVALID_SLOT, which every scan already skips.  info[0] counts the haystacks
+// this call removed (a duplicate or an already removed one counts once), info[1] sums their lengths.
+__global__ void k_remove(const uint32_t* __restrict__ which, uint64_t n, const uint16_t* __restrict__ slot_of,
+                         uint32_t* __restrict__ slot_meta, unsigned long long* __restrict__ info) {
+    for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) {
+        const uint64_t idx = which[j], tile = idx >> FRZ_TILE_SHIFT;
+        const uint32_t old = atomicExch(slot_meta + tile * FRZ_TILE + slot_of[idx], FRZ_INVALID_SLOT);
+        if (old != FRZ_INVALID_SLOT) {
+            atomicAdd(info, 1ull);
+            atomicAdd(info + 1, (unsigned long long)(old >> FRZ_TILE_SHIFT));
+        }
+    }
+}
+
+// units of every tile, from its last group (the compaction's input)
+__global__ void k_tile_units(const FrzGroupDesc* __restrict__ groups, uint32_t n_tiles, uint64_t* __restrict__ out) {
+    for (uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; t < n_tiles; t += (uint64_t)gridDim.x * blockDim.x) {
+        const FrzGroupDesc g = groups[t * FRZ_GROUPS_PER_TILE + FRZ_GROUPS_PER_TILE - 1];
+        out[t] = (uint64_t)g.unit_off + (uint64_t)g.gunits * FRZ_GROUP;
+    }
+}
+
+// Compaction: one block per tile copies its units to new_base[t] of a fresh arena and points tile_base / abs_off there.
+__global__ void __launch_bounds__(256) k_compact(const uint4* __restrict__ old_data, uint4* __restrict__ new_data,
+                                                 FrzGroupDesc* __restrict__ groups, uint64_t* __restrict__ tile_base,
+                                                 const uint64_t* __restrict__ new_base) {
+    const uint64_t t = blockIdx.x;
+    const uint64_t ob = tile_base[t], nb = new_base[t];
+    const FrzGroupDesc last = groups[t * FRZ_GROUPS_PER_TILE + FRZ_GROUPS_PER_TILE - 1];
+    const uint64_t units = (uint64_t)last.unit_off + (uint64_t)last.gunits * FRZ_GROUP;
+    __syncthreads();   // every thread has read the old tile_base / descriptors before they are rewritten below
+    for (uint64_t u = threadIdx.x; u < units; u += blockDim.x) new_data[nb + u] = old_data[ob + u];
+    if (threadIdx.x < FRZ_GROUPS_PER_TILE) {
+        FrzGroupDesc& g = groups[t * FRZ_GROUPS_PER_TILE + threadIdx.x];
+        g.abs_off = nb + g.unit_off;
+    }
+    if (threadIdx.x == 0) tile_base[t] = nb;
+}
+
+// longest group of the corpus, in units per slot (FrzCorpusView::max_gunits)
+__global__ void k_max_gunits(const FrzGroupDesc* __restrict__ groups, uint64_t n_groups, unsigned int* __restrict__ out) {
+    uint32_t mx = 0;
+    for (uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; g < n_groups; g += (uint64_t)gridDim.x * blockDim.x)
+        mx = max(mx, groups[g].gunits);
+    for (int d = 16; d > 0; d >>= 1) mx = max(mx, __shfl_xor_sync(0xffffffffu, mx, d));
+    if ((threadIdx.x & 31) == 0 && mx) atomicMax(out, mx);
 }
 
 template <typename OffT>
-__global__ void k_rebase_offsets(const OffT* __restrict__ in, uint64_t n_new, const uint64_t* __restrict__ tail_info,
+__global__ void k_rebase_offsets(const OffT* __restrict__ in, uint64_t n_new, const unsigned long long* __restrict__ base_ptr,
                                  uint64_t* __restrict__ out) {
-    const uint64_t base = tail_info[0], off0 = (uint64_t)in[0];
+    const uint64_t base = *base_ptr, off0 = (uint64_t)in[0];
     for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j <= n_new; j += (uint64_t)gridDim.x * blockDim.x)
         out[j] = base + ((uint64_t)in[j] - off0);
 }
@@ -434,9 +570,100 @@ frz_status ingest_host_t(FrzIngest& ing, const uint8_t* h_bytes, const OffT* h_o
     return FRZ_OK;
 }
 
+// Carves the staging buffer ing.d_offsets into 16-byte aligned pieces.
+struct Carve {
+    uint8_t* p;
+    template <typename T>
+    T* take(uint64_t count) {
+        T* r = reinterpret_cast<T*>(p);
+        p += (count * sizeof(T) + 15) & ~15ull;
+        return r;
+    }
+    static uint64_t size(uint64_t count, uint64_t elem) { return (count * elem + 15) & ~15ull; }
+};
+
+// Device buffers of one unpack: staged haystack s = b * 1024 + i is local index i of tiles[b] (see k_unpack_offsets).
+struct Unpack {
+    unsigned long long* info;   // kInfoWords words
+    uint64_t* staged;           // offsets of the staged haystacks (and of an append's new ones behind them)
+    uint64_t* tile_sum;         // [n_list] bytes per listed tile → their exclusive scan
+    uint32_t* tiles;            // [n_list] ascending; the partial last tile of the corpus can only come last
+    uint8_t* dead;              // [n_list * 1024]
+    uint32_t* repl = nullptr;   // [n_list * 1024] or nullptr (no replacements)
+    uint64_t* r_off = nullptr;  // replacement offsets (from 0)
+    uint32_t n_list = 0, last_cnt = 0;
+    uint64_t staged_n() const { return (uint64_t)(n_list - 1) * FRZ_TILE + last_cnt; }
+};
+
+// Step 1 of an unpack: offsets of the staged haystacks, their total in info[kInfoStaged] and staged[staged_n()], and
+// the info block back on the host (the byte count sizes the staging buffer).
+frz_status unpack_offsets(const FrzCorpusStorage* st, const Unpack& u, cudaStream_t stream, uint64_t h_info[kInfoWords]) {
+    FRZ_CUDA_TRY(cudaMemsetAsync(u.info, 0, kInfoWords * sizeof(uint64_t), stream));
+    k_unpack_offsets<<<u.n_list, 1024, 0, stream>>>(st->slot_meta.get(), st->slot_of.get(), st->groups.get(), st->tile_base.get(), u.tiles,
+                                                    u.n_list, u.last_cnt, u.repl, u.r_off, u.staged, u.tile_sum, u.dead, u.info);
+    k_scan_u64<<<1, 1024, 0, stream>>>(u.tile_sum, u.tile_sum, u.n_list, 0, reinterpret_cast<uint64_t*>(u.info + kInfoStaged));
+    FRZ_CUDA_TRY(cudaMemcpyAsync(u.staged + u.staged_n(), u.info + kInfoStaged, sizeof(uint64_t), cudaMemcpyDeviceToDevice, stream));
+    FRZ_CUDA_TRY(cudaMemcpyAsync(h_info, u.info, kInfoWords * sizeof(uint64_t), cudaMemcpyDeviceToHost, stream));
+    FRZ_CUDA_TRY(cudaStreamSynchronize(stream));
+    return FRZ_OK;
+}
+
+// Step 2: the staged bytes, into out_bytes (r_bytes: the uploaded replacement bytes, if any).
+frz_status unpack_bytes(const FrzCorpusStorage* st, const Unpack& u, const uint8_t* r_bytes, uint8_t* out_bytes, cudaStream_t stream) {
+    const uint64_t n = u.staged_n();
+    const uint32_t blocks = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((n + 7) / 8, (uint64_t)frz_sm_count() * 8));
+    k_unpack_bytes<<<blocks, 256, 0, stream>>>(st->data.get(), st->groups.get(), st->slot_meta.get(), st->slot_of.get(), u.tiles, n, u.repl,
+                                               u.r_off, r_bytes, u.dead, u.tile_sum, u.staged, out_bytes);
+    FRZ_CUDA_TRY(cudaGetLastError());
+    return FRZ_OK;
+}
+
+// After the re-pack of the listed tiles: their removed, unreplaced haystacks are removed again.
+frz_status unpack_mark_dead(FrzCorpusStorage* st, const Unpack& u, cudaStream_t stream) {
+    const uint64_t n = u.staged_n();
+    const uint32_t blocks = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((n + 255) / 256, (uint64_t)frz_sm_count() * 8));
+    k_mark_dead<<<blocks, 256, 0, stream>>>(u.dead, n, u.tiles, st->slot_of.get(), st->slot_meta.get());
+    FRZ_CUDA_TRY(cudaGetLastError());
+    return FRZ_OK;
+}
+
+// Copies every tile's units into a fresh arena, in tile order and without gaps (the layout a fresh pack has).  Peak device
+// memory: the old arena plus the new one.
+frz_status compact_arena(FrzCorpusStorage* st, cudaStream_t stream) {
+    const uint32_t T = st->n_tiles;
+    if (T == 0) return FRZ_OK;
+    uint64_t* d_units = st->scratch_tile_units.get();
+    uint64_t* d_total = d_units + st->tile_base.cap();
+    k_tile_units<<<(T + 255) / 256, 256, 0, stream>>>(st->groups.get(), T, d_units);
+    k_scan_u64<<<1, 1024, 0, stream>>>(d_units, d_units, T, 0, d_total);
+    uint64_t total = 0;
+    FRZ_CUDA_TRY(cudaMemcpyAsync(&total, d_total, sizeof total, cudaMemcpyDeviceToHost, stream));
+    FRZ_CUDA_TRY(cudaStreamSynchronize(stream));
+    FrzDevArray<uint4> fresh;
+    FRZ_TRY(fresh.reserve(total + total / 16 + 1024));
+    k_compact<<<T, 256, 0, stream>>>(st->data.get(), fresh.get(), st->groups.get(), st->tile_base.get(), d_units);
+    FRZ_CUDA_TRY(cudaGetLastError());
+    FRZ_CUDA_TRY(cudaStreamSynchronize(stream));   // the old arena is freed below
+    st->data = std::move(fresh);
+    st->total_units = total;
+    st->dead_units = 0;
+    return FRZ_OK;
+}
+
+// An edit that leaves more dead units than live ones compacts the arena.  It runs last, once the edit is complete, and it is
+// only an optimisation: when the new arena cannot be allocated, the corpus keeps its dead space (compact_arena changes
+// nothing before that allocation has succeeded) and the next edit tries again.
+frz_status maybe_compact(FrzCorpusStorage* st, cudaStream_t stream) {
+    if (st->dead_units <= st->total_units - st->dead_units) return FRZ_OK;
+    const frz_status s = compact_arena(st, stream);
+    return s == FRZ_ERR_OOM ? FRZ_OK : s;
+}
+
 // Incremental append (SURVEY §8(f) rank 1).  Tiles are independent, so only the partial last tile is
 // re-bucketed: it is unpacked to raw bytes, the new haystacks are staged behind it, and tiles
-// [n_old / 1024, n_tiles_new) are planned, scanned (carry = first unit of the old tail tile) and copied.
+// [n_old / 1024, n_tiles_new) are planned, scanned and copied.  The tail is re-packed in place (carry = first unit of the
+// old tail tile) while that tile ends where the arena ends — always so for a corpus that was never edited — and at the
+// arena's end otherwise.
 template <typename OffT>
 frz_status append_host_t(FrzIngest& ing, const uint8_t* h_bytes, const OffT* h_offsets, uint64_t n_new, cudaStream_t stream,
                          FrzCorpusStorage* st) {
@@ -454,35 +681,131 @@ frz_status append_host_t(FrzIngest& ing, const uint8_t* h_bytes, const OffT* h_o
     const uint64_t off0 = (uint64_t)h_offsets[0];
     const uint64_t new_bytes = (uint64_t)h_offsets[n_new] - off0;
     const uint32_t n_tiles = (uint32_t)((n + FRZ_TILE - 1) / FRZ_TILE);
-    // staging layout in ing.d_offsets: [tail_info: 2 u64][staged offsets: cnt + n_new + 1 u64][raw new offsets]
-    const uint64_t staged_words = 2 + (uint64_t)cnt + n_new + 1;
-    FRZ_TRY(ing.reserve(0, staged_words * 8 + (n_new + 1) * sizeof(OffT) + 16));
-    uint64_t* d_info = reinterpret_cast<uint64_t*>(ing.d_offsets.get());
-    uint64_t* d_staged = d_info + 2;
-    OffT* d_raw = reinterpret_cast<OffT*>(d_staged + cnt + n_new + 1);
-    uint64_t info[2] = {0, st->total_units};
+    // staging layout in ing.d_offsets: [info][staged offsets: cnt + n_new + 1][tile_sum: 1][tiles: 1][dead: 1024][raw new offsets]
+    FRZ_TRY(ing.reserve(0, Carve::size(kInfoWords, 8) + Carve::size((uint64_t)cnt + n_new + 1, 8) + 32 + Carve::size(FRZ_TILE, 1) +
+                               Carve::size(n_new + 1, sizeof(OffT))));
+    Carve cv{ing.d_offsets.get()};
+    Unpack u;
+    u.info = cv.take<unsigned long long>(kInfoWords);
+    u.staged = cv.take<uint64_t>((uint64_t)cnt + n_new + 1);
+    u.tile_sum = cv.take<uint64_t>(1);
+    u.tiles = cv.take<uint32_t>(1);
+    u.dead = cv.take<uint8_t>(FRZ_TILE);
+    OffT* d_raw = cv.take<OffT>(n_new + 1);
+    u.n_list = 1;
+    u.last_cnt = cnt;
+    uint64_t info[kInfoWords] = {};
+    uint64_t carry_in = st->total_units;
     if (cnt) {
-        k_tail_offsets<<<1, 1024, 0, stream>>>(st->slot_meta.get(), st->slot_of.get(), st->tile_base.get(), t_last, cnt, d_staged, d_info);
-        FRZ_CUDA_TRY(cudaMemcpyAsync(info, d_info, 16, cudaMemcpyDeviceToHost, stream));
-        FRZ_CUDA_TRY(cudaStreamSynchronize(stream));
+        FRZ_CUDA_TRY(cudaMemcpyAsync(u.tiles, &t_last, sizeof t_last, cudaMemcpyHostToDevice, stream));
+        FRZ_TRY(unpack_offsets(st, u, stream, info));
+        if (info[kInfoTileEnd] == st->total_units) carry_in = info[kInfoTileBase];   // the tail ends the arena: re-pack it in place
     } else {
-        FRZ_CUDA_TRY(cudaMemcpyAsync(d_info, info, 16, cudaMemcpyHostToDevice, stream));
+        FRZ_CUDA_TRY(cudaMemsetAsync(u.info, 0, kInfoWords * sizeof(uint64_t), stream));
     }
-    const uint64_t tail_bytes = info[0], carry_in = info[1];
+    const uint64_t tail_bytes = info[kInfoStaged];
     FRZ_TRY(ing.reserve(tail_bytes + new_bytes, 0));
-    if (cnt)
-        k_tail_bytes<<<32, 256, 0, stream>>>(st->data.get(), st->groups.get(), st->slot_meta.get(), st->slot_of.get(), t_last, cnt, d_staged,
-                                             ing.d_bytes.get());
+    if (cnt) FRZ_TRY(unpack_bytes(st, u, nullptr, ing.d_bytes.get(), stream));
     if (new_bytes) FRZ_CUDA_TRY(cudaMemcpyAsync(ing.d_bytes.get() + tail_bytes, h_bytes + off0, new_bytes, cudaMemcpyHostToDevice, stream));
     FRZ_CUDA_TRY(cudaMemcpyAsync(d_raw, h_offsets, (n_new + 1) * sizeof(OffT), cudaMemcpyHostToDevice, stream));
-    k_rebase_offsets<OffT><<<256, 256, 0, stream>>>(d_raw, n_new, d_info, d_staged + cnt);
+    k_rebase_offsets<OffT><<<256, 256, 0, stream>>>(d_raw, n_new, u.info + kInfoStaged, u.staged + cnt);
     FRZ_CUDA_TRY(cudaGetLastError());
     FRZ_TRY(pack_reserve(st, n_tiles, t_last, stream));
     st->n = n;
     st->n_tiles = n_tiles;
     st->total_bytes += new_bytes;
-    FRZ_TRY(pack_plan<uint64_t>(st, d_staged, n, t_last, idx0, carry_in, true, stream));
-    return pack_copy<uint64_t>(st, ing.d_bytes.get(), d_staged, t_last, idx0, 0, tail_bytes + new_bytes, t_last, n_tiles, stream);
+    if (cnt && carry_in != info[kInfoTileBase]) st->dead_units += info[kInfoOldUnits];   // the old tail's units are left behind
+    FRZ_TRY(pack_plan<uint64_t>(st, u.staged, n, t_last, idx0, carry_in, true, stream));
+    FRZ_TRY(pack_copy<uint64_t>(st, ing.d_bytes.get(), u.staged, t_last, idx0, 0, tail_bytes + new_bytes, t_last, n_tiles, stream));
+    if (cnt && st->n_removed) FRZ_TRY(unpack_mark_dead(st, u, stream));
+    return maybe_compact(st, stream);
+}
+
+// Replace: the tiles holding `which` are unpacked in one batch with the new strings substituted, planned as the tiles of
+// a scratch corpus whose units go to the end of the arena, and their metadata is scattered over the old tiles'.  Their old
+// unit ranges become dead space.  The caller has checked the arguments (indices in range, no duplicates, lengths).
+template <typename OffT>
+frz_status replace_host_t(FrzIngest& ing, FrzCorpusStorage& scratch, const uint32_t* which, uint64_t n, const uint8_t* h_bytes,
+                          const OffT* h_offsets, cudaStream_t stream, FrzCorpusStorage* st) {
+    std::vector<uint32_t> tiles(n);
+    for (uint64_t j = 0; j < n; j++) tiles[j] = which[j] >> FRZ_TILE_SHIFT;
+    std::sort(tiles.begin(), tiles.end());
+    tiles.erase(std::unique(tiles.begin(), tiles.end()), tiles.end());
+    const uint32_t T = (uint32_t)tiles.size();
+    const uint32_t tail_cnt = (uint32_t)(st->n % FRZ_TILE);
+    Unpack u;
+    u.n_list = T;
+    u.last_cnt = (tiles.back() == st->n_tiles - 1 && tail_cnt) ? tail_cnt : FRZ_TILE;
+    const uint64_t staged_n = u.staged_n();
+    std::vector<uint32_t> slot_pos(n);
+    std::vector<uint64_t> r_off(n + 1);
+    const uint64_t off0 = (uint64_t)h_offsets[0];
+    for (uint64_t j = 0; j < n; j++) {
+        const uint32_t b = (uint32_t)(std::lower_bound(tiles.begin(), tiles.end(), which[j] >> FRZ_TILE_SHIFT) - tiles.begin());
+        slot_pos[j] = b * FRZ_TILE + (which[j] & (FRZ_TILE - 1));
+    }
+    for (uint64_t j = 0; j <= n; j++) r_off[j] = (uint64_t)h_offsets[j] - off0;
+    const uint64_t r_total = r_off[n];
+    const uint64_t slots = (uint64_t)T * FRZ_TILE;
+    FRZ_TRY(ing.reserve(0, Carve::size(kInfoWords, 8) + Carve::size(slots + 1, 8) + Carve::size(T, 8) + Carve::size(T, 4) + Carve::size(slots, 4) +
+                               Carve::size(slots, 1) + Carve::size(n + 1, 8) + Carve::size(n, 4) + 16));
+    Carve cv{ing.d_offsets.get()};
+    u.info = cv.take<unsigned long long>(kInfoWords);
+    u.staged = cv.take<uint64_t>(slots + 1);
+    u.tile_sum = cv.take<uint64_t>(T);
+    u.tiles = cv.take<uint32_t>(T);
+    u.repl = cv.take<uint32_t>(slots);
+    u.dead = cv.take<uint8_t>(slots);
+    u.r_off = cv.take<uint64_t>(n + 1);
+    uint32_t* d_slot_pos = cv.take<uint32_t>(n);
+    // the scratch metadata first: everything that can run out of memory before the corpus changes
+    scratch.n = staged_n;
+    scratch.n_tiles = T;
+    FRZ_TRY(pack_reserve(&scratch, T, 0, stream));
+    FRZ_CUDA_TRY(cudaMemcpyAsync(u.tiles, tiles.data(), (size_t)T * 4, cudaMemcpyHostToDevice, stream));
+    FRZ_CUDA_TRY(cudaMemcpyAsync(u.r_off, r_off.data(), (n + 1) * 8, cudaMemcpyHostToDevice, stream));
+    FRZ_CUDA_TRY(cudaMemcpyAsync(d_slot_pos, slot_pos.data(), n * 4, cudaMemcpyHostToDevice, stream));
+    FRZ_CUDA_TRY(cudaMemsetAsync(u.repl, 0xFF, slots * 4, stream));
+    k_mark_repl<<<(uint32_t)std::min<uint64_t>((n + 255) / 256, (uint64_t)frz_sm_count() * 8), 256, 0, stream>>>(d_slot_pos, n, u.repl);
+    uint64_t info[kInfoWords] = {};
+    FRZ_TRY(unpack_offsets(st, u, stream, info));
+    const uint64_t staged_bytes = info[kInfoStaged];
+    const uint64_t r_at = (staged_bytes + 15) & ~15ull;   // the replacement bytes, behind the staged ones
+    FRZ_TRY(ing.reserve(r_at + r_total, 0));
+    if (r_total) FRZ_CUDA_TRY(cudaMemcpyAsync(ing.d_bytes.get() + r_at, h_bytes + off0, r_total, cudaMemcpyHostToDevice, stream));
+    FRZ_TRY(unpack_bytes(st, u, ing.d_bytes.get() + r_at, ing.d_bytes.get(), stream));
+    // plan + copy as a corpus of T tiles whose units start at the arena's end; the arena moves into the scratch for that
+    scratch.data = std::move(st->data);
+    scratch.total_units = st->total_units;
+    frz_status s = pack_plan<uint64_t>(&scratch, u.staged, staged_n, 0, 0, st->total_units, true, stream);
+    if (s == FRZ_OK) s = pack_copy<uint64_t>(&scratch, ing.d_bytes.get(), u.staged, 0, 0, 0, staged_bytes, 0, T, stream);
+    st->data = std::move(scratch.data);
+    FRZ_TRY(s);
+    k_scatter_tiles<<<T, 256, 0, stream>>>(u.tiles, scratch.tile_base.get(), scratch.groups.get(), scratch.slot_meta.get(), scratch.slot_of.get(),
+                                           scratch.slot_sig.get(), st->tile_base.get(), st->groups.get(), st->slot_meta.get(),
+                                           st->slot_of.get(), st->slot_sig.get());
+    // from here on the new tiles are in place: the host state follows them at once, and the longest-group bound can only
+    // grow with them (the batch's own longest group, from the plan), so that no later failure leaves it below the truth
+    const bool had_removed = st->n_removed != 0;
+    st->total_units = scratch.total_units;
+    st->dead_units += info[kInfoOldUnits];
+    st->total_bytes = st->total_bytes + r_total - info[kInfoOldBytes];
+    st->n_removed -= info[kInfoRevived];
+    st->max_gunits = std::max(st->max_gunits, scratch.max_gunits);
+    FRZ_CUDA_TRY(cudaGetLastError());
+    if (had_removed) FRZ_TRY(unpack_mark_dead(st, u, stream));
+    // the longest group may also have shrunk: recount it over every tile (the kernels specialise on it), before the
+    // compaction, which moves units but leaves the groups' sizes as they are
+    unsigned int* d_max = reinterpret_cast<unsigned int*>(u.info);
+    FRZ_CUDA_TRY(cudaMemsetAsync(d_max, 0, sizeof(unsigned int), stream));
+    const uint64_t n_groups = (uint64_t)st->n_tiles * FRZ_GROUPS_PER_TILE;
+    k_max_gunits<<<(uint32_t)std::min<uint64_t>((n_groups + 255) / 256, (uint64_t)frz_sm_count() * 8), 256, 0, stream>>>(st->groups.get(),
+                                                                                                                        n_groups, d_max);
+    unsigned int mx = 0;
+    FRZ_CUDA_TRY(cudaMemcpyAsync(&mx, d_max, sizeof mx, cudaMemcpyDeviceToHost, stream));
+    FRZ_CUDA_TRY(cudaStreamSynchronize(stream));
+    st->max_gunits = mx;
+    return maybe_compact(st, stream);
 }
 
 }  // namespace
@@ -517,4 +840,30 @@ frz_status frz_append_host(FrzIngest& ing, const uint8_t* h_bytes, const void* h
                            cudaStream_t stream, FrzCorpusStorage* st) {
     if (offset_width == 4) return append_host_t<uint32_t>(ing, h_bytes, static_cast<const uint32_t*>(h_offsets), n_new, stream, st);
     return append_host_t<uint64_t>(ing, h_bytes, static_cast<const uint64_t*>(h_offsets), n_new, stream, st);
+}
+
+// Marks haystacks which[0..n) removed (indices checked by the caller).  Their bytes stay where they are.
+frz_status frz_remove_host(FrzIngest& ing, const uint32_t* which, uint64_t n, cudaStream_t stream, FrzCorpusStorage* st) {
+    FRZ_TRY(ing.reserve(0, 16 + n * sizeof(uint32_t)));
+    unsigned long long* d_info = reinterpret_cast<unsigned long long*>(ing.d_offsets.get());
+    uint32_t* d_which = reinterpret_cast<uint32_t*>(d_info + 2);
+    FRZ_CUDA_TRY(cudaMemsetAsync(d_info, 0, 16, stream));
+    FRZ_CUDA_TRY(cudaMemcpyAsync(d_which, which, n * sizeof(uint32_t), cudaMemcpyHostToDevice, stream));
+    k_remove<<<(uint32_t)std::min<uint64_t>((n + 255) / 256, (uint64_t)frz_sm_count() * 8), 256, 0, stream>>>(d_which, n, st->slot_of.get(),
+                                                                                                               st->slot_meta.get(), d_info);
+    FRZ_CUDA_TRY(cudaGetLastError());
+    uint64_t info[2] = {0, 0};
+    FRZ_CUDA_TRY(cudaMemcpyAsync(info, d_info, sizeof info, cudaMemcpyDeviceToHost, stream));
+    FRZ_CUDA_TRY(cudaStreamSynchronize(stream));
+    st->n_removed += info[0];
+    st->total_bytes -= info[1];
+    return FRZ_OK;
+}
+
+// Replaces haystacks which[j] by host Arrow strings (arguments checked by the caller), re-packing only their tiles.
+frz_status frz_replace_host(FrzIngest& ing, FrzCorpusStorage& scratch, const uint32_t* which, uint64_t n, const uint8_t* h_bytes,
+                            const void* h_offsets, int offset_width, cudaStream_t stream, FrzCorpusStorage* st) {
+    if (offset_width == 4)
+        return replace_host_t<uint32_t>(ing, scratch, which, n, h_bytes, static_cast<const uint32_t*>(h_offsets), stream, st);
+    return replace_host_t<uint64_t>(ing, scratch, which, n, h_bytes, static_cast<const uint64_t*>(h_offsets), stream, st);
 }

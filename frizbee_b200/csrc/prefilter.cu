@@ -715,6 +715,7 @@ __global__ void __launch_bounds__(128) k_match_indices(const FrzCorpusView cv, c
         const uint32_t tile = idx >> FRZ_TILE_SHIFT;
         const uint32_t slot = cv.slot_of[idx];
         const uint32_t meta = cv.slot_meta[(uint64_t)tile * FRZ_TILE + slot];
+        if (meta == FRZ_INVALID_SLOT) continue;   // a removed haystack (frz_corpus_remove) matches nothing
         const int len = (int)(meta >> FRZ_TILE_SHIFT);
         const FrzGroupDesc gd = cv.groups[tile * FRZ_GROUPS_PER_TILE + (slot >> 5)];
         const GlobalAcc ga{cv.data + frz_slot_unit0(gd, slot & 31)};

@@ -152,7 +152,8 @@ FRZ_API void frz_query_destroy(frz_query* q);
 
 /* ----------------------------------------------------------------- corpus */
 
-/* A haystack list, packed and resident in HBM on one device.  Read-only for matchers (only frz_corpus_append mutates it),
+/* A haystack list, packed and resident in HBM on one device.  Read-only for matchers (only frz_corpus_append, _remove and
+ * _replace mutate it),
  * reusable across matchers/needles (the interactive use: haystacks fixed, needle changes).
  * Replaces the `&[S: AsRef<str>]` argument of Matcher::match_list (src/matcher/mod.rs:212).
  * Input is Arrow-style: `bytes` = concatenated UTF-8, `offsets[n+1]` monotone byte offsets. */
@@ -171,6 +172,29 @@ FRZ_API frz_status frz_corpus_create_arrow(const uint8_t* bytes, const void* off
  * Vec<String> it later passes to Matcher::match_list, src/matcher/mod.rs:212.) */
 FRZ_API frz_status frz_corpus_append(frz_corpus* c, const uint8_t* bytes, const void* offsets, int offset_width,
                              uint64_t n_new);
+/* In-place edits.  (Reference side: the caller removing or rewriting entries of the Vec<String> it later passes to
+ * Matcher::match_list, src/matcher/mod.rs:212.)  After any sequence of create / append / remove / replace, every match call
+ * on the corpus (frz_match_list, _top, _into, frz_match_indices, frz_match_shard_device, frz_match_list_parallel*) returns
+ * what it returns on a fresh corpus of the current list, minus the rows of removed indices, in the same order;
+ * frz_match_indices reports a removed row as not matching.  Both calls are synchronous and check every argument on the
+ * host before anything changes, so a refused call leaves the corpus as it was; the caller must not run them concurrently
+ * with a match on the same corpus.  n == 0 is a no-op that makes no CUDA call.  An index >= frz_corpus_len, or a NULL
+ * array with n > 0, is FRZ_ERR_INVALID_ARG.
+ *
+ * Haystacks which[0..n) stop matching in every call on this corpus.  Indices do not move: frz_corpus_len is unchanged
+ * and later appends continue after it.  Removing a removed haystack is a no-op; duplicates in `which` are allowed. */
+FRZ_API frz_status frz_corpus_remove(frz_corpus* c, const uint32_t* which, uint64_t n);
+/* Haystack which[j] becomes bytes[offsets[j], offsets[j+1]) (Arrow buffers, offset width 4 or 8, host memory); a removed
+ * haystack comes back.  Only the tiles holding `which` are re-packed, in one batch, at the end of the packed arena; when
+ * the space they leave behind outgrows the live data the arena is compacted into a fresh one (old and new arena are held
+ * together while the units move).  The compaction is the last step and only an optimisation: when its arena cannot be
+ * allocated the call still succeeds, keeps the dead space and the next edit tries again.  Device memory beyond
+ * frz_corpus_device_bytes while the call runs: the touched tiles' raw bytes, the new strings and the touched tiles'
+ * metadata (about a second copy of the list when every tile is touched); the corpus keeps this staging for its next edit
+ * only while it is under 64 MiB, a larger one is given back when the call returns.
+ * A duplicate index is FRZ_ERR_INVALID_ARG, a replacement over 4194302 bytes FRZ_ERR_UNSUPPORTED. */
+FRZ_API frz_status frz_corpus_replace(frz_corpus* c, const uint32_t* which, uint64_t n, const uint8_t* bytes,
+                                      const void* offsets, int offset_width);
 /* same, from a pointer array + lengths (the layout a Rust `&[&str]` has) */
 FRZ_API frz_status frz_corpus_create_ptrs(const uint8_t* const* ptrs, const uint32_t* lens, uint64_t n,
                                   int device, frz_corpus** out);
@@ -184,9 +208,9 @@ FRZ_API frz_status frz_corpus_create_device(const uint8_t* d_bytes, const uint64
                                     uint64_t total_bytes, int device, void* stream, frz_corpus** out);
 /* Every constructor, frz_corpus_append and the end-to-end calls refuse a haystack longer than 4194302 bytes (4 MiB - 2)
  * with FRZ_ERR_UNSUPPORTED; a refused append leaves the corpus as it was. */
-FRZ_API uint64_t frz_corpus_len(const frz_corpus* c);
-FRZ_API uint64_t frz_corpus_total_bytes(const frz_corpus* c);   /* sum of haystack lengths */
-FRZ_API uint64_t frz_corpus_device_bytes(const frz_corpus* c);  /* HBM footprint of the packed form */
+FRZ_API uint64_t frz_corpus_len(const frz_corpus* c);           /* size of the index space (removed indices included) */
+FRZ_API uint64_t frz_corpus_total_bytes(const frz_corpus* c);   /* sum of the live (not removed) haystacks' lengths */
+FRZ_API uint64_t frz_corpus_device_bytes(const frz_corpus* c);  /* HBM footprint of the packed form (dead arena space included) */
 FRZ_API int frz_corpus_device(const frz_corpus* c);
 FRZ_API void frz_corpus_destroy(frz_corpus* c);
 
@@ -373,6 +397,9 @@ FRZ_API frz_status frz_corpus_debug_image(const frz_corpus* c, void* tile_base, 
 /* Test aid: bytes of device memory the library holds right now, over every device (corpora, matchers, communicators
  * and internal scratch).  Lets tests check that repeated calls and destroyed objects leave nothing behind. */
 FRZ_API uint64_t frz_debug_device_bytes(void);
+/* Test aid: the most bytes frz_debug_device_bytes has held since the last call with reset != 0 (which first sets the mark
+ * to the current value): the peak device memory of the calls in between. */
+FRZ_API uint64_t frz_debug_device_bytes_peak(int reset);
 
 /* radix_sort_matches (src/sort.rs:6-40): stable, descending score; `matches` is host memory. */
 FRZ_API frz_status frz_radix_sort_matches(frz_match* matches, uint64_t n, int device);
