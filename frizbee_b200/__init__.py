@@ -16,7 +16,7 @@ import numpy as np
 from .types import (CaseMatching, CConfig, CMatch, Config, CPattern, Match, Matching, Pattern, Scoring,
                     SortStrategy, UnicodeMatching, as_pattern, pattern_array)
 
-__all__ = ["Matcher", "Corpus", "Pattern", "Config", "Scoring", "Match", "SortStrategy", "CaseMatching",
+__all__ = ["Matcher", "Corpus", "Subset", "Pattern", "Config", "Scoring", "Match", "SortStrategy", "CaseMatching",
            "UnicodeMatching", "Matching", "FrizbeeError", "parse_query", "parse_atom", "radix_sort_matches",
            "MATCH_DTYPE", "lib", "lib_path"]
 
@@ -91,6 +91,13 @@ def lib():
     L.frz_matcher_last_timings.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(u64)]
     L.frz_match_list.argtypes = [vp, vp, vp, u64, C.POINTER(u64)]
     L.frz_match_list_top.argtypes = [vp, vp, u64, vp, C.POINTER(u64), C.POINTER(u64)]
+    L.frz_subset_create.argtypes = [vp, vp, u64, C.POINTER(vp)]
+    L.frz_subset_len.restype = u64
+    L.frz_subset_len.argtypes = [vp]
+    L.frz_subset_destroy.argtypes = [vp]
+    L.frz_subset_destroy.restype = None
+    L.frz_match_list_subset.argtypes = [vp, vp, vp, vp, u64, C.POINTER(u64)]
+    L.frz_match_list_subset_top.argtypes = [vp, vp, vp, u64, vp, C.POINTER(u64), C.POINTER(u64)]
     L.frz_match_list_into.argtypes = [vp, vp, u32, vp, u64, C.POINTER(u64)]
     L.frz_match_list_host.argtypes = [vp, vp, vp, u64, C.c_int, vp, u64, C.POINTER(u64)]
     L.frz_match_list_host_arrow.argtypes = [vp, vp, vp, C.c_int, u64, C.c_int, vp, u64, C.POINTER(u64)]
@@ -234,6 +241,14 @@ class Corpus:
         data, offsets = pack_host(haystacks)
         return self.replace(which, data, offsets)
 
+    def subset(self, which) -> "Subset":
+        """The rows `which` (any order, duplicates allowed) as a resident subset for Matcher.match_list_subset_array and
+        match_list_subset_top_array.  Close it before the corpus."""
+        which = np.ascontiguousarray(which, dtype=np.uint32)
+        h = C.c_void_p()
+        _check(lib().frz_subset_create(self._h, which.ctypes.data if which.size else None, len(which), C.byref(h)))
+        return Subset(h, self)
+
     def __len__(self):
         return self.n
 
@@ -248,6 +263,28 @@ class Corpus:
     def close(self):
         if self._h:
             lib().frz_corpus_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class Subset:
+    """A chosen set of rows of one resident Corpus (frz_subset); membership is by index and survives corpus edits."""
+
+    def __init__(self, handle, corpus: Corpus):
+        self._h = handle
+        self.corpus = corpus
+
+    def __len__(self):
+        return lib().frz_subset_len(self._h)
+
+    def close(self):
+        if self._h:
+            lib().frz_subset_destroy(self._h)
             self._h = None
 
     def __del__(self):
@@ -349,6 +386,21 @@ class Matcher:
         finally:
             if owned:
                 corpus.close()
+
+    def match_list_subset_array(self, corpus: Corpus, subset: Subset, out: Optional[np.ndarray] = None) -> np.ndarray:
+        """match_list_array(corpus) restricted to the subset's members (frz_match_list_subset), in the same order."""
+        if out is None:
+            out = np.empty(max(1, len(subset)), dtype=MATCH_DTYPE)
+        n = C.c_uint64()
+        _check(lib().frz_match_list_subset(self._h, corpus._h, subset._h, out.ctypes.data, len(out), C.byref(n)))
+        return out[: n.value]
+
+    def match_list_subset_top_array(self, corpus: Corpus, subset: Subset, k: int) -> Tuple[np.ndarray, int]:
+        """The first k rows of match_list_subset_array (frz_match_list_subset_top): (array of min(k, total) matches, total)."""
+        out = np.empty(max(1, min(int(k), len(subset))), dtype=MATCH_DTYPE)
+        n, total = C.c_uint64(), C.c_uint64()
+        _check(lib().frz_match_list_subset_top(self._h, corpus._h, subset._h, int(k), out.ctypes.data, C.byref(n), C.byref(total)))
+        return out[: n.value], total.value
 
     def match_list_into_array(self, haystacks, index_offset: int = 0, device: int = 0) -> np.ndarray:
         """Specialized::match_list / Matcher::match_list_into: index order, unsorted."""

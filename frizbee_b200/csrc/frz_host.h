@@ -239,6 +239,8 @@ struct FrzWorkspace {
     FrzDevArray<uint64_t> retain_base;
     FrzDevArray<uint8_t> retain_keep;
     FrzDevArray<uint16_t> unicode_scratch;  // unicode.cu: per-thread row state of the per-scalar Smith-Waterman
+    FrzDevArray<uint32_t> subset_meta;      // [n_tiles * 1024] slot metadata of a subset call: non-members are unused slots
+    FrzDevArray<FrzMatchDev> subset_list;   // [2 * members] list-form subset call: member records, then the live ones compacted
     FrzEvent ev[4];                         // call start, scan done, scoring done, call end
     bool ev_rec[4] = {false, false, false, false};  // recorded during the current call
 };

@@ -844,13 +844,6 @@ __global__ void k_reverse(const FrzMatchDev* in, FrzMatchDev* out, const unsigne
     for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (unsigned long long)gridDim.x * blockDim.x)
         out[n - 1 - i] = in[i];
 }
-// candidate bitmap over haystack indices (relative to index_offset)
-__global__ void k_bitmap_set(const FrzMatchDev* cand, uint64_t n, uint32_t index_offset, uint32_t* bitmap) {
-    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
-        uint32_t idx = cand[i].index - index_offset;
-        atomicOr(&bitmap[idx >> 5], 1u << (idx & 31));
-    }
-}
 // keep[i] = candidate i is (not) hit; hits are index-ordered → binary search
 __device__ __forceinline__ long long find_hit(const FrzMatchDev* hits, uint64_t nh, uint32_t index) {
     uint64_t lo = 0, hi = nh;
@@ -947,6 +940,47 @@ __global__ void __launch_bounds__(kCompactBlock) k_live_keep(const uint32_t* __r
         block_count[blockIdx.x] = s;
     }
 }
+// Slot metadata of a subset call: slot s keeps its metadata when its haystack, index (s & ~1023) + (meta & 1023), is below
+// n_bits with its bit set in `bits`; every other slot becomes FRZ_INVALID_SLOT, which the matching kernels skip.  Four
+// slots of one tile per thread (n_slots is a multiple of FRZ_TILE).
+__global__ void k_subset_meta(const uint4* __restrict__ slot_meta, uint64_t n_quads, const uint32_t* __restrict__ bits, uint64_t n_bits,
+                              uint4* __restrict__ out) {
+    for (uint64_t q = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; q < n_quads; q += (uint64_t)gridDim.x * blockDim.x) {
+        const uint64_t tile0 = (q * 4) & ~(uint64_t)(FRZ_TILE - 1);
+        uint32_t v[4];
+        *reinterpret_cast<uint4*>(v) = slot_meta[q];
+#pragma unroll
+        for (int j = 0; j < 4; j++) {
+            const uint64_t idx = tile0 + (v[j] & (FRZ_TILE - 1));
+            if (v[j] == FRZ_INVALID_SLOT || idx >= n_bits || !((bits[idx >> 5] >> (idx & 31)) & 1u)) v[j] = FRZ_INVALID_SLOT;
+        }
+        out[q] = *reinterpret_cast<const uint4*>(v);
+    }
+}
+// The list form of a subset call: cand[j] = member j as a match record, keep[j] = its slot is in use (removed members are
+// dropped: the candidate-list prefilter reads their slot metadata unchecked), with per-block counts as k_retain_count
+// writes them for the retain compaction.
+__global__ void __launch_bounds__(kCompactBlock) k_member_keep(const uint32_t* __restrict__ members, uint64_t n,
+                                                               const uint32_t* __restrict__ slot_meta, const uint16_t* __restrict__ slot_of,
+                                                               uint32_t* block_count, uint8_t* keep, FrzMatchDev* cand) {
+    __shared__ uint32_t wc[32];
+    const uint64_t i = (uint64_t)blockIdx.x * kCompactBlock + threadIdx.x;
+    bool k = false;
+    if (i < n) {
+        const uint32_t idx = members[i];
+        k = slot_meta[(idx & ~(uint32_t)(FRZ_TILE - 1)) + slot_of[idx]] != FRZ_INVALID_SLOT;
+        keep[i] = k;
+        cand[i] = FrzMatchDev{idx, 0, 0, 0};
+    }
+    const uint32_t b = __ballot_sync(0xffffffffu, k);
+    if ((threadIdx.x & 31) == 0) wc[threadIdx.x >> 5] = __popc(b);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        uint32_t s = 0;
+        for (int w = 0; w < 32; w++) s += wc[w];
+        block_count[blockIdx.x] = s;
+    }
+}
 
 frz_status ensure_workspace(frz_matcher* m, const FrzCorpusStorage& cs, uint64_t survivor_cap) {
     FrzWorkspace& ws = m->ws;
@@ -1020,14 +1054,16 @@ frz_status needle_table(frz_matcher* m, const Compiled& c, const FrzNeedleTab** 
     return FRZ_OK;
 }
 
-// One pattern over the corpus (optionally restricted to a candidate bitmap) → index-ordered matches in
-// d_out (reversed order if `reversed`); the count is left in ws.counters->total (device).
-frz_status run_pattern(frz_matcher* m, const FrzCorpusStorage& cs, const Compiled& c, const uint32_t* cand_bitmap,
+// One pattern over the corpus (optionally restricted to a candidate list) → index-ordered matches in d_out (reversed
+// order if `reversed`); the count is left in ws.counters->total (device).  masked_meta (subset calls): slot metadata to
+// read in place of the corpus's own, nullptr = the corpus's.
+frz_status run_pattern(frz_matcher* m, const FrzCorpusStorage& cs, const Compiled& c, const uint32_t* masked_meta,
                        uint32_t index_offset, bool reversed, FrzMatchDev* d_out, cudaStream_t stream, FrzLaunchStats* st,
                        bool record_events, const FrzMatchDev* cand_list = nullptr, uint64_t n_cand = 0,
                        const FrzScoreHist& hist = FrzScoreHist()) {
     FrzWorkspace& ws = m->ws;
-    const FrzCorpusView cv = cs.view();
+    FrzCorpusView cv = cs.view();
+    if (masked_meta) cv.slot_meta = masked_meta;
     uint64_t cap = std::max(ws.survivor_cap(), initial_survivor_cap(cs, c.dev));
     FRZ_TRY(ensure_workspace(m, cs, cap));
     const FrzNeedleTab* ntab = nullptr;
@@ -1039,7 +1075,7 @@ frz_status run_pattern(frz_matcher* m, const FrzCorpusStorage& cs, const Compile
     else FRZ_TRY(frz_launch_prefilter(cv, c.dev, ws, stream, st, ntab));
     FRZ_TRY(frz_launch_tile_scan(cv, ws, stream, st));
     if (record_events) { cudaEventRecord(ws.ev[1].get(), stream); ws.ev_rec[1] = true; }
-    if (m->early_count_dst && !cand_list && !cand_bitmap && m->compiled.size() == 1) {
+    if (m->early_count_dst && !cand_list && m->compiled.size() == 1) {
         // single pattern: every survivor becomes exactly one match, so the scan total is the final count
         FRZ_CUDA_TRY(cudaMemcpyAsync(m->early_count_dst, &ws.counters.get()->total, sizeof(uint64_t), cudaMemcpyDeviceToDevice, stream));
         FRZ_CUDA_TRY(cudaEventRecord(m->count_ev.get(), stream));
@@ -1075,16 +1111,19 @@ int grid_for(uint64_t n, int block) {
 }
 
 // Every index of the corpus, ascending, into `out` (count in ws.counters->total): the list of the empty matcher and the
-// start of an all-negated one.  A corpus with removed haystacks fills `tmp` and keeps only the live indices.
+// start of an all-negated one.  A corpus with removed haystacks, or a subset call (masked_meta, as in run_pattern), fills
+// `tmp` and keeps only the indices whose slot is in use.
 frz_status fill_all(frz_matcher* m, const FrzCorpusStorage& cs, uint32_t index_offset, FrzMatchDev* out, FrzMatchDev* tmp,
-                    cudaStream_t stream, FrzLaunchStats* st) {
+                    cudaStream_t stream, FrzLaunchStats* st, const uint32_t* masked_meta = nullptr) {
     FrzWorkspace& ws = m->ws;
-    k_fill_all<<<grid_for(cs.n, 256), 256, 0, stream>>>(cs.n_removed ? tmp : out, cs.n, index_offset, ws.counters.get());
+    const bool filter = cs.n_removed || masked_meta;
+    k_fill_all<<<grid_for(cs.n, 256), 256, 0, stream>>>(filter ? tmp : out, cs.n, index_offset, ws.counters.get());
     st->launches++;
-    if (cs.n_removed) {
+    if (filter && cs.n) {
         FRZ_TRY(ensure_retain_buffers(m, cs.n));
         const uint32_t nb = (uint32_t)((cs.n + kCompactBlock - 1) / kCompactBlock);
-        k_live_keep<<<nb, kCompactBlock, 0, stream>>>(cs.slot_meta.get(), cs.slot_of.get(), cs.n, ws.retain_cnt.get(), ws.retain_keep.get());
+        k_live_keep<<<nb, kCompactBlock, 0, stream>>>(masked_meta ? masked_meta : cs.slot_meta.get(), cs.slot_of.get(), cs.n,
+                                                      ws.retain_cnt.get(), ws.retain_keep.get());
         k_scan_blocks<<<1, 1024, 0, stream>>>(ws.retain_cnt.get(), ws.retain_base.get(), nb, ws.counters.get());
         k_retain_scatter<<<nb, kCompactBlock, 0, stream>>>(tmp, cs.n, ws.retain_keep.get(), ws.retain_base.get(), out);
         st->launches += 3;
@@ -1093,14 +1132,36 @@ frz_status fill_all(frz_matcher* m, const FrzCorpusStorage& cs, uint32_t index_o
     return FRZ_OK;
 }
 
+// The rows of a subset call, in one of two forms (DESIGN.md §4.9): slot metadata in which non-members are unused slots
+// (masked form), or the live members, index-ordered, as a candidate list (list form).  The default scope is the whole
+// corpus.
+struct SubsetScope {
+    const uint32_t* masked_meta = nullptr;
+    const FrzMatchDev* list = nullptr;
+    uint64_t n_list = 0;
+};
+
+// the list form's members → `out` as the start of a list, count → ws.counters->total
+frz_status copy_scope_list(frz_matcher* m, const SubsetScope& scope, FrzMatchDev* out, cudaStream_t stream) {
+    FrzWorkspace& ws = m->ws;
+    FRZ_CUDA_TRY(cudaMemcpyAsync(out, scope.list, scope.n_list * sizeof(FrzMatchDev), cudaMemcpyDeviceToDevice, stream));
+    ws.h_counters.get()->total = scope.n_list;
+    FRZ_CUDA_TRY(cudaMemcpyAsync(&ws.counters.get()->total, &ws.h_counters.get()->total, sizeof(unsigned long long), cudaMemcpyHostToDevice, stream));
+    return FRZ_OK;
+}
+
 // match_list_into over all compiled patterns → index-ordered device list; returns pointer + leaves the
 // count in ws.counters->total.  `final_reversed` asks for the list in descending index order.  `score_hist` (optional):
 // the caller will sort the list by score; where the scoring kernels emit the list directly and one sort pass will do,
-// they also build the sort's histogram, returned there (score_hist->counts stays nullptr otherwise).
+// they also build the sort's histogram, returned there (score_hist->counts stays nullptr otherwise).  scope: the rows of
+// a subset call.  The list form's base pattern takes the members as its candidate list, and the empty and all-negated
+// matchers start from them.
 frz_status match_into_device(frz_matcher* m, const FrzCorpusStorage& cs, uint32_t index_offset, bool final_reversed,
                              FrzMatchDev** d_result, uint32_t* score_bound, cudaStream_t stream, FrzLaunchStats* st,
-                             FrzMatchDev* prefer_out = nullptr, FrzScoreHist* score_hist = nullptr) {
+                             FrzMatchDev* prefer_out = nullptr, FrzScoreHist* score_hist = nullptr,
+                             const SubsetScope& scope = SubsetScope()) {
     FrzWorkspace& ws = m->ws;
+    const uint32_t* masked_meta = scope.masked_meta;
     if ((uint64_t)cs.n + index_offset > 0xFFFFFFFFull)
         return frz_fail(FRZ_ERR_TOO_MANY_ITEMS, "too many items in haystack, will overflow the u32 index: %llu > %u (index offset: %u)",
                         (unsigned long long)cs.n + index_offset, 0xFFFFFFFFu, index_offset);
@@ -1109,7 +1170,8 @@ frz_status match_into_device(frz_matcher* m, const FrzCorpusStorage& cs, uint32_
     if (pats.empty()) {  // CompiledPatterns::Empty (src/matcher/mod.rs:380-383)
         FRZ_TRY(ensure_workspace(m, cs, 1));
         FRZ_CUDA_TRY(cudaMemsetAsync(ws.counters.get(), 0, sizeof(FrzCounters), stream));
-        FRZ_TRY(fill_all(m, cs, index_offset, ws.matches_a.get(), ws.matches_b.get(), stream, st));
+        if (scope.list) FRZ_TRY(copy_scope_list(m, scope, ws.matches_a.get(), stream));
+        else FRZ_TRY(fill_all(m, cs, index_offset, ws.matches_a.get(), ws.matches_b.get(), stream, st, masked_meta));
         if (final_reversed) {
             k_reverse<<<grid_for(cs.n, 256), 256, 0, stream>>>(ws.matches_a.get(), ws.matches_b.get(), &ws.counters.get()->total);
             st->launches++;
@@ -1126,7 +1188,8 @@ frz_status match_into_device(frz_matcher* m, const FrzCorpusStorage& cs, uint32_
             FRZ_TRY(frz_sort_fused_prepare(ws.sort, cs.n, pats[0].score_bound, stream, &hist));
             *score_hist = hist;
         }
-        FRZ_TRY(run_pattern(m, cs, pats[0], nullptr, index_offset, final_reversed, dst, stream, st, true, nullptr, 0, hist));
+        FRZ_TRY(run_pattern(m, cs, pats[0], masked_meta, index_offset, final_reversed, dst, stream, st, true, scope.list, scope.n_list,
+                            hist));
         *d_result = dst;
         *score_bound = pats[0].score_bound;
         return FRZ_OK;
@@ -1141,14 +1204,20 @@ frz_status match_into_device(frz_matcher* m, const FrzCorpusStorage& cs, uint32_
     uint64_t nc = 0;
     uint64_t bound = 0;
     if (base >= 0) {
-        FRZ_TRY(run_pattern(m, cs, pats[base], nullptr, index_offset, false, cand, stream, st, true));
+        FRZ_TRY(run_pattern(m, cs, pats[base], masked_meta, index_offset, false, cand, stream, st, true, scope.list, scope.n_list));
         FRZ_TRY(read_counters(m, stream));
         nc = ws.h_counters.get()->total;
         bound = pats[base].score_bound;
+    } else if (scope.list) {
+        FRZ_TRY(copy_scope_list(m, scope, cand, stream));
+        nc = scope.n_list;
     } else {
         FRZ_CUDA_TRY(cudaMemsetAsync(ws.counters.get(), 0, sizeof(FrzCounters), stream));
-        FRZ_TRY(fill_all(m, cs, index_offset, cand, spare, stream, st));
-        nc = cs.n - cs.n_removed;
+        FRZ_TRY(fill_all(m, cs, index_offset, cand, spare, stream, st, masked_meta));
+        if (masked_meta) {   // the members in use are counted on the device
+            FRZ_TRY(read_counters(m, stream));
+            nc = ws.h_counters.get()->total;
+        } else nc = cs.n - cs.n_removed;
     }
     FRZ_TRY(ensure_retain_buffers(m, cs.n));
     uint32_t* d_block_cnt = ws.retain_cnt.get();
@@ -1209,10 +1278,10 @@ __global__ void k_copy_n(const FrzMatchDev* __restrict__ in, FrzMatchDev* __rest
 
 // `final_out` (optional, device, >= corpus length): where the final list must land.  `limit` (top-K calls): only the first
 // `limit` positions of the final list are written (the sort's last scatter and the final copy drop the rest); the count in
-// ws.counters->total stays the full match count.
+// ws.counters->total stays the full match count.  scope: as in match_into_device.
 frz_status match_list_device(frz_matcher* m, const FrzCorpusStorage& cs, uint32_t index_offset, uint8_t sort,
                              FrzMatchDev** d_result, cudaStream_t stream, FrzLaunchStats* st, FrzMatchDev* final_out = nullptr,
-                             uint32_t limit = kFrzNoLimit) {
+                             uint32_t limit = kFrzNoLimit, const SubsetScope& scope = SubsetScope()) {
     FrzWorkspace& ws = m->ws;
     const bool reversed = sort == FRZ_SORT_INDEX_DESC || sort == FRZ_SORT_SCORE_THEN_INDEX_DESC;
     const bool by_score = sort == FRZ_SORT_SCORE_THEN_INDEX_ASC || sort == FRZ_SORT_SCORE_THEN_INDEX_DESC;
@@ -1223,7 +1292,7 @@ frz_status match_list_device(frz_matcher* m, const FrzCorpusStorage& cs, uint32_
     uint32_t bound = 0;
     FrzScoreHist hist;
     FRZ_TRY(match_into_device(m, cs, index_offset, reversed, &d_list, &bound, stream, st, will_sort ? nullptr : final_out,
-                              will_sort ? &hist : nullptr));
+                              will_sort ? &hist : nullptr, scope));
     // `!self.patterns.is_empty() && sort.is_by_score()` (src/matcher/mod.rs:218)
     if (will_sort) {
         FrzMatchDev* other = final_out ? final_out : (d_list == ws.matches_a.get() ? ws.matches_b.get() : ws.matches_a.get());
@@ -1293,17 +1362,15 @@ frz_status copy_out_top(frz_matcher* m, FrzMatchDev* d_list, uint64_t k, frz_mat
     return FRZ_OK;
 }
 
-}  // namespace
-
-extern "C" frz_status frz_match_list(frz_matcher* m, const frz_corpus* corpus, frz_match* out, uint64_t cap, uint64_t* n_out) {
-    if (!m || !corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
-    FRZ_TRY(ensure_device(corpus->st.device));
+// Matcher::match_list → host.  scope: the rows of a subset call (match_into_device).
+frz_status match_list_host_out(frz_matcher* m, const frz_corpus* corpus, const SubsetScope& scope, frz_match* out, uint64_t cap,
+                               uint64_t* n_out) {
     cudaStream_t stream = nullptr;
     FrzLaunchStats st;
     FrzMatchDev* d_list = nullptr;
     frz_status s = FRZ_OK;
     for (int attempt = 0; attempt < 2; attempt++) {
-        s = match_list_device(m, corpus->st, 0, m->config.sort, &d_list, stream, &st);
+        s = match_list_device(m, corpus->st, 0, m->config.sort, &d_list, stream, &st, nullptr, kFrzNoLimit, scope);
         if (s == FRZ_OK) s = copy_out(m, d_list, out, cap, n_out, stream);
         if (s != kRetryOverflow) break;
         FRZ_TRY(ensure_workspace(m, corpus->st, std::max<uint64_t>(corpus->st.n, 1)));  // worst-case lists, then once more
@@ -1314,18 +1381,15 @@ extern "C" frz_status frz_match_list(frz_matcher* m, const frz_corpus* corpus, f
 }
 
 // Matcher::match_list followed by truncation to the first k rows: the same pipeline with a limit on the final scatter and copy
-extern "C" frz_status frz_match_list_top(frz_matcher* m, const frz_corpus* corpus, uint64_t k, frz_match* out, uint64_t* n_out,
-                                         uint64_t* n_total) {
-    if (!m || !corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
-    if (!out && k > 0) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
-    FRZ_TRY(ensure_device(corpus->st.device));
+frz_status match_list_top_host_out(frz_matcher* m, const frz_corpus* corpus, const SubsetScope& scope, uint64_t k, frz_match* out,
+                                   uint64_t* n_out, uint64_t* n_total) {
     cudaStream_t stream = nullptr;
     FrzLaunchStats st;
     FrzMatchDev* d_list = nullptr;
     const uint32_t limit = (uint32_t)std::min<uint64_t>(k, kFrzNoLimit);   // a list never holds more than 2^32 - 1 matches
     frz_status s = FRZ_OK;
     for (int attempt = 0; attempt < 2; attempt++) {
-        s = match_list_device(m, corpus->st, 0, m->config.sort, &d_list, stream, &st, nullptr, limit);
+        s = match_list_device(m, corpus->st, 0, m->config.sort, &d_list, stream, &st, nullptr, limit, scope);
         if (s == FRZ_OK) s = copy_out_top(m, d_list, k, out, n_out, n_total, stream);
         if (s != kRetryOverflow) break;
         FRZ_TRY(ensure_workspace(m, corpus->st, std::max<uint64_t>(corpus->st.n, 1)));  // worst-case lists, then once more
@@ -1333,6 +1397,145 @@ extern "C" frz_status frz_match_list_top(frz_matcher* m, const frz_corpus* corpu
     if (s == kRetryOverflow) s = frz_fail(FRZ_ERR_CUDA, "survivor list overflow persisted");
     collect_timings(m, st);
     return s;
+}
+
+}  // namespace
+
+extern "C" frz_status frz_match_list(frz_matcher* m, const frz_corpus* corpus, frz_match* out, uint64_t cap, uint64_t* n_out) {
+    if (!m || !corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    FRZ_TRY(ensure_device(corpus->st.device));
+    return match_list_host_out(m, corpus, SubsetScope(), out, cap, n_out);
+}
+
+extern "C" frz_status frz_match_list_top(frz_matcher* m, const frz_corpus* corpus, uint64_t k, frz_match* out, uint64_t* n_out,
+                                         uint64_t* n_total) {
+    if (!m || !corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    if (!out && k > 0) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
+    FRZ_TRY(ensure_device(corpus->st.device));
+    return match_list_top_host_out(m, corpus, SubsetScope(), k, out, n_out, n_total);
+}
+
+// ---------------------------------------------------------------------------------- subsets
+// A bitmap over the indices [0, n_bits) of the corpus at creation (later appends lie beyond it and are not members), and
+// the same members as an ascending list.
+struct frz_subset {
+    const frz_corpus* corpus;
+    FrzDevArray<uint32_t> bits;      // ceil(n_bits / 32) words on the corpus's device (masked form)
+    FrzDevArray<uint32_t> members;   // n_members ascending indices on the corpus's device (list form)
+    uint64_t n_bits;
+    uint64_t n_members;              // distinct members
+};
+
+extern "C" frz_status frz_subset_create(const frz_corpus* c, const uint32_t* which, uint64_t n, frz_subset** out) {
+    if (!c || !out || (n && !which)) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    FRZ_TRY(check_indices(c, which, n));
+    auto s = std::make_unique<frz_subset>();
+    s->corpus = c;
+    s->n_bits = c->st.n;
+    std::vector<uint32_t> bits((s->n_bits + 31) / 32, 0);
+    for (uint64_t j = 0; j < n; j++) bits[which[j] >> 5] |= 1u << (which[j] & 31);
+    std::vector<uint32_t> members;
+    for (size_t w = 0; w < bits.size(); w++)
+        for (uint32_t x = bits[w]; x; x &= x - 1) members.push_back((uint32_t)(w * 32 + __builtin_ctz(x)));
+    s->n_members = members.size();
+    if (!bits.empty()) {
+        FRZ_TRY(ensure_device(c->st.device));
+        FRZ_TRY(s->bits.reserve(bits.size()));
+        FRZ_CUDA_TRY(cudaMemcpy(s->bits.get(), bits.data(), bits.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    }
+    if (!members.empty()) {
+        FRZ_TRY(s->members.reserve(members.size()));
+        FRZ_CUDA_TRY(cudaMemcpy(s->members.get(), members.data(), members.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    }
+    *out = s.release();
+    return FRZ_OK;
+}
+extern "C" uint64_t frz_subset_len(const frz_subset* s) { return s ? s->n_members : 0; }
+extern "C" void frz_subset_destroy(frz_subset* s) { delete s; }
+
+// A subset call takes the list form when its members are at most FRZ_SUBSET_LIST_PERMILLE / 1000 of the corpus, the masked
+// form otherwise (DESIGN.md §4.9: the threshold comes from tools/bench_subset.py).  Comparison builds set -1 (masked form
+// only) or 1000 (list form only): `python frizbee_b200/build.py --variant NAME --define FRZ_SUBSET_LIST_PERMILLE=V`.
+#ifndef FRZ_SUBSET_LIST_PERMILLE
+#define FRZ_SUBSET_LIST_PERMILLE 20
+#endif
+
+namespace {
+frz_status check_subset_call(const frz_matcher* m, const frz_corpus* corpus, const frz_subset* s) {
+    if (!m || !corpus || !s) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    if (s->corpus != corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "the subset was made on another corpus");
+    return ensure_device(corpus->st.device);
+}
+
+// The rows of a subset call, built in the matcher's workspace on every call, so edits of the corpus between calls need no
+// bookkeeping.  Masked form: the corpus's slot metadata with every non-member an unused slot.  List form: the members
+// whose slots are in use, index-ordered.  *none: no row can match (the list form found no member in use), the caller
+// returns an empty list without running the pipeline.  An empty corpus keeps the default scope: it has no row.
+frz_status subset_scope(frz_matcher* m, const frz_corpus* corpus, const frz_subset& s, cudaStream_t stream, SubsetScope* out,
+                        bool* none) {
+    const FrzCorpusStorage& cs = corpus->st;
+    *out = SubsetScope();
+    *none = false;
+    if (cs.n == 0) return FRZ_OK;
+    FrzWorkspace& ws = m->ws;
+    FRZ_TRY(ensure_workspace(m, cs, 0));   // (on this device; the lists are sized by the match call)
+    constexpr int kListPermille = FRZ_SUBSET_LIST_PERMILLE;
+    if (kListPermille >= 0 && s.n_members * 1000 <= cs.n * (uint64_t)std::max(kListPermille, 0)) {
+        const uint64_t n = s.n_members;
+        if (n == 0) { *none = true; return FRZ_OK; }
+        FRZ_TRY(ws.subset_list.reserve(2 * n));
+        FRZ_TRY(ensure_retain_buffers(m, n));
+        FrzMatchDev* tmp = ws.subset_list.get();
+        FrzMatchDev* list = tmp + n;
+        const uint32_t nb = (uint32_t)((n + kCompactBlock - 1) / kCompactBlock);
+        FRZ_CUDA_TRY(cudaMemsetAsync(ws.counters.get(), 0, sizeof(FrzCounters), stream));
+        k_member_keep<<<nb, kCompactBlock, 0, stream>>>(s.members.get(), n, cs.slot_meta.get(), cs.slot_of.get(), ws.retain_cnt.get(),
+                                                        ws.retain_keep.get(), tmp);
+        k_scan_blocks<<<1, 1024, 0, stream>>>(ws.retain_cnt.get(), ws.retain_base.get(), nb, ws.counters.get());
+        k_retain_scatter<<<nb, kCompactBlock, 0, stream>>>(tmp, n, ws.retain_keep.get(), ws.retain_base.get(), list);
+        FRZ_CUDA_TRY(cudaGetLastError());
+        FRZ_TRY(read_counters(m, stream));
+        out->list = list;
+        out->n_list = ws.h_counters.get()->total;
+        *none = out->n_list == 0;
+        return FRZ_OK;
+    }
+    const uint64_t n_slots = (uint64_t)cs.n_tiles * FRZ_TILE;
+    FRZ_TRY(ws.subset_meta.reserve(n_slots));
+    k_subset_meta<<<grid_for(n_slots / 4, 256), 256, 0, stream>>>(reinterpret_cast<const uint4*>(cs.slot_meta.get()), n_slots / 4,
+                                                                  s.bits.get(), s.n_bits, reinterpret_cast<uint4*>(ws.subset_meta.get()));
+    FRZ_CUDA_TRY(cudaGetLastError());
+    out->masked_meta = ws.subset_meta.get();
+    return FRZ_OK;
+}
+}  // namespace
+
+extern "C" frz_status frz_match_list_subset(frz_matcher* m, const frz_corpus* corpus, const frz_subset* s, frz_match* out, uint64_t cap,
+                                            uint64_t* n_out) {
+    FRZ_TRY(check_subset_call(m, corpus, s));
+    SubsetScope scope;
+    bool none = false;
+    FRZ_TRY(subset_scope(m, corpus, *s, nullptr, &scope, &none));
+    if (none) {
+        if (n_out) *n_out = 0;
+        return FRZ_OK;
+    }
+    return match_list_host_out(m, corpus, scope, out, cap, n_out);
+}
+
+extern "C" frz_status frz_match_list_subset_top(frz_matcher* m, const frz_corpus* corpus, const frz_subset* s, uint64_t k, frz_match* out,
+                                                uint64_t* n_out, uint64_t* n_total) {
+    FRZ_TRY(check_subset_call(m, corpus, s));
+    if (!out && k > 0) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
+    SubsetScope scope;
+    bool none = false;
+    FRZ_TRY(subset_scope(m, corpus, *s, nullptr, &scope, &none));
+    if (none) {
+        if (n_out) *n_out = 0;
+        if (n_total) *n_total = 0;
+        return FRZ_OK;
+    }
+    return match_list_top_host_out(m, corpus, scope, k, out, n_out, n_total);
 }
 
 extern "C" frz_status frz_match_list_into(frz_matcher* m, const frz_corpus* corpus, uint32_t index_offset, frz_match* out,

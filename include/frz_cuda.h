@@ -252,6 +252,40 @@ FRZ_API frz_status frz_match_list(frz_matcher* m, const frz_corpus* corpus,
 FRZ_API frz_status frz_match_list_top(frz_matcher* m, const frz_corpus* corpus, uint64_t k,
                               frz_match* out, uint64_t* n_out, uint64_t* n_total);
 
+/* ---------------------------------------------------------------- subsets
+ *
+ * A chosen set of rows of a resident corpus, matched without staging them again: a picker scoped to one directory, a
+ * history search limited to this session, "search within these results".  (Reference side: the caller passing a
+ * smaller slice to Matcher::match_list, src/matcher/mod.rs:212.)  A subset is a bitmap over the corpus's indices,
+ * resident on the corpus's device.  Each subset call derives, in one pass over the tiles, slot metadata in which every
+ * non-member is an unused slot, and runs the match pipeline of the full call through it.
+ *
+ * frz_match_list_subset(m, c, s) is bit-identical to [r for r in frz_match_list(m, c) if r.index is a member of s], in
+ * the same order, for every matcher and sort strategy (per-haystack results do not depend on the other rows, and the
+ * sorts are stable on (score, index)).  The empty matcher returns the live members in index order, reversed for the
+ * *_DESC strategies.
+ *
+ * A subset belongs to the corpus it was made on: another corpus is FRZ_ERR_INVALID_ARG, and it must be destroyed before
+ * that corpus.  The match calls only read it, so several matchers may use it at once.  Membership is by index and
+ * survives edits of the corpus: rows appended after frz_subset_create are not members, a removed member stops matching
+ * as everywhere else, a replaced member stays a member with its new text. */
+typedef struct frz_subset frz_subset;
+/* The set {which[0..n)} of indices of `c` (any order, duplicates allowed), resident on c's device.  An index >=
+ * frz_corpus_len(c), or NULL with n > 0, is FRZ_ERR_INVALID_ARG; n == 0 is the empty set. */
+FRZ_API frz_status frz_subset_create(const frz_corpus* c, const uint32_t* which, uint64_t n, frz_subset** out);
+/* distinct indices given at creation, rows removed before or after it included (those never match, so the live count
+ * can be lower) */
+FRZ_API uint64_t frz_subset_len(const frz_subset* s);
+FRZ_API void frz_subset_destroy(frz_subset* s);
+/* frz_match_list restricted to the members: same arguments and capacity rule (FRZ_ERR_CAPACITY, *n_out = needed; room
+ * for frz_subset_len(s) matches suffices) */
+FRZ_API frz_status frz_match_list_subset(frz_matcher* m, const frz_corpus* corpus, const frz_subset* s,
+                                         frz_match* out, uint64_t cap, uint64_t* n_out);
+/* frz_match_list_top restricted to the members: same rules as frz_match_list_top.  The first min(k, total) rows of
+ * frz_match_list_subset's list; *n_total = its length.  Room for min(k, frz_subset_len(s)) matches in `out` suffices. */
+FRZ_API frz_status frz_match_list_subset_top(frz_matcher* m, const frz_corpus* corpus, const frz_subset* s, uint64_t k,
+                                             frz_match* out, uint64_t* n_out, uint64_t* n_total);
+
 /* Specialized::match_list / Matcher::match_list_into (src/matcher/algo.rs:17-22,
  * src/matcher/mod.rs:373-392): matches appended in input (index-ascending) order,
  * indices offset by `index_offset`, no sort. */
