@@ -13,6 +13,10 @@
 #include "unicode_path.cuh"
 
 frz_status frz_fail(frz_status s, const char* fmt, ...);
+// Argument checks of the entry points (host.cu), with their status codes and messages.
+frz_status frz_ensure_device(int device);                                  // a valid device, made current
+frz_status frz_check_offset_width(int offset_width);                       // Arrow offsets of 4 or 8 bytes
+frz_status frz_check_index_range(uint64_t n, uint32_t index_offset);       // the indices of n rows from index_offset fit in u32
 inline int frz_current_device() { int d = 0; cudaGetDevice(&d); return d; }
 // SMs of the current device (cached per device): persistent grids and grid caps are multiples of it
 inline int frz_sm_count() {

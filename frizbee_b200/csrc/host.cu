@@ -70,7 +70,7 @@ extern "C" void frz_config_default(frz_config* c) {
     c->emulate_lanes = 0;
 }
 
-static frz_status ensure_device(int device) {
+frz_status frz_ensure_device(int device) {
     int n = 0;
     cudaError_t e = cudaGetDeviceCount(&n);
     if (e != cudaSuccess || n == 0) {
@@ -80,6 +80,19 @@ static frz_status ensure_device(int device) {
     }
     if (device < 0 || device >= n) return frz_fail(FRZ_ERR_INVALID_ARG, "device %d out of range (have %d)", device, n);
     FRZ_CUDA_TRY(cudaSetDevice(device));
+    return FRZ_OK;
+}
+
+frz_status frz_check_offset_width(int offset_width) {
+    if (offset_width != 4 && offset_width != 8) return frz_fail(FRZ_ERR_INVALID_ARG, "offset_width must be 4 or 8");
+    return FRZ_OK;
+}
+
+// Matcher::guard_against_haystack_overflow (src/matcher/mod.rs:438-446)
+frz_status frz_check_index_range(uint64_t n, uint32_t index_offset) {
+    if (n + index_offset > 0xFFFFFFFFull)
+        return frz_fail(FRZ_ERR_TOO_MANY_ITEMS, "too many items in haystack, will overflow the u32 index: %llu > %u (index offset: %u)",
+                        (unsigned long long)(n + index_offset), 0xFFFFFFFFu, index_offset);
     return FRZ_OK;
 }
 
@@ -230,7 +243,7 @@ extern "C" frz_status frz_corpus_create_device(const uint8_t* d_bytes, const uin
                                                uint64_t total_bytes, int device, void* stream, frz_corpus** out) {
     if (!out) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
     if (n > 0xFFFFFFFFull) return frz_fail(FRZ_ERR_TOO_MANY_ITEMS, "too many items in haystack: %llu", (unsigned long long)n);
-    FRZ_TRY(ensure_device(device));
+    FRZ_TRY(frz_ensure_device(device));
     auto c = std::make_unique<frz_corpus>();
     c->st.device = device;
     frz_status s = frz_pack_corpus_device(d_bytes, d_offsets, 8, n, total_bytes, (cudaStream_t)stream, &c->st);
@@ -246,9 +259,9 @@ extern "C" frz_status frz_corpus_create_device(const uint8_t* d_bytes, const uin
 extern "C" frz_status frz_corpus_create_arrow(const uint8_t* bytes, const void* offsets, int offset_width, uint64_t n, int device,
                                               frz_corpus** out) {
     if (!out || !offsets) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
-    if (offset_width != 4 && offset_width != 8) return frz_fail(FRZ_ERR_INVALID_ARG, "offset_width must be 4 or 8");
+    FRZ_TRY(frz_check_offset_width(offset_width));
     if (n > 0xFFFFFFFFull) return frz_fail(FRZ_ERR_TOO_MANY_ITEMS, "too many items in haystack: %llu", (unsigned long long)n);
-    FRZ_TRY(ensure_device(device));
+    FRZ_TRY(frz_ensure_device(device));
     auto c = std::make_unique<frz_corpus>();
     c->st.device = device;
     FrzIngest ing;
@@ -269,9 +282,9 @@ extern "C" frz_status frz_corpus_create(const uint8_t* bytes, const uint64_t* of
 // call on the same corpus.
 extern "C" frz_status frz_corpus_append(frz_corpus* c, const uint8_t* bytes, const void* offsets, int offset_width, uint64_t n_new) {
     if (!c || (n_new && !offsets)) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
-    if (offset_width != 4 && offset_width != 8) return frz_fail(FRZ_ERR_INVALID_ARG, "offset_width must be 4 or 8");
+    FRZ_TRY(frz_check_offset_width(offset_width));
     if (n_new == 0) return FRZ_OK;
-    FRZ_TRY(ensure_device(c->st.device));
+    FRZ_TRY(frz_ensure_device(c->st.device));
     if (!c->ingest) c->ingest = std::make_unique<FrzIngest>();
     cudaStream_t stream = nullptr;
     FRZ_TRY(frz_append_host(*c->ingest, bytes, offsets, offset_width, n_new, stream, &c->st));
@@ -292,7 +305,7 @@ extern "C" frz_status frz_corpus_remove(frz_corpus* c, const uint32_t* which, ui
     if (!c || (n && !which)) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
     if (n == 0) return FRZ_OK;
     FRZ_TRY(check_indices(c, which, n));
-    FRZ_TRY(ensure_device(c->st.device));
+    FRZ_TRY(frz_ensure_device(c->st.device));
     if (!c->ingest) c->ingest = std::make_unique<FrzIngest>();
     return frz_remove_host(*c->ingest, which, n, nullptr, &c->st);
 }
@@ -310,7 +323,7 @@ static frz_status check_replacement_lengths(const OffT* off, uint64_t n) {
 extern "C" frz_status frz_corpus_replace(frz_corpus* c, const uint32_t* which, uint64_t n, const uint8_t* bytes, const void* offsets,
                                          int offset_width) {
     if (!c || (n && (!which || !offsets))) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
-    if (offset_width != 4 && offset_width != 8) return frz_fail(FRZ_ERR_INVALID_ARG, "offset_width must be 4 or 8");
+    FRZ_TRY(frz_check_offset_width(offset_width));
     if (n == 0) return FRZ_OK;
     FRZ_TRY(check_indices(c, which, n));
     std::vector<uint32_t> sorted(which, which + n);
@@ -322,7 +335,7 @@ extern "C" frz_status frz_corpus_replace(frz_corpus* c, const uint32_t* which, u
     const uint64_t r_bytes = offset_width == 4 ? (uint64_t)(static_cast<const uint32_t*>(offsets)[n] - static_cast<const uint32_t*>(offsets)[0])
                                                : static_cast<const uint64_t*>(offsets)[n] - static_cast<const uint64_t*>(offsets)[0];
     if (r_bytes && !bytes) return frz_fail(FRZ_ERR_INVALID_ARG, "null bytes");
-    FRZ_TRY(ensure_device(c->st.device));
+    FRZ_TRY(frz_ensure_device(c->st.device));
     if (!c->ingest) c->ingest = std::make_unique<FrzIngest>();
     if (!c->edit_tiles) c->edit_tiles = std::make_unique<FrzCorpusStorage>();
     const frz_status s = frz_replace_host(*c->ingest, *c->edit_tiles, which, n, bytes, offsets, offset_width, nullptr, &c->st);
@@ -381,7 +394,7 @@ extern "C" frz_status frz_corpus_debug_image(const frz_corpus* c, void* tile_bas
         if (sizes[i] != need[i])
             return frz_fail(FRZ_ERR_INVALID_ARG, "buffer %d holds %llu bytes, the image needs %llu", i, (unsigned long long)sizes[i],
                             (unsigned long long)need[i]);
-    FRZ_TRY(ensure_device(s.device));
+    FRZ_TRY(frz_ensure_device(s.device));
     for (int i = 0; i < 6; i++)
         if (need[i]) FRZ_CUDA_TRY(cudaMemcpy(dst[i], src[i], need[i], cudaMemcpyDeviceToHost));
     return FRZ_OK;
@@ -452,6 +465,29 @@ frz_status guard_against_score_overflow(const frz_scoring& s, size_t needle_len,
     return FRZ_OK;
 }
 
+// case_needle (src/prefilter/mod.rs:49-65): the byte a needle byte also matches, an ASCII letter in the other case unless
+// the match respects case
+uint8_t case_flip(uint8_t ch, bool case_sensitive) {
+    if (case_sensitive) return ch;
+    if (ch >= 'a' && ch <= 'z') return (uint8_t)(ch - 32);
+    if (ch >= 'A' && ch <= 'Z') return (uint8_t)(ch + 32);
+    return ch;
+}
+
+// The byte classes (frz_device.cuh: frz_sig_bucket) that hold one / two or more of the needle's bytes.  On the unicode
+// path only the needle's ASCII scalars count: a non-ASCII scalar and its case flip may differ in every byte, an ASCII
+// scalar is matched by the same letter in either case, which the classes fold.
+void sig_need_masks(const uint8_t* nd, size_t n, bool needs_unicode, FrzPatternDev* d) {
+    uint32_t cnt[32] = {0};
+    for (size_t i = 0; i < n; i++)
+        if (!needs_unicode || nd[i] < 0x80) cnt[frz_sig_bucket(nd[i])]++;
+    d->sig_need1 = d->sig_need2 = 0;
+    for (int b = 0; b < 32; b++) {
+        if (cnt[b] >= 1) d->sig_need1 |= 1u << b;
+        if (cnt[b] >= 2) d->sig_need2 |= 1u << b;
+    }
+}
+
 struct Compiled {
     FrzPatternDev dev;
     bool negated = false;
@@ -512,7 +548,7 @@ frz_status compile_pattern(const OwnedPattern& src, const frz_config& mcfg, bool
             const uint8_t ch = nd[i];
             c.un.c[i] = ch;
             c.un.f[i] = ch;
-            c.un.bflip[i] = case_sensitive ? ch : (ch >= 'a' && ch <= 'z') ? (uint8_t)(ch - 32) : (ch >= 'A' && ch <= 'Z') ? (uint8_t)(ch + 32) : ch;
+            c.un.bflip[i] = case_flip(ch, case_sensitive);
         }
     }
     d.n = (int)n;
@@ -520,12 +556,8 @@ frz_status compile_pattern(const OwnedPattern& src, const frz_config& mcfg, bool
     d.case_sensitive = case_sensitive;
     FrzNeedleTab tab;   // per-position data; FrzPatternDev keeps its first FRZ_MAX_NEEDLE positions
     memset(&tab, 0, sizeof tab);
-    for (size_t i = 0; i < n; i++) {  // case_needle (src/prefilter/mod.rs:49-65)
-        uint8_t ch = nd[i], fl;
-        if (case_sensitive) fl = ch;
-        else if (ch >= 'a' && ch <= 'z') fl = (uint8_t)(ch - 32);
-        else if (ch >= 'A' && ch <= 'Z') fl = (uint8_t)(ch + 32);
-        else fl = ch;
+    for (size_t i = 0; i < n; i++) {
+        const uint8_t ch = nd[i], fl = case_flip(ch, case_sensitive);
         tab.c[i] = ch; tab.flip[i] = fl;
         tab.om[i] = fl != ch ? 0x20 : 0;
         tab.tg[i] = fl != ch ? (uint8_t)(ch | 0x20) : ch;
@@ -568,19 +600,10 @@ frz_status compile_pattern(const OwnedPattern& src, const frz_config& mcfg, bool
         FRZ_TRY(guard_against_score_overflow(sc, n, sat_add16(maxb, sc.matching_case_bonus), 0));
         d.typo_mode = FRZ_T_LITERAL;
         d.min_hay_len = 0;
-        {   // a literal match holds every needle byte (either case): signature test with no typo budget
-            // (unicode path: only the needle's ASCII scalars count — a non-ASCII scalar and its case flip may differ in
-            // every byte, an ASCII scalar is matched by the same letter in either case, which the classes fold)
-            uint32_t cnt[32] = {0};
-            for (size_t i = 0; i < n; i++)
-                if (!needs_unicode || nd[i] < 0x80) cnt[frz_sig_bucket(nd[i])]++;
-            for (int b2 = 0; b2 < 32; b2++) {
-                if (cnt[b2] >= 1) d.sig_need1 |= 1u << b2;
-                if (cnt[b2] >= 2) d.sig_need2 |= 1u << b2;
-            }
-            d.sig_on = 1;
-            d.sig_k = 0;
-        }
+        // a literal match holds every needle byte (either case): signature test with no typo budget
+        sig_need_masks(nd, n, needs_unicode, &d);
+        d.sig_on = 1;
+        d.sig_k = 0;
         d.pf_lanes = 64; d.sw_lanes = 64; d.score_bits = 16;
         uint64_t b = (uint64_t)n * ((uint64_t)sc.match_score + sc.matching_case_bonus + maxb) + sc.prefix_bonus + sc.exact_match_bonus;
         c.score_bound = (uint32_t)std::min<uint64_t>(b, 0xFFFF);
@@ -659,16 +682,9 @@ frz_status compile_pattern(const OwnedPattern& src, const frz_config& mcfg, bool
         // k typos holds a common subsequence of n - k needle bytes (the k >= 1 trackers never accept what LCS rejects,
         // DESIGN.md §2), so per byte class at most k needle bytes in total may lack a partner:
         //     sum_c max(0, m_c - cnt_c) <= k     >=     popc(need1 & ~occurs) + popc(need2 & ~occurs_twice)
-        // The unicode trackers are the same trackers over needle SCALARS; there only the ASCII scalars are counted (see the
-        // literal branch above), which keeps the sum a lower bound.
-        uint32_t cnt[32] = {0};
-        for (size_t i = 0; i < n; i++)
-            if (!needs_unicode || nd[i] < 0x80) cnt[frz_sig_bucket(nd[i])]++;
-        d.sig_need1 = d.sig_need2 = 0;
-        for (int b2 = 0; b2 < 32; b2++) {
-            if (cnt[b2] >= 1) d.sig_need1 |= 1u << b2;
-            if (cnt[b2] >= 2) d.sig_need2 |= 1u << b2;
-        }
+        // The unicode trackers are the same trackers over needle SCALARS; there only the ASCII scalars are counted
+        // (sig_need_masks), which keeps the sum a lower bound.
+        sig_need_masks(nd, n, needs_unicode, &d);
         d.sig_on = max_typos >= 0 ? 1 : 0;                       // NO_PREFILTER scores everything
         d.sig_k = max_typos < 0 ? 0 : std::min<int>(max_typos, 64);
     }
@@ -867,16 +883,47 @@ __global__ void k_combine_hits(const FrzMatchDev* cand, uint64_t nc, FrzMatchDev
         hits[i] = h;
     }
 }
-// negated extra pattern: retain candidates that were NOT hit (src/matcher/multi.rs:124-132).
-// Stable compaction: per-block ballot counts → single-block scan → scatter.
+// haystack idx's slot is in use: it was not removed (frz_corpus_remove), and a subset call's masked metadata keeps it
+__device__ __forceinline__ bool slot_in_use(const uint32_t* __restrict__ slot_meta, const uint16_t* __restrict__ slot_of, uint64_t idx) {
+    return slot_meta[(idx & ~(uint64_t)(FRZ_TILE - 1)) + slot_of[idx]] != FRZ_INVALID_SLOT;
+}
+
+// Stable compaction of a list: per-block ballot counts (k_keep) → single-block scan → scatter.  The row rules of k_keep:
+// negated extra pattern: retain the candidates that were NOT hit (src/matcher/multi.rs:124-132)
+struct NotHit {
+    const FrzMatchDev* cand;
+    const FrzMatchDev* hits;
+    uint64_t nh;
+    __device__ bool operator()(uint64_t i) const { return find_hit(hits, nh, cand[i].index) < 0; }
+};
+// a k_fill_all list (row i = haystack i): retain the haystacks whose slot is in use
+struct LiveIndex {
+    const uint32_t* slot_meta;
+    const uint16_t* slot_of;
+    __device__ bool operator()(uint64_t i) const { return slot_in_use(slot_meta, slot_of, i); }
+};
+// the list form of a subset call: cand[i] = member i as a match record, retained when its slot is in use (removed members
+// are dropped: the candidate-list prefilter reads their slot metadata unchecked)
+struct LiveMember {
+    const uint32_t* members;
+    const uint32_t* slot_meta;
+    const uint16_t* slot_of;
+    FrzMatchDev* cand;
+    __device__ bool operator()(uint64_t i) const {
+        const uint32_t idx = members[i];
+        cand[i] = FrzMatchDev{idx, 0, 0, 0};
+        return slot_in_use(slot_meta, slot_of, idx);
+    }
+};
 constexpr int kCompactBlock = 1024;
-__global__ void __launch_bounds__(kCompactBlock) k_retain_count(const FrzMatchDev* cand, uint64_t nc, const FrzMatchDev* hits, uint64_t nh,
-                                                                uint32_t* block_count, uint8_t* keep) {
+// keep[i] = rule(i) for the n rows, and the kept rows of each block → block_count
+template <class Rule>
+__global__ void __launch_bounds__(kCompactBlock) k_keep(Rule rule, uint64_t n, uint32_t* block_count, uint8_t* keep) {
     __shared__ uint32_t wc[32];
-    uint64_t i = (uint64_t)blockIdx.x * kCompactBlock + threadIdx.x;
-    bool k = i < nc && find_hit(hits, nh, cand[i].index) < 0;
-    if (i < nc) keep[i] = k;
-    uint32_t b = __ballot_sync(0xffffffffu, k);
+    const uint64_t i = (uint64_t)blockIdx.x * kCompactBlock + threadIdx.x;
+    const bool k = i < n && rule(i);
+    if (i < n) keep[i] = k;
+    const uint32_t b = __ballot_sync(0xffffffffu, k);
     if ((threadIdx.x & 31) == 0) wc[threadIdx.x >> 5] = __popc(b);
     __syncthreads();
     if (threadIdx.x == 0) {
@@ -923,23 +970,6 @@ __global__ void __launch_bounds__(1024) k_scan_blocks(const uint32_t* cnt, uint6
     }
     if (threadIdx.x == 0) ctr->total = carry;
 }
-// keep[i] = haystack i was not removed (its slot metadata is not FRZ_INVALID_SLOT), with per-block counts as k_retain_count
-// writes them: the retain compaction then drops removed rows from a k_fill_all list
-__global__ void __launch_bounds__(kCompactBlock) k_live_keep(const uint32_t* __restrict__ slot_meta, const uint16_t* __restrict__ slot_of,
-                                                             uint64_t n, uint32_t* block_count, uint8_t* keep) {
-    __shared__ uint32_t wc[32];
-    const uint64_t i = (uint64_t)blockIdx.x * kCompactBlock + threadIdx.x;
-    const bool k = i < n && slot_meta[(i & ~(uint64_t)(FRZ_TILE - 1)) + slot_of[i]] != FRZ_INVALID_SLOT;
-    if (i < n) keep[i] = k;
-    const uint32_t b = __ballot_sync(0xffffffffu, k);
-    if ((threadIdx.x & 31) == 0) wc[threadIdx.x >> 5] = __popc(b);
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        uint32_t s = 0;
-        for (int w = 0; w < 32; w++) s += wc[w];
-        block_count[blockIdx.x] = s;
-    }
-}
 // Slot metadata of a subset call: slot s keeps its metadata when its haystack, index (s & ~1023) + (meta & 1023), is below
 // n_bits with its bit set in `bits`; every other slot becomes FRZ_INVALID_SLOT, which the matching kernels skip.  Four
 // slots of one tile per thread (n_slots is a multiple of FRZ_TILE).
@@ -955,30 +985,6 @@ __global__ void k_subset_meta(const uint4* __restrict__ slot_meta, uint64_t n_qu
             if (v[j] == FRZ_INVALID_SLOT || idx >= n_bits || !((bits[idx >> 5] >> (idx & 31)) & 1u)) v[j] = FRZ_INVALID_SLOT;
         }
         out[q] = *reinterpret_cast<const uint4*>(v);
-    }
-}
-// The list form of a subset call: cand[j] = member j as a match record, keep[j] = its slot is in use (removed members are
-// dropped: the candidate-list prefilter reads their slot metadata unchecked), with per-block counts as k_retain_count
-// writes them for the retain compaction.
-__global__ void __launch_bounds__(kCompactBlock) k_member_keep(const uint32_t* __restrict__ members, uint64_t n,
-                                                               const uint32_t* __restrict__ slot_meta, const uint16_t* __restrict__ slot_of,
-                                                               uint32_t* block_count, uint8_t* keep, FrzMatchDev* cand) {
-    __shared__ uint32_t wc[32];
-    const uint64_t i = (uint64_t)blockIdx.x * kCompactBlock + threadIdx.x;
-    bool k = false;
-    if (i < n) {
-        const uint32_t idx = members[i];
-        k = slot_meta[(idx & ~(uint32_t)(FRZ_TILE - 1)) + slot_of[idx]] != FRZ_INVALID_SLOT;
-        keep[i] = k;
-        cand[i] = FrzMatchDev{idx, 0, 0, 0};
-    }
-    const uint32_t b = __ballot_sync(0xffffffffu, k);
-    if ((threadIdx.x & 31) == 0) wc[threadIdx.x >> 5] = __popc(b);
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        uint32_t s = 0;
-        for (int w = 0; w < 32; w++) s += wc[w];
-        block_count[blockIdx.x] = s;
     }
 }
 
@@ -1014,7 +1020,7 @@ frz_status ensure_multi_buffers(frz_matcher* m, uint64_t n) {
     return m->ws.multi_b.reserve(std::max<uint64_t>(n, 1));
 }
 
-// stable-compaction scratch (k_retain_count / k_live_keep → k_scan_blocks → k_retain_scatter) for lists of up to n entries
+// stable-compaction scratch (k_keep → k_scan_blocks → k_retain_scatter) for lists of up to n entries
 frz_status ensure_retain_buffers(frz_matcher* m, uint64_t n) {
     FrzWorkspace& ws = m->ws;
     if (ws.retain_keep.cap() >= n) return FRZ_OK;
@@ -1022,6 +1028,22 @@ frz_status ensure_retain_buffers(frz_matcher* m, uint64_t n) {
     FRZ_TRY(ws.retain_cnt.reserve(nb_max));
     FRZ_TRY(ws.retain_base.reserve(nb_max));
     return ws.retain_keep.reserve(n);
+}
+
+// Stable compaction of the n >= 1 rows of `in`: the rows that `rule` keeps → `out`, in order, their count →
+// ws.counters->total.
+template <class Rule>
+frz_status retain_rows(frz_matcher* m, Rule rule, const FrzMatchDev* in, uint64_t n, FrzMatchDev* out, cudaStream_t stream,
+                       FrzLaunchStats* st) {
+    FrzWorkspace& ws = m->ws;
+    FRZ_TRY(ensure_retain_buffers(m, n));
+    const uint32_t nb = (uint32_t)((n + kCompactBlock - 1) / kCompactBlock);
+    k_keep<<<nb, kCompactBlock, 0, stream>>>(rule, n, ws.retain_cnt.get(), ws.retain_keep.get());
+    k_scan_blocks<<<1, 1024, 0, stream>>>(ws.retain_cnt.get(), ws.retain_base.get(), nb, ws.counters.get());
+    k_retain_scatter<<<nb, kCompactBlock, 0, stream>>>(in, n, ws.retain_keep.get(), ws.retain_base.get(), out);
+    st->launches += 3;
+    FRZ_CUDA_TRY(cudaGetLastError());
+    return FRZ_OK;
 }
 
 uint64_t initial_survivor_cap(const FrzCorpusStorage& cs, const FrzPatternDev& d) {
@@ -1054,6 +1076,47 @@ frz_status needle_table(frz_matcher* m, const Compiled& c, const FrzNeedleTab** 
     return FRZ_OK;
 }
 
+// timing event i of the current call (FrzWorkspace::ev)
+void record_ev(FrzWorkspace& ws, int i, cudaStream_t stream) {
+    cudaEventRecord(ws.ev[i].get(), stream);
+    ws.ev_rec[i] = true;
+}
+
+// the start of a match call: no timing event recorded yet, no single-pass sort table
+void reset_call_state(frz_matcher* m) {
+    for (bool& f : m->ws.ev_rec) f = false;
+    m->last_sort_bins = 0;
+}
+
+// shard calls: ws.counters->total → *dst, then count_ev
+frz_status publish_count(frz_matcher* m, uint64_t* dst, cudaStream_t stream) {
+    FRZ_CUDA_TRY(cudaMemcpyAsync(dst, &m->ws.counters.get()->total, sizeof(uint64_t), cudaMemcpyDeviceToDevice, stream));
+    FRZ_CUDA_TRY(cudaEventRecord(m->count_ev.get(), stream));
+    m->count_published = true;
+    return FRZ_OK;
+}
+
+// An asynchronous shard call: body(&st) enqueues the call's work on `stream`.  Meanwhile the count goes to d_count as soon
+// as it is known (the body publishes it early where it can, else it is published after the body) and the score sort
+// records its table event.  frz_matcher_last_timings reads the events once the stream is idle.
+template <class Body>
+frz_status shard_call(frz_matcher* m, uint64_t* d_count, cudaStream_t stream, Body&& body) {
+    if (!m->count_ev) FRZ_TRY(frz_event_create(m->count_ev, cudaEventDisableTiming));
+    FrzLaunchStats st;
+    m->early_count_dst = d_count;
+    m->count_published = false;
+    m->ws.sort.arm_table_ev = true;
+    m->ws.sort.table_ev_recorded = false;
+    const frz_status s = body(&st);
+    m->early_count_dst = nullptr;
+    m->ws.sort.arm_table_ev = false;
+    FRZ_TRY(s);
+    if (!m->count_published) FRZ_TRY(publish_count(m, d_count, stream));
+    m->last_launches = st.launches;
+    m->timings_pending = true;
+    return FRZ_OK;
+}
+
 // One pattern over the corpus (optionally restricted to a candidate list) → index-ordered matches in d_out (reversed
 // order if `reversed`); the count is left in ws.counters->total (device).  masked_meta (subset calls): slot metadata to
 // read in place of the corpus's own, nullptr = the corpus's.
@@ -1069,18 +1132,14 @@ frz_status run_pattern(frz_matcher* m, const FrzCorpusStorage& cs, const Compile
     const FrzNeedleTab* ntab = nullptr;
     FRZ_TRY(needle_table(m, c, &ntab));
     FRZ_CUDA_TRY(cudaMemsetAsync(ws.counters.get(), 0, sizeof(FrzCounters), stream));
-    if (record_events) { cudaEventRecord(ws.ev[0].get(), stream); ws.ev_rec[0] = true; }
+    if (record_events) record_ev(ws, 0, stream);
     if (c.unicode) FRZ_TRY(frz_launch_unicode(cv, c.dev, c.un, c.usc, cand_list, n_cand, index_offset, ws, stream, st));
     else if (cand_list) FRZ_TRY(frz_launch_prefilter_list(cv, c.dev, cand_list, n_cand, index_offset, ws, stream, st, ntab));
     else FRZ_TRY(frz_launch_prefilter(cv, c.dev, ws, stream, st, ntab));
     FRZ_TRY(frz_launch_tile_scan(cv, ws, stream, st));
-    if (record_events) { cudaEventRecord(ws.ev[1].get(), stream); ws.ev_rec[1] = true; }
-    if (m->early_count_dst && !cand_list && m->compiled.size() == 1) {
-        // single pattern: every survivor becomes exactly one match, so the scan total is the final count
-        FRZ_CUDA_TRY(cudaMemcpyAsync(m->early_count_dst, &ws.counters.get()->total, sizeof(uint64_t), cudaMemcpyDeviceToDevice, stream));
-        FRZ_CUDA_TRY(cudaEventRecord(m->count_ev.get(), stream));
-        m->count_published = true;
-    }
+    if (record_events) record_ev(ws, 1, stream);
+    // single pattern: every survivor becomes exactly one match, so the scan total is the final count
+    if (m->early_count_dst && !cand_list && m->compiled.size() == 1) FRZ_TRY(publish_count(m, m->early_count_dst, stream));
     // A survivor-list overflow (lists are sized by a heuristic unless the pattern can match everything)
     // only sets a sticky device flag; whoever reads the counters back re-runs with worst-case lists.
     if (c.unicode) {
@@ -1091,7 +1150,7 @@ frz_status run_pattern(frz_matcher* m, const FrzCorpusStorage& cs, const Compile
     } else {
         FRZ_TRY(frz_launch_sw(cv, c.dev, index_offset, reversed, ws, d_out, stream, st, hist, ntab));
     }
-    if (record_events) { cudaEventRecord(ws.ev[2].get(), stream); ws.ev_rec[2] = true; }
+    if (record_events) record_ev(ws, 2, stream);
     return FRZ_OK;
 }
 
@@ -1119,35 +1178,35 @@ frz_status fill_all(frz_matcher* m, const FrzCorpusStorage& cs, uint32_t index_o
     const bool filter = cs.n_removed || masked_meta;
     k_fill_all<<<grid_for(cs.n, 256), 256, 0, stream>>>(filter ? tmp : out, cs.n, index_offset, ws.counters.get());
     st->launches++;
-    if (filter && cs.n) {
-        FRZ_TRY(ensure_retain_buffers(m, cs.n));
-        const uint32_t nb = (uint32_t)((cs.n + kCompactBlock - 1) / kCompactBlock);
-        k_live_keep<<<nb, kCompactBlock, 0, stream>>>(masked_meta ? masked_meta : cs.slot_meta.get(), cs.slot_of.get(), cs.n,
-                                                      ws.retain_cnt.get(), ws.retain_keep.get());
-        k_scan_blocks<<<1, 1024, 0, stream>>>(ws.retain_cnt.get(), ws.retain_base.get(), nb, ws.counters.get());
-        k_retain_scatter<<<nb, kCompactBlock, 0, stream>>>(tmp, cs.n, ws.retain_keep.get(), ws.retain_base.get(), out);
-        st->launches += 3;
-    }
+    if (filter && cs.n)
+        FRZ_TRY(retain_rows(m, LiveIndex{masked_meta ? masked_meta : cs.slot_meta.get(), cs.slot_of.get()}, tmp, cs.n, out, stream, st));
     FRZ_CUDA_TRY(cudaGetLastError());
     return FRZ_OK;
 }
 
 // The rows of a subset call, in one of two forms (DESIGN.md §4.9): slot metadata in which non-members are unused slots
 // (masked form), or the live members, index-ordered, as a candidate list (list form).  The default scope is the whole
-// corpus.
+// corpus.  none: no row can match (the list form found no member in use), the call returns an empty list without running
+// the pipeline.
 struct SubsetScope {
     const uint32_t* masked_meta = nullptr;
     const FrzMatchDev* list = nullptr;
     uint64_t n_list = 0;
+    bool none = false;
 };
+
+// a count known on the host → ws.counters->total
+frz_status set_count(frz_matcher* m, uint64_t n, cudaStream_t stream) {
+    FrzWorkspace& ws = m->ws;
+    ws.h_counters.get()->total = n;
+    FRZ_CUDA_TRY(cudaMemcpyAsync(&ws.counters.get()->total, &ws.h_counters.get()->total, sizeof(unsigned long long), cudaMemcpyHostToDevice, stream));
+    return FRZ_OK;
+}
 
 // the list form's members → `out` as the start of a list, count → ws.counters->total
 frz_status copy_scope_list(frz_matcher* m, const SubsetScope& scope, FrzMatchDev* out, cudaStream_t stream) {
-    FrzWorkspace& ws = m->ws;
     FRZ_CUDA_TRY(cudaMemcpyAsync(out, scope.list, scope.n_list * sizeof(FrzMatchDev), cudaMemcpyDeviceToDevice, stream));
-    ws.h_counters.get()->total = scope.n_list;
-    FRZ_CUDA_TRY(cudaMemcpyAsync(&ws.counters.get()->total, &ws.h_counters.get()->total, sizeof(unsigned long long), cudaMemcpyHostToDevice, stream));
-    return FRZ_OK;
+    return set_count(m, scope.n_list, stream);
 }
 
 // match_list_into over all compiled patterns → index-ordered device list; returns pointer + leaves the
@@ -1162,9 +1221,7 @@ frz_status match_into_device(frz_matcher* m, const FrzCorpusStorage& cs, uint32_
                              const SubsetScope& scope = SubsetScope()) {
     FrzWorkspace& ws = m->ws;
     const uint32_t* masked_meta = scope.masked_meta;
-    if ((uint64_t)cs.n + index_offset > 0xFFFFFFFFull)
-        return frz_fail(FRZ_ERR_TOO_MANY_ITEMS, "too many items in haystack, will overflow the u32 index: %llu > %u (index offset: %u)",
-                        (unsigned long long)cs.n + index_offset, 0xFFFFFFFFu, index_offset);
+    FRZ_TRY(frz_check_index_range(cs.n, index_offset));
     const auto& pats = m->compiled;
     *score_bound = 0;
     if (pats.empty()) {  // CompiledPatterns::Empty (src/matcher/mod.rs:380-383)
@@ -1219,10 +1276,7 @@ frz_status match_into_device(frz_matcher* m, const FrzCorpusStorage& cs, uint32_
             nc = ws.h_counters.get()->total;
         } else nc = cs.n - cs.n_removed;
     }
-    FRZ_TRY(ensure_retain_buffers(m, cs.n));
-    uint32_t* d_block_cnt = ws.retain_cnt.get();
-    uint64_t* d_block_base = ws.retain_base.get();
-    uint8_t* d_keep = ws.retain_keep.get();
+    FRZ_TRY(ensure_retain_buffers(m, cs.n));   // once, for every negated pattern below
     frz_status status = FRZ_OK;
     for (size_t pi = 0; pi < pats.size() && status == FRZ_OK; pi++) {
         if ((int)pi == base || nc == 0) continue;
@@ -1233,11 +1287,7 @@ frz_status match_into_device(frz_matcher* m, const FrzCorpusStorage& cs, uint32_
             FRZ_TRY(read_counters(m, stream));
             const uint64_t nh = ws.h_counters.get()->total;
             if (pats[pi].negated) {
-                const uint32_t nb = (uint32_t)((nc + kCompactBlock - 1) / kCompactBlock);
-                k_retain_count<<<nb, kCompactBlock, 0, stream>>>(cand, nc, ws.matches_a.get(), nh, d_block_cnt, d_keep);
-                k_scan_blocks<<<1, 1024, 0, stream>>>(d_block_cnt, d_block_base, nb, ws.counters.get());
-                k_retain_scatter<<<nb, kCompactBlock, 0, stream>>>(cand, nc, d_keep, d_block_base, spare);
-                st->launches += 3;
+                FRZ_TRY(retain_rows(m, NotHit{cand, ws.matches_a.get(), nh}, cand, nc, spare, stream, st));
                 FRZ_TRY(read_counters(m, stream));
                 nc = ws.h_counters.get()->total;
                 std::swap(cand, spare);
@@ -1254,8 +1304,7 @@ frz_status match_into_device(frz_matcher* m, const FrzCorpusStorage& cs, uint32_
     }
     FRZ_TRY(status);
     // publish: count → counters.total, list → matches_a (reversed if asked)
-    ws.h_counters.get()->total = nc;
-    FRZ_CUDA_TRY(cudaMemcpyAsync(&ws.counters.get()->total, &ws.h_counters.get()->total, sizeof(unsigned long long), cudaMemcpyHostToDevice, stream));
+    FRZ_TRY(set_count(m, nc, stream));
     if (final_reversed) {
         k_reverse<<<grid_for(nc, 256), 256, 0, stream>>>(cand, ws.matches_a.get(), &ws.counters.get()->total);
         st->launches++;
@@ -1286,8 +1335,7 @@ frz_status match_list_device(frz_matcher* m, const FrzCorpusStorage& cs, uint32_
     const bool reversed = sort == FRZ_SORT_INDEX_DESC || sort == FRZ_SORT_SCORE_THEN_INDEX_DESC;
     const bool by_score = sort == FRZ_SORT_SCORE_THEN_INDEX_ASC || sort == FRZ_SORT_SCORE_THEN_INDEX_DESC;
     const bool will_sort = by_score && !m->compiled.empty();
-    for (bool& f : ws.ev_rec) f = false;
-    m->last_sort_bins = 0;
+    reset_call_state(m);
     FrzMatchDev* d_list = nullptr;
     uint32_t bound = 0;
     FrzScoreHist hist;
@@ -1312,8 +1360,7 @@ frz_status match_list_device(frz_matcher* m, const FrzCorpusStorage& cs, uint32_
         st->launches++;
         d_list = final_out;
     }
-    cudaEventRecord(ws.ev[3].get(), stream);
-    ws.ev_rec[3] = true;
+    record_ev(ws, 3, stream);
     *d_result = d_list;
     return FRZ_OK;
 }
@@ -1333,10 +1380,15 @@ void collect_timings(frz_matcher* m, const FrzLaunchStats& st) {
 }
 namespace {
 
-frz_status copy_out(frz_matcher* m, FrzMatchDev* d_list, frz_match* out, uint64_t cap, uint64_t* n_out, cudaStream_t stream) {
+// The first min(limit, total) matches of d_list → host (a top-K call passes cap = limit, so it never fails on capacity);
+// *n_out = their number, *n_total = all matches.
+frz_status copy_out(frz_matcher* m, FrzMatchDev* d_list, uint64_t limit, frz_match* out, uint64_t cap, uint64_t* n_out,
+                    uint64_t* n_total, cudaStream_t stream) {
     FRZ_TRY(read_counters(m, stream));
-    const uint64_t n = m->ws.h_counters.get()->total;
+    const uint64_t total = m->ws.h_counters.get()->total;
+    const uint64_t n = std::min(limit, total);
     if (n_out) *n_out = n;
+    if (n_total) *n_total = total;
     if (n > cap) return frz_fail(FRZ_ERR_CAPACITY, "output capacity %llu < %llu matches", (unsigned long long)cap, (unsigned long long)n);
     if (n) {
         if (!out) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
@@ -1347,50 +1399,24 @@ frz_status copy_out(frz_matcher* m, FrzMatchDev* d_list, frz_match* out, uint64_
     return FRZ_OK;
 }
 
-// top-K: the first min(k, total) matches → host; never a capacity error
-frz_status copy_out_top(frz_matcher* m, FrzMatchDev* d_list, uint64_t k, frz_match* out, uint64_t* n_out, uint64_t* n_total,
-                        cudaStream_t stream) {
-    FRZ_TRY(read_counters(m, stream));
-    const uint64_t total = m->ws.h_counters.get()->total;
-    const uint64_t n = std::min(k, total);
-    if (n_out) *n_out = n;
-    if (n_total) *n_total = total;
-    if (n) {
-        FRZ_CUDA_TRY(cudaMemcpyAsync(out, d_list, n * sizeof(frz_match), cudaMemcpyDeviceToHost, stream));
-        FRZ_CUDA_TRY(cudaStreamSynchronize(stream));
+// Matcher::match_list (into, from index_offset, in `sort` order) → host, truncated to its first `limit` rows (top-K calls:
+// the same pipeline with a limit on the final scatter and copy; UINT64_MAX for the whole list).  scope: the rows of a subset
+// call (match_into_device).
+frz_status match_list_host(frz_matcher* m, const frz_corpus* corpus, uint32_t index_offset, uint8_t sort, uint64_t limit,
+                           const SubsetScope& scope, frz_match* out, uint64_t cap, uint64_t* n_out, uint64_t* n_total) {
+    if (scope.none) {
+        if (n_out) *n_out = 0;
+        if (n_total) *n_total = 0;
+        return FRZ_OK;
     }
-    return FRZ_OK;
-}
-
-// Matcher::match_list → host.  scope: the rows of a subset call (match_into_device).
-frz_status match_list_host_out(frz_matcher* m, const frz_corpus* corpus, const SubsetScope& scope, frz_match* out, uint64_t cap,
-                               uint64_t* n_out) {
     cudaStream_t stream = nullptr;
     FrzLaunchStats st;
     FrzMatchDev* d_list = nullptr;
+    const uint32_t dev_limit = (uint32_t)std::min<uint64_t>(limit, kFrzNoLimit);   // a list never holds more than 2^32 - 1 matches
     frz_status s = FRZ_OK;
     for (int attempt = 0; attempt < 2; attempt++) {
-        s = match_list_device(m, corpus->st, 0, m->config.sort, &d_list, stream, &st, nullptr, kFrzNoLimit, scope);
-        if (s == FRZ_OK) s = copy_out(m, d_list, out, cap, n_out, stream);
-        if (s != kRetryOverflow) break;
-        FRZ_TRY(ensure_workspace(m, corpus->st, std::max<uint64_t>(corpus->st.n, 1)));  // worst-case lists, then once more
-    }
-    if (s == kRetryOverflow) s = frz_fail(FRZ_ERR_CUDA, "survivor list overflow persisted");
-    collect_timings(m, st);
-    return s;
-}
-
-// Matcher::match_list followed by truncation to the first k rows: the same pipeline with a limit on the final scatter and copy
-frz_status match_list_top_host_out(frz_matcher* m, const frz_corpus* corpus, const SubsetScope& scope, uint64_t k, frz_match* out,
-                                   uint64_t* n_out, uint64_t* n_total) {
-    cudaStream_t stream = nullptr;
-    FrzLaunchStats st;
-    FrzMatchDev* d_list = nullptr;
-    const uint32_t limit = (uint32_t)std::min<uint64_t>(k, kFrzNoLimit);   // a list never holds more than 2^32 - 1 matches
-    frz_status s = FRZ_OK;
-    for (int attempt = 0; attempt < 2; attempt++) {
-        s = match_list_device(m, corpus->st, 0, m->config.sort, &d_list, stream, &st, nullptr, limit, scope);
-        if (s == FRZ_OK) s = copy_out_top(m, d_list, k, out, n_out, n_total, stream);
+        s = match_list_device(m, corpus->st, index_offset, sort, &d_list, stream, &st, nullptr, dev_limit, scope);
+        if (s == FRZ_OK) s = copy_out(m, d_list, limit, out, cap, n_out, n_total, stream);
         if (s != kRetryOverflow) break;
         FRZ_TRY(ensure_workspace(m, corpus->st, std::max<uint64_t>(corpus->st.n, 1)));  // worst-case lists, then once more
     }
@@ -1403,16 +1429,16 @@ frz_status match_list_top_host_out(frz_matcher* m, const frz_corpus* corpus, con
 
 extern "C" frz_status frz_match_list(frz_matcher* m, const frz_corpus* corpus, frz_match* out, uint64_t cap, uint64_t* n_out) {
     if (!m || !corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
-    FRZ_TRY(ensure_device(corpus->st.device));
-    return match_list_host_out(m, corpus, SubsetScope(), out, cap, n_out);
+    FRZ_TRY(frz_ensure_device(corpus->st.device));
+    return match_list_host(m, corpus, 0, m->config.sort, UINT64_MAX, SubsetScope(), out, cap, n_out, nullptr);
 }
 
 extern "C" frz_status frz_match_list_top(frz_matcher* m, const frz_corpus* corpus, uint64_t k, frz_match* out, uint64_t* n_out,
                                          uint64_t* n_total) {
     if (!m || !corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
     if (!out && k > 0) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
-    FRZ_TRY(ensure_device(corpus->st.device));
-    return match_list_top_host_out(m, corpus, SubsetScope(), k, out, n_out, n_total);
+    FRZ_TRY(frz_ensure_device(corpus->st.device));
+    return match_list_host(m, corpus, 0, m->config.sort, k, SubsetScope(), out, k, n_out, n_total);
 }
 
 // ---------------------------------------------------------------------------------- subsets
@@ -1439,7 +1465,7 @@ extern "C" frz_status frz_subset_create(const frz_corpus* c, const uint32_t* whi
         for (uint32_t x = bits[w]; x; x &= x - 1) members.push_back((uint32_t)(w * 32 + __builtin_ctz(x)));
     s->n_members = members.size();
     if (!bits.empty()) {
-        FRZ_TRY(ensure_device(c->st.device));
+        FRZ_TRY(frz_ensure_device(c->st.device));
         FRZ_TRY(s->bits.reserve(bits.size()));
         FRZ_CUDA_TRY(cudaMemcpy(s->bits.get(), bits.data(), bits.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
     }
@@ -1464,40 +1490,32 @@ namespace {
 frz_status check_subset_call(const frz_matcher* m, const frz_corpus* corpus, const frz_subset* s) {
     if (!m || !corpus || !s) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
     if (s->corpus != corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "the subset was made on another corpus");
-    return ensure_device(corpus->st.device);
+    return frz_ensure_device(corpus->st.device);
 }
 
 // The rows of a subset call, built in the matcher's workspace on every call, so edits of the corpus between calls need no
 // bookkeeping.  Masked form: the corpus's slot metadata with every non-member an unused slot.  List form: the members
-// whose slots are in use, index-ordered.  *none: no row can match (the list form found no member in use), the caller
-// returns an empty list without running the pipeline.  An empty corpus keeps the default scope: it has no row.
-frz_status subset_scope(frz_matcher* m, const frz_corpus* corpus, const frz_subset& s, cudaStream_t stream, SubsetScope* out,
-                        bool* none) {
+// whose slots are in use, index-ordered.  An empty corpus keeps the default scope: it has no row.
+frz_status subset_scope(frz_matcher* m, const frz_corpus* corpus, const frz_subset& s, cudaStream_t stream, SubsetScope* out) {
     const FrzCorpusStorage& cs = corpus->st;
     *out = SubsetScope();
-    *none = false;
     if (cs.n == 0) return FRZ_OK;
     FrzWorkspace& ws = m->ws;
     FRZ_TRY(ensure_workspace(m, cs, 0));   // (on this device; the lists are sized by the match call)
     constexpr int kListPermille = FRZ_SUBSET_LIST_PERMILLE;
     if (kListPermille >= 0 && s.n_members * 1000 <= cs.n * (uint64_t)std::max(kListPermille, 0)) {
         const uint64_t n = s.n_members;
-        if (n == 0) { *none = true; return FRZ_OK; }
+        if (n == 0) { out->none = true; return FRZ_OK; }
         FRZ_TRY(ws.subset_list.reserve(2 * n));
-        FRZ_TRY(ensure_retain_buffers(m, n));
         FrzMatchDev* tmp = ws.subset_list.get();
         FrzMatchDev* list = tmp + n;
-        const uint32_t nb = (uint32_t)((n + kCompactBlock - 1) / kCompactBlock);
         FRZ_CUDA_TRY(cudaMemsetAsync(ws.counters.get(), 0, sizeof(FrzCounters), stream));
-        k_member_keep<<<nb, kCompactBlock, 0, stream>>>(s.members.get(), n, cs.slot_meta.get(), cs.slot_of.get(), ws.retain_cnt.get(),
-                                                        ws.retain_keep.get(), tmp);
-        k_scan_blocks<<<1, 1024, 0, stream>>>(ws.retain_cnt.get(), ws.retain_base.get(), nb, ws.counters.get());
-        k_retain_scatter<<<nb, kCompactBlock, 0, stream>>>(tmp, n, ws.retain_keep.get(), ws.retain_base.get(), list);
-        FRZ_CUDA_TRY(cudaGetLastError());
+        FrzLaunchStats uncounted;   // (the launches of a call are those of its pipeline)
+        FRZ_TRY(retain_rows(m, LiveMember{s.members.get(), cs.slot_meta.get(), cs.slot_of.get(), tmp}, tmp, n, list, stream, &uncounted));
         FRZ_TRY(read_counters(m, stream));
         out->list = list;
         out->n_list = ws.h_counters.get()->total;
-        *none = out->n_list == 0;
+        out->none = out->n_list == 0;
         return FRZ_OK;
     }
     const uint64_t n_slots = (uint64_t)cs.n_tiles * FRZ_TILE;
@@ -1514,13 +1532,8 @@ extern "C" frz_status frz_match_list_subset(frz_matcher* m, const frz_corpus* co
                                             uint64_t* n_out) {
     FRZ_TRY(check_subset_call(m, corpus, s));
     SubsetScope scope;
-    bool none = false;
-    FRZ_TRY(subset_scope(m, corpus, *s, nullptr, &scope, &none));
-    if (none) {
-        if (n_out) *n_out = 0;
-        return FRZ_OK;
-    }
-    return match_list_host_out(m, corpus, scope, out, cap, n_out);
+    FRZ_TRY(subset_scope(m, corpus, *s, nullptr, &scope));
+    return match_list_host(m, corpus, 0, m->config.sort, UINT64_MAX, scope, out, cap, n_out, nullptr);
 }
 
 extern "C" frz_status frz_match_list_subset_top(frz_matcher* m, const frz_corpus* corpus, const frz_subset* s, uint64_t k, frz_match* out,
@@ -1528,33 +1541,15 @@ extern "C" frz_status frz_match_list_subset_top(frz_matcher* m, const frz_corpus
     FRZ_TRY(check_subset_call(m, corpus, s));
     if (!out && k > 0) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
     SubsetScope scope;
-    bool none = false;
-    FRZ_TRY(subset_scope(m, corpus, *s, nullptr, &scope, &none));
-    if (none) {
-        if (n_out) *n_out = 0;
-        if (n_total) *n_total = 0;
-        return FRZ_OK;
-    }
-    return match_list_top_host_out(m, corpus, scope, k, out, n_out, n_total);
+    FRZ_TRY(subset_scope(m, corpus, *s, nullptr, &scope));
+    return match_list_host(m, corpus, 0, m->config.sort, k, scope, out, k, n_out, n_total);
 }
 
 extern "C" frz_status frz_match_list_into(frz_matcher* m, const frz_corpus* corpus, uint32_t index_offset, frz_match* out,
                                           uint64_t cap, uint64_t* n_out) {
     if (!m || !corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
-    FRZ_TRY(ensure_device(corpus->st.device));
-    cudaStream_t stream = nullptr;
-    FrzLaunchStats st;
-    FrzMatchDev* d_list = nullptr;
-    frz_status s = FRZ_OK;
-    for (int attempt = 0; attempt < 2; attempt++) {
-        s = match_list_device(m, corpus->st, index_offset, FRZ_SORT_INDEX_ASC, &d_list, stream, &st);
-        if (s == FRZ_OK) s = copy_out(m, d_list, out, cap, n_out, stream);
-        if (s != kRetryOverflow) break;
-        FRZ_TRY(ensure_workspace(m, corpus->st, std::max<uint64_t>(corpus->st.n, 1)));
-    }
-    if (s == kRetryOverflow) s = frz_fail(FRZ_ERR_CUDA, "survivor list overflow persisted");
-    collect_timings(m, st);
-    return s;
+    FRZ_TRY(frz_ensure_device(corpus->st.device));
+    return match_list_host(m, corpus, index_offset, FRZ_SORT_INDEX_ASC, UINT64_MAX, SubsetScope(), out, cap, n_out, nullptr);
 }
 
 namespace {   // defined with the shard calls below
@@ -1567,12 +1562,12 @@ frz_status match_streamed_impl(frz_matcher* m, const uint8_t* bytes, const void*
 extern "C" frz_status frz_match_list_host_arrow(frz_matcher* m, const uint8_t* bytes, const void* offsets, int offset_width, uint64_t n,
                                                 int device, frz_match* out, uint64_t cap, uint64_t* n_out) {
     if (!m || !offsets) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
-    if (offset_width != 4 && offset_width != 8) return frz_fail(FRZ_ERR_INVALID_ARG, "offset_width must be 4 or 8");
+    FRZ_TRY(frz_check_offset_width(offset_width));
     if (n > 0xFFFFFFFFull) return frz_fail(FRZ_ERR_TOO_MANY_ITEMS, "too many items in haystack: %llu", (unsigned long long)n);
     if (streamed_eligible(m, n, 0)) {   // the match pipeline runs while the list streams in (frz_match_shard_streamed)
         FrzMatchDev* d_list = nullptr;
         FRZ_TRY(match_streamed_impl(m, bytes, offsets, offset_width, n, device, 0, nullptr, nullptr, nullptr, &d_list));
-        const frz_status s = copy_out(m, d_list, out, cap, n_out, nullptr);
+        const frz_status s = copy_out(m, d_list, UINT64_MAX, out, cap, n_out, nullptr, nullptr);
         m->timings_pending = false;
         FrzLaunchStats st; st.launches = m->last_launches;
         collect_timings(m, st);
@@ -1600,9 +1595,9 @@ frz_corpus& e2e_corpus_on(frz_matcher* m, int device) {
 frz_status frz_matcher_ingest_e2e(frz_matcher* m, const uint8_t* bytes, const void* offsets, int offset_width, uint64_t n, int device,
                                   const frz_corpus** out) {
     if (!m || !offsets || !out) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
-    if (offset_width != 4 && offset_width != 8) return frz_fail(FRZ_ERR_INVALID_ARG, "offset_width must be 4 or 8");
+    FRZ_TRY(frz_check_offset_width(offset_width));
     if (n > 0xFFFFFFFFull) return frz_fail(FRZ_ERR_TOO_MANY_ITEMS, "too many items in haystack: %llu", (unsigned long long)n);
-    FRZ_TRY(ensure_device(device));
+    FRZ_TRY(frz_ensure_device(device));
     cudaStream_t stream = nullptr;
     frz_corpus& c = e2e_corpus_on(m, device);
     FRZ_TRY(frz_ingest_host(m->e2e_ingest, bytes, offsets, offset_width, n, stream, &c.st));
@@ -1647,7 +1642,7 @@ __global__ void k_rows_removed(const uint32_t* __restrict__ slot_meta, const uin
                                uint64_t n, uint64_t corpus_n, uint8_t* __restrict__ removed) {
     for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) {
         const uint64_t idx = which[j];
-        removed[j] = idx < corpus_n && slot_meta[(idx & ~(uint64_t)(FRZ_TILE - 1)) + slot_of[idx]] == FRZ_INVALID_SLOT;
+        removed[j] = idx < corpus_n && !slot_in_use(slot_meta, slot_of, idx);
     }
 }
 
@@ -1677,7 +1672,7 @@ extern "C" frz_status frz_match_indices(frz_matcher* m, const frz_corpus* corpus
         if (c.is_long())
             return frz_fail(FRZ_ERR_UNSUPPORTED, "match_indices handles needles of up to %d bytes (this one has %d)", FRZ_MAX_NEEDLE, c.dev.n);
     if (n == 0) return FRZ_OK;
-    FRZ_TRY(ensure_device(corpus->st.device));
+    FRZ_TRY(frz_ensure_device(corpus->st.device));
     if (m->compiled.size() == 1 && !m->compiled[0].negated)   // CompiledPatterns::Single
         return match_indices_one(m->compiled[0], corpus, which, n, out_matches, out_indices, stride, out_counts);
     // CompiledPatterns::Multi → match_one_indices_multi (src/matcher/multi.rs:56-79): a negated atom that matches drops the
@@ -1729,31 +1724,18 @@ extern "C" frz_status frz_match_shard_device(frz_matcher* m, const frz_corpus* s
 frz_status frz_match_shard_device_top(frz_matcher* m, const frz_corpus* shard, uint32_t index_offset, frz_match* d_out, uint64_t cap,
                                       uint64_t* d_count, void* stream_, uint32_t limit) {
     if (!m || !shard || !d_out || !d_count) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
-    FRZ_TRY(ensure_device(shard->st.device));
+    FRZ_TRY(frz_ensure_device(shard->st.device));
     cudaStream_t stream = (cudaStream_t)stream_;
-    FrzLaunchStats st;
-    FrzMatchDev* d_list = nullptr;
     // asynchronous entry point: nobody reads the overflow flag back, so size the lists for the worst case
     FRZ_TRY(ensure_workspace(m, shard->st, std::max<uint64_t>(shard->st.n, 1)));
     // the run can never exceed the shard size; the caller sizes d_out as >= shard length
     if (cap < shard->st.n) return frz_fail(FRZ_ERR_CAPACITY, "d_out must hold the whole shard (%llu)", (unsigned long long)shard->st.n);
-    if (!m->count_ev) FRZ_TRY(frz_event_create(m->count_ev, cudaEventDisableTiming));
-    m->early_count_dst = d_count;
-    m->count_published = false;
-    m->ws.sort.arm_table_ev = true;
-    m->ws.sort.table_ev_recorded = false;
-    const frz_status ms = match_list_device(m, shard->st, index_offset, m->config.sort, &d_list, stream, &st, reinterpret_cast<FrzMatchDev*>(d_out),
-                                            limit);
-    m->early_count_dst = nullptr;
-    m->ws.sort.arm_table_ev = false;
-    FRZ_TRY(ms);
-    if (!m->count_published) {   // multi-pattern / empty pattern: the count exists only at the end
-        FRZ_CUDA_TRY(cudaMemcpyAsync(d_count, &m->ws.counters.get()->total, sizeof(uint64_t), cudaMemcpyDeviceToDevice, stream));
-        FRZ_CUDA_TRY(cudaEventRecord(m->count_ev.get(), stream));
-    }
-    m->last_launches = st.launches;
-    m->timings_pending = true;   // events were recorded; frz_matcher_last_timings reads them once the stream is idle
-    return FRZ_OK;
+    // (the count of a multi-pattern or empty matcher exists only at the end)
+    return shard_call(m, d_count, stream, [&](FrzLaunchStats* st) {
+        FrzMatchDev* d_list = nullptr;
+        return match_list_device(m, shard->st, index_offset, m->config.sort, &d_list, stream, st, reinterpret_cast<FrzMatchDev*>(d_out),
+                                 limit);
+    });
 }
 
 // Makes `stream` wait until the count of the last frz_match_shard_device call has been written to its d_count
@@ -1801,12 +1783,9 @@ frz_status streamed_range(StreamedCtx& x, uint32_t t0, uint32_t t1, bool last) {
     FRZ_TRY(frz_launch_prefilter(cv, x.c->dev, ws, x.stream, x.st, x.ntab));
     FRZ_TRY(frz_launch_tile_scan(cv, ws, x.stream, x.st, ws.stream_total.get()));
     if (last) {
-        cudaEventRecord(ws.ev[1].get(), x.stream); ws.ev_rec[1] = true;
-        if (m->early_count_dst) {   // the running count is final: publish it before the last range is scored
-            FRZ_CUDA_TRY(cudaMemcpyAsync(m->early_count_dst, &ws.counters.get()->total, sizeof(uint64_t), cudaMemcpyDeviceToDevice, x.stream));
-            FRZ_CUDA_TRY(cudaEventRecord(m->count_ev.get(), x.stream));
-            m->count_published = true;
-        }
+        record_ev(ws, 1, x.stream);
+        // the running count is final: publish it before the last range is scored
+        if (m->early_count_dst) FRZ_TRY(publish_count(m, m->early_count_dst, x.stream));
     }
     FRZ_TRY(frz_launch_sw(cv, x.c->dev, off, false, ws, x.dst, x.stream, x.st, FrzScoreHist(), x.ntab));
     return FRZ_OK;
@@ -1838,7 +1817,7 @@ bool streamed_eligible(const frz_matcher* m, uint64_t n, uint32_t index_offset) 
 frz_status frz_match_shard_streamed(frz_matcher* m, const uint8_t* bytes, const void* offsets, int offset_width, uint64_t n, int device,
                                     uint32_t index_offset, frz_match* d_out, uint64_t cap, uint64_t* d_count, void* stream_) {
     if (!m || !offsets || !d_out || !d_count) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
-    if (offset_width != 4 && offset_width != 8) return frz_fail(FRZ_ERR_INVALID_ARG, "offset_width must be 4 or 8");
+    FRZ_TRY(frz_check_offset_width(offset_width));
     if (!streamed_eligible(m, n, index_offset)) {
         const frz_corpus* shard = nullptr;
         FRZ_TRY(frz_matcher_ingest_e2e(m, bytes, offsets, offset_width, n, device, &shard));
@@ -1853,54 +1832,37 @@ namespace {
 frz_status match_streamed_impl(frz_matcher* m, const uint8_t* bytes, const void* offsets, int offset_width, uint64_t n, int device,
                                uint32_t index_offset, FrzMatchDev* d_out, uint64_t* d_count, cudaStream_t stream, FrzMatchDev** d_result) {
     const uint8_t sort = m->config.sort;
-    FRZ_TRY(ensure_device(device));
+    FRZ_TRY(frz_ensure_device(device));
     frz_corpus& c = e2e_corpus_on(m, device);
     c.st.n = n;
     c.st.n_tiles = (uint32_t)((n + FRZ_TILE - 1) / FRZ_TILE);
     FrzWorkspace& ws = m->ws;
     FRZ_TRY(ensure_workspace(m, c.st, std::max<uint64_t>(n, 1)));   // nobody reads the overflow flag back: worst-case lists
-    if (!m->count_ev) FRZ_TRY(frz_event_create(m->count_ev, cudaEventDisableTiming));
     const Compiled& pat = m->compiled[0];
     const bool will_sort = sort == FRZ_SORT_SCORE_THEN_INDEX_ASC;
     FrzMatchDev* final_out = d_out ? d_out : ws.matches_b.get();
     if (!d_count) d_count = reinterpret_cast<uint64_t*>(ws.stream_total.get() + 1);
     if (d_result) *d_result = final_out;
-    FrzLaunchStats st;
-    for (bool& f : ws.ev_rec) f = false;
-    m->last_sort_bins = 0;
-    m->early_count_dst = d_count;
-    m->count_published = false;
-    ws.sort.arm_table_ev = true;
-    ws.sort.table_ev_recorded = false;
-    StreamedCtx x;
-    x.m = m; x.c = &pat; x.index_offset = index_offset; x.dst = will_sort ? ws.matches_a.get() : final_out; x.stream = stream; x.st = &st;
-    FRZ_TRY(needle_table(m, pat, &x.ntab));   // a synchronous upload, so before the first H2D chunk
-    x.pending_t0 = 0; x.chunks_pending = 0;
-    x.group = 4;   // a range per four H2D chunks (about 1/8 of the list): the tail after the last chunk is one range + the sort
-    const frz_status ms = [&]() -> frz_status {
+    return shard_call(m, d_count, stream, [&](FrzLaunchStats* st) -> frz_status {
+        reset_call_state(m);
+        StreamedCtx x;
+        x.m = m; x.c = &pat; x.index_offset = index_offset; x.dst = will_sort ? ws.matches_a.get() : final_out; x.stream = stream; x.st = st;
+        FRZ_TRY(needle_table(m, pat, &x.ntab));   // a synchronous upload, so before the first H2D chunk
+        x.pending_t0 = 0; x.chunks_pending = 0;
+        x.group = 4;   // a range per four H2D chunks (about 1/8 of the list): the tail after the last chunk is one range + the sort
         FRZ_CUDA_TRY(cudaMemsetAsync(ws.stream_total.get(), 0, sizeof(unsigned long long), stream));
-        cudaEventRecord(ws.ev[0].get(), stream); ws.ev_rec[0] = true;
+        record_ev(ws, 0, stream);
         FRZ_TRY(frz_ingest_host(m->e2e_ingest, bytes, offsets, offset_width, n, stream, &c.st, streamed_after_chunk, &x));
-        cudaEventRecord(ws.ev[2].get(), stream); ws.ev_rec[2] = true;
+        record_ev(ws, 2, stream);
         if (will_sort) {
             FrzMatchDev* tmp = nullptr;
             if (pat.score_bound >= 1024) { FRZ_TRY(ensure_multi_buffers(m, n)); tmp = ws.multi_a.get(); }
-            FRZ_TRY(frz_launch_sort_by_score_dev(ws.matches_a.get(), tmp, final_out, &ws.counters.get()->total, pat.score_bound, ws.sort, stream, &st));
+            FRZ_TRY(frz_launch_sort_by_score_dev(ws.matches_a.get(), tmp, final_out, &ws.counters.get()->total, pat.score_bound, ws.sort, stream, st));
             m->last_sort_bins = frz_sort_single_pass_bins(pat.score_bound);
         }
-        cudaEventRecord(ws.ev[3].get(), stream); ws.ev_rec[3] = true;
+        record_ev(ws, 3, stream);
         return FRZ_OK;
-    }();
-    m->early_count_dst = nullptr;
-    ws.sort.arm_table_ev = false;
-    FRZ_TRY(ms);
-    if (!m->count_published) {   // (cannot happen with >= 1 chunk; kept for symmetry with frz_match_shard_device)
-        FRZ_CUDA_TRY(cudaMemcpyAsync(d_count, &ws.counters.get()->total, sizeof(uint64_t), cudaMemcpyDeviceToDevice, stream));
-        FRZ_CUDA_TRY(cudaEventRecord(m->count_ev.get(), stream));
-    }
-    m->last_launches = st.launches;
-    m->timings_pending = true;
-    return FRZ_OK;
+    });
 }
 }  // namespace
 
@@ -2061,7 +2023,7 @@ frz_status frz_merge_runs_ex(FrzMergeScratch& ms, const FrzMatchDev* runs, uint6
 extern "C" frz_status frz_merge_runs_device(const frz_match* d_runs, uint64_t run_stride, const uint64_t* run_counts_host,
                                             int n_runs, uint8_t sort, uint32_t score_bound_in, frz_match* d_out, int device, void* stream_) {
     if (!d_runs || !run_counts_host || !d_out || n_runs <= 0 || n_runs > FRZ_MERGE_MAX_RUNS) return frz_fail(FRZ_ERR_INVALID_ARG, "bad argument");
-    FRZ_TRY(ensure_device(device));
+    FRZ_TRY(frz_ensure_device(device));
     if (device >= 64) return frz_fail(FRZ_ERR_INVALID_ARG, "device index too large");
     // grow-only per-device scratch (tables only: the run metadata travels as kernel parameters).  Calls for one device
     // must be stream-ordered with each other, as documented in the header.  Never destroyed: its destructors would run
@@ -2076,7 +2038,7 @@ extern "C" frz_status frz_merge_runs_device(const frz_match* d_runs, uint64_t ru
 extern "C" frz_status frz_radix_sort_matches(frz_match* matches, uint64_t n, int device) {
     if (n == 0) return FRZ_OK;
     if (!matches) return frz_fail(FRZ_ERR_INVALID_ARG, "null matches");
-    FRZ_TRY(ensure_device(device));
+    FRZ_TRY(frz_ensure_device(device));
     FrzDevArray<FrzMatchDev> d_a, d_b, d_c;
     FrzDevArray<unsigned long long> d_n;
     FrzSortScratch ss;

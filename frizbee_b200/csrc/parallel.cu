@@ -360,19 +360,6 @@ struct frz_comm {
 
 namespace {
 
-frz_status set_device(int device) {
-    int n = 0;
-    cudaError_t e = cudaGetDeviceCount(&n);
-    if (e != cudaSuccess || n == 0) {
-        cudaGetLastError();
-        return frz_fail(FRZ_ERR_NO_DEVICE, "no CUDA device available (%s); this library has no CPU fallback",
-                        e == cudaSuccess ? "device count is 0" : cudaGetErrorString(e));
-    }
-    if (device < 0 || device >= n) return frz_fail(FRZ_ERR_INVALID_ARG, "device %d out of range (have %d)", device, n);
-    FRZ_CUDA_TRY(cudaSetDevice(device));
-    return FRZ_OK;
-}
-
 // what the rank's owners do not free themselves: its matcher clone, its peers' mappings and its NCCL communicator
 void rank_release(RankCtx& r) {
     cudaSetDevice(r.device);
@@ -386,8 +373,18 @@ void rank_release(RankCtx& r) {
     r.nccl = nullptr;
 }
 
+// the rank's clone of m (parallel.rs:46 — `matcher.clone()` per worker), made again whenever m's compiled patterns changed
+frz_status refresh_clone(RankCtx& r, const frz_matcher* m) {
+    if (r.clone && r.clone_epoch == frz_matcher_epoch(m)) return FRZ_OK;
+    if (r.clone) frz_matcher_destroy(r.clone);
+    r.clone = nullptr;
+    FRZ_TRY(frz_matcher_clone(m, &r.clone));
+    r.clone_epoch = frz_matcher_epoch(m);
+    return FRZ_OK;
+}
+
 frz_status rank_init(RankCtx& r) {
-    FRZ_TRY(set_device(r.device));
+    FRZ_TRY(frz_ensure_device(r.device));
     FRZ_TRY(frz_stream_create(r.side, cudaStreamNonBlocking));
     FRZ_TRY(r.d_count.reserve(2));
     FRZ_CUDA_TRY(cudaMemset(r.d_count.get(), 0, 2 * sizeof(unsigned long long)));
@@ -407,7 +404,7 @@ void host_block_release(HostBlock& b) {
 // exchange of a few host words between the ranks of a multi-process communicator, over NCCL (set-up time only)
 frz_status exchange_words(frz_comm* c, const uint64_t* mine, int n_words, uint64_t* all /* [world * n_words] */) {
     RankCtx& r = c->ranks[0];
-    FRZ_TRY(set_device(r.device));
+    FRZ_TRY(frz_ensure_device(r.device));
     FrzDevArray<unsigned long long> d_in, d_out;
     FRZ_TRY(d_in.reserve(n_words));
     FRZ_TRY(d_out.reserve((size_t)c->world * n_words));
@@ -568,7 +565,7 @@ frz_status host_block_alloc(frz_comm* c, uint64_t bytes, HostBlock* out) {
         const int world = c->world;
         for (int g = 0; g < world; g++)
             first_touch_near(c->ranks[g].device, static_cast<unsigned char*>(b.ptr), bytes * (uint64_t)g / world, bytes * (uint64_t)(g + 1) / world);
-        FRZ_TRY(set_device(c->ranks[0].device));
+        FRZ_TRY(frz_ensure_device(c->ranks[0].device));
         if (cudaHostRegister(b.ptr, bytes, cudaHostRegisterPortable | cudaHostRegisterMapped) != cudaSuccess) {
             cudaGetLastError();
             munmap(b.ptr, bytes);
@@ -605,7 +602,7 @@ frz_status host_block_alloc(frz_comm* c, uint64_t bytes, HostBlock* out) {
     std::vector<uint64_t> oks(c->world);
     FRZ_TRY(exchange_words(c, &ok, 1, oks.data()));
     if (ok) {
-        FRZ_TRY(set_device(c->ranks[0].device));
+        FRZ_TRY(frz_ensure_device(c->ranks[0].device));
         if (cudaHostRegister(b.ptr, bytes, cudaHostRegisterPortable | cudaHostRegisterMapped) == cudaSuccess) b.registered = true;
         else { cudaGetLastError(); ok = 0; }
     }
@@ -640,7 +637,7 @@ frz_status comm_finish_setup(frz_comm* c, bool slices) {
     c->ctrl_host = reinterpret_cast<volatile uint64_t*>(c->ctrl.ptr);
     if (c->p2p_exchange && c->local_form) {   // one process: plain peer access between every pair of devices
         for (RankCtx& a : c->ranks) {
-            FRZ_TRY(set_device(a.device));
+            FRZ_TRY(frz_ensure_device(a.device));
             for (RankCtx& b : c->ranks) {
                 if (a.device == b.device) continue;
                 int can = 0;
@@ -656,7 +653,7 @@ frz_status comm_finish_setup(frz_comm* c, bool slices) {
         c->tables_host = reinterpret_cast<volatile uint32_t*>(c->tables.ptr);
     }
     for (RankCtx& r : c->ranks) {
-        FRZ_TRY(set_device(r.device));
+        FRZ_TRY(frz_ensure_device(r.device));
         void* dp = nullptr;
         FRZ_CUDA_TRY(cudaHostGetDevicePointer(&dp, c->ctrl.ptr, 0));
         r.ctrl_dev = reinterpret_cast<uint64_t*>(dp);
@@ -716,7 +713,7 @@ struct HostShard {
 // only the first K' = min(limit, total) positions of the merged list are produced; UINT64_MAX for the whole list.
 frz_status rank_step(frz_comm* c, RankCtx& r, frz_matcher* m, const frz_corpus* shard, const HostShard* hs, uint32_t index_offset, uint64_t seq,
                      frz_match* out_host, uint64_t cap, bool want_host, bool want_slices, uint64_t limit, StepResult* res) {
-    FRZ_TRY(set_device(r.device));
+    FRZ_TRY(frz_ensure_device(r.device));
     cudaStream_t main = nullptr;   // the device's legacy default stream: ordered with the caller's own default-stream work
     const int world = c->world;
     const int parity = (int)(seq & 1);
@@ -724,12 +721,7 @@ frz_status rank_step(frz_comm* c, RankCtx& r, frz_matcher* m, const frz_corpus* 
     if (shard && frz_corpus_device(shard) != r.device)
         return frz_fail(FRZ_ERR_INVALID_ARG, "shard of rank %d lives on device %d, the communicator expects device %d", r.rank,
                         frz_corpus_device(shard), r.device);
-    if (!r.clone || r.clone_epoch != frz_matcher_epoch(m)) {   // parallel.rs:46 — `matcher.clone()` per worker
-        if (r.clone) frz_matcher_destroy(r.clone);
-        r.clone = nullptr;
-        FRZ_TRY(frz_matcher_clone(m, &r.clone));
-        r.clone_epoch = frz_matcher_epoch(m);
-    }
+    FRZ_TRY(refresh_clone(r, m));
     const uint64_t n_local = hs ? hs->n : frz_corpus_len(shard);
     FRZ_TRY(r.run.reserve(std::max<uint64_t>(n_local, 1)));
     FRZ_CUDA_TRY(cudaEventRecord(r.ev[0].get(), main));
@@ -1083,7 +1075,7 @@ extern "C" frz_status frz_corpus_create_sharded(const uint8_t* bytes, const void
                                                 frz_corpus** shards_out) {
     if (!c || !shards_out || !offsets) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
     if (!c->local_form) return frz_fail(FRZ_ERR_INVALID_ARG, "frz_corpus_create_sharded needs a local (single-process) communicator");
-    if (offset_width != 4 && offset_width != 8) return frz_fail(FRZ_ERR_INVALID_ARG, "offset_width must be 4 or 8");
+    FRZ_TRY(frz_check_offset_width(offset_width));
     if (n > 0xFFFFFFFFull) return frz_fail(FRZ_ERR_TOO_MANY_ITEMS, "too many items in haystack, will overflow the u32 index: %llu", (unsigned long long)n);
     const int world = c->world;
     const uint64_t per = (n + world - 1) / world;   // shard g = [g * ceil(N/G), (g+1) * ceil(N/G))   (SURVEY.md §8(e))
@@ -1115,10 +1107,7 @@ frz_status match_list_parallel_local(frz_matcher* m, const frz_corpus* const* sh
         offs[g] = total_items;
         total_items += frz_corpus_len(shards[g]);
     }
-    // Matcher::guard_against_haystack_overflow (src/matcher/mod.rs:438-446)
-    if (total_items > 0xFFFFFFFFull)
-        return frz_fail(FRZ_ERR_TOO_MANY_ITEMS, "too many items in haystack, will overflow the u32 index: %llu > %u (index offset: 0)",
-                        (unsigned long long)total_items, 0xFFFFFFFFu);
+    FRZ_TRY(frz_check_index_range(total_items, 0));
     const uint64_t seq = ++c->seq;
     std::vector<StepResult> res(c->world);
     if (c->world == 1) {
@@ -1166,9 +1155,7 @@ extern "C" frz_status frz_match_list_parallel_rank(frz_matcher* m, const frz_cor
                                                    uint64_t cap, uint64_t* n_out, const frz_match** d_out) {
     if (!m || !c || !shard) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
     if (c->local_form && c->world != 1) return frz_fail(FRZ_ERR_INVALID_ARG, "local communicator: call frz_match_list_parallel");
-    if ((uint64_t)index_offset + frz_corpus_len(shard) > 0xFFFFFFFFull)
-        return frz_fail(FRZ_ERR_TOO_MANY_ITEMS, "too many items in haystack, will overflow the u32 index: %llu > %u (index offset: %u)",
-                        (unsigned long long)index_offset + frz_corpus_len(shard), 0xFFFFFFFFu, index_offset);
+    FRZ_TRY(frz_check_index_range(frz_corpus_len(shard), index_offset));
     std::lock_guard<std::mutex> lock(c->mu);
     const uint64_t seq = ++c->seq;
     StepResult res;
@@ -1184,9 +1171,7 @@ extern "C" frz_status frz_match_list_parallel_rank_top(frz_matcher* m, const frz
                                                        frz_match* out, uint64_t* n_out, uint64_t* n_total, const frz_match** d_out) {
     if (!m || !c || !shard) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
     if (c->local_form && c->world != 1) return frz_fail(FRZ_ERR_INVALID_ARG, "local communicator: call frz_match_list_parallel_top");
-    if ((uint64_t)index_offset + frz_corpus_len(shard) > 0xFFFFFFFFull)
-        return frz_fail(FRZ_ERR_TOO_MANY_ITEMS, "too many items in haystack, will overflow the u32 index: %llu > %u (index offset: %u)",
-                        (unsigned long long)index_offset + frz_corpus_len(shard), 0xFFFFFFFFu, index_offset);
+    FRZ_TRY(frz_check_index_range(frz_corpus_len(shard), index_offset));
     std::lock_guard<std::mutex> lock(c->mu);
     const uint64_t seq = ++c->seq;
     StepResult res;
@@ -1203,19 +1188,12 @@ extern "C" frz_status frz_match_list_parallel_rank_host(frz_matcher* m, const ui
                                                         uint32_t index_offset, frz_comm* c, frz_match* out, uint64_t cap, uint64_t* n_out) {
     if (!m || !c || !offsets) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
     if (c->local_form && c->world != 1) return frz_fail(FRZ_ERR_INVALID_ARG, "local communicator: shard with frz_corpus_create_sharded and call frz_match_list_parallel");
-    if ((uint64_t)index_offset + n > 0xFFFFFFFFull)
-        return frz_fail(FRZ_ERR_TOO_MANY_ITEMS, "too many items in haystack, will overflow the u32 index: %llu > %u (index offset: %u)",
-                        (unsigned long long)index_offset + n, 0xFFFFFFFFu, index_offset);
+    FRZ_TRY(frz_check_index_range(n, index_offset));
     std::lock_guard<std::mutex> lock(c->mu);
     RankCtx& r = c->ranks[0];
-    FRZ_TRY(set_device(r.device));
-    if (!r.clone || r.clone_epoch != frz_matcher_epoch(m)) {
-        if (r.clone) frz_matcher_destroy(r.clone);
-        r.clone = nullptr;
-        FRZ_TRY(frz_matcher_clone(m, &r.clone));
-        r.clone_epoch = frz_matcher_epoch(m);
-    }
-    if (offset_width != 4 && offset_width != 8) return frz_fail(FRZ_ERR_INVALID_ARG, "offset_width must be 4 or 8");
+    FRZ_TRY(frz_ensure_device(r.device));
+    FRZ_TRY(refresh_clone(r, m));
+    FRZ_TRY(frz_check_offset_width(offset_width));
     const HostShard hs{bytes, offsets, offset_width, n};
     const uint64_t seq = ++c->seq;
     StepResult res;
@@ -1231,7 +1209,7 @@ extern "C" frz_status frz_comm_last_timings(frz_comm* c, int local_index, float*
     if (ms4) {
         ms4[0] = ms4[1] = ms4[2] = ms4[3] = 0;
         if (r.ev_valid) {
-            FRZ_TRY(set_device(r.device));
+            FRZ_TRY(frz_ensure_device(r.device));
             FRZ_CUDA_TRY(cudaEventSynchronize(r.ev[3].get()));
             cudaEventElapsedTime(&ms4[0], r.ev[0].get(), r.ev[1].get());
             cudaEventElapsedTime(&ms4[1], r.ev[1].get(), r.ev[2].get());
