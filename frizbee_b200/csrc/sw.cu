@@ -102,8 +102,11 @@ __device__ __forceinline__ uint32_t score_window(const FrzPatternDev& pat, const
     const uint64_t pos = match_position(rec, reversed != 0, rv, ctr);   // loads overlap the DP
     uint32_t hw[CC / 4];
     window_from_units<CC>(u, wr.startlo, wr.W, hw);
+    // Only a window that is a whole haystack as long as the needle can equal it: the record says so before any needle
+    // byte is read.  Deciding it before the DP also means the window words need not stay live across it.
+    bool exact = false;
+    if (wr.start0 && wr.full_end && wr.W == pat.n) exact = window_equals_needle(hw, wr.W, pat);
     uint32_t score = SwCore<LANES, COLS, WRAP8, VAR, CC>::run(hw, wr.W, pat, wr.start0, sw_smem);
-    bool exact = wr.start0 && wr.full_end && window_equals_needle(hw, wr.W, pat);
     if (exact) score = (score + pat.exact_bonus) & 0xffffu;
     store_match(rec, pos, score, exact, index_offset, out, hist);
     return score;

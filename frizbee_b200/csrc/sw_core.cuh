@@ -162,6 +162,7 @@ struct SwCore {
     static constexpr bool SMEM = COLS > 64 || kSw64RowsInSmem<LANES, WRAP8>;
     static constexpr bool PAIR = COLS <= 64 && SMEM;
     static constexpr size_t smem_bytes = SMEM ? 2 * R * kSwThreads * sizeof(uint32_t) : 0;
+    static constexpr bool kGaplessLastRow = !WRAP8 && COLS <= 64;   // see run()
 
     // ---- diagonal + up of needle row i at register r, in place (H[r-1] must still hold row i-1).  up: the needle byte
     // is an uppercase letter (rare), whose exact-case bonus moves from the non-upper to the upper haystack bytes.
@@ -299,6 +300,12 @@ struct SwCore {
 #pragma unroll R
                 for (int r = R - 1; r >= 0; r--) diag_up(H, M, r, rows.get(r), p, i, COLS > 64 && !WRAP8 && upper_row);
             }
+            // The last row's gap propagation cannot change the score.  Every gap penalty is <= 0 per lane and every cell
+            // >= 0, so a gap step H[j] = max(H[j - s] + pen, H[j], 0) never raises a cell above the largest cell to its
+            // left, and the maximum over the leading chunks read below is the one the diagonal + up step leaves.  Not
+            // with WRAP8 (the u8 wrap makes the arithmetic non-monotone), and not for 128 columns, whose rows already
+            // spill and which ptxas then spills further.
+            if (kGaplessLastRow && i == p.n - 1) break;
             // ---- horizontal gap propagation, chunk by chunk (ascii_gap.rs gap_step!) ----
 #pragma unroll
             for (int c = 0; c < NCH; c++) {
