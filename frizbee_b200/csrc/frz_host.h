@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <algorithm>
 #include <atomic>
 #include <memory>
 #include <string>
@@ -25,6 +26,10 @@ inline int frz_sm_count() {
     int& c = count_dev[d & 63];
     if (c <= 0 && (cudaDeviceGetAttribute(&c, cudaDevAttrMultiProcessorCount, d) != cudaSuccess || c <= 0)) c = 132;   // H100 SXM
     return c;
+}
+// a grid of `block`-thread blocks over n items, at most 16 blocks per SM
+inline int grid_for(uint64_t n, int block) {
+    return (int)std::max<uint64_t>(1, std::min<uint64_t>((n + block - 1) / block, (uint64_t)frz_sm_count() * 16));
 }
 
 #define FRZ_CUDA_TRY(expr)                                                                         \
@@ -293,17 +298,27 @@ frz_status frz_sort_fused_prepare(FrzSortScratch& ss, uint64_t n_cap, uint32_t s
 frz_status frz_launch_sort_fused(const FrzMatchDev* d_in, FrzMatchDev* d_out, const unsigned long long* n_ptr, const FrzScoreHist& hist,
                                  FrzSortScratch& ss, cudaStream_t stream, FrzLaunchStats* st, uint32_t limit = kFrzNoLimit);
 
-// k-way merge of per-shard runs (host.cu) with caller-owned scratch — one per concurrent user (parallel.cu: one per rank)
+// k-way merge of per-shard runs (merge.cu) with caller-owned scratch — one per concurrent user (parallel.cu: one per rank)
 #define FRZ_MERGE_MAX_RUNS 64
 struct FrzMergeScratch {
     FrzSortScratch sort;                      // of the concatenate-and-sort fallback
-    FrzDevArray<uint32_t> tables;             // gt / pos0 tables of the scatter merge
+    FrzDevArray<uint32_t> tables;             // pos0 / gt tables of the scatter merge (merge_plan.cuh)
     FrzDevArray<FrzMatchDev> cat;
     FrzDevArray<FrzMatchDev> tmp;
     FrzDevArray<unsigned long long> d_total;
 };
 frz_status frz_merge_runs_ex(FrzMergeScratch& ms, const FrzMatchDev* runs, uint64_t run_stride, const uint64_t* run_counts_host,
                              int n_runs, uint8_t sort, uint32_t score_bound, FrzMatchDev* d_out, cudaStream_t stream);
+// The merge's scatter over one piece per run (k_merge_scatter): piece q is run q's elements [a[q], a[q] + n[q]) at src + src[q],
+// stored at their merged positions minus lo.  The whole merge passes whole runs and lo = 0, the slice exchange its pieces.
+struct FrzMergePieces {
+    uint64_t src[FRZ_MERGE_MAX_RUNS];
+    uint32_t n[FRZ_MERGE_MAX_RUNS];
+    uint32_t a[FRZ_MERGE_MAX_RUNS];
+    uint32_t lo;
+};
+frz_status frz_launch_merge_scatter(const FrzMatchDev* src, const FrzMergePieces& pieces, int n_runs, const uint32_t* tables, int bins,
+                                    int blocks_per_sm, FrzMatchDev* out, cudaStream_t stream);
 
 // Matcher internals the multi-GPU layer needs (host.cu)
 uint64_t frz_matcher_epoch(const frz_matcher* m);                  // changes whenever the compiled patterns change

@@ -1164,11 +1164,6 @@ frz_status read_counters(frz_matcher* m, cudaStream_t stream) {
     return FRZ_OK;
 }
 
-int grid_for(uint64_t n, int block) {
-    uint64_t g = (n + block - 1) / block;
-    return (int)std::max<uint64_t>(1, std::min<uint64_t>(g, (uint64_t)frz_sm_count() * 16));
-}
-
 // Every index of the corpus, ascending, into `out` (count in ws.counters->total): the list of the empty matcher and the
 // start of an all-negated one.  A corpus with removed haystacks, or a subset call (masked_meta, as in run_pattern), fills
 // `tmp` and keeps only the indices whose slot is in use.
@@ -1866,87 +1861,6 @@ frz_status match_streamed_impl(frz_matcher* m, const uint8_t* bytes, const void*
 }
 }  // namespace
 
-namespace {
-// Run metadata travels BY VALUE as a kernel parameter (1 KB of the 4 KB parameter space): no staging buffer, so
-// back-to-back merges with different counts cannot race and the entry point needs no per-call H2D copy.
-struct MergeMeta {
-    uint64_t counts[FRZ_MERGE_MAX_RUNS];   // valid entries of run r
-    uint64_t bases[FRZ_MERGE_MAX_RUNS];    // concatenation offset of the r-th run in merge order
-    uint64_t total;
-};
-
-__global__ void k_gather_runs(const FrzMatchDev* runs, uint64_t stride, const __grid_constant__ MergeMeta meta, int n_runs,
-                              int reverse_runs, FrzMatchDev* out, unsigned long long* d_total) {
-    if (blockIdx.x == 0 && threadIdx.x == 0 && d_total) *d_total = meta.total;
-    for (int r = 0; r < n_runs; r++) {
-        const int src_run = reverse_runs ? n_runs - 1 - r : r;
-        const FrzMatchDev* src = runs + (uint64_t)src_run * stride;
-        const uint64_t cnt = meta.counts[src_run], base = meta.bases[r];
-        for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < cnt; i += (uint64_t)gridDim.x * blockDim.x)
-            out[base + i] = src[i];
-    }
-}
-
-// ---- k-way merge of score-sorted runs (src/k_merge.rs:90-131) without comparing heads -------------------
-// Every run is sorted by score descending, so "the elements of run r with score s" is the index range
-// [gt[r][s], gt[r][s-1]) where gt[r][s] = #elements of run r with score > s — a binary search per (r, s).
-// The merged position of that block is  Σ_r' gt[r'][s]  (everything with a higher score)  +  the sizes of the
-// same-score blocks of the runs that come earlier in the merge order; one scatter pass places the elements.
-constexpr int kMergeMaxBins = 4096;
-
-__global__ void k_merge_bounds(const FrzMatchDev* __restrict__ runs, uint64_t stride, const __grid_constant__ MergeMeta meta,
-                               int n_runs, int bins, uint32_t* __restrict__ gt) {
-    const int t = blockIdx.x * blockDim.x + threadIdx.x;
-    if (t >= n_runs * bins) return;
-    const int r = t / bins;
-    const uint32_t s = (uint32_t)(t - r * bins);
-    const FrzMatchDev* run = runs + (uint64_t)r * stride;
-    uint64_t lo = 0, hi = meta.counts[r];   // first index whose score <= s
-    while (lo < hi) {
-        const uint64_t mid = (lo + hi) >> 1;
-        if (run[mid].score > s) lo = mid + 1; else hi = mid;
-    }
-    gt[t] = (uint32_t)lo;
-}
-
-// pos0[r][s] = merged position of the first element of run r's score-s block.  One thread per score.
-__global__ void k_merge_bases(const uint32_t* __restrict__ gt, const __grid_constant__ MergeMeta meta, int n_runs, int bins,
-                              int reverse_runs, uint32_t* __restrict__ pos0) {
-    const int s = blockIdx.x * blockDim.x + threadIdx.x;
-    if (s >= bins) return;
-    uint32_t higher = 0;
-    for (int r = 0; r < n_runs; r++) higher += gt[r * bins + s];
-    uint32_t acc = higher;
-    for (int k = 0; k < n_runs; k++) {
-        const int r = reverse_runs ? n_runs - 1 - k : k;
-        pos0[r * bins + s] = acc;
-        const uint32_t ge = s == 0 ? (uint32_t)meta.counts[r] : gt[r * bins + s - 1];   // #elements with score >= s
-        acc += ge - gt[r * bins + s];
-    }
-}
-
-// One pass over the gathered runs: gridDim.y = n_runs rows of blocks, one row per run, so every run streams at
-// full width (the first version looped over the runs inside one grid: short runs left most blocks idle).
-__global__ void __launch_bounds__(256) k_merge_scatter(const FrzMatchDev* __restrict__ runs, uint64_t stride,
-                                                       const __grid_constant__ MergeMeta meta, int bins,
-                                                       const uint32_t* __restrict__ gt, const uint32_t* __restrict__ pos0,
-                                                       FrzMatchDev* __restrict__ out) {
-    const int r = blockIdx.y;
-    const FrzMatchDev* run = runs + (uint64_t)r * stride;
-    const uint64_t cnt = meta.counts[r];
-    const uint32_t* gtr = gt + (size_t)r * bins;
-    const uint32_t* p0r = pos0 + (size_t)r * bins;
-    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < cnt; i += (uint64_t)gridDim.x * blockDim.x) {
-        const FrzMatchDev m = run[i];
-        const uint32_t s = min((uint32_t)m.score, (uint32_t)bins - 1);
-        out[p0r[s] + ((uint32_t)i - gtr[s])] = m;
-    }
-}
-}  // namespace
-
-// k_merge_matches_by (src/k_merge.rs:90-131).  Runs are index-range shards in rank order, each already
-// ordered per `sort`; concatenating them in (reverse) rank order and stable-sorting by score yields
-// exactly the reference's k-way merge (ties resolve by index because the shards are index-ordered).
 // Debugging / test aid: the compiled device pattern of pattern i (the struct the kernels receive), so that host
 // builds of the kernel cores (tests/test_kernel_logic_cpu.py) run with exactly the constants the GPU gets.
 extern "C" frz_status frz_matcher_debug_pattern(const frz_matcher* m, size_t i, void* out, size_t out_size) {
@@ -1967,72 +1881,6 @@ extern "C" uint32_t frz_matcher_score_bound(const frz_matcher* m) {
     uint64_t b = 0;
     for (const auto& c : m->compiled) if (!c.negated) b += c.score_bound;
     return (uint32_t)std::min<uint64_t>(b, 0xFFFF);
-}
-
-// k_merge_matches_by on `stream` with caller-owned scratch (one per concurrent user; grow-only).
-frz_status frz_merge_runs_ex(FrzMergeScratch& ms, const FrzMatchDev* runs, uint64_t run_stride, const uint64_t* run_counts_host,
-                             int n_runs, uint8_t sort, uint32_t score_bound_in, FrzMatchDev* d_out, cudaStream_t stream) {
-    if (!runs || !run_counts_host || !d_out || n_runs <= 0 || n_runs > FRZ_MERGE_MAX_RUNS) return frz_fail(FRZ_ERR_INVALID_ARG, "bad argument");
-    const bool reversed = sort == FRZ_SORT_INDEX_DESC || sort == FRZ_SORT_SCORE_THEN_INDEX_DESC;
-    const bool by_score = sort == FRZ_SORT_SCORE_THEN_INDEX_ASC || sort == FRZ_SORT_SCORE_THEN_INDEX_DESC;
-    const uint32_t score_bound = score_bound_in ? score_bound_in : 0xFFFF;
-    MergeMeta meta;
-    memset(&meta, 0, sizeof meta);
-    uint64_t total = 0;
-    for (int r = 0; r < n_runs; r++) {
-        meta.counts[r] = run_counts_host[r];
-        const int src_run = reversed ? n_runs - 1 - r : r;
-        meta.bases[r] = total;
-        total += run_counts_host[src_run];
-    }
-    meta.total = total;
-    if (!ms.d_total.get()) {   // first use, all or nothing: a failed set-up leaves the scratch empty
-        FrzMergeScratch fresh;
-        FRZ_TRY(frz_sort_hist_alloc(fresh.sort.hist));
-        FRZ_TRY(fresh.tables.reserve((size_t)2 * FRZ_MERGE_MAX_RUNS * kMergeMaxBins));
-        FRZ_TRY(fresh.d_total.reserve(1));
-        ms = std::move(fresh);
-    }
-    const int bins = (int)std::min<uint32_t>(score_bound, 0xFFFFu) + 1;
-    if (total == 0) return FRZ_OK;
-    if (by_score && bins <= kMergeMaxBins && total <= 0xFFFFFFFFull) {
-        // score-sorted runs: boundaries by binary search, one scatter pass (no concatenation, no re-sort)
-        uint32_t* gt = ms.tables.get();
-        uint32_t* pos0 = gt + (size_t)FRZ_MERGE_MAX_RUNS * kMergeMaxBins;
-        k_merge_bounds<<<(n_runs * bins + 255) / 256, 256, 0, stream>>>(runs, run_stride, meta, n_runs, bins, gt);
-        k_merge_bases<<<(bins + 127) / 128, 128, 0, stream>>>(gt, meta, n_runs, bins, reversed ? 1 : 0, pos0);
-        uint64_t longest = 0;
-        for (int r = 0; r < n_runs; r++) longest = std::max(longest, run_counts_host[r]);
-        const dim3 grid((unsigned)std::max<uint64_t>(1, std::min<uint64_t>((longest + 255) / 256, frz_sm_count() * 8 / std::max(n_runs, 1) + 1)), (unsigned)n_runs);
-        k_merge_scatter<<<grid, 256, 0, stream>>>(runs, run_stride, meta, bins, gt, pos0, d_out);
-        FRZ_CUDA_TRY(cudaGetLastError());
-        return FRZ_OK;  // asynchronous on `stream`
-    }
-    if (by_score) {
-        FRZ_TRY(ms.cat.reserve(total, total + total / 4 + 1024));
-        FRZ_TRY(ms.tmp.reserve(total, total + total / 4 + 1024));
-    }
-    FrzMatchDev* dst = by_score ? ms.cat.get() : d_out;
-    k_gather_runs<<<grid_for(total / std::max(n_runs, 1) + 1, 256), 256, 0, stream>>>(runs, run_stride, meta, n_runs, reversed ? 1 : 0, dst,
-                                                                                     ms.d_total.get());
-    if (by_score) FRZ_TRY(frz_launch_sort_by_score_dev(ms.cat.get(), ms.tmp.get(), d_out, ms.d_total.get(), score_bound, ms.sort, stream, nullptr));
-    FRZ_CUDA_TRY(cudaGetLastError());
-    return FRZ_OK;  // asynchronous on `stream`
-}
-
-extern "C" frz_status frz_merge_runs_device(const frz_match* d_runs, uint64_t run_stride, const uint64_t* run_counts_host,
-                                            int n_runs, uint8_t sort, uint32_t score_bound_in, frz_match* d_out, int device, void* stream_) {
-    if (!d_runs || !run_counts_host || !d_out || n_runs <= 0 || n_runs > FRZ_MERGE_MAX_RUNS) return frz_fail(FRZ_ERR_INVALID_ARG, "bad argument");
-    FRZ_TRY(frz_ensure_device(device));
-    if (device >= 64) return frz_fail(FRZ_ERR_INVALID_ARG, "device index too large");
-    // grow-only per-device scratch (tables only: the run metadata travels as kernel parameters).  Calls for one device
-    // must be stream-ordered with each other, as documented in the header.  Never destroyed: its destructors would run
-    // at process exit, when the CUDA runtime may already be gone.
-    static FrzMergeScratch* const scratch = new FrzMergeScratch[64];
-    static std::mutex mu;
-    std::lock_guard<std::mutex> lock(mu);
-    return frz_merge_runs_ex(scratch[device], reinterpret_cast<const FrzMatchDev*>(d_runs), run_stride, run_counts_host, n_runs, sort,
-                             score_bound_in, reinterpret_cast<FrzMatchDev*>(d_out), (cudaStream_t)stream_);
 }
 
 extern "C" frz_status frz_radix_sort_matches(frz_match* matches, uint64_t n, int device) {

@@ -20,11 +20,9 @@
 // machine, so that it can be tested.  The all-gather form serves device-out calls and host-out calls without per-score
 // tables (a score bound that needs the two-pass sort).
 //
-// The only per-step collective is that all-gather.  The match counts (the `Vec` lengths the k-merge reads) are
-// published by each GPU into a small pinned host block shared by all ranks — a 1-thread kernel right after the tile
-// scan, i.e. BEFORE the scoring kernels — and every rank's host thread polls the block; the same block carries the
-// "my slice has landed" flags that end a host-out step.  In the multi-process form the block (and the output
-// buffer) is a memfd segment that every rank maps and pins.
+// The only per-step collective is that all-gather.  The match counts, published before the scoring kernels, the score
+// tables and the "my slice has landed" flags cross a small pinned host block that every rank polls; in the multi-process
+// form the block (and the output buffer) is a memfd segment that every rank maps and pins.
 //
 // Top-K calls (frz_match_list_parallel*_top) keep only the first K' = min(k, total) positions of the merged list: a run keeps its
 // order in the merge, so nothing past a run's own first k can land there — every GPU sorts only its run's first k, the slice
@@ -55,6 +53,7 @@
 
 #include "frz_device.cuh"
 #include "frz_host.h"
+#include "merge_plan.cuh"
 
 #if defined(__x86_64__)
 #include <immintrin.h>
@@ -168,37 +167,8 @@ __global__ void __launch_bounds__(256) k_publish_table(volatile uint32_t* dst, c
     }
 }
 
-// Slice form of the k-way merge: this rank received, from every run q, exactly the elements [a_q, a_q + n_q) that land in
-// its slice [lo, hi) of the merged list.  Element i of piece q with score s goes to
-//     pos0[q][s] + (a_q + i - gt[q][s]) - lo
-// (pos0 = merged position of the first element of run q's score-s block, gt = how many of run q score higher than s).
-struct SliceMeta {
-    uint32_t off[kMaxWorld];   // start of piece q in the receive buffer
-    uint32_t n[kMaxWorld];     // its length
-    uint32_t a[kMaxWorld];     // its first element's index inside run q
-    unsigned long long lo;
-};
-__global__ void __launch_bounds__(256) k_slice_scatter(const FrzMatchDev* __restrict__ recv, const __grid_constant__ SliceMeta meta,
-                                                       const uint32_t* __restrict__ gt, const unsigned long long* __restrict__ pos0,
-                                                       int bins, FrzMatchDev* __restrict__ out) {
-    const int q = blockIdx.y;
-    const FrzMatchDev* piece = recv + meta.off[q];
-    const uint32_t n = meta.n[q], a = meta.a[q];
-    const uint32_t* gtq = gt + (size_t)q * bins;
-    const unsigned long long* p0q = pos0 + (size_t)q * bins;
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-        const FrzMatchDev m = piece[i];
-        const uint32_t s = bins > 1 ? min((uint32_t)m.score, (uint32_t)bins - 1) : 0u;
-        out[p0q[s] + (a + i - gtq[s]) - meta.lo] = m;
-    }
-}
-
 // ---- P2P placement: the exchange and the k-way merge in one pass over peer memory ------------------------------------
-// Rank q holds run q sorted; with every rank's score table it knows pos0[s] (merged position of the first element of its
-// score-s block) and gt[s] (how many of its elements score higher), so element i with score s belongs at merged position
-// pos0[s] + (i - gt[s]).  Position x lives in the slice of rank p with lo[p] <= x < lo[p + 1] (lo[p] = total * p / world): the
-// element is stored into rank p's slice buffer, which is this GPU's own memory for p == q and NVLink peer memory otherwise.
-// Consecutive elements of a score block land on consecutive addresses, so the stores coalesce.  The block that finishes
+// Element x of the merged list goes to the slice buffer of the rank p with lo[p] <= x < lo[p + 1].  Consecutive elements of a score block land on consecutive addresses, so the stores coalesce.  The block that finishes
 // last raises this rank's flag in every peer's header (after a system-scope fence) and then waits for every peer's flag
 // in its OWN header: when the kernel ends, this rank's slice is complete and the stream-ordered device→host copy may run.
 constexpr size_t kPlaceHeaderBytes = 2048;
@@ -209,14 +179,14 @@ struct PlaceHeader {
 static_assert(sizeof(PlaceHeader) <= kPlaceHeaderBytes, "place header");
 struct PlaceMeta {
     unsigned char* peer[kMaxWorld];             // every rank's place buffer (header + slice elements) as mapped on THIS device
-    unsigned long long lo[kMaxWorld + 1];       // slice boundaries in the merged list
+    uint64_t lo[kMaxWorld + 1];                 // slice boundaries in the merged list
     unsigned long long total;                   // positions kept: the merged list's length, or K' of a top-K call
     int world, rank, bins, parity;
 };
 __global__ void __launch_bounds__(256) k_place(const FrzMatchDev* __restrict__ run, unsigned long long n, const __grid_constant__ PlaceMeta meta,
-                                               const unsigned long long* __restrict__ pos0, const uint32_t* __restrict__ gt,
+                                               const uint32_t* __restrict__ pos0, const uint32_t* __restrict__ gt,
                                                unsigned long long seq, unsigned long long timeout_ns, volatile unsigned long long* err_slot) {
-    __shared__ unsigned long long lo_s[kMaxWorld + 1];
+    __shared__ uint64_t lo_s[kMaxWorld + 1];
     __shared__ FrzMatchDev* dst_s[kMaxWorld];
     __shared__ int last_s;
     const int world = meta.world, bins = meta.bins;
@@ -226,12 +196,10 @@ __global__ void __launch_bounds__(256) k_place(const FrzMatchDev* __restrict__ r
     const unsigned long long total = meta.total;
     for (unsigned long long i = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (unsigned long long)gridDim.x * blockDim.x) {
         const FrzMatchDev m = run[i];
-        const uint32_t s = bins > 1 ? min((uint32_t)m.score, (uint32_t)bins - 1) : 0u;
+        const uint32_t s = frzmerge::bin_of(m.score, bins);
         const unsigned long long x = pos0[s] + (i - gt[s]);
         if (x >= total) continue;   // beyond the first K' of a top-K call
-        int p = (int)min((unsigned long long)(world - 1), x * (unsigned long long)world / total);   // lo[p] = floor(total * p / world): at most one off
-        while (p > 0 && x < lo_s[p]) p--;
-        while (p + 1 < world && x >= lo_s[p + 1]) p++;
+        const int p = frzmerge::slice_of(x, total, world, lo_s);
         dst_s[p][x - lo_s[p]] = m;
     }
     __threadfence_system();   // this thread's peer stores are performed before the block signs off
@@ -301,16 +269,12 @@ struct RankCtx {
     uint64_t clone_epoch = 0;
     FrzDevArray<FrzMatchDev> run;          // this rank's locally ordered run
     FrzDevArray<unsigned long long> d_count;
-    FrzDevArray<FrzMatchDev> gathered;
+    FrzDevArray<FrzMatchDev> gathered;     // the all-gather's runs, or the pieces the slice exchange received
     FrzDevArray<FrzMatchDev> merged;
     FrzMergeScratch merge;
-    // slice exchange (host-out calls): pieces received from every run, device copies of the gt / pos0 tables, pinned staging
-    FrzDevArray<FrzMatchDev> recv;
-    // [world * kTableBins] u64 pos0, then as many u32 gt (d_gt, h_gt): the tables travel in ONE host→device copy
-    FrzDevArray<unsigned long long> d_pos0;
-    FrzPinnedArray<unsigned long long> h_pos0;
-    uint32_t* d_gt = nullptr;
-    uint32_t* h_gt = nullptr;
+    // host-out calls: the merge's table rows (merge_plan.cuh), staged on the host and copied to the device in ONE copy
+    FrzDevArray<uint32_t> d_tables;
+    FrzPinnedArray<uint32_t> h_tables;
     // P2P placement (host-out calls): my slice buffer (header + elements), exported to the peers; theirs mapped here
     FrzDevArray<unsigned char> place_raw;
     uint64_t place_cap = 0;                 // elements
@@ -360,15 +324,20 @@ struct frz_comm {
 
 namespace {
 
+// forgets the peers' slice buffers mapped on this rank's device, closing the cudaIpc mappings
+void drop_peer_mappings(RankCtx& r) {
+    for (int q = 0; q < kMaxWorld; q++) {
+        if (r.peer_ipc[q] && r.peer_raw[q]) cudaIpcCloseMemHandle(r.peer_raw[q]);
+        r.peer_raw[q] = nullptr; r.peer_ipc[q] = false;
+    }
+}
+
 // what the rank's owners do not free themselves: its matcher clone, its peers' mappings and its NCCL communicator
 void rank_release(RankCtx& r) {
     cudaSetDevice(r.device);
     if (r.clone) frz_matcher_destroy(r.clone);
     r.clone = nullptr;
-    for (int q = 0; q < kMaxWorld; q++) {
-        if (r.peer_ipc[q] && r.peer_raw[q]) cudaIpcCloseMemHandle(r.peer_raw[q]);
-        r.peer_raw[q] = nullptr; r.peer_ipc[q] = false;
-    }
+    drop_peer_mappings(r);
     if (r.nccl) nccl_api().CommDestroy(r.nccl);
     r.nccl = nullptr;
 }
@@ -448,10 +417,7 @@ frz_status ensure_place_buffers(frz_comm* c, RankCtx& r, uint64_t need, bool* re
     if (r.place_cap >= need) { *ready = true; return FRZ_OK; }
     const int world = c->world;
     FRZ_CUDA_TRY(cudaDeviceSynchronize());   // nothing of mine may still read or write the old buffers
-    for (int q = 0; q < world; q++) {
-        if (r.peer_ipc[q] && r.peer_raw[q]) cudaIpcCloseMemHandle(r.peer_raw[q]);
-        r.peer_raw[q] = nullptr; r.peer_ipc[q] = false;
-    }
+    drop_peer_mappings(r);
     uint64_t w[10], all[kMaxWorld * 10];
     memset(w, 0, sizeof w);
     FRZ_TRY(allgather_words(c, r, w, 1, all));   // everybody has dropped its mappings: the owners may free
@@ -488,10 +454,7 @@ frz_status ensure_place_buffers(frz_comm* c, RankCtx& r, uint64_t need, bool* re
     FRZ_TRY(allgather_words(c, r, &okw, 1, all));   // also: nobody stores into a buffer before its owner has zeroed the header
     for (int q = 0; q < world; q++) ok = ok && all[q] == 1;
     if (!ok) {   // every rank sees the same verdict: P2P placement is off for this communicator from now on
-        for (int q = 0; q < world; q++) {
-            if (r.peer_ipc[q] && r.peer_raw[q]) cudaIpcCloseMemHandle(r.peer_raw[q]);
-            r.peer_raw[q] = nullptr; r.peer_ipc[q] = false;
-        }
+        drop_peer_mappings(r);
         r.place_raw.reset();
         r.place_cap = 0;
         if (&r == &c->ranks[0]) c->p2p_exchange = false;   // one writer; the other workers read it at their next call
@@ -660,11 +623,8 @@ frz_status comm_finish_setup(frz_comm* c, bool slices) {
         if (c->world > 1) {
             FRZ_CUDA_TRY(cudaHostGetDevicePointer(&dp, c->tables.ptr, 0));
             r.table_dev = reinterpret_cast<uint32_t*>(dp);
-            const size_t entries = (size_t)c->world * kTableBins;
-            FRZ_TRY(r.d_pos0.reserve(entries + entries / 2));   // entries u64 + entries u32 (entries is even)
-            r.d_gt = reinterpret_cast<uint32_t*>(r.d_pos0.get() + entries);
-            FRZ_TRY(r.h_pos0.reserve(entries + entries / 2));
-            r.h_gt = reinterpret_cast<uint32_t*>(r.h_pos0.get() + entries);
+            FRZ_TRY(r.d_tables.reserve(frzmerge::table_row(c->world, kTableBins)));
+            FRZ_TRY(r.h_tables.reserve(frzmerge::table_row(c->world, kTableBins)));
         }
     }
     return FRZ_OK;
@@ -691,14 +651,6 @@ void worker_main(Worker* w, int device) {
 }
 
 // ------------------------------------------------------------------------------------------ one rank's step
-struct StepResult {
-    frz_status status = FRZ_OK;
-    std::string error;
-    uint64_t total = 0;
-    uint64_t kept = 0;      // min(limit, total): the length of the list the call returns
-    const FrzMatchDev* d_merged = nullptr;
-};
-
 // a shard that arrives as HOST Arrow buffers (end-to-end calls): matched while it streams in (host.cu: frz_match_shard_streamed)
 struct HostShard {
     const uint8_t* bytes;
@@ -707,241 +659,248 @@ struct HostShard {
     uint64_t n;
 };
 
-// Everything one GPU does for one match_list_parallel call.  `seq` is the step number shared by all ranks.
-// `want_slices`: the caller only needs the list in host memory (no device copy of the whole merged list): slice exchange allowed.
-// Exactly one of `shard` (resident packed corpus) and `hs` (host buffers) is given.  `limit` (top-K calls, resident shards only):
-// only the first K' = min(limit, total) positions of the merged list are produced; UINT64_MAX for the whole list.
-frz_status rank_step(frz_comm* c, RankCtx& r, frz_matcher* m, const frz_corpus* shard, const HostShard* hs, uint32_t index_offset, uint64_t seq,
-                     frz_match* out_host, uint64_t cap, bool want_host, bool want_slices, uint64_t limit, StepResult* res) {
+// One rank's step of one call.  The entry point sets the call's arguments: `want_slices` = the caller only needs the list in
+// host memory, so the host-out exchange forms may run; `limit` (top-K calls, resident shards only) = only the first
+// K' = min(limit, total) merged positions are produced, UINT64_MAX for the whole list.  rank_step fills in the rest.
+struct Step {
+    frz_matcher* m;
+    frz_match* out_host;
+    uint64_t cap;
+    bool want_host, want_slices;
+    uint64_t limit;
+    frz_comm* c;
+    RankCtx* r;
+    uint64_t seq;
+    int world, parity;
+    cudaStream_t main;              // the device's legacy default stream: ordered with the caller's own work
+    uint64_t counts[kMaxWorld];
+    uint64_t kept[kMaxWorld];       // the part of run q the merge can need: its first min(limit, n_q) elements
+    uint64_t stride, total, kept_total;
+    uint64_t kp;                    // K': the positions of the merged list this call produces
+    uint64_t lo[kMaxWorld + 1];     // slice boundaries: rank p copies [lo[p], lo[p + 1]) of the merged list out
+    bool by_score, reversed;
+    int bins;                       // of the runs' score tables (1 when the runs are not ordered by score)
+    const volatile uint32_t* gt;    // every rank's published score table (kTableBins apart), or null without them
+    const FrzMatchDev* d_part;      // what an exchange form leaves: the merged list, or in the host-out forms its slice lo[rank]..
+    const FrzMatchDev* d_merged;    // the result: the device copy of the whole merged list, if there is one
+    frz_status status;
+    std::string error;
+};
+
+// P2P placement (k_place): only this rank's table row is needed
+frz_status place_p2p(Step& st) {
+    RankCtx& r = *st.r;
+    const size_t row = frzmerge::table_row(r.rank, st.bins);
+    frzmerge::plan_tables(st.world, st.bins, st.reversed, st.gt, kTableBins, st.counts, r.rank, r.h_tables.get(), st.lo, st.world, nullptr);
+    FRZ_CUDA_TRY(cudaMemcpyAsync(r.d_tables.get() + row, r.h_tables.get() + row, (size_t)2 * st.bins * sizeof(uint32_t), cudaMemcpyHostToDevice, st.main));
+    PlaceMeta meta{};
+    memcpy(meta.peer, r.peer_raw, sizeof meta.peer);
+    memcpy(meta.lo, st.lo, sizeof meta.lo);
+    meta.total = st.kp; meta.world = st.world; meta.rank = r.rank; meta.bins = st.bins; meta.parity = st.parity;
+    const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((st.kept[r.rank] + 255) / 256, (uint64_t)frz_sm_count() * 4));
+    const uint32_t* d_row = r.d_tables.get() + row;
+    k_place<<<grid, 256, 0, st.main>>>(r.run.get(), st.kept[r.rank], meta, d_row, d_row + st.bins, st.seq, (unsigned long long)(poll_timeout_s() * 1e9),
+                                       reinterpret_cast<volatile unsigned long long*>(r.ctrl_dev + kCtrlPlaceErr + r.rank));
+    FRZ_CUDA_TRY(cudaGetLastError());
+    st.d_part = reinterpret_cast<const FrzMatchDev*>(r.place_raw.get() + kPlaceHeaderBytes);
+    return FRZ_OK;
+}
+
+// Slice exchange: ONE grouped ncclSend/ncclRecv moves exactly the ranges of the runs every rank copies out (1/G of the
+// all-gather's bytes), then the merge's scatter over the received pieces builds this rank's slice
+frz_status exchange_slices(Step& st) {
+    RankCtx& r = *st.r;
+    const int world = st.world, me = r.rank;
+    static thread_local std::vector<uint64_t> A;   // [q][p]: elements of run q before lo[p]
+    A.assign((size_t)world * (world + 1), 0);
+    frzmerge::plan_tables(world, st.bins, st.reversed, st.gt, kTableBins, st.counts, -1, r.h_tables.get(), st.lo, world, A.data());
+    const uint64_t lo = st.lo[me], mine = st.lo[me + 1] - lo;
+    FRZ_TRY(r.gathered.reserve(std::max<uint64_t>(mine, 1), mine + mine / 4 + 1024));
+    FRZ_TRY(r.merged.reserve(std::max<uint64_t>(mine, 1), mine + mine / 4 + 1024));
+    FrzMergePieces pieces{};
+    pieces.lo = (uint32_t)lo;
+    uint64_t off = 0;
+    for (int q = 0; q < world; q++) {
+        const uint64_t a = A[(size_t)q * (world + 1) + me], b = A[(size_t)q * (world + 1) + me + 1];
+        pieces.src[q] = off; pieces.n[q] = (uint32_t)(b - a); pieces.a[q] = (uint32_t)a;
+        off += b - a;
+    }
+    if (off != mine) return frz_fail(FRZ_ERR_NCCL, "slice exchange: the ranks' score tables are inconsistent (%llu != %llu)",
+                                     (unsigned long long)off, (unsigned long long)mine);
+    FRZ_CUDA_TRY(cudaMemcpyAsync(r.d_tables.get(), r.h_tables.get(), frzmerge::table_row(world, st.bins) * sizeof(uint32_t), cudaMemcpyHostToDevice,
+                                 st.main));
+    FRZ_NCCL_TRY(nccl_api().GroupStart());
+    for (int p = 0; p < world; p++) {
+        const uint64_t a = A[(size_t)me * (world + 1) + p], b = A[(size_t)me * (world + 1) + p + 1];
+        if (b > a) FRZ_NCCL_TRY(nccl_api().Send(r.run.get() + a, (size_t)(b - a), ncclUint64, p, r.nccl, st.main));
+    }
+    for (int q = 0; q < world; q++)
+        if (pieces.n[q]) FRZ_NCCL_TRY(nccl_api().Recv(r.gathered.get() + pieces.src[q], (size_t)pieces.n[q], ncclUint64, q, r.nccl, st.main));
+    FRZ_NCCL_TRY(nccl_api().GroupEnd());
+    FRZ_TRY(frz_launch_merge_scatter(r.gathered.get(), pieces, world, r.d_tables.get(), st.bins, 4, r.merged.get(), st.main));
+    st.d_part = r.merged.get();
+    return FRZ_OK;
+}
+
+// All-gather + merge: ONE ncclAllGather of the runs, padded to the longest, then the k-way merge of their kept prefixes
+frz_status gather_and_merge(Step& st) {
+    RankCtx& r = *st.r;
+    if (r.run.cap() < st.stride) {
+        // another rank's run is longer than this rank's whole shard (ceil partitioning leaves the last shard short, or
+        // empty): the all-gather reads `stride` elements from every rank, so move the run into a buffer that long
+        FrzDevArray<FrzMatchDev> bigger;
+        FRZ_TRY(bigger.reserve(st.stride));
+        FRZ_CUDA_TRY(cudaMemcpyAsync(bigger.get(), r.run.get(), st.kept[r.rank] * sizeof(FrzMatchDev), cudaMemcpyDeviceToDevice, st.main));
+        FRZ_CUDA_TRY(cudaStreamSynchronize(st.main));
+        r.run = std::move(bigger);
+    }
+    const uint64_t need = (uint64_t)st.world * st.stride;
+    FRZ_TRY(r.gathered.reserve(need, need + need / 4 + 1024));
+    FRZ_TRY(r.merged.reserve(st.kept_total, st.kept_total + st.kept_total / 4 + 1024));
+    if (r.nccl) {
+        FRZ_NCCL_TRY(nccl_api().AllGather(r.run.get(), r.gathered.get(), (size_t)st.stride, ncclUint64, r.nccl, st.main));
+    } else {   // world 1 without a communicator (local form + force flag): the gather of one run is a copy
+        FRZ_CUDA_TRY(cudaMemcpyAsync(r.gathered.get(), r.run.get(), st.stride * sizeof(FrzMatchDev), cudaMemcpyDeviceToDevice, st.main));
+    }
+    FRZ_TRY(frz_merge_runs_ex(r.merge, r.gathered.get(), st.stride, st.kept, st.world, frz_matcher_sort(st.m), frz_matcher_score_bound(st.m),
+                              r.merged.get(), st.main));
+    st.d_part = r.merged.get();
+    return FRZ_OK;
+}
+
+// Everything one GPU does for one match_list_parallel call.  `seq` is the step number shared by all ranks.  Exactly one of
+// `shard` (resident packed corpus) and `hs` (host buffers) is given.
+frz_status rank_step(frz_comm* c, RankCtx& r, Step& st, const frz_corpus* shard, const HostShard* hs, uint32_t index_offset, uint64_t seq) {
     FRZ_TRY(frz_ensure_device(r.device));
-    cudaStream_t main = nullptr;   // the device's legacy default stream: ordered with the caller's own default-stream work
-    const int world = c->world;
-    const int parity = (int)(seq & 1);
-    if (!m || (!shard && !hs)) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    st.c = c; st.r = &r; st.seq = seq; st.world = c->world; st.parity = (int)(seq & 1); st.main = nullptr;
+    if (!st.m || (!shard && !hs)) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
     if (shard && frz_corpus_device(shard) != r.device)
         return frz_fail(FRZ_ERR_INVALID_ARG, "shard of rank %d lives on device %d, the communicator expects device %d", r.rank,
                         frz_corpus_device(shard), r.device);
-    FRZ_TRY(refresh_clone(r, m));
+    FRZ_TRY(refresh_clone(r, st.m));
     const uint64_t n_local = hs ? hs->n : frz_corpus_len(shard);
     FRZ_TRY(r.run.reserve(std::max<uint64_t>(n_local, 1)));
-    FRZ_CUDA_TRY(cudaEventRecord(r.ev[0].get(), main));
+    FRZ_CUDA_TRY(cudaEventRecord(r.ev[0].get(), st.main));
     // ---- local pipeline (asynchronous): prefilter → count published → scoring → local order
     if (hs)
         FRZ_TRY(frz_match_shard_streamed(r.clone, hs->bytes, hs->offsets, hs->offset_width, hs->n, r.device, index_offset,
-                                         reinterpret_cast<frz_match*>(r.run.get()), r.run.cap(), reinterpret_cast<uint64_t*>(r.d_count.get()), main));
+                                         reinterpret_cast<frz_match*>(r.run.get()), r.run.cap(), reinterpret_cast<uint64_t*>(r.d_count.get()), st.main));
     else
         FRZ_TRY(frz_match_shard_device_top(r.clone, shard, index_offset, reinterpret_cast<frz_match*>(r.run.get()), r.run.cap(),
-                                           reinterpret_cast<uint64_t*>(r.d_count.get()), main, (uint32_t)std::min<uint64_t>(limit, kFrzNoLimit)));
+                                           reinterpret_cast<uint64_t*>(r.d_count.get()), st.main, (uint32_t)std::min<uint64_t>(st.limit, kFrzNoLimit)));
     FRZ_TRY(frz_matcher_wait_count(r.clone, r.side.get()));
-    k_publish<<<1, 1, 0, r.side.get()>>>(reinterpret_cast<volatile unsigned long long*>(r.ctrl_dev + kCtrlCount + parity * kMaxWorld + r.rank),
+    k_publish<<<1, 1, 0, r.side.get()>>>(reinterpret_cast<volatile unsigned long long*>(r.ctrl_dev + kCtrlCount + st.parity * kMaxWorld + r.rank),
                                          r.d_count.get(), seq);
     FRZ_CUDA_TRY(cudaGetLastError());
-    FRZ_CUDA_TRY(cudaEventRecord(r.ev[1].get(), main));
+    FRZ_CUDA_TRY(cudaEventRecord(r.ev[1].get(), st.main));
     // ---- the Vec lengths of all workers (k_merge.rs:96-104): polled from the shared block while the GPU scores
-    uint64_t counts[kMaxWorld];
-    FRZ_TRY(wait_slots(c->ctrl_host + kCtrlCount + parity * kMaxWorld, world, seq, counts, "match count"));
-    // kept[q]: the part of run q the merge can need — its first min(limit, n_q) elements (all of them for a full call)
-    uint64_t kept[kMaxWorld], stride = 1, total = 0, kept_total = 0;
-    for (int k = 0; k < world; k++) {
-        kept[k] = std::min(counts[k], limit);
-        stride = std::max(stride, kept[k]);
-        total += counts[k];
-        kept_total += kept[k];
+    FRZ_TRY(wait_slots(c->ctrl_host + kCtrlCount + st.parity * kMaxWorld, st.world, seq, st.counts, "match count"));
+    st.stride = 1; st.total = 0; st.kept_total = 0;
+    for (int q = 0; q < st.world; q++) {
+        st.kept[q] = std::min(st.counts[q], st.limit);
+        st.stride = std::max(st.stride, st.kept[q]);
+        st.total += st.counts[q];
+        st.kept_total += st.kept[q];
     }
-    const uint64_t kp = std::min(total, limit);   // K': positions of the merged list this call produces
-    res->total = total;
-    res->kept = kp;
-    const bool collective = world > 1 || c->force_nccl;
-    const FrzMatchDev* d_final = r.run.get();
-    uint64_t d_final_first = 0;   // merged position of d_final[0] (non-zero in the slice form)
-    bool placed = false;          // the P2P placement ran this step
-    // ---- host-out calls: SLICE EXCHANGE.  A rank copies only its slice [lo, hi) of the merged list to the host, and the
-    // elements of run q that land in that slice are ONE contiguous range of run q (a run's elements keep their order in the
-    // merged list).  With every rank's per-score table (published like the counts) each rank computes those ranges on the
-    // host and ONE grouped ncclSend/ncclRecv moves exactly them: 1/G of the all-gather's bytes and 1/G of its merge work.
-    const uint8_t sort_mode = frz_matcher_sort(m);
-    const bool by_score = (sort_mode == FRZ_SORT_SCORE_THEN_INDEX_ASC || sort_mode == FRZ_SORT_SCORE_THEN_INDEX_DESC) &&
-                          frz_matcher_num_patterns(m) > 0;
-    const bool reversed = sort_mode == FRZ_SORT_INDEX_DESC || sort_mode == FRZ_SORT_SCORE_THEN_INDEX_DESC;
-    int bins = 1;
-    const uint32_t* d_table = nullptr;
-    if (by_score) d_table = frz_matcher_last_sort_table(r.clone, &bins);
-    const bool slice_form = want_host && want_slices && world > 1 && r.nccl && (!by_score || bins > 0) && kp > 0 &&
-                            total <= 0xFFFFFFFFull;
-    if (slice_form) {
-        if (kp > cap) {
-            FRZ_CUDA_TRY(cudaStreamSynchronize(main));
-            return frz_fail(FRZ_ERR_CAPACITY, "output capacity %llu < %llu matches", (unsigned long long)cap, (unsigned long long)kp);
+    st.kp = std::min(st.total, st.limit);
+    for (int p = 0; p <= st.world; p++) st.lo[p] = frzmerge::slice_lo(st.kp, p, st.world);
+    if (st.want_host) {   // every rank sees the same counts, so every rank takes this exit: no collective is left unbalanced
+        if (st.kp > st.cap) {
+            FRZ_CUDA_TRY(cudaStreamSynchronize(st.main));
+            return frz_fail(FRZ_ERR_CAPACITY, "output capacity %llu < %llu matches", (unsigned long long)st.cap, (unsigned long long)st.kp);
         }
-        if (!out_host) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
-        // the slice buffers of the P2P placement (collective, grow-only), else the NCCL slice exchange
-        bool place_ready = false;
-        FRZ_TRY(ensure_place_buffers(c, r, kp / (uint64_t)world + 2, &place_ready));
-        // 1. my table → shared block (after the local pipeline on the main stream), everybody's tables ← shared block
-        volatile uint32_t* tab_host = c->tables_host + ((size_t)parity * world) * kTableBins;
-        if (by_score) {
-            // the table is final one kernel before the run (after the sort's scan, before its scatter): publish it from the side
-            // stream at that point, so the tables cross the host block — and the host prepares the exchange — while the scatter runs
-            cudaStream_t pub = main;
+        if (st.kp && !st.out_host) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
+    }
+    const uint8_t sort_mode = frz_matcher_sort(st.m);
+    st.by_score = (sort_mode == FRZ_SORT_SCORE_THEN_INDEX_ASC || sort_mode == FRZ_SORT_SCORE_THEN_INDEX_DESC) && frz_matcher_num_patterns(st.m) > 0;
+    st.reversed = sort_mode == FRZ_SORT_INDEX_DESC || sort_mode == FRZ_SORT_SCORE_THEN_INDEX_DESC;
+    st.bins = 1;
+    const uint32_t* d_table = st.by_score ? frz_matcher_last_sort_table(r.clone, &st.bins) : nullptr;
+    // ---- the exchange (see the top of this file)
+    const bool host_out_form = st.want_host && st.want_slices && st.world > 1 && r.nccl && (!st.by_score || st.bins > 0) && st.kp > 0 &&
+                               st.total <= 0xFFFFFFFFull;
+    st.d_part = r.run.get();
+    bool placed = false;   // k_place ran this step
+    if (host_out_form) {
+        FRZ_TRY(ensure_place_buffers(c, r, st.kp / (uint64_t)st.world + 2, &placed));   // collective: every rank takes the same form
+        if (st.by_score) {
+            // my table → the shared block, then everybody's.  The table is final one kernel before the run (after the sort's
+            // scan, before its scatter): publish it from the side stream at that point, so the tables cross the host block —
+            // and the host prepares the exchange — while the scatter runs
+            cudaStream_t pub = st.main;
             if (cudaEvent_t tev = frz_matcher_table_event(r.clone)) {
                 FRZ_CUDA_TRY(cudaStreamWaitEvent(r.side.get(), tev, 0));
                 pub = r.side.get();
             }
-            k_publish_table<<<1, 256, 0, pub>>>(r.table_dev + ((size_t)parity * world + r.rank) * kTableBins, d_table, bins,
-                                                reinterpret_cast<volatile unsigned long long*>(r.ctrl_dev + kCtrlTable + parity * kMaxWorld + r.rank), seq);
+            k_publish_table<<<1, 256, 0, pub>>>(r.table_dev + ((size_t)st.parity * st.world + r.rank) * kTableBins, d_table, st.bins,
+                                                reinterpret_cast<volatile unsigned long long*>(r.ctrl_dev + kCtrlTable + st.parity * kMaxWorld + r.rank), seq);
             FRZ_CUDA_TRY(cudaGetLastError());
-            FRZ_TRY(wait_slots(c->ctrl_host + kCtrlTable + parity * kMaxWorld, world, seq, nullptr, "score table"));
+            FRZ_TRY(wait_slots(c->ctrl_host + kCtrlTable + st.parity * kMaxWorld, st.world, seq, nullptr, "score table"));
+            st.gt = c->tables_host + (size_t)st.parity * st.world * kTableBins;
         }
-        // 2. merged positions: pos0[q][s] = everything scoring higher than s in any run + the score-s blocks of the runs
-        //    that precede q in merge order; A[q][p] = how many elements of run q lie before slice boundary lo_p
-        uint64_t lo_p[kMaxWorld + 1];
-        for (int p2 = 0; p2 <= world; p2++) lo_p[p2] = kp * (uint64_t)p2 / (uint64_t)world;
-      if (place_ready) {
-        // ---- P2P PLACEMENT: only MY run's rows of pos0 / gt are needed; k_place stores every element of my run at its merged
-        // position inside the owning rank's slice buffer (peer memory over NVLink) and ends when all peers have done the same
-        auto gt_at = [&](int q, int sc) -> uint64_t { return by_score ? (uint64_t)tab_host[(size_t)q * kTableBins + sc] : 0ull; };
-        uint64_t* hp = reinterpret_cast<uint64_t*>(r.h_pos0.get());
-        uint32_t* hg = reinterpret_cast<uint32_t*>(hp + bins);
-        for (int sc = bins - 1; sc >= 0; sc--) {
-            uint64_t acc = 0;
-            for (int q = 0; q < world; q++) acc += gt_at(q, sc);
-            for (int k = 0; k < world; k++) {
-                const int q = reversed ? world - 1 - k : k;
-                const uint64_t gtq = gt_at(q, sc);
-                if (q == r.rank) { hp[sc] = acc; hg[sc] = (uint32_t)gtq; break; }
-                acc += (sc == 0 ? counts[q] : gt_at(q, sc - 1)) - gtq;
-            }
-        }
-        FRZ_CUDA_TRY(cudaMemcpyAsync(r.d_pos0.get(), r.h_pos0.get(), (size_t)bins * (sizeof(uint64_t) + sizeof(uint32_t)), cudaMemcpyHostToDevice, main));
-        PlaceMeta meta;
-        memset(&meta, 0, sizeof meta);
-        for (int q = 0; q < world; q++) meta.peer[q] = r.peer_raw[q];
-        for (int p2 = 0; p2 <= world; p2++) meta.lo[p2] = lo_p[p2];
-        meta.total = kp; meta.world = world; meta.rank = r.rank; meta.bins = bins; meta.parity = parity;
-        const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>((kept[r.rank] + 255) / 256, (uint64_t)frz_sm_count() * 4));
-        k_place<<<grid, 256, 0, main>>>(r.run.get(), kept[r.rank], meta, r.d_pos0.get(), reinterpret_cast<const uint32_t*>(r.d_pos0.get() + bins), seq, (unsigned long long)(poll_timeout_s() * 1e9),
-                                         reinterpret_cast<volatile unsigned long long*>(r.ctrl_dev + kCtrlPlaceErr + r.rank));
-        FRZ_CUDA_TRY(cudaGetLastError());
-        placed = true;
-        d_final = reinterpret_cast<const FrzMatchDev*>(r.place_raw.get() + kPlaceHeaderBytes);
-        d_final_first = lo_p[r.rank];
-      } else {
-        static thread_local std::vector<uint64_t> A;
-        A.assign((size_t)world * (world + 1), 0);
-        auto gt_of = [&](int q, int sc) -> uint64_t { return by_score ? (uint64_t)tab_host[(size_t)q * kTableBins + sc] : 0ull; };
-        for (int sc = bins - 1; sc >= 0; sc--) {
-            uint64_t higher = 0;
-            for (int q = 0; q < world; q++) higher += gt_of(q, sc);
-            uint64_t acc = higher;
-            for (int k = 0; k < world; k++) {
-                const int q = reversed ? world - 1 - k : k;
-                const uint64_t gtq = gt_of(q, sc);
-                const uint64_t ge = sc == 0 ? counts[q] : gt_of(q, sc - 1);
-                const uint64_t size = ge - gtq;
-                r.h_pos0.get()[(size_t)q * bins + sc] = acc;
-                r.h_gt[(size_t)q * bins + sc] = (uint32_t)gtq;
-                if (size) {
-                    for (int p2 = 0; p2 <= world; p2++) {
-                        const uint64_t b = lo_p[p2];
-                        if (b > acc) A[(size_t)q * (world + 1) + p2] += std::min<uint64_t>(b - acc, size);
-                    }
-                }
-                acc += size;
-            }
-        }
-        // 3. ONE grouped exchange: to every rank p the part of my run it needs, from every run q the part I need
-        const uint64_t lo = lo_p[r.rank], hi = lo_p[r.rank + 1];
-        const uint64_t mine = hi - lo;
-        FRZ_TRY(r.recv.reserve(std::max<uint64_t>(mine, 1), mine + mine / 4 + 1024));
-        FRZ_TRY(r.merged.reserve(std::max<uint64_t>(mine, 1), mine + mine / 4 + 1024));
-        SliceMeta meta;
-        memset(&meta, 0, sizeof meta);
-        meta.lo = lo;
-        uint64_t off = 0, longest = 0;
-        for (int q = 0; q < world; q++) {
-            const uint64_t a = A[(size_t)q * (world + 1) + r.rank], b = A[(size_t)q * (world + 1) + r.rank + 1];
-            meta.off[q] = (uint32_t)off; meta.n[q] = (uint32_t)(b - a); meta.a[q] = (uint32_t)a;
-            off += b - a;
-            longest = std::max(longest, b - a);
-        }
-        if (off != mine) return frz_fail(FRZ_ERR_NCCL, "slice exchange: the ranks' score tables are inconsistent (%llu != %llu)",
-                                         (unsigned long long)off, (unsigned long long)mine);
-        FRZ_CUDA_TRY(cudaMemcpyAsync(r.d_pos0.get(), r.h_pos0.get(), (size_t)world * kTableBins * (sizeof(unsigned long long) + sizeof(uint32_t)),
-                                     cudaMemcpyHostToDevice, main));   // pos0 and gt in one copy (fixed layout, <= 96 KB)
-        FRZ_NCCL_TRY(nccl_api().GroupStart());
-        for (int p2 = 0; p2 < world; p2++) {
-            const uint64_t a = A[(size_t)r.rank * (world + 1) + p2], b = A[(size_t)r.rank * (world + 1) + p2 + 1];
-            if (b > a) FRZ_NCCL_TRY(nccl_api().Send(r.run.get() + a, (size_t)(b - a), ncclUint64, p2, r.nccl, main));
-        }
-        for (int q = 0; q < world; q++)
-            if (meta.n[q]) FRZ_NCCL_TRY(nccl_api().Recv(r.recv.get() + meta.off[q], (size_t)meta.n[q], ncclUint64, q, r.nccl, main));
-        FRZ_NCCL_TRY(nccl_api().GroupEnd());
-        // 4. my slice of the k-way merge
-        if (mine) {
-            const dim3 grid((unsigned)std::max<uint64_t>(1, std::min<uint64_t>((longest + 255) / 256, frz_sm_count() * 4 / world + 1)), (unsigned)world);
-            k_slice_scatter<<<grid, 256, 0, main>>>(r.recv.get(), meta, r.d_gt, r.d_pos0.get(), bins, r.merged.get());
-            FRZ_CUDA_TRY(cudaGetLastError());
-        }
-        d_final = r.merged.get();
-        d_final_first = lo;
-      }
-    } else if (collective) {
-        if (r.run.cap() < stride) {
-            // another rank's run is longer than this rank's whole shard (ceil partitioning leaves the last shard short, or
-            // empty): the all-gather reads `stride` elements from every rank, so move the run into a buffer that long
-            FrzDevArray<FrzMatchDev> bigger;
-            FRZ_TRY(bigger.reserve(stride));
-            FRZ_CUDA_TRY(cudaMemcpyAsync(bigger.get(), r.run.get(), kept[r.rank] * sizeof(FrzMatchDev), cudaMemcpyDeviceToDevice, main));
-            FRZ_CUDA_TRY(cudaStreamSynchronize(main));
-            r.run = std::move(bigger);
-        }
-        const uint64_t need = (uint64_t)world * stride;
-        FRZ_TRY(r.gathered.reserve(need, need + need / 4 + 1024));
-        FRZ_TRY(r.merged.reserve(kept_total, kept_total + kept_total / 4 + 1024));
-        // ---- THE collective: one all-gather of the per-shard (score, index) runs over NVLink
-        if (r.nccl) {
-            FRZ_NCCL_TRY(nccl_api().AllGather(r.run.get(), r.gathered.get(), (size_t)stride, ncclUint64, r.nccl, main));
-        } else {   // world 1 without a communicator (local form + force flag): the gather of one run is a copy
-            FRZ_CUDA_TRY(cudaMemcpyAsync(r.gathered.get(), r.run.get(), stride * sizeof(FrzMatchDev), cudaMemcpyDeviceToDevice, main));
-        }
-        // ---- k_merge_matches_by on this GPU (of the runs' kept prefixes: the merged list's first K' are the same)
-        FRZ_TRY(frz_merge_runs_ex(r.merge, r.gathered.get(), stride, kept, world, frz_matcher_sort(m), frz_matcher_score_bound(m),
-                                  r.merged.get(), main));
-        d_final = r.merged.get();
+        FRZ_TRY(placed ? place_p2p(st) : exchange_slices(st));
+    } else if (st.world > 1 || c->force_nccl) {
+        FRZ_TRY(gather_and_merge(st));
     }
-    res->d_merged = slice_form ? nullptr : d_final;
-    FRZ_CUDA_TRY(cudaEventRecord(r.ev[2].get(), main));
-    if (want_host) {
-        if (kp > cap) {   // every rank sees the same counts, so every rank takes this exit: no collective is left unbalanced
-            FRZ_CUDA_TRY(cudaStreamSynchronize(main));
-            return frz_fail(FRZ_ERR_CAPACITY, "output capacity %llu < %llu matches", (unsigned long long)cap, (unsigned long long)kp);
-        }
-        if (kp && !out_host) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
-        // this rank's slice of the merged list → host (all ranks hold the whole list: the copy uses every PCIe link)
-        const uint64_t lo = kp * (uint64_t)r.rank / (uint64_t)world, hi = kp * (uint64_t)(r.rank + 1) / (uint64_t)world;
-        if (hi > lo)
-            FRZ_CUDA_TRY(cudaMemcpyAsync(out_host + lo, d_final + (lo - d_final_first), (hi - lo) * sizeof(FrzMatchDev), cudaMemcpyDeviceToHost, main));
-    }
-    FRZ_CUDA_TRY(cudaEventRecord(r.ev[3].get(), main));
+    st.d_merged = host_out_form ? nullptr : st.d_part;
+    FRZ_CUDA_TRY(cudaEventRecord(r.ev[2].get(), st.main));
+    // ---- this rank's slice of the merged list → host (all ranks hold their slice: the copy uses every PCIe link)
+    const uint64_t lo = st.lo[r.rank], hi = st.lo[r.rank + 1];
+    if (st.want_host && hi > lo)
+        FRZ_CUDA_TRY(cudaMemcpyAsync(st.out_host + lo, (host_out_form ? st.d_part : st.d_part + lo), (hi - lo) * sizeof(FrzMatchDev), cudaMemcpyDeviceToHost, st.main));
+    FRZ_CUDA_TRY(cudaEventRecord(r.ev[3].get(), st.main));
     r.ev_valid = true;
-    if (want_host && !c->local_form && world > 1) {
+    const bool done_flags = st.want_host && !c->local_form && st.world > 1;
+    if (done_flags) {
         // "my slice has landed", stream-ordered after the copy; the call returns once every rank has said so
-        k_publish<<<1, 1, 0, main>>>(reinterpret_cast<volatile unsigned long long*>(r.ctrl_dev + kCtrlDone + parity * kMaxWorld + r.rank), nullptr, seq);
+        k_publish<<<1, 1, 0, st.main>>>(reinterpret_cast<volatile unsigned long long*>(r.ctrl_dev + kCtrlDone + st.parity * kMaxWorld + r.rank), nullptr, seq);
         FRZ_CUDA_TRY(cudaGetLastError());
     }
-    FRZ_CUDA_TRY(cudaStreamSynchronize(main));
+    FRZ_CUDA_TRY(cudaStreamSynchronize(st.main));
     if (placed && __atomic_load_n(const_cast<const uint64_t*>(c->ctrl_host + kCtrlPlaceErr + r.rank), __ATOMIC_ACQUIRE) == seq)
         return frz_fail(FRZ_ERR_NCCL, "rank %d: a peer GPU did not place its matches within %.0f s (peer failed or ranks made different calls)",
                         r.rank, poll_timeout_s());
-    if (want_host && !c->local_form && world > 1)
-        FRZ_TRY(wait_slots(c->ctrl_host + kCtrlDone + parity * kMaxWorld, world, seq, nullptr, "copy-out flag"));
+    if (done_flags) FRZ_TRY(wait_slots(c->ctrl_host + kCtrlDone + st.parity * kMaxWorld, st.world, seq, nullptr, "copy-out flag"));
     return FRZ_OK;
 }
 
-void run_job(frz_comm* c, RankCtx& r, frz_matcher* m, const frz_corpus* shard, uint32_t offset, uint64_t seq, frz_match* out,
-             uint64_t cap, bool want_host, uint64_t limit, StepResult* res) {
-    res->status = rank_step(c, r, m, shard, nullptr, offset, seq, out, cap, want_host, true, limit, res);
-    if (res->status != FRZ_OK) res->error = frz_last_error();
+// One collective call after the entry point's argument checks: lock, step number, the step on every rank this process drives
+// (local rank g: shards[g] from index offsets[g], or hs) and the results.  The errors of a local call name the GPU.
+frz_status parallel_call(frz_comm* c, const Step& call, const frz_corpus* const* shards, const HostShard* hs, const uint32_t* offsets,
+                         bool local_call, uint64_t* n_out, uint64_t* n_total, const frz_match** d_out) {
+    std::lock_guard<std::mutex> lock(c->mu);
+    const uint64_t seq = ++c->seq;
+    std::vector<Step> res(c->ranks.size(), call);
+    auto run = [&](int g) {
+        res[g].status = rank_step(c, c->ranks[g], res[g], shards ? shards[g] : nullptr, hs, offsets[g], seq);
+        if (res[g].status != FRZ_OK) res[g].error = frz_last_error();
+    };
+    if (c->workers.empty()) {
+        run(0);
+    } else {
+        for (size_t g = 0; g < c->workers.size(); g++) {
+            Worker* w = c->workers[g].get();
+            {
+                std::lock_guard<std::mutex> lk(w->mu);
+                w->job = [&run, g] { run((int)g); };
+                w->done = false;
+                w->has_job = true;
+            }
+            w->cv.notify_all();
+        }
+        for (auto& wp : c->workers) {
+            Worker* w = wp.get();
+            std::unique_lock<std::mutex> lk(w->mu);
+            w->cv.wait(lk, [&] { return w->done; });
+        }
+    }
+    if (n_out) *n_out = res[0].kp;
+    if (n_total) *n_total = res[0].total;
+    if (d_out) *d_out = reinterpret_cast<const frz_match*>(res[0].d_merged);
+    if (!local_call) return res[0].status;
+    for (size_t g = 0; g < res.size(); g++)
+        if (res[g].status != FRZ_OK) return frz_fail(res[g].status, "GPU %d: %s", c->ranks[g].device, res[g].error.c_str());
+    return FRZ_OK;
 }
 
 }  // namespace
@@ -1100,42 +1059,15 @@ frz_status match_list_parallel_local(frz_matcher* m, const frz_corpus* const* sh
     if (!m || !c || !shards) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
     if (!c->local_form) return frz_fail(FRZ_ERR_INVALID_ARG, "multi-process communicator: call frz_match_list_parallel_rank on every rank");
     if (n_shards != c->world) return frz_fail(FRZ_ERR_INVALID_ARG, "%d shards for a communicator of %d GPUs", n_shards, c->world);
-    std::lock_guard<std::mutex> lock(c->mu);
-    uint64_t offs[kMaxWorld], total_items = 0;
+    uint32_t offs[kMaxWorld];
+    uint64_t total_items = 0;
     for (int g = 0; g < n_shards; g++) {
         if (!shards[g]) return frz_fail(FRZ_ERR_INVALID_ARG, "null shard %d", g);
-        offs[g] = total_items;
+        offs[g] = (uint32_t)total_items;
         total_items += frz_corpus_len(shards[g]);
     }
     FRZ_TRY(frz_check_index_range(total_items, 0));
-    const uint64_t seq = ++c->seq;
-    std::vector<StepResult> res(c->world);
-    if (c->world == 1) {
-        run_job(c, c->ranks[0], m, shards[0], 0, seq, out, cap, true, limit, &res[0]);
-    } else {
-        for (int g = 0; g < c->world; g++) {
-            Worker* w = c->workers[g].get();
-            {
-                std::lock_guard<std::mutex> lk(w->mu);
-                w->job = [c, g, m, shards, &offs, seq, out, cap, limit, &res] {
-                    run_job(c, c->ranks[g], m, shards[g], (uint32_t)offs[g], seq, out, cap, true, limit, &res[g]);
-                };
-                w->done = false;
-                w->has_job = true;
-            }
-            w->cv.notify_all();
-        }
-        for (int g = 0; g < c->world; g++) {
-            Worker* w = c->workers[g].get();
-            std::unique_lock<std::mutex> lk(w->mu);
-            w->cv.wait(lk, [&] { return w->done; });
-        }
-    }
-    if (n_out) *n_out = limit == UINT64_MAX ? res[0].total : res[0].kept;
-    if (n_total) *n_total = res[0].total;
-    for (int g = 0; g < c->world; g++)
-        if (res[g].status != FRZ_OK) return frz_fail(res[g].status, "GPU %d: %s", c->ranks[g].device, res[g].error.c_str());
-    return FRZ_OK;
+    return parallel_call(c, Step{m, out, cap, true, true, limit}, shards, nullptr, offs, true, n_out, n_total, nullptr);
 }
 }  // namespace
 
@@ -1156,14 +1088,8 @@ extern "C" frz_status frz_match_list_parallel_rank(frz_matcher* m, const frz_cor
     if (!m || !c || !shard) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
     if (c->local_form && c->world != 1) return frz_fail(FRZ_ERR_INVALID_ARG, "local communicator: call frz_match_list_parallel");
     FRZ_TRY(frz_check_index_range(frz_corpus_len(shard), index_offset));
-    std::lock_guard<std::mutex> lock(c->mu);
-    const uint64_t seq = ++c->seq;
-    StepResult res;
-    const bool want_host = out != nullptr || cap != 0;
-    const frz_status s = rank_step(c, c->ranks[0], m, shard, nullptr, index_offset, seq, out, cap, want_host, d_out == nullptr, UINT64_MAX, &res);
-    if (n_out) *n_out = res.total;
-    if (d_out) *d_out = reinterpret_cast<const frz_match*>(res.d_merged);
-    return s;
+    const Step a{m, out, cap, out != nullptr || cap != 0, d_out == nullptr, UINT64_MAX};
+    return parallel_call(c, a, &shard, nullptr, &index_offset, false, n_out, nullptr, d_out);
 }
 
 // one rank of match_list_parallel followed by truncation to the first k rows; `out`: the shared segment (room for k), or NULL
@@ -1172,14 +1098,8 @@ extern "C" frz_status frz_match_list_parallel_rank_top(frz_matcher* m, const frz
     if (!m || !c || !shard) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
     if (c->local_form && c->world != 1) return frz_fail(FRZ_ERR_INVALID_ARG, "local communicator: call frz_match_list_parallel_top");
     FRZ_TRY(frz_check_index_range(frz_corpus_len(shard), index_offset));
-    std::lock_guard<std::mutex> lock(c->mu);
-    const uint64_t seq = ++c->seq;
-    StepResult res;
-    const frz_status s = rank_step(c, c->ranks[0], m, shard, nullptr, index_offset, seq, out, out ? k : 0, out != nullptr, d_out == nullptr, k, &res);
-    if (n_out) *n_out = res.kept;
-    if (n_total) *n_total = res.total;
-    if (d_out) *d_out = reinterpret_cast<const frz_match*>(res.d_merged);
-    return s;
+    const Step a{m, out, out ? k : 0, out != nullptr, d_out == nullptr, k};
+    return parallel_call(c, a, &shard, nullptr, &index_offset, false, n_out, n_total, d_out);
 }
 
 // End to end on one rank: the shard arrives as HOST Arrow buffers (streamed H2D + pack into the clone's reusable arena),
@@ -1189,17 +1109,9 @@ extern "C" frz_status frz_match_list_parallel_rank_host(frz_matcher* m, const ui
     if (!m || !c || !offsets) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
     if (c->local_form && c->world != 1) return frz_fail(FRZ_ERR_INVALID_ARG, "local communicator: shard with frz_corpus_create_sharded and call frz_match_list_parallel");
     FRZ_TRY(frz_check_index_range(n, index_offset));
-    std::lock_guard<std::mutex> lock(c->mu);
-    RankCtx& r = c->ranks[0];
-    FRZ_TRY(frz_ensure_device(r.device));
-    FRZ_TRY(refresh_clone(r, m));
     FRZ_TRY(frz_check_offset_width(offset_width));
     const HostShard hs{bytes, offsets, offset_width, n};
-    const uint64_t seq = ++c->seq;
-    StepResult res;
-    const frz_status s = rank_step(c, r, m, nullptr, &hs, index_offset, seq, out, cap, true, true, UINT64_MAX, &res);
-    if (n_out) *n_out = res.total;
-    return s;
+    return parallel_call(c, Step{m, out, cap, true, true, UINT64_MAX}, nullptr, &hs, &index_offset, false, n_out, nullptr, nullptr);
 }
 
 extern "C" frz_status frz_comm_last_timings(frz_comm* c, int local_index, float* ms4, const frz_matcher** clone) {

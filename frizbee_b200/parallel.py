@@ -254,8 +254,22 @@ def merge_runs_host(runs: List[np.ndarray], sort: SortStrategy) -> np.ndarray:
     return cat[order]
 
 
+def block_bases(gt: np.ndarray, counts, reverse_runs: bool) -> np.ndarray:
+    """pos0[q][s]: the merged position of the first element of run q's score-s block (csrc/merge_plan.cuh) — everything
+    scoring higher in any run plus the score-s blocks of the runs that precede q in merge order.  gt[q][s]: how many
+    elements of run q score higher than s; counts[q]: run q's length."""
+    gt = np.asarray(gt, dtype=np.int64)
+    ge = np.concatenate([np.asarray(counts, dtype=np.int64)[:, None], gt[:, :-1]], axis=1)   # ge[q][s] = count(score >= s)
+    pos0 = np.zeros_like(gt)
+    acc = gt.sum(axis=0)
+    for q in (range(len(gt) - 1, -1, -1) if reverse_runs else range(len(gt))):
+        pos0[q] = acc
+        acc = acc + ge[q] - gt[q]
+    return pos0
+
+
 def placement_host(runs: List[np.ndarray], sort: SortStrategy, bins: int = 1024, limit: Optional[int] = None) -> List[np.ndarray]:
-    """Host specification of the P2P placement (csrc/parallel.cu: k_place + the position arithmetic of rank_step): from every
+    """Host specification of the P2P placement (csrc/parallel.cu: k_place, csrc/merge_plan.cuh: the position arithmetic): from every
     run's per-score table gt[q][s] (how many elements of run q score higher than s) each rank derives, for ITS run only,
     pos0[s] — the merged position of the first element of its score-s block = everything scoring higher in any run + the
     score-s blocks of the runs that precede it in merge order — and stores element i (score s) at merged position
@@ -281,17 +295,9 @@ def placement_host(runs: List[np.ndarray], sort: SortStrategy, bins: int = 1024,
             sc = np.minimum(r["score"].astype(np.int64), nb - 1)
             hist = np.bincount(sc, minlength=nb)
             gt[q] = hist[::-1].cumsum()[::-1] - hist          # strictly higher
-    ge = np.concatenate([np.asarray(counts, dtype=np.int64)[:, None], gt[:, :-1]], axis=1)   # ge[q][s] = count(score >= s)
-    order = list(range(world))[::-1] if sort.is_reversed() else list(range(world))
+    pos0_all = block_bases(gt, counts, sort.is_reversed())
     for me, r in enumerate(runs):
-        pos0 = np.zeros(nb, dtype=np.int64)
-        for s in range(nb):
-            acc = int(gt[:, s].sum())
-            for q in order:
-                if q == me:
-                    break
-                acc += int(ge[q][s] - gt[q][s])
-            pos0[s] = acc
+        pos0 = pos0_all[me]   # (each rank needs its own row only)
         r = r if limit is None else r[:limit]
         i = np.arange(len(r), dtype=np.int64)
         s_of = np.minimum(r["score"].astype(np.int64), nb - 1) if by_score else np.zeros(len(r), dtype=np.int64)
@@ -326,16 +332,7 @@ def match_list_parallel_placement_gloo(run: np.ndarray, sort: SortStrategy, bins
     counts, gt = tab[:, 0], tab[:, 1:]
     total = int(counts.sum())
     lo = [total * p // world for p in range(world + 1)]
-    ge = np.concatenate([counts[:, None], gt[:, :-1]], axis=1)
-    order = list(range(world))[::-1] if sort.is_reversed() else list(range(world))
-    pos0 = np.zeros(nb, dtype=np.int64)
-    for s in range(nb):
-        acc = int(gt[:, s].sum())
-        for q in order:
-            if q == me:
-                break
-            acc += int(ge[q][s] - gt[q][s])
-        pos0[s] = acc
+    pos0 = block_bases(gt, counts, sort.is_reversed())[me]
     i = np.arange(len(run), dtype=np.int64)
     s_of = np.minimum(run["score"].astype(np.int64), nb - 1) if by_score else np.zeros(len(run), dtype=np.int64)
     x = pos0[s_of] + (i - gt[me][s_of])
