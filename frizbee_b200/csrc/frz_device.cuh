@@ -200,6 +200,14 @@ struct FrzCounters {
 #if defined(__CUDACC__)   // device-only helpers (the structs above are shared with host-side test builds)
 __device__ __forceinline__ uint32_t frz_lane() { return threadIdx.x & 31; }
 
+// Programmatic dependent launch (frz_launch_dependent).  A kernel launched that way can be scheduled before the kernel
+// ahead of it on the stream has finished, so it calls frz_wait_prior_grid() before its first global memory access:
+// the wait returns once every prior grid has completed and its writes are visible (it is a no-op in a normal launch).
+// Because every dependent kernel waits before touching memory, a kernel may let its dependent be scheduled at any point
+// (frz_allow_dependent_launch): that only moves the dependent's launch and block scheduling under this kernel's tail.
+__device__ __forceinline__ void frz_wait_prior_grid() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
+__device__ __forceinline__ void frz_allow_dependent_launch() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+
 // Byte accessor of one packed haystack for the per-thread correctness paths (unicode.cu, k_match_indices):
 // `base` is the pointer to unit 0 of the slot (its units are contiguous), `shift` the window start.
 struct FrzPackedHay {

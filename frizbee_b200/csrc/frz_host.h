@@ -32,6 +32,25 @@ inline int grid_for(uint64_t n, int block) {
     return (int)std::max<uint64_t>(1, std::min<uint64_t>((n + block - 1) / block, (uint64_t)frz_sm_count() * 16));
 }
 
+// Launches `k` with programmatic stream serialization: its blocks may be scheduled while the kernel ahead of it on the
+// stream drains its tail (and run before it completes when that kernel calls frz_allow_dependent_launch).  `k` must call
+// frz_wait_prior_grid() before its first global memory access (frz_device.cuh).  Any other stream operation ahead of it
+// (a copy, a memset, an event record) orders it as a normal launch would.
+template <typename... KArgs, typename... Args>
+inline cudaError_t frz_launch_dependent(void (*k)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, Args&&... args) {
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = grid;
+    cfg.blockDim = block;
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = stream;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    return cudaLaunchKernelEx(&cfg, k, std::forward<Args>(args)...);
+}
+
 #define FRZ_CUDA_TRY(expr)                                                                         \
     do {                                                                                           \
         cudaError_t _e = (expr);                                                                   \

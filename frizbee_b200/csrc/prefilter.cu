@@ -618,6 +618,8 @@ __global__ void __launch_bounds__(kThreads) k_prefilter_list_long(const FrzCorpu
 // its tile's survivors in index order) and the tile's survivor count.  One warp per tile.
 __global__ void __launch_bounds__(256) k_tile_rank(const uint32_t* __restrict__ surv_bitmap, uint16_t* __restrict__ word_prefix,
                                                    uint32_t* __restrict__ tile_count, uint32_t n_tiles) {
+    frz_wait_prior_grid();
+    frz_allow_dependent_launch();
     const uint32_t tile = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = frz_lane();
     if (tile >= n_tiles) return;
     const uint32_t c = __popc(surv_bitmap[(uint64_t)tile * 32 + lane]);
@@ -642,6 +644,8 @@ __global__ void __launch_bounds__(1024) k_tile_scan(const uint32_t* __restrict__
                                                     uint32_t n, FrzCounters* __restrict__ ctr, unsigned long long* carry) {
     __shared__ uint64_t warp_sum[32];
     __shared__ uint32_t cnt_s[kTileScanSmem];
+    frz_wait_prior_grid();
+    frz_allow_dependent_launch();
     const bool in_smem = n <= kTileScanSmem;
     if (in_smem) {
         for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) cnt_s[i] = tile_count[i];
@@ -891,11 +895,12 @@ frz_status frz_launch_prefilter(const FrzCorpusView& cv, const FrzPatternDev& pa
 frz_status frz_launch_tile_scan(const FrzCorpusView& cv, FrzWorkspace& ws, cudaStream_t stream, FrzLaunchStats* st,
                                 unsigned long long* carry) {
     if (cv.n_tiles) {
-        k_tile_rank<<<(cv.n_tiles * 32 + 255) / 256, 256, 0, stream>>>(ws.surv_bitmap.get(), ws.word_prefix.get(), ws.tile_count.get(), cv.n_tiles);
+        FRZ_CUDA_TRY(frz_launch_dependent(k_tile_rank, (cv.n_tiles * 32 + 255) / 256, 256, 0, stream, ws.surv_bitmap.get(),
+                                          ws.word_prefix.get(), ws.tile_count.get(), cv.n_tiles));
         if (st) st->launches++;
     }
-    k_tile_scan<<<1, 1024, 0, stream>>>(ws.tile_count.get(), ws.tile_out_base.get(), cv.n_tiles, ws.counters.get(), carry);
-    FRZ_CUDA_TRY(cudaGetLastError());
+    FRZ_CUDA_TRY(frz_launch_dependent(k_tile_scan, 1, 1024, 0, stream, ws.tile_count.get(), ws.tile_out_base.get(), cv.n_tiles,
+                                      ws.counters.get(), carry));
     if (st) st->launches++;
     return FRZ_OK;
 }

@@ -13,7 +13,10 @@
 //
 // The fused single-pass sort (frz_sort_fused_prepare / frz_launch_sort_fused) has no histogram kernel: the scoring kernels
 // count every match they emit into FrzScoreHist (per score digit, per 2048-element segment of its index-ordered position),
-// k_sort_scan_rows scans that histogram (and re-zeroes it), and k_sort_scatter_seg places one segment per block.
+// k_sort_scan_rows scans that histogram (and re-zeroes it), and k_sort_scatter_seg sorts one segment per block and writes
+// it out as whole score runs.  Both are launched dependent (frz_launch_dependent): each waits for the kernel ahead of it
+// before its first memory access.  The multi-GPU table event recorded between them still marks the scan's completion: an
+// event orders like any stream operation, and the scatter after it starts early only behind a kernel.
 //
 // The element count lives in device memory (it is produced by the previous stage), so the whole
 // match_list pipeline runs without a host round trip until the final copy-out.
@@ -25,6 +28,8 @@
 #include "frz_host.h"
 
 #include <algorithm>
+
+#include <cub/block/block_radix_sort.cuh>
 
 namespace {
 
@@ -88,6 +93,8 @@ __global__ void __launch_bounds__(256) k_sort_scan_rows(uint32_t* __restrict__ h
                                                         unsigned int* __restrict__ done_counter) {
     __shared__ bool is_last;
     __shared__ uint32_t wsum[8];
+    frz_wait_prior_grid();   // the histogram and the count come from the scoring kernels
+    frz_allow_dependent_launch();
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int d = blockIdx.x * 8 + warp;
     if (d < bins) {
@@ -202,70 +209,77 @@ __global__ void __launch_bounds__(kSortWarps * 32) k_sort_scatter(const FrzMatch
 }
 
 // The fused single-pass scatter: one block per 2^kFrzSortSegShift-element segment of the list (a persistent grid strides over
-// the segments).  Warp w owns the segment's w-th run of kSegRounds * 32 elements and loads all of it at once (coalesced, every
-// load in flight).  It ranks its run stably, 32 elements per round: __match_any_sync gives the rank inside the round, and the
-// round's leader of each digit adds the round's count to the warp's digit counter in shared memory, whose old value it
-// broadcasts.  A per-digit exclusive prefix over the warps, plus digit_base[d] + pref[d][segment] (the scoring kernels'
-// histogram, scanned), then gives every element its final position: (score desc, index asc) exactly.
+// the segments).  The block sorts its segment in shared memory and writes it out as whole digit runs:
+//   1. load: thread t loads the segment's elements t*8 .. t*8+7 (the blocked order cub's stable sort ranks by) and stages
+//      them in shared memory;
+//   2. sort: the key of element p is ((bins-1 - digit) << 11) | p, sorted by cub::BlockRadixSort over the digit bits only.
+//      The sort is stable, so every digit run keeps index order, and the low 11 bits carry the element's position;
+//   3. runs: rank r of the sorted segment starts a run where its digit differs from rank r-1's; that rank stores
+//      off[d] = digit_base[d] + pref[d][segment] - r, so the element of rank r goes to off[d] + r;
+//   4. store: thread t writes ranks t, t+256, ... (striped), so consecutive threads write consecutive addresses of a run.
+// Elements past the end of the list (last segment) get digit 0's key: they sort behind every real digit-0 element (their
+// positions are larger) and so take exactly the ranks >= the segment's element count, which are not stored.
 constexpr int kSegThreads = 256;
-constexpr int kSegWarps = kSegThreads / 32;
-constexpr int kSegRounds = (1 << kFrzSortSegShift) / kSegThreads;   // elements per lane
-static_assert(kSegRounds * kSegThreads == (1 << kFrzSortSegShift), "a segment is a whole number of block-wide rounds");
+constexpr int kSegItems = (1 << kFrzSortSegShift) / kSegThreads;   // elements per thread
+static_assert(kSegItems * kSegThreads == (1 << kFrzSortSegShift), "a segment is a whole number of block-wide rounds");
+static_assert(kSegItems % 2 == 0, "the blocked load moves two elements per 16-byte load");
+using SegSort = cub::BlockRadixSort<uint32_t, kSegThreads, kSegItems>;
 
 __global__ void __launch_bounds__(kSegThreads) k_sort_scatter_seg(const FrzMatchDev* __restrict__ in, FrzMatchDev* __restrict__ out,
                                                                   const unsigned long long* __restrict__ n_ptr, int bins,
                                                                   const uint32_t* __restrict__ pref, uint32_t stride,
                                                                   const uint32_t* __restrict__ digit_base, uint32_t limit) {
-    extern __shared__ uint32_t sm[];   // [kSegWarps][bins]: per-warp digit counters, then each warp's output base per digit
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    uint32_t* cnt = sm + warp * bins;
+    constexpr int kSeg = 1 << kFrzSortSegShift;
+    __shared__ union {
+        typename SegSort::TempStorage sort;
+        uint16_t digit[kSeg];   // digit of each sorted rank (after the sort)
+    } tmp;
+    __shared__ uint2 elem[kSeg];         // the segment, index order
+    __shared__ uint32_t off[kMaxBins];   // per digit present in the segment: output position of rank 0 of its run
+    frz_wait_prior_grid();   // pref and digit_base come from k_sort_scan_rows
     const unsigned long long n = *n_ptr;
-    const uint32_t nseg = (uint32_t)((n + (1ull << kFrzSortSegShift) - 1) >> kFrzSortSegShift);
+    const uint32_t nseg = (uint32_t)((n + kSeg - 1) >> kFrzSortSegShift);
     const uint32_t mask = (uint32_t)bins - 1;
-    const uint32_t lt = (1u << lane) - 1;
+    const int end_bit = kFrzSortSegShift + 32 - __clz(mask);   // bins is a power of two
+    const int t = threadIdx.x;
     for (uint32_t seg = blockIdx.x; seg < nseg; seg += gridDim.x) {
-        for (int d = threadIdx.x; d < kSegWarps * bins; d += kSegThreads) sm[d] = 0;
-        const unsigned long long first = ((unsigned long long)seg << kFrzSortSegShift) + warp * (kSegRounds * 32) + lane;
-        FrzMatchDev m[kSegRounds];
+        const unsigned long long seg0 = (unsigned long long)seg << kFrzSortSegShift;
+        const uint32_t cnt = (uint32_t)min(n - seg0, (unsigned long long)kSeg);
+        const uint4* src = reinterpret_cast<const uint4*>(in + seg0) + t * (kSegItems / 2);
+        uint32_t key[kSegItems];
 #pragma unroll
-        for (int r = 0; r < kSegRounds; r++) {
-            m[r].index = 0; m[r].score = 0; m[r].exact = 0; m[r].pad = 0;
-            if (first + r * 32 < n) m[r] = in[first + r * 32];
+        for (int j = 0; j < kSegItems / 2; j++) {
+            const uint32_t p = t * kSegItems + 2 * j;
+            uint4 v = make_uint4(0, 0, 0, 0);
+            if (p + 1 < cnt) v = src[j];
+            else if (p < cnt) { const uint2 h = *reinterpret_cast<const uint2*>(src + j); v.x = h.x; v.y = h.y; }
+            reinterpret_cast<uint4*>(elem)[p >> 1] = v;
+            // FrzMatchDev word 1: score in the low 16 bits
+            key[2 * j] = ((mask - (v.y & mask)) << kFrzSortSegShift) | p;
+            key[2 * j + 1] = ((mask - (v.w & mask)) << kFrzSortSegShift) | (p + 1);
+        }
+        // past the end: digit 0 (above), sorted behind every real element of that digit
+        SegSort(tmp.sort).SortBlockedToStriped(key, kFrzSortSegShift, end_bit);
+        __syncthreads();   // the sort's storage becomes the digit array
+#pragma unroll
+        for (int j = 0; j < kSegItems; j++) tmp.digit[t + j * kSegThreads] = (uint16_t)(mask - (key[j] >> kFrzSortSegShift));
+        __syncthreads();
+#pragma unroll
+        for (int j = 0; j < kSegItems; j++) {
+            const uint32_t r = t + j * kSegThreads;
+            const uint32_t d = tmp.digit[r];
+            if (r < cnt && (r == 0 || tmp.digit[r - 1] != d)) off[d] = digit_base[d] + pref[(size_t)d * stride + seg] - r;
         }
         __syncthreads();
-        uint32_t rank[kSegRounds];
 #pragma unroll
-        for (int r = 0; r < kSegRounds; r++) {
-            const bool valid = first + r * 32 < n;
-            const uint32_t d = valid ? (uint32_t)m[r].score & mask : (uint32_t)bins + lane;   // sentinel: matches nobody
-            const uint32_t peers = __match_any_sync(0xffffffffu, d);
-            const int leader = __ffs(peers) - 1;
-            uint32_t old = 0;
-            if (valid && lane == leader) old = atomicAdd(&cnt[d], (uint32_t)__popc(peers));
-            rank[r] = __shfl_sync(0xffffffffu, old, leader) + __popc(peers & lt);
-        }
-        __syncthreads();
-        // per digit: exclusive prefix over the warps, offset by where the digit's run of this segment starts in the output
-        for (int d = threadIdx.x; d < bins; d += kSegThreads) {
-            uint32_t tot = 0;
-#pragma unroll
-            for (int w = 0; w < kSegWarps; w++) tot += sm[w * bins + d];
-            uint32_t run = tot ? digit_base[d] + pref[(size_t)d * stride + seg] : 0u;
-#pragma unroll
-            for (int w = 0; w < kSegWarps; w++) {
-                const uint32_t c = sm[w * bins + d];
-                sm[w * bins + d] = run;
-                run += c;
+        for (int j = 0; j < kSegItems; j++) {
+            const uint32_t r = t + j * kSegThreads;
+            if (r < cnt) {
+                const uint32_t pos = off[mask - (key[j] >> kFrzSortSegShift)] + r;
+                if (pos < limit) reinterpret_cast<uint2*>(out)[pos] = elem[key[j] & (kSeg - 1)];
             }
         }
-        __syncthreads();
-#pragma unroll
-        for (int r = 0; r < kSegRounds; r++)
-            if (first + r * 32 < n) {
-                const uint32_t pos = cnt[(uint32_t)m[r].score & mask] + rank[r];
-                if (pos < limit) out[pos] = m[r];
-            }
-        __syncthreads();   // the counters are reset for the next segment
+        __syncthreads();   // elem, off and the sort storage are reused by the next segment
     }
 }
 
@@ -345,17 +359,16 @@ frz_status frz_launch_sort_fused(const FrzMatchDev* d_in, FrzMatchDev* d_out, co
     uint32_t* totals = ss.hist.get() + (size_t)kMaxBins * kV;
     uint32_t* digit_base = totals + kMaxBins;
     unsigned int* done_counter = reinterpret_cast<unsigned int*>(digit_base + kMaxBins);
-    k_sort_scan_rows<4, true><<<(bins + 7) / 8, 256, 0, stream>>>(h.counts, pref, h.stride, n_ptr, bins, totals, digit_base, done_counter);
-    FRZ_CUDA_TRY(cudaGetLastError());
+    FRZ_CUDA_TRY(frz_launch_dependent(k_sort_scan_rows<4, true>, (bins + 7) / 8, 256, 0, stream, h.counts, pref, h.stride, n_ptr, bins,
+                                      totals, digit_base, done_counter));
     ss.fused_dirty = false;
     if (ss.arm_table_ev && ss.table_ev) {   // digit_base is final: the multi-GPU layer publishes it while the scatter runs
         FRZ_CUDA_TRY(cudaEventRecord(ss.table_ev.get(), stream));
         ss.table_ev_recorded = true;
     }
-    const size_t smem = (size_t)kSegWarps * bins * sizeof(uint32_t);
     const int grid = (int)std::max<uint32_t>(1, std::min<uint32_t>(h.stride, (uint32_t)frz_sm_count() * 4));
-    k_sort_scatter_seg<<<grid, kSegThreads, smem, stream>>>(d_in, d_out, n_ptr, bins, pref, h.stride, digit_base, limit);
-    FRZ_CUDA_TRY(cudaGetLastError());
+    FRZ_CUDA_TRY(frz_launch_dependent(k_sort_scatter_seg, grid, kSegThreads, 0, stream, d_in, d_out, n_ptr, bins, pref, h.stride,
+                                      digit_base, limit));
     if (st) st->launches += 2;
     return FRZ_OK;
 }

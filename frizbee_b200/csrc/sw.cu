@@ -171,6 +171,8 @@ __global__ void __launch_bounds__(kSwThreads, (kSw64MinBlocks<LANES, WRAP8>)) k_
                                                    const FrzScoreHist hist) {
     __shared__ Sw64Stage stage;
     __shared__ __align__(16) uint32_t rows_smem[kSw64RowsInSmem<LANES, WRAP8> ? 2 * 32 * kSwThreads : 1];
+    frz_wait_prior_grid();   // the survivor lists and class counts come from the prefilter stage
+    frz_allow_dependent_launch();
     const uint32_t lane = frz_lane();
     unsigned long long cnt[4];
     uint32_t items_end[4];   // cumulative item counts in processing order CC64, CC56, CC48, CC40
@@ -562,14 +564,14 @@ frz_status launch_sw_lanes(const FrzCorpusView& cv, const FrzPatternDev& pat, ui
     // kSwVarLanePen: gap_extend == 0 < gap_open_x, whose penalties the default IMAD form gets wrong (SwCore).
     const bool lane_pen = !pat.wrap8 && pat.gap_extend == 0 && pat.gap_open_x > 0;
     if (pat.wrap8)
-        k_sw64<LANES, true><<<frz_sm_count() * kSw64MinBlocks<LANES, true>, kSwThreads, 0, stream>>>(
-            cv, pat, ws.lists(), ws.survivor_cap(), rank_view(ws), ws.counters.get(), index_offset, rev, d_out, hist);
+        FRZ_CUDA_TRY(frz_launch_dependent(k_sw64<LANES, true>, frz_sm_count() * kSw64MinBlocks<LANES, true>, kSwThreads, 0, stream,
+            cv, pat, ws.lists(), ws.survivor_cap(), rank_view(ws), ws.counters.get(), index_offset, rev, d_out, hist));
     else if (lane_pen)
-        k_sw64<LANES, false, 8 | kSwVarLanePen><<<frz_sm_count() * kSw64MinBlocks<LANES, false>, kSwThreads, 0, stream>>>(
-            cv, pat, ws.lists(), ws.survivor_cap(), rank_view(ws), ws.counters.get(), index_offset, rev, d_out, hist);
+        FRZ_CUDA_TRY(frz_launch_dependent(k_sw64<LANES, false, 8 | kSwVarLanePen>, frz_sm_count() * kSw64MinBlocks<LANES, false>, kSwThreads, 0, stream,
+            cv, pat, ws.lists(), ws.survivor_cap(), rank_view(ws), ws.counters.get(), index_offset, rev, d_out, hist));
     else
-        k_sw64<LANES, false, 8><<<frz_sm_count() * kSw64MinBlocks<LANES, false>, kSwThreads, 0, stream>>>(
-            cv, pat, ws.lists(), ws.survivor_cap(), rank_view(ws), ws.counters.get(), index_offset, rev, d_out, hist);
+        FRZ_CUDA_TRY(frz_launch_dependent(k_sw64<LANES, false, 8>, frz_sm_count() * kSw64MinBlocks<LANES, false>, kSwThreads, 0, stream,
+            cv, pat, ws.lists(), ws.survivor_cap(), rank_view(ws), ws.counters.get(), index_offset, rev, d_out, hist));
     // windows of 65..128 bytes only exist when some haystack of the corpus is longer than 64 bytes (recorded at pack time)
     if (cv.max_gunits <= 4) { FRZ_CUDA_TRY(cudaGetLastError()); return FRZ_OK; }
     const size_t smem = SwCore<LANES, 128, false>::smem_bytes;
