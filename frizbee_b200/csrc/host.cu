@@ -1870,6 +1870,17 @@ extern "C" frz_status frz_matcher_debug_pattern(const frz_matcher* m, size_t i, 
     return FRZ_OK;
 }
 
+// Debugging / test aid: the needle and scoring constants pattern i hands to the unicode, literal and traceback kernels
+// (k_unicode, k_match_indices), so that host builds of unicode_path.cuh / indices_path.cuh run with exactly them.
+extern "C" frz_status frz_matcher_debug_unicode(const frz_matcher* m, size_t i, void* un, size_t un_size, void* usc, size_t usc_size) {
+    if (!m || !un || !usc || i >= m->compiled.size()) return frz_fail(FRZ_ERR_INVALID_ARG, "pattern index out of range");
+    if (un_size != sizeof(FrzUNeedle) || usc_size != sizeof(FrzUScoring))
+        return frz_fail(FRZ_ERR_INVALID_ARG, "expected buffers of %zu and %zu bytes", sizeof(FrzUNeedle), sizeof(FrzUScoring));
+    memcpy(un, &m->compiled[i].un, sizeof(FrzUNeedle));
+    memcpy(usc, &m->compiled[i].usc, sizeof(FrzUScoring));
+    return FRZ_OK;
+}
+
 extern "C" uint64_t frz_debug_device_bytes(void) { return g_frz_device_bytes.load(); }
 extern "C" uint64_t frz_debug_device_bytes_peak(int reset) {
     if (reset) g_frz_device_bytes_peak.store(g_frz_device_bytes.load());

@@ -419,6 +419,10 @@ FRZ_API uint32_t frz_matcher_score_bound(const frz_matcher* m);
 /* Test aid: copies the compiled device pattern (frizbee_b200/csrc/frz_device.cuh: FrzPatternDev) of pattern i; out_size
  * must equal its size.  Lets host builds of the kernel cores run with exactly the constants the GPU receives. */
 FRZ_API frz_status frz_matcher_debug_pattern(const frz_matcher* m, size_t i, void* out, size_t out_size);
+/* Test aid: copies the needle (frizbee_b200/csrc/unicode_path.cuh: FrzUNeedle) and scoring constants (FrzUScoring) that
+ * pattern i hands to the unicode, literal and traceback kernels; un_size / usc_size must equal their sizes.  Lets host
+ * builds of unicode_path.cuh and indices_path.cuh run with exactly the constants the GPU receives. */
+FRZ_API frz_status frz_matcher_debug_unicode(const frz_matcher* m, size_t i, void* un, size_t un_size, void* usc, size_t usc_size);
 
 /* Test aid: copies the packed image of a corpus (frizbee_b200/csrc/frz_device.cuh, DESIGN.md §3) to host buffers, in
  * this order: tile_base (u64 per tile), groups (FrzGroupDesc, 16 bytes per group), slot_meta (u32 per slot), slot_of

@@ -71,6 +71,8 @@ int literal(const P& p, const uint8_t* hay, int len, int* pos, uint32_t* score) 
 }  // namespace
 
 extern "C" {
+size_t h_pattern_size() { return sizeof(FrzPatternDev); }
+
 // The scanning form of the pattern's typo mode on a FrzPatternDev (needles of up to FRZ_MAX_NEEDLE bytes).
 // Returns 1/0 = matched, -1 = the typo mode has no prefilter form.
 int h_scan_window(const void* pat_bytes, const uint8_t* hay, int len, int* start, int* end) {

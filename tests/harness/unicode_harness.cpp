@@ -67,4 +67,25 @@ int h_lit_find(const uint8_t* needle, size_t n, int case_sensitive, const uint16
     Flat h{hay};
     return frzu::lit_find(nd, sc, h, len, mode, pos, score) ? 1 : 0;
 }
+
+// The same kernels on a ready needle and scoring: the library's own (frz_matcher_debug_unicode), so that the tests run
+// with exactly the constants the GPU kernels receive.
+size_t h_uneedle_size() { return sizeof(FrzUNeedle); }
+size_t h_uscoring_size() { return sizeof(FrzUScoring); }
+void h_scoring_of(const uint16_t* scoring9, int score_bits, FrzUScoring* out) { *out = scoring_of(scoring9, score_bits == 8); }
+int h_sw_score_c(const FrzUNeedle* nd, const FrzUScoring* sc, const uint8_t* hay, int len, int include_prefix, int lanes, int score_bits) {
+    std::vector<uint16_t> scratch((size_t)2 * (nd->n + 1) * lanes);
+    Flat h{hay};
+    return (int)frzu::sw_score(*nd, *sc, h, len, include_prefix != 0, lanes, score_bits == 8, scratch.data());
+}
+int h_sw_indices_c(const FrzUNeedle* nd, int unicode, const FrzUScoring* sc, const uint8_t* hay, int len, int start_pos, int max_typos,
+                   int lanes, int score_bits, uint32_t* out, int cap, int* n_out) {
+    std::vector<uint16_t> scratch(frzi::indices_scratch_elems(unicode ? nd->n : nd->nbytes, lanes));
+    Flat h{hay};
+    return (int)frzi::sw_indices(*nd, unicode != 0, *sc, h, len, start_pos, max_typos, lanes, score_bits == 8, scratch.data(), out, cap, n_out);
+}
+int h_lit_find_c(const FrzUNeedle* nd, const FrzUScoring* sc, const uint8_t* hay, int len, int mode, int* pos, uint32_t* score) {
+    Flat h{hay};
+    return frzu::lit_find(*nd, *sc, h, len, mode, pos, score) ? 1 : 0;
+}
 }

@@ -1,13 +1,13 @@
 """Scorings for the kernel tests: the edge cases where the Smith-Waterman kernels' arithmetic changes form, followed by
-random draws of all nine `Scoring` fields.  Every scoring returned is one the library compiles for a fuzzy needle of up
-to `max_needle` bytes at every lane width: the library's bounds (score overflow guard, signed 16-bit cell range,
+random draws of all nine `Scoring` fields.  Every scoring `scorings` returns is one the library compiles for a fuzzy
+needle of up to `max_needle` bytes at every lane width: the library's bounds (score overflow guard, signed 16-bit cell range,
 gap-penalty range) all grow with the needle length and the lane width, so checking the longest needle at the widest
 lanes checks every shorter one."""
 import random
 from typing import List
 
 import frizbee_b200 as F
-from frizbee_b200.types import Config, Scoring
+from frizbee_b200.types import Config, Matching, Scoring, UnicodeMatching
 
 FIELDS = ("match_score", "mismatch_penalty", "gap_open_penalty", "gap_extend_penalty", "prefix_bonus",
           "capitalization_bonus", "matching_case_bonus", "exact_match_bonus", "delimiter_bonus")
@@ -71,12 +71,84 @@ def _draw(rng: random.Random) -> Scoring:
     return Scoring(**{f: one() for f in FIELDS})
 
 
-def scorings(seed: int, count: int, max_needle: int) -> List[Scoring]:
-    """The accepted edge cases, then random accepted scorings up to `count` in all."""
-    out = [sc for sc in edge_cases(max_needle) if accepted(sc, max_needle)]
+def _sweep(edges: List[Scoring], ok, seed: int, count: int, max_needle: int) -> List[Scoring]:
+    out = [sc for sc in edges if ok(sc, max_needle)]
     rng = random.Random(seed)
     while len(out) < count:
         sc = _draw(rng)
-        if accepted(sc, max_needle):
+        if ok(sc, max_needle):
             out.append(sc)
     return out
+
+
+def scorings(seed: int, count: int, max_needle: int) -> List[Scoring]:
+    """The accepted edge cases, then random accepted scorings up to `count` in all."""
+    return _sweep(edge_cases(max_needle), accepted, seed, count, max_needle)
+
+
+# The unicode kernels keep true u8 / u16 lanes and the literal matcher adds in u32: neither has the byte path's signed
+# 16-bit cell bound, only the u16 score guard.  So they accept scorings whose scores reach 32 768-65 535, which
+# `accepted` refuses.  A needle of `max_needle` ASCII scalars is the longest the unicode guard (which counts scalars)
+# sees for `max_needle` bytes.
+def accepted_unicode(sc: Scoring, max_needle: int) -> bool:
+    try:
+        F.Matcher(b"a" * max_needle, Config(max_typos=None, unicode=UnicodeMatching.Always, scoring=sc, emulate_lanes=64)).close()
+    except F.FrizbeeError:
+        return False
+    return True
+
+
+def accepted_literal(sc: Scoring, max_needle: int) -> bool:
+    try:
+        F.Matcher(b"a" * max_needle, Config(matching=Matching.Substring, scoring=sc)).close()
+    except F.FrizbeeError:
+        return False
+    return True
+
+
+# the bonuses of the default scoring are all 4: these make capitalization, matching case and delimiter distinguishable
+DISTINCT_BONUSES = Scoring(capitalization_bonus=3, matching_case_bonus=11, delimiter_bonus=29, prefix_bonus=7)
+# zero gap and mismatch penalties: traceback cells tie between diagonal, left and up
+TIES = Scoring(mismatch_penalty=0, gap_open_penalty=0, gap_extend_penalty=0)
+
+
+def high_match_score(max_needle: int, sc: Scoring = Scoring()) -> int:
+    """The largest match_score that the unicode guard accepts for `max_needle` scalars with the other fields of `sc`:
+    a needle of that many scalars matched in full scores just under 65 536."""
+    lo, hi = 0, 0xFFFF
+    while lo < hi:
+        mid = (lo + hi + 1) // 2
+        if accepted_unicode(Scoring(**{**sc.__dict__, "match_score": mid}), max_needle):
+            lo = mid
+        else:
+            hi = mid - 1
+    return lo
+
+
+def unicode_edge_cases(max_needle: int) -> List[Scoring]:
+    m_hi = high_match_score(max_needle)
+    return [DISTINCT_BONUSES, TIES, Scoring(**{**TIES.__dict__, "prefix_bonus": 0, "matching_case_bonus": 0}),
+            Scoring(match_score=m_hi), Scoring(match_score=m_hi // 2 + 1, gap_extend_penalty=0, delimiter_bonus=300),
+            Scoring(match_score=m_hi, mismatch_penalty=0, gap_open_penalty=0, gap_extend_penalty=0)] + edge_cases(max_needle)
+
+
+def literal_edge_cases(max_needle: int) -> List[Scoring]:
+    d = Scoring()
+    per_char = d.match_score + d.matching_case_bonus + max(d.capitalization_bonus, d.delimiter_bonus)
+    # the largest exact_match_bonus the literal guard accepts for a needle of max_needle bytes
+    exact_max = 0xFFFF - d.prefix_bonus - d.mismatch_penalty - max_needle * per_char
+    return [DISTINCT_BONUSES, Scoring(exact_match_bonus=exact_max), Scoring(exact_match_bonus=exact_max // 2, prefix_bonus=0),
+            Scoring(match_score=(0xFFFF - 40) // max_needle - 8), Scoring(**{f: 0 for f in FIELDS}),
+            Scoring(capitalization_bonus=500, delimiter_bonus=0, matching_case_bonus=0),
+            Scoring(capitalization_bonus=0, delimiter_bonus=500, prefix_bonus=0)]
+
+
+def unicode_scorings(seed: int, count: int, max_needle: int) -> List[Scoring]:
+    """`scorings` for the unicode kernels: accepted for a unicode needle of `max_needle` bytes, high scores included."""
+    return _sweep(unicode_edge_cases(max_needle), accepted_unicode, seed, count, max_needle)
+
+
+def literal_scorings(seed: int, count: int, max_needle: int) -> List[Scoring]:
+    """`scorings` for the literal matcher: accepted for a literal needle of `max_needle` bytes, exact_match_bonus up to
+    its guard included."""
+    return _sweep(literal_edge_cases(max_needle), accepted_literal, seed, count, max_needle)
