@@ -16,7 +16,7 @@ import numpy as np
 from .types import (CaseMatching, CConfig, CMatch, Config, CPattern, Match, Matching, Pattern, Scoring,
                     SortStrategy, UnicodeMatching, as_pattern, pattern_array)
 
-__all__ = ["Matcher", "Corpus", "Subset", "Pattern", "Config", "Scoring", "Match", "SortStrategy", "CaseMatching",
+__all__ = ["Matcher", "Corpus", "Subset", "Boost", "Pattern", "Config", "Scoring", "Match", "SortStrategy", "CaseMatching",
            "UnicodeMatching", "Matching", "FrizbeeError", "parse_query", "parse_atom", "radix_sort_matches",
            "MATCH_DTYPE", "lib", "lib_path"]
 
@@ -98,6 +98,11 @@ def lib():
     L.frz_subset_destroy.restype = None
     L.frz_match_list_subset.argtypes = [vp, vp, vp, vp, u64, C.POINTER(u64)]
     L.frz_match_list_subset_top.argtypes = [vp, vp, vp, u64, vp, C.POINTER(u64), C.POINTER(u64)]
+    L.frz_boost_create.argtypes = [vp, vp, u64, C.POINTER(vp)]
+    L.frz_boost_set.argtypes = [vp, vp, vp, u64]
+    L.frz_boost_destroy.argtypes = [vp]
+    L.frz_boost_destroy.restype = None
+    L.frz_match_list_ranked.argtypes = [vp, vp, vp, vp, u64, vp, C.POINTER(u64), C.POINTER(u64)]
     L.frz_match_list_into.argtypes = [vp, vp, u32, vp, u64, C.POINTER(u64)]
     L.frz_match_list_host.argtypes = [vp, vp, vp, u64, C.c_int, vp, u64, C.POINTER(u64)]
     L.frz_match_list_host_arrow.argtypes = [vp, vp, vp, C.c_int, u64, C.c_int, vp, u64, C.POINTER(u64)]
@@ -249,6 +254,14 @@ class Corpus:
         _check(lib().frz_subset_create(self._h, which.ctypes.data if which.size else None, len(which), C.byref(h)))
         return Subset(h, self)
 
+    def boost(self, values=None) -> "Boost":
+        """A resident per-row boost for Matcher.match_list_ranked_array: values[i] (int16) is the boost of row i, rows
+        past len(values) have 0; at most len(self) values.  Close it before the corpus."""
+        values = np.ascontiguousarray(np.zeros(0, np.int16) if values is None else values, dtype=np.int16)
+        h = C.c_void_p()
+        _check(lib().frz_boost_create(self._h, values.ctypes.data if values.size else None, len(values), C.byref(h)))
+        return Boost(h, self)
+
     def __len__(self):
         return self.n
 
@@ -285,6 +298,35 @@ class Subset:
     def close(self):
         if self._h:
             lib().frz_subset_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class Boost:
+    """A signed 16-bit boost per row of one resident Corpus (frz_boost), kept by index across corpus edits."""
+
+    def __init__(self, handle, corpus: Corpus):
+        self._h = handle
+        self.corpus = corpus
+
+    def set(self, which, values) -> "Boost":
+        """boost[which[j]] = values[j]; any row below len(corpus), appended ones included, each at most once."""
+        which = np.ascontiguousarray(which, dtype=np.uint32)
+        values = np.ascontiguousarray(values, dtype=np.int16)
+        if len(values) != len(which):
+            raise ValueError(f"{len(which)} indices need {len(which)} values, got {len(values)}")
+        _check(lib().frz_boost_set(self._h, which.ctypes.data if which.size else None,
+                                   values.ctypes.data if values.size else None, len(which)))
+        return self
+
+    def close(self):
+        if self._h:
+            lib().frz_boost_destroy(self._h)
             self._h = None
 
     def __del__(self):
@@ -400,6 +442,22 @@ class Matcher:
         out = np.empty(max(1, min(int(k), len(subset))), dtype=MATCH_DTYPE)
         n, total = C.c_uint64(), C.c_uint64()
         _check(lib().frz_match_list_subset_top(self._h, corpus._h, subset._h, int(k), out.ctypes.data, C.byref(n), C.byref(total)))
+        return out[: n.value], total.value
+
+    def match_list_ranked_array(self, corpus: Corpus, boost: Boost, k: Optional[int] = None, subset: Optional[Subset] = None,
+                                out: Optional[np.ndarray] = None) -> Tuple[np.ndarray, int]:
+        """The rows of match_list_array(corpus) (or of its subset), ranked by clamp(score + boost[index], 0, 65535), ties in
+        the strategy's index order, truncated to the first k (frz_match_list_ranked): (array of min(k, total) rows, total).
+        k=None ranks the whole list.  `out` (optional) needs room for min(k, len(corpus), len(subset)) rows."""
+        k = 0xFFFFFFFFFFFFFFFF if k is None else int(k)
+        need = min(k, corpus.n, len(subset) if subset is not None else corpus.n)
+        if out is None:
+            out = np.empty(max(1, need), dtype=MATCH_DTYPE)
+        elif len(out) < need:
+            raise ValueError(f"out holds {len(out)} matches; this ranked call needs {need}")
+        n, total = C.c_uint64(), C.c_uint64()
+        _check(lib().frz_match_list_ranked(self._h, corpus._h, subset._h if subset is not None else None, boost._h, k,
+                                           out.ctypes.data, C.byref(n), C.byref(total)))
         return out[: n.value], total.value
 
     def match_list_into_array(self, haystacks, index_offset: int = 0, device: int = 0) -> np.ndarray:

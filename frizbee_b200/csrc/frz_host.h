@@ -307,6 +307,11 @@ constexpr uint32_t kFrzNoLimit = 0xFFFFFFFFu;
 frz_status frz_launch_sort_by_score_dev(const FrzMatchDev* d_in, FrzMatchDev* d_tmp, FrzMatchDev* d_out,
                                         const unsigned long long* n_ptr, uint32_t score_bound, FrzSortScratch& ss,
                                         cudaStream_t stream, FrzLaunchStats* st, uint32_t limit = kFrzNoLimit);
+// The same sort by descending key = clamp(score + boost[index], 0, 65535), boost 0 at indices >= n_boost (ranked calls).
+// key_bound: host-known upper bound of any key; d_tmp is used when it is >= 1024.
+frz_status frz_launch_sort_by_key_dev(const FrzMatchDev* d_in, FrzMatchDev* d_tmp, FrzMatchDev* d_out,
+                                      const unsigned long long* n_ptr, const int16_t* boost, uint32_t n_boost, uint32_t key_bound,
+                                      FrzSortScratch& ss, cudaStream_t stream, FrzLaunchStats* st, uint32_t limit = kFrzNoLimit);
 frz_status frz_sort_hist_alloc(FrzDevArray<uint32_t>& out);
 const uint32_t* frz_sort_digit_base(const FrzSortScratch& ss);
 int frz_sort_single_pass_bins(uint32_t score_bound);   // bins of the single-pass sort for this bound, 0 = two passes

@@ -1320,24 +1320,33 @@ __global__ void k_copy_n(const FrzMatchDev* __restrict__ in, FrzMatchDev* __rest
         out[i] = in[i];
 }
 
+// The boost of a ranked call (frz_match_list_ranked): the list is sorted by key = clamp(score + boost[index], 0, 65535).
+struct Ranking {
+    const int16_t* boost = nullptr;   // n values on the corpus's device; indices >= n have boost 0
+    uint32_t n = 0;
+    uint32_t max_boost = 0;           // >= every boost value (0 when none is positive): the key bound is score bound + this
+};
+
 // `final_out` (optional, device, >= corpus length): where the final list must land.  `limit` (top-K calls): only the first
 // `limit` positions of the final list are written (the sort's last scatter and the final copy drop the rest); the count in
-// ws.counters->total stays the full match count.  scope: as in match_into_device.
+// ws.counters->total stays the full match count.  scope: as in match_into_device.  rank (optional): sort by the ranking's
+// key instead, under every strategy and for the empty matcher too (the strategy's direction only orders ties).
 frz_status match_list_device(frz_matcher* m, const FrzCorpusStorage& cs, uint32_t index_offset, uint8_t sort,
                              FrzMatchDev** d_result, cudaStream_t stream, FrzLaunchStats* st, FrzMatchDev* final_out = nullptr,
-                             uint32_t limit = kFrzNoLimit, const SubsetScope& scope = SubsetScope()) {
+                             uint32_t limit = kFrzNoLimit, const SubsetScope& scope = SubsetScope(), const Ranking* rank = nullptr) {
     FrzWorkspace& ws = m->ws;
     const bool reversed = sort == FRZ_SORT_INDEX_DESC || sort == FRZ_SORT_SCORE_THEN_INDEX_DESC;
     const bool by_score = sort == FRZ_SORT_SCORE_THEN_INDEX_ASC || sort == FRZ_SORT_SCORE_THEN_INDEX_DESC;
-    const bool will_sort = by_score && !m->compiled.empty();
+    const bool will_sort = rank || (by_score && !m->compiled.empty());
     reset_call_state(m);
     FrzMatchDev* d_list = nullptr;
     uint32_t bound = 0;
-    FrzScoreHist hist;
+    FrzScoreHist hist;   // the fused histogram counts scores, so a ranked sort never asks for it
     FRZ_TRY(match_into_device(m, cs, index_offset, reversed, &d_list, &bound, stream, st, will_sort ? nullptr : final_out,
-                              will_sort ? &hist : nullptr, scope));
+                              will_sort && !rank ? &hist : nullptr, scope));
     // `!self.patterns.is_empty() && sort.is_by_score()` (src/matcher/mod.rs:218)
     if (will_sort) {
+        if (rank) bound = (uint32_t)std::min<uint64_t>((uint64_t)bound + rank->max_boost, 0xFFFF);   // the key bound
         FrzMatchDev* other = final_out ? final_out : (d_list == ws.matches_a.get() ? ws.matches_b.get() : ws.matches_a.get());
         // two-pass sort (score bound >= 1024) needs a scratch list of the corpus size: the multi-pattern ping-pong
         // buffer is free at this point (d_list is never multi_a); grow it whenever THIS corpus is larger
@@ -1346,9 +1355,14 @@ frz_status match_list_device(frz_matcher* m, const FrzCorpusStorage& cs, uint32_
             FRZ_TRY(ensure_multi_buffers(m, cs.n));
             tmp = ws.multi_a.get();
         }
-        if (hist.counts) FRZ_TRY(frz_launch_sort_fused(d_list, other, &ws.counters.get()->total, hist, ws.sort, stream, st, limit));
-        else FRZ_TRY(frz_launch_sort_by_score_dev(d_list, tmp, other, &ws.counters.get()->total, bound, ws.sort, stream, st, limit));
-        m->last_sort_bins = frz_sort_single_pass_bins(bound);
+        const unsigned long long* n_ptr = &ws.counters.get()->total;
+        if (rank) {
+            FRZ_TRY(frz_launch_sort_by_key_dev(d_list, tmp, other, n_ptr, rank->boost, rank->n, bound, ws.sort, stream, st, limit));
+        } else {
+            if (hist.counts) FRZ_TRY(frz_launch_sort_fused(d_list, other, n_ptr, hist, ws.sort, stream, st, limit));
+            else FRZ_TRY(frz_launch_sort_by_score_dev(d_list, tmp, other, n_ptr, bound, ws.sort, stream, st, limit));
+            m->last_sort_bins = frz_sort_single_pass_bins(bound);   // a per-score table (the multi-GPU merge reads it)
+        }
         d_list = other;
     } else if (final_out && d_list != final_out) {
         k_copy_n<<<grid_for(std::min<uint64_t>(cs.n, limit), 256), 256, 0, stream>>>(d_list, final_out, &ws.counters.get()->total, limit);
@@ -1396,9 +1410,10 @@ frz_status copy_out(frz_matcher* m, FrzMatchDev* d_list, uint64_t limit, frz_mat
 
 // Matcher::match_list (into, from index_offset, in `sort` order) → host, truncated to its first `limit` rows (top-K calls:
 // the same pipeline with a limit on the final scatter and copy; UINT64_MAX for the whole list).  scope: the rows of a subset
-// call (match_into_device).
+// call (match_into_device).  rank: a ranked call (match_list_device).
 frz_status match_list_host(frz_matcher* m, const frz_corpus* corpus, uint32_t index_offset, uint8_t sort, uint64_t limit,
-                           const SubsetScope& scope, frz_match* out, uint64_t cap, uint64_t* n_out, uint64_t* n_total) {
+                           const SubsetScope& scope, frz_match* out, uint64_t cap, uint64_t* n_out, uint64_t* n_total,
+                           const Ranking* rank = nullptr) {
     if (scope.none) {
         if (n_out) *n_out = 0;
         if (n_total) *n_total = 0;
@@ -1410,7 +1425,7 @@ frz_status match_list_host(frz_matcher* m, const frz_corpus* corpus, uint32_t in
     const uint32_t dev_limit = (uint32_t)std::min<uint64_t>(limit, kFrzNoLimit);   // a list never holds more than 2^32 - 1 matches
     frz_status s = FRZ_OK;
     for (int attempt = 0; attempt < 2; attempt++) {
-        s = match_list_device(m, corpus->st, index_offset, sort, &d_list, stream, &st, nullptr, dev_limit, scope);
+        s = match_list_device(m, corpus->st, index_offset, sort, &d_list, stream, &st, nullptr, dev_limit, scope, rank);
         if (s == FRZ_OK) s = copy_out(m, d_list, limit, out, cap, n_out, n_total, stream);
         if (s != kRetryOverflow) break;
         FRZ_TRY(ensure_workspace(m, corpus->st, std::max<uint64_t>(corpus->st.n, 1)));  // worst-case lists, then once more
@@ -1538,6 +1553,90 @@ extern "C" frz_status frz_match_list_subset_top(frz_matcher* m, const frz_corpus
     SubsetScope scope;
     FRZ_TRY(subset_scope(m, corpus, *s, nullptr, &scope));
     return match_list_host(m, corpus, 0, m->config.sort, k, scope, out, k, n_out, n_total);
+}
+
+// ---------------------------------------------------------------------------------- ranked calls
+// A signed 16-bit boost per index of one corpus, on its device.  Indices at and past `values.cap()` have boost 0.
+struct frz_boost {
+    const frz_corpus* corpus;
+    FrzDevArray<int16_t> values;
+    int32_t max_set = 0;   // the largest value ever set, at least 0: bounds every boost (the sort's key bound)
+};
+
+namespace {
+__global__ void k_boost_scatter(const uint2* __restrict__ set, uint64_t n, int16_t* __restrict__ values) {
+    for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x)
+        values[set[j].x] = (int16_t)set[j].y;
+}
+
+// b->values grows to `n` entries, the old values kept and the new ones zero (FrzDevArray drops its contents when it grows)
+frz_status grow_boost(frz_boost* b, uint64_t n) {
+    if (b->values.cap() >= n) return FRZ_OK;
+    FrzDevArray<int16_t> grown;
+    FRZ_TRY(grown.reserve(n));
+    FRZ_CUDA_TRY(cudaMemset(grown.get(), 0, n * sizeof(int16_t)));
+    if (b->values.cap())
+        FRZ_CUDA_TRY(cudaMemcpy(grown.get(), b->values.get(), b->values.cap() * sizeof(int16_t), cudaMemcpyDeviceToDevice));
+    b->values = std::move(grown);
+    return FRZ_OK;
+}
+}  // namespace
+
+extern "C" frz_status frz_boost_create(const frz_corpus* c, const int16_t* values, uint64_t n, frz_boost** out) {
+    if (!c || !out || (n && !values)) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    if (n > c->st.n)
+        return frz_fail(FRZ_ERR_INVALID_ARG, "%llu boost values for a corpus of %llu haystacks", (unsigned long long)n,
+                        (unsigned long long)c->st.n);
+    auto b = std::make_unique<frz_boost>();
+    b->corpus = c;
+    if (n) {
+        FRZ_TRY(frz_ensure_device(c->st.device));
+        FRZ_TRY(b->values.reserve(n));
+        FRZ_CUDA_TRY(cudaMemcpy(b->values.get(), values, n * sizeof(int16_t), cudaMemcpyHostToDevice));
+        b->max_set = std::max<int32_t>(0, *std::max_element(values, values + n));
+    }
+    *out = b.release();
+    return FRZ_OK;
+}
+
+extern "C" frz_status frz_boost_set(frz_boost* b, const uint32_t* which, const int16_t* values, uint64_t n) {
+    if (!b || (n && (!which || !values))) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    if (n == 0) return FRZ_OK;
+    FRZ_TRY(check_indices(b->corpus, which, n));
+    std::vector<uint2> set(n);
+    for (uint64_t j = 0; j < n; j++) set[j] = make_uint2(which[j], (uint32_t)(uint16_t)values[j]);
+    std::vector<uint32_t> sorted(which, which + n);
+    std::sort(sorted.begin(), sorted.end());
+    for (uint64_t j = 1; j < n; j++)
+        if (sorted[j] == sorted[j - 1]) return frz_fail(FRZ_ERR_INVALID_ARG, "index %u is set twice", sorted[j]);
+    FRZ_TRY(frz_ensure_device(b->corpus->st.device));
+    if (sorted.back() >= b->values.cap()) FRZ_TRY(grow_boost(b, b->corpus->st.n));
+    FrzDevArray<uint2> d_set;   // (index, value) pairs: one copy, one scatter
+    FRZ_TRY(d_set.reserve(n));
+    FRZ_CUDA_TRY(cudaMemcpy(d_set.get(), set.data(), n * sizeof(uint2), cudaMemcpyHostToDevice));
+    k_boost_scatter<<<grid_for(n, 256), 256>>>(d_set.get(), n, b->values.get());
+    FRZ_CUDA_TRY(cudaGetLastError());
+    FRZ_CUDA_TRY(cudaStreamSynchronize(nullptr));
+    b->max_set = std::max<int32_t>(b->max_set, *std::max_element(values, values + n));
+    return FRZ_OK;
+}
+
+extern "C" void frz_boost_destroy(frz_boost* b) { delete b; }
+
+extern "C" frz_status frz_match_list_ranked(frz_matcher* m, const frz_corpus* corpus, const frz_subset* s, const frz_boost* b,
+                                            uint64_t k, frz_match* out, uint64_t* n_out, uint64_t* n_total) {
+    if (!m || !corpus || !b) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    if (!out && k > 0) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
+    if (b->corpus != corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "the boost was made on another corpus");
+    if (s) FRZ_TRY(check_subset_call(m, corpus, s));
+    FRZ_TRY(frz_ensure_device(corpus->st.device));
+    SubsetScope scope;
+    if (s) FRZ_TRY(subset_scope(m, corpus, *s, nullptr, &scope));
+    Ranking rank;
+    rank.boost = b->values.get();
+    rank.n = (uint32_t)b->values.cap();
+    rank.max_boost = (uint32_t)b->max_set;
+    return match_list_host(m, corpus, 0, m->config.sort, k, scope, out, k, n_out, n_total, &rank);
 }
 
 extern "C" frz_status frz_match_list_into(frz_matcher* m, const frz_corpus* corpus, uint32_t index_offset, frz_match* out,

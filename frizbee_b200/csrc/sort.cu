@@ -24,6 +24,10 @@
 // Top-K calls (frz_match_list_top): the final scatter of every sort takes a limit and stores only the positions below it —
 // every element's final position is known before its store, so the first `limit` elements of the sorted list are exactly
 // the ones written.  Full sorts pass kFrzNoLimit.
+//
+// Ranked calls (frz_match_list_ranked) sort by a key in place of the score: k_sort_hist and k_sort_scatter take the digit
+// source as a template parameter (ScoreKey, BoostKey), and frz_launch_sort_by_key_dev runs the same one- or two-pass
+// histogram-kernel sort on clamp(score + boost[index], 0, 65535).  The elements keep their raw scores.
 #include "frz_device.cuh"
 #include "frz_host.h"
 
@@ -49,13 +53,29 @@ __device__ __forceinline__ void segment_of(unsigned long long n, int v, unsigned
     *hi = b < n ? b : n;
 }
 
-__device__ __forceinline__ uint32_t digit_of(const FrzMatchDev& m, int shift, uint32_t mask) {
-    return ((uint32_t)m.score >> shift) & mask;
+// The digit source of k_sort_hist / k_sort_scatter: the 16-bit key an element is sorted by.  Either way the element itself
+// is moved unchanged.
+struct ScoreKey {   // the score sort
+    __device__ __forceinline__ uint32_t operator()(const FrzMatchDev& m) const { return m.score; }
+};
+struct BoostKey {   // the ranked sort: clamp(score + boost[index], 0, 65535), boost 0 at and past index n
+    const int16_t* boost;
+    uint32_t n;
+    __device__ __forceinline__ uint32_t operator()(const FrzMatchDev& m) const {
+        const int b = m.index < n ? (int)__ldg(boost + m.index) : 0;
+        return (uint32_t)min(max((int)m.score + b, 0), 0xFFFF);
+    }
+};
+
+template <class Key>
+__device__ __forceinline__ uint32_t digit_of(const FrzMatchDev& m, int shift, uint32_t mask, const Key& key) {
+    return (key(m) >> shift) & mask;
 }
 
+template <class Key>
 __global__ void __launch_bounds__(kSortWarps * 32) k_sort_hist(const FrzMatchDev* __restrict__ in,
                                                                const unsigned long long* __restrict__ n_ptr, int shift,
-                                                               int bins, uint32_t* __restrict__ hist) {
+                                                               int bins, uint32_t* __restrict__ hist, Key key) {
     extern __shared__ uint32_t sm[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     uint32_t* cnt = sm + warp * bins;
@@ -69,12 +89,12 @@ __global__ void __launch_bounds__(kSortWarps * 32) k_sort_hist(const FrzMatchDev
     unsigned long long i = lo + lane;
     for (; i + 96 < hi; i += 128) {
         const FrzMatchDev a = in[i], b = in[i + 32], c = in[i + 64], d = in[i + 96];
-        atomicAdd(&cnt[digit_of(a, shift, mask)], 1u);
-        atomicAdd(&cnt[digit_of(b, shift, mask)], 1u);
-        atomicAdd(&cnt[digit_of(c, shift, mask)], 1u);
-        atomicAdd(&cnt[digit_of(d, shift, mask)], 1u);
+        atomicAdd(&cnt[digit_of(a, shift, mask, key)], 1u);
+        atomicAdd(&cnt[digit_of(b, shift, mask, key)], 1u);
+        atomicAdd(&cnt[digit_of(c, shift, mask, key)], 1u);
+        atomicAdd(&cnt[digit_of(d, shift, mask, key)], 1u);
     }
-    for (; i < hi; i += 32) atomicAdd(&cnt[digit_of(in[i], shift, mask)], 1u);
+    for (; i < hi; i += 32) atomicAdd(&cnt[digit_of(in[i], shift, mask, key)], 1u);
     __syncwarp();
     for (int d = lane; d < bins; d += 32) hist[(size_t)d * kV + v] = cnt[d];
 }
@@ -172,10 +192,11 @@ __global__ void __launch_bounds__(256) k_sort_scan_rows(uint32_t* __restrict__ h
     if (threadIdx.x == 0) *done_counter = 0;   // ready for the next pass
 }
 
+template <class Key>
 __global__ void __launch_bounds__(kSortWarps * 32) k_sort_scatter(const FrzMatchDev* __restrict__ in, FrzMatchDev* __restrict__ out,
                                                                   const unsigned long long* __restrict__ n_ptr, int shift, int bins,
                                                                   const uint32_t* __restrict__ hist,
-                                                                  const uint32_t* __restrict__ digit_base, uint32_t limit) {
+                                                                  const uint32_t* __restrict__ digit_base, uint32_t limit, Key key) {
     extern __shared__ uint32_t sm[];
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     uint32_t* cnt = sm + warp * bins;
@@ -196,7 +217,7 @@ __global__ void __launch_bounds__(kSortWarps * 32) k_sort_scatter(const FrzMatch
         const FrzMatchDev m = nxt;
         if (i + 32 < hi) nxt = in[i + 32];
         uint32_t d = (uint32_t)bins + lane;  // sentinel: matches nobody
-        if (valid) d = digit_of(m, shift, mask);
+        if (valid) d = digit_of(m, shift, mask, key);
         const uint32_t peers = __match_any_sync(0xffffffffu, d);
         const uint32_t rank = __popc(peers & ((1u << lane) - 1));
         uint32_t pos = 0;
@@ -283,16 +304,16 @@ __global__ void __launch_bounds__(kSegThreads) k_sort_scatter_seg(const FrzMatch
     }
 }
 
-}  // namespace
-
-// n_ptr: device pointer to the element count.  score_bound: host-known upper bound of any score.
-frz_status frz_launch_sort_by_score_dev(const FrzMatchDev* d_in, FrzMatchDev* d_tmp, FrzMatchDev* d_out,
-                                        const unsigned long long* n_ptr, uint32_t score_bound, FrzSortScratch& ss,
-                                        cudaStream_t stream, FrzLaunchStats* st, uint32_t limit) {
+// The histogram-kernel sort of the list at d_in by descending Key (stable): one pass when the key bound allows it, else
+// the reference's two 8-bit LSD passes.  n_ptr: device pointer to the element count.  bound: host-known upper bound of
+// any key.
+template <class Key>
+frz_status launch_sort_dev(const FrzMatchDev* d_in, FrzMatchDev* d_tmp, FrzMatchDev* d_out, const unsigned long long* n_ptr,
+                           uint32_t bound, Key key, FrzSortScratch& ss, cudaStream_t stream, FrzLaunchStats* st, uint32_t limit) {
     uint32_t* const hist = ss.hist.get();
     auto pass = [&](const FrzMatchDev* src, FrzMatchDev* dst, int shift, int bins, uint32_t keep) -> frz_status {
         const size_t smem = (size_t)kSortWarps * bins * sizeof(uint32_t);
-        k_sort_hist<<<kSortBlocks, kSortWarps * 32, smem, stream>>>(src, n_ptr, shift, bins, hist);
+        k_sort_hist<<<kSortBlocks, kSortWarps * 32, smem, stream>>>(src, n_ptr, shift, bins, hist, key);
         uint32_t* totals = hist + (size_t)kMaxBins * kV;
         uint32_t* digit_base = totals + kMaxBins;
         unsigned int* done_counter = reinterpret_cast<unsigned int*>(digit_base + kMaxBins);   // zeroed at allocation, self-resetting
@@ -302,17 +323,31 @@ frz_status frz_launch_sort_by_score_dev(const FrzMatchDev* d_in, FrzMatchDev* d_
             FRZ_CUDA_TRY(cudaEventRecord(ss.table_ev.get(), stream));
             ss.table_ev_recorded = true;
         }
-        k_sort_scatter<<<kSortBlocks, kSortWarps * 32, smem, stream>>>(src, dst, n_ptr, shift, bins, hist, digit_base, keep);
+        k_sort_scatter<<<kSortBlocks, kSortWarps * 32, smem, stream>>>(src, dst, n_ptr, shift, bins, hist, digit_base, keep, key);
         FRZ_CUDA_TRY(cudaGetLastError());
         if (st) st->launches += 3;
         return FRZ_OK;
     };
-    if (score_bound < 256) return pass(d_in, d_out, 0, 256, limit);
-    if (score_bound < 512) return pass(d_in, d_out, 0, 512, limit);
-    if (score_bound < 1024) return pass(d_in, d_out, 0, 1024, limit);
+    if (bound < 256) return pass(d_in, d_out, 0, 256, limit);
+    if (bound < 512) return pass(d_in, d_out, 0, 512, limit);
+    if (bound < 1024) return pass(d_in, d_out, 0, 1024, limit);
     // the reference's two 8-bit LSD passes (src/sort.rs:8-39); only the second one knows final positions
     FRZ_TRY(pass(d_in, d_tmp, 0, 256, kFrzNoLimit));
     return pass(d_tmp, d_out, 8, 256, limit);
+}
+
+}  // namespace
+
+frz_status frz_launch_sort_by_score_dev(const FrzMatchDev* d_in, FrzMatchDev* d_tmp, FrzMatchDev* d_out,
+                                        const unsigned long long* n_ptr, uint32_t score_bound, FrzSortScratch& ss,
+                                        cudaStream_t stream, FrzLaunchStats* st, uint32_t limit) {
+    return launch_sort_dev(d_in, d_tmp, d_out, n_ptr, score_bound, ScoreKey(), ss, stream, st, limit);
+}
+
+frz_status frz_launch_sort_by_key_dev(const FrzMatchDev* d_in, FrzMatchDev* d_tmp, FrzMatchDev* d_out,
+                                      const unsigned long long* n_ptr, const int16_t* boost, uint32_t n_boost, uint32_t key_bound,
+                                      FrzSortScratch& ss, cudaStream_t stream, FrzLaunchStats* st, uint32_t limit) {
+    return launch_sort_dev(d_in, d_tmp, d_out, n_ptr, key_bound, BoostKey{boost, n_boost}, ss, stream, st, limit);
 }
 
 // allocates the sort scratch on the current device: counts, totals, digit_base + the pass-completion counter of

@@ -286,6 +286,44 @@ FRZ_API frz_status frz_match_list_subset(frz_matcher* m, const frz_corpus* corpu
 FRZ_API frz_status frz_match_list_subset_top(frz_matcher* m, const frz_corpus* corpus, const frz_subset* s, uint64_t k,
                                              frz_match* out, uint64_t* n_out, uint64_t* n_total);
 
+/* ---------------------------------------------------------------- ranked calls
+ *
+ * Completion menus, history searches and file pickers rank rows by the fuzzy score plus a per-row prior (frecency,
+ * recency, pinned items).  The reference has no such method: its callers re-rank Matcher::match_list's output
+ * (src/matcher/mod.rs:212-222) themselves.  These calls replace that re-rank and return only the first k rows.
+ *
+ * A boost is a signed 16-bit value per index of a corpus, resident on the corpus's device; indices without a value have
+ * boost 0.  A row's key is clamp(score + boost[index], 0, 65535), computed in 32-bit arithmetic.
+ * frz_match_list_ranked(m, c, s, b, k) takes the rows of frz_match_list_into(m, c, 0) (restricted to the members of s
+ * as frz_match_list_subset does), reverses them under IndexDesc / ScoreThenIndexDesc, sorts them stably by descending
+ * key, and returns the first min(k, total) rows.  The rows are those of frz_match_list, bit for bit; only their order
+ * differs.  Equal keys keep index order (ascending, or descending for the *_DESC strategies); raw scores do not break
+ * ties.  Every strategy ranks by key, and the empty matcher ranks too: it lists the live rows by descending boost.  With
+ * an all-zero boost under ScoreThenIndexAsc / Desc the result equals frz_match_list_top(m, c, k).
+ *
+ * A boost belongs to the corpus it was made on: another corpus is FRZ_ERR_INVALID_ARG, and it must be destroyed before
+ * that corpus.  Ranked calls only read it, so several matchers may share one.  Boosts are kept by index across corpus
+ * edits: a removed row stops matching, a replaced row keeps its boost, and rows appended after frz_boost_create have
+ * boost 0 until frz_boost_set gives them one. */
+typedef struct frz_boost frz_boost;
+/* The reference has no such method (see above).  values[i] is the boost of index i for i < n; the others are 0.
+ * n > frz_corpus_len(c), or NULL values with n > 0, is FRZ_ERR_INVALID_ARG; n == 0 is an all-zero boost. */
+FRZ_API frz_status frz_boost_create(const frz_corpus* c, const int16_t* values, uint64_t n, frz_boost** out);
+/* The reference has no such method (see above).  boost[which[j]] = values[j] for j < n.  An index >=
+ * frz_corpus_len(c) at the time of the call (rows appended since creation may be set), a duplicate index, or NULL arrays
+ * with n > 0 is FRZ_ERR_INVALID_ARG; every argument is checked before anything changes, so a refused call leaves the
+ * boost as it was.  n == 0 does nothing.  Synchronous; it must not run concurrently with a ranked call reading b. */
+FRZ_API frz_status frz_boost_set(frz_boost* b, const uint32_t* which, const int16_t* values, uint64_t n);
+FRZ_API void frz_boost_destroy(frz_boost* b);
+/* The reference has no such method (see above).  The first min(k, total) rows ranked by key; *n_total = total (may be
+ * NULL).  s: NULL for the whole corpus, or a subset of the same corpus.  Same rules as frz_match_list_top: `out` is HOST
+ * memory with room for k matches (min(k, frz_corpus_len(c)) suffices, or min(k, frz_subset_len(s)) with a subset),
+ * k = 0 only counts, k = UINT64_MAX ranks the whole list, a NULL `out` with k > 0 is FRZ_ERR_INVALID_ARG, and the call
+ * never returns FRZ_ERR_CAPACITY.  A NULL matcher, corpus or boost, or a boost or subset of another corpus, is
+ * FRZ_ERR_INVALID_ARG. */
+FRZ_API frz_status frz_match_list_ranked(frz_matcher* m, const frz_corpus* c, const frz_subset* s, const frz_boost* b,
+                                         uint64_t k, frz_match* out, uint64_t* n_out, uint64_t* n_total);
+
 /* Specialized::match_list / Matcher::match_list_into (src/matcher/algo.rs:17-22,
  * src/matcher/mod.rs:373-392): matches appended in input (index-ascending) order,
  * indices offset by `index_offset`, no sort. */
