@@ -374,27 +374,42 @@ __global__ void __launch_bounds__(kScanThreads, 6) k_sig_scan(const FrzCorpusVie
 // Stage 1 of the whole-corpus byte path  k_scan_window — the signature scan of k_sig_scan and the exact reference
 // window (process_candidate) in one persistent kernel.  The scan keeps HBM busy and leaves the ALUs idle, the window
 // machine the other way round; in one kernel an SM's warps do both at once, and the candidates never leave the SM.
-// Each warp:
-//   - walks its statically strided 128-slot chunks like k_sig_scan (TMA stages, per-warp mbarriers) and appends the
-//     records of the haystacks that pass the length gate and the signature test to its shared-memory ring;
-//   - after each chunk, takes every 32 records in the ring as a BATCH (lane per candidate): their haystack units travel
-//     global → shared with cp.async while the warp scans on, and the batch is windowed and emitted when the next one is
-//     taken (or at the end).  The chunk's TMA refill is issued before any batch runs, so the warp's DRAM requests stay
-//     in flight (bulk copies hold no registers) while it runs the state machine.
+// The two jobs run on different warps of a block, so that each runs at its own rate:
+//   - the PRODUCER warp (warp 0) walks the block's statically strided 128-slot chunks like k_sig_scan (kProdStages TMA
+//     stages on its own mbarriers, each refilled as soon as it has been read) and appends the records of the haystacks
+//     that pass the length gate and the signature test to the block's candidate QUEUE: kQueueSlots slots of 32 records,
+//     each with a "full" and an "empty" mbarrier.  A full slot is published as one batch; when every slot is taken the
+//     producer waits for one to be freed (backpressure, nothing is dropped).  At the end it publishes the last partial
+//     batch and one empty batch per window warp as the done marker.
+//   - each WINDOW warp claims the next batch (a shared counter), copies its records to registers (lane per candidate) and
+//     frees the slot, starts the cp.async copies of their haystack units into one of its two unit stages, and then windows
+//     and emits the batch it claimed before — so one batch's units are in flight while the warp runs the other.
 // Haystacks of more than four units (staged == false) are read by the mask builders straight from the corpus.
-constexpr int kFusedStages = 2;   // TMA stages per warp: two keep four blocks per SM within the shared memory
+constexpr int kWinWarps = 3;                           // window warps per block, after the producer warp
+constexpr int kScanWinThreads = 32 * (1 + kWinWarps);
+constexpr int kProdStages = 6;                         // TMA stages of the producer warp
+constexpr int kQueueSlots = 8;                         // 32-record batch slots of the candidate queue (a power of two)
+// a window warp waits for at most one batch, so batch b's slot was freed by batch b - kQueueSlots before b is claimed
+static_assert(kQueueSlots >= kWinWarps && (kQueueSlots & (kQueueSlots - 1)) == 0, "queue slots");
 struct WinStage {
     uint4 units[32][5];   // [lane][unit]: the lane's four units contiguous like in the packed corpus; the fifth pads the row
                           // to 80 bytes, which makes the warp's 16-byte accesses bank-conflict-free (rows of 64 would be 4-way)
 };
-struct __align__(16) ScanWinSmem {   // one warp's part of the dynamic shared memory
-    CandRec ring[kScanRing];         // at most 31 left over + 128 new records between two batch takes
-    ScanStage stage[kFusedStages];
-    WinStage win;
-    uint64_t bar[kFusedStages];
+struct __align__(16) ScanWinSmem {   // the block's dynamic shared memory, before the occurrence tables
+    ScanStage stage[kProdStages];
+    CandRec queue[kQueueSlots * 32];
+    WinStage win[kWinWarps][2];
+    uint64_t stage_bar[kProdStages];
+    uint64_t full_bar[kQueueSlots];    // 32 arrivals (the producer's lanes): the slot holds a batch
+    uint64_t empty_bar[kQueueSlots];   // 32 arrivals (the consuming warp's lanes): the slot's records are in registers
+    uint32_t queue_n[kQueueSlots];     // records in the slot's batch; 0 = no more batches
+    uint32_t next_batch;               // the window warps' claim counter
 };
-// The kWarps ScanWinSmem are followed by one occurrence table per warp (OccTable's layout) of `occ_rows` rows: only the
-// rows the mask builders touch, n_distinct (+ n for the single-chunk forms' position masks).
+// ScanWinSmem is followed by one occurrence table per window warp (OccTable's layout) of `occ_rows` rows: only the rows
+// the mask builders touch, n_distinct (+ n for the single-chunk forms' position masks).
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
 
 // The needle as process_candidate reads it: the pattern itself, or (LONG) the block's staged copy of its FrzNeedleTab.
 template <bool LONG>
@@ -405,53 +420,127 @@ __device__ __forceinline__ std::conditional_t<LONG, LongPat, const FrzPatternDev
 }
 
 // k_scan_window (needles of up to FRZ_MAX_NEEDLE bytes) and k_scan_window_long (longer needles: the dynamic shared memory
-// holds the needle table after the warps' parts, where the occurrence tables would be — a long needle has none).
+// holds the needle table after ScanWinSmem, where the occurrence tables would be — a long needle has none).
 template <int MODE, bool LONG>
 __device__ __forceinline__ void scan_window(const FrzCorpusView& cv, const FrzPatternDev& pat, int use_sig, int occ_rows,
                                             const FrzSurvLists& lists, unsigned long long surv_cap,
                                             uint32_t* __restrict__ surv_bitmap, FrzCounters* __restrict__ ctr,
                                             const FrzNeedleTab* ntab) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
+    frz_allow_dependent_launch();
     const uint32_t lane = frz_lane(), warp = threadIdx.x >> 5;
-    ScanWinSmem& sm = reinterpret_cast<ScanWinSmem*>(smem_raw)[warp];
-    uint2 (*occ)[32] = reinterpret_cast<uint2 (*)[32]>(smem_raw + sizeof(ScanWinSmem) * kWarps) + (size_t)warp * occ_rows;
+    ScanWinSmem& sm = *reinterpret_cast<ScanWinSmem*>(smem_raw);
     __shared__ uint8_t cid_s[FRZ_MAX_NEEDLE];
     if (threadIdx.x < FRZ_MAX_NEEDLE) cid_s[threadIdx.x] = pat.cid[threadIdx.x];
-    const auto& pv = needle_view<LONG>(pat, ntab, smem_raw + sizeof(ScanWinSmem) * kWarps);
-    if (lane == 0)
-        for (int i = 0; i < kFusedStages; i++) mbar_init(&sm.bar[i], 1);
+    const auto& pv = needle_view<LONG>(pat, ntab, smem_raw + sizeof(ScanWinSmem));
+    if (threadIdx.x == 0) {
+        for (int i = 0; i < kProdStages; i++) mbar_init(&sm.stage_bar[i], 1);
+        for (int i = 0; i < kQueueSlots; i++) {
+            mbar_init(&sm.full_bar[i], 32);
+            mbar_init(&sm.empty_bar[i], 32);
+        }
+        sm.next_batch = 0;
+    }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     __syncthreads();
+    const uint4 none = make_uint4(0xFFFFFFFFu, 0u, 0u, 0u);
+    uint4* queue = reinterpret_cast<uint4*>(sm.queue);
+    if (warp == 0) {   // ---- producer
+        const uint32_t total_chunks = cv.n_tiles * (FRZ_TILE / 128);   // 128 slots (4 groups) per chunk
+        const uint32_t tx_bytes = (uint32_t)(sizeof(uint32_t) * 128 + sizeof(FrzGroupDesc) * 4) + (use_sig ? (uint32_t)sizeof(uint2) * 128 : 0u);
+        uint32_t req = blockIdx.x;   // next chunk to REQUEST
+        auto issue = [&](int st) {
+            if (req < total_chunks && lane == 0) {
+                const uint64_t slot0 = (uint64_t)req * 128;
+                mbar_expect_tx(&sm.stage_bar[st], tx_bytes);
+                bulk_g2s(sm.stage[st].meta, cv.slot_meta + slot0, (uint32_t)sizeof(uint32_t) * 128, &sm.stage_bar[st]);
+                if (use_sig) bulk_g2s(sm.stage[st].sig, cv.slot_sig + slot0, (uint32_t)sizeof(uint2) * 128, &sm.stage_bar[st]);
+                bulk_g2s(sm.stage[st].desc, cv.groups + (size_t)req * 4, (uint32_t)sizeof(FrzGroupDesc) * 4, &sm.stage_bar[st]);
+            }
+            req += gridDim.x;
+        };
+        uint32_t count = 0;       // records appended so far; record r goes to queue[r % (kQueueSlots * 32)], batch r / 32
+        uint32_t acquired = 0;    // batches whose slot may be written
+        uint32_t published = 0;   // batches handed to the window warps
+        auto acquire = [&](uint32_t upto) {   // makes batches < upto writable: batch b reuses the slot of batch b - kQueueSlots
+            for (; acquired < upto; acquired++)
+                if (acquired >= (uint32_t)kQueueSlots)
+                    mbar_wait(&sm.empty_bar[acquired % kQueueSlots], (acquired / kQueueSlots - 1) & 1);
+        };
+        auto publish = [&](uint32_t n) {   // every lane arrives after its own record stores
+            if (lane == 0) sm.queue_n[published % kQueueSlots] = n;
+            mbar_arrive(&sm.full_bar[published % kQueueSlots]);
+            published++;
+        };
+        // length gate + signature test of one slot
+        auto test_slot = [&](uint32_t m, uint32_t p1, uint32_t p2) {
+            bool pass = m != FRZ_INVALID_SLOT && (int)(m >> FRZ_TILE_SHIFT) >= pat.min_hay_len;
+            if (use_sig) pass = pass && frz_sig_pass(pat.sig_need1, pat.sig_need2, pat.sig_k, p1, p2);
+            return pass;
+        };
+        // a passing lane appends its record behind the chunk's `before` earlier records
+        auto put = [&](uint32_t ballot, uint32_t before, uint32_t m, uint32_t slot_global, unsigned long long unit0) {
+            if (ballot >> lane & 1u)
+                queue[(count + before + __popc(ballot & ((1u << lane) - 1))) & (kQueueSlots * 32 - 1)] =
+                    make_uint4(slot_global, m, (uint32_t)unit0, (uint32_t)(unit0 >> 32));
+        };
+#pragma unroll
+        for (int i = 0; i < kProdStages; i++) issue(i);
+        int st = 0;
+        uint32_t parity = 0;
+        for (uint32_t cur = blockIdx.x; cur < total_chunks; cur += gridDim.x) {
+            mbar_wait(&sm.stage_bar[st], parity);
+            const uint4 meta = reinterpret_cast<const uint4*>(sm.stage[st].meta)[lane];
+            uint4 sig0 = make_uint4(0u, 0u, 0u, 0u), sig1 = sig0;
+            if (use_sig) {
+                sig0 = reinterpret_cast<const uint4*>(sm.stage[st].sig)[2 * lane];
+                sig1 = reinterpret_cast<const uint4*>(sm.stage[st].sig)[2 * lane + 1];
+            }
+            const unsigned long long grp_off = sm.stage[st].desc[lane >> 3].abs_off;
+            const uint32_t gunits = sm.stage[st].desc[lane >> 3].gunits;
+            __syncwarp();
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic reads of the stage before its async refill
+            issue(st);
+            // lane L owns slots 4L .. 4L+3 of the chunk, all in group L / 8
+            const uint32_t slot_g = cur * 128 + lane * 4;                   // == tile << 10 | slot of this lane's first slot
+            const unsigned long long unit0 = grp_off + (unsigned long long)((lane * 4) & 31) * gunits;   // slot-major group
+            // the four tests are independent: one queue acquisition and one publication per chunk
+            const uint32_t b0 = __ballot_sync(0xffffffffu, test_slot(meta.x, sig0.x, sig0.y));
+            const uint32_t b1 = __ballot_sync(0xffffffffu, test_slot(meta.y, sig0.z, sig0.w));
+            const uint32_t b2 = __ballot_sync(0xffffffffu, test_slot(meta.z, sig1.x, sig1.y));
+            const uint32_t b3 = __ballot_sync(0xffffffffu, test_slot(meta.w, sig1.z, sig1.w));
+            const uint32_t n0 = __popc(b0), n01 = n0 + __popc(b1), n012 = n01 + __popc(b2), n = n012 + __popc(b3);
+            if (n) {
+                acquire((count + n + 31) / 32);
+                put(b0, 0, meta.x, slot_g, unit0);
+                put(b1, n0, meta.y, slot_g + 1, unit0 + gunits);
+                put(b2, n01, meta.z, slot_g + 2, unit0 + 2 * gunits);
+                put(b3, n012, meta.w, slot_g + 3, unit0 + 3 * gunits);
+                count += n;
+                while (published < count / 32) publish(32);
+            }
+            if (++st == kProdStages) { st = 0; parity ^= 1; }
+        }
+        if (count % 32) publish(count % 32);   // partial batch: lanes >= its size are inactive
+        for (int w = 0; w < kWinWarps; w++) {  // the done markers: every window warp stops at the first it claims
+            acquire(published + 1);
+            publish(0);
+        }
+        return;
+    }
+    // ---- window warps
+    const uint32_t ww = warp - 1;
+    uint2 (*occ)[32] = reinterpret_cast<uint2 (*)[32]>(smem_raw + sizeof(ScanWinSmem)) + (size_t)ww * occ_rows;
     const bool staged = cv.max_gunits <= 4;   // every haystack fits the four staged units
     // (single_chunk_ok implies occ_rows > 0.  Testing that kernel argument first keeps the FRZ_T_0 / FRZ_T_1 code that
     // CUDA 12.9's ptxas schedules best: when the first test is on max_gunits, the prefilter stage of the max_typos=1
     // benchmark measured about 4% slower on an H100 SXM at 400 W.)
     const bool single = (MODE == FRZ_T_0 || MODE == FRZ_T_1) && occ_rows > 0 && single_chunk_ok(pat, cv.max_gunits);
-    const uint32_t n_warps = gridDim.x * kWarps;
-    const uint32_t total_chunks = cv.n_tiles * (FRZ_TILE / 128);   // 128 slots (4 groups) per chunk
-    const uint32_t tx_bytes = (uint32_t)(sizeof(uint32_t) * 128 + sizeof(FrzGroupDesc) * 4) + (use_sig ? (uint32_t)sizeof(uint2) * 128 : 0u);
-    uint32_t req = blockIdx.x * kWarps + warp;   // next chunk to REQUEST
-    auto issue = [&](int st) {
-        if (req < total_chunks && lane == 0) {
-            const uint64_t slot0 = (uint64_t)req * 128;
-            mbar_expect_tx(&sm.bar[st], tx_bytes);
-            bulk_g2s(sm.stage[st].meta, cv.slot_meta + slot0, (uint32_t)sizeof(uint32_t) * 128, &sm.bar[st]);
-            if (use_sig) bulk_g2s(sm.stage[st].sig, cv.slot_sig + slot0, (uint32_t)sizeof(uint2) * 128, &sm.bar[st]);
-            bulk_g2s(sm.stage[st].desc, cv.groups + (size_t)req * 4, (uint32_t)sizeof(FrzGroupDesc) * 4, &sm.bar[st]);
-        }
-        req += n_warps;
-    };
-    uint4* ring = reinterpret_cast<uint4*>(sm.ring);
-    uint32_t head = 0, count = 0;
-    // the batch whose units are in flight: this lane's candidate record (x == 0xFFFFFFFF: none)
-    uint4 batch = make_uint4(0xFFFFFFFFu, 0u, 0u, 0u);
-    bool batch_pending = false;
     Emit pending;
     pending.ok = false; pending.cls = 0; pending.peers = 0; pending.base_raw = 0;
     pending.rec.tile = 0; pending.rec.slot_rank = 0; pending.rec.start = 0; pending.rec.end = 0;
-    auto run_batch = [&]() {
-        __pipeline_wait_prior(0);
-        __syncwarp();
+    // windows and emits one batch: this lane's candidate record (x == 0xFFFFFFFF: none), its units in unit stage `ws`
+    auto run_batch = [&](const uint4& batch, int ws) {
         const bool active = batch.x != 0xFFFFFFFFu;
         Cand cd;
         cd.tile = batch.x >> FRZ_TILE_SHIFT;
@@ -459,7 +548,7 @@ __device__ __forceinline__ void scan_window(const FrzCorpusView& cv, const FrzPa
         cd.li = batch.y & (FRZ_TILE - 1);
         cd.len = (int)(batch.y >> FRZ_TILE_SHIFT);
         cd.base = cv.data + (((unsigned long long)batch.w << 32) | batch.z);
-        cd.units = staged ? &sm.win.units[lane][0] : cd.base;
+        cd.units = staged ? &sm.win[ww][ws].units[lane][0] : cd.base;
         Emit cur;
         process_candidate<MODE>(cv, pv, cid_s, occ, cd, active, surv_bitmap, &cur, single);
         emit_commit(pending, lists, surv_cap, ctr);      // the previous batch's list space has arrived by now
@@ -467,78 +556,54 @@ __device__ __forceinline__ void scan_window(const FrzCorpusView& cv, const FrzPa
         pending = cur;
         __syncwarp();
     };
-    // the n (<= 32) oldest ring records become the next batch; the previous batch runs first (one unit stage)
-    auto take_batch = [&](uint32_t n) {
-        if (batch_pending) run_batch();
-        batch = lane < n ? ring[(head + lane) & (kScanRing - 1)] : make_uint4(0xFFFFFFFFu, 0u, 0u, 0u);
-        head = (head + n) & (kScanRing - 1);
-        count -= n;
+    uint4 prev = none;   // the claimed batch whose units are in flight
+    int prev_ws = -1;
+    for (;;) {
+        uint32_t b = 0;
+        if (lane == 0) b = atomicAdd(&sm.next_batch, 1u);
+        b = __shfl_sync(0xffffffffu, b, 0);
+        const uint32_t s = b % kQueueSlots;
+        mbar_wait(&sm.full_bar[s], (b / kQueueSlots) & 1);
+        const uint32_t n = sm.queue_n[s];
+        const uint4 batch = lane < n ? queue[s * 32 + lane] : none;
+        mbar_arrive(&sm.empty_bar[s]);
+        if (n == 0) break;
+        const int ws = prev_ws < 0 ? 0 : prev_ws ^ 1;
         if (staged && batch.x != 0xFFFFFFFFu) {
             const int units = ((int)(batch.y >> FRZ_TILE_SHIFT) + 15) >> 4;
             const uint4* base = cv.data + (((unsigned long long)batch.w << 32) | batch.z);
 #pragma unroll
             for (int k = 0; k < 4; k++)
-                if (k < units) __pipeline_memcpy_async(&sm.win.units[lane][k], base + k, 16);
+                if (k < units) __pipeline_memcpy_async(&sm.win[ww][ws].units[lane][k], base + k, 16);
         }
         __pipeline_commit();
-        batch_pending = true;
-    };
-    // length gate + signature test of one slot; passing lanes append their record to the ring
-    auto test_slot = [&](uint32_t m, uint32_t p1, uint32_t p2, uint32_t slot_global, unsigned long long unit0) {
-        bool pass = m != FRZ_INVALID_SLOT && (int)(m >> FRZ_TILE_SHIFT) >= pat.min_hay_len;
-        if (use_sig) pass = pass && frz_sig_pass(pat.sig_need1, pat.sig_need2, pat.sig_k, p1, p2);
-        const uint32_t ballot = __ballot_sync(0xffffffffu, pass);
-        if (pass)
-            ring[(head + count + __popc(ballot & ((1u << lane) - 1))) & (kScanRing - 1)] =
-                make_uint4(slot_global, m, (uint32_t)unit0, (uint32_t)(unit0 >> 32));
-        count += __popc(ballot);
-    };
-    uint32_t cur = req;
-#pragma unroll
-    for (int i = 0; i < kFusedStages; i++) issue(i);
-    int st = 0;
-    uint32_t parity = 0;
-    while (cur < total_chunks) {
-        mbar_wait(&sm.bar[st], parity);
-        const uint4 meta = reinterpret_cast<const uint4*>(sm.stage[st].meta)[lane];
-        uint4 sig0 = make_uint4(0u, 0u, 0u, 0u), sig1 = sig0;
-        if (use_sig) {
-            sig0 = reinterpret_cast<const uint4*>(sm.stage[st].sig)[2 * lane];
-            sig1 = reinterpret_cast<const uint4*>(sm.stage[st].sig)[2 * lane + 1];
+        if (prev_ws >= 0) {
+            __pipeline_wait_prior(1);
+            __syncwarp();
+            run_batch(prev, prev_ws);
         }
-        const unsigned long long grp_off = sm.stage[st].desc[lane >> 3].abs_off;
-        const uint32_t gunits = sm.stage[st].desc[lane >> 3].gunits;
-        __syncwarp();
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic reads of the stage before its async refill
-        issue(st);
-        // lane L owns slots 4L .. 4L+3 of the chunk, all in group L / 8
-        const uint32_t slot_g = cur * 128 + lane * 4;                   // == tile << 10 | slot of this lane's first slot
-        const unsigned long long unit0 = grp_off + (unsigned long long)((lane * 4) & 31) * gunits;   // slot-major group
-        test_slot(meta.x, sig0.x, sig0.y, slot_g, unit0);
-        test_slot(meta.y, sig0.z, sig0.w, slot_g + 1, unit0 + gunits);
-        test_slot(meta.z, sig1.x, sig1.y, slot_g + 2, unit0 + 2 * gunits);
-        test_slot(meta.w, sig1.z, sig1.w, slot_g + 3, unit0 + 3 * gunits);
-        __syncwarp();
-        while (count >= 32) take_batch(32);
-        cur += n_warps;
-        if (++st == kFusedStages) { st = 0; parity ^= 1; }
+        prev = batch;
+        prev_ws = ws;
     }
-    if (count) take_batch(count);   // partial batch: lanes >= count are inactive
-    if (batch_pending) run_batch();
+    if (prev_ws >= 0) {
+        __pipeline_wait_prior(0);
+        __syncwarp();
+        run_batch(prev, prev_ws);
+    }
     emit_commit(pending, lists, surv_cap, ctr);
 }
 template <int MODE>
-__global__ void __launch_bounds__(kThreads, 4) k_scan_window(const FrzCorpusView cv, const __grid_constant__ FrzPatternDev pat,
-                                                             int use_sig, int occ_rows, const FrzSurvLists lists,
-                                                             unsigned long long surv_cap, uint32_t* __restrict__ surv_bitmap,
-                                                             FrzCounters* __restrict__ ctr) {
+__global__ void __launch_bounds__(kScanWinThreads, 5) k_scan_window(const FrzCorpusView cv, const __grid_constant__ FrzPatternDev pat,
+                                                                    int use_sig, int occ_rows, const FrzSurvLists lists,
+                                                                    unsigned long long surv_cap, uint32_t* __restrict__ surv_bitmap,
+                                                                    FrzCounters* __restrict__ ctr) {
     scan_window<MODE, false>(cv, pat, use_sig, occ_rows, lists, surv_cap, surv_bitmap, ctr, nullptr);
 }
 template <int MODE>
-__global__ void __launch_bounds__(kThreads, 4) k_scan_window_long(const FrzCorpusView cv, const __grid_constant__ FrzPatternDev pat,
-                                                                  int use_sig, int occ_rows, const FrzSurvLists lists,
-                                                                  unsigned long long surv_cap, uint32_t* __restrict__ surv_bitmap,
-                                                                  FrzCounters* __restrict__ ctr, const FrzNeedleTab* ntab) {
+__global__ void __launch_bounds__(kScanWinThreads, 5) k_scan_window_long(const FrzCorpusView cv, const __grid_constant__ FrzPatternDev pat,
+                                                                         int use_sig, int occ_rows, const FrzSurvLists lists,
+                                                                         unsigned long long surv_cap, uint32_t* __restrict__ surv_bitmap,
+                                                                         FrzCounters* __restrict__ ctr, const FrzNeedleTab* ntab) {
     scan_window<MODE, true>(cv, pat, use_sig, occ_rows, lists, surv_cap, surv_bitmap, ctr, ntab);
 }
 
@@ -833,19 +898,19 @@ frz_status frz_launch_prefilter(const FrzCorpusView& cv, const FrzPatternDev& pa
     const int use_sig = pat.typo_mode != FRZ_T_NONE && pat.sig_on;
     const int occ_rows = pat.n_distinct ? std::min(kMaxDistinct, pat.n_distinct + pat.n) : 0;
     const uint32_t total_chunks = cv.n_tiles * (FRZ_TILE / 128);
-    if (pat.n > FRZ_MAX_NEEDLE) {   // long needle (n_distinct 0: no occurrence tables), the table after the warps' parts
-        const size_t smem = sizeof(ScanWinSmem) * kWarps + kLongPatSmem;
+    if (pat.n > FRZ_MAX_NEEDLE) {   // long needle (n_distinct 0: no occurrence tables), the table after ScanWinSmem
+        const size_t smem = sizeof(ScanWinSmem) + kLongPatSmem;
 #define FRZ_PF_LAUNCH_LONG(MODE)                                                                                          \
     do {                                                                                                                 \
         static int bps_dev[64] = {};                                                                                     \
         int& bps = bps_dev[frz_current_device() & 63];                                                                   \
         if (!bps) {                                                                                                      \
             FRZ_CUDA_TRY(cudaFuncSetAttribute(k_scan_window_long<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-            FRZ_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_scan_window_long<MODE>, kThreads, smem)); \
+            FRZ_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_scan_window_long<MODE>, kScanWinThreads, smem)); \
             if (bps < 1) bps = 1;                                                                                        \
         }                                                                                                                \
-        const uint32_t grid = std::max<uint32_t>(1, std::min<uint32_t>((uint32_t)(sms * bps), (total_chunks + kWarps - 1) / kWarps)); \
-        k_scan_window_long<MODE><<<grid, kThreads, smem, stream>>>(cv, pat, use_sig, 0, ws.lists(), ws.survivor_cap(),     \
+        const uint32_t grid = std::max<uint32_t>(1, std::min<uint32_t>((uint32_t)(sms * bps), total_chunks));   /* a producer per block */ \
+        k_scan_window_long<MODE><<<grid, kScanWinThreads, smem, stream>>>(cv, pat, use_sig, 0, ws.lists(), ws.survivor_cap(),     \
                                                                    ws.surv_bitmap.get(), ws.counters.get(), ntab);                   \
     } while (0)
         switch (pat.typo_mode) {
@@ -862,19 +927,19 @@ frz_status frz_launch_prefilter(const FrzCorpusView& cv, const FrzPatternDev& pa
         if (st) st->launches++;
         return FRZ_OK;
     }
-    const size_t smem = (sizeof(ScanWinSmem) + sizeof(uint2) * 32 * occ_rows) * kWarps;
-    const size_t smem_max = (sizeof(ScanWinSmem) + sizeof(OccTable)) * kWarps;
+    const size_t smem = sizeof(ScanWinSmem) + sizeof(uint2) * 32 * occ_rows * kWinWarps;
+    const size_t smem_max = sizeof(ScanWinSmem) + sizeof(OccTable) * kWinWarps;
 #define FRZ_PF_LAUNCH(MODE)                                                                                              \
     do {                                                                                                                 \
         static int bps_dev[64][kMaxDistinct + 1] = {};   /* blocks per SM by device and occurrence-table rows */         \
         int& bps = bps_dev[frz_current_device() & 63][occ_rows];                                                         \
         if (!bps) {                                                                                                      \
             FRZ_CUDA_TRY(cudaFuncSetAttribute(k_scan_window<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max)); \
-            FRZ_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_scan_window<MODE>, kThreads, smem));      \
+            FRZ_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_scan_window<MODE>, kScanWinThreads, smem)); \
             if (bps < 1) bps = 1;                                                                                        \
         }                                                                                                                \
-        const uint32_t grid = std::max<uint32_t>(1, std::min<uint32_t>((uint32_t)(sms * bps), (total_chunks + kWarps - 1) / kWarps)); \
-        k_scan_window<MODE><<<grid, kThreads, smem, stream>>>(cv, pat, use_sig, occ_rows, ws.lists(), ws.survivor_cap(),   \
+        const uint32_t grid = std::max<uint32_t>(1, std::min<uint32_t>((uint32_t)(sms * bps), total_chunks));   /* a producer per block */ \
+        k_scan_window<MODE><<<grid, kScanWinThreads, smem, stream>>>(cv, pat, use_sig, occ_rows, ws.lists(), ws.survivor_cap(),   \
                                                               ws.surv_bitmap.get(), ws.counters.get());                              \
     } while (0)
     switch (pat.typo_mode) {
