@@ -91,6 +91,11 @@ def lib():
     L.frz_matcher_last_timings.argtypes = [vp, C.POINTER(C.c_float), C.POINTER(u64)]
     L.frz_match_list.argtypes = [vp, vp, vp, u64, C.POINTER(u64)]
     L.frz_match_list_top.argtypes = [vp, vp, u64, vp, C.POINTER(u64), C.POINTER(u64)]
+    L.frz_match_list_batch_top.argtypes = [vp, u64, vp, u64, vp, vp, vp]
+    L.frz_debug_batch_limits.argtypes = [u64, u64]
+    L.frz_debug_batch_limits.restype = None
+    L.frz_debug_batch_last.argtypes = [vp]
+    L.frz_debug_batch_last.restype = None
     L.frz_subset_create.argtypes = [vp, vp, u64, C.POINTER(vp)]
     L.frz_subset_len.restype = u64
     L.frz_subset_len.argtypes = [vp]
@@ -514,6 +519,31 @@ class Matcher:
             self.close()
         except Exception:
             pass
+
+
+def match_list_batch_top(matchers, corpus: Corpus, k: int) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """frz_match_list_batch_top: every matcher's match_list_top_array(corpus, k) in one call.  Returns a (q, k) array of
+    MATCH_DTYPE (row j's first n_out[j] entries are matcher j's rows; the rest are zero), n_out and n_total (int64, length q)."""
+    q, k = len(matchers), int(k)
+    handles = (C.c_void_p * max(q, 1))(*[m._h.value for m in matchers])
+    out = np.zeros((q, k), dtype=MATCH_DTYPE)
+    n_out = np.zeros(q, dtype=np.uint64)
+    n_total = np.zeros(q, dtype=np.uint64)
+    _check(lib().frz_match_list_batch_top(handles, q, corpus._h, k, out.ctypes.data if out.size else None, n_out.ctypes.data,
+                                          n_total.ctypes.data))
+    return out, n_out.astype(np.int64), n_total.astype(np.int64)
+
+
+def batch_last() -> dict:
+    """Test aid (frz_debug_batch_last): what this thread's last match_list_batch_top did."""
+    v = np.zeros(4, dtype=np.uint64)
+    lib().frz_debug_batch_last(v.ctypes.data)
+    return {"batched": int(v[0]), "overflowed": int(v[1]), "sub_batches": int(v[2]), "launches": int(v[3])}
+
+
+def batch_limits(max_rows: int = 0, min_queries: int = 0):
+    """Test aid (frz_debug_batch_limits): the batched path's corpus-size and query-count limits; 0 restores a default."""
+    lib().frz_debug_batch_limits(int(max_rows), int(min_queries))
 
 
 def radix_sort_matches(arr: np.ndarray, device: int = 0) -> np.ndarray:

@@ -1,0 +1,116 @@
+// batch.cu — the last stage of a batched top-K sub-batch (frz_match_list_batch_top, DESIGN.md §4.11): every query's first
+// min(k, total) rows out of its index-ordered list, in one launch of one block per query.  The position arithmetic is
+// batch_plan.cuh's (shared with the CPU tests).
+#include "frz_device.cuh"
+
+#include "batch_plan.cuh"
+#include "frz_host.h"
+
+namespace {
+
+constexpr int kTopThreads = 1024;
+static_assert(kFrzBatchMaxK <= kTopThreads, "one kept row per thread in the sort");
+
+// exclusive count of the block's threads before this one with `f` set, and the block's count in *all (every thread)
+__device__ __forceinline__ uint32_t block_excl_count(bool f, uint32_t* warp_cnt, uint32_t* all) {
+    const uint32_t lane = frz_lane(), warp = threadIdx.x >> 5;
+    const uint32_t ballot = __ballot_sync(0xffffffffu, f);
+    if (lane == 0) warp_cnt[warp] = __popc(ballot);
+    __syncthreads();
+    uint32_t before = 0, sum = 0;
+    for (uint32_t w = 0; w < blockDim.x / 32; w++) {
+        const uint32_t c = warp_cnt[w];
+        before += w < warp ? c : 0;
+        sum += c;
+    }
+    __syncthreads();   // warp_cnt is reused by the next call
+    *all = sum;
+    return before + __popc(ballot & ((1u << lane) - 1));
+}
+
+__global__ void __launch_bounds__(kTopThreads) k_batch_top(const FrzBatchDev b, uint32_t k, FrzMatchDev* __restrict__ rows,
+                                                           unsigned long long* __restrict__ totals) {
+    __shared__ uint32_t hist[kFrzBatchBins];
+    __shared__ uint64_t keys[kFrzBatchMaxK];
+    __shared__ uint32_t warp_cnt[32];
+    __shared__ int hi_bin;
+    __shared__ unsigned long long above_hi;
+    __shared__ FrzBatchCut cut;
+    const uint32_t j = blockIdx.x;
+    const uint64_t total = b.ctr[j].total;
+    const unsigned int err = b.ctr[j].error;
+    if (threadIdx.x == 0) totals[j] = err ? kFrzBatchOverflow : total;
+    const uint32_t n_rows = (uint32_t)frz_batch_rows(k, total);
+    if (err || n_rows == 0) return;   // an overflowed sub-batch is run again query by query
+    const FrzMatchDev* __restrict__ list = b.lists + j * b.list_stride;
+    FrzMatchDev* __restrict__ out = rows + frz_batch_row0(j, k);
+    if (!b.by_score[j]) {   // index order: the list's head
+        for (uint32_t i = threadIdx.x; i < n_rows; i += blockDim.x) out[i] = list[i];
+        return;
+    }
+    // the cut: high score byte, then low score byte within the selected high bin
+    for (uint32_t i = threadIdx.x; i < kFrzBatchBins; i += blockDim.x) hist[i] = 0;
+    __syncthreads();
+    for (uint64_t i = threadIdx.x; i < total; i += blockDim.x) atomicAdd(&hist[list[i].score >> 8], 1u);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        uint64_t a = 0;
+        hi_bin = frz_batch_cut_hi(hist, n_rows, &a);
+        above_hi = a;
+    }
+    __syncthreads();
+    for (uint32_t i = threadIdx.x; i < kFrzBatchBins; i += blockDim.x) hist[i] = 0;
+    __syncthreads();
+    const uint32_t hb = (uint32_t)hi_bin;
+    for (uint64_t i = threadIdx.x; i < total; i += blockDim.x) {
+        const uint32_t s = list[i].score;
+        if ((s >> 8) == hb) atomicAdd(&hist[s & 255u], 1u);
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) cut = frz_batch_cut_lo(hist, hi_bin, above_hi, n_rows);
+    __syncthreads();
+    const FrzBatchCut c = cut;
+    // the kept rows, in list order
+    uint64_t eq_base = 0;
+    uint32_t kept = 0;
+    for (uint64_t base = 0; base < total && kept < n_rows; base += blockDim.x) {
+        const uint64_t i = base + threadIdx.x;
+        const bool valid = i < total;
+        const uint32_t s = valid ? list[i].score : 0u;
+        uint32_t n_eq = 0, n_keep = 0;
+        const uint32_t eq_before = block_excl_count(valid && s == c.threshold, warp_cnt, &n_eq);
+        const bool keep = valid && frz_batch_keep(s, c, eq_base + eq_before);
+        const uint32_t pos = kept + block_excl_count(keep, warp_cnt, &n_keep);
+        if (keep) keys[pos] = frz_batch_key(s, (uint32_t)i);
+        eq_base += n_eq;
+        kept += n_keep;
+    }
+    // bitonic sort of the kept keys (padded to a power of two)
+    uint32_t p2 = 1;
+    while (p2 < n_rows) p2 <<= 1;
+    for (uint32_t i = n_rows + threadIdx.x; i < p2; i += blockDim.x) keys[i] = ~0ull;
+    __syncthreads();
+    for (uint32_t size = 2; size <= p2; size <<= 1) {
+        for (uint32_t stride = size >> 1; stride > 0; stride >>= 1) {
+            const uint32_t i = threadIdx.x, partner = i ^ stride;
+            if (i < p2 && partner > i) {
+                const uint64_t x = keys[i], y = keys[partner];
+                if ((x > y) == ((i & size) == 0)) { keys[i] = y; keys[partner] = x; }
+            }
+            __syncthreads();
+        }
+    }
+    for (uint32_t i = threadIdx.x; i < n_rows; i += blockDim.x) out[i] = list[frz_batch_key_pos(keys[i])];
+}
+
+}  // namespace
+
+frz_status frz_launch_batch_top(const FrzBatchDev& b, uint32_t nq, uint32_t k, FrzMatchDev* rows, unsigned long long* totals,
+                                cudaStream_t stream, FrzLaunchStats* st) {
+    if (nq == 0) return FRZ_OK;
+    if (k > kFrzBatchMaxK) return frz_fail(FRZ_ERR_INVALID_ARG, "batched top-K serves k <= %u", kFrzBatchMaxK);
+    k_batch_top<<<nq, kTopThreads, 0, stream>>>(b, k, rows, totals);
+    FRZ_CUDA_TRY(cudaGetLastError());
+    if (st) st->launches++;
+    return FRZ_OK;
+}

@@ -205,6 +205,8 @@ struct frz_corpus {
     // metadata of the tiles a frz_corpus_replace re-packs (grow-only; a replace releases it, and the ingest staging, once
     // they pass 64 MiB)
     std::unique_ptr<FrzCorpusStorage> edit_tiles;
+    // pinned staging of frz_match_list_batch_top (patterns up, rows and counts down), grow-only
+    mutable FrzPinnedArray<uint8_t> batch_stage;
 };
 
 // pack.cu
@@ -321,6 +323,54 @@ int frz_sort_single_pass_bins(uint32_t score_bound);   // bins of the single-pas
 frz_status frz_sort_fused_prepare(FrzSortScratch& ss, uint64_t n_cap, uint32_t score_bound, cudaStream_t stream, FrzScoreHist* out);
 frz_status frz_launch_sort_fused(const FrzMatchDev* d_in, FrzMatchDev* d_out, const unsigned long long* n_ptr, const FrzScoreHist& hist,
                                  FrzSortScratch& ss, cudaStream_t stream, FrzLaunchStats* st, uint32_t limit = kFrzNoLimit);
+
+// One sub-batch of frz_match_list_batch_top (host.cu, DESIGN.md §4.11) on the device.  Query j (0 <= j < the sub-batch's
+// size) owns slice j of every array; its kernels see exactly the buffers a single-query call's kernels see.  A batched
+// launch covers a group of queries (FrzBatchGroup, a kernel argument): block row blockIdx.y runs query grp.j[blockIdx.y].
+constexpr uint32_t kFrzBatchMaxSub = 64;   // queries of one sub-batch
+struct FrzBatchGroup {
+    uint16_t j[kFrzBatchMaxSub];
+};
+struct FrzBatchDev {
+    const FrzPatternDev* pats;        // [j] compiled pattern
+    const uint8_t* reversed;          // [j] 1: the list is written in descending index order (the *_DESC strategies)
+    const uint8_t* by_score;          // [j] 1: the rows are ordered by score (the ScoreThenIndex strategies)
+    FrzSurvivor* surv;                // [j][class][surv_cap]
+    unsigned long long surv_cap;      // per query and class
+    FrzCounters* ctr;                 // [j]
+    uint32_t* surv_bitmap;            // [j][n_tiles * 32]
+    uint16_t* word_prefix;            // [j][n_tiles * 32]
+    uint32_t* tile_count;             // [j][n_tiles]
+    uint64_t* tile_out_base;          // [j][n_tiles]
+    FrzMatchDev* lists;               // [j][list_stride] index-ordered matches
+    uint64_t list_stride;
+};
+#if defined(__CUDACC__)
+__device__ __forceinline__ FrzSurvLists frz_batch_lists(const FrzBatchDev& b, uint32_t j) {
+    FrzSurvLists l;
+    for (int c = 0; c < FRZ_N_CLASSES; c++) l.p[c] = b.surv + ((uint64_t)j * FRZ_N_CLASSES + c) * b.surv_cap;
+    return l;
+}
+// the block's copy of query j's pattern (call before the block's first barrier, then __syncthreads)
+__device__ __forceinline__ void frz_batch_stage_pattern(const FrzBatchDev& b, uint32_t j, FrzPatternDev* pat_s) {
+    static_assert(sizeof(FrzPatternDev) % 4 == 0, "pattern words");
+    const uint32_t* src = reinterpret_cast<const uint32_t*>(b.pats + j);
+    uint32_t* dst = reinterpret_cast<uint32_t*>(pat_s);
+    for (uint32_t i = threadIdx.x; i < sizeof(FrzPatternDev) / 4; i += blockDim.x) dst[i] = src[i];
+}
+#endif
+// Stages of a sub-batch, all asynchronous on `stream`.  h_pats: host copies of the nq patterns (they choose the kernel
+// variants).  prefilter.cu: one k_scan_window_batch launch per typo mode present (the counters and bitmaps must be zeroed), then the
+// per-query tile ranks and scans
+frz_status frz_launch_prefilter_batch(const FrzCorpusView& cv, const FrzBatchDev& b, const FrzPatternDev* h_pats, uint32_t nq,
+                                      cudaStream_t stream, FrzLaunchStats* st);
+// sw.cu: the scoring classes of frz_launch_sw, one launch per kernel variant present
+frz_status frz_launch_sw_batch(const FrzCorpusView& cv, const FrzBatchDev& b, const FrzPatternDev* h_pats, uint32_t nq,
+                               cudaStream_t stream, FrzLaunchStats* st);
+// batch.cu: per query, its first min(k, total) rows → rows[j * k ...] and its total → totals[j], or kFrzBatchOverflow
+// there when its sticky device error is set (k <= kFrzBatchMaxK)
+frz_status frz_launch_batch_top(const FrzBatchDev& b, uint32_t nq, uint32_t k, FrzMatchDev* rows, unsigned long long* totals,
+                                cudaStream_t stream, FrzLaunchStats* st);
 
 // k-way merge of per-shard runs (merge.cu) with caller-owned scratch — one per concurrent user (parallel.cu: one per rank)
 #define FRZ_MERGE_MAX_RUNS 64

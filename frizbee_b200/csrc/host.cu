@@ -19,6 +19,7 @@
 #include <memory>
 #include <mutex>
 
+#include "batch_plan.cuh"
 #include "frz_device.cuh"
 #include "frz_host.h"
 #include "unicode_needle.h"
@@ -1449,6 +1450,207 @@ extern "C" frz_status frz_match_list_top(frz_matcher* m, const frz_corpus* corpu
     if (!out && k > 0) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
     FRZ_TRY(frz_ensure_device(corpus->st.device));
     return match_list_host(m, corpus, 0, m->config.sort, k, SubsetScope(), out, k, n_out, n_total);
+}
+
+// ---------------------------------------------------------------------------------- batched top-K
+// frz_match_list_batch_top (DESIGN.md §4.11).  Queries of the batched class run in sub-batches whose every stage is one
+// launch (per kernel variant present) over all of the sub-batch's queries, with one upload, one read-back and one
+// synchronise per sub-batch; every other query, and every query of an overflowed sub-batch, runs frz_match_list_top's
+// pipeline.
+namespace {
+
+// Device scratch of one sub-batch's queries, in one allocation: a fixed budget, so a batch call holds the same scratch for
+// every q (its size depends on the corpus: larger corpora get smaller sub-batches, and a corpus whose queries do not fit two
+// to a sub-batch is answered query by query).
+constexpr uint64_t kBatchScratchBytes = 512ull << 20;
+// Where the batched path is faster than a loop of frz_match_list_top (tools/bench_batch.py on an H100 SXM, DESIGN.md §4.11):
+// at 100 k rows from 64 queries on, not at 8 queries (the call's fixed costs); at 1 M rows for max_typos = 0 queries only
+// (with a typo budget, short needles pass more rows than the survivor lists hold, and the overflowed sub-batches run
+// again query by query).  Elsewhere the call runs the loop.
+constexpr uint64_t kBatchMaxRows = 1ull << 18;
+constexpr uint64_t kBatchMaxRowsNoTypo = 1ull << 21;   // FRZ_T_0 queries
+constexpr uint64_t kBatchMinQueries = 32;
+// The limits in force (frz_debug_batch_limits changes them for tests and tools/bench_batch.py) and what the calling
+// thread's last batch call did (frz_debug_batch_last).
+std::atomic<uint64_t> g_batch_max_rows{kBatchMaxRows};
+std::atomic<uint64_t> g_batch_min_queries{kBatchMinQueries};
+thread_local uint64_t g_batch_last[4] = {0, 0, 0, 0};   // batched queries, overflowed queries, sub-batches, launches
+
+struct BatchLayout {
+    uint64_t nt = 0, stride = 0, cap = 0, k = 0;
+    uint64_t off[13] = {};   // byte offsets of the arrays below, in this order
+    uint64_t bytes = 0;
+    enum { CTR, BITMAP, PREFIX, TCOUNT, TBASE, SURV, LISTS, PATS, REV, BYSC, TOTALS, ROWS, END };
+    // queries per sub-batch for this corpus and k (0: fewer than two fit the budget)
+    static uint64_t per_query(const FrzCorpusStorage& cs, uint64_t k, uint64_t cap) {
+        const uint64_t nt = cs.n_tiles;
+        return sizeof(FrzCounters) + nt * 32 * (sizeof(uint32_t) + sizeof(uint16_t)) + nt * (sizeof(uint32_t) + sizeof(uint64_t)) +
+               FRZ_N_CLASSES * cap * sizeof(FrzSurvivor) + std::max<uint64_t>(cs.n, 1) * sizeof(FrzMatchDev) + sizeof(FrzPatternDev) + 2 +
+               sizeof(unsigned long long) + k * sizeof(FrzMatchDev) + 13 * 256 / 2;
+    }
+    BatchLayout(const FrzCorpusStorage& cs, uint64_t k_, uint64_t cap_, uint64_t qs) : nt(cs.n_tiles), stride(std::max<uint64_t>(cs.n, 1)), cap(cap_), k(k_) {
+        const uint64_t size[END] = {qs * sizeof(FrzCounters), qs * nt * 32 * sizeof(uint32_t), qs * nt * 32 * sizeof(uint16_t),
+                                    qs * nt * sizeof(uint32_t), qs * nt * sizeof(uint64_t), qs * FRZ_N_CLASSES * cap * sizeof(FrzSurvivor),
+                                    qs * stride * sizeof(FrzMatchDev), qs * sizeof(FrzPatternDev), qs, qs,
+                                    qs * sizeof(unsigned long long), qs * k * sizeof(FrzMatchDev)};
+        uint64_t at = 0;
+        for (int i = 0; i < END; i++) {
+            // CTR..BITMAP are zeroed as one range, PATS..BYSC uploaded as one, TOTALS..ROWS read back as one
+            const bool packed = i == BITMAP || i == REV || i == BYSC || i == ROWS;
+            if (!packed) at = (at + 255) & ~255ull;
+            else at = (at + 7) & ~7ull;
+            off[i] = at;
+            at += size[i];
+        }
+        off[END] = at;
+        bytes = at;
+    }
+};
+
+// the survivor-list length per class and query: frz_match_list_top's first attempt (initial_survivor_cap, which is the
+// same for every pattern that is not FRZ_T_NONE)
+uint64_t batch_survivor_cap(const FrzCorpusStorage& cs) {
+    return std::min<uint64_t>(std::max<uint64_t>(cs.n / 4, 1 << 16), std::max<uint64_t>(cs.n, 1));
+}
+
+// the batched class: one compiled fuzzy byte pattern of up to FRZ_MAX_NEEDLE bytes, not negated (and, when it can match
+// every row, a survivor list that can hold them all)
+bool batchable(const frz_matcher* m, const FrzCorpusStorage& cs) {
+    if (m->compiled.size() != 1) return false;
+    const Compiled& c = m->compiled[0];
+    if (c.negated || c.literal || c.unicode || c.is_long() || c.dev.typo_mode == FRZ_T_LITERAL) return false;
+    return c.dev.typo_mode != FRZ_T_NONE || batch_survivor_cap(cs) >= std::max<uint64_t>(cs.n, 1);
+}
+// the selection of the batched path for such a query (kBatchMaxRows, kBatchMaxRowsNoTypo)
+bool batch_selected(const frz_matcher* m, const FrzCorpusStorage& cs) {
+    const uint64_t max_rows = g_batch_max_rows.load();
+    const uint64_t limit = m->compiled[0].dev.typo_mode == FRZ_T_0 ? std::max(max_rows, kBatchMaxRowsNoTypo) : max_rows;
+    return cs.n <= limit;
+}
+
+frz_status batch_single(frz_matcher* m, const frz_corpus* c, uint64_t k, frz_match* out, uint64_t* n_out, uint64_t* n_total) {
+    return match_list_host(m, c, 0, m->config.sort, k, SubsetScope(), out, k, n_out, n_total);
+}
+
+// One sub-batch: queries which[0..ns) of ms, all of the batched class.  *overflow: a survivor list overflowed, nothing was
+// written to the results (the caller runs the queries one by one).
+frz_status batch_run(frz_matcher* const* ms, const uint64_t* which, uint32_t ns, const frz_corpus* c, uint64_t k,
+                     const BatchLayout& L, uint8_t* d, frz_match* out, uint64_t* n_out, uint64_t* n_total, bool* overflow,
+                     FrzLaunchStats& st) {
+    const FrzCorpusStorage& cs = c->st;
+    cudaStream_t stream = nullptr;
+    *overflow = false;
+    const uint64_t up = L.off[BatchLayout::TOTALS] - L.off[BatchLayout::PATS];
+    const uint64_t down = L.off[BatchLayout::END] - L.off[BatchLayout::TOTALS];
+    FRZ_TRY(c->batch_stage.reserve(std::max(up, down)));
+    uint8_t* h = c->batch_stage.get();
+    FrzPatternDev* h_pats = reinterpret_cast<FrzPatternDev*>(h);
+    uint8_t* h_rev = h + (L.off[BatchLayout::REV] - L.off[BatchLayout::PATS]);
+    uint8_t* h_bysc = h + (L.off[BatchLayout::BYSC] - L.off[BatchLayout::PATS]);
+    for (uint32_t j = 0; j < ns; j++) {
+        const frz_matcher* m = ms[which[j]];
+        const uint8_t sort = m->config.sort;
+        h_pats[j] = m->compiled[0].dev;
+        h_rev[j] = sort == FRZ_SORT_INDEX_DESC || sort == FRZ_SORT_SCORE_THEN_INDEX_DESC;
+        h_bysc[j] = sort == FRZ_SORT_SCORE_THEN_INDEX_ASC || sort == FRZ_SORT_SCORE_THEN_INDEX_DESC;
+    }
+    FrzBatchDev b;
+    b.pats = reinterpret_cast<const FrzPatternDev*>(d + L.off[BatchLayout::PATS]);
+    b.reversed = d + L.off[BatchLayout::REV];
+    b.by_score = d + L.off[BatchLayout::BYSC];
+    b.surv = reinterpret_cast<FrzSurvivor*>(d + L.off[BatchLayout::SURV]);
+    b.surv_cap = L.cap;
+    b.ctr = reinterpret_cast<FrzCounters*>(d + L.off[BatchLayout::CTR]);
+    b.surv_bitmap = reinterpret_cast<uint32_t*>(d + L.off[BatchLayout::BITMAP]);
+    b.word_prefix = reinterpret_cast<uint16_t*>(d + L.off[BatchLayout::PREFIX]);
+    b.tile_count = reinterpret_cast<uint32_t*>(d + L.off[BatchLayout::TCOUNT]);
+    b.tile_out_base = reinterpret_cast<uint64_t*>(d + L.off[BatchLayout::TBASE]);
+    b.lists = reinterpret_cast<FrzMatchDev*>(d + L.off[BatchLayout::LISTS]);
+    b.list_stride = L.stride;
+    unsigned long long* totals = reinterpret_cast<unsigned long long*>(d + L.off[BatchLayout::TOTALS]);
+    FrzMatchDev* rows = reinterpret_cast<FrzMatchDev*>(d + L.off[BatchLayout::ROWS]);
+    FRZ_CUDA_TRY(cudaMemcpyAsync(d + L.off[BatchLayout::PATS], h, up, cudaMemcpyHostToDevice, stream));
+    FRZ_CUDA_TRY(cudaMemsetAsync(d + L.off[BatchLayout::CTR], 0,
+                                 L.off[BatchLayout::BITMAP] + (uint64_t)ns * L.nt * 32 * sizeof(uint32_t) - L.off[BatchLayout::CTR], stream));
+    const FrzCorpusView cv = cs.view();
+    FRZ_TRY(frz_launch_prefilter_batch(cv, b, h_pats, ns, stream, &st));
+    FRZ_TRY(frz_launch_sw_batch(cv, b, h_pats, ns, stream, &st));
+    FRZ_TRY(frz_launch_batch_top(b, ns, (uint32_t)k, rows, totals, stream, &st));
+    // the staged patterns are not read again: the read-back may reuse the staging
+    FRZ_CUDA_TRY(cudaMemcpyAsync(h, totals, down, cudaMemcpyDeviceToHost, stream));
+    FRZ_CUDA_TRY(cudaStreamSynchronize(stream));
+    const unsigned long long* h_totals = reinterpret_cast<const unsigned long long*>(h);
+    const frz_match* h_rows = reinterpret_cast<const frz_match*>(h + (L.off[BatchLayout::ROWS] - L.off[BatchLayout::TOTALS]));
+    for (uint32_t j = 0; j < ns; j++)
+        if (h_totals[j] == kFrzBatchOverflow) { *overflow = true; return FRZ_OK; }
+    for (uint32_t j = 0; j < ns; j++) {
+        const uint64_t q = which[j], n = frz_batch_rows(k, h_totals[j]);
+        n_out[q] = n;
+        if (n_total) n_total[q] = h_totals[j];
+        if (n) memcpy(out + q * k, h_rows + frz_batch_row0(j, k), n * sizeof(frz_match));
+    }
+    return FRZ_OK;
+}
+
+}  // namespace
+
+extern "C" frz_status frz_match_list_batch_top(frz_matcher* const* ms, uint64_t q, const frz_corpus* corpus, uint64_t k, frz_match* out,
+                                               uint64_t* n_out, uint64_t* n_total) {
+    if (!ms || !corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    for (uint64_t j = 0; j < q; j++)
+        if (!ms[j]) return frz_fail(FRZ_ERR_INVALID_ARG, "null matcher at %llu", (unsigned long long)j);
+    if (q && !n_out) return frz_fail(FRZ_ERR_INVALID_ARG, "null n_out");
+    if (k && (q > UINT64_MAX / k || q * k > SIZE_MAX / sizeof(frz_match)))
+        return frz_fail(FRZ_ERR_INVALID_ARG, "q * k overflows: q = %llu, k = %llu", (unsigned long long)q, (unsigned long long)k);
+    if (q * k > 0 && !out) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
+    if (q == 0) return FRZ_OK;
+    int n_dev = 0;
+    if (cudaGetDeviceCount(&n_dev) != cudaSuccess || n_dev == 0) {
+        cudaGetLastError();
+        return frz_fail(FRZ_ERR_NO_DEVICE, "no CUDA device available; this library has no CPU fallback");
+    }
+    FRZ_TRY(frz_ensure_device(corpus->st.device));
+    const FrzCorpusStorage& cs = corpus->st;
+    FRZ_TRY(frz_check_index_range(cs.n, 0));
+    for (uint64_t& v : g_batch_last) v = 0;
+    auto single = [&](uint64_t j) { return batch_single(ms[j], corpus, k, k ? out + j * k : nullptr, &n_out[j], n_total ? &n_total[j] : nullptr); };
+    std::vector<uint64_t> batched;
+    const uint64_t cap = batch_survivor_cap(cs);
+    const uint64_t fit = k <= kFrzBatchMaxK ? kBatchScratchBytes / BatchLayout::per_query(cs, k, cap) : 0;
+    const uint64_t qs_max = std::min<uint64_t>(fit, kFrzBatchMaxSub);
+    for (uint64_t j = 0; j < q; j++) {
+        if (qs_max >= 2 && batchable(ms[j], cs) && batch_selected(ms[j], cs)) batched.push_back(j);
+        else FRZ_TRY(single(j));
+    }
+    if (batched.size() < std::max<uint64_t>(2, g_batch_min_queries.load())) {   // a few queries cost what a loop of frz_match_list_top costs
+        for (uint64_t j : batched) FRZ_TRY(single(j));
+        return FRZ_OK;
+    }
+    const uint64_t qs = std::min<uint64_t>(qs_max, batched.size());
+    const BatchLayout L(cs, k, cap, qs);
+    FrzDevArray<uint8_t> scratch;   // released when the call returns
+    FRZ_TRY(scratch.reserve(L.bytes));
+    for (uint64_t s = 0; s < batched.size(); s += qs) {
+        const uint32_t ns = (uint32_t)std::min<uint64_t>(qs, batched.size() - s);
+        bool overflow = false;
+        FrzLaunchStats st;
+        FRZ_TRY(batch_run(ms, batched.data() + s, ns, corpus, k, L, scratch.get(), out, n_out, n_total, &overflow, st));
+        g_batch_last[overflow ? 1 : 0] += ns;
+        g_batch_last[2]++;
+        g_batch_last[3] += st.launches;
+        if (overflow)   // the single-query pipeline retries with worst-case lists
+            for (uint32_t j = 0; j < ns; j++) FRZ_TRY(single(batched[s + j]));
+    }
+    return FRZ_OK;
+}
+
+extern "C" void frz_debug_batch_limits(uint64_t max_rows, uint64_t min_queries) {
+    g_batch_max_rows = max_rows ? max_rows : kBatchMaxRows;
+    g_batch_min_queries = min_queries ? min_queries : kBatchMinQueries;
+}
+
+extern "C" void frz_debug_batch_last(uint64_t out[4]) {
+    for (int i = 0; i < 4; i++) out[i] = g_batch_last[i];
 }
 
 // ---------------------------------------------------------------------------------- subsets

@@ -607,6 +607,56 @@ __global__ void __launch_bounds__(kScanWinThreads, 5) k_scan_window_long(const F
     scan_window<MODE, true>(cv, pat, use_sig, occ_rows, lists, surv_cap, surv_bitmap, ctr, ntab);
 }
 
+// k_scan_window over the queries of a batch group (frz_match_list_batch_top): block row y runs query grp.j[y] with the
+// buffers of that query, on a copy of its pattern in shared memory.  The dynamic shared memory is sized for the group's
+// largest occurrence table.
+template <int MODE>
+__global__ void __launch_bounds__(kScanWinThreads, 5) k_scan_window_batch(const FrzCorpusView cv, const FrzBatchDev b,
+                                                                          const __grid_constant__ FrzBatchGroup grp) {
+    __shared__ FrzPatternDev pat_s;
+    const uint32_t j = grp.j[blockIdx.y];
+    frz_batch_stage_pattern(b, j, &pat_s);
+    __syncthreads();
+    const int use_sig = pat_s.typo_mode != FRZ_T_NONE && pat_s.sig_on;
+    const int occ_rows = pat_s.n_distinct ? min(kMaxDistinct, pat_s.n_distinct + pat_s.n) : 0;
+    scan_window<MODE, false>(cv, pat_s, use_sig, occ_rows, frz_batch_lists(b, j), b.surv_cap,
+                             b.surv_bitmap + (uint64_t)j * cv.n_tiles * 32, b.ctr + j, nullptr);
+}
+
+// k_tile_scan for each query of a sub-batch: block j scans query j's tile counts (a contiguous run of tiles per thread).
+__global__ void __launch_bounds__(1024) k_tile_scan_batch(const FrzBatchDev b, uint32_t n) {
+    __shared__ uint64_t warp_sum[32];
+    const uint32_t j = blockIdx.x;
+    const uint32_t* cnt = b.tile_count + (uint64_t)j * n;
+    uint64_t* out = b.tile_out_base + (uint64_t)j * n;
+    const uint32_t per = (n + blockDim.x - 1) / blockDim.x;
+    const uint32_t lo = min(threadIdx.x * per, n), hi = min(lo + per, n);
+    uint64_t sum = 0;
+    for (uint32_t i = lo; i < hi; i++) sum += cnt[i];
+    uint64_t x = sum;
+    for (int d = 1; d < 32; d <<= 1) {
+        uint64_t y = __shfl_up_sync(0xffffffffu, x, d);
+        if (frz_lane() >= (uint32_t)d) x += y;
+    }
+    if (frz_lane() == 31) warp_sum[threadIdx.x >> 5] = x;
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        uint64_t w = warp_sum[threadIdx.x], xs = w;
+        for (int d = 1; d < 32; d <<= 1) {
+            uint64_t y = __shfl_up_sync(0xffffffffu, xs, d);
+            if (frz_lane() >= (uint32_t)d) xs += y;
+        }
+        warp_sum[threadIdx.x] = xs - w;
+    }
+    __syncthreads();
+    uint64_t run = warp_sum[threadIdx.x >> 5] + x - sum;
+    for (uint32_t i = lo; i < hi; i++) {
+        out[i] = run;
+        run += cnt[i];
+    }
+    if (threadIdx.x == blockDim.x - 1) b.ctr[j].total = run;
+}
+
 // Candidate-list mode (multi-pattern, src/matcher/multi.rs:108-120): the extra patterns are evaluated only
 // on the haystacks that survived the previous patterns.  The list is already compact, so each warp takes 32
 // candidates at a time straight to phase B.
@@ -954,6 +1004,58 @@ frz_status frz_launch_prefilter(const FrzCorpusView& cv, const FrzPatternDev& pa
 #undef FRZ_PF_LAUNCH
     FRZ_CUDA_TRY(cudaGetLastError());
     if (st) st->launches++;
+    return FRZ_OK;
+}
+
+// Stage 1 of a batch sub-batch: one k_scan_window_batch launch per typo mode present, its grid split evenly over the
+// mode's queries (as many blocks in all as one single-query launch), then every query's tile ranks (one k_tile_rank over
+// the sub-batch's bitmaps, which lie back to back) and tile scans (one k_tile_scan_batch).
+frz_status frz_launch_prefilter_batch(const FrzCorpusView& cv, const FrzBatchDev& b, const FrzPatternDev* h_pats, uint32_t nq,
+                                      cudaStream_t stream, FrzLaunchStats* st) {
+    if (cv.n_tiles == 0 || nq == 0) return FRZ_OK;
+    const int sms = frz_sm_count();
+    const uint32_t total_chunks = cv.n_tiles * (FRZ_TILE / 128);
+    const size_t smem_max = sizeof(ScanWinSmem) + sizeof(OccTable) * kWinWarps;
+    for (int mode = FRZ_T_0; mode <= FRZ_T_NONE; mode++) {
+        FrzBatchGroup grp;
+        uint32_t ng = 0;
+        int occ_max = 0;
+        for (uint32_t j = 0; j < nq; j++) {
+            if (h_pats[j].typo_mode != mode) continue;
+            grp.j[ng++] = (uint16_t)j;
+            const FrzPatternDev& p = h_pats[j];
+            occ_max = std::max(occ_max, p.n_distinct ? std::min(kMaxDistinct, p.n_distinct + p.n) : 0);
+        }
+        if (ng == 0) continue;
+        const size_t smem = sizeof(ScanWinSmem) + sizeof(uint2) * 32 * occ_max * kWinWarps;
+#define FRZ_PFB_LAUNCH(MODE)                                                                                             \
+    do {                                                                                                                 \
+        static int bps_dev[64][kMaxDistinct + 1] = {};                                                                   \
+        int& bps = bps_dev[frz_current_device() & 63][occ_max];                                                          \
+        if (!bps) {                                                                                                      \
+            FRZ_CUDA_TRY(cudaFuncSetAttribute(k_scan_window_batch<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max)); \
+            FRZ_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps, k_scan_window_batch<MODE>, kScanWinThreads, smem)); \
+            if (bps < 1) bps = 1;                                                                                        \
+        }                                                                                                                \
+        const uint32_t gx = std::max<uint32_t>(1, std::min<uint32_t>((uint32_t)(sms * bps) / ng, total_chunks));         \
+        k_scan_window_batch<MODE><<<dim3(gx, ng), kScanWinThreads, smem, stream>>>(cv, b, grp);                          \
+    } while (0)
+        switch (mode) {
+            case FRZ_T_0: FRZ_PFB_LAUNCH(FRZ_T_0); break;
+            case FRZ_T_1: FRZ_PFB_LAUNCH(FRZ_T_1); break;
+            case FRZ_T_2: FRZ_PFB_LAUNCH(FRZ_T_2); break;
+            case FRZ_T_MANY: FRZ_PFB_LAUNCH(FRZ_T_MANY); break;
+            default: FRZ_PFB_LAUNCH(FRZ_T_NONE); break;
+        }
+#undef FRZ_PFB_LAUNCH
+        FRZ_CUDA_TRY(cudaGetLastError());
+        if (st) st->launches++;
+    }
+    const uint32_t tiles = cv.n_tiles * nq;
+    k_tile_rank<<<(tiles * 32 + 255) / 256, 256, 0, stream>>>(b.surv_bitmap, b.word_prefix, b.tile_count, tiles);
+    k_tile_scan_batch<<<nq, 1024, 0, stream>>>(b, cv.n_tiles);
+    FRZ_CUDA_TRY(cudaGetLastError());
+    if (st) st->launches += 2;
     return FRZ_OK;
 }
 

@@ -134,11 +134,9 @@ __device__ __forceinline__ uint32_t score_survivor(const FrzCorpusView& cv, cons
 // Windows of 65..128 bytes: one window per thread, score rows in shared memory, survivors strided over a
 // persistent grid.
 template <int LANES, int COLS, bool WRAP8, int VAR = 0>
-__global__ void __launch_bounds__(kSwThreads) k_sw(const FrzCorpusView cv, const __grid_constant__ FrzPatternDev pat,
-                                                   const FrzSurvivor* __restrict__ surv, unsigned long long surv_cap, int cls,
-                                                   const FrzRankView rv, FrzCounters* __restrict__ ctr,
-                                                   uint32_t index_offset, int reversed, FrzMatchDev* __restrict__ out,
-                                                   const FrzScoreHist hist) {
+__device__ __forceinline__ void sw_run(const FrzCorpusView& cv, const FrzPatternDev& pat, const FrzSurvivor* __restrict__ surv,
+                                       unsigned long long surv_cap, int cls, const FrzRankView& rv, FrzCounters* __restrict__ ctr,
+                                       uint32_t index_offset, int reversed, FrzMatchDev* __restrict__ out, const FrzScoreHist& hist) {
     extern __shared__ __align__(16) uint32_t sw_smem[];
     const unsigned long long count = min(ctr->class_count[cls], surv_cap);
     uint32_t local_max = 0;
@@ -149,6 +147,14 @@ __global__ void __launch_bounds__(kSwThreads) k_sw(const FrzCorpusView cv, const
     }
     local_max = __reduce_max_sync(0xffffffffu, local_max);
     if (frz_lane() == 0 && local_max) atomicMax(&ctr->max_score, local_max);
+}
+template <int LANES, int COLS, bool WRAP8, int VAR = 0>
+__global__ void __launch_bounds__(kSwThreads) k_sw(const FrzCorpusView cv, const __grid_constant__ FrzPatternDev pat,
+                                                   const FrzSurvivor* __restrict__ surv, unsigned long long surv_cap, int cls,
+                                                   const FrzRankView rv, FrzCounters* __restrict__ ctr,
+                                                   uint32_t index_offset, int reversed, FrzMatchDev* __restrict__ out,
+                                                   const FrzScoreHist hist) {
+    sw_run<LANES, COLS, WRAP8, VAR>(cv, pat, surv, surv_cap, cls, rv, ctr, index_offset, reversed, out, hist);
 }
 
 // Windows of <= 64 bytes: the four column classes (CC64 first: longest items first) share one persistent
@@ -164,11 +170,9 @@ struct Sw64Stage {
 };
 
 template <int LANES, bool WRAP8, int VAR = 0>
-__global__ void __launch_bounds__(kSwThreads, (kSw64MinBlocks<LANES, WRAP8>)) k_sw64(const FrzCorpusView cv, const __grid_constant__ FrzPatternDev pat,
-                                                     const FrzSurvLists lists, unsigned long long surv_cap,
-                                                     const FrzRankView rv, FrzCounters* __restrict__ ctr,
-                                                     uint32_t index_offset, int reversed, FrzMatchDev* __restrict__ out,
-                                                   const FrzScoreHist hist) {
+__device__ __forceinline__ void sw64_run(const FrzCorpusView cv, const FrzPatternDev& pat, const FrzSurvLists lists,
+                                         unsigned long long surv_cap, const FrzRankView rv, FrzCounters* __restrict__ ctr,
+                                         uint32_t index_offset, int reversed, FrzMatchDev* __restrict__ out, const FrzScoreHist hist) {
     __shared__ Sw64Stage stage;
     __shared__ __align__(16) uint32_t rows_smem[kSw64RowsInSmem<LANES, WRAP8> ? 2 * 32 * kSwThreads : 1];
     frz_wait_prior_grid();   // the survivor lists and class counts come from the prefilter stage
@@ -277,6 +281,14 @@ __global__ void __launch_bounds__(kSwThreads, (kSw64MinBlocks<LANES, WRAP8>)) k_
     local_max = __reduce_max_sync(0xffffffffu, local_max);
     if (lane == 0 && local_max) atomicMax(&ctr->max_score, local_max);
 }
+template <int LANES, bool WRAP8, int VAR = 0>
+__global__ void __launch_bounds__(kSwThreads, (kSw64MinBlocks<LANES, WRAP8>)) k_sw64(const FrzCorpusView cv, const __grid_constant__ FrzPatternDev pat,
+                                                     const FrzSurvLists lists, unsigned long long surv_cap,
+                                                     const FrzRankView rv, FrzCounters* __restrict__ ctr,
+                                                     uint32_t index_offset, int reversed, FrzMatchDev* __restrict__ out,
+                                                   const FrzScoreHist hist) {
+    sw64_run<LANES, WRAP8, VAR>(cv, pat, lists, surv_cap, rv, ctr, index_offset, reversed, out, hist);
+}
 
 // ---- generic fallback: windows of 129..1024 bytes (row-major, local-memory rows) and the greedy scorer for
 // ---- windows > 1024 (sw_generic.cuh).  One window per thread.
@@ -290,11 +302,9 @@ struct GenericHay {
     __device__ __forceinline__ uint32_t operator()(int i) const { return hay_byte(base, start + i); }
 };
 
-__global__ void __launch_bounds__(64) k_sw_generic(const FrzCorpusView cv, const __grid_constant__ FrzPatternDev pat,
-                                                   const FrzSurvivor* __restrict__ surv, unsigned long long surv_cap, int cls,
-                                                   const FrzRankView rv, FrzCounters* __restrict__ ctr,
-                                                   uint32_t index_offset, int reversed, FrzMatchDev* __restrict__ out,
-                                                   const FrzScoreHist hist) {
+__device__ __forceinline__ void sw_generic_run(const FrzCorpusView& cv, const FrzPatternDev& pat, const FrzSurvivor* __restrict__ surv,
+                                               unsigned long long surv_cap, int cls, const FrzRankView& rv, FrzCounters* __restrict__ ctr,
+                                               uint32_t index_offset, int reversed, FrzMatchDev* __restrict__ out, const FrzScoreHist& hist) {
     const unsigned long long count = min(ctr->class_count[cls], surv_cap);
     uint32_t local_max = 0;
     for (unsigned long long j = (unsigned long long)blockIdx.x * blockDim.x + threadIdx.x; j < count;
@@ -324,6 +334,13 @@ __global__ void __launch_bounds__(64) k_sw_generic(const FrzCorpusView cv, const
         local_max = max(local_max, score);
     }
     if (local_max) atomicMax(&ctr->max_score, local_max);
+}
+__global__ void __launch_bounds__(64) k_sw_generic(const FrzCorpusView cv, const __grid_constant__ FrzPatternDev pat,
+                                                   const FrzSurvivor* __restrict__ surv, unsigned long long surv_cap, int cls,
+                                                   const FrzRankView rv, FrzCounters* __restrict__ ctr,
+                                                   uint32_t index_offset, int reversed, FrzMatchDev* __restrict__ out,
+                                                   const FrzScoreHist hist) {
+    sw_generic_run(cv, pat, surv, surv_cap, cls, rv, ctr, index_offset, reversed, out, hist);
 }
 
 // literal patterns: the prefilter stage already produced (score, exact); just place the match
@@ -597,7 +614,97 @@ frz_status launch_sw_lanes(const FrzCorpusView& cv, const FrzPatternDev& pat, ui
     return FRZ_OK;
 }
 
+// ---- the scoring classes over the queries of a batch group (frz_match_list_batch_top): block row y scores query grp.j[y]'s
+// ---- survivors into its own list, with its pattern copied to shared memory.  No histogram: k_batch_top builds its own.
+__device__ __forceinline__ FrzRankView batch_rank(const FrzBatchDev& b, uint32_t n_tiles, uint32_t j) {
+    const uint64_t t0 = (uint64_t)j * n_tiles;
+    return FrzRankView{b.tile_out_base + t0, b.surv_bitmap + t0 * 32, b.word_prefix + t0 * 32};
+}
+template <int LANES, bool WRAP8, int VAR>
+__global__ void __launch_bounds__(kSwThreads, (kSw64MinBlocks<LANES, WRAP8>)) k_sw64_batch(const FrzCorpusView cv, const FrzBatchDev b,
+                                                                                          const __grid_constant__ FrzBatchGroup grp) {
+    __shared__ FrzPatternDev pat_s;
+    const uint32_t j = grp.j[blockIdx.y];
+    frz_batch_stage_pattern(b, j, &pat_s);
+    __syncthreads();
+    sw64_run<LANES, WRAP8, VAR>(cv, pat_s, frz_batch_lists(b, j), b.surv_cap, batch_rank(b, cv.n_tiles, j), b.ctr + j, 0, b.reversed[j],
+                                b.lists + j * b.list_stride, FrzScoreHist());
+}
+template <int LANES, bool WRAP8, int VAR>
+__global__ void __launch_bounds__(kSwThreads) k_sw_batch(const FrzCorpusView cv, const FrzBatchDev b, const __grid_constant__ FrzBatchGroup grp) {
+    __shared__ FrzPatternDev pat_s;
+    const uint32_t j = grp.j[blockIdx.y];
+    frz_batch_stage_pattern(b, j, &pat_s);
+    __syncthreads();
+    sw_run<LANES, 128, WRAP8, VAR>(cv, pat_s, frz_batch_lists(b, j).p[FRZ_C_COLS128], b.surv_cap, FRZ_C_COLS128, batch_rank(b, cv.n_tiles, j),
+                                   b.ctr + j, 0, b.reversed[j], b.lists + j * b.list_stride, FrzScoreHist());
+}
+__global__ void __launch_bounds__(64) k_sw_generic_batch(const FrzCorpusView cv, const FrzBatchDev b, const __grid_constant__ FrzBatchGroup grp) {
+    __shared__ FrzPatternDev pat_s;
+    const uint32_t j = grp.j[blockIdx.y];
+    frz_batch_stage_pattern(b, j, &pat_s);
+    __syncthreads();
+    sw_generic_run(cv, pat_s, frz_batch_lists(b, j).p[FRZ_C_GENERIC], b.surv_cap, FRZ_C_GENERIC, batch_rank(b, cv.n_tiles, j), b.ctr + j, 0,
+                   b.reversed[j], b.lists + j * b.list_stride, FrzScoreHist());
+}
+
+// the k_sw64 / k_sw variant frz_launch_sw picks for a pattern: 0 wrap8, 1 lane penalties, 2 the default
+int sw_variant(const FrzPatternDev& p) { return p.wrap8 ? 0 : (p.gap_extend == 0 && p.gap_open_x > 0) ? 1 : 2; }
+
+template <int LANES>
+frz_status launch_sw_batch_lanes(const FrzCorpusView& cv, const FrzBatchDev& b, const FrzPatternDev* h_pats, uint32_t nq,
+                                 cudaStream_t stream, FrzLaunchStats* st) {
+    for (int var = 0; var < 3; var++) {
+        FrzBatchGroup grp;
+        uint32_t ng = 0;
+        for (uint32_t j = 0; j < nq; j++)
+            if (h_pats[j].sw_lanes == LANES && sw_variant(h_pats[j]) == var) grp.j[ng++] = (uint16_t)j;
+        if (ng == 0) continue;
+        // the blocks of one single-query launch, split over the group (each query claims its own work items)
+        const uint32_t gx64 = std::max<uint32_t>(1, (uint32_t)(frz_sm_count() * kSw64MinBlocks<LANES, false>) / ng);
+        if (var == 0) k_sw64_batch<LANES, true, 0><<<dim3(gx64, ng), kSwThreads, 0, stream>>>(cv, b, grp);
+        else if (var == 1) k_sw64_batch<LANES, false, 8 | kSwVarLanePen><<<dim3(gx64, ng), kSwThreads, 0, stream>>>(cv, b, grp);
+        else k_sw64_batch<LANES, false, 8><<<dim3(gx64, ng), kSwThreads, 0, stream>>>(cv, b, grp);
+        if (st) st->launches++;
+        if (cv.max_gunits <= 4) continue;   // no window of 65..128 bytes
+        const size_t smem = SwCore<LANES, 128, false>::smem_bytes;
+        static bool attr_set_dev[64] = {};
+        bool& attr_set = attr_set_dev[frz_current_device() & 63];
+        if (!attr_set) {
+            FRZ_CUDA_TRY(cudaFuncSetAttribute(k_sw_batch<LANES, true, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            FRZ_CUDA_TRY(cudaFuncSetAttribute(k_sw_batch<LANES, false, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            FRZ_CUDA_TRY(cudaFuncSetAttribute(k_sw_batch<LANES, false, kSwVarLanePen>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            attr_set = true;
+        }
+        const uint32_t gx = std::max<uint32_t>(1, (uint32_t)(frz_sm_count() * 2) / ng);
+        if (var == 0) k_sw_batch<LANES, true, 0><<<dim3(gx, ng), kSwThreads, smem, stream>>>(cv, b, grp);
+        else if (var == 1) k_sw_batch<LANES, false, kSwVarLanePen><<<dim3(gx, ng), kSwThreads, smem, stream>>>(cv, b, grp);
+        else k_sw_batch<LANES, false, 0><<<dim3(gx, ng), kSwThreads, smem, stream>>>(cv, b, grp);
+        if (st) st->launches++;
+    }
+    FRZ_CUDA_TRY(cudaGetLastError());
+    return FRZ_OK;
+}
+
 }  // namespace
+
+frz_status frz_launch_sw_batch(const FrzCorpusView& cv, const FrzBatchDev& b, const FrzPatternDev* h_pats, uint32_t nq,
+                               cudaStream_t stream, FrzLaunchStats* st) {
+    if (cv.n_tiles == 0 || nq == 0) return FRZ_OK;
+    FRZ_TRY(launch_sw_batch_lanes<64>(cv, b, h_pats, nq, stream, st));
+    FRZ_TRY(launch_sw_batch_lanes<32>(cv, b, h_pats, nq, stream, st));
+    FRZ_TRY(launch_sw_batch_lanes<16>(cv, b, h_pats, nq, stream, st));
+    FRZ_TRY(launch_sw_batch_lanes<8>(cv, b, h_pats, nq, stream, st));
+    if (cv.max_gunits > 8) {   // windows > 128 bytes need a haystack > 128 bytes
+        FrzBatchGroup grp;
+        for (uint32_t j = 0; j < nq; j++) grp.j[j] = (uint16_t)j;
+        const uint32_t gx = std::max<uint32_t>(1, (uint32_t)(frz_sm_count() * 2) / nq);
+        k_sw_generic_batch<<<dim3(gx, nq), 64, 0, stream>>>(cv, b, grp);
+        FRZ_CUDA_TRY(cudaGetLastError());
+        if (st) st->launches++;
+    }
+    return FRZ_OK;
+}
 
 frz_status frz_launch_sw(const FrzCorpusView& cv, const FrzPatternDev& pat, uint32_t index_offset, bool reversed,
                          FrzWorkspace& ws, FrzMatchDev* d_out, cudaStream_t stream, FrzLaunchStats* st, const FrzScoreHist& hist,

@@ -252,6 +252,37 @@ FRZ_API frz_status frz_match_list(frz_matcher* m, const frz_corpus* corpus,
 FRZ_API frz_status frz_match_list_top(frz_matcher* m, const frz_corpus* corpus, uint64_t k,
                               frz_match* out, uint64_t* n_out, uint64_t* n_total);
 
+/* The reference has no such method: Matcher::match_list (src/matcher/mod.rs:212-222) of each of q matchers over one
+ * list, each truncated to its first k rows as by frz_match_list_top — many queries against one resident corpus (a fuzzy
+ * join, a service answering many users, "did you mean" for a batch of identifiers) in one call.
+ * For every j < q, out[j*k .. j*k + n_out[j]), n_out[j] and n_total[j] are bit for bit what frz_match_list_top(ms[j],
+ * corpus, k, ...) returns, for every matcher, config and sort strategy; rows out[j*k + n_out[j] .. (j+1)*k) are not
+ * written.  `out` is HOST memory with room for q*k matches; n_total may be NULL; k = 0 only counts (out may then be NULL);
+ * q = 0 is a no-op that makes no CUDA call.  A NULL ms, any NULL ms[j], a NULL corpus, a NULL n_out with q > 0, a NULL out
+ * with q*k > 0, or a q*k that overflows uint64_t or size_t is FRZ_ERR_INVALID_ARG, checked before any device work.  A
+ * matcher may appear more than once in ms; the call only reads the matchers' compiled patterns.  Blocking; neither the
+ * matchers nor the corpus may be used concurrently by another call.  Never FRZ_ERR_CAPACITY.
+ * Queries of one compiled pattern that is fuzzy, not negated, on the byte path and at most 64 bytes long, with k <= 1024,
+ * on a corpus of at most 2^18 rows (2^21 for max_typos = 0), when a call has at least 32 of them, run in sub-batches whose every stage covers all
+ * of the sub-batch's queries in one launch (per kernel variant present), with one upload, one read-back and one
+ * synchronise per sub-batch (DESIGN.md §4.11: where that was measured faster than a loop).  The sub-batch's device scratch has a fixed budget,
+ * so the memory a call holds does not grow with q (beyond it: the rows and patterns of a sub-batch); it is released when
+ * the call returns.  Every other query (multi-pattern, negated, literal modes, unicode, 65-1024-byte needles, the empty
+ * matcher, k > 1024, larger corpora and smaller batches) runs frz_match_list_top's pipeline inside the same call, one
+ * after another: correct, but not faster than a loop. */
+FRZ_API frz_status frz_match_list_batch_top(frz_matcher* const* ms, uint64_t q, const frz_corpus* corpus, uint64_t k,
+                                            frz_match* out, uint64_t* n_out, uint64_t* n_total);
+/* Test aid: the corpus-size and query-count limits of frz_match_list_batch_top's batched path, process-wide (0 restores
+ * a limit's default: 2^18 rows, 32 queries; max_typos = 0 queries batch up to the larger of max_rows and 2^21 rows;
+ * fewer than 2 queries never batch).  Lets tests reach the batched kernels with
+ * small batches and tools/bench_batch.py time the batched path on both sides of the defaults.  Not for concurrent use with
+ * batch calls. */
+FRZ_API void frz_debug_batch_limits(uint64_t max_rows, uint64_t min_queries);
+/* Test aid: what the calling thread's last frz_match_list_batch_top did: [0] queries answered by the batched kernels,
+ * [1] queries of sub-batches whose survivor lists overflowed (answered again by frz_match_list_top's pipeline),
+ * [2] sub-batches run, [3] kernel launches of the batched path.  All zero after a call that ran no sub-batch. */
+FRZ_API void frz_debug_batch_last(uint64_t out[4]);
+
 /* ---------------------------------------------------------------- subsets
  *
  * A chosen set of rows of a resident corpus, matched without staging them again: a picker scoped to one directory, a
