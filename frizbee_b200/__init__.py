@@ -92,6 +92,7 @@ def lib():
     L.frz_match_list.argtypes = [vp, vp, vp, u64, C.POINTER(u64)]
     L.frz_match_list_top.argtypes = [vp, vp, u64, vp, C.POINTER(u64), C.POINTER(u64)]
     L.frz_match_list_batch_top.argtypes = [vp, u64, vp, u64, vp, vp, vp]
+    L.frz_match_list_batch.argtypes = [vp, u64, vp, vp, vp, u64, vp, vp, vp]
     L.frz_debug_batch_limits.argtypes = [u64, u64]
     L.frz_debug_batch_limits.restype = None
     L.frz_debug_batch_last.argtypes = [vp]
@@ -534,8 +535,33 @@ def match_list_batch_top(matchers, corpus: Corpus, k: int) -> Tuple[np.ndarray, 
     return out, n_out.astype(np.int64), n_total.astype(np.int64)
 
 
+def match_list_batch(matchers, corpus: Corpus, k: int, subsets=None, boosts=None) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """frz_match_list_batch: match_list_batch_top where query j may have its own subset and boost.  subsets / boosts: None,
+    or one Subset / Boost / None per matcher.  Query j's rows are those of matcher j's match_list_ranked_array(corpus,
+    boosts[j], k, subsets[j]) when it has a boost, else of match_list_subset_top_array(corpus, subsets[j], k) when it has
+    a subset, else of match_list_top_array(corpus, k).  Returns the (q, k) rows, n_out and n_total as match_list_batch_top."""
+    q, k = len(matchers), int(k)
+
+    def handles(xs, what):
+        if xs is None:
+            return None
+        xs = list(xs)
+        if len(xs) != q:
+            raise ValueError(f"{q} matchers need {q} {what}, got {len(xs)}")
+        return (C.c_void_p * max(q, 1))(*[x._h.value if x is not None else None for x in xs])
+
+    hs, hb = handles(subsets, "subsets"), handles(boosts, "boosts")
+    ms = (C.c_void_p * max(q, 1))(*[m._h.value for m in matchers])
+    out = np.zeros((q, k), dtype=MATCH_DTYPE)
+    n_out = np.zeros(q, dtype=np.uint64)
+    n_total = np.zeros(q, dtype=np.uint64)
+    _check(lib().frz_match_list_batch(ms, q, corpus._h, hs, hb, k, out.ctypes.data if out.size else None, n_out.ctypes.data,
+                                      n_total.ctypes.data))
+    return out, n_out.astype(np.int64), n_total.astype(np.int64)
+
+
 def batch_last() -> dict:
-    """Test aid (frz_debug_batch_last): what this thread's last match_list_batch_top did."""
+    """Test aid (frz_debug_batch_last): what this thread's last match_list_batch_top or match_list_batch did."""
     v = np.zeros(4, dtype=np.uint64)
     lib().frz_debug_batch_last(v.ctypes.data)
     return {"batched": int(v[0]), "overflowed": int(v[1]), "sub_batches": int(v[2]), "launches": int(v[3])}

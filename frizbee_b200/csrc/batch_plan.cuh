@@ -8,6 +8,12 @@
 //                             histograms (high, then low score byte): the threshold score T, the rows above it, and how many
 //                             rows scoring exactly T are kept (the first ones in list order).  The kept rows are then ordered
 //                             by (descending score, list position), which is the stable sort's order.
+//
+// A scoped or ranked query (frz_match_list_batch) first drops the rows of its list that are not members of its subset
+// (frz_batch_member); its total is the members' count.  It is then ordered as above on the value
+//   v = ranked ? clamp(score + boost[index], 0, 65535) : score                       (frz_batch_ranked_value)
+// and a ranked query is ordered by v under every strategy (the strategy's direction only orders ties, through the list).
+// An index-ordered query that is not ranked keeps its first `rows` members in list order.
 #pragma once
 #include <stdint.h>
 
@@ -66,3 +72,14 @@ FRZ_BP_HD bool frz_batch_keep(uint32_t score, const FrzBatchCut& c, uint64_t eq_
 // Sort key of a kept row: ascending keys are the stable descending-score order.
 FRZ_BP_HD uint64_t frz_batch_key(uint32_t score, uint32_t list_pos) { return (uint64_t)(0xFFFFu - score) << 32 | list_pos; }
 FRZ_BP_HD uint32_t frz_batch_key_pos(uint64_t key) { return (uint32_t)key; }
+
+// Membership of a row in a subset bitmap over the indices [0, n_bits) (frz_subset: rows appended after the subset was made
+// lie past n_bits and are not members).
+FRZ_BP_HD bool frz_batch_member(const uint32_t* bits, uint64_t n_bits, uint32_t index) {
+    return index < n_bits && (bits[index >> 5] >> (index & 31) & 1u);
+}
+// The ranked value of a row, in 32-bit arithmetic: boost is boost[index], or 0 for an index past the boost array.
+FRZ_BP_HD uint32_t frz_batch_ranked_value(uint32_t score, int32_t boost) {
+    const int32_t v = (int32_t)score + boost;
+    return v < 0 ? 0u : v > 0xFFFF ? 0xFFFFu : (uint32_t)v;
+}

@@ -205,7 +205,7 @@ struct frz_corpus {
     // metadata of the tiles a frz_corpus_replace re-packs (grow-only; a replace releases it, and the ingest staging, once
     // they pass 64 MiB)
     std::unique_ptr<FrzCorpusStorage> edit_tiles;
-    // pinned staging of frz_match_list_batch_top (patterns up, rows and counts down), grow-only
+    // pinned staging of frz_match_list_batch (patterns up, rows and counts down), grow-only
     mutable FrzPinnedArray<uint8_t> batch_stage;
 };
 
@@ -367,10 +367,22 @@ frz_status frz_launch_prefilter_batch(const FrzCorpusView& cv, const FrzBatchDev
 // sw.cu: the scoring classes of frz_launch_sw, one launch per kernel variant present
 frz_status frz_launch_sw_batch(const FrzCorpusView& cv, const FrzBatchDev& b, const FrzPatternDev* h_pats, uint32_t nq,
                                cudaStream_t stream, FrzLaunchStats* st);
+// The subset and boost of one query of frz_match_list_batch (host.cu), read by k_batch_top<ScopedKey> (batch.cu).  A query
+// without either has scoped = ranked = 0 and is answered as by frz_match_list_batch_top.
+struct FrzBatchScope {
+    const uint32_t* bits;    // scoped: the subset's bitmap over [0, n_bits) (frz_batch_member)
+    const int16_t* boost;    // ranked: boost[index] for index < n_boost, 0 past it
+    uint64_t n_bits;
+    uint32_t n_boost;
+    uint8_t scoped;          // 1: only the subset's members are rows of the query
+    uint8_t ranked;          // 1: the rows are ordered by clamp(score + boost[index], 0, 65535) under every strategy
+    uint8_t pad[2];
+};
 // batch.cu: per query, its first min(k, total) rows → rows[j * k ...] and its total → totals[j], or kFrzBatchOverflow
-// there when its sticky device error is set (k <= kFrzBatchMaxK)
-frz_status frz_launch_batch_top(const FrzBatchDev& b, uint32_t nq, uint32_t k, FrzMatchDev* rows, unsigned long long* totals,
-                                cudaStream_t stream, FrzLaunchStats* st);
+// there when its sticky device error is set (k <= kFrzBatchMaxK).  scopes: nullptr, or the nq queries' FrzBatchScope
+// records on the device (a sub-batch with a scoped or ranked query).
+frz_status frz_launch_batch_top(const FrzBatchDev& b, const FrzBatchScope* scopes, uint32_t nq, uint32_t k, FrzMatchDev* rows,
+                                unsigned long long* totals, cudaStream_t stream, FrzLaunchStats* st);
 
 // k-way merge of per-shard runs (merge.cu) with caller-owned scratch — one per concurrent user (parallel.cu: one per rank)
 #define FRZ_MERGE_MAX_RUNS 64

@@ -1453,10 +1453,10 @@ extern "C" frz_status frz_match_list_top(frz_matcher* m, const frz_corpus* corpu
 }
 
 // ---------------------------------------------------------------------------------- batched top-K
-// frz_match_list_batch_top (DESIGN.md §4.11).  Queries of the batched class run in sub-batches whose every stage is one
-// launch (per kernel variant present) over all of the sub-batch's queries, with one upload, one read-back and one
-// synchronise per sub-batch; every other query, and every query of an overflowed sub-batch, runs frz_match_list_top's
-// pipeline.
+// frz_match_list_batch and frz_match_list_batch_top (DESIGN.md §4.11).  Queries of the batched class run in sub-batches
+// whose every stage is one launch (per kernel variant present) over all of the sub-batch's queries, with one upload, one
+// read-back and one synchronise per sub-batch; every other query, and every query of an overflowed sub-batch, runs its
+// single-query call's pipeline (frz_match_list_top, _subset_top or _ranked).  The entry points follow the ranked calls.
 namespace {
 
 // Device scratch of one sub-batch's queries, in one allocation: a fixed budget, so a batch call holds the same scratch for
@@ -1478,25 +1478,25 @@ thread_local uint64_t g_batch_last[4] = {0, 0, 0, 0};   // batched queries, over
 
 struct BatchLayout {
     uint64_t nt = 0, stride = 0, cap = 0, k = 0;
-    uint64_t off[13] = {};   // byte offsets of the arrays below, in this order
+    uint64_t off[14] = {};   // byte offsets of the arrays below, in this order
     uint64_t bytes = 0;
-    enum { CTR, BITMAP, PREFIX, TCOUNT, TBASE, SURV, LISTS, PATS, REV, BYSC, TOTALS, ROWS, END };
+    enum { CTR, BITMAP, PREFIX, TCOUNT, TBASE, SURV, LISTS, PATS, REV, BYSC, SCOPE, TOTALS, ROWS, END };
     // queries per sub-batch for this corpus and k (0: fewer than two fit the budget)
     static uint64_t per_query(const FrzCorpusStorage& cs, uint64_t k, uint64_t cap) {
         const uint64_t nt = cs.n_tiles;
         return sizeof(FrzCounters) + nt * 32 * (sizeof(uint32_t) + sizeof(uint16_t)) + nt * (sizeof(uint32_t) + sizeof(uint64_t)) +
                FRZ_N_CLASSES * cap * sizeof(FrzSurvivor) + std::max<uint64_t>(cs.n, 1) * sizeof(FrzMatchDev) + sizeof(FrzPatternDev) + 2 +
-               sizeof(unsigned long long) + k * sizeof(FrzMatchDev) + 13 * 256 / 2;
+               sizeof(FrzBatchScope) + sizeof(unsigned long long) + k * sizeof(FrzMatchDev) + 13 * 256 / 2;
     }
     BatchLayout(const FrzCorpusStorage& cs, uint64_t k_, uint64_t cap_, uint64_t qs) : nt(cs.n_tiles), stride(std::max<uint64_t>(cs.n, 1)), cap(cap_), k(k_) {
         const uint64_t size[END] = {qs * sizeof(FrzCounters), qs * nt * 32 * sizeof(uint32_t), qs * nt * 32 * sizeof(uint16_t),
                                     qs * nt * sizeof(uint32_t), qs * nt * sizeof(uint64_t), qs * FRZ_N_CLASSES * cap * sizeof(FrzSurvivor),
                                     qs * stride * sizeof(FrzMatchDev), qs * sizeof(FrzPatternDev), qs, qs,
-                                    qs * sizeof(unsigned long long), qs * k * sizeof(FrzMatchDev)};
+                                    qs * sizeof(FrzBatchScope), qs * sizeof(unsigned long long), qs * k * sizeof(FrzMatchDev)};
         uint64_t at = 0;
         for (int i = 0; i < END; i++) {
-            // CTR..BITMAP are zeroed as one range, PATS..BYSC uploaded as one, TOTALS..ROWS read back as one
-            const bool packed = i == BITMAP || i == REV || i == BYSC || i == ROWS;
+            // CTR..BITMAP are zeroed as one range, PATS..SCOPE uploaded as one, TOTALS..ROWS read back as one
+            const bool packed = i == BITMAP || i == REV || i == BYSC || i == SCOPE || i == ROWS;
             if (!packed) at = (at + 255) & ~255ull;
             else at = (at + 7) & ~7ull;
             off[i] = at;
@@ -1528,15 +1528,12 @@ bool batch_selected(const frz_matcher* m, const FrzCorpusStorage& cs) {
     return cs.n <= limit;
 }
 
-frz_status batch_single(frz_matcher* m, const frz_corpus* c, uint64_t k, frz_match* out, uint64_t* n_out, uint64_t* n_total) {
-    return match_list_host(m, c, 0, m->config.sort, k, SubsetScope(), out, k, n_out, n_total);
-}
-
-// One sub-batch: queries which[0..ns) of ms, all of the batched class.  *overflow: a survivor list overflowed, nothing was
+// One sub-batch: queries which[0..ns) of ms, all of the batched class.  scopes: nullptr when no query of the call is scoped
+// or ranked, else every query's subset and boost (indexed as ms).  *overflow: a survivor list overflowed, nothing was
 // written to the results (the caller runs the queries one by one).
-frz_status batch_run(frz_matcher* const* ms, const uint64_t* which, uint32_t ns, const frz_corpus* c, uint64_t k,
-                     const BatchLayout& L, uint8_t* d, frz_match* out, uint64_t* n_out, uint64_t* n_total, bool* overflow,
-                     FrzLaunchStats& st) {
+frz_status batch_run(frz_matcher* const* ms, const FrzBatchScope* scopes, const uint64_t* which, uint32_t ns, const frz_corpus* c,
+                     uint64_t k, const BatchLayout& L, uint8_t* d, frz_match* out, uint64_t* n_out, uint64_t* n_total,
+                     bool* overflow, FrzLaunchStats& st) {
     const FrzCorpusStorage& cs = c->st;
     cudaStream_t stream = nullptr;
     *overflow = false;
@@ -1547,12 +1544,16 @@ frz_status batch_run(frz_matcher* const* ms, const uint64_t* which, uint32_t ns,
     FrzPatternDev* h_pats = reinterpret_cast<FrzPatternDev*>(h);
     uint8_t* h_rev = h + (L.off[BatchLayout::REV] - L.off[BatchLayout::PATS]);
     uint8_t* h_bysc = h + (L.off[BatchLayout::BYSC] - L.off[BatchLayout::PATS]);
+    FrzBatchScope* h_scope = reinterpret_cast<FrzBatchScope*>(h + (L.off[BatchLayout::SCOPE] - L.off[BatchLayout::PATS]));
+    bool scoped = false;   // a query of the sub-batch is scoped or ranked: the last stage is k_batch_top<ScopedKey>
     for (uint32_t j = 0; j < ns; j++) {
         const frz_matcher* m = ms[which[j]];
         const uint8_t sort = m->config.sort;
         h_pats[j] = m->compiled[0].dev;
         h_rev[j] = sort == FRZ_SORT_INDEX_DESC || sort == FRZ_SORT_SCORE_THEN_INDEX_DESC;
         h_bysc[j] = sort == FRZ_SORT_SCORE_THEN_INDEX_ASC || sort == FRZ_SORT_SCORE_THEN_INDEX_DESC;
+        h_scope[j] = scopes ? scopes[which[j]] : FrzBatchScope();
+        scoped |= h_scope[j].scoped || h_scope[j].ranked;
     }
     FrzBatchDev b;
     b.pats = reinterpret_cast<const FrzPatternDev*>(d + L.off[BatchLayout::PATS]);
@@ -1575,7 +1576,8 @@ frz_status batch_run(frz_matcher* const* ms, const uint64_t* which, uint32_t ns,
     const FrzCorpusView cv = cs.view();
     FRZ_TRY(frz_launch_prefilter_batch(cv, b, h_pats, ns, stream, &st));
     FRZ_TRY(frz_launch_sw_batch(cv, b, h_pats, ns, stream, &st));
-    FRZ_TRY(frz_launch_batch_top(b, ns, (uint32_t)k, rows, totals, stream, &st));
+    const FrzBatchScope* d_scope = reinterpret_cast<const FrzBatchScope*>(d + L.off[BatchLayout::SCOPE]);
+    FRZ_TRY(frz_launch_batch_top(b, scoped ? d_scope : nullptr, ns, (uint32_t)k, rows, totals, stream, &st));
     // the staged patterns are not read again: the read-back may reuse the staging
     FRZ_CUDA_TRY(cudaMemcpyAsync(h, totals, down, cudaMemcpyDeviceToHost, stream));
     FRZ_CUDA_TRY(cudaStreamSynchronize(stream));
@@ -1593,56 +1595,6 @@ frz_status batch_run(frz_matcher* const* ms, const uint64_t* which, uint32_t ns,
 }
 
 }  // namespace
-
-extern "C" frz_status frz_match_list_batch_top(frz_matcher* const* ms, uint64_t q, const frz_corpus* corpus, uint64_t k, frz_match* out,
-                                               uint64_t* n_out, uint64_t* n_total) {
-    if (!ms || !corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
-    for (uint64_t j = 0; j < q; j++)
-        if (!ms[j]) return frz_fail(FRZ_ERR_INVALID_ARG, "null matcher at %llu", (unsigned long long)j);
-    if (q && !n_out) return frz_fail(FRZ_ERR_INVALID_ARG, "null n_out");
-    if (k && (q > UINT64_MAX / k || q * k > SIZE_MAX / sizeof(frz_match)))
-        return frz_fail(FRZ_ERR_INVALID_ARG, "q * k overflows: q = %llu, k = %llu", (unsigned long long)q, (unsigned long long)k);
-    if (q * k > 0 && !out) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
-    if (q == 0) return FRZ_OK;
-    int n_dev = 0;
-    if (cudaGetDeviceCount(&n_dev) != cudaSuccess || n_dev == 0) {
-        cudaGetLastError();
-        return frz_fail(FRZ_ERR_NO_DEVICE, "no CUDA device available; this library has no CPU fallback");
-    }
-    FRZ_TRY(frz_ensure_device(corpus->st.device));
-    const FrzCorpusStorage& cs = corpus->st;
-    FRZ_TRY(frz_check_index_range(cs.n, 0));
-    for (uint64_t& v : g_batch_last) v = 0;
-    auto single = [&](uint64_t j) { return batch_single(ms[j], corpus, k, k ? out + j * k : nullptr, &n_out[j], n_total ? &n_total[j] : nullptr); };
-    std::vector<uint64_t> batched;
-    const uint64_t cap = batch_survivor_cap(cs);
-    const uint64_t fit = k <= kFrzBatchMaxK ? kBatchScratchBytes / BatchLayout::per_query(cs, k, cap) : 0;
-    const uint64_t qs_max = std::min<uint64_t>(fit, kFrzBatchMaxSub);
-    for (uint64_t j = 0; j < q; j++) {
-        if (qs_max >= 2 && batchable(ms[j], cs) && batch_selected(ms[j], cs)) batched.push_back(j);
-        else FRZ_TRY(single(j));
-    }
-    if (batched.size() < std::max<uint64_t>(2, g_batch_min_queries.load())) {   // a few queries cost what a loop of frz_match_list_top costs
-        for (uint64_t j : batched) FRZ_TRY(single(j));
-        return FRZ_OK;
-    }
-    const uint64_t qs = std::min<uint64_t>(qs_max, batched.size());
-    const BatchLayout L(cs, k, cap, qs);
-    FrzDevArray<uint8_t> scratch;   // released when the call returns
-    FRZ_TRY(scratch.reserve(L.bytes));
-    for (uint64_t s = 0; s < batched.size(); s += qs) {
-        const uint32_t ns = (uint32_t)std::min<uint64_t>(qs, batched.size() - s);
-        bool overflow = false;
-        FrzLaunchStats st;
-        FRZ_TRY(batch_run(ms, batched.data() + s, ns, corpus, k, L, scratch.get(), out, n_out, n_total, &overflow, st));
-        g_batch_last[overflow ? 1 : 0] += ns;
-        g_batch_last[2]++;
-        g_batch_last[3] += st.launches;
-        if (overflow)   // the single-query pipeline retries with worst-case lists
-            for (uint32_t j = 0; j < ns; j++) FRZ_TRY(single(batched[s + j]));
-    }
-    return FRZ_OK;
-}
 
 extern "C" void frz_debug_batch_limits(uint64_t max_rows, uint64_t min_queries) {
     g_batch_max_rows = max_rows ? max_rows : kBatchMaxRows;
@@ -1782,6 +1734,14 @@ frz_status grow_boost(frz_boost* b, uint64_t n) {
     b->values = std::move(grown);
     return FRZ_OK;
 }
+
+Ranking ranking_of(const frz_boost& b) {
+    Ranking rank;
+    rank.boost = b.values.get();
+    rank.n = (uint32_t)b.values.cap();
+    rank.max_boost = (uint32_t)b.max_set;
+    return rank;
+}
 }  // namespace
 
 extern "C" frz_status frz_boost_create(const frz_corpus* c, const int16_t* values, uint64_t n, frz_boost** out) {
@@ -1834,11 +1794,109 @@ extern "C" frz_status frz_match_list_ranked(frz_matcher* m, const frz_corpus* co
     FRZ_TRY(frz_ensure_device(corpus->st.device));
     SubsetScope scope;
     if (s) FRZ_TRY(subset_scope(m, corpus, *s, nullptr, &scope));
-    Ranking rank;
-    rank.boost = b->values.get();
-    rank.n = (uint32_t)b->values.cap();
-    rank.max_boost = (uint32_t)b->max_set;
+    const Ranking rank = ranking_of(*b);
     return match_list_host(m, corpus, 0, m->config.sort, k, scope, out, k, n_out, n_total, &rank);
+}
+
+// ---------------------------------------------------------------------------------- batched top-K: entry points
+namespace {
+// query j's single-query call: frz_match_list_ranked with a boost, else frz_match_list_subset_top with a subset, else
+// frz_match_list_top
+frz_status batch_single(frz_matcher* m, const frz_corpus* c, const frz_subset* s, const frz_boost* b, uint64_t k, frz_match* out,
+                        uint64_t* n_out, uint64_t* n_total) {
+    SubsetScope scope;
+    if (s) FRZ_TRY(subset_scope(m, c, *s, nullptr, &scope));
+    if (!b) return match_list_host(m, c, 0, m->config.sort, k, scope, out, k, n_out, n_total);
+    const Ranking rank = ranking_of(*b);
+    return match_list_host(m, c, 0, m->config.sort, k, scope, out, k, n_out, n_total, &rank);
+}
+}  // namespace
+
+extern "C" frz_status frz_match_list_batch(frz_matcher* const* ms, uint64_t q, const frz_corpus* corpus,
+                                           const frz_subset* const* subsets, const frz_boost* const* boosts, uint64_t k,
+                                           frz_match* out, uint64_t* n_out, uint64_t* n_total) {
+    if (!ms || !corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    for (uint64_t j = 0; j < q; j++)
+        if (!ms[j]) return frz_fail(FRZ_ERR_INVALID_ARG, "null matcher at %llu", (unsigned long long)j);
+    for (uint64_t j = 0; j < q; j++) {
+        if (subsets && subsets[j] && subsets[j]->corpus != corpus)
+            return frz_fail(FRZ_ERR_INVALID_ARG, "the subset of query %llu was made on another corpus", (unsigned long long)j);
+        if (boosts && boosts[j] && boosts[j]->corpus != corpus)
+            return frz_fail(FRZ_ERR_INVALID_ARG, "the boost of query %llu was made on another corpus", (unsigned long long)j);
+    }
+    if (q && !n_out) return frz_fail(FRZ_ERR_INVALID_ARG, "null n_out");
+    if (k && (q > UINT64_MAX / k || q * k > SIZE_MAX / sizeof(frz_match)))
+        return frz_fail(FRZ_ERR_INVALID_ARG, "q * k overflows: q = %llu, k = %llu", (unsigned long long)q, (unsigned long long)k);
+    if (q * k > 0 && !out) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
+    if (q == 0) return FRZ_OK;
+    int n_dev = 0;
+    if (cudaGetDeviceCount(&n_dev) != cudaSuccess || n_dev == 0) {
+        cudaGetLastError();
+        return frz_fail(FRZ_ERR_NO_DEVICE, "no CUDA device available; this library has no CPU fallback");
+    }
+    FRZ_TRY(frz_ensure_device(corpus->st.device));
+    const FrzCorpusStorage& cs = corpus->st;
+    FRZ_TRY(frz_check_index_range(cs.n, 0));
+    for (uint64_t& v : g_batch_last) v = 0;
+    auto subset_of = [&](uint64_t j) { return subsets ? subsets[j] : nullptr; };
+    auto boost_of = [&](uint64_t j) { return boosts ? boosts[j] : nullptr; };
+    auto single = [&](uint64_t j) {
+        return batch_single(ms[j], corpus, subset_of(j), boost_of(j), k, k ? out + j * k : nullptr, &n_out[j],
+                            n_total ? &n_total[j] : nullptr);
+    };
+    std::vector<uint64_t> batched;
+    const uint64_t cap = batch_survivor_cap(cs);
+    const uint64_t fit = k <= kFrzBatchMaxK ? kBatchScratchBytes / BatchLayout::per_query(cs, k, cap) : 0;
+    const uint64_t qs_max = std::min<uint64_t>(fit, kFrzBatchMaxSub);
+    for (uint64_t j = 0; j < q; j++) {
+        if (qs_max >= 2 && batchable(ms[j], cs) && batch_selected(ms[j], cs)) batched.push_back(j);
+        else FRZ_TRY(single(j));
+    }
+    if (batched.size() < std::max<uint64_t>(2, g_batch_min_queries.load())) {   // a few queries cost what a loop of single calls costs
+        for (uint64_t j : batched) FRZ_TRY(single(j));
+        return FRZ_OK;
+    }
+    // every query's subset and boost, as k_batch_top<ScopedKey> reads them (none when no query has either)
+    std::vector<FrzBatchScope> scopes;
+    for (uint64_t j : batched) {
+        const frz_subset* s = subset_of(j);
+        const frz_boost* b = boost_of(j);
+        if (!s && !b) continue;
+        if (scopes.empty()) scopes.resize(q);
+        FrzBatchScope& r = scopes[j];
+        if (s) {
+            r.scoped = 1;
+            r.bits = s->bits.get();
+            r.n_bits = s->n_bits;
+        }
+        if (b) {
+            r.ranked = 1;
+            r.boost = b->values.get();
+            r.n_boost = (uint32_t)b->values.cap();
+        }
+    }
+    const uint64_t qs = std::min<uint64_t>(qs_max, batched.size());
+    const BatchLayout L(cs, k, cap, qs);
+    FrzDevArray<uint8_t> scratch;   // released when the call returns
+    FRZ_TRY(scratch.reserve(L.bytes));
+    for (uint64_t s = 0; s < batched.size(); s += qs) {
+        const uint32_t ns = (uint32_t)std::min<uint64_t>(qs, batched.size() - s);
+        bool overflow = false;
+        FrzLaunchStats st;
+        FRZ_TRY(batch_run(ms, scopes.empty() ? nullptr : scopes.data(), batched.data() + s, ns, corpus, k, L, scratch.get(), out,
+                          n_out, n_total, &overflow, st));
+        g_batch_last[overflow ? 1 : 0] += ns;
+        g_batch_last[2]++;
+        g_batch_last[3] += st.launches;
+        if (overflow)   // the single-query pipeline retries with worst-case lists
+            for (uint32_t j = 0; j < ns; j++) FRZ_TRY(single(batched[s + j]));
+    }
+    return FRZ_OK;
+}
+
+extern "C" frz_status frz_match_list_batch_top(frz_matcher* const* ms, uint64_t q, const frz_corpus* corpus, uint64_t k, frz_match* out,
+                                               uint64_t* n_out, uint64_t* n_total) {
+    return frz_match_list_batch(ms, q, corpus, nullptr, nullptr, k, out, n_out, n_total);
 }
 
 extern "C" frz_status frz_match_list_into(frz_matcher* m, const frz_corpus* corpus, uint32_t index_offset, frz_match* out,

@@ -272,14 +272,16 @@ FRZ_API frz_status frz_match_list_top(frz_matcher* m, const frz_corpus* corpus, 
  * after another: correct, but not faster than a loop. */
 FRZ_API frz_status frz_match_list_batch_top(frz_matcher* const* ms, uint64_t q, const frz_corpus* corpus, uint64_t k,
                                             frz_match* out, uint64_t* n_out, uint64_t* n_total);
-/* Test aid: the corpus-size and query-count limits of frz_match_list_batch_top's batched path, process-wide (0 restores
+/* Test aid: the corpus-size and query-count limits of the batched path of frz_match_list_batch_top and
+ * frz_match_list_batch, process-wide (0 restores
  * a limit's default: 2^18 rows, 32 queries; max_typos = 0 queries batch up to the larger of max_rows and 2^21 rows;
  * fewer than 2 queries never batch).  Lets tests reach the batched kernels with
  * small batches and tools/bench_batch.py time the batched path on both sides of the defaults.  Not for concurrent use with
  * batch calls. */
 FRZ_API void frz_debug_batch_limits(uint64_t max_rows, uint64_t min_queries);
-/* Test aid: what the calling thread's last frz_match_list_batch_top did: [0] queries answered by the batched kernels,
- * [1] queries of sub-batches whose survivor lists overflowed (answered again by frz_match_list_top's pipeline),
+/* Test aid: what the calling thread's last frz_match_list_batch_top or frz_match_list_batch did: [0] queries answered by
+ * the batched kernels, [1] queries of sub-batches whose survivor lists overflowed (answered again by their single-query
+ * call's pipeline),
  * [2] sub-batches run, [3] kernel launches of the batched path.  All zero after a call that ran no sub-batch. */
 FRZ_API void frz_debug_batch_last(uint64_t out[4]);
 
@@ -354,6 +356,23 @@ FRZ_API void frz_boost_destroy(frz_boost* b);
  * FRZ_ERR_INVALID_ARG. */
 FRZ_API frz_status frz_match_list_ranked(frz_matcher* m, const frz_corpus* c, const frz_subset* s, const frz_boost* b,
                                          uint64_t k, frz_match* out, uint64_t* n_out, uint64_t* n_total);
+
+/* frz_match_list_batch_top (above) where each query may have its own subset and boost, in one call: a service whose users
+ * each search their own rows (a subset) ranked by a prior (a boost).  The reference has no such method (see the subset
+ * and ranked calls above).  For every j < q, out[j*k .. j*k + n_out[j]), n_out[j] and n_total[j] are bit for bit what the
+ * matching single-query call returns, for every matcher, config and sort strategy:
+ *   boosts[j] != NULL:       frz_match_list_ranked(ms[j], corpus, subsets[j], boosts[j], k, ...);
+ *   else subsets[j] != NULL: frz_match_list_subset_top(ms[j], corpus, subsets[j], k, ...);
+ *   else:                    frz_match_list_top(ms[j], corpus, k, ...).
+ * subsets and boosts may be NULL, meaning every entry is NULL; frz_match_list_batch(ms, q, c, NULL, NULL, k, ...) is
+ * frz_match_list_batch_top(ms, q, c, k, ...).  All other argument rules, the batched class and its limits are
+ * frz_match_list_batch_top's.  A subset or boost made on another corpus is FRZ_ERR_INVALID_ARG; every argument is checked
+ * before any device work.  The same subset, boost or matcher may appear for many queries; the call only reads them.
+ * A batched-class query runs the batched kernels whether or not it is scoped or ranked: its non-members are scored with
+ * the rest of the corpus and dropped when its rows are chosen (DESIGN.md §4.11). */
+FRZ_API frz_status frz_match_list_batch(frz_matcher* const* ms, uint64_t q, const frz_corpus* corpus,
+                                        const frz_subset* const* subsets, const frz_boost* const* boosts, uint64_t k,
+                                        frz_match* out, uint64_t* n_out, uint64_t* n_total);
 
 /* Specialized::match_list / Matcher::match_list_into (src/matcher/algo.rs:17-22,
  * src/matcher/mod.rs:373-392): matches appended in input (index-ascending) order,
