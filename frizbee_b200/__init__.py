@@ -16,11 +16,13 @@ import numpy as np
 from .types import (CaseMatching, CConfig, CMatch, Config, CPattern, Match, Matching, Pattern, Scoring,
                     SortStrategy, UnicodeMatching, as_pattern, pattern_array)
 
-__all__ = ["Matcher", "Corpus", "Subset", "Boost", "Pattern", "Config", "Scoring", "Match", "SortStrategy", "CaseMatching",
+__all__ = ["Matcher", "Corpus", "Subset", "Boost", "Groups", "GROUP_NONE", "Pattern", "Config", "Scoring", "Match", "SortStrategy", "CaseMatching",
            "UnicodeMatching", "Matching", "FrizbeeError", "parse_query", "parse_atom", "radix_sort_matches",
            "MATCH_DTYPE", "lib", "lib_path"]
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
+GROUP_NONE = 0xFFFFFFFF   # FRZ_GROUP_NONE: a row in no group
+_U64_MAX = 0xFFFFFFFFFFFFFFFF   # UINT64_MAX: no k limit / no per-group cap
 MATCH_DTYPE = np.dtype([("index", "<u4"), ("score", "<u2"), ("exact", "u1"), ("_pad", "u1")])
 
 STATUS_NAMES = {0: "FRZ_OK", 1: "FRZ_ERR_INVALID_ARG", 2: "FRZ_ERR_NEEDLE_TOO_LONG", 3: "FRZ_ERR_GAP_OVERFLOW",
@@ -109,6 +111,13 @@ def lib():
     L.frz_boost_destroy.argtypes = [vp]
     L.frz_boost_destroy.restype = None
     L.frz_match_list_ranked.argtypes = [vp, vp, vp, vp, u64, vp, C.POINTER(u64), C.POINTER(u64)]
+    L.frz_groups_create.argtypes = [vp, vp, u64, u64, C.POINTER(vp)]
+    L.frz_groups_set.argtypes = [vp, vp, vp, u64]
+    L.frz_groups_count.restype = u64
+    L.frz_groups_count.argtypes = [vp]
+    L.frz_groups_destroy.argtypes = [vp]
+    L.frz_groups_destroy.restype = None
+    L.frz_match_list_collapsed.argtypes = [vp, vp, vp, vp, vp, u64, u64, vp, C.POINTER(u64), C.POINTER(u64), vp]
     L.frz_match_list_into.argtypes = [vp, vp, u32, vp, u64, C.POINTER(u64)]
     L.frz_match_list_host.argtypes = [vp, vp, vp, u64, C.c_int, vp, u64, C.POINTER(u64)]
     L.frz_match_list_host_arrow.argtypes = [vp, vp, vp, C.c_int, u64, C.c_int, vp, u64, C.POINTER(u64)]
@@ -268,6 +277,18 @@ class Corpus:
         _check(lib().frz_boost_create(self._h, values.ctypes.data if values.size else None, len(values), C.byref(h)))
         return Boost(h, self)
 
+    def groups(self, ids=None, n_groups: Optional[int] = None) -> "Groups":
+        """A resident group id per row for Matcher.match_list_collapsed_array: ids[i] (uint32) is the group of row i, or
+        GROUP_NONE; rows past len(ids) are in no group; at most len(self) ids.  n_groups defaults to one more than the
+        largest id that is not GROUP_NONE (1 when there is none).  Close it before the corpus."""
+        ids = np.ascontiguousarray(np.zeros(0, np.uint32) if ids is None else ids, dtype=np.uint32)
+        if n_groups is None:
+            real = ids[ids != GROUP_NONE]
+            n_groups = int(real.max()) + 1 if real.size else 1
+        h = C.c_void_p()
+        _check(lib().frz_groups_create(self._h, ids.ctypes.data if ids.size else None, len(ids), int(n_groups), C.byref(h)))
+        return Groups(h, self)
+
     def __len__(self):
         return self.n
 
@@ -333,6 +354,39 @@ class Boost:
     def close(self):
         if self._h:
             lib().frz_boost_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class Groups:
+    """A group id per row of one resident Corpus (frz_groups), kept by index across corpus edits."""
+
+    def __init__(self, handle, corpus: Corpus):
+        self._h = handle
+        self.corpus = corpus
+
+    def set(self, which, ids) -> "Groups":
+        """group[which[j]] = ids[j] (an id below len(self), or GROUP_NONE); any row below len(corpus), appended ones
+        included, each at most once."""
+        which = np.ascontiguousarray(which, dtype=np.uint32)
+        ids = np.ascontiguousarray(ids, dtype=np.uint32)
+        if len(ids) != len(which):
+            raise ValueError(f"{len(which)} indices need {len(which)} ids, got {len(ids)}")
+        _check(lib().frz_groups_set(self._h, which.ctypes.data if which.size else None, ids.ctypes.data if ids.size else None,
+                                    len(which)))
+        return self
+
+    def __len__(self):
+        return lib().frz_groups_count(self._h)
+
+    def close(self):
+        if self._h:
+            lib().frz_groups_destroy(self._h)
             self._h = None
 
     def __del__(self):
@@ -464,6 +518,31 @@ class Matcher:
         n, total = C.c_uint64(), C.c_uint64()
         _check(lib().frz_match_list_ranked(self._h, corpus._h, subset._h if subset is not None else None, boost._h, k,
                                            out.ctypes.data, C.byref(n), C.byref(total)))
+        return out[: n.value], total.value
+
+    def match_list_collapsed_array(self, corpus: Corpus, groups: Groups, k: Optional[int] = None,
+                                   per_group: Optional[int] = 1, subset: Optional[Subset] = None, boost: Optional[Boost] = None,
+                                   counts: bool = False, out: Optional[np.ndarray] = None):
+        """The rows of the uncollapsed list L (match_list_ranked_array(corpus, boost, subset=subset) with a boost, else
+        match_list_subset_array with a subset, else match_list_array), keeping in L's order the rows in no group and the
+        first per_group rows of each group, truncated to the first k (frz_match_list_collapsed).  Returns (rows, total), or
+        (rows, total, counts) with counts=True: the rows of L per group (uint32, len(groups) entries), before collapsing.
+        k=None returns every kept row; per_group is 1..32, or None for no cap.  `out` (optional) needs room for
+        min(k, len(corpus), len(subset)) rows."""
+        k = _U64_MAX if k is None else int(k)
+        per_group = _U64_MAX if per_group is None else int(per_group)
+        need = min(k, corpus.n, len(subset) if subset is not None else corpus.n)
+        if out is None:
+            out = np.empty(max(1, need), dtype=MATCH_DTYPE)
+        elif len(out) < need:
+            raise ValueError(f"out holds {len(out)} matches; this collapsed call needs {need}")
+        cnt = np.zeros(len(groups), dtype=np.uint32) if counts else None
+        n, total = C.c_uint64(), C.c_uint64()
+        _check(lib().frz_match_list_collapsed(self._h, corpus._h, subset._h if subset is not None else None,
+                                              boost._h if boost is not None else None, groups._h, per_group, k, out.ctypes.data,
+                                              C.byref(n), C.byref(total), cnt.ctypes.data if counts else None))
+        if counts:
+            return out[: n.value], total.value, cnt
         return out[: n.value], total.value
 
     def match_list_into_array(self, haystacks, index_offset: int = 0, device: int = 0) -> np.ndarray:

@@ -1,0 +1,97 @@
+// collapse.cu — the per-group count and the rounds of the collapsed call (frz_match_list_collapsed, DESIGN.md §4.12).
+// The row rule is collapse_plan.cuh's; host.cu compacts the kept rows and sorts them.
+#include "collapse_plan.cuh"
+#include "frz_host.h"
+
+namespace {
+
+constexpr int kCollapseBlock = 256;
+constexpr unsigned kFullWarp = 0xffffffffu;
+
+__device__ __forceinline__ uint64_t row_key(const FrzCollapseDev& c, const FrzMatchDev& r) {
+    const int32_t b = c.order == FRZ_COLLAPSE_BY_KEY && r.index < c.n_boost ? (int32_t)c.boost[r.index] : 0;
+    return frz_collapse_key(c.order, c.reversed != 0, r.score, b, r.index);
+}
+
+// The three kernels walk the list warp by warp (row i0 + lane, i0 warp-uniform), so every lane of a warp reaches the warp
+// intrinsics together; lanes past the list's end hold no group.
+
+// counts[group] += the list's rows in it; taken[i] = 0.  A warp adds once per distinct group among its lanes, so a group
+// holding every row costs one atomic per warp.
+__global__ void __launch_bounds__(kCollapseBlock) k_collapse_count(FrzCollapseDev c, const FrzMatchDev* __restrict__ list,
+                                                                  const unsigned long long* __restrict__ n_ptr) {
+    const unsigned long long n = *n_ptr;
+    const uint32_t lane = threadIdx.x & 31;
+    const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+    for (uint64_t i0 = (uint64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31u); i0 < n; i0 += stride) {
+        const uint64_t i = i0 + lane;
+        uint32_t g = kFrzGroupNone;
+        if (i < n) {
+            g = frz_collapse_group(c.ids, c.n_ids, list[i].index);
+            c.taken[i] = 0;
+        }
+        const uint32_t peers = __match_any_sync(kFullWarp, g);
+        if (g != kFrzGroupNone && lane == (uint32_t)__ffs(peers) - 1) atomicAdd(&c.counts[g], (uint32_t)__popc(peers));
+    }
+}
+
+// One round, first half: best[group] = the largest entry among the group's contenders.  A warp whose lanes all contend for
+// one group reduces in registers and makes one atomic; an atomic that cannot raise the entry is skipped.
+__global__ void __launch_bounds__(kCollapseBlock) k_collapse_max(FrzCollapseDev c, const FrzMatchDev* __restrict__ list,
+                                                                const unsigned long long* __restrict__ n_ptr) {
+    const unsigned long long n = *n_ptr;
+    const uint32_t lane = threadIdx.x & 31;
+    const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+    for (uint64_t i0 = (uint64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31u); i0 < n; i0 += stride) {
+        const uint64_t i = i0 + lane;
+        uint32_t g = kFrzGroupNone;
+        unsigned long long e = 0;
+        if (i < n) {
+            const FrzMatchDev r = list[i];
+            const uint32_t rg = frz_collapse_group(c.ids, c.n_ids, r.index);
+            if (rg != kFrzGroupNone && frz_collapse_contends(rg, c.counts[rg], c.per_group, c.taken[i] != 0)) {
+                g = rg;
+                e = frz_collapse_entry(row_key(c, r));
+            }
+        }
+        const uint32_t peers = __match_any_sync(kFullWarp, g);
+        if (g != kFrzGroupNone && peers == kFullWarp) {   // warp-uniform: every lane contends for g
+#pragma unroll
+            for (int d = 16; d >= 1; d >>= 1) e = max(e, __shfl_xor_sync(kFullWarp, e, d));
+            if (lane == 0 && e > __ldcg(&c.best[g])) atomicMax(&c.best[g], e);
+        } else if (g != kFrzGroupNone && e > __ldcg(&c.best[g])) {
+            atomicMax(&c.best[g], e);
+        }
+    }
+}
+
+// One round, second half: the contender whose entry is the max is taken, and resets the entry for the next round.
+__global__ void __launch_bounds__(kCollapseBlock) k_collapse_take(FrzCollapseDev c, const FrzMatchDev* __restrict__ list,
+                                                                 const unsigned long long* __restrict__ n_ptr) {
+    const unsigned long long n = *n_ptr;
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+        const FrzMatchDev r = list[i];
+        const uint32_t g = frz_collapse_group(c.ids, c.n_ids, r.index);
+        if (g == kFrzGroupNone || !frz_collapse_contends(g, c.counts[g], c.per_group, c.taken[i] != 0)) continue;
+        if (frz_collapse_entry(row_key(c, r)) == __ldcg(&c.best[g])) {
+            c.taken[i] = 1;
+            c.best[g] = 0;
+        }
+    }
+}
+
+}  // namespace
+
+frz_status frz_launch_collapse(const FrzCollapseDev& c, const FrzMatchDev* list, const unsigned long long* n_ptr, uint64_t n_cap,
+                               uint64_t n_groups, uint32_t rounds, cudaStream_t stream, FrzLaunchStats* st) {
+    FRZ_CUDA_TRY(cudaMemsetAsync(c.counts, 0, n_groups * sizeof(uint32_t), stream));
+    const int grid = grid_for(n_cap, kCollapseBlock);
+    k_collapse_count<<<grid, kCollapseBlock, 0, stream>>>(c, list, n_ptr);
+    for (uint32_t r = 0; r < rounds; r++) {
+        k_collapse_max<<<grid, kCollapseBlock, 0, stream>>>(c, list, n_ptr);
+        k_collapse_take<<<grid, kCollapseBlock, 0, stream>>>(c, list, n_ptr);
+    }
+    st->launches += 1 + 2 * (uint64_t)rounds;
+    FRZ_CUDA_TRY(cudaGetLastError());
+    return FRZ_OK;
+}

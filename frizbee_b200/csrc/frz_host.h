@@ -271,6 +271,9 @@ struct FrzWorkspace {
     FrzDevArray<uint16_t> unicode_scratch;  // unicode.cu: per-thread row state of the per-scalar Smith-Waterman
     FrzDevArray<uint32_t> subset_meta;      // [n_tiles * 1024] slot metadata of a subset call: non-members are unused slots
     FrzDevArray<FrzMatchDev> subset_list;   // [2 * members] list-form subset call: member records, then the live ones compacted
+    FrzDevArray<uint32_t> collapse_counts;  // [n_groups] collapsed call: the list's rows per group
+    FrzDevArray<unsigned long long> collapse_best;  // [n_groups] its round table, all zero between calls
+    FrzDevArray<uint8_t> collapse_taken;    // [corpus length] its rows taken in a round
     FrzEvent ev[4];                         // call start, scan done, scoring done, call end
     bool ev_rec[4] = {false, false, false, false};  // recorded during the current call
 };
@@ -383,6 +386,24 @@ struct FrzBatchScope {
 // records on the device (a sub-batch with a scoped or ranked query).
 frz_status frz_launch_batch_top(const FrzBatchDev& b, const FrzBatchScope* scopes, uint32_t nq, uint32_t k, FrzMatchDev* rows,
                                 unsigned long long* totals, cudaStream_t stream, FrzLaunchStats* st);
+
+// The groups of a collapsed call on the device (frz_match_list_collapsed, host.cu; the rule is collapse_plan.cuh's).
+struct FrzCollapseDev {
+    const uint32_t* ids;         // group of index i < n_ids (frz_groups); indices past it are in no group
+    const int16_t* boost;        // FRZ_COLLAPSE_BY_KEY: boost[index] for index < n_boost, 0 past it
+    uint32_t* counts;            // [n_groups] rows of the list per group
+    unsigned long long* best;    // [n_groups] a round's max entry (frz_collapse_entry); zero between rounds and calls
+    uint8_t* taken;              // [list rows] taken in a round
+    uint64_t n_ids;
+    uint32_t n_boost;
+    uint32_t per_group;          // 1..32 (0xFFFFFFFF: no cap, every count fits)
+    uint8_t order;               // FrzCollapseOrder
+    uint8_t reversed;            // 1: the *_DESC strategies
+};
+// collapse.cu: counts = zero, then the count pass over the list (its length at *n_ptr, at most n_cap rows), then `rounds`
+// rounds (a max pass and a take pass each).  c.best must be zero on entry; it is zero again when the rounds have run.
+frz_status frz_launch_collapse(const FrzCollapseDev& c, const FrzMatchDev* list, const unsigned long long* n_ptr, uint64_t n_cap,
+                               uint64_t n_groups, uint32_t rounds, cudaStream_t stream, FrzLaunchStats* st);
 
 // k-way merge of per-shard runs (merge.cu) with caller-owned scratch — one per concurrent user (parallel.cu: one per rank)
 #define FRZ_MERGE_MAX_RUNS 64

@@ -20,6 +20,7 @@
 #include <mutex>
 
 #include "batch_plan.cuh"
+#include "collapse_plan.cuh"
 #include "frz_device.cuh"
 #include "frz_host.h"
 #include "unicode_needle.h"
@@ -916,6 +917,15 @@ struct LiveMember {
         return slot_in_use(slot_meta, slot_of, idx);
     }
 };
+// a collapsed call's list: retain the rows of C (collapse_plan.cuh), after the rounds
+struct CollapseKeep {
+    FrzCollapseDev c;
+    const FrzMatchDev* list;
+    __device__ bool operator()(uint64_t i) const {
+        const uint32_t g = frz_collapse_group(c.ids, c.n_ids, list[i].index);
+        return frz_collapse_keep(g, g == kFrzGroupNone ? 0u : c.counts[g], c.per_group, c.taken[i] != 0);
+    }
+};
 constexpr int kCompactBlock = 1024;
 // keep[i] = rule(i) for the n rows, and the kept rows of each block → block_count
 template <class Rule>
@@ -1328,13 +1338,61 @@ struct Ranking {
     uint32_t max_boost = 0;           // >= every boost value (0 when none is positive): the key bound is score bound + this
 };
 
+// The groups of a collapsed call (frz_match_list_collapsed): of the list, only the rows of C (collapse_plan.cuh) are sorted
+// and returned, and the list's rows per group are left in ws.collapse_counts.
+struct Collapse {
+    const uint32_t* ids = nullptr;    // group of index i < n_ids, on the corpus's device
+    uint64_t n_ids = 0;
+    uint64_t n_groups = 0;
+    uint64_t per_group = 0;           // 1..kFrzCollapseMaxPerGroup, or UINT64_MAX: no cap (only the counts)
+};
+
+// The collapsed call's steps between the list and its sort (DESIGN.md §4.12): the count pass, per_group rounds, and the
+// stable compaction of the kept rows into the other list buffer (*d_list then points there, and ws.counters->total holds
+// |C|).  order: what the rows' order keys rank by.  The list's length is read back first (a survivor-list overflow
+// returns kRetryOverflow there): the passes and the compaction then cover the list, not the corpus.
+frz_status collapse_list(frz_matcher* m, const FrzCorpusStorage& cs, const Collapse& col, uint8_t order, bool reversed,
+                         const Ranking* rank, FrzMatchDev** d_list, cudaStream_t stream, FrzLaunchStats* st) {
+    FrzWorkspace& ws = m->ws;
+    FRZ_TRY(read_counters(m, stream));
+    const uint64_t n_list = ws.h_counters.get()->total;
+    const uint64_t n_cap = std::max<uint64_t>(cs.n, 1);
+    FRZ_TRY(ws.collapse_counts.reserve(col.n_groups));
+    if (ws.collapse_best.cap() < col.n_groups) {   // a new table starts zero; the rounds leave it zero
+        FRZ_TRY(ws.collapse_best.reserve(col.n_groups));
+        FRZ_CUDA_TRY(cudaMemsetAsync(ws.collapse_best.get(), 0, col.n_groups * sizeof(unsigned long long), stream));
+    }
+    FRZ_TRY(ws.collapse_taken.reserve(n_cap));
+    const bool capped = col.per_group != UINT64_MAX;
+    FrzCollapseDev c;
+    c.ids = col.ids;
+    c.n_ids = col.n_ids;
+    c.boost = rank ? rank->boost : nullptr;
+    c.n_boost = rank ? rank->n : 0;
+    c.counts = ws.collapse_counts.get();
+    c.best = ws.collapse_best.get();
+    c.taken = ws.collapse_taken.get();
+    c.per_group = capped ? (uint32_t)col.per_group : 0xFFFFFFFFu;
+    c.order = order;
+    c.reversed = reversed;
+    const unsigned long long* n_ptr = &ws.counters.get()->total;
+    FRZ_TRY(frz_launch_collapse(c, *d_list, n_ptr, std::max<uint64_t>(n_list, 1), col.n_groups, capped ? c.per_group : 0, stream, st));
+    if (!capped || n_list == 0) return FRZ_OK;
+    FrzMatchDev* kept = *d_list == ws.matches_a.get() ? ws.matches_b.get() : ws.matches_a.get();
+    FRZ_TRY(retain_rows(m, CollapseKeep{c, *d_list}, *d_list, n_list, kept, stream, st));
+    *d_list = kept;
+    return FRZ_OK;
+}
+
 // `final_out` (optional, device, >= corpus length): where the final list must land.  `limit` (top-K calls): only the first
 // `limit` positions of the final list are written (the sort's last scatter and the final copy drop the rest); the count in
 // ws.counters->total stays the full match count.  scope: as in match_into_device.  rank (optional): sort by the ranking's
-// key instead, under every strategy and for the empty matcher too (the strategy's direction only orders ties).
+// key instead, under every strategy and for the empty matcher too (the strategy's direction only orders ties).  col
+// (optional, host calls only: final_out == nullptr): collapse the list before its sort (collapse_list).
 frz_status match_list_device(frz_matcher* m, const FrzCorpusStorage& cs, uint32_t index_offset, uint8_t sort,
                              FrzMatchDev** d_result, cudaStream_t stream, FrzLaunchStats* st, FrzMatchDev* final_out = nullptr,
-                             uint32_t limit = kFrzNoLimit, const SubsetScope& scope = SubsetScope(), const Ranking* rank = nullptr) {
+                             uint32_t limit = kFrzNoLimit, const SubsetScope& scope = SubsetScope(), const Ranking* rank = nullptr,
+                             const Collapse* col = nullptr) {
     FrzWorkspace& ws = m->ws;
     const bool reversed = sort == FRZ_SORT_INDEX_DESC || sort == FRZ_SORT_SCORE_THEN_INDEX_DESC;
     const bool by_score = sort == FRZ_SORT_SCORE_THEN_INDEX_ASC || sort == FRZ_SORT_SCORE_THEN_INDEX_DESC;
@@ -1342,9 +1400,14 @@ frz_status match_list_device(frz_matcher* m, const FrzCorpusStorage& cs, uint32_
     reset_call_state(m);
     FrzMatchDev* d_list = nullptr;
     uint32_t bound = 0;
-    FrzScoreHist hist;   // the fused histogram counts scores, so a ranked sort never asks for it
+    // the fused histogram counts the scores of every row of the list, so a ranked or collapsed sort never asks for it
+    FrzScoreHist hist;
     FRZ_TRY(match_into_device(m, cs, index_offset, reversed, &d_list, &bound, stream, st, will_sort ? nullptr : final_out,
-                              will_sort && !rank ? &hist : nullptr, scope));
+                              will_sort && !rank && !col ? &hist : nullptr, scope));
+    if (col) {
+        const uint8_t order = rank ? FRZ_COLLAPSE_BY_KEY : will_sort ? FRZ_COLLAPSE_BY_SCORE : FRZ_COLLAPSE_BY_INDEX;
+        FRZ_TRY(collapse_list(m, cs, *col, order, reversed, rank, &d_list, stream, st));
+    }
     // `!self.patterns.is_empty() && sort.is_by_score()` (src/matcher/mod.rs:218)
     if (will_sort) {
         if (rank) bound = (uint32_t)std::min<uint64_t>((uint64_t)bound + rank->max_boost, 0xFFFF);   // the key bound
@@ -1411,13 +1474,15 @@ frz_status copy_out(frz_matcher* m, FrzMatchDev* d_list, uint64_t limit, frz_mat
 
 // Matcher::match_list (into, from index_offset, in `sort` order) → host, truncated to its first `limit` rows (top-K calls:
 // the same pipeline with a limit on the final scatter and copy; UINT64_MAX for the whole list).  scope: the rows of a subset
-// call (match_into_device).  rank: a ranked call (match_list_device).
+// call (match_into_device).  rank: a ranked call, col: a collapsed call (match_list_device); group_counts (optional, host,
+// col->n_groups entries) receives the list's rows per group.
 frz_status match_list_host(frz_matcher* m, const frz_corpus* corpus, uint32_t index_offset, uint8_t sort, uint64_t limit,
                            const SubsetScope& scope, frz_match* out, uint64_t cap, uint64_t* n_out, uint64_t* n_total,
-                           const Ranking* rank = nullptr) {
+                           const Ranking* rank = nullptr, const Collapse* col = nullptr, uint32_t* group_counts = nullptr) {
     if (scope.none) {
         if (n_out) *n_out = 0;
         if (n_total) *n_total = 0;
+        if (col && group_counts) memset(group_counts, 0, col->n_groups * sizeof(uint32_t));
         return FRZ_OK;
     }
     cudaStream_t stream = nullptr;
@@ -1426,12 +1491,17 @@ frz_status match_list_host(frz_matcher* m, const frz_corpus* corpus, uint32_t in
     const uint32_t dev_limit = (uint32_t)std::min<uint64_t>(limit, kFrzNoLimit);   // a list never holds more than 2^32 - 1 matches
     frz_status s = FRZ_OK;
     for (int attempt = 0; attempt < 2; attempt++) {
-        s = match_list_device(m, corpus->st, index_offset, sort, &d_list, stream, &st, nullptr, dev_limit, scope, rank);
+        s = match_list_device(m, corpus->st, index_offset, sort, &d_list, stream, &st, nullptr, dev_limit, scope, rank, col);
         if (s == FRZ_OK) s = copy_out(m, d_list, limit, out, cap, n_out, n_total, stream);
         if (s != kRetryOverflow) break;
         FRZ_TRY(ensure_workspace(m, corpus->st, std::max<uint64_t>(corpus->st.n, 1)));  // worst-case lists, then once more
     }
     if (s == kRetryOverflow) s = frz_fail(FRZ_ERR_CUDA, "survivor list overflow persisted");
+    if (s == FRZ_OK && col && group_counts) {
+        FRZ_CUDA_TRY(cudaMemcpyAsync(group_counts, m->ws.collapse_counts.get(), col->n_groups * sizeof(uint32_t), cudaMemcpyDeviceToHost,
+                                     stream));
+        FRZ_CUDA_TRY(cudaStreamSynchronize(stream));
+    }
     collect_timings(m, st);
     return s;
 }
@@ -1796,6 +1866,111 @@ extern "C" frz_status frz_match_list_ranked(frz_matcher* m, const frz_corpus* co
     if (s) FRZ_TRY(subset_scope(m, corpus, *s, nullptr, &scope));
     const Ranking rank = ranking_of(*b);
     return match_list_host(m, corpus, 0, m->config.sort, k, scope, out, k, n_out, n_total, &rank);
+}
+
+// ---------------------------------------------------------------------------------- collapsed calls
+// A group id per index of one corpus, on its device.  Indices at and past `ids.cap()` are in no group.
+struct frz_groups {
+    const frz_corpus* corpus;
+    FrzDevArray<uint32_t> ids;
+    uint64_t n_groups;
+};
+
+namespace {
+__global__ void k_groups_scatter(const uint2* __restrict__ set, uint64_t n, uint32_t* __restrict__ ids) {
+    for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x)
+        ids[set[j].x] = set[j].y;
+}
+
+// every id is below n_groups or FRZ_GROUP_NONE
+frz_status check_group_ids(const uint32_t* ids, uint64_t n, uint64_t n_groups) {
+    for (uint64_t j = 0; j < n; j++)
+        if (ids[j] != FRZ_GROUP_NONE && ids[j] >= n_groups)
+            return frz_fail(FRZ_ERR_INVALID_ARG, "group id %u is not below n_groups = %llu", ids[j], (unsigned long long)n_groups);
+    return FRZ_OK;
+}
+
+// g->ids grows to `n` entries, the old ids kept and the new ones FRZ_GROUP_NONE (FrzDevArray drops its contents when it grows)
+frz_status grow_groups(frz_groups* g, uint64_t n) {
+    if (g->ids.cap() >= n) return FRZ_OK;
+    FrzDevArray<uint32_t> grown;
+    FRZ_TRY(grown.reserve(n));
+    FRZ_CUDA_TRY(cudaMemset(grown.get(), 0xFF, n * sizeof(uint32_t)));
+    if (g->ids.cap())
+        FRZ_CUDA_TRY(cudaMemcpy(grown.get(), g->ids.get(), g->ids.cap() * sizeof(uint32_t), cudaMemcpyDeviceToDevice));
+    g->ids = std::move(grown);
+    return FRZ_OK;
+}
+}  // namespace
+
+extern "C" frz_status frz_groups_create(const frz_corpus* c, const uint32_t* ids, uint64_t n, uint64_t n_groups, frz_groups** out) {
+    if (!c || !out || (n && !ids)) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    if (n > c->st.n)
+        return frz_fail(FRZ_ERR_INVALID_ARG, "%llu group ids for a corpus of %llu haystacks", (unsigned long long)n,
+                        (unsigned long long)c->st.n);
+    if (n_groups == 0 || n_groups > FRZ_GROUP_NONE)
+        return frz_fail(FRZ_ERR_INVALID_ARG, "n_groups = %llu is not in 1 .. 2^32 - 1", (unsigned long long)n_groups);
+    FRZ_TRY(check_group_ids(ids, n, n_groups));
+    auto g = std::make_unique<frz_groups>();
+    g->corpus = c;
+    g->n_groups = n_groups;
+    if (n) {
+        FRZ_TRY(frz_ensure_device(c->st.device));
+        FRZ_TRY(g->ids.reserve(n));
+        FRZ_CUDA_TRY(cudaMemcpy(g->ids.get(), ids, n * sizeof(uint32_t), cudaMemcpyHostToDevice));
+    }
+    *out = g.release();
+    return FRZ_OK;
+}
+
+extern "C" frz_status frz_groups_set(frz_groups* g, const uint32_t* which, const uint32_t* ids, uint64_t n) {
+    if (!g || (n && (!which || !ids))) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    if (n == 0) return FRZ_OK;
+    FRZ_TRY(check_indices(g->corpus, which, n));
+    FRZ_TRY(check_group_ids(ids, n, g->n_groups));
+    std::vector<uint32_t> sorted(which, which + n);
+    std::sort(sorted.begin(), sorted.end());
+    for (uint64_t j = 1; j < n; j++)
+        if (sorted[j] == sorted[j - 1]) return frz_fail(FRZ_ERR_INVALID_ARG, "index %u is set twice", sorted[j]);
+    std::vector<uint2> set(n);
+    for (uint64_t j = 0; j < n; j++) set[j] = make_uint2(which[j], ids[j]);
+    FRZ_TRY(frz_ensure_device(g->corpus->st.device));
+    if (sorted.back() >= g->ids.cap()) FRZ_TRY(grow_groups(g, g->corpus->st.n));
+    FrzDevArray<uint2> d_set;   // (index, id) pairs: one copy, one scatter
+    FRZ_TRY(d_set.reserve(n));
+    FRZ_CUDA_TRY(cudaMemcpy(d_set.get(), set.data(), n * sizeof(uint2), cudaMemcpyHostToDevice));
+    k_groups_scatter<<<grid_for(n, 256), 256>>>(d_set.get(), n, g->ids.get());
+    FRZ_CUDA_TRY(cudaGetLastError());
+    FRZ_CUDA_TRY(cudaStreamSynchronize(nullptr));
+    return FRZ_OK;
+}
+
+extern "C" uint64_t frz_groups_count(const frz_groups* g) { return g ? g->n_groups : 0; }
+extern "C" void frz_groups_destroy(frz_groups* g) { delete g; }
+
+extern "C" frz_status frz_match_list_collapsed(frz_matcher* m, const frz_corpus* corpus, const frz_subset* s, const frz_boost* b,
+                                               const frz_groups* g, uint64_t per_group, uint64_t k, frz_match* out, uint64_t* n_out,
+                                               uint64_t* n_total, uint32_t* group_counts) {
+    if (!m || !corpus || !g) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    if (per_group == 0) return frz_fail(FRZ_ERR_INVALID_ARG, "per_group = 0");
+    if (per_group > kFrzCollapseMaxPerGroup && per_group != UINT64_MAX)
+        return frz_fail(FRZ_ERR_UNSUPPORTED, "per_group = %llu: at most %llu rows per group, or UINT64_MAX for no cap",
+                        (unsigned long long)per_group, (unsigned long long)kFrzCollapseMaxPerGroup);
+    if (!out && k > 0) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
+    if (g->corpus != corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "the groups were made on another corpus");
+    if (b && b->corpus != corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "the boost was made on another corpus");
+    if (s && s->corpus != corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "the subset was made on another corpus");
+    FRZ_TRY(frz_ensure_device(corpus->st.device));
+    SubsetScope scope;
+    if (s) FRZ_TRY(subset_scope(m, corpus, *s, nullptr, &scope));
+    Ranking rank;
+    if (b) rank = ranking_of(*b);
+    Collapse col;
+    col.ids = g->ids.get();
+    col.n_ids = g->ids.cap();
+    col.n_groups = g->n_groups;
+    col.per_group = per_group;
+    return match_list_host(m, corpus, 0, m->config.sort, k, scope, out, k, n_out, n_total, b ? &rank : nullptr, &col, group_counts);
 }
 
 // ---------------------------------------------------------------------------------- batched top-K: entry points

@@ -357,6 +357,44 @@ FRZ_API void frz_boost_destroy(frz_boost* b);
 FRZ_API frz_status frz_match_list_ranked(frz_matcher* m, const frz_corpus* c, const frz_subset* s, const frz_boost* b,
                                          uint64_t k, frz_match* out, uint64_t* n_out, uint64_t* n_total);
 
+/* ------------------------------------------------ collapsed calls: groups
+ *
+ * Rows that belong together (every execution of one command in a shell history, every hit of one file in a live grep,
+ * every item of one section of a launcher) collapsed to their best rows on the device, with a match count per group.  The
+ * reference has no such method: its caller de-duplicates or buckets Matcher::match_list's output itself
+ * (src/matcher/mod.rs:212-222), which here means fetching the whole list.
+ *
+ * A group handle gives each corpus index a group id below n_groups, or FRZ_GROUP_NONE.  It follows frz_boost's rules: it
+ * belongs to the corpus it was made on (another corpus is FRZ_ERR_INVALID_ARG, and it must be destroyed before that
+ * corpus), calls only read it, so several matchers may share one, and ids are kept by index across corpus edits: a
+ * removed row stops matching, a replaced row keeps its group, and rows appended after frz_groups_create are in no group
+ * until frz_groups_set gives them one. */
+#define FRZ_GROUP_NONE 0xFFFFFFFFu
+typedef struct frz_groups frz_groups;
+/* ids[i] is the group of index i for i < n; every other index is in no group.  n > frz_corpus_len(c), n_groups outside
+ * 1 .. 2^32 - 1, an id >= n_groups other than FRZ_GROUP_NONE, or NULL ids with n > 0 is FRZ_ERR_INVALID_ARG. */
+FRZ_API frz_status frz_groups_create(const frz_corpus* c, const uint32_t* ids, uint64_t n, uint64_t n_groups, frz_groups** out);
+/* group[which[j]] = ids[j] for j < n.  An index >= frz_corpus_len(c) at the time of the call (rows appended since creation
+ * may be set), a duplicate index, an id >= n_groups other than FRZ_GROUP_NONE, or NULL arrays with n > 0 is
+ * FRZ_ERR_INVALID_ARG; every argument is checked before anything changes.  n == 0 does nothing.  Synchronous; it must not
+ * run concurrently with a call reading g. */
+FRZ_API frz_status frz_groups_set(frz_groups* g, const uint32_t* which, const uint32_t* ids, uint64_t n);
+FRZ_API uint64_t frz_groups_count(const frz_groups* g);   /* n_groups (0 for NULL) */
+FRZ_API void frz_groups_destroy(frz_groups* g);
+/* Let L be the list frz_match_list_ranked(m, c, s, b, UINT64_MAX) returns when b is given, else frz_match_list_subset(m,
+ * c, s) when s is given, else frz_match_list(m, c).  Let C be the rows of L, in L's order, that are in no group or that
+ * have fewer than per_group earlier rows of L in their group.  The call writes C[0 : min(k, |C|)] to `out`, bit for bit,
+ * their number to *n_out and |C| to *n_total (may be NULL).  group_counts (may be NULL) is a host array of n_groups
+ * entries: entry j receives the rows of L in group j, counted before collapsing.
+ * per_group: 1 .. 32, or UINT64_MAX for no cap (C = L: the uncollapsed call plus the counts).  0 is FRZ_ERR_INVALID_ARG,
+ * any other value FRZ_ERR_UNSUPPORTED.  The other rules are frz_match_list_ranked's: k = 0 only counts, k = UINT64_MAX
+ * returns all of C, the call never returns FRZ_ERR_CAPACITY, and a NULL out with k > 0, a NULL matcher, corpus or groups,
+ * or a subset, boost or groups handle of another corpus is FRZ_ERR_INVALID_ARG, checked before any device work.
+ * Blocking. */
+FRZ_API frz_status frz_match_list_collapsed(frz_matcher* m, const frz_corpus* c, const frz_subset* s, const frz_boost* b,
+                                            const frz_groups* g, uint64_t per_group, uint64_t k, frz_match* out,
+                                            uint64_t* n_out, uint64_t* n_total, uint32_t* group_counts);
+
 /* frz_match_list_batch_top (above) where each query may have its own subset and boost, in one call: a service whose users
  * each search their own rows (a subset) ranked by a prior (a boost).  The reference has no such method (see the subset
  * and ranked calls above).  For every j < q, out[j*k .. j*k + n_out[j]), n_out[j] and n_total[j] are bit for bit what the
