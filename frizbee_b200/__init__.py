@@ -95,6 +95,7 @@ def lib():
     L.frz_match_list_top.argtypes = [vp, vp, u64, vp, C.POINTER(u64), C.POINTER(u64)]
     L.frz_match_list_batch_top.argtypes = [vp, u64, vp, u64, vp, vp, vp]
     L.frz_match_list_batch.argtypes = [vp, u64, vp, vp, vp, u64, vp, vp, vp]
+    L.frz_match_list_batch_collapsed.argtypes = [vp, u64, vp, vp, vp, vp, vp, u64, vp, vp, vp, vp]
     L.frz_debug_batch_limits.argtypes = [u64, u64]
     L.frz_debug_batch_limits.restype = None
     L.frz_debug_batch_last.argtypes = [vp]
@@ -614,28 +615,57 @@ def match_list_batch_top(matchers, corpus: Corpus, k: int) -> Tuple[np.ndarray, 
     return out, n_out.astype(np.int64), n_total.astype(np.int64)
 
 
+def _handles(xs, q: int, what: str):
+    """One handle (or NULL) per query of a batched call, or NULL for xs = None."""
+    if xs is None:
+        return None
+    xs = list(xs)
+    if len(xs) != q:
+        raise ValueError(f"{q} matchers need {q} {what}, got {len(xs)}")
+    return (C.c_void_p * max(q, 1))(*[x._h.value if x is not None else None for x in xs])
+
+
 def match_list_batch(matchers, corpus: Corpus, k: int, subsets=None, boosts=None) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
     """frz_match_list_batch: match_list_batch_top where query j may have its own subset and boost.  subsets / boosts: None,
     or one Subset / Boost / None per matcher.  Query j's rows are those of matcher j's match_list_ranked_array(corpus,
     boosts[j], k, subsets[j]) when it has a boost, else of match_list_subset_top_array(corpus, subsets[j], k) when it has
     a subset, else of match_list_top_array(corpus, k).  Returns the (q, k) rows, n_out and n_total as match_list_batch_top."""
     q, k = len(matchers), int(k)
-
-    def handles(xs, what):
-        if xs is None:
-            return None
-        xs = list(xs)
-        if len(xs) != q:
-            raise ValueError(f"{q} matchers need {q} {what}, got {len(xs)}")
-        return (C.c_void_p * max(q, 1))(*[x._h.value if x is not None else None for x in xs])
-
-    hs, hb = handles(subsets, "subsets"), handles(boosts, "boosts")
+    hs, hb = _handles(subsets, q, "subsets"), _handles(boosts, q, "boosts")
     ms = (C.c_void_p * max(q, 1))(*[m._h.value for m in matchers])
     out = np.zeros((q, k), dtype=MATCH_DTYPE)
     n_out = np.zeros(q, dtype=np.uint64)
     n_total = np.zeros(q, dtype=np.uint64)
     _check(lib().frz_match_list_batch(ms, q, corpus._h, hs, hb, k, out.ctypes.data if out.size else None, n_out.ctypes.data,
                                       n_total.ctypes.data))
+    return out, n_out.astype(np.int64), n_total.astype(np.int64)
+
+
+def match_list_batch_collapsed(matchers, corpus: Corpus, k: int, groups, per_group=1, subsets=None, boosts=None, counts: bool = False):
+    """frz_match_list_batch_collapsed: match_list_batch where query j may also collapse its rows by groups[j].  groups: one
+    Groups or None per matcher; per_group: an int (1..32), None (no cap), or one such value per matcher.  Query j's rows are
+    those of matcher j's match_list_collapsed_array(corpus, groups[j], k, per_group[j], subsets[j], boosts[j]) when it has
+    groups, else those of match_list_batch.  Returns the (q, k) rows, n_out and n_total as match_list_batch_top, and with
+    counts=True also a list of each query's rows per group (uint32, len(groups[j]) entries; None for a query without groups)."""
+    q, k = len(matchers), int(k)
+    groups = list(groups) if groups is not None else [None] * q
+    hs, hb, hg = _handles(subsets, q, "subsets"), _handles(boosts, q, "boosts"), _handles(groups, q, "groups")
+    if per_group is None or isinstance(per_group, (int, np.integer)):
+        per_group = [per_group] * q
+    per_group = list(per_group)
+    if len(per_group) != q:
+        raise ValueError(f"{q} matchers need {q} per_group values, got {len(per_group)}")
+    pg = np.array([_U64_MAX if p is None else int(p) for p in per_group] or [1], dtype=np.uint64)
+    cnt = [np.zeros(len(g), dtype=np.uint32) if counts and g is not None else None for g in groups]
+    hc = (C.c_void_p * max(q, 1))(*[c.ctypes.data if c is not None else None for c in cnt]) if counts else None
+    ms = (C.c_void_p * max(q, 1))(*[m._h.value for m in matchers])
+    out = np.zeros((q, k), dtype=MATCH_DTYPE)
+    n_out = np.zeros(q, dtype=np.uint64)
+    n_total = np.zeros(q, dtype=np.uint64)
+    _check(lib().frz_match_list_batch_collapsed(ms, q, corpus._h, hs, hb, hg, pg.ctypes.data, k, out.ctypes.data if out.size else None,
+                                                n_out.ctypes.data, n_total.ctypes.data, hc))
+    if counts:
+        return out, n_out.astype(np.int64), n_total.astype(np.int64), cnt
     return out, n_out.astype(np.int64), n_total.astype(np.int64)
 
 

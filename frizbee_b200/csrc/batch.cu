@@ -3,6 +3,7 @@
 // batch_plan.cuh's (shared with the CPU tests).
 #include "frz_device.cuh"
 
+#include "batch_collapse_plan.cuh"
 #include "batch_plan.cuh"
 #include "frz_host.h"
 
@@ -65,6 +66,42 @@ struct ScopedKey {
         const uint32_t i = m->index;
         return frz_batch_ranked_value(m->score, i < q.n_boost ? (int32_t)__ldg(q.boost + i) : 0);
     }
+};
+
+// CollapsedKey (frz_match_list_batch_collapsed): a grouped query's rows are the members of its subset that its collapse
+// keeps (frz_collapse_keep, after the rounds of collapse.cu); its total is their number, |C|.  Value and order are
+// ScopedKey's.  A query without groups is answered as under ScopedKey.
+struct CollapsedKey {
+    static constexpr bool kScoped = true;
+    FrzBatchTables t;
+    const FrzMatchDev* lists;
+    uint64_t list_stride;
+    struct Query {
+        FrzBatchScope s;
+        FrzBatchCollapse c;
+        const uint32_t* counts;    // the query's count table
+        const uint8_t* taken;      // [list row]
+        const FrzMatchDev* list;
+        bool scoped;               // its rows are a filter of its list: a subset, or groups with a cap
+    };
+    __device__ __forceinline__ Query query(uint32_t j) const {
+        Query q;
+        q.s = t.scopes[j];
+        q.c = t.cols[j];
+        q.counts = t.counts + q.c.table;
+        q.taken = t.taken + j * list_stride;
+        q.list = lists + j * list_stride;
+        q.scoped = q.s.scoped || (q.c.ids && frz_batch_collapse_rounds(q.c.per_group) > 0);
+        return q;
+    }
+    __device__ __forceinline__ static bool by_value(const Query& q, bool by_score) { return ScopedKey::by_value(q.s, by_score); }
+    __device__ __forceinline__ static bool member(const Query& q, const FrzMatchDev* m) {
+        if (!ScopedKey::member(q.s, m)) return false;
+        if (!q.c.ids) return true;
+        const uint32_t g = frz_collapse_group(q.c.ids, q.c.n_ids, m->index);
+        return frz_collapse_keep(g, g == kFrzGroupNone ? 0u : q.counts[g], q.c.per_group, q.taken[m - q.list] != 0);
+    }
+    __device__ __forceinline__ static uint32_t value(const Query& q, const FrzMatchDev* m) { return ScopedKey::value(q.s, m); }
 };
 
 template <class Key>
@@ -178,5 +215,15 @@ frz_status frz_launch_batch_top(const FrzBatchDev& b, const FrzBatchScope* scope
     else k_batch_top<<<nq, kTopThreads, 0, stream>>>(b, k, rows, totals, ScoreKey());
     FRZ_CUDA_TRY(cudaGetLastError());
     if (st) st->launches++;
+    return FRZ_OK;
+}
+
+frz_status frz_launch_batch_top_collapsed(const FrzBatchDev& b, const FrzBatchTables& t, uint32_t nq, uint32_t k, FrzMatchDev* rows,
+                                          unsigned long long* totals, cudaStream_t stream, FrzLaunchStats* st) {
+    if (nq == 0) return FRZ_OK;
+    if (k > kFrzBatchMaxK) return frz_fail(FRZ_ERR_INVALID_ARG, "batched top-K serves k <= %u", kFrzBatchMaxK);
+    k_batch_top<<<nq, kTopThreads, 0, stream>>>(b, k, rows, totals, CollapsedKey{t, b.lists, b.list_stride});
+    FRZ_CUDA_TRY(cudaGetLastError());
+    st->launches++;
     return FRZ_OK;
 }

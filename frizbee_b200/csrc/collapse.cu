@@ -1,5 +1,7 @@
-// collapse.cu — the per-group count and the rounds of the collapsed call (frz_match_list_collapsed, DESIGN.md §4.12).
-// The row rule is collapse_plan.cuh's; host.cu compacts the kept rows and sorts them.
+// collapse.cu — the per-group count and the rounds of the collapsed call (frz_match_list_collapsed, DESIGN.md §4.12), and
+// of the batched collapsed call's sub-batches (frz_match_list_batch_collapsed, §4.11).  The row rule is collapse_plan.cuh's;
+// host.cu compacts the kept rows and sorts them, or k_batch_top<CollapsedKey> (batch.cu) cuts them per query.
+#include "batch_collapse_plan.cuh"
 #include "collapse_plan.cuh"
 #include "frz_host.h"
 
@@ -80,7 +82,118 @@ __global__ void __launch_bounds__(kCollapseBlock) k_collapse_take(FrzCollapseDev
     }
 }
 
+// The batched passes (frz_match_list_batch_collapsed): block row blockIdx.y walks query j = blockIdx.y's list as the kernels
+// above walk one list, over the rows that are members of its subset (non-members are in the list: the subset is applied
+// late), with its own tables.  A query without groups, with its device error set, or past its rounds leaves at once.
+struct BatchQuery {
+    FrzBatchCollapse c;
+    FrzBatchScope s;
+    const FrzMatchDev* list;
+    uint8_t* taken;
+    unsigned long long n;
+    uint8_t reversed;
+};
+__device__ __forceinline__ bool batch_query(const FrzBatchDev& b, const FrzBatchTables& t, uint32_t j, BatchQuery* q) {
+    q->c = t.cols[j];
+    if (!q->c.ids || b.ctr[j].error) return false;
+    q->s = t.scopes[j];
+    q->list = b.lists + j * b.list_stride;
+    q->taken = t.taken + j * b.list_stride;
+    q->n = b.ctr[j].total;
+    q->reversed = b.reversed[j];
+    return true;
+}
+// the group of a list row, kFrzGroupNone for a row in no group or not a member of the query's subset
+__device__ __forceinline__ uint32_t batch_group(const BatchQuery& q, uint32_t index) {
+    if (q.s.scoped && !frz_batch_member(q.s.bits, q.s.n_bits, index)) return kFrzGroupNone;
+    return frz_collapse_group(q.c.ids, q.c.n_ids, index);
+}
+__device__ __forceinline__ uint64_t batch_entry(const BatchQuery& q, const FrzMatchDev& r) {
+    const int32_t b = q.c.order == FRZ_COLLAPSE_BY_KEY && r.index < q.s.n_boost ? (int32_t)q.s.boost[r.index] : 0;
+    return frz_collapse_entry(frz_collapse_key(q.c.order, q.reversed != 0, r.score, b, r.index));
+}
+
+__global__ void __launch_bounds__(kCollapseBlock) k_batch_collapse_count(const FrzBatchDev b, const FrzBatchTables t) {
+    BatchQuery q;
+    if (!batch_query(b, t, blockIdx.y, &q)) return;
+    uint32_t* counts = t.counts + q.c.table;
+    const uint32_t lane = threadIdx.x & 31;
+    const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+    for (uint64_t i0 = (uint64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31u); i0 < q.n; i0 += stride) {
+        const uint64_t i = i0 + lane;
+        uint32_t g = kFrzGroupNone;
+        if (i < q.n) {
+            g = batch_group(q, q.list[i].index);
+            q.taken[i] = 0;
+        }
+        const uint32_t peers = __match_any_sync(kFullWarp, g);
+        if (g != kFrzGroupNone && lane == (uint32_t)__ffs(peers) - 1) atomicAdd(&counts[g], (uint32_t)__popc(peers));
+    }
+}
+
+__global__ void __launch_bounds__(kCollapseBlock) k_batch_collapse_max(const FrzBatchDev b, const FrzBatchTables t, uint32_t round) {
+    BatchQuery q;
+    if (!batch_query(b, t, blockIdx.y, &q) || !frz_batch_collapse_in_round(q.c.per_group, round)) return;
+    const uint32_t* counts = t.counts + q.c.table;
+    unsigned long long* best = t.best + q.c.table;
+    const uint32_t lane = threadIdx.x & 31;
+    const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+    for (uint64_t i0 = (uint64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31u); i0 < q.n; i0 += stride) {
+        const uint64_t i = i0 + lane;
+        uint32_t g = kFrzGroupNone;
+        unsigned long long e = 0;
+        if (i < q.n) {
+            const FrzMatchDev r = q.list[i];
+            const uint32_t rg = batch_group(q, r.index);
+            if (rg != kFrzGroupNone && frz_collapse_contends(rg, counts[rg], q.c.per_group, q.taken[i] != 0)) {
+                g = rg;
+                e = batch_entry(q, r);
+            }
+        }
+        const uint32_t peers = __match_any_sync(kFullWarp, g);
+        if (g != kFrzGroupNone && peers == kFullWarp) {   // warp-uniform: every lane contends for g
+#pragma unroll
+            for (int d = 16; d >= 1; d >>= 1) e = max(e, __shfl_xor_sync(kFullWarp, e, d));
+            if (lane == 0 && e > __ldcg(&best[g])) atomicMax(&best[g], e);
+        } else if (g != kFrzGroupNone && e > __ldcg(&best[g])) {
+            atomicMax(&best[g], e);
+        }
+    }
+}
+
+__global__ void __launch_bounds__(kCollapseBlock) k_batch_collapse_take(const FrzBatchDev b, const FrzBatchTables t, uint32_t round) {
+    BatchQuery q;
+    if (!batch_query(b, t, blockIdx.y, &q) || !frz_batch_collapse_in_round(q.c.per_group, round)) return;
+    const uint32_t* counts = t.counts + q.c.table;
+    unsigned long long* best = t.best + q.c.table;
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < q.n; i += (uint64_t)gridDim.x * blockDim.x) {
+        const FrzMatchDev r = q.list[i];
+        const uint32_t g = batch_group(q, r.index);
+        if (g == kFrzGroupNone || !frz_collapse_contends(g, counts[g], q.c.per_group, q.taken[i] != 0)) continue;
+        if (batch_entry(q, r) == __ldcg(&best[g])) {
+            q.taken[i] = 1;
+            best[g] = 0;
+        }
+    }
+}
+
 }  // namespace
+
+frz_status frz_launch_batch_collapse(const FrzBatchDev& b, const FrzBatchTables& t, uint32_t nq, uint32_t rounds, cudaStream_t stream,
+                                     FrzLaunchStats* st) {
+    if (nq == 0) return FRZ_OK;
+    // as many blocks in all as the single-query passes over one list of list_stride rows
+    const uint32_t gx = (uint32_t)std::max<uint64_t>(1, (uint64_t)grid_for(b.list_stride, kCollapseBlock) / nq);
+    const dim3 grid(gx, nq);
+    k_batch_collapse_count<<<grid, kCollapseBlock, 0, stream>>>(b, t);
+    for (uint32_t r = 0; r < rounds; r++) {
+        k_batch_collapse_max<<<grid, kCollapseBlock, 0, stream>>>(b, t, r);
+        k_batch_collapse_take<<<grid, kCollapseBlock, 0, stream>>>(b, t, r);
+    }
+    st->launches += 1 + 2 * (uint64_t)rounds;
+    FRZ_CUDA_TRY(cudaGetLastError());
+    return FRZ_OK;
+}
 
 frz_status frz_launch_collapse(const FrzCollapseDev& c, const FrzMatchDev* list, const unsigned long long* n_ptr, uint64_t n_cap,
                                uint64_t n_groups, uint32_t rounds, cudaStream_t stream, FrzLaunchStats* st) {

@@ -387,6 +387,23 @@ struct FrzBatchScope {
 frz_status frz_launch_batch_top(const FrzBatchDev& b, const FrzBatchScope* scopes, uint32_t nq, uint32_t k, FrzMatchDev* rows,
                                 unsigned long long* totals, cudaStream_t stream, FrzLaunchStats* st);
 
+// The groups of a sub-batch of frz_match_list_batch_collapsed (host.cu; the per-query arithmetic is batch_collapse_plan.cuh's).
+struct FrzBatchCollapse;
+struct FrzBatchTables {
+    const FrzBatchCollapse* cols;   // [j] the query's groups (ids == nullptr: none), on the device
+    const FrzBatchScope* scopes;    // [j] its subset and boost
+    uint32_t* counts;               // [slot][n_groups_max] the list's member rows per group
+    unsigned long long* best;       // [slot][n_groups_max] a round's max entry; zero between rounds and calls
+    uint8_t* taken;                 // [j][list_stride] the list's rows taken in a round
+};
+// collapse.cu: the count pass over every grouped query's list (counts must be zero), then `rounds` rounds of a max pass and
+// a take pass, each one launch over the nq queries.  A query with its sticky device error set is skipped.
+frz_status frz_launch_batch_collapse(const FrzBatchDev& b, const FrzBatchTables& t, uint32_t nq, uint32_t rounds, cudaStream_t stream,
+                                     FrzLaunchStats* st);
+// batch.cu: frz_launch_batch_top whose rows are, for a grouped query, the kept rows of its collapse (k_batch_top<CollapsedKey>)
+frz_status frz_launch_batch_top_collapsed(const FrzBatchDev& b, const FrzBatchTables& t, uint32_t nq, uint32_t k, FrzMatchDev* rows,
+                                          unsigned long long* totals, cudaStream_t stream, FrzLaunchStats* st);
+
 // The groups of a collapsed call on the device (frz_match_list_collapsed, host.cu; the rule is collapse_plan.cuh's).
 struct FrzCollapseDev {
     const uint32_t* ids;         // group of index i < n_ids (frz_groups); indices past it are in no group

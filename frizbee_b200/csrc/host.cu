@@ -19,6 +19,7 @@
 #include <memory>
 #include <mutex>
 
+#include "batch_collapse_plan.cuh"
 #include "batch_plan.cuh"
 #include "collapse_plan.cuh"
 #include "frz_device.cuh"
@@ -1523,15 +1524,18 @@ extern "C" frz_status frz_match_list_top(frz_matcher* m, const frz_corpus* corpu
 }
 
 // ---------------------------------------------------------------------------------- batched top-K
-// frz_match_list_batch and frz_match_list_batch_top (DESIGN.md §4.11).  Queries of the batched class run in sub-batches
-// whose every stage is one launch (per kernel variant present) over all of the sub-batch's queries, with one upload, one
-// read-back and one synchronise per sub-batch; every other query, and every query of an overflowed sub-batch, runs its
-// single-query call's pipeline (frz_match_list_top, _subset_top or _ranked).  The entry points follow the ranked calls.
+// frz_match_list_batch_collapsed, frz_match_list_batch and frz_match_list_batch_top (DESIGN.md §4.11).  Queries of the
+// batched class run in sub-batches whose every stage is one launch (per kernel variant present) over all of the
+// sub-batch's queries, with one upload, one read-back and one synchronise per sub-batch; every other query, and every
+// query of an overflowed sub-batch, runs its single-query call's pipeline (frz_match_list_top, _subset_top, _ranked or
+// _collapsed).  The entry points follow the collapsed calls.
 namespace {
 
 // Device scratch of one sub-batch's queries, in one allocation: a fixed budget, so a batch call holds the same scratch for
 // every q (its size depends on the corpus: larger corpora get smaller sub-batches, and a corpus whose queries do not fit two
-// to a sub-batch is answered query by query).
+// to a sub-batch is answered query by query).  A call with grouped queries adds each query's group tables at the largest
+// n_groups among its batched grouped queries (batch_collapse_plan.cuh), so its sub-batches hold fewer queries; a grouped
+// query whose tables alone do not fit two to a sub-batch (more than about 22 M groups) runs frz_match_list_collapsed.
 constexpr uint64_t kBatchScratchBytes = 512ull << 20;
 // Where the batched path is faster than a loop of frz_match_list_top (tools/bench_batch.py on an H100 SXM, DESIGN.md §4.11):
 // at 100 k rows from 64 queries on, not at 8 queries (the call's fixed costs); at 1 M rows for max_typos = 0 queries only
@@ -1540,6 +1544,10 @@ constexpr uint64_t kBatchScratchBytes = 512ull << 20;
 constexpr uint64_t kBatchMaxRows = 1ull << 18;
 constexpr uint64_t kBatchMaxRowsNoTypo = 1ull << 21;   // FRZ_T_0 queries
 constexpr uint64_t kBatchMinQueries = 32;
+// A grouped query that wants the counts of more groups than this runs frz_match_list_collapsed: its counts' read-back
+// through the sub-batch's staging then costs more than the loop saves (tools/bench_batch_collapsed.py on an H100 SXM,
+// DESIGN.md §4.11: ahead of the loop with 100 k groups, behind it with 1 M).
+constexpr uint64_t kBatchMaxCountedGroups = 1ull << 18;
 // The limits in force (frz_debug_batch_limits changes them for tests and tools/bench_batch.py) and what the calling
 // thread's last batch call did (frz_debug_batch_last).
 std::atomic<uint64_t> g_batch_max_rows{kBatchMaxRows};
@@ -1548,9 +1556,10 @@ thread_local uint64_t g_batch_last[4] = {0, 0, 0, 0};   // batched queries, over
 
 struct BatchLayout {
     uint64_t nt = 0, stride = 0, cap = 0, k = 0;
-    uint64_t off[14] = {};   // byte offsets of the arrays below, in this order
+    uint64_t groups = 0;     // entries of each query slot's group tables (0: no query of the call has groups)
+    uint64_t off[18] = {};   // byte offsets of the arrays below, in this order
     uint64_t bytes = 0;
-    enum { CTR, BITMAP, PREFIX, TCOUNT, TBASE, SURV, LISTS, PATS, REV, BYSC, SCOPE, TOTALS, ROWS, END };
+    enum { CTR, BITMAP, PREFIX, TCOUNT, TBASE, SURV, LISTS, BEST, TAKEN, PATS, REV, BYSC, SCOPE, COLS, TOTALS, ROWS, COUNTS, END };
     // queries per sub-batch for this corpus and k (0: fewer than two fit the budget)
     static uint64_t per_query(const FrzCorpusStorage& cs, uint64_t k, uint64_t cap) {
         const uint64_t nt = cs.n_tiles;
@@ -1558,15 +1567,18 @@ struct BatchLayout {
                FRZ_N_CLASSES * cap * sizeof(FrzSurvivor) + std::max<uint64_t>(cs.n, 1) * sizeof(FrzMatchDev) + sizeof(FrzPatternDev) + 2 +
                sizeof(FrzBatchScope) + sizeof(unsigned long long) + k * sizeof(FrzMatchDev) + 13 * 256 / 2;
     }
-    BatchLayout(const FrzCorpusStorage& cs, uint64_t k_, uint64_t cap_, uint64_t qs) : nt(cs.n_tiles), stride(std::max<uint64_t>(cs.n, 1)), cap(cap_), k(k_) {
+    BatchLayout(const FrzCorpusStorage& cs, uint64_t k_, uint64_t cap_, uint64_t qs, uint64_t groups_ = 0)
+        : nt(cs.n_tiles), stride(std::max<uint64_t>(cs.n, 1)), cap(cap_), k(k_), groups(groups_) {
+        const uint64_t g = groups ? qs : 0;   // the group arrays exist only in a call with grouped queries
         const uint64_t size[END] = {qs * sizeof(FrzCounters), qs * nt * 32 * sizeof(uint32_t), qs * nt * 32 * sizeof(uint16_t),
                                     qs * nt * sizeof(uint32_t), qs * nt * sizeof(uint64_t), qs * FRZ_N_CLASSES * cap * sizeof(FrzSurvivor),
-                                    qs * stride * sizeof(FrzMatchDev), qs * sizeof(FrzPatternDev), qs, qs,
-                                    qs * sizeof(FrzBatchScope), qs * sizeof(unsigned long long), qs * k * sizeof(FrzMatchDev)};
+                                    qs * stride * sizeof(FrzMatchDev), g * groups * sizeof(unsigned long long), g * stride,
+                                    qs * sizeof(FrzPatternDev), qs, qs, qs * sizeof(FrzBatchScope), g * sizeof(FrzBatchCollapse),
+                                    qs * sizeof(unsigned long long), qs * k * sizeof(FrzMatchDev), g * groups * sizeof(uint32_t)};
         uint64_t at = 0;
         for (int i = 0; i < END; i++) {
-            // CTR..BITMAP are zeroed as one range, PATS..SCOPE uploaded as one, TOTALS..ROWS read back as one
-            const bool packed = i == BITMAP || i == REV || i == BYSC || i == SCOPE || i == ROWS;
+            // CTR..BITMAP are zeroed as one range, PATS..COLS uploaded as one, TOTALS..COUNTS read back as one
+            const bool packed = i == BITMAP || i == REV || i == BYSC || i == SCOPE || i == COLS || i == ROWS || i == COUNTS;
             if (!packed) at = (at + 255) & ~255ull;
             else at = (at + 7) & ~7ull;
             off[i] = at;
@@ -1598,24 +1610,33 @@ bool batch_selected(const frz_matcher* m, const FrzCorpusStorage& cs) {
     return cs.n <= limit;
 }
 
+// The groups of a call's queries, indexed as ms (frz_match_list_batch_collapsed).
+struct BatchGroups {
+    const FrzBatchCollapse* cols = nullptr;   // [j] ids == nullptr: no groups (cols == nullptr: no query of the call has any)
+    const uint64_t* n_groups = nullptr;       // [j]
+    uint32_t* const* counts = nullptr;        // [j] the caller's count array, or nullptr (counts == nullptr: none)
+};
+
 // One sub-batch: queries which[0..ns) of ms, all of the batched class.  scopes: nullptr when no query of the call is scoped
-// or ranked, else every query's subset and boost (indexed as ms).  *overflow: a survivor list overflowed, nothing was
-// written to the results (the caller runs the queries one by one).
-frz_status batch_run(frz_matcher* const* ms, const FrzBatchScope* scopes, const uint64_t* which, uint32_t ns, const frz_corpus* c,
-                     uint64_t k, const BatchLayout& L, uint8_t* d, frz_match* out, uint64_t* n_out, uint64_t* n_total,
-                     bool* overflow, FrzLaunchStats& st) {
+// or ranked, else every query's subset and boost (indexed as ms).  gr: the call's groups (L.groups > 0 when it has any).
+// *overflow: a survivor list overflowed, nothing was written to the results (the caller runs the queries one by one).
+frz_status batch_run(frz_matcher* const* ms, const FrzBatchScope* scopes, const BatchGroups& gr, const uint64_t* which, uint32_t ns,
+                     const frz_corpus* c, uint64_t k, const BatchLayout& L, uint8_t* d, frz_match* out, uint64_t* n_out,
+                     uint64_t* n_total, bool* overflow, FrzLaunchStats& st) {
     const FrzCorpusStorage& cs = c->st;
     cudaStream_t stream = nullptr;
     *overflow = false;
     const uint64_t up = L.off[BatchLayout::TOTALS] - L.off[BatchLayout::PATS];
-    const uint64_t down = L.off[BatchLayout::END] - L.off[BatchLayout::TOTALS];
-    FRZ_TRY(c->batch_stage.reserve(std::max(up, down)));
+    FRZ_TRY(c->batch_stage.reserve(std::max(up, L.off[BatchLayout::END] - L.off[BatchLayout::TOTALS])));
     uint8_t* h = c->batch_stage.get();
     FrzPatternDev* h_pats = reinterpret_cast<FrzPatternDev*>(h);
     uint8_t* h_rev = h + (L.off[BatchLayout::REV] - L.off[BatchLayout::PATS]);
     uint8_t* h_bysc = h + (L.off[BatchLayout::BYSC] - L.off[BatchLayout::PATS]);
     FrzBatchScope* h_scope = reinterpret_cast<FrzBatchScope*>(h + (L.off[BatchLayout::SCOPE] - L.off[BatchLayout::PATS]));
+    FrzBatchCollapse* h_cols = reinterpret_cast<FrzBatchCollapse*>(h + (L.off[BatchLayout::COLS] - L.off[BatchLayout::PATS]));
     bool scoped = false;   // a query of the sub-batch is scoped or ranked: the last stage is k_batch_top<ScopedKey>
+    uint8_t grouped[kFrzBatchMaxSub] = {}, wants[kFrzBatchMaxSub] = {};
+    uint32_t slot[kFrzBatchMaxSub] = {}, n_grouped = 0, rounds = 0;
     for (uint32_t j = 0; j < ns; j++) {
         const frz_matcher* m = ms[which[j]];
         const uint8_t sort = m->config.sort;
@@ -1624,7 +1645,20 @@ frz_status batch_run(frz_matcher* const* ms, const FrzBatchScope* scopes, const 
         h_bysc[j] = sort == FRZ_SORT_SCORE_THEN_INDEX_ASC || sort == FRZ_SORT_SCORE_THEN_INDEX_DESC;
         h_scope[j] = scopes ? scopes[which[j]] : FrzBatchScope();
         scoped |= h_scope[j].scoped || h_scope[j].ranked;
+        if (gr.cols && gr.cols[which[j]].ids) {
+            grouped[j] = 1;
+            wants[j] = gr.counts && gr.counts[which[j]];
+            n_grouped++;
+            rounds = std::max(rounds, frz_batch_collapse_rounds(gr.cols[which[j]].per_group));
+        }
     }
+    // the group tables: a slot per grouped query, those whose counts are read back first
+    const uint32_t n_back = frz_batch_collapse_slots(grouped, wants, ns, slot);
+    for (uint32_t j = 0; j < ns && L.groups; j++) {
+        h_cols[j] = gr.cols[which[j]];
+        h_cols[j].table = frz_batch_collapse_table(slot[j], L.groups);
+    }
+    const uint64_t down = L.off[BatchLayout::COUNTS] + n_back * L.groups * sizeof(uint32_t) - L.off[BatchLayout::TOTALS];
     FrzBatchDev b;
     b.pats = reinterpret_cast<const FrzPatternDev*>(d + L.off[BatchLayout::PATS]);
     b.reversed = d + L.off[BatchLayout::REV];
@@ -1647,12 +1681,25 @@ frz_status batch_run(frz_matcher* const* ms, const FrzBatchScope* scopes, const 
     FRZ_TRY(frz_launch_prefilter_batch(cv, b, h_pats, ns, stream, &st));
     FRZ_TRY(frz_launch_sw_batch(cv, b, h_pats, ns, stream, &st));
     const FrzBatchScope* d_scope = reinterpret_cast<const FrzBatchScope*>(d + L.off[BatchLayout::SCOPE]);
-    FRZ_TRY(frz_launch_batch_top(b, scoped ? d_scope : nullptr, ns, (uint32_t)k, rows, totals, stream, &st));
+    if (n_grouped) {   // the collapse, then the kept rows' cut
+        FrzBatchTables t;
+        t.cols = reinterpret_cast<const FrzBatchCollapse*>(d + L.off[BatchLayout::COLS]);
+        t.scopes = d_scope;
+        t.counts = reinterpret_cast<uint32_t*>(d + L.off[BatchLayout::COUNTS]);
+        t.best = reinterpret_cast<unsigned long long*>(d + L.off[BatchLayout::BEST]);
+        t.taken = d + L.off[BatchLayout::TAKEN];
+        FRZ_CUDA_TRY(cudaMemsetAsync(t.counts, 0, n_grouped * L.groups * sizeof(uint32_t), stream));
+        FRZ_TRY(frz_launch_batch_collapse(b, t, ns, rounds, stream, &st));
+        FRZ_TRY(frz_launch_batch_top_collapsed(b, t, ns, (uint32_t)k, rows, totals, stream, &st));
+    } else {
+        FRZ_TRY(frz_launch_batch_top(b, scoped ? d_scope : nullptr, ns, (uint32_t)k, rows, totals, stream, &st));
+    }
     // the staged patterns are not read again: the read-back may reuse the staging
     FRZ_CUDA_TRY(cudaMemcpyAsync(h, totals, down, cudaMemcpyDeviceToHost, stream));
     FRZ_CUDA_TRY(cudaStreamSynchronize(stream));
     const unsigned long long* h_totals = reinterpret_cast<const unsigned long long*>(h);
     const frz_match* h_rows = reinterpret_cast<const frz_match*>(h + (L.off[BatchLayout::ROWS] - L.off[BatchLayout::TOTALS]));
+    const uint32_t* h_counts = reinterpret_cast<const uint32_t*>(h + (L.off[BatchLayout::COUNTS] - L.off[BatchLayout::TOTALS]));
     for (uint32_t j = 0; j < ns; j++)
         if (h_totals[j] == kFrzBatchOverflow) { *overflow = true; return FRZ_OK; }
     for (uint32_t j = 0; j < ns; j++) {
@@ -1660,6 +1707,7 @@ frz_status batch_run(frz_matcher* const* ms, const FrzBatchScope* scopes, const 
         n_out[q] = n;
         if (n_total) n_total[q] = h_totals[j];
         if (n) memcpy(out + q * k, h_rows + frz_batch_row0(j, k), n * sizeof(frz_match));
+        if (wants[j]) memcpy(gr.counts[q], h_counts + frz_batch_collapse_table(slot[j], L.groups), gr.n_groups[q] * sizeof(uint32_t));
     }
     return FRZ_OK;
 }
@@ -1901,6 +1949,15 @@ frz_status grow_groups(frz_groups* g, uint64_t n) {
     g->ids = std::move(grown);
     return FRZ_OK;
 }
+
+Collapse collapse_of(const frz_groups& g, uint64_t per_group) {
+    Collapse col;
+    col.ids = g.ids.get();
+    col.n_ids = g.ids.cap();
+    col.n_groups = g.n_groups;
+    col.per_group = per_group;
+    return col;
+}
 }  // namespace
 
 extern "C" frz_status frz_groups_create(const frz_corpus* c, const uint32_t* ids, uint64_t n, uint64_t n_groups, frz_groups** out) {
@@ -1965,39 +2022,52 @@ extern "C" frz_status frz_match_list_collapsed(frz_matcher* m, const frz_corpus*
     if (s) FRZ_TRY(subset_scope(m, corpus, *s, nullptr, &scope));
     Ranking rank;
     if (b) rank = ranking_of(*b);
-    Collapse col;
-    col.ids = g->ids.get();
-    col.n_ids = g->ids.cap();
-    col.n_groups = g->n_groups;
-    col.per_group = per_group;
+    const Collapse col = collapse_of(*g, per_group);
     return match_list_host(m, corpus, 0, m->config.sort, k, scope, out, k, n_out, n_total, b ? &rank : nullptr, &col, group_counts);
 }
 
 // ---------------------------------------------------------------------------------- batched top-K: entry points
 namespace {
-// query j's single-query call: frz_match_list_ranked with a boost, else frz_match_list_subset_top with a subset, else
-// frz_match_list_top
-frz_status batch_single(frz_matcher* m, const frz_corpus* c, const frz_subset* s, const frz_boost* b, uint64_t k, frz_match* out,
-                        uint64_t* n_out, uint64_t* n_total) {
+// query j's single-query call: frz_match_list_collapsed with groups, else frz_match_list_ranked with a boost, else
+// frz_match_list_subset_top with a subset, else frz_match_list_top
+frz_status batch_single(frz_matcher* m, const frz_corpus* c, const frz_subset* s, const frz_boost* b, const frz_groups* g,
+                        uint64_t per_group, uint64_t k, frz_match* out, uint64_t* n_out, uint64_t* n_total, uint32_t* group_counts) {
     SubsetScope scope;
     if (s) FRZ_TRY(subset_scope(m, c, *s, nullptr, &scope));
-    if (!b) return match_list_host(m, c, 0, m->config.sort, k, scope, out, k, n_out, n_total);
-    const Ranking rank = ranking_of(*b);
-    return match_list_host(m, c, 0, m->config.sort, k, scope, out, k, n_out, n_total, &rank);
+    Ranking rank;
+    if (b) rank = ranking_of(*b);
+    if (!g) return match_list_host(m, c, 0, m->config.sort, k, scope, out, k, n_out, n_total, b ? &rank : nullptr);
+    const Collapse col = collapse_of(*g, per_group);
+    return match_list_host(m, c, 0, m->config.sort, k, scope, out, k, n_out, n_total, b ? &rank : nullptr, &col, group_counts);
 }
 }  // namespace
 
 extern "C" frz_status frz_match_list_batch(frz_matcher* const* ms, uint64_t q, const frz_corpus* corpus,
                                            const frz_subset* const* subsets, const frz_boost* const* boosts, uint64_t k,
                                            frz_match* out, uint64_t* n_out, uint64_t* n_total) {
+    return frz_match_list_batch_collapsed(ms, q, corpus, subsets, boosts, nullptr, nullptr, k, out, n_out, n_total, nullptr);
+}
+
+extern "C" frz_status frz_match_list_batch_collapsed(frz_matcher* const* ms, uint64_t q, const frz_corpus* corpus,
+                                                     const frz_subset* const* subsets, const frz_boost* const* boosts,
+                                                     const frz_groups* const* groups, const uint64_t* per_group, uint64_t k,
+                                                     frz_match* out, uint64_t* n_out, uint64_t* n_total, uint32_t* const* group_counts) {
     if (!ms || !corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
     for (uint64_t j = 0; j < q; j++)
         if (!ms[j]) return frz_fail(FRZ_ERR_INVALID_ARG, "null matcher at %llu", (unsigned long long)j);
+    for (uint64_t j = 0; per_group && j < q; j++) {
+        if (per_group[j] == 0) return frz_fail(FRZ_ERR_INVALID_ARG, "per_group = 0 at %llu", (unsigned long long)j);
+        if (per_group[j] > kFrzCollapseMaxPerGroup && per_group[j] != UINT64_MAX)
+            return frz_fail(FRZ_ERR_UNSUPPORTED, "per_group = %llu at %llu: at most %llu rows per group, or UINT64_MAX for no cap",
+                            (unsigned long long)per_group[j], (unsigned long long)j, (unsigned long long)kFrzCollapseMaxPerGroup);
+    }
     for (uint64_t j = 0; j < q; j++) {
         if (subsets && subsets[j] && subsets[j]->corpus != corpus)
             return frz_fail(FRZ_ERR_INVALID_ARG, "the subset of query %llu was made on another corpus", (unsigned long long)j);
         if (boosts && boosts[j] && boosts[j]->corpus != corpus)
             return frz_fail(FRZ_ERR_INVALID_ARG, "the boost of query %llu was made on another corpus", (unsigned long long)j);
+        if (groups && groups[j] && groups[j]->corpus != corpus)
+            return frz_fail(FRZ_ERR_INVALID_ARG, "the groups of query %llu were made on another corpus", (unsigned long long)j);
     }
     if (q && !n_out) return frz_fail(FRZ_ERR_INVALID_ARG, "null n_out");
     if (k && (q > UINT64_MAX / k || q * k > SIZE_MAX / sizeof(frz_match)))
@@ -2015,17 +2085,30 @@ extern "C" frz_status frz_match_list_batch(frz_matcher* const* ms, uint64_t q, c
     for (uint64_t& v : g_batch_last) v = 0;
     auto subset_of = [&](uint64_t j) { return subsets ? subsets[j] : nullptr; };
     auto boost_of = [&](uint64_t j) { return boosts ? boosts[j] : nullptr; };
+    auto groups_of = [&](uint64_t j) { return groups ? groups[j] : nullptr; };
+    auto per_group_of = [&](uint64_t j) { return per_group ? per_group[j] : 1; };
+    auto counts_of = [&](uint64_t j) { return group_counts ? group_counts[j] : nullptr; };
     auto single = [&](uint64_t j) {
-        return batch_single(ms[j], corpus, subset_of(j), boost_of(j), k, k ? out + j * k : nullptr, &n_out[j],
-                            n_total ? &n_total[j] : nullptr);
+        return batch_single(ms[j], corpus, subset_of(j), boost_of(j), groups_of(j), per_group_of(j), k, k ? out + j * k : nullptr,
+                            &n_out[j], n_total ? &n_total[j] : nullptr, counts_of(j));
     };
     std::vector<uint64_t> batched;
     const uint64_t cap = batch_survivor_cap(cs);
-    const uint64_t fit = k <= kFrzBatchMaxK ? kBatchScratchBytes / BatchLayout::per_query(cs, k, cap) : 0;
+    const uint64_t base = BatchLayout::per_query(cs, k, cap);
+    const uint64_t fit = k <= kFrzBatchMaxK ? kBatchScratchBytes / base : 0;
     const uint64_t qs_max = std::min<uint64_t>(fit, kFrzBatchMaxSub);
+    const uint64_t list_rows = std::max<uint64_t>(cs.n, 1);
+    uint64_t n_groups_max = 0;   // the largest n_groups among the batched grouped queries
     for (uint64_t j = 0; j < q; j++) {
-        if (qs_max >= 2 && batchable(ms[j], cs) && batch_selected(ms[j], cs)) batched.push_back(j);
-        else FRZ_TRY(single(j));
+        const frz_groups* g = groups_of(j);
+        if (qs_max >= 2 && batchable(ms[j], cs) && batch_selected(ms[j], cs) &&
+            (!g || (frz_batch_collapse_fit(kBatchScratchBytes, base, g->n_groups, list_rows) &&
+                    (!counts_of(j) || g->n_groups <= kBatchMaxCountedGroups)))) {
+            batched.push_back(j);
+            if (g) n_groups_max = std::max(n_groups_max, g->n_groups);
+        } else {
+            FRZ_TRY(single(j));
+        }
     }
     if (batched.size() < std::max<uint64_t>(2, g_batch_min_queries.load())) {   // a few queries cost what a loop of single calls costs
         for (uint64_t j : batched) FRZ_TRY(single(j));
@@ -2050,15 +2133,43 @@ extern "C" frz_status frz_match_list_batch(frz_matcher* const* ms, uint64_t q, c
             r.n_boost = (uint32_t)b->values.cap();
         }
     }
-    const uint64_t qs = std::min<uint64_t>(qs_max, batched.size());
-    const BatchLayout L(cs, k, cap, qs);
+    // every query's groups, as the batched collapse reads them (none when no batched query has groups)
+    std::vector<FrzBatchCollapse> cols;
+    std::vector<uint64_t> n_groups;
+    for (uint64_t j : batched) {
+        const frz_groups* g = groups_of(j);
+        if (!g) continue;
+        if (cols.empty()) { cols.resize(q, FrzBatchCollapse()); n_groups.resize(q, 0); }
+        const uint8_t sort = ms[j]->config.sort;
+        FrzBatchCollapse& r = cols[j];
+        r.ids = g->ids.get();
+        r.n_ids = g->ids.cap();
+        r.per_group = per_group_of(j) == UINT64_MAX ? 0xFFFFFFFFu : (uint32_t)per_group_of(j);
+        r.order = boost_of(j) ? FRZ_COLLAPSE_BY_KEY
+                : sort == FRZ_SORT_SCORE_THEN_INDEX_ASC || sort == FRZ_SORT_SCORE_THEN_INDEX_DESC ? FRZ_COLLAPSE_BY_SCORE
+                : FRZ_COLLAPSE_BY_INDEX;
+        n_groups[j] = g->n_groups;
+    }
+    BatchGroups gr;
+    if (!cols.empty()) {
+        gr.cols = cols.data();
+        gr.n_groups = n_groups.data();
+        gr.counts = group_counts;
+    }
+    const uint64_t qs_fit = n_groups_max ? std::min<uint64_t>(frz_batch_collapse_fit(kBatchScratchBytes, base, n_groups_max, list_rows),
+                                                              kFrzBatchMaxSub)
+                                         : qs_max;
+    const uint64_t qs = std::min<uint64_t>(qs_fit, batched.size());
+    const BatchLayout L(cs, k, cap, qs, n_groups_max);
     FrzDevArray<uint8_t> scratch;   // released when the call returns
     FRZ_TRY(scratch.reserve(L.bytes));
+    if (L.groups)   // the round tables start zero, and every sub-batch's rounds leave them zero
+        FRZ_CUDA_TRY(cudaMemsetAsync(scratch.get() + L.off[BatchLayout::BEST], 0, L.off[BatchLayout::TAKEN] - L.off[BatchLayout::BEST]));
     for (uint64_t s = 0; s < batched.size(); s += qs) {
         const uint32_t ns = (uint32_t)std::min<uint64_t>(qs, batched.size() - s);
         bool overflow = false;
         FrzLaunchStats st;
-        FRZ_TRY(batch_run(ms, scopes.empty() ? nullptr : scopes.data(), batched.data() + s, ns, corpus, k, L, scratch.get(), out,
+        FRZ_TRY(batch_run(ms, scopes.empty() ? nullptr : scopes.data(), gr, batched.data() + s, ns, corpus, k, L, scratch.get(), out,
                           n_out, n_total, &overflow, st));
         g_batch_last[overflow ? 1 : 0] += ns;
         g_batch_last[2]++;

@@ -272,14 +272,15 @@ FRZ_API frz_status frz_match_list_top(frz_matcher* m, const frz_corpus* corpus, 
  * after another: correct, but not faster than a loop. */
 FRZ_API frz_status frz_match_list_batch_top(frz_matcher* const* ms, uint64_t q, const frz_corpus* corpus, uint64_t k,
                                             frz_match* out, uint64_t* n_out, uint64_t* n_total);
-/* Test aid: the corpus-size and query-count limits of the batched path of frz_match_list_batch_top and
- * frz_match_list_batch, process-wide (0 restores
+/* Test aid: the corpus-size and query-count limits of the batched path of frz_match_list_batch_top,
+ * frz_match_list_batch and frz_match_list_batch_collapsed, process-wide (0 restores
  * a limit's default: 2^18 rows, 32 queries; max_typos = 0 queries batch up to the larger of max_rows and 2^21 rows;
  * fewer than 2 queries never batch).  Lets tests reach the batched kernels with
  * small batches and tools/bench_batch.py time the batched path on both sides of the defaults.  Not for concurrent use with
  * batch calls. */
 FRZ_API void frz_debug_batch_limits(uint64_t max_rows, uint64_t min_queries);
-/* Test aid: what the calling thread's last frz_match_list_batch_top or frz_match_list_batch did: [0] queries answered by
+/* Test aid: what the calling thread's last frz_match_list_batch_top, frz_match_list_batch or
+ * frz_match_list_batch_collapsed did: [0] queries answered by
  * the batched kernels, [1] queries of sub-batches whose survivor lists overflowed (answered again by their single-query
  * call's pipeline),
  * [2] sub-batches run, [3] kernel launches of the batched path.  All zero after a call that ran no sub-batch. */
@@ -411,6 +412,25 @@ FRZ_API frz_status frz_match_list_collapsed(frz_matcher* m, const frz_corpus* c,
 FRZ_API frz_status frz_match_list_batch(frz_matcher* const* ms, uint64_t q, const frz_corpus* corpus,
                                         const frz_subset* const* subsets, const frz_boost* const* boosts, uint64_t k,
                                         frz_match* out, uint64_t* n_out, uint64_t* n_total);
+
+/* frz_match_list_batch (above) where each query may also collapse its rows by its own groups, in one call: a service that
+ * shows each of its users their distinct commands, their best hits per file or their section sizes.  For every j < q,
+ * out[j*k .. j*k + n_out[j]), n_out[j], n_total[j] and, when given, group_counts[j] are bit for bit what the matching
+ * single-query call returns:
+ *   groups[j] != NULL: frz_match_list_collapsed(ms[j], corpus, subsets[j], boosts[j], groups[j], per_group[j], k, ...,
+ *                      group_counts[j]);
+ *   else:              query j of frz_match_list_batch (ranked, subset-top or top).
+ * groups, subsets, boosts and group_counts may be NULL, meaning every entry is NULL; group_counts[j] (NULL, or a host array
+ * of frz_groups_count(groups[j]) entries) is read only for a query with groups.  per_group may be NULL, meaning 1 for every
+ * query; every entry follows frz_match_list_collapsed's rule (1 .. 32 or UINT64_MAX; 0 is FRZ_ERR_INVALID_ARG, any other
+ * value FRZ_ERR_UNSUPPORTED).  A groups handle made on another corpus is FRZ_ERR_INVALID_ARG.  Every other rule is
+ * frz_match_list_batch's, and every argument is checked before any device work.  A batched-class query with groups runs
+ * the batched kernels, except one whose groups hold more than about 22 M ids, or one that asks for the counts of more
+ * than 2^18 groups: those run the single-query call inside the same call (DESIGN.md §4.11). */
+FRZ_API frz_status frz_match_list_batch_collapsed(frz_matcher* const* ms, uint64_t q, const frz_corpus* corpus,
+                                                  const frz_subset* const* subsets, const frz_boost* const* boosts,
+                                                  const frz_groups* const* groups, const uint64_t* per_group, uint64_t k,
+                                                  frz_match* out, uint64_t* n_out, uint64_t* n_total, uint32_t* const* group_counts);
 
 /* Specialized::match_list / Matcher::match_list_into (src/matcher/algo.rs:17-22,
  * src/matcher/mod.rs:373-392): matches appended in input (index-ascending) order,
