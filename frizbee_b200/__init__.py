@@ -119,6 +119,7 @@ def lib():
     L.frz_groups_destroy.argtypes = [vp]
     L.frz_groups_destroy.restype = None
     L.frz_match_list_collapsed.argtypes = [vp, vp, vp, vp, vp, u64, u64, vp, C.POINTER(u64), C.POINTER(u64), vp]
+    L.frz_match_list_columns.argtypes = [vp, vp, u64, C.c_uint8, vp, vp, vp, u64, u64, vp, C.POINTER(u64), C.POINTER(u64), vp]
     L.frz_match_list_into.argtypes = [vp, vp, u32, vp, u64, C.POINTER(u64)]
     L.frz_match_list_host.argtypes = [vp, vp, vp, u64, C.c_int, vp, u64, C.POINTER(u64)]
     L.frz_match_list_host_arrow.argtypes = [vp, vp, vp, C.c_int, u64, C.c_int, vp, u64, C.POINTER(u64)]
@@ -667,6 +668,44 @@ def match_list_batch_collapsed(matchers, corpus: Corpus, k: int, groups, per_gro
     if counts:
         return out, n_out.astype(np.int64), n_total.astype(np.int64), cnt
     return out, n_out.astype(np.int64), n_total.astype(np.int64)
+
+
+def match_list_columns(matchers, columns, k: Optional[int] = None, sort: SortStrategy = SortStrategy.ScoreThenIndexAsc,
+                       subset: Optional[Subset] = None, boost: Optional[Boost] = None, groups: Optional[Groups] = None,
+                       per_group: Optional[int] = 1, counts: bool = False, out: Optional[np.ndarray] = None):
+    """frz_match_list_columns: rows with several text fields, matcher j searching columns[j] (Corpus objects of one length:
+    row i is haystack i of every column).  A row matches when it matches in every column; its score is the saturating sum
+    of the column scores and its exact flag their OR.  The list is ordered by `sort` (the matchers' own sort settings are
+    not read), ranked by boost when one is given, collapsed by groups when they are given (per_group 1..32, or None for no
+    cap), and truncated to the first k rows.  subset / boost / groups may be handles of any of the columns.  Returns
+    (rows, total), or (rows, total, counts) with counts=True (the list's rows per group, before collapsing).  k=None returns
+    every row; `out` (optional) needs room for min(k, len(columns[0]), len(subset)) rows.  Put the most selective column
+    first: the order changes only the speed."""
+    matchers, columns = list(matchers), list(columns)
+    if len(matchers) != len(columns):
+        raise ValueError(f"{len(matchers)} matchers for {len(columns)} columns")
+    k = _U64_MAX if k is None else int(k)
+    per_group = _U64_MAX if per_group is None else int(per_group)
+    n = columns[0].n if columns else 0
+    need = min(k, n, len(subset) if subset is not None else n)
+    if out is None:
+        out = np.empty(max(1, need), dtype=MATCH_DTYPE)
+    elif len(out) < need:
+        raise ValueError(f"out holds {len(out)} matches; this columns call needs {need}")
+    if counts and groups is None:
+        raise ValueError("counts=True needs groups")
+    cnt = np.zeros(len(groups), dtype=np.uint32) if counts else None
+    q = len(matchers)
+    ms = (C.c_void_p * max(q, 1))(*[m._h.value for m in matchers])
+    cs = (C.c_void_p * max(q, 1))(*[c._h.value for c in columns])
+    n_out, total = C.c_uint64(), C.c_uint64()
+    _check(lib().frz_match_list_columns(ms, cs, q, int(sort), subset._h if subset is not None else None,
+                                        boost._h if boost is not None else None, groups._h if groups is not None else None,
+                                        per_group, k, out.ctypes.data, C.byref(n_out), C.byref(total),
+                                        cnt.ctypes.data if counts else None))
+    if counts:
+        return out[: n_out.value], total.value, cnt
+    return out[: n_out.value], total.value
 
 
 def batch_last() -> dict:

@@ -918,6 +918,23 @@ struct LiveMember {
         return slot_in_use(slot_meta, slot_of, idx);
     }
 };
+// a list of frz_match_list_columns: retain the rows whose slot is in use in each of up to kLiveColumns further columns
+// (the candidate-list kernels read a candidate's slot metadata unchecked, so a row removed in a later column must leave
+// the list before that column is read)
+constexpr int kLiveColumns = 8;
+struct LiveInColumns {
+    const FrzMatchDev* list;
+    uint32_t index_offset;
+    int n;
+    const uint32_t* slot_meta[kLiveColumns];
+    const uint16_t* slot_of[kLiveColumns];
+    __device__ bool operator()(uint64_t i) const {
+        const uint64_t idx = list[i].index - index_offset;
+        for (int c = 0; c < n; c++)
+            if (!slot_in_use(slot_meta[c], slot_of[c], idx)) return false;
+        return true;
+    }
+};
 // a collapsed call's list: retain the rows of C (collapse_plan.cuh), after the rounds
 struct CollapseKeep {
     FrzCollapseDev c;
@@ -1063,12 +1080,13 @@ uint64_t initial_survivor_cap(const FrzCorpusStorage& cs, const FrzPatternDev& d
     return std::min<uint64_t>(std::max<uint64_t>(cs.n / 4, 1 << 16), std::max<uint64_t>(cs.n, 1));
 }
 
-// A long needle's FrzNeedleTab on the workspace's device, uploaded once per compiled pattern set (build_patterns starts a
-// new epoch) and device; nullptr for other needles.
-frz_status needle_table(frz_matcher* m, const Compiled& c, const FrzNeedleTab** out) {
+// A long needle's FrzNeedleTab on `device` (the device of the call's workspace, which is m's own unless m's pattern runs in
+// another matcher's frz_match_list_columns call), uploaded once per compiled pattern set (build_patterns starts a new
+// epoch) and device; nullptr for other needles.
+frz_status needle_table(frz_matcher* m, const Compiled& c, int device, const FrzNeedleTab** out) {
     *out = nullptr;
     if (!c.is_long()) return FRZ_OK;
-    if (!m->ntab.get() || m->ntab.device() != m->ws.device || m->ntab_epoch != m->epoch) {
+    if (!m->ntab.get() || m->ntab.device() != device || m->ntab_epoch != m->epoch) {
         m->ntab.reset();
         m->ntab_epoch = 0;
         size_t k = 0;
@@ -1131,18 +1149,19 @@ frz_status shard_call(frz_matcher* m, uint64_t* d_count, cudaStream_t stream, Bo
 
 // One pattern over the corpus (optionally restricted to a candidate list) → index-ordered matches in d_out (reversed
 // order if `reversed`); the count is left in ws.counters->total (device).  masked_meta (subset calls): slot metadata to
-// read in place of the corpus's own, nullptr = the corpus's.
+// read in place of the corpus's own, nullptr = the corpus's.  owner: the matcher whose pattern c is, when it is not m
+// (frz_match_list_columns runs every column's patterns in ms[0]'s workspace).
 frz_status run_pattern(frz_matcher* m, const FrzCorpusStorage& cs, const Compiled& c, const uint32_t* masked_meta,
                        uint32_t index_offset, bool reversed, FrzMatchDev* d_out, cudaStream_t stream, FrzLaunchStats* st,
                        bool record_events, const FrzMatchDev* cand_list = nullptr, uint64_t n_cand = 0,
-                       const FrzScoreHist& hist = FrzScoreHist()) {
+                       const FrzScoreHist& hist = FrzScoreHist(), frz_matcher* owner = nullptr) {
     FrzWorkspace& ws = m->ws;
     FrzCorpusView cv = cs.view();
     if (masked_meta) cv.slot_meta = masked_meta;
     uint64_t cap = std::max(ws.survivor_cap(), initial_survivor_cap(cs, c.dev));
     FRZ_TRY(ensure_workspace(m, cs, cap));
     const FrzNeedleTab* ntab = nullptr;
-    FRZ_TRY(needle_table(m, c, &ntab));
+    FRZ_TRY(needle_table(owner ? owner : m, c, ws.device, &ntab));
     FRZ_CUDA_TRY(cudaMemsetAsync(ws.counters.get(), 0, sizeof(FrzCounters), stream));
     if (record_events) record_ev(ws, 0, stream);
     if (c.unicode) FRZ_TRY(frz_launch_unicode(cv, c.dev, c.un, c.usc, cand_list, n_cand, index_offset, ws, stream, st));
@@ -1216,6 +1235,116 @@ frz_status copy_scope_list(frz_matcher* m, const SubsetScope& scope, FrzMatchDev
     return set_count(m, scope.n_list, stream);
 }
 
+// One pattern of the multi-pattern loop (match_patterns) and the column it reads.  A matcher's own patterns all read the
+// call's corpus; frz_match_list_columns gives each column's patterns their column.  owner: the matcher the compiled
+// pattern belongs to (its long-needle table).
+struct ColumnPattern {
+    const Compiled* c;
+    frz_matcher* owner;
+    const FrzCorpusStorage* cs;
+};
+
+// The columns of a frz_match_list_columns call, as match_patterns takes them: every column's patterns in column order,
+// the further columns with removed rows, and whether any matcher has a compiled pattern (the score sort's condition).
+struct Columns {
+    std::vector<ColumnPattern> pats;
+    std::vector<const FrzCorpusStorage*> live;
+    bool any_compiled = false;
+};
+
+// CompiledPatterns::Multi (src/matcher/multi.rs:84-152), each pattern over its own column; all columns share one index
+// space and so one tile count.  The base, the first non-negated pattern, is scanned over its column, restricted to scope;
+// every later pattern runs on the surviving candidates against its own column.  Without a base the list starts from every
+// live row (or the scope's members).  cs: the base's column, else the column whose live rows start the list; scope is
+// built against its slot metadata.  live: further columns with removed rows, whose removed rows leave the starting
+// list before any later pattern reads it (LiveInColumns; empty for a matcher's own patterns).  Counts are read back
+// between patterns.  The list lands in ws.matches_a (reversed if final_reversed), its count in ws.counters->total, and
+// *score_bound is the saturating sum of the non-negated patterns' bounds.
+frz_status match_patterns(frz_matcher* m, const std::vector<ColumnPattern>& pats, const FrzCorpusStorage& cs,
+                          const std::vector<const FrzCorpusStorage*>& live, uint32_t index_offset, bool final_reversed,
+                          FrzMatchDev** d_result, uint32_t* score_bound, cudaStream_t stream, FrzLaunchStats* st,
+                          const SubsetScope& scope) {
+    FrzWorkspace& ws = m->ws;
+    const uint32_t* masked_meta = scope.masked_meta;
+    FRZ_TRY(ensure_workspace(m, cs, pats.empty() ? 1 : initial_survivor_cap(cs, pats[0].c->dev)));
+    FRZ_TRY(ensure_multi_buffers(m, cs.n));
+    int base = -1;
+    for (size_t i = 0; i < pats.size(); i++) if (!pats[i].c->negated) { base = (int)i; break; }
+    FrzMatchDev* cand = ws.multi_a.get();
+    FrzMatchDev* spare = ws.multi_b.get();
+    uint64_t nc = 0;
+    uint64_t bound = 0;
+    if (base >= 0) {
+        FRZ_TRY(run_pattern(m, cs, *pats[base].c, masked_meta, index_offset, false, cand, stream, st, true, scope.list, scope.n_list,
+                            FrzScoreHist(), pats[base].owner));
+        FRZ_TRY(read_counters(m, stream));
+        nc = ws.h_counters.get()->total;
+        bound = pats[base].c->score_bound;
+    } else if (scope.list) {
+        FRZ_TRY(copy_scope_list(m, scope, cand, stream));
+        nc = scope.n_list;
+    } else {
+        FRZ_CUDA_TRY(cudaMemsetAsync(ws.counters.get(), 0, sizeof(FrzCounters), stream));
+        FRZ_TRY(fill_all(m, cs, index_offset, cand, spare, stream, st, masked_meta));
+        if (masked_meta) {   // the members in use are counted on the device
+            FRZ_TRY(read_counters(m, stream));
+            nc = ws.h_counters.get()->total;
+        } else nc = cs.n - cs.n_removed;
+    }
+    for (size_t c0 = 0; c0 < live.size() && nc > 0; c0 += kLiveColumns) {
+        LiveInColumns rule{cand, index_offset, (int)std::min<size_t>(kLiveColumns, live.size() - c0), {}, {}};
+        for (int c = 0; c < rule.n; c++) {
+            rule.slot_meta[c] = live[c0 + c]->slot_meta.get();
+            rule.slot_of[c] = live[c0 + c]->slot_of.get();
+        }
+        FRZ_TRY(retain_rows(m, rule, cand, nc, spare, stream, st));
+        FRZ_TRY(read_counters(m, stream));
+        nc = ws.h_counters.get()->total;
+        std::swap(cand, spare);
+    }
+    FRZ_TRY(ensure_retain_buffers(m, cs.n));   // once, for every negated pattern below
+    frz_status status = FRZ_OK;
+    for (size_t pi = 0; pi < pats.size() && status == FRZ_OK; pi++) {
+        if ((int)pi == base || nc == 0) continue;
+        const Compiled& pat = *pats[pi].c;
+        status = [&]() -> frz_status {
+            // evaluate the pattern on the surviving candidates only, against its own column; hits land in ws.matches_a,
+            // index-ordered, with real indices
+            FRZ_TRY(run_pattern(m, *pats[pi].cs, pat, nullptr, index_offset, false, ws.matches_a.get(), stream, st, false, cand, nc,
+                                FrzScoreHist(), pats[pi].owner));
+            FRZ_TRY(read_counters(m, stream));
+            const uint64_t nh = ws.h_counters.get()->total;
+            if (pat.negated) {
+                FRZ_TRY(retain_rows(m, NotHit{cand, ws.matches_a.get(), nh}, cand, nc, spare, stream, st));
+                FRZ_TRY(read_counters(m, stream));
+                nc = ws.h_counters.get()->total;
+                std::swap(cand, spare);
+            } else {
+                k_combine_hits<<<grid_for(nh, 256), 256, 0, stream>>>(cand, nc, ws.matches_a.get(), nh);
+                st->launches++;
+                FRZ_CUDA_TRY(cudaMemcpyAsync(spare, ws.matches_a.get(), nh * sizeof(FrzMatchDev), cudaMemcpyDeviceToDevice, stream));
+                std::swap(cand, spare);
+                nc = nh;
+                bound += pat.score_bound;
+            }
+            return FRZ_OK;
+        }();
+    }
+    FRZ_TRY(status);
+    // publish: count → counters.total, list → matches_a (reversed if asked)
+    FRZ_TRY(set_count(m, nc, stream));
+    if (final_reversed) {
+        k_reverse<<<grid_for(nc, 256), 256, 0, stream>>>(cand, ws.matches_a.get(), &ws.counters.get()->total);
+        st->launches++;
+    } else {
+        FRZ_CUDA_TRY(cudaMemcpyAsync(ws.matches_a.get(), cand, nc * sizeof(FrzMatchDev), cudaMemcpyDeviceToDevice, stream));
+    }
+    FRZ_CUDA_TRY(cudaGetLastError());
+    *d_result = ws.matches_a.get();
+    *score_bound = (uint32_t)std::min<uint64_t>(bound, 0xFFFF);
+    return FRZ_OK;
+}
+
 // match_list_into over all compiled patterns → index-ordered device list; returns pointer + leaves the
 // count in ws.counters->total.  `final_reversed` asks for the list in descending index order.  `score_hist` (optional):
 // the caller will sort the list by score; where the scoring kernels emit the list directly and one sort pass will do,
@@ -1258,70 +1387,11 @@ frz_status match_into_device(frz_matcher* m, const FrzCorpusStorage& cs, uint32_
         *score_bound = pats[0].score_bound;
         return FRZ_OK;
     }
-    // CompiledPatterns::Multi (src/matcher/multi.rs:84-152).  Counts are read back between patterns.
-    FRZ_TRY(ensure_workspace(m, cs, initial_survivor_cap(cs, pats[0].dev)));
-    FRZ_TRY(ensure_multi_buffers(m, cs.n));
-    int base = -1;
-    for (size_t i = 0; i < pats.size(); i++) if (!pats[i].negated) { base = (int)i; break; }
-    FrzMatchDev* cand = ws.multi_a.get();
-    FrzMatchDev* spare = ws.multi_b.get();
-    uint64_t nc = 0;
-    uint64_t bound = 0;
-    if (base >= 0) {
-        FRZ_TRY(run_pattern(m, cs, pats[base], masked_meta, index_offset, false, cand, stream, st, true, scope.list, scope.n_list));
-        FRZ_TRY(read_counters(m, stream));
-        nc = ws.h_counters.get()->total;
-        bound = pats[base].score_bound;
-    } else if (scope.list) {
-        FRZ_TRY(copy_scope_list(m, scope, cand, stream));
-        nc = scope.n_list;
-    } else {
-        FRZ_CUDA_TRY(cudaMemsetAsync(ws.counters.get(), 0, sizeof(FrzCounters), stream));
-        FRZ_TRY(fill_all(m, cs, index_offset, cand, spare, stream, st, masked_meta));
-        if (masked_meta) {   // the members in use are counted on the device
-            FRZ_TRY(read_counters(m, stream));
-            nc = ws.h_counters.get()->total;
-        } else nc = cs.n - cs.n_removed;
-    }
-    FRZ_TRY(ensure_retain_buffers(m, cs.n));   // once, for every negated pattern below
-    frz_status status = FRZ_OK;
-    for (size_t pi = 0; pi < pats.size() && status == FRZ_OK; pi++) {
-        if ((int)pi == base || nc == 0) continue;
-        status = [&]() -> frz_status {
-            // evaluate the pattern on the surviving candidates only; hits land in ws.matches_a, index-ordered,
-            // with real indices
-            FRZ_TRY(run_pattern(m, cs, pats[pi], nullptr, index_offset, false, ws.matches_a.get(), stream, st, false, cand, nc));
-            FRZ_TRY(read_counters(m, stream));
-            const uint64_t nh = ws.h_counters.get()->total;
-            if (pats[pi].negated) {
-                FRZ_TRY(retain_rows(m, NotHit{cand, ws.matches_a.get(), nh}, cand, nc, spare, stream, st));
-                FRZ_TRY(read_counters(m, stream));
-                nc = ws.h_counters.get()->total;
-                std::swap(cand, spare);
-            } else {
-                k_combine_hits<<<grid_for(nh, 256), 256, 0, stream>>>(cand, nc, ws.matches_a.get(), nh);
-                st->launches++;
-                FRZ_CUDA_TRY(cudaMemcpyAsync(spare, ws.matches_a.get(), nh * sizeof(FrzMatchDev), cudaMemcpyDeviceToDevice, stream));
-                std::swap(cand, spare);
-                nc = nh;
-                bound += pats[pi].score_bound;
-            }
-            return FRZ_OK;
-        }();
-    }
-    FRZ_TRY(status);
-    // publish: count → counters.total, list → matches_a (reversed if asked)
-    FRZ_TRY(set_count(m, nc, stream));
-    if (final_reversed) {
-        k_reverse<<<grid_for(nc, 256), 256, 0, stream>>>(cand, ws.matches_a.get(), &ws.counters.get()->total);
-        st->launches++;
-    } else {
-        FRZ_CUDA_TRY(cudaMemcpyAsync(ws.matches_a.get(), cand, nc * sizeof(FrzMatchDev), cudaMemcpyDeviceToDevice, stream));
-    }
-    FRZ_CUDA_TRY(cudaGetLastError());
-    *d_result = ws.matches_a.get();
-    *score_bound = (uint32_t)std::min<uint64_t>(bound, 0xFFFF);
-    return FRZ_OK;
+    // CompiledPatterns::Multi: every pattern over this corpus
+    std::vector<ColumnPattern> cols;
+    cols.reserve(pats.size());
+    for (const Compiled& c : pats) cols.push_back(ColumnPattern{&c, m, &cs});
+    return match_patterns(m, cols, cs, {}, index_offset, final_reversed, d_result, score_bound, stream, st, scope);
 }
 
 // Matcher::match_list on device: into (+reverse) (+stable score sort).  Result pointer + device count.
@@ -1389,22 +1459,24 @@ frz_status collapse_list(frz_matcher* m, const FrzCorpusStorage& cs, const Colla
 // `limit` positions of the final list are written (the sort's last scatter and the final copy drop the rest); the count in
 // ws.counters->total stays the full match count.  scope: as in match_into_device.  rank (optional): sort by the ranking's
 // key instead, under every strategy and for the empty matcher too (the strategy's direction only orders ties).  col
-// (optional, host calls only: final_out == nullptr): collapse the list before its sort (collapse_list).
+// (optional, host calls only: final_out == nullptr): collapse the list before its sort (collapse_list).  cols (optional,
+// host calls only): the list is that of a frz_match_list_columns call, whose starting column is cs (match_patterns).
 frz_status match_list_device(frz_matcher* m, const FrzCorpusStorage& cs, uint32_t index_offset, uint8_t sort,
                              FrzMatchDev** d_result, cudaStream_t stream, FrzLaunchStats* st, FrzMatchDev* final_out = nullptr,
                              uint32_t limit = kFrzNoLimit, const SubsetScope& scope = SubsetScope(), const Ranking* rank = nullptr,
-                             const Collapse* col = nullptr) {
+                             const Collapse* col = nullptr, const Columns* cols = nullptr) {
     FrzWorkspace& ws = m->ws;
     const bool reversed = sort == FRZ_SORT_INDEX_DESC || sort == FRZ_SORT_SCORE_THEN_INDEX_DESC;
     const bool by_score = sort == FRZ_SORT_SCORE_THEN_INDEX_ASC || sort == FRZ_SORT_SCORE_THEN_INDEX_DESC;
-    const bool will_sort = rank || (by_score && !m->compiled.empty());
+    const bool will_sort = rank || (by_score && (cols ? cols->any_compiled : !m->compiled.empty()));
     reset_call_state(m);
     FrzMatchDev* d_list = nullptr;
     uint32_t bound = 0;
     // the fused histogram counts the scores of every row of the list, so a ranked or collapsed sort never asks for it
     FrzScoreHist hist;
-    FRZ_TRY(match_into_device(m, cs, index_offset, reversed, &d_list, &bound, stream, st, will_sort ? nullptr : final_out,
-                              will_sort && !rank && !col ? &hist : nullptr, scope));
+    if (cols) FRZ_TRY(match_patterns(m, cols->pats, cs, cols->live, index_offset, reversed, &d_list, &bound, stream, st, scope));
+    else FRZ_TRY(match_into_device(m, cs, index_offset, reversed, &d_list, &bound, stream, st, will_sort ? nullptr : final_out,
+                                   will_sort && !rank && !col ? &hist : nullptr, scope));
     if (col) {
         const uint8_t order = rank ? FRZ_COLLAPSE_BY_KEY : will_sort ? FRZ_COLLAPSE_BY_SCORE : FRZ_COLLAPSE_BY_INDEX;
         FRZ_TRY(collapse_list(m, cs, *col, order, reversed, rank, &d_list, stream, st));
@@ -1476,10 +1548,12 @@ frz_status copy_out(frz_matcher* m, FrzMatchDev* d_list, uint64_t limit, frz_mat
 // Matcher::match_list (into, from index_offset, in `sort` order) → host, truncated to its first `limit` rows (top-K calls:
 // the same pipeline with a limit on the final scatter and copy; UINT64_MAX for the whole list).  scope: the rows of a subset
 // call (match_into_device).  rank: a ranked call, col: a collapsed call (match_list_device); group_counts (optional, host,
-// col->n_groups entries) receives the list's rows per group.
+// col->n_groups entries) receives the list's rows per group.  cols: a frz_match_list_columns call whose starting column is
+// corpus (match_list_device).
 frz_status match_list_host(frz_matcher* m, const frz_corpus* corpus, uint32_t index_offset, uint8_t sort, uint64_t limit,
                            const SubsetScope& scope, frz_match* out, uint64_t cap, uint64_t* n_out, uint64_t* n_total,
-                           const Ranking* rank = nullptr, const Collapse* col = nullptr, uint32_t* group_counts = nullptr) {
+                           const Ranking* rank = nullptr, const Collapse* col = nullptr, uint32_t* group_counts = nullptr,
+                           const Columns* cols = nullptr) {
     if (scope.none) {
         if (n_out) *n_out = 0;
         if (n_total) *n_total = 0;
@@ -1492,7 +1566,7 @@ frz_status match_list_host(frz_matcher* m, const frz_corpus* corpus, uint32_t in
     const uint32_t dev_limit = (uint32_t)std::min<uint64_t>(limit, kFrzNoLimit);   // a list never holds more than 2^32 - 1 matches
     frz_status s = FRZ_OK;
     for (int attempt = 0; attempt < 2; attempt++) {
-        s = match_list_device(m, corpus->st, index_offset, sort, &d_list, stream, &st, nullptr, dev_limit, scope, rank, col);
+        s = match_list_device(m, corpus->st, index_offset, sort, &d_list, stream, &st, nullptr, dev_limit, scope, rank, col, cols);
         if (s == FRZ_OK) s = copy_out(m, d_list, limit, out, cap, n_out, n_total, stream);
         if (s != kRetryOverflow) break;
         FRZ_TRY(ensure_workspace(m, corpus->st, std::max<uint64_t>(corpus->st.n, 1)));  // worst-case lists, then once more
@@ -2026,6 +2100,66 @@ extern "C" frz_status frz_match_list_collapsed(frz_matcher* m, const frz_corpus*
     return match_list_host(m, corpus, 0, m->config.sort, k, scope, out, k, n_out, n_total, b ? &rank : nullptr, &col, group_counts);
 }
 
+// ---------------------------------------------------------------------------------- column calls
+// Several text fields of the same rows, one matcher per field (DESIGN.md §4.13): the multi-pattern loop over every
+// column's patterns in column order, each against its own column (match_patterns), then the ranked, collapsed and top-K
+// steps of the single-corpus calls.
+extern "C" frz_status frz_match_list_columns(frz_matcher* const* ms, const frz_corpus* const* cols, uint64_t n_cols, uint8_t sort,
+                                             const frz_subset* s, const frz_boost* b, const frz_groups* g, uint64_t per_group,
+                                             uint64_t k, frz_match* out, uint64_t* n_out, uint64_t* n_total, uint32_t* group_counts) {
+    if (n_cols == 0) return frz_fail(FRZ_ERR_INVALID_ARG, "n_cols = 0: a columns call needs at least one column");
+    if (!ms || !cols) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    for (uint64_t c = 0; c < n_cols; c++)
+        if (!ms[c] || !cols[c]) return frz_fail(FRZ_ERR_INVALID_ARG, "null matcher or corpus of column %llu", (unsigned long long)c);
+    const FrzCorpusStorage& first = cols[0]->st;
+    for (uint64_t c = 1; c < n_cols; c++) {
+        if (cols[c]->st.device != first.device)
+            return frz_fail(FRZ_ERR_INVALID_ARG, "column %llu is on device %d, column 0 on device %d", (unsigned long long)c,
+                            cols[c]->st.device, first.device);
+        if (cols[c]->st.n != first.n)
+            return frz_fail(FRZ_ERR_INVALID_ARG, "column %llu holds %llu rows, column 0 holds %llu: the columns must share one index space",
+                            (unsigned long long)c, (unsigned long long)cols[c]->st.n, (unsigned long long)first.n);
+    }
+    FRZ_TRY(frz_check_index_range(first.n, 0));
+    if (sort > FRZ_SORT_INDEX_DESC) return frz_fail(FRZ_ERR_INVALID_ARG, "sort = %u is not a sort strategy", (unsigned)sort);
+    if (g && per_group == 0) return frz_fail(FRZ_ERR_INVALID_ARG, "per_group = 0");
+    if (g && per_group > kFrzCollapseMaxPerGroup && per_group != UINT64_MAX)
+        return frz_fail(FRZ_ERR_UNSUPPORTED, "per_group = %llu: at most %llu rows per group, or UINT64_MAX for no cap",
+                        (unsigned long long)per_group, (unsigned long long)kFrzCollapseMaxPerGroup);
+    if (!out && k > 0) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
+    // membership, boosts and group ids are by index, so a handle of any column serves every column
+    const auto of_a_column = [&](const frz_corpus* h) { return std::find(cols, cols + n_cols, h) != cols + n_cols; };
+    if (s && !of_a_column(s->corpus)) return frz_fail(FRZ_ERR_INVALID_ARG, "the subset was made on none of the columns");
+    if (b && !of_a_column(b->corpus)) return frz_fail(FRZ_ERR_INVALID_ARG, "the boost was made on none of the columns");
+    if (g && !of_a_column(g->corpus)) return frz_fail(FRZ_ERR_INVALID_ARG, "the groups were made on none of the columns");
+    FRZ_TRY(frz_ensure_device(first.device));
+    // the list starts from the column of the first non-negated pattern (its base, scanned in full), else from column 0
+    Columns cs;
+    uint64_t start = n_cols;
+    for (uint64_t c = 0; c < n_cols; c++) {
+        for (const Compiled& p : ms[c]->compiled) {
+            cs.pats.push_back(ColumnPattern{&p, ms[c], &cols[c]->st});
+            if (!p.negated && start == n_cols) start = c;
+        }
+        cs.any_compiled |= !ms[c]->compiled.empty();
+    }
+    if (start == n_cols) start = 0;
+    for (uint64_t c = 0; c < n_cols; c++) {   // the other columns' removed rows (none: no extra launch)
+        const FrzCorpusStorage* st = &cols[c]->st;
+        if (cols[c] != cols[start] && st->n_removed && std::find(cs.live.begin(), cs.live.end(), st) == cs.live.end())
+            cs.live.push_back(st);
+    }
+    frz_matcher* m = ms[0];
+    SubsetScope scope;
+    if (s) FRZ_TRY(subset_scope(m, cols[start], *s, nullptr, &scope));
+    Ranking rank;
+    if (b) rank = ranking_of(*b);
+    Collapse col;
+    if (g) col = collapse_of(*g, per_group);
+    return match_list_host(m, cols[start], 0, sort, k, scope, out, k, n_out, n_total, b ? &rank : nullptr, g ? &col : nullptr,
+                           group_counts, &cs);
+}
+
 // ---------------------------------------------------------------------------------- batched top-K: entry points
 namespace {
 // query j's single-query call: frz_match_list_collapsed with groups, else frz_match_list_ranked with a boost, else
@@ -2487,7 +2621,7 @@ frz_status match_streamed_impl(frz_matcher* m, const uint8_t* bytes, const void*
         reset_call_state(m);
         StreamedCtx x;
         x.m = m; x.c = &pat; x.index_offset = index_offset; x.dst = will_sort ? ws.matches_a.get() : final_out; x.stream = stream; x.st = st;
-        FRZ_TRY(needle_table(m, pat, &x.ntab));   // a synchronous upload, so before the first H2D chunk
+        FRZ_TRY(needle_table(m, pat, m->ws.device, &x.ntab));   // a synchronous upload, so before the first H2D chunk
         x.pending_t0 = 0; x.chunks_pending = 0;
         x.group = 4;   // a range per four H2D chunks (about 1/8 of the list): the tail after the last chunk is one range + the sort
         FRZ_CUDA_TRY(cudaMemsetAsync(ws.stream_total.get(), 0, sizeof(unsigned long long), stream));

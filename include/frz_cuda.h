@@ -396,6 +396,51 @@ FRZ_API frz_status frz_match_list_collapsed(frz_matcher* m, const frz_corpus* c,
                                             const frz_groups* g, uint64_t per_group, uint64_t k, frz_match* out,
                                             uint64_t* n_out, uint64_t* n_total, uint32_t* group_counts);
 
+/* ------------------------------------------------ column calls
+ *
+ * Rows with several text fields, each searched by its own query (file name + directory, command + working directory,
+ * symbol + container, title + artist): a matcher per column, rows must match every column, scores add up.  The reference
+ * has no such method; it is its multi-pattern rule (src/matcher/multi.rs:83-152) where each pattern reads its own column.
+ *
+ * Column c is the corpus cols[c], searched by ms[c].  All columns share one index space: row i is haystack i of every
+ * column, and n is their common frz_corpus_len.  Let L_c be the rows of frz_match_list_into(ms[c], cols[c], 0) (an empty
+ * matcher, or one whose patterns are all negated, lists every row it does not exclude, with score 0).  Row i matches
+ * when i < n, it is live (not removed) in every column, it is a member of s when s is given, and it is in every L_c.  Its
+ * record is index i, score min(65535, sum_c score_c(i)) and exact OR_c exact_c(i).  The list L: the matching rows in
+ * index order, reversed under the *_DESC strategies, then
+ *   b given:                                    ranked by key exactly as frz_match_list_ranked (every strategy);
+ *   else some matcher has a compiled pattern
+ *        and sort is ScoreThenIndexAsc / Desc:  sorted stably by descending score (src/matcher/mod.rs:218);
+ *   else:                                       left in that order.
+ * g given: C is L collapsed exactly as frz_match_list_collapsed collapses its L, and group_counts (may be NULL; a host
+ * array of frz_groups_count(g) entries) receives L's rows per group.  Otherwise C = L.  The call writes C[0 : min(k, |C|)]
+ * to `out` (HOST memory; min(k, frz_corpus_len, frz_subset_len(s)) entries suffice), their number to *n_out and |C| to
+ * *n_total (may be NULL).  k = 0 only counts, k = UINT64_MAX returns all of C, and the call never returns
+ * FRZ_ERR_CAPACITY.  per_group is read only when g is given: 1 .. 32 or UINT64_MAX; 0 is FRZ_ERR_INVALID_ARG, any other
+ * value FRZ_ERR_UNSUPPORTED.  sort is an FRZ_SORT_* value; the matchers' own sort settings are not read.
+ *
+ * The order of the columns does not change the result (saturating addition of non-negative scores is associative, and
+ * OR commutes), only the speed: the first column with a non-negated pattern is scanned in full, and every later pattern
+ * runs on the rows that are still candidates, about 7 to 10 times slower per row than the full scan (DESIGN.md §4.9,
+ * §4.13).  Put the most selective column first.  Every call, even with one column and one pattern, takes the
+ * multi-pattern path: ms[0]'s device scratch grows by two candidate lists of 8 bytes per row (about 160 MB at 10 M rows,
+ * kept for later calls), and a by-score sort does not get the histogram the single-pattern calls build while scoring.
+ *
+ * FRZ_ERR_INVALID_ARG, checked in this order before any device work: n_cols == 0; a NULL ms, cols, ms[c] or cols[c];
+ * columns on different devices; columns whose frz_corpus_len differ at the time of the call (after an append to some
+ * columns only, until the others catch up); then FRZ_ERR_TOO_MANY_ITEMS for more rows than u32 indices reach; then
+ * FRZ_ERR_INVALID_ARG for a sort above 3; per_group 0 with groups (then FRZ_ERR_UNSUPPORTED for a
+ * per_group out of range); a NULL out with k > 0; a subset, boost or groups handle made on none of the given columns.
+ * Membership, boosts and group ids are by index, so a handle of any column serves.
+ *
+ * A column or a matcher may appear more than once.  Blocking.  The call runs on ms[0]'s device scratch and stream, and
+ * frz_matcher_last_timings(ms[0]) reports it; the other matchers are only read, apart from their long-needle table, which
+ * is uploaded to the columns' device.  None of the matchers, columns or handles may be used by another call meanwhile. */
+FRZ_API frz_status frz_match_list_columns(frz_matcher* const* ms, const frz_corpus* const* cols, uint64_t n_cols,
+                                          uint8_t sort, const frz_subset* s, const frz_boost* b, const frz_groups* g,
+                                          uint64_t per_group, uint64_t k, frz_match* out, uint64_t* n_out,
+                                          uint64_t* n_total, uint32_t* group_counts);
+
 /* frz_match_list_batch_top (above) where each query may have its own subset and boost, in one call: a service whose users
  * each search their own rows (a subset) ranked by a prior (a boost).  The reference has no such method (see the subset
  * and ranked calls above).  For every j < q, out[j*k .. j*k + n_out[j]), n_out[j] and n_total[j] are bit for bit what the
