@@ -120,6 +120,7 @@ def lib():
     L.frz_groups_destroy.restype = None
     L.frz_match_list_collapsed.argtypes = [vp, vp, vp, vp, vp, u64, u64, vp, C.POINTER(u64), C.POINTER(u64), vp]
     L.frz_match_list_columns.argtypes = [vp, vp, u64, C.c_uint8, vp, vp, vp, u64, u64, vp, C.POINTER(u64), C.POINTER(u64), vp]
+    L.frz_match_list_batch_columns.argtypes = [vp, u64, vp, u64, C.c_uint8, vp, vp, vp, vp, u64, vp, vp, vp, vp]
     L.frz_match_list_into.argtypes = [vp, vp, u32, vp, u64, C.POINTER(u64)]
     L.frz_match_list_host.argtypes = [vp, vp, vp, u64, C.c_int, vp, u64, C.POINTER(u64)]
     L.frz_match_list_host_arrow.argtypes = [vp, vp, vp, C.c_int, u64, C.c_int, vp, u64, C.POINTER(u64)]
@@ -708,8 +709,44 @@ def match_list_columns(matchers, columns, k: Optional[int] = None, sort: SortStr
     return out[: n_out.value], total.value
 
 
+def match_list_batch_columns(matchers, columns, k: int, sort: SortStrategy = SortStrategy.ScoreThenIndexAsc, subsets=None,
+                             boosts=None, groups=None, per_group=1, counts: bool = False):
+    """frz_match_list_batch_columns: match_list_columns for many queries over the same columns in one call.  matchers: q
+    sequences of len(columns) matchers, matchers[j][c] searching columns[c].  subsets / boosts / groups: None, or one handle
+    (of any column) or None per query; per_group: an int (1..32), None (no cap), or one such value per query.  Query j's
+    rows are those of match_list_columns(matchers[j], columns, k, sort, subsets[j], boosts[j], groups[j], per_group[j]).
+    Returns the (q, k) rows, n_out and n_total as match_list_batch_top, and with counts=True also a list of each query's
+    rows per group (uint32, len(groups[j]) entries; None for a query without groups)."""
+    matchers, columns = [list(m) for m in matchers], list(columns)
+    q, k, n_cols = len(matchers), int(k), len(columns)
+    for j, mj in enumerate(matchers):
+        if len(mj) != n_cols:
+            raise ValueError(f"query {j} has {len(mj)} matchers for {n_cols} columns")
+    groups = list(groups) if groups is not None else [None] * q
+    hs, hb, hg = _handles(subsets, q, "subsets"), _handles(boosts, q, "boosts"), _handles(groups, q, "groups")
+    if per_group is None or isinstance(per_group, (int, np.integer)):
+        per_group = [per_group] * q
+    per_group = list(per_group)
+    if len(per_group) != q:
+        raise ValueError(f"{q} queries need {q} per_group values, got {len(per_group)}")
+    pg = np.array([_U64_MAX if p is None else int(p) for p in per_group] or [1], dtype=np.uint64)
+    cnt = [np.zeros(len(g), dtype=np.uint32) if counts and g is not None else None for g in groups]
+    hc = (C.c_void_p * max(q, 1))(*[c.ctypes.data if c is not None else None for c in cnt]) if counts else None
+    ms = (C.c_void_p * max(q * n_cols, 1))(*[m._h.value for mj in matchers for m in mj])
+    cs = (C.c_void_p * max(n_cols, 1))(*[c._h.value for c in columns])
+    out = np.zeros((q, k), dtype=MATCH_DTYPE)
+    n_out = np.zeros(q, dtype=np.uint64)
+    n_total = np.zeros(q, dtype=np.uint64)
+    _check(lib().frz_match_list_batch_columns(ms, q, cs, n_cols, int(sort), hs, hb, hg, pg.ctypes.data, k,
+                                              out.ctypes.data if out.size else None, n_out.ctypes.data, n_total.ctypes.data, hc))
+    if counts:
+        return out, n_out.astype(np.int64), n_total.astype(np.int64), cnt
+    return out, n_out.astype(np.int64), n_total.astype(np.int64)
+
+
 def batch_last() -> dict:
-    """Test aid (frz_debug_batch_last): what this thread's last match_list_batch_top or match_list_batch did."""
+    """Test aid (frz_debug_batch_last): what this thread's last batched call (match_list_batch_top, match_list_batch,
+    match_list_batch_collapsed or match_list_batch_columns) did."""
     v = np.zeros(4, dtype=np.uint64)
     lib().frz_debug_batch_last(v.ctypes.data)
     return {"batched": int(v[0]), "overflowed": int(v[1]), "sub_batches": int(v[2]), "launches": int(v[3])}

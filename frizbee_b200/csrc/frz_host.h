@@ -404,6 +404,26 @@ frz_status frz_launch_batch_collapse(const FrzBatchDev& b, const FrzBatchTables&
 frz_status frz_launch_batch_top_collapsed(const FrzBatchDev& b, const FrzBatchTables& t, uint32_t nq, uint32_t k, FrzMatchDev* rows,
                                           unsigned long long* totals, cudaStream_t stream, FrzLaunchStats* st);
 
+// The join of a sub-batch of frz_match_list_batch_columns (host.cu; the per-row rule is batch_columns_plan.cuh's).
+struct FrzColumnFold;
+struct FrzBatchColumnsDev {
+    uint32_t* acc;                 // [j][list_stride] the query's accumulator per row (zero before the first fold)
+    uint32_t* err;                 // [j] the sticky device error of the query's column stages (zero before the first fold)
+    const FrzColumnFold* fold;     // [c][nq] how query j folds column c
+    const uint8_t* need;           // [j] the columns query j folds
+    uint64_t n_rows;
+};
+// prefilter.cu: k_tile_scan_batch alone (tile_out_base and ctr[j].total from tile_count, for the nq queries)
+frz_status frz_launch_tile_scan_batch(const FrzBatchDev& b, uint32_t n_tiles, uint32_t nq, cudaStream_t stream, FrzLaunchStats* st);
+// batch_columns.cu: fold column c into every query's accumulator, from the lists its batched stages left in b's slots (cv:
+// the column, for the rows live in it), one launch over the nq queries
+frz_status frz_launch_batch_columns_fold(const FrzBatchDev& b, const FrzBatchColumnsDev& d, const FrzCorpusView& cv, uint32_t c,
+                                         uint32_t nq, cudaStream_t stream, FrzLaunchStats* st);
+// batch_columns.cu: every query's rows that matched each column it folds → b.lists[j] (index order, reversed when
+// b.reversed[j]), their number → b.ctr[j].total and its error word → b.ctr[j].error: the list k_batch_top cuts
+frz_status frz_launch_batch_columns_join(const FrzBatchDev& b, const FrzBatchColumnsDev& d, uint32_t n_tiles, uint32_t nq,
+                                         cudaStream_t stream, FrzLaunchStats* st);
+
 // The groups of a collapsed call on the device (frz_match_list_collapsed, host.cu; the rule is collapse_plan.cuh's).
 struct FrzCollapseDev {
     const uint32_t* ids;         // group of index i < n_ids (frz_groups); indices past it are in no group

@@ -20,6 +20,7 @@
 #include <mutex>
 
 #include "batch_collapse_plan.cuh"
+#include "batch_columns_plan.cuh"
 #include "batch_plan.cuh"
 #include "collapse_plan.cuh"
 #include "frz_device.cuh"
@@ -1598,11 +1599,11 @@ extern "C" frz_status frz_match_list_top(frz_matcher* m, const frz_corpus* corpu
 }
 
 // ---------------------------------------------------------------------------------- batched top-K
-// frz_match_list_batch_collapsed, frz_match_list_batch and frz_match_list_batch_top (DESIGN.md §4.11).  Queries of the
-// batched class run in sub-batches whose every stage is one launch (per kernel variant present) over all of the
-// sub-batch's queries, with one upload, one read-back and one synchronise per sub-batch; every other query, and every
-// query of an overflowed sub-batch, runs its single-query call's pipeline (frz_match_list_top, _subset_top, _ranked or
-// _collapsed).  The entry points follow the collapsed calls.
+// frz_match_list_batch_collapsed, frz_match_list_batch and frz_match_list_batch_top (DESIGN.md §4.11), and
+// frz_match_list_batch_columns (§4.13).  Queries of the batched class run in sub-batches whose every stage is one launch
+// (per kernel variant present, and per column) over all of the sub-batch's queries, with one upload, one read-back and one
+// synchronise per sub-batch; every other query, and every query of an overflowed sub-batch, runs its single-query call's
+// pipeline (frz_match_list_top, _subset_top, _ranked, _collapsed or _columns).  The entry points follow the column calls.
 namespace {
 
 // Device scratch of one sub-batch's queries, in one allocation: a fixed budget, so a batch call holds the same scratch for
@@ -1622,18 +1623,26 @@ constexpr uint64_t kBatchMinQueries = 32;
 // through the sub-batch's staging then costs more than the loop saves (tools/bench_batch_collapsed.py on an H100 SXM,
 // DESIGN.md §4.11: ahead of the loop with 100 k groups, behind it with 1 M).
 constexpr uint64_t kBatchMaxCountedGroups = 1ull << 18;
+// A column query (frz_match_list_batch_columns) with a typo budget in some column batches only up to this many rows, and
+// one whose every pattern has max_typos = 0 only up to kBatchMaxRows (tools/bench_batch_columns.py on an H100 SXM, DESIGN.md
+// §4.13: with a typo budget, or at 1 M rows, the short needles of a second column pass more rows than the survivor lists
+// hold, and the overflowed sub-batches run again query by query, behind the loop).
+constexpr uint64_t kBatchColumnsMaxRowsTypo = 0;
 // The limits in force (frz_debug_batch_limits changes them for tests and tools/bench_batch.py) and what the calling
 // thread's last batch call did (frz_debug_batch_last).
 std::atomic<uint64_t> g_batch_max_rows{kBatchMaxRows};
+std::atomic<uint64_t> g_batch_columns_typo_rows{kBatchColumnsMaxRowsTypo};
 std::atomic<uint64_t> g_batch_min_queries{kBatchMinQueries};
 thread_local uint64_t g_batch_last[4] = {0, 0, 0, 0};   // batched queries, overflowed queries, sub-batches, launches
 
 struct BatchLayout {
     uint64_t nt = 0, stride = 0, cap = 0, k = 0;
     uint64_t groups = 0;     // entries of each query slot's group tables (0: no query of the call has groups)
-    uint64_t off[18] = {};   // byte offsets of the arrays below, in this order
+    uint64_t n_cols = 0;     // columns of a frz_match_list_batch_columns call (0: a single-corpus call)
+    uint64_t off[21] = {};   // byte offsets of the arrays below, in this order
     uint64_t bytes = 0;
-    enum { CTR, BITMAP, PREFIX, TCOUNT, TBASE, SURV, LISTS, BEST, TAKEN, PATS, REV, BYSC, SCOPE, COLS, TOTALS, ROWS, COUNTS, END };
+    enum { CTR, BITMAP, PREFIX, TCOUNT, TBASE, SURV, LISTS, BEST, TAKEN, ACC, JERR, PATS, REV, BYSC, SCOPE, COLS, CMAP, TOTALS, ROWS,
+           COUNTS, END };
     // queries per sub-batch for this corpus and k (0: fewer than two fit the budget)
     static uint64_t per_query(const FrzCorpusStorage& cs, uint64_t k, uint64_t cap) {
         const uint64_t nt = cs.n_tiles;
@@ -1641,18 +1650,24 @@ struct BatchLayout {
                FRZ_N_CLASSES * cap * sizeof(FrzSurvivor) + std::max<uint64_t>(cs.n, 1) * sizeof(FrzMatchDev) + sizeof(FrzPatternDev) + 2 +
                sizeof(FrzBatchScope) + sizeof(unsigned long long) + k * sizeof(FrzMatchDev) + 13 * 256 / 2;
     }
-    BatchLayout(const FrzCorpusStorage& cs, uint64_t k_, uint64_t cap_, uint64_t qs, uint64_t groups_ = 0)
-        : nt(cs.n_tiles), stride(std::max<uint64_t>(cs.n, 1)), cap(cap_), k(k_), groups(groups_) {
+    // n_cols_ > 0 (a column call) adds each query's accumulator and error word, a pattern slot per column and query, and
+    // the fold records (batch_columns_plan.cuh); a single-corpus call gets the layout it had before column calls existed
+    BatchLayout(const FrzCorpusStorage& cs, uint64_t k_, uint64_t cap_, uint64_t qs, uint64_t groups_ = 0, uint64_t n_cols_ = 0)
+        : nt(cs.n_tiles), stride(std::max<uint64_t>(cs.n, 1)), cap(cap_), k(k_), groups(groups_), n_cols(n_cols_) {
         const uint64_t g = groups ? qs : 0;   // the group arrays exist only in a call with grouped queries
+        const uint64_t c = n_cols ? qs : 0;   // the join arrays only in a column call
         const uint64_t size[END] = {qs * sizeof(FrzCounters), qs * nt * 32 * sizeof(uint32_t), qs * nt * 32 * sizeof(uint16_t),
                                     qs * nt * sizeof(uint32_t), qs * nt * sizeof(uint64_t), qs * FRZ_N_CLASSES * cap * sizeof(FrzSurvivor),
                                     qs * stride * sizeof(FrzMatchDev), g * groups * sizeof(unsigned long long), g * stride,
-                                    qs * sizeof(FrzPatternDev), qs, qs, qs * sizeof(FrzBatchScope), g * sizeof(FrzBatchCollapse),
+                                    c * stride * sizeof(uint32_t), c * sizeof(uint32_t),
+                                    qs * std::max<uint64_t>(n_cols, 1) * sizeof(FrzPatternDev), qs, qs, qs * sizeof(FrzBatchScope),
+                                    g * sizeof(FrzBatchCollapse), c * (n_cols * sizeof(FrzColumnFold) + 1),
                                     qs * sizeof(unsigned long long), qs * k * sizeof(FrzMatchDev), g * groups * sizeof(uint32_t)};
         uint64_t at = 0;
         for (int i = 0; i < END; i++) {
-            // CTR..BITMAP are zeroed as one range, PATS..COLS uploaded as one, TOTALS..COUNTS read back as one
-            const bool packed = i == BITMAP || i == REV || i == BYSC || i == SCOPE || i == COLS || i == ROWS || i == COUNTS;
+            // CTR..BITMAP are zeroed as one range, ACC..JERR too, PATS..CMAP uploaded as one, TOTALS..COUNTS read back as one
+            const bool packed = i == BITMAP || i == JERR || i == REV || i == BYSC || i == SCOPE || i == COLS || i == CMAP || i == ROWS ||
+                                i == COUNTS;
             if (!packed) at = (at + 255) & ~255ull;
             else at = (at + 7) & ~7ull;
             off[i] = at;
@@ -1684,6 +1699,28 @@ bool batch_selected(const frz_matcher* m, const FrzCorpusStorage& cs) {
     return cs.n <= limit;
 }
 
+// The columns of a frz_match_list_batch_columns call: query j's matcher for column c is ms[j * n_cols + c].
+struct BatchColumns {
+    const frz_corpus* const* cols = nullptr;
+    uint64_t n_cols = 0;
+    uint8_t sort = 0;
+};
+// the batched class of a column query: every column's matcher of the batched class or without a pattern, at least one
+// pattern, at most kFrzBatchMaxColumns columns, and rows within the row limit (g_batch_max_rows when every pattern has
+// max_typos = 0, else g_batch_columns_typo_rows)
+bool batch_columns_selected(frz_matcher* const* mj, const BatchColumns& bc) {
+    if (bc.n_cols > kFrzBatchMaxColumns) return false;
+    bool any = false, all_t0 = true;
+    for (uint64_t c = 0; c < bc.n_cols; c++) {
+        const frz_matcher* m = mj[c];
+        if (m->compiled.empty()) continue;
+        if (!batchable(m, bc.cols[c]->st)) return false;
+        any = true;
+        all_t0 &= m->compiled[0].dev.typo_mode == FRZ_T_0;
+    }
+    return any && bc.cols[0]->st.n <= (all_t0 ? g_batch_max_rows.load() : g_batch_columns_typo_rows.load());
+}
+
 // The groups of a call's queries, indexed as ms (frz_match_list_batch_collapsed).
 struct BatchGroups {
     const FrzBatchCollapse* cols = nullptr;   // [j] ids == nullptr: no groups (cols == nullptr: no query of the call has any)
@@ -1693,10 +1730,12 @@ struct BatchGroups {
 
 // One sub-batch: queries which[0..ns) of ms, all of the batched class.  scopes: nullptr when no query of the call is scoped
 // or ranked, else every query's subset and boost (indexed as ms).  gr: the call's groups (L.groups > 0 when it has any).
+// bc: a column call (c is its column 0): each column's stages run for the queries with a pattern in it, in slots of their
+// own, and the join (batch_columns.cu) leaves each query's list where the cut reads it.
 // *overflow: a survivor list overflowed, nothing was written to the results (the caller runs the queries one by one).
 frz_status batch_run(frz_matcher* const* ms, const FrzBatchScope* scopes, const BatchGroups& gr, const uint64_t* which, uint32_t ns,
                      const frz_corpus* c, uint64_t k, const BatchLayout& L, uint8_t* d, frz_match* out, uint64_t* n_out,
-                     uint64_t* n_total, bool* overflow, FrzLaunchStats& st) {
+                     uint64_t* n_total, bool* overflow, FrzLaunchStats& st, const BatchColumns* bc = nullptr) {
     const FrzCorpusStorage& cs = c->st;
     cudaStream_t stream = nullptr;
     *overflow = false;
@@ -1712,9 +1751,8 @@ frz_status batch_run(frz_matcher* const* ms, const FrzBatchScope* scopes, const 
     uint8_t grouped[kFrzBatchMaxSub] = {}, wants[kFrzBatchMaxSub] = {};
     uint32_t slot[kFrzBatchMaxSub] = {}, n_grouped = 0, rounds = 0;
     for (uint32_t j = 0; j < ns; j++) {
-        const frz_matcher* m = ms[which[j]];
-        const uint8_t sort = m->config.sort;
-        h_pats[j] = m->compiled[0].dev;
+        const uint8_t sort = bc ? bc->sort : ms[which[j]]->config.sort;
+        if (!bc) h_pats[j] = ms[which[j]]->compiled[0].dev;
         h_rev[j] = sort == FRZ_SORT_INDEX_DESC || sort == FRZ_SORT_SCORE_THEN_INDEX_DESC;
         h_bysc[j] = sort == FRZ_SORT_SCORE_THEN_INDEX_ASC || sort == FRZ_SORT_SCORE_THEN_INDEX_DESC;
         h_scope[j] = scopes ? scopes[which[j]] : FrzBatchScope();
@@ -1731,6 +1769,26 @@ frz_status batch_run(frz_matcher* const* ms, const FrzBatchScope* scopes, const 
     for (uint32_t j = 0; j < ns && L.groups; j++) {
         h_cols[j] = gr.cols[which[j]];
         h_cols[j].table = frz_batch_collapse_table(slot[j], L.groups);
+    }
+    // a column call's patterns: column c's queries with a pattern take its slots 0, 1, ... in query order
+    FrzColumnFold* h_fold = reinterpret_cast<FrzColumnFold*>(h + (L.off[BatchLayout::CMAP] - L.off[BatchLayout::PATS]));
+    uint8_t* h_need = reinterpret_cast<uint8_t*>(h_fold + L.n_cols * ns);
+    std::vector<uint32_t> n_slots(L.n_cols, 0);
+    std::vector<uint8_t> folded(L.n_cols, 0);
+    for (uint32_t j = 0; j < ns && bc; j++) h_need[j] = 0;
+    for (uint64_t col = 0; col < L.n_cols; col++) {
+        for (uint32_t j = 0; j < ns; j++) {
+            const frz_matcher* m = ms[which[j] * L.n_cols + col];
+            FrzColumnFold& f = h_fold[col * ns + j];
+            f.pass = h_need[j];
+            if (!m->compiled.empty()) {
+                f.slot = (uint8_t)n_slots[col];
+                h_pats[col * ns + n_slots[col]++] = m->compiled[0].dev;
+            } else {
+                f.slot = bc->cols[col]->st.n_removed ? kFrzColumnLive : kFrzColumnSkip;
+            }
+            if (f.slot != kFrzColumnSkip) { h_need[j]++; folded[col] = 1; }
+        }
     }
     const uint64_t down = L.off[BatchLayout::COUNTS] + n_back * L.groups * sizeof(uint32_t) - L.off[BatchLayout::TOTALS];
     FrzBatchDev b;
@@ -1749,11 +1807,37 @@ frz_status batch_run(frz_matcher* const* ms, const FrzBatchScope* scopes, const 
     unsigned long long* totals = reinterpret_cast<unsigned long long*>(d + L.off[BatchLayout::TOTALS]);
     FrzMatchDev* rows = reinterpret_cast<FrzMatchDev*>(d + L.off[BatchLayout::ROWS]);
     FRZ_CUDA_TRY(cudaMemcpyAsync(d + L.off[BatchLayout::PATS], h, up, cudaMemcpyHostToDevice, stream));
-    FRZ_CUDA_TRY(cudaMemsetAsync(d + L.off[BatchLayout::CTR], 0,
-                                 L.off[BatchLayout::BITMAP] + (uint64_t)ns * L.nt * 32 * sizeof(uint32_t) - L.off[BatchLayout::CTR], stream));
-    const FrzCorpusView cv = cs.view();
-    FRZ_TRY(frz_launch_prefilter_batch(cv, b, h_pats, ns, stream, &st));
-    FRZ_TRY(frz_launch_sw_batch(cv, b, h_pats, ns, stream, &st));
+    // the counters and survivor bitmaps of the first nq slots start zero
+    const auto clear_slots = [&](uint32_t nq) {
+        return cudaMemsetAsync(d + L.off[BatchLayout::CTR], 0,
+                               L.off[BatchLayout::BITMAP] + (uint64_t)nq * L.nt * 32 * sizeof(uint32_t) - L.off[BatchLayout::CTR], stream);
+    };
+    if (!bc) {
+        FRZ_CUDA_TRY(clear_slots(ns));
+        const FrzCorpusView cv = cs.view();
+        FRZ_TRY(frz_launch_prefilter_batch(cv, b, h_pats, ns, stream, &st));
+        FRZ_TRY(frz_launch_sw_batch(cv, b, h_pats, ns, stream, &st));
+    } else {   // each column's stages, folded into the accumulators, then every query's joined list
+        FrzBatchColumnsDev jd;
+        jd.acc = reinterpret_cast<uint32_t*>(d + L.off[BatchLayout::ACC]);
+        jd.err = reinterpret_cast<uint32_t*>(d + L.off[BatchLayout::JERR]);
+        jd.fold = reinterpret_cast<const FrzColumnFold*>(d + L.off[BatchLayout::CMAP]);
+        jd.need = d + L.off[BatchLayout::CMAP] + (h_need - reinterpret_cast<uint8_t*>(h_fold));
+        jd.n_rows = cs.n;
+        FRZ_CUDA_TRY(cudaMemsetAsync(jd.acc, 0, L.off[BatchLayout::JERR] + ns * sizeof(uint32_t) - L.off[BatchLayout::ACC], stream));
+        for (uint64_t col = 0; col < L.n_cols; col++) {
+            const FrzCorpusView cv = bc->cols[col]->st.view();
+            FrzBatchDev bcol = b;
+            bcol.pats = b.pats + col * ns;
+            if (n_slots[col]) {
+                FRZ_CUDA_TRY(clear_slots(n_slots[col]));
+                FRZ_TRY(frz_launch_prefilter_batch(cv, bcol, h_pats + col * ns, n_slots[col], stream, &st));
+                FRZ_TRY(frz_launch_sw_batch(cv, bcol, h_pats + col * ns, n_slots[col], stream, &st));
+            }
+            if (folded[col]) FRZ_TRY(frz_launch_batch_columns_fold(bcol, jd, cv, (uint32_t)col, ns, stream, &st));
+        }
+        FRZ_TRY(frz_launch_batch_columns_join(b, jd, (uint32_t)L.nt, ns, stream, &st));
+    }
     const FrzBatchScope* d_scope = reinterpret_cast<const FrzBatchScope*>(d + L.off[BatchLayout::SCOPE]);
     if (n_grouped) {   // the collapse, then the kept rows' cut
         FrzBatchTables t;
@@ -1790,6 +1874,7 @@ frz_status batch_run(frz_matcher* const* ms, const FrzBatchScope* scopes, const 
 
 extern "C" void frz_debug_batch_limits(uint64_t max_rows, uint64_t min_queries) {
     g_batch_max_rows = max_rows ? max_rows : kBatchMaxRows;
+    g_batch_columns_typo_rows = max_rows ? max_rows : kBatchColumnsMaxRowsTypo;
     g_batch_min_queries = min_queries ? min_queries : kBatchMinQueries;
 }
 
@@ -2182,32 +2267,35 @@ extern "C" frz_status frz_match_list_batch(frz_matcher* const* ms, uint64_t q, c
     return frz_match_list_batch_collapsed(ms, q, corpus, subsets, boosts, nullptr, nullptr, k, out, n_out, n_total, nullptr);
 }
 
-extern "C" frz_status frz_match_list_batch_collapsed(frz_matcher* const* ms, uint64_t q, const frz_corpus* corpus,
-                                                     const frz_subset* const* subsets, const frz_boost* const* boosts,
-                                                     const frz_groups* const* groups, const uint64_t* per_group, uint64_t k,
-                                                     frz_match* out, uint64_t* n_out, uint64_t* n_total, uint32_t* const* group_counts) {
-    if (!ms || !corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
-    for (uint64_t j = 0; j < q; j++)
-        if (!ms[j]) return frz_fail(FRZ_ERR_INVALID_ARG, "null matcher at %llu", (unsigned long long)j);
-    for (uint64_t j = 0; per_group && j < q; j++) {
-        if (per_group[j] == 0) return frz_fail(FRZ_ERR_INVALID_ARG, "per_group = 0 at %llu", (unsigned long long)j);
-        if (per_group[j] > kFrzCollapseMaxPerGroup && per_group[j] != UINT64_MAX)
-            return frz_fail(FRZ_ERR_UNSUPPORTED, "per_group = %llu at %llu: at most %llu rows per group, or UINT64_MAX for no cap",
-                            (unsigned long long)per_group[j], (unsigned long long)j, (unsigned long long)kFrzCollapseMaxPerGroup);
-    }
-    for (uint64_t j = 0; j < q; j++) {
-        if (subsets && subsets[j] && subsets[j]->corpus != corpus)
-            return frz_fail(FRZ_ERR_INVALID_ARG, "the subset of query %llu was made on another corpus", (unsigned long long)j);
-        if (boosts && boosts[j] && boosts[j]->corpus != corpus)
-            return frz_fail(FRZ_ERR_INVALID_ARG, "the boost of query %llu was made on another corpus", (unsigned long long)j);
-        if (groups && groups[j] && groups[j]->corpus != corpus)
-            return frz_fail(FRZ_ERR_INVALID_ARG, "the groups of query %llu were made on another corpus", (unsigned long long)j);
-    }
-    if (q && !n_out) return frz_fail(FRZ_ERR_INVALID_ARG, "null n_out");
-    if (k && (q > UINT64_MAX / k || q * k > SIZE_MAX / sizeof(frz_match)))
-        return frz_fail(FRZ_ERR_INVALID_ARG, "q * k overflows: q = %llu, k = %llu", (unsigned long long)q, (unsigned long long)k);
-    if (q * k > 0 && !out) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
-    if (q == 0) return FRZ_OK;
+namespace {
+// The arguments of a batched call, checked (frz_match_list_batch_collapsed, frz_match_list_batch_columns).  bc: a column
+// call, whose query j has the matchers ms[j * n_cols ..] and whose corpus is its column 0.
+struct BatchCall {
+    frz_matcher* const* ms;
+    uint64_t q;
+    const frz_corpus* corpus;
+    const BatchColumns* bc;
+    const frz_subset* const* subsets;
+    const frz_boost* const* boosts;
+    const frz_groups* const* groups;
+    const uint64_t* per_group;
+    uint64_t k;
+    frz_match* out;
+    uint64_t* n_out;
+    uint64_t* n_total;
+    uint32_t* const* group_counts;
+};
+
+// The driver of the batched calls: the queries of the batched class run in sub-batches (batch_run), every other query, and
+// every query of an overflowed sub-batch, its single-query call.
+frz_status batch_drive(const BatchCall& a) {
+    frz_matcher* const* ms = a.ms;
+    const uint64_t q = a.q, k = a.k;
+    const frz_corpus* corpus = a.corpus;
+    const BatchColumns* bc = a.bc;
+    frz_match* out = a.out;
+    uint64_t* n_out = a.n_out;
+    uint64_t* n_total = a.n_total;
     int n_dev = 0;
     if (cudaGetDeviceCount(&n_dev) != cudaSuccess || n_dev == 0) {
         cudaGetLastError();
@@ -2217,25 +2305,33 @@ extern "C" frz_status frz_match_list_batch_collapsed(frz_matcher* const* ms, uin
     const FrzCorpusStorage& cs = corpus->st;
     FRZ_TRY(frz_check_index_range(cs.n, 0));
     for (uint64_t& v : g_batch_last) v = 0;
-    auto subset_of = [&](uint64_t j) { return subsets ? subsets[j] : nullptr; };
-    auto boost_of = [&](uint64_t j) { return boosts ? boosts[j] : nullptr; };
-    auto groups_of = [&](uint64_t j) { return groups ? groups[j] : nullptr; };
-    auto per_group_of = [&](uint64_t j) { return per_group ? per_group[j] : 1; };
-    auto counts_of = [&](uint64_t j) { return group_counts ? group_counts[j] : nullptr; };
+    auto subset_of = [&](uint64_t j) { return a.subsets ? a.subsets[j] : nullptr; };
+    auto boost_of = [&](uint64_t j) { return a.boosts ? a.boosts[j] : nullptr; };
+    auto groups_of = [&](uint64_t j) { return a.groups ? a.groups[j] : nullptr; };
+    auto per_group_of = [&](uint64_t j) { return a.per_group ? a.per_group[j] : 1; };
+    auto counts_of = [&](uint64_t j) { return a.group_counts ? a.group_counts[j] : nullptr; };
+    auto sort_of = [&](uint64_t j) { return bc ? bc->sort : ms[j]->config.sort; };
     auto single = [&](uint64_t j) {
-        return batch_single(ms[j], corpus, subset_of(j), boost_of(j), groups_of(j), per_group_of(j), k, k ? out + j * k : nullptr,
-                            &n_out[j], n_total ? &n_total[j] : nullptr, counts_of(j));
+        frz_match* oj = k ? out + j * k : nullptr;
+        uint64_t* tj = n_total ? &n_total[j] : nullptr;
+        if (bc)
+            return frz_match_list_columns(ms + j * bc->n_cols, bc->cols, bc->n_cols, bc->sort, subset_of(j), boost_of(j), groups_of(j),
+                                          per_group_of(j), k, oj, &n_out[j], tj, counts_of(j));
+        return batch_single(ms[j], corpus, subset_of(j), boost_of(j), groups_of(j), per_group_of(j), k, oj, &n_out[j], tj, counts_of(j));
+    };
+    auto selected = [&](uint64_t j) {
+        return bc ? batch_columns_selected(ms + j * bc->n_cols, *bc) : batchable(ms[j], cs) && batch_selected(ms[j], cs);
     };
     std::vector<uint64_t> batched;
     const uint64_t cap = batch_survivor_cap(cs);
-    const uint64_t base = BatchLayout::per_query(cs, k, cap);
+    const uint64_t list_rows = std::max<uint64_t>(cs.n, 1);
+    const uint64_t base = BatchLayout::per_query(cs, k, cap) + (bc ? frz_batch_columns_bytes(bc->n_cols, list_rows, sizeof(FrzPatternDev)) : 0);
     const uint64_t fit = k <= kFrzBatchMaxK ? kBatchScratchBytes / base : 0;
     const uint64_t qs_max = std::min<uint64_t>(fit, kFrzBatchMaxSub);
-    const uint64_t list_rows = std::max<uint64_t>(cs.n, 1);
     uint64_t n_groups_max = 0;   // the largest n_groups among the batched grouped queries
     for (uint64_t j = 0; j < q; j++) {
         const frz_groups* g = groups_of(j);
-        if (qs_max >= 2 && batchable(ms[j], cs) && batch_selected(ms[j], cs) &&
+        if (qs_max >= 2 && selected(j) &&
             (!g || (frz_batch_collapse_fit(kBatchScratchBytes, base, g->n_groups, list_rows) &&
                     (!counts_of(j) || g->n_groups <= kBatchMaxCountedGroups)))) {
             batched.push_back(j);
@@ -2274,7 +2370,7 @@ extern "C" frz_status frz_match_list_batch_collapsed(frz_matcher* const* ms, uin
         const frz_groups* g = groups_of(j);
         if (!g) continue;
         if (cols.empty()) { cols.resize(q, FrzBatchCollapse()); n_groups.resize(q, 0); }
-        const uint8_t sort = ms[j]->config.sort;
+        const uint8_t sort = sort_of(j);
         FrzBatchCollapse& r = cols[j];
         r.ids = g->ids.get();
         r.n_ids = g->ids.cap();
@@ -2288,13 +2384,13 @@ extern "C" frz_status frz_match_list_batch_collapsed(frz_matcher* const* ms, uin
     if (!cols.empty()) {
         gr.cols = cols.data();
         gr.n_groups = n_groups.data();
-        gr.counts = group_counts;
+        gr.counts = a.group_counts;
     }
     const uint64_t qs_fit = n_groups_max ? std::min<uint64_t>(frz_batch_collapse_fit(kBatchScratchBytes, base, n_groups_max, list_rows),
                                                               kFrzBatchMaxSub)
                                          : qs_max;
     const uint64_t qs = std::min<uint64_t>(qs_fit, batched.size());
-    const BatchLayout L(cs, k, cap, qs, n_groups_max);
+    const BatchLayout L(cs, k, cap, qs, n_groups_max, bc ? bc->n_cols : 0);
     FrzDevArray<uint8_t> scratch;   // released when the call returns
     FRZ_TRY(scratch.reserve(L.bytes));
     if (L.groups)   // the round tables start zero, and every sub-batch's rounds leave them zero
@@ -2304,7 +2400,7 @@ extern "C" frz_status frz_match_list_batch_collapsed(frz_matcher* const* ms, uin
         bool overflow = false;
         FrzLaunchStats st;
         FRZ_TRY(batch_run(ms, scopes.empty() ? nullptr : scopes.data(), gr, batched.data() + s, ns, corpus, k, L, scratch.get(), out,
-                          n_out, n_total, &overflow, st));
+                          n_out, n_total, &overflow, st, bc));
         g_batch_last[overflow ? 1 : 0] += ns;
         g_batch_last[2]++;
         g_batch_last[3] += st.launches;
@@ -2312,6 +2408,89 @@ extern "C" frz_status frz_match_list_batch_collapsed(frz_matcher* const* ms, uin
             for (uint32_t j = 0; j < ns; j++) FRZ_TRY(single(batched[s + j]));
     }
     return FRZ_OK;
+}
+
+}  // namespace
+
+extern "C" frz_status frz_match_list_batch_collapsed(frz_matcher* const* ms, uint64_t q, const frz_corpus* corpus,
+                                                     const frz_subset* const* subsets, const frz_boost* const* boosts,
+                                                     const frz_groups* const* groups, const uint64_t* per_group, uint64_t k,
+                                                     frz_match* out, uint64_t* n_out, uint64_t* n_total, uint32_t* const* group_counts) {
+    if (!ms || !corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    for (uint64_t j = 0; j < q; j++)
+        if (!ms[j]) return frz_fail(FRZ_ERR_INVALID_ARG, "null matcher at %llu", (unsigned long long)j);
+    for (uint64_t j = 0; per_group && j < q; j++) {
+        if (per_group[j] == 0) return frz_fail(FRZ_ERR_INVALID_ARG, "per_group = 0 at %llu", (unsigned long long)j);
+        if (per_group[j] > kFrzCollapseMaxPerGroup && per_group[j] != UINT64_MAX)
+            return frz_fail(FRZ_ERR_UNSUPPORTED, "per_group = %llu at %llu: at most %llu rows per group, or UINT64_MAX for no cap",
+                            (unsigned long long)per_group[j], (unsigned long long)j, (unsigned long long)kFrzCollapseMaxPerGroup);
+    }
+    for (uint64_t j = 0; j < q; j++) {
+        if (subsets && subsets[j] && subsets[j]->corpus != corpus)
+            return frz_fail(FRZ_ERR_INVALID_ARG, "the subset of query %llu was made on another corpus", (unsigned long long)j);
+        if (boosts && boosts[j] && boosts[j]->corpus != corpus)
+            return frz_fail(FRZ_ERR_INVALID_ARG, "the boost of query %llu was made on another corpus", (unsigned long long)j);
+        if (groups && groups[j] && groups[j]->corpus != corpus)
+            return frz_fail(FRZ_ERR_INVALID_ARG, "the groups of query %llu were made on another corpus", (unsigned long long)j);
+    }
+    if (q && !n_out) return frz_fail(FRZ_ERR_INVALID_ARG, "null n_out");
+    if (k && (q > UINT64_MAX / k || q * k > SIZE_MAX / sizeof(frz_match)))
+        return frz_fail(FRZ_ERR_INVALID_ARG, "q * k overflows: q = %llu, k = %llu", (unsigned long long)q, (unsigned long long)k);
+    if (q * k > 0 && !out) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
+    if (q == 0) return FRZ_OK;
+    return batch_drive(BatchCall{ms, q, corpus, nullptr, subsets, boosts, groups, per_group, k, out, n_out, n_total, group_counts});
+}
+
+// Query j is frz_match_list_columns(ms + j * n_cols, cols, n_cols, sort, subsets[j], boosts[j], groups[j], per_group[j], ...);
+// its batched class joins its columns on the device (batch_run, batch_columns.cu).
+extern "C" frz_status frz_match_list_batch_columns(frz_matcher* const* ms, uint64_t q, const frz_corpus* const* cols, uint64_t n_cols,
+                                                   uint8_t sort, const frz_subset* const* subsets, const frz_boost* const* boosts,
+                                                   const frz_groups* const* groups, const uint64_t* per_group, uint64_t k,
+                                                   frz_match* out, uint64_t* n_out, uint64_t* n_total, uint32_t* const* group_counts) {
+    if (n_cols == 0) return frz_fail(FRZ_ERR_INVALID_ARG, "n_cols = 0: a columns call needs at least one column");
+    if (!ms || !cols) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    for (uint64_t c = 0; c < n_cols; c++)
+        if (!cols[c]) return frz_fail(FRZ_ERR_INVALID_ARG, "null corpus of column %llu", (unsigned long long)c);
+    if (q > UINT64_MAX / n_cols || q * n_cols > SIZE_MAX / sizeof(frz_matcher*))
+        return frz_fail(FRZ_ERR_INVALID_ARG, "q * n_cols overflows: q = %llu, n_cols = %llu", (unsigned long long)q, (unsigned long long)n_cols);
+    for (uint64_t i = 0; i < q * n_cols; i++)
+        if (!ms[i])
+            return frz_fail(FRZ_ERR_INVALID_ARG, "null matcher of query %llu, column %llu", (unsigned long long)(i / n_cols),
+                            (unsigned long long)(i % n_cols));
+    const FrzCorpusStorage& first = cols[0]->st;
+    for (uint64_t c = 1; c < n_cols; c++) {
+        if (cols[c]->st.device != first.device)
+            return frz_fail(FRZ_ERR_INVALID_ARG, "column %llu is on device %d, column 0 on device %d", (unsigned long long)c,
+                            cols[c]->st.device, first.device);
+        if (cols[c]->st.n != first.n)
+            return frz_fail(FRZ_ERR_INVALID_ARG, "column %llu holds %llu rows, column 0 holds %llu: the columns must share one index space",
+                            (unsigned long long)c, (unsigned long long)cols[c]->st.n, (unsigned long long)first.n);
+    }
+    FRZ_TRY(frz_check_index_range(first.n, 0));
+    if (sort > FRZ_SORT_INDEX_DESC) return frz_fail(FRZ_ERR_INVALID_ARG, "sort = %u is not a sort strategy", (unsigned)sort);
+    for (uint64_t j = 0; per_group && j < q; j++) {
+        if (per_group[j] == 0) return frz_fail(FRZ_ERR_INVALID_ARG, "per_group = 0 at %llu", (unsigned long long)j);
+        if (per_group[j] > kFrzCollapseMaxPerGroup && per_group[j] != UINT64_MAX)
+            return frz_fail(FRZ_ERR_UNSUPPORTED, "per_group = %llu at %llu: at most %llu rows per group, or UINT64_MAX for no cap",
+                            (unsigned long long)per_group[j], (unsigned long long)j, (unsigned long long)kFrzCollapseMaxPerGroup);
+    }
+    // membership, boosts and group ids are by index, so a handle of any column serves every column
+    const auto of_a_column = [&](const frz_corpus* h) { return std::find(cols, cols + n_cols, h) != cols + n_cols; };
+    for (uint64_t j = 0; j < q; j++) {
+        if (subsets && subsets[j] && !of_a_column(subsets[j]->corpus))
+            return frz_fail(FRZ_ERR_INVALID_ARG, "the subset of query %llu was made on none of the columns", (unsigned long long)j);
+        if (boosts && boosts[j] && !of_a_column(boosts[j]->corpus))
+            return frz_fail(FRZ_ERR_INVALID_ARG, "the boost of query %llu was made on none of the columns", (unsigned long long)j);
+        if (groups && groups[j] && !of_a_column(groups[j]->corpus))
+            return frz_fail(FRZ_ERR_INVALID_ARG, "the groups of query %llu were made on none of the columns", (unsigned long long)j);
+    }
+    if (q && !n_out) return frz_fail(FRZ_ERR_INVALID_ARG, "null n_out");
+    if (k && (q > UINT64_MAX / k || q * k > SIZE_MAX / sizeof(frz_match)))
+        return frz_fail(FRZ_ERR_INVALID_ARG, "q * k overflows: q = %llu, k = %llu", (unsigned long long)q, (unsigned long long)k);
+    if (q * k > 0 && !out) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
+    if (q == 0) return FRZ_OK;
+    const BatchColumns bc{cols, n_cols, sort};
+    return batch_drive(BatchCall{ms, q, cols[0], &bc, subsets, boosts, groups, per_group, k, out, n_out, n_total, group_counts});
 }
 
 extern "C" frz_status frz_match_list_batch_top(frz_matcher* const* ms, uint64_t q, const frz_corpus* corpus, uint64_t k, frz_match* out,

@@ -1059,6 +1059,14 @@ frz_status frz_launch_prefilter_batch(const FrzCorpusView& cv, const FrzBatchDev
     return FRZ_OK;
 }
 
+frz_status frz_launch_tile_scan_batch(const FrzBatchDev& b, uint32_t n_tiles, uint32_t nq, cudaStream_t stream, FrzLaunchStats* st) {
+    if (nq == 0) return FRZ_OK;
+    k_tile_scan_batch<<<nq, 1024, 0, stream>>>(b, n_tiles);
+    FRZ_CUDA_TRY(cudaGetLastError());
+    st->launches++;
+    return FRZ_OK;
+}
+
 frz_status frz_launch_tile_scan(const FrzCorpusView& cv, FrzWorkspace& ws, cudaStream_t stream, FrzLaunchStats* st,
                                 unsigned long long* carry) {
     if (cv.n_tiles) {

@@ -273,14 +273,15 @@ FRZ_API frz_status frz_match_list_top(frz_matcher* m, const frz_corpus* corpus, 
 FRZ_API frz_status frz_match_list_batch_top(frz_matcher* const* ms, uint64_t q, const frz_corpus* corpus, uint64_t k,
                                             frz_match* out, uint64_t* n_out, uint64_t* n_total);
 /* Test aid: the corpus-size and query-count limits of the batched path of frz_match_list_batch_top,
- * frz_match_list_batch and frz_match_list_batch_collapsed, process-wide (0 restores
+ * frz_match_list_batch, frz_match_list_batch_collapsed and frz_match_list_batch_columns, process-wide (0 restores
  * a limit's default: 2^18 rows, 32 queries; max_typos = 0 queries batch up to the larger of max_rows and 2^21 rows;
- * fewer than 2 queries never batch).  Lets tests reach the batched kernels with
+ * fewer than 2 queries never batch).  For frz_match_list_batch_columns, max_rows limits every query, and a query with a
+ * typo budget in some column batches only when max_rows is set (by default it runs frz_match_list_columns).  Lets tests reach the batched kernels with
  * small batches and tools/bench_batch.py time the batched path on both sides of the defaults.  Not for concurrent use with
  * batch calls. */
 FRZ_API void frz_debug_batch_limits(uint64_t max_rows, uint64_t min_queries);
-/* Test aid: what the calling thread's last frz_match_list_batch_top, frz_match_list_batch or
- * frz_match_list_batch_collapsed did: [0] queries answered by
+/* Test aid: what the calling thread's last frz_match_list_batch_top, frz_match_list_batch,
+ * frz_match_list_batch_collapsed or frz_match_list_batch_columns did: [0] queries answered by
  * the batched kernels, [1] queries of sub-batches whose survivor lists overflowed (answered again by their single-query
  * call's pipeline),
  * [2] sub-batches run, [3] kernel launches of the batched path.  All zero after a call that ran no sub-batch. */
@@ -476,6 +477,37 @@ FRZ_API frz_status frz_match_list_batch_collapsed(frz_matcher* const* ms, uint64
                                                   const frz_subset* const* subsets, const frz_boost* const* boosts,
                                                   const frz_groups* const* groups, const uint64_t* per_group, uint64_t k,
                                                   frz_match* out, uint64_t* n_out, uint64_t* n_total, uint32_t* const* group_counts);
+
+/* frz_match_list_columns (above) for q queries over the same columns in one call: a service answering many users'
+ * multi-field searches (file name + directory, command + working directory) over one set of columns.  Query j's matchers
+ * are ms[j*n_cols .. (j+1)*n_cols), matcher c searching cols[c].  For every j < q, out[j*k .. j*k + n_out[j]), n_out[j],
+ * n_total[j] and, when given, group_counts[j] are bit for bit what frz_match_list_columns(ms + j*n_cols, cols, n_cols, sort,
+ * subsets[j], boosts[j], groups[j], per_group[j], k, ..., group_counts[j]) returns; rows out[j*k + n_out[j] .. (j+1)*k)
+ * are not written.  subsets, boosts, groups and group_counts may be NULL, meaning every entry is NULL; per_group may be
+ * NULL, meaning 1 for every query (frz_match_list_batch_collapsed's conventions).  sort is one FRZ_SORT_* value for every
+ * query; the matchers' own sort settings are not read.
+ *
+ * Checked in this order before any device work: FRZ_ERR_INVALID_ARG for n_cols == 0; a NULL ms or cols; a NULL cols[c];
+ * q*n_cols overflowing uint64_t or size_t; a NULL ms[i] for i < q*n_cols; columns on different devices; columns whose
+ * frz_corpus_len differ (after an append to some columns only); then FRZ_ERR_TOO_MANY_ITEMS for more rows than u32 indices
+ * reach; then FRZ_ERR_INVALID_ARG for a sort above 3; per_group[j] 0 (then FRZ_ERR_UNSUPPORTED for a per_group[j] out of
+ * 1 .. 32 other than UINT64_MAX; every entry is checked, with or without groups); a subset, boost or groups handle made on
+ * none of the columns; a NULL n_out with q > 0; q*k overflowing uint64_t or size_t; a NULL out with q*k > 0.  q = 0 then
+ * returns FRZ_OK without any CUDA call.  Never FRZ_ERR_CAPACITY.  A matcher or a column may appear more than once.
+ * Blocking; none of the matchers, columns or handles may be used by another call meanwhile.
+ *
+ * A query runs the batched kernels when every column's matcher either has no compiled pattern or has one pattern that is
+ * fuzzy, not negated, on the byte path and at most 64 bytes long; at least one column has a pattern; every pattern has
+ * max_typos = 0; k <= 1024; there are at most 255 columns; the columns hold at most 2^18 rows; and the call has at least
+ * 32 such queries (frz_debug_batch_limits moves the row and query limits, and lets queries with a typo budget batch too).
+ * DESIGN.md §4.13 measured that rule: queries with a typo budget, and corpora of 1 M rows, lost to the loop there.  Each sub-batch scans every column once for
+ * the queries with a pattern in it and joins the columns per row on the device (DESIGN.md §4.13).  Grouped queries
+ * follow frz_match_list_batch_collapsed's rules.  Every other query, and every query of a sub-batch whose survivor lists
+ * overflowed, runs frz_match_list_columns inside the same call. */
+FRZ_API frz_status frz_match_list_batch_columns(frz_matcher* const* ms, uint64_t q, const frz_corpus* const* cols, uint64_t n_cols,
+                                                uint8_t sort, const frz_subset* const* subsets, const frz_boost* const* boosts,
+                                                const frz_groups* const* groups, const uint64_t* per_group, uint64_t k,
+                                                frz_match* out, uint64_t* n_out, uint64_t* n_total, uint32_t* const* group_counts);
 
 /* Specialized::match_list / Matcher::match_list_into (src/matcher/algo.rs:17-22,
  * src/matcher/mod.rs:373-392): matches appended in input (index-ascending) order,
