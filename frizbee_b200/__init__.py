@@ -16,12 +16,13 @@ import numpy as np
 from .types import (CaseMatching, CConfig, CMatch, Config, CPattern, Match, Matching, Pattern, Scoring,
                     SortStrategy, UnicodeMatching, as_pattern, pattern_array)
 
-__all__ = ["Matcher", "Corpus", "Subset", "Boost", "Groups", "GROUP_NONE", "Pattern", "Config", "Scoring", "Match", "SortStrategy", "CaseMatching",
+__all__ = ["Matcher", "Corpus", "Subset", "Boost", "Groups", "GROUP_NONE", "Attr", "Where", "ATTR_NULL", "Pattern", "Config", "Scoring", "Match", "SortStrategy", "CaseMatching",
            "UnicodeMatching", "Matching", "FrizbeeError", "parse_query", "parse_atom", "radix_sort_matches",
            "MATCH_DTYPE", "lib", "lib_path"]
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 GROUP_NONE = 0xFFFFFFFF   # FRZ_GROUP_NONE: a row in no group
+ATTR_NULL = -(2**63)      # FRZ_ATTR_NULL: a row with no value for an attribute
 _U64_MAX = 0xFFFFFFFFFFFFFFFF   # UINT64_MAX: no k limit / no per-group cap
 MATCH_DTYPE = np.dtype([("index", "<u4"), ("score", "<u2"), ("exact", "u1"), ("_pad", "u1")])
 
@@ -107,6 +108,11 @@ def lib():
     L.frz_subset_destroy.restype = None
     L.frz_match_list_subset.argtypes = [vp, vp, vp, vp, u64, C.POINTER(u64)]
     L.frz_match_list_subset_top.argtypes = [vp, vp, vp, u64, vp, C.POINTER(u64), C.POINTER(u64)]
+    L.frz_attr_create.argtypes = [vp, vp, u64, C.POINTER(vp)]
+    L.frz_attr_set.argtypes = [vp, vp, vp, u64]
+    L.frz_attr_destroy.argtypes = [vp]
+    L.frz_attr_destroy.restype = None
+    L.frz_subset_where.argtypes = [vp, vp, u64, vp]
     L.frz_boost_create.argtypes = [vp, vp, u64, C.POINTER(vp)]
     L.frz_boost_set.argtypes = [vp, vp, vp, u64]
     L.frz_boost_destroy.argtypes = [vp]
@@ -272,6 +278,19 @@ class Corpus:
         _check(lib().frz_subset_create(self._h, which.ctypes.data if which.size else None, len(which), C.byref(h)))
         return Subset(h, self)
 
+    def attr(self, values=None) -> "Attr":
+        """A resident int64 attribute per row for Corpus.where / Subset.where: values[i] is the value of row i, rows past
+        len(values) (and values equal to ATTR_NULL) have none; at most len(self) values.  Close it before the corpus."""
+        values = np.ascontiguousarray(np.zeros(0, np.int64) if values is None else values, dtype=np.int64)
+        h = C.c_void_p()
+        _check(lib().frz_attr_create(self._h, values.ctypes.data if values.size else None, len(values), C.byref(h)))
+        return Attr(h, self)
+
+    def where(self, *clauses: "Where", base: Optional["Subset"] = None) -> "Subset":
+        """A new subset of the rows for which every clause holds (and which are members of `base`, when given), filled on
+        the device (frz_subset_where).  Close it before the corpus."""
+        return self.subset([]).where(*clauses, base=base)
+
     def boost(self, values=None) -> "Boost":
         """A resident per-row boost for Matcher.match_list_ranked_array: values[i] (int16) is the boost of row i, rows
         past len(values) have 0; at most len(self) values.  Close it before the corpus."""
@@ -325,6 +344,19 @@ class Subset:
     def __len__(self):
         return lib().frz_subset_len(self._h)
 
+    def where(self, *clauses: "Where", base: Optional["Subset"] = None) -> "Subset":
+        """Refills this subset with the rows of its corpus for which every clause holds and which are members of `base`
+        (when given; it may be this subset), on the device (frz_subset_where).  Returns self."""
+        arr = (_CWhereClause * max(1, len(clauses)))()
+        for j, w in enumerate(clauses):
+            arr[j].attr = w.attr._h
+            arr[j].lo, arr[j].hi = w.lo, w.hi
+            arr[j].in_ = w.values.ctypes.data if w.values is not None and w.values.size else None
+            arr[j].n_in = 0 if w.values is None else len(w.values)
+            arr[j].negate = int(w.negate)
+        _check(lib().frz_subset_where(self._h, arr if clauses else None, len(clauses), base._h if base is not None else None))
+        return self
+
     def close(self):
         if self._h:
             lib().frz_subset_destroy(self._h)
@@ -357,6 +389,62 @@ class Boost:
     def close(self):
         if self._h:
             lib().frz_boost_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class _CWhereClause(C.Structure):
+    _fields_ = [("attr", C.c_void_p), ("lo", C.c_int64), ("hi", C.c_int64), ("in_", C.c_void_p), ("n_in", C.c_uint64),
+                ("negate", C.c_int32)]
+
+
+class Where:
+    """One clause of Corpus.where / Subset.where (frz_where_clause): lo <= v <= hi, or v in values, v being a row's value in
+    `attr`; ~clause holds where the test fails.  A row without a value fails every clause, negated or not."""
+
+    def __init__(self, attr: "Attr", lo: int = 0, hi: int = -1, values=None, negate: bool = False):
+        self.attr, self.lo, self.hi, self.negate = attr, int(lo), int(hi), bool(negate)
+        self.values = None if values is None else np.ascontiguousarray(values, dtype=np.int64)
+
+    def __invert__(self) -> "Where":
+        return Where(self.attr, self.lo, self.hi, self.values, not self.negate)
+
+
+class Attr:
+    """A signed 64-bit value per row of one resident Corpus (frz_attr), kept by index across corpus edits."""
+
+    def __init__(self, handle, corpus: Corpus):
+        self._h = handle
+        self.corpus = corpus
+
+    def set(self, which, values) -> "Attr":
+        """value[which[j]] = values[j] (ATTR_NULL clears it); any row below len(corpus), appended ones included, each at
+        most once."""
+        which = np.ascontiguousarray(which, dtype=np.uint32)
+        values = np.ascontiguousarray(values, dtype=np.int64)
+        if len(values) != len(which):
+            raise ValueError(f"{len(which)} indices need {len(which)} values, got {len(values)}")
+        _check(lib().frz_attr_set(self._h, which.ctypes.data if which.size else None,
+                                  values.ctypes.data if values.size else None, len(which)))
+        return self
+
+    def between(self, lo: int, hi: int) -> Where:
+        """The clause lo <= v <= hi (it holds for no value when lo > hi)."""
+        return Where(self, lo, hi)
+
+    def isin(self, values) -> Where:
+        """The clause "v is one of values" (any order, duplicates allowed; an empty list holds for no value)."""
+        values = np.ascontiguousarray(values, dtype=np.int64)
+        return Where(self, values=values) if values.size else Where(self, 0, -1)
+
+    def close(self):
+        if self._h:
+            lib().frz_attr_destroy(self._h)
             self._h = None
 
     def __del__(self):

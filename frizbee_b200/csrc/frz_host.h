@@ -442,6 +442,13 @@ struct FrzCollapseDev {
 frz_status frz_launch_collapse(const FrzCollapseDev& c, const FrzMatchDev* list, const unsigned long long* n_ptr, uint64_t n_cap,
                                uint64_t n_groups, uint32_t rounds, cudaStream_t stream, FrzLaunchStats* st);
 
+// The fill of frz_subset_where (host.cu; the rule and FrzWhereDev are where_plan.cuh's).
+struct FrzWhereDev;
+// where.cu: w.bits and w.chunk_count from the clauses and the base (k_where)
+frz_status frz_launch_where(const FrzWhereDev& w, cudaStream_t stream);
+// where.cu: the members of bits[0 .. ceil(n / 32)) in ascending order, chunk c's from members[chunk_base[c]] (k_where_members)
+frz_status frz_launch_where_members(const uint32_t* bits, uint64_t n, const uint64_t* chunk_base, uint32_t* members, cudaStream_t stream);
+
 // k-way merge of per-shard runs (merge.cu) with caller-owned scratch — one per concurrent user (parallel.cu: one per rank)
 #define FRZ_MERGE_MAX_RUNS 64
 struct FrzMergeScratch {

@@ -27,6 +27,7 @@
 #include "frz_host.h"
 #include "unicode_needle.h"
 #include "indices_path.cuh"
+#include "where_plan.cuh"
 
 // ------------------------------------------------------------------------------------ errors
 
@@ -1891,6 +1892,11 @@ struct frz_subset {
     FrzDevArray<uint32_t> members;   // n_members ascending indices on the corpus's device (list form)
     uint64_t n_bits;
     uint64_t n_members;              // distinct members
+    // frz_subset_where's grow-only scratch
+    FrzDevArray<uint32_t> chunk_count;      // members per chunk of kFrzWhereChunk indices
+    FrzDevArray<uint64_t> chunk_base;       // their exclusive scan
+    FrzDevArray<FrzCounters> counters;      // ->total: the member count k_scan_blocks leaves
+    FrzDevArray<int64_t> sets;              // every set clause's sorted distinct values
 };
 
 extern "C" frz_status frz_subset_create(const frz_corpus* c, const uint32_t* which, uint64_t n, frz_subset** out) {
@@ -1984,6 +1990,160 @@ extern "C" frz_status frz_match_list_subset_top(frz_matcher* m, const frz_corpus
     SubsetScope scope;
     FRZ_TRY(subset_scope(m, corpus, *s, nullptr, &scope));
     return match_list_host(m, corpus, 0, m->config.sort, k, scope, out, k, n_out, n_total);
+}
+
+// ---------------------------------------------------------------------------------- subsets from attributes
+static_assert(kFrzAttrNull == FRZ_ATTR_NULL && kFrzWhereMaxClauses == FRZ_WHERE_MAX_CLAUSES && kFrzWhereMaxIn == FRZ_WHERE_MAX_IN,
+              "where_plan.cuh mirrors frz_cuda.h");
+
+// A signed 64-bit value per index of one corpus, on its device.  Indices at and past `values.cap()` are null.
+struct frz_attr {
+    const frz_corpus* corpus;
+    FrzDevArray<int64_t> values;
+};
+
+namespace {
+// (index, value) pairs: x is the index
+__global__ void k_attr_scatter(const longlong2* __restrict__ set, uint64_t n, int64_t* __restrict__ values) {
+    for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x)
+        values[set[j].x] = set[j].y;
+}
+
+__global__ void k_attr_fill_null(int64_t* __restrict__ values, uint64_t from, uint64_t to) {
+    for (uint64_t i = from + (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < to; i += (uint64_t)gridDim.x * blockDim.x)
+        values[i] = kFrzAttrNull;
+}
+
+// a->values grows to `n` entries, the old values kept and the new ones null (FrzDevArray drops its contents when it grows,
+// and FRZ_ATTR_NULL is no byte pattern cudaMemset can write)
+frz_status grow_attr(frz_attr* a, uint64_t n) {
+    const uint64_t old = a->values.cap();
+    if (old >= n) return FRZ_OK;
+    FrzDevArray<int64_t> grown;
+    FRZ_TRY(grown.reserve(n));
+    k_attr_fill_null<<<grid_for(n - old, 256), 256>>>(grown.get(), old, n);
+    FRZ_CUDA_TRY(cudaGetLastError());
+    if (old) FRZ_CUDA_TRY(cudaMemcpy(grown.get(), a->values.get(), old * sizeof(int64_t), cudaMemcpyDeviceToDevice));
+    FRZ_CUDA_TRY(cudaStreamSynchronize(nullptr));
+    a->values = std::move(grown);
+    return FRZ_OK;
+}
+
+// The device work of frz_subset_where once every argument has passed: k_where writes the bitmap and the chunk counts,
+// k_scan_blocks scans the counts, one 8-byte read-back gives the member count, and k_where_members writes the list.  The
+// bitmap is written in place unless it must grow; then into a new array, because `base` may be s's old bitmap.
+frz_status where_fill(frz_subset* s, FrzWhereDev& w, const std::vector<int64_t>& sets, const frz_subset* base) {
+    const uint64_t n = s->corpus->st.n;
+    w.has_base = base != nullptr;   // (read before s is emptied: base may be s)
+    w.base = base ? base->bits.get() : nullptr;
+    w.n_base = base ? base->n_bits : 0;
+    s->n_bits = 0;   // empty until the fill completes
+    s->n_members = 0;
+    if (n == 0) return FRZ_OK;
+    const uint64_t n_words = (n + 31) / 32, n_chunks = (n + kFrzWhereChunk - 1) / kFrzWhereChunk;
+    FRZ_TRY(s->chunk_count.reserve(n_chunks));
+    FRZ_TRY(s->chunk_base.reserve(n_chunks));
+    FRZ_TRY(s->counters.reserve(1));
+    if (!sets.empty()) {
+        FRZ_TRY(s->sets.reserve(sets.size(), std::max<uint64_t>(sets.size(), 64)));
+        FRZ_CUDA_TRY(cudaMemcpy(s->sets.get(), sets.data(), sets.size() * sizeof(int64_t), cudaMemcpyHostToDevice));
+    }
+    FrzDevArray<uint32_t> grown;
+    if (s->bits.cap() < n_words) FRZ_TRY(grown.reserve(n_words));
+    w.sets = s->sets.get();
+    w.n_sets = (uint32_t)sets.size();
+    w.bits = grown.get() ? grown.get() : s->bits.get();
+    w.chunk_count = s->chunk_count.get();
+    w.n = n;
+    FRZ_TRY(frz_launch_where(w, nullptr));
+    k_scan_blocks<<<1, 1024>>>(s->chunk_count.get(), s->chunk_base.get(), (uint32_t)n_chunks, s->counters.get());
+    FRZ_CUDA_TRY(cudaGetLastError());
+    uint64_t total = 0;
+    FRZ_CUDA_TRY(cudaMemcpy(&total, &s->counters.get()->total, sizeof(total), cudaMemcpyDeviceToHost));
+    if (grown.get()) s->bits = std::move(grown);
+    if (total) {
+        FRZ_TRY(s->members.reserve(total));
+        FRZ_TRY(frz_launch_where_members(s->bits.get(), n, s->chunk_base.get(), s->members.get(), nullptr));
+        FRZ_CUDA_TRY(cudaStreamSynchronize(nullptr));
+    }
+    s->n_bits = n;
+    s->n_members = total;
+    return FRZ_OK;
+}
+}  // namespace
+
+extern "C" frz_status frz_attr_create(const frz_corpus* c, const int64_t* values, uint64_t n, frz_attr** out) {
+    if (!c || !out || (n && !values)) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    if (n > c->st.n)
+        return frz_fail(FRZ_ERR_INVALID_ARG, "%llu attribute values for a corpus of %llu haystacks", (unsigned long long)n,
+                        (unsigned long long)c->st.n);
+    auto a = std::make_unique<frz_attr>();
+    a->corpus = c;
+    if (n) {
+        FRZ_TRY(frz_ensure_device(c->st.device));
+        FRZ_TRY(a->values.reserve(n));
+        FRZ_CUDA_TRY(cudaMemcpy(a->values.get(), values, n * sizeof(int64_t), cudaMemcpyHostToDevice));
+    }
+    *out = a.release();
+    return FRZ_OK;
+}
+
+extern "C" frz_status frz_attr_set(frz_attr* a, const uint32_t* which, const int64_t* values, uint64_t n) {
+    if (!a || (n && (!which || !values))) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    if (n == 0) return FRZ_OK;
+    FRZ_TRY(check_indices(a->corpus, which, n));
+    std::vector<uint32_t> sorted(which, which + n);
+    std::sort(sorted.begin(), sorted.end());
+    for (uint64_t j = 1; j < n; j++)
+        if (sorted[j] == sorted[j - 1]) return frz_fail(FRZ_ERR_INVALID_ARG, "index %u is set twice", sorted[j]);
+    std::vector<longlong2> set(n);
+    for (uint64_t j = 0; j < n; j++) set[j] = make_longlong2((long long)which[j], (long long)values[j]);
+    FRZ_TRY(frz_ensure_device(a->corpus->st.device));
+    if (sorted.back() >= a->values.cap()) FRZ_TRY(grow_attr(a, a->corpus->st.n));
+    FrzDevArray<longlong2> d_set;   // (index, value) pairs: one copy, one scatter
+    FRZ_TRY(d_set.reserve(n));
+    FRZ_CUDA_TRY(cudaMemcpy(d_set.get(), set.data(), n * sizeof(longlong2), cudaMemcpyHostToDevice));
+    k_attr_scatter<<<grid_for(n, 256), 256>>>(d_set.get(), n, a->values.get());
+    FRZ_CUDA_TRY(cudaGetLastError());
+    FRZ_CUDA_TRY(cudaStreamSynchronize(nullptr));
+    return FRZ_OK;
+}
+
+extern "C" void frz_attr_destroy(frz_attr* a) { delete a; }
+
+extern "C" frz_status frz_subset_where(frz_subset* s, const frz_where_clause* clauses, uint64_t n_clauses, const frz_subset* base) {
+    if (!s || (n_clauses && !clauses)) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    if (n_clauses > FRZ_WHERE_MAX_CLAUSES)
+        return frz_fail(FRZ_ERR_UNSUPPORTED, "%llu clauses (at most %d)", (unsigned long long)n_clauses, FRZ_WHERE_MAX_CLAUSES);
+    uint64_t n_in = 0;
+    for (uint64_t j = 0; j < n_clauses; j++) {
+        if (!clauses[j].attr || (clauses[j].n_in && !clauses[j].in)) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument in clause %llu", (unsigned long long)j);
+        n_in += std::min<uint64_t>(clauses[j].n_in, (uint64_t)FRZ_WHERE_MAX_IN + 1);   // (no overflow)
+    }
+    if (n_in > FRZ_WHERE_MAX_IN) return frz_fail(FRZ_ERR_UNSUPPORTED, "more than %d set values", FRZ_WHERE_MAX_IN);
+    for (uint64_t j = 0; j < n_clauses; j++)
+        for (uint64_t v = 0; v < clauses[j].n_in; v++)
+            if (clauses[j].in[v] == FRZ_ATTR_NULL)
+                return frz_fail(FRZ_ERR_INVALID_ARG, "set value %llu of clause %llu is FRZ_ATTR_NULL", (unsigned long long)v, (unsigned long long)j);
+    for (uint64_t j = 0; j < n_clauses; j++)
+        if (clauses[j].attr->corpus != s->corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "the attribute was made on another corpus");
+    if (base && base->corpus != s->corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "the base subset was made on another corpus");
+    FrzWhereDev w = {};
+    std::vector<int64_t> sets;
+    for (uint64_t j = 0; j < n_clauses; j++) {
+        const frz_where_clause& cl = clauses[j];
+        FrzWhereClauseDev& d = w.clauses[j];
+        d.values = cl.attr->values.get();
+        d.n_values = cl.attr->values.cap();
+        d.lo = cl.lo;
+        d.hi = cl.hi;
+        d.in_off = (uint32_t)sets.size();
+        d.n_in = cl.n_in ? frz_where_pack_set(cl.in, cl.n_in, sets) : 0;
+        d.negate = cl.negate != 0;
+    }
+    w.n_clauses = (uint32_t)n_clauses;
+    FRZ_TRY(frz_ensure_device(s->corpus->st.device));
+    return where_fill(s, w, sets, base);
 }
 
 // ---------------------------------------------------------------------------------- ranked calls

@@ -321,6 +321,62 @@ FRZ_API frz_status frz_match_list_subset(frz_matcher* m, const frz_corpus* corpu
 FRZ_API frz_status frz_match_list_subset_top(frz_matcher* m, const frz_corpus* corpus, const frz_subset* s, uint64_t k,
                                              frz_match* out, uint64_t* n_out, uint64_t* n_total);
 
+/* ---------------------------------------------------------------- subsets from attributes
+ *
+ * A filter on structured fields of the rows that changes with every request: a shell history searched "from the last 7
+ * days, exit status != 0, on this host", a file picker searched "*.rs or *.toml, modified since yesterday", a launcher
+ * searched "in these three categories".  The reference has no such method: its callers filter the haystacks themselves
+ * before Matcher::match_list (src/matcher/mod.rs:212).  Here the fields stay resident beside the corpus as attribute
+ * handles, and frz_subset_where fills an ordinary subset from a conjunction of clauses over them on the device, so every
+ * call that takes a subset (the subset, ranked, collapsed, column and batched calls) filters without any change.
+ *
+ * An attribute is a signed 64-bit value per index of a corpus, resident on the corpus's device; FRZ_ATTR_NULL, and every
+ * index without a value, is "no value", which never satisfies a clause, negated or not.  It follows frz_boost's rules: it
+ * belongs to the corpus it was made on (another corpus is FRZ_ERR_INVALID_ARG, and it must be destroyed before that
+ * corpus), and values are kept by index across corpus edits: a removed row keeps its value, a replaced row keeps its
+ * value, and rows appended after frz_attr_create are null until frz_attr_set gives them a value.
+ *
+ * To filter per request, create an empty subset once (frz_subset_create(c, NULL, 0, &s)) and refill it with
+ * frz_subset_where: its device buffers only grow, so steady-state requests allocate nothing. */
+#define FRZ_ATTR_NULL INT64_MIN          /* "no value": never satisfies a clause, negated or not */
+#define FRZ_WHERE_MAX_CLAUSES 8
+#define FRZ_WHERE_MAX_IN 4096            /* set values over all clauses of one call */
+typedef struct frz_attr frz_attr;
+/* The reference has no such method (see above).  values[i] is the value of index i for i < n; the others are null.
+ * n > frz_corpus_len(c), or NULL values with n > 0, is FRZ_ERR_INVALID_ARG; n == 0 is an all-null attribute. */
+FRZ_API frz_status frz_attr_create(const frz_corpus* c, const int64_t* values, uint64_t n, frz_attr** out);
+/* The reference has no such method (see above).  value[which[j]] = values[j] for j < n (FRZ_ATTR_NULL clears a value).
+ * An index >= frz_corpus_len(c) at the time of the call (rows appended since creation may be set), a duplicate index, or
+ * NULL arrays with n > 0 is FRZ_ERR_INVALID_ARG; every argument is checked before anything changes, so a refused call
+ * leaves the attribute as it was.  n == 0 does nothing.  Synchronous; it must not run concurrently with a
+ * frz_subset_where reading a. */
+FRZ_API frz_status frz_attr_set(frz_attr* a, const uint32_t* which, const int64_t* values, uint64_t n);
+FRZ_API void frz_attr_destroy(frz_attr* a);
+
+/* One clause of frz_subset_where over v, an index's value in `attr`. */
+typedef struct frz_where_clause {
+    const frz_attr* attr;
+    int64_t lo, hi;          /* range clause (n_in == 0): lo <= v <= hi  (lo > hi: holds for no value) */
+    const int64_t* in;       /* set clause (n_in > 0): v is one of in[0..n_in), any order, duplicates allowed */
+    uint64_t n_in;
+    int32_t negate;          /* nonzero: the clause holds where its test fails (still never for a null value) */
+} frz_where_clause;
+
+/* The reference has no such method (see above).  Replaces the contents of s, which keeps its corpus c: afterwards s holds
+ * exactly the indices i < frz_corpus_len(c) that are members of `base` (when base is not NULL; indices at or beyond its
+ * bitmap's length are not members) and for which every clause holds.  n_clauses == 0 selects every index, restricted to
+ * base.  Removed rows are included as frz_subset_create includes them: frz_subset_len counts them and the match calls
+ * skip them.  For every call that takes a subset, the filled s behaves bit for bit like frz_subset_create(c, <those
+ * indices>).  base may be s itself (refining in place).  Synchronous: it returns after the member count is read back.  It
+ * must not run concurrently with a call that reads s or base.
+ *
+ * Checked in this order before any device work, leaving s as it was: a NULL s, or NULL clauses with n_clauses > 0
+ * (FRZ_ERR_INVALID_ARG); more than FRZ_WHERE_MAX_CLAUSES clauses (FRZ_ERR_UNSUPPORTED); a NULL attr, or NULL in with
+ * n_in > 0 (FRZ_ERR_INVALID_ARG); more than FRZ_WHERE_MAX_IN set values in all (FRZ_ERR_UNSUPPORTED); a set value equal
+ * to FRZ_ATTR_NULL (FRZ_ERR_INVALID_ARG); an attribute or base of another corpus (FRZ_ERR_INVALID_ARG).  A failure after
+ * the checks (out of device memory, for example) leaves s as the empty set, never half-written. */
+FRZ_API frz_status frz_subset_where(frz_subset* s, const frz_where_clause* clauses, uint64_t n_clauses, const frz_subset* base);
+
 /* ---------------------------------------------------------------- ranked calls
  *
  * Completion menus, history searches and file pickers rank rows by the fuzzy score plus a per-row prior (frecency,
