@@ -13,10 +13,10 @@ from typing import Iterable, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 
-from .types import (CaseMatching, CConfig, CMatch, Config, CPattern, Match, Matching, Pattern, Scoring,
+from .types import (CaseMatching, CConfig, CMatch, Config, CPattern, Match, Matching, Order, Pattern, Scoring,
                     SortStrategy, UnicodeMatching, as_pattern, pattern_array)
 
-__all__ = ["Matcher", "Corpus", "Subset", "Boost", "Groups", "GROUP_NONE", "Attr", "Where", "ATTR_NULL", "Pattern", "Config", "Scoring", "Match", "SortStrategy", "CaseMatching",
+__all__ = ["Matcher", "Corpus", "Subset", "Boost", "Groups", "GROUP_NONE", "Attr", "Where", "ATTR_NULL", "Pattern", "Config", "Scoring", "Match", "SortStrategy", "Order", "CaseMatching",
            "UnicodeMatching", "Matching", "FrizbeeError", "parse_query", "parse_atom", "radix_sort_matches",
            "MATCH_DTYPE", "lib", "lib_path"]
 
@@ -118,6 +118,7 @@ def lib():
     L.frz_boost_destroy.argtypes = [vp]
     L.frz_boost_destroy.restype = None
     L.frz_match_list_ranked.argtypes = [vp, vp, vp, vp, u64, vp, C.POINTER(u64), C.POINTER(u64)]
+    L.frz_match_list_ordered.argtypes = [vp, vp, vp, vp, vp, u32, u64, vp, C.POINTER(u64), C.POINTER(u64)]
     L.frz_groups_create.argtypes = [vp, vp, u64, u64, C.POINTER(vp)]
     L.frz_groups_set.argtypes = [vp, vp, vp, u64]
     L.frz_groups_count.restype = u64
@@ -609,6 +610,26 @@ class Matcher:
         n, total = C.c_uint64(), C.c_uint64()
         _check(lib().frz_match_list_ranked(self._h, corpus._h, subset._h if subset is not None else None, boost._h, k,
                                            out.ctypes.data, C.byref(n), C.byref(total)))
+        return out[: n.value], total.value
+
+    def match_list_ordered_array(self, corpus: Corpus, attr: Attr, order: Order = Order.AttrDesc, k: Optional[int] = None,
+                                 subset: Optional[Subset] = None, boost: Optional[Boost] = None,
+                                 out: Optional[np.ndarray] = None) -> Tuple[np.ndarray, int]:
+        """The rows of match_list_array(corpus) (or of its subset) ordered by attr (frz_match_list_ordered): by value
+        (Order.AttrDesc / AttrAsc) or by score, clamp(score + boost[index], 0, 65535) with a boost, then by value
+        (ScoreThenAttrDesc / Asc); rows without a value go last, and remaining ties keep the strategy's index order.
+        Truncated to the first k: (array of min(k, total) rows, total).  k=None orders the whole list.  `out` (optional)
+        needs room for min(k, len(corpus), len(subset)) rows."""
+        k = _U64_MAX if k is None else int(k)
+        need = min(k, corpus.n, len(subset) if subset is not None else corpus.n)
+        if out is None:
+            out = np.empty(max(1, need), dtype=MATCH_DTYPE)
+        elif len(out) < need:
+            raise ValueError(f"out holds {len(out)} matches; this ordered call needs {need}")
+        n, total = C.c_uint64(), C.c_uint64()
+        _check(lib().frz_match_list_ordered(self._h, corpus._h, subset._h if subset is not None else None,
+                                            boost._h if boost is not None else None, attr._h, int(order), k, out.ctypes.data,
+                                            C.byref(n), C.byref(total)))
         return out[: n.value], total.value
 
     def match_list_collapsed_array(self, corpus: Corpus, groups: Groups, k: Optional[int] = None,

@@ -11,6 +11,7 @@
 
 #include "../../include/frz_cuda.h"
 #include "frz_device.cuh"
+#include "order_plan.cuh"
 #include "unicode_path.cuh"
 
 frz_status frz_fail(frz_status s, const char* fmt, ...);
@@ -274,6 +275,12 @@ struct FrzWorkspace {
     FrzDevArray<uint32_t> collapse_counts;  // [n_groups] collapsed call: the list's rows per group
     FrzDevArray<unsigned long long> collapse_best;  // [n_groups] its round table, all zero between calls
     FrzDevArray<uint8_t> collapse_taken;    // [corpus length] its rows taken in a round
+    FrzDevArray<FrzOrderKey> order_keys;    // [list rows] ordered call: the order key of each list row
+    FrzDevArray<uint32_t> order_cand;       // [2 * list rows] its select's candidate positions (two pass parities)
+    FrzDevArray<uint32_t> order_sel;        // [list rows] its selected positions
+    FrzDevArray<uint32_t> order_hist;       // [kFrzOrderBins] a select pass's digit counts, zero between passes
+    FrzDevArray<FrzOrderState> order_state;
+    FrzPinnedArray<FrzOrderState> h_order_state;
     FrzEvent ev[4];                         // call start, scan done, scoring done, call end
     bool ev_rec[4] = {false, false, false, false};  // recorded during the current call
 };
@@ -448,6 +455,30 @@ struct FrzWhereDev;
 frz_status frz_launch_where(const FrzWhereDev& w, cudaStream_t stream);
 // where.cu: the members of bits[0 .. ceil(n / 32)) in ascending order, chunk c's from members[chunk_base[c]] (k_where_members)
 frz_status frz_launch_where_members(const uint32_t* bits, uint64_t n, const uint64_t* chunk_base, uint32_t* members, cudaStream_t stream);
+
+// The ordered call (host.cu, DESIGN.md §4.15; the key and the pick are order_plan.cuh's), all asynchronous on `stream`.
+// order.cu: zero *st, then the key of each of the *n_ptr list rows (n_cap bounds it) → keys, and st's n and bit masks
+frz_status frz_launch_order_keys(const FrzMatchDev* list, const unsigned long long* n_ptr, uint64_t n_cap, const FrzOrderDev& o,
+                                 FrzOrderKey* keys, FrzOrderState* st, cudaStream_t stream, FrzLaunchStats* ls);
+// order.cu: the select of the `need` rows of largest key among the n = st->n list rows, over the digits shifts[0 ..
+// n_shifts) (most significant first; frz_order_digits), as frz_order_pick with `fit`: their positions → sel, their number
+// → st->n_sel.  hist: zero; cand: 2 * n entries.
+frz_status frz_launch_order_select(const FrzOrderKey* keys, FrzOrderState* st, uint32_t* hist, uint32_t* cand, uint32_t* sel,
+                                   uint64_t n, uint64_t need, const uint32_t* shifts, uint32_t n_shifts, uint64_t fit,
+                                   cudaStream_t stream, FrzLaunchStats* ls);
+// order.cu: the *n_ptr (<= kFrzOrderBlockRows) rows at positions sel[..] of list (sel null: positions 0 ..) sorted by key
+// in one block; the first `limit` → out
+frz_status frz_launch_order_sort_block(const FrzMatchDev* list, const FrzOrderKey* keys, const uint32_t* sel,
+                                       const unsigned long long* n_ptr, uint32_t limit, FrzMatchDev* out, cudaStream_t stream,
+                                       FrzLaunchStats* ls);
+// order.cu: out[j] = list[sel[j]] for j < *n_ptr (<= n_cap)
+frz_status frz_launch_order_gather(const FrzMatchDev* list, const uint32_t* sel, const unsigned long long* n_ptr, uint64_t n_cap,
+                                   FrzMatchDev* out, cudaStream_t stream, FrzLaunchStats* ls);
+// sort.cu: the *n_ptr rows at d_in sorted by descending order key, LSD over shifts[0 .. n_shifts) in reverse (n_shifts >= 1,
+// every digit in which two rows differ); the first `limit` land in d_out.  d_tmp: scratch of the same size.
+frz_status frz_launch_sort_by_order_dev(const FrzMatchDev* d_in, FrzMatchDev* d_tmp, FrzMatchDev* d_out, const unsigned long long* n_ptr,
+                                        const FrzOrderDev& o, const uint32_t* shifts, uint32_t n_shifts, FrzSortScratch& ss,
+                                        cudaStream_t stream, FrzLaunchStats* st, uint32_t limit = kFrzNoLimit);
 
 // k-way merge of per-shard runs (merge.cu) with caller-owned scratch — one per concurrent user (parallel.cu: one per rank)
 #define FRZ_MERGE_MAX_RUNS 64

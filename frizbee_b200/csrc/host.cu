@@ -1457,20 +1457,87 @@ frz_status collapse_list(frz_matcher* m, const FrzCorpusStorage& cs, const Colla
     return FRZ_OK;
 }
 
+// The attribute of an ordered call (frz_match_list_ordered): the list is sorted by its order key (order_plan.cuh).
+struct Ordering {
+    FrzOrderDev dev;   // the attribute, the boost (n_boost == 0: none), the order; `reversed` is set by the call
+};
+
+// The ordered call's steps after the list (DESIGN.md §4.15), in place of the sort: the list's length is read back first (a
+// survivor-list overflow returns kRetryOverflow there), then the keys are computed and their varying bits read back, and
+// the select narrows the list to its first `limit` rows (skipped when they are all of it).  A selection of at most
+// kFrzOrderBlockRows rows is sorted by one block, a larger one by the LSD histogram-kernel sort.  *d_list then points at
+// the first min(limit, total) rows in order.
+frz_status order_list(frz_matcher* m, const FrzCorpusStorage& cs, const Ordering& ord, bool reversed, uint32_t limit,
+                      FrzMatchDev** d_list, cudaStream_t stream, FrzLaunchStats* st) {
+    FrzWorkspace& ws = m->ws;
+    FRZ_TRY(read_counters(m, stream));
+    const uint64_t n = ws.h_counters.get()->total;
+    if (n <= 1 || limit == 0) return FRZ_OK;   // nothing to order, or nothing to return
+    FRZ_TRY(ws.order_keys.reserve(n));
+    FRZ_TRY(ws.order_state.reserve(1));
+    FRZ_TRY(ws.h_order_state.reserve(1));
+    FrzOrderDev o = ord.dev;
+    o.reversed = reversed;
+    FrzOrderState* dst = ws.order_state.get();
+    const unsigned long long* n_ptr = &ws.counters.get()->total;
+    FRZ_TRY(frz_launch_order_keys(*d_list, n_ptr, n, o, ws.order_keys.get(), dst, stream, st));
+    FRZ_CUDA_TRY(cudaMemcpyAsync(ws.h_order_state.get(), dst, sizeof(FrzOrderState), cudaMemcpyDeviceToHost, stream));
+    FRZ_CUDA_TRY(cudaStreamSynchronize(stream));
+    const FrzOrderState& h = *ws.h_order_state.get();
+    uint32_t shifts[kFrzOrderMaxDigits];
+    const uint32_t n_shifts = frz_order_digits(h.vary_hi & h.flip_hi, h.vary_lo & h.flip_lo, shifts);
+    const uint64_t k = std::min<uint64_t>(limit, n);
+    const bool select = k < n;
+    // with k rows to return, a block-sorted selection may stop as soon as it fits in the block (frz_order_pick's fit)
+    const uint64_t fit = k <= kFrzOrderBlockRows ? kFrzOrderBlockRows : 0;
+    const uint64_t n_sel_max = select && !fit ? k : fit ? std::min<uint64_t>(n, fit) : n;
+    const unsigned long long* sel_n = n_ptr;
+    const uint32_t* sel = nullptr;
+    if (select && !(fit && n <= fit)) {
+        FRZ_TRY(ws.order_cand.reserve(2 * n));
+        FRZ_TRY(ws.order_sel.reserve(n));
+        if (!ws.order_hist.get()) {
+            FRZ_TRY(ws.order_hist.reserve(kFrzOrderBins));
+            FRZ_CUDA_TRY(cudaMemsetAsync(ws.order_hist.get(), 0, kFrzOrderBins * sizeof(uint32_t), stream));
+        }
+        FRZ_TRY(frz_launch_order_select(ws.order_keys.get(), dst, ws.order_hist.get(), ws.order_cand.get(), ws.order_sel.get(), n, k,
+                                        shifts, n_shifts, fit, stream, st));
+        sel_n = &dst->n_sel;
+        sel = ws.order_sel.get();
+    }
+    FrzMatchDev* other = *d_list == ws.matches_a.get() ? ws.matches_b.get() : ws.matches_a.get();
+    if (n_sel_max <= kFrzOrderBlockRows) {
+        FRZ_TRY(frz_launch_order_sort_block(*d_list, ws.order_keys.get(), sel, sel_n, limit, other, stream, st));
+        *d_list = other;
+        return FRZ_OK;
+    }
+    FRZ_TRY(ensure_multi_buffers(m, cs.n));
+    if (sel) {   // the selection's rows in a list of their own, sorted back into the list's buffer
+        FRZ_TRY(frz_launch_order_gather(*d_list, sel, sel_n, k, other, stream, st));
+        FRZ_TRY(frz_launch_sort_by_order_dev(other, ws.multi_a.get(), *d_list, sel_n, o, shifts, n_shifts, ws.sort, stream, st, limit));
+        return FRZ_OK;
+    }
+    FRZ_TRY(frz_launch_sort_by_order_dev(*d_list, ws.multi_a.get(), other, n_ptr, o, shifts, n_shifts, ws.sort, stream, st, limit));
+    *d_list = other;
+    return FRZ_OK;
+}
+
 // `final_out` (optional, device, >= corpus length): where the final list must land.  `limit` (top-K calls): only the first
 // `limit` positions of the final list are written (the sort's last scatter and the final copy drop the rest); the count in
 // ws.counters->total stays the full match count.  scope: as in match_into_device.  rank (optional): sort by the ranking's
 // key instead, under every strategy and for the empty matcher too (the strategy's direction only orders ties).  col
 // (optional, host calls only: final_out == nullptr): collapse the list before its sort (collapse_list).  cols (optional,
-// host calls only): the list is that of a frz_match_list_columns call, whose starting column is cs (match_patterns).
+// host calls only): the list is that of a frz_match_list_columns call, whose starting column is cs (match_patterns).  ord
+// (optional, host calls only): order the list by the attribute instead (order_list), under every strategy and for the
+// empty matcher too.
 frz_status match_list_device(frz_matcher* m, const FrzCorpusStorage& cs, uint32_t index_offset, uint8_t sort,
                              FrzMatchDev** d_result, cudaStream_t stream, FrzLaunchStats* st, FrzMatchDev* final_out = nullptr,
                              uint32_t limit = kFrzNoLimit, const SubsetScope& scope = SubsetScope(), const Ranking* rank = nullptr,
-                             const Collapse* col = nullptr, const Columns* cols = nullptr) {
+                             const Collapse* col = nullptr, const Columns* cols = nullptr, const Ordering* ord = nullptr) {
     FrzWorkspace& ws = m->ws;
     const bool reversed = sort == FRZ_SORT_INDEX_DESC || sort == FRZ_SORT_SCORE_THEN_INDEX_DESC;
     const bool by_score = sort == FRZ_SORT_SCORE_THEN_INDEX_ASC || sort == FRZ_SORT_SCORE_THEN_INDEX_DESC;
-    const bool will_sort = rank || (by_score && (cols ? cols->any_compiled : !m->compiled.empty()));
+    const bool will_sort = rank || ord || (by_score && (cols ? cols->any_compiled : !m->compiled.empty()));
     reset_call_state(m);
     FrzMatchDev* d_list = nullptr;
     uint32_t bound = 0;
@@ -1478,13 +1545,14 @@ frz_status match_list_device(frz_matcher* m, const FrzCorpusStorage& cs, uint32_
     FrzScoreHist hist;
     if (cols) FRZ_TRY(match_patterns(m, cols->pats, cs, cols->live, index_offset, reversed, &d_list, &bound, stream, st, scope));
     else FRZ_TRY(match_into_device(m, cs, index_offset, reversed, &d_list, &bound, stream, st, will_sort ? nullptr : final_out,
-                                   will_sort && !rank && !col ? &hist : nullptr, scope));
+                                   will_sort && !rank && !col && !ord ? &hist : nullptr, scope));
     if (col) {
         const uint8_t order = rank ? FRZ_COLLAPSE_BY_KEY : will_sort ? FRZ_COLLAPSE_BY_SCORE : FRZ_COLLAPSE_BY_INDEX;
         FRZ_TRY(collapse_list(m, cs, *col, order, reversed, rank, &d_list, stream, st));
     }
-    // `!self.patterns.is_empty() && sort.is_by_score()` (src/matcher/mod.rs:218)
-    if (will_sort) {
+    if (ord) {
+        FRZ_TRY(order_list(m, cs, *ord, reversed, limit, &d_list, stream, st));
+    } else if (will_sort) {   // `!self.patterns.is_empty() && sort.is_by_score()` (src/matcher/mod.rs:218)
         if (rank) bound = (uint32_t)std::min<uint64_t>((uint64_t)bound + rank->max_boost, 0xFFFF);   // the key bound
         FrzMatchDev* other = final_out ? final_out : (d_list == ws.matches_a.get() ? ws.matches_b.get() : ws.matches_a.get());
         // two-pass sort (score bound >= 1024) needs a scratch list of the corpus size: the multi-pattern ping-pong
@@ -1551,11 +1619,11 @@ frz_status copy_out(frz_matcher* m, FrzMatchDev* d_list, uint64_t limit, frz_mat
 // the same pipeline with a limit on the final scatter and copy; UINT64_MAX for the whole list).  scope: the rows of a subset
 // call (match_into_device).  rank: a ranked call, col: a collapsed call (match_list_device); group_counts (optional, host,
 // col->n_groups entries) receives the list's rows per group.  cols: a frz_match_list_columns call whose starting column is
-// corpus (match_list_device).
+// corpus (match_list_device).  ord: an ordered call (match_list_device).
 frz_status match_list_host(frz_matcher* m, const frz_corpus* corpus, uint32_t index_offset, uint8_t sort, uint64_t limit,
                            const SubsetScope& scope, frz_match* out, uint64_t cap, uint64_t* n_out, uint64_t* n_total,
                            const Ranking* rank = nullptr, const Collapse* col = nullptr, uint32_t* group_counts = nullptr,
-                           const Columns* cols = nullptr) {
+                           const Columns* cols = nullptr, const Ordering* ord = nullptr) {
     if (scope.none) {
         if (n_out) *n_out = 0;
         if (n_total) *n_total = 0;
@@ -1568,7 +1636,7 @@ frz_status match_list_host(frz_matcher* m, const frz_corpus* corpus, uint32_t in
     const uint32_t dev_limit = (uint32_t)std::min<uint64_t>(limit, kFrzNoLimit);   // a list never holds more than 2^32 - 1 matches
     frz_status s = FRZ_OK;
     for (int attempt = 0; attempt < 2; attempt++) {
-        s = match_list_device(m, corpus->st, index_offset, sort, &d_list, stream, &st, nullptr, dev_limit, scope, rank, col, cols);
+        s = match_list_device(m, corpus->st, index_offset, sort, &d_list, stream, &st, nullptr, dev_limit, scope, rank, col, cols, ord);
         if (s == FRZ_OK) s = copy_out(m, d_list, limit, out, cap, n_out, n_total, stream);
         if (s != kRetryOverflow) break;
         FRZ_TRY(ensure_workspace(m, corpus->st, std::max<uint64_t>(corpus->st.n, 1)));  // worst-case lists, then once more
@@ -2233,6 +2301,33 @@ extern "C" frz_status frz_match_list_ranked(frz_matcher* m, const frz_corpus* co
     if (s) FRZ_TRY(subset_scope(m, corpus, *s, nullptr, &scope));
     const Ranking rank = ranking_of(*b);
     return match_list_host(m, corpus, 0, m->config.sort, k, scope, out, k, n_out, n_total, &rank);
+}
+
+// ---------------------------------------------------------------------------------- ordered calls
+static_assert(FRZ_ORDER_SCORE_THEN_ATTR_DESC == kFrzOrderScoreFirst && FRZ_ORDER_SCORE_THEN_ATTR_ASC + 1 == kFrzOrderCount &&
+                  (FRZ_ORDER_ATTR_ASC & 1) && (FRZ_ORDER_SCORE_THEN_ATTR_ASC & 1) && !(FRZ_ORDER_ATTR_DESC & 1),
+              "order_plan.cuh mirrors frz_cuda.h");
+
+extern "C" frz_status frz_match_list_ordered(frz_matcher* m, const frz_corpus* corpus, const frz_subset* s, const frz_boost* b,
+                                             const frz_attr* a, uint32_t order, uint64_t k, frz_match* out, uint64_t* n_out,
+                                             uint64_t* n_total) {
+    if (!m || !corpus || !a) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    if (!out && k > 0) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
+    if (order >= kFrzOrderCount) return frz_fail(FRZ_ERR_INVALID_ARG, "order %u (at most %u)", order, kFrzOrderCount - 1);
+    if (a->corpus != corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "the attribute was made on another corpus");
+    if (b && b->corpus != corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "the boost was made on another corpus");
+    if (s) FRZ_TRY(check_subset_call(m, corpus, s));
+    FRZ_TRY(frz_ensure_device(corpus->st.device));
+    SubsetScope scope;
+    if (s) FRZ_TRY(subset_scope(m, corpus, *s, nullptr, &scope));
+    Ordering ord;
+    ord.dev = FrzOrderDev{};
+    ord.dev.values = a->values.get();
+    ord.dev.n_values = a->values.cap();
+    ord.dev.boost = b ? b->values.get() : nullptr;
+    ord.dev.n_boost = b ? (uint32_t)b->values.cap() : 0;
+    ord.dev.order = order;
+    return match_list_host(m, corpus, 0, m->config.sort, k, scope, out, k, n_out, n_total, nullptr, nullptr, nullptr, nullptr, &ord);
 }
 
 // ---------------------------------------------------------------------------------- collapsed calls

@@ -28,8 +28,12 @@
 // Ranked calls (frz_match_list_ranked) sort by a key in place of the score: k_sort_hist and k_sort_scatter take the digit
 // source as a template parameter (ScoreKey, BoostKey), and frz_launch_sort_by_key_dev runs the same one- or two-pass
 // histogram-kernel sort on clamp(score + boost[index], 0, 65535).  The elements keep their raw scores.
+//
+// The ordered call's multi-block sort (frz_match_list_ordered, DESIGN.md §4.15) runs the same 8-bit passes, least
+// significant first, over the digits of its 112-bit order key (OrderKey), skipping digits no two rows differ in.
 #include "frz_device.cuh"
 #include "frz_host.h"
+#include "order_plan.cuh"
 
 #include <algorithm>
 
@@ -304,29 +308,37 @@ __global__ void __launch_bounds__(kSegThreads) k_sort_scatter_seg(const FrzMatch
     }
 }
 
+// One histogram-kernel pass: the list at src scattered to dst, stably by descending digit (Key >> shift) & (bins - 1).
+// Only the positions below `keep` are stored.
+template <class Key>
+frz_status sort_pass(const FrzMatchDev* src, FrzMatchDev* dst, const unsigned long long* n_ptr, int shift, int bins, uint32_t keep,
+                     Key key, FrzSortScratch& ss, cudaStream_t stream, FrzLaunchStats* st) {
+    uint32_t* const hist = ss.hist.get();
+    const size_t smem = (size_t)kSortWarps * bins * sizeof(uint32_t);
+    k_sort_hist<<<kSortBlocks, kSortWarps * 32, smem, stream>>>(src, n_ptr, shift, bins, hist, key);
+    uint32_t* totals = hist + (size_t)kMaxBins * kV;
+    uint32_t* digit_base = totals + kMaxBins;
+    unsigned int* done_counter = reinterpret_cast<unsigned int*>(digit_base + kMaxBins);   // zeroed at allocation, self-resetting
+    k_sort_scan_rows<kV / 128, false><<<(bins + 7) / 8, 256, 0, stream>>>(hist, hist, kV, nullptr, bins, totals,
+                                                                           digit_base, done_counter);
+    if (ss.arm_table_ev && ss.table_ev) {   // digit_base is final: the multi-GPU layer publishes it while the scatter runs
+        FRZ_CUDA_TRY(cudaEventRecord(ss.table_ev.get(), stream));
+        ss.table_ev_recorded = true;
+    }
+    k_sort_scatter<<<kSortBlocks, kSortWarps * 32, smem, stream>>>(src, dst, n_ptr, shift, bins, hist, digit_base, keep, key);
+    FRZ_CUDA_TRY(cudaGetLastError());
+    if (st) st->launches += 3;
+    return FRZ_OK;
+}
+
 // The histogram-kernel sort of the list at d_in by descending Key (stable): one pass when the key bound allows it, else
 // the reference's two 8-bit LSD passes.  n_ptr: device pointer to the element count.  bound: host-known upper bound of
 // any key.
 template <class Key>
 frz_status launch_sort_dev(const FrzMatchDev* d_in, FrzMatchDev* d_tmp, FrzMatchDev* d_out, const unsigned long long* n_ptr,
                            uint32_t bound, Key key, FrzSortScratch& ss, cudaStream_t stream, FrzLaunchStats* st, uint32_t limit) {
-    uint32_t* const hist = ss.hist.get();
     auto pass = [&](const FrzMatchDev* src, FrzMatchDev* dst, int shift, int bins, uint32_t keep) -> frz_status {
-        const size_t smem = (size_t)kSortWarps * bins * sizeof(uint32_t);
-        k_sort_hist<<<kSortBlocks, kSortWarps * 32, smem, stream>>>(src, n_ptr, shift, bins, hist, key);
-        uint32_t* totals = hist + (size_t)kMaxBins * kV;
-        uint32_t* digit_base = totals + kMaxBins;
-        unsigned int* done_counter = reinterpret_cast<unsigned int*>(digit_base + kMaxBins);   // zeroed at allocation, self-resetting
-        k_sort_scan_rows<kV / 128, false><<<(bins + 7) / 8, 256, 0, stream>>>(hist, hist, kV, nullptr, bins, totals,
-                                                                               digit_base, done_counter);
-        if (ss.arm_table_ev && ss.table_ev) {   // digit_base is final: the multi-GPU layer publishes it while the scatter runs
-            FRZ_CUDA_TRY(cudaEventRecord(ss.table_ev.get(), stream));
-            ss.table_ev_recorded = true;
-        }
-        k_sort_scatter<<<kSortBlocks, kSortWarps * 32, smem, stream>>>(src, dst, n_ptr, shift, bins, hist, digit_base, keep, key);
-        FRZ_CUDA_TRY(cudaGetLastError());
-        if (st) st->launches += 3;
-        return FRZ_OK;
+        return sort_pass(src, dst, n_ptr, shift, bins, keep, key, ss, stream, st);
     };
     if (bound < 256) return pass(d_in, d_out, 0, 256, limit);
     if (bound < 512) return pass(d_in, d_out, 0, 512, limit);
@@ -335,6 +347,16 @@ frz_status launch_sort_dev(const FrzMatchDev* d_in, FrzMatchDev* d_tmp, FrzMatch
     FRZ_TRY(pass(d_in, d_tmp, 0, 256, kFrzNoLimit));
     return pass(d_tmp, d_out, 8, 256, limit);
 }
+
+// The digit source of the ordered call's sort (frz_match_list_ordered): digit `shift` of the row's order key
+// (order_plan.cuh), recomputed from the record, its attribute value and its boost.
+struct OrderKey {
+    FrzOrderDev o;
+    uint32_t shift;
+    __device__ __forceinline__ uint32_t operator()(const FrzMatchDev& m) const {
+        return frz_order_digit(frz_order_row_key(o, m.index, m.score), shift);
+    }
+};
 
 }  // namespace
 
@@ -348,6 +370,20 @@ frz_status frz_launch_sort_by_key_dev(const FrzMatchDev* d_in, FrzMatchDev* d_tm
                                       const unsigned long long* n_ptr, const int16_t* boost, uint32_t n_boost, uint32_t key_bound,
                                       FrzSortScratch& ss, cudaStream_t stream, FrzLaunchStats* st, uint32_t limit) {
     return launch_sort_dev(d_in, d_tmp, d_out, n_ptr, key_bound, BoostKey{boost, n_boost}, ss, stream, st, limit);
+}
+
+frz_status frz_launch_sort_by_order_dev(const FrzMatchDev* d_in, FrzMatchDev* d_tmp, FrzMatchDev* d_out, const unsigned long long* n_ptr,
+                                        const FrzOrderDev& o, const uint32_t* shifts, uint32_t n_shifts, FrzSortScratch& ss,
+                                        cudaStream_t stream, FrzLaunchStats* st, uint32_t limit) {
+    if (n_shifts == 0) return frz_fail(FRZ_ERR_INVALID_ARG, "an ordered sort needs a digit");
+    const FrzMatchDev* src = d_in;
+    for (uint32_t i = 0; i < n_shifts; i++) {   // least significant digit first; the last pass lands in d_out
+        FrzMatchDev* dst = (n_shifts - 1 - i) % 2 == 0 ? d_out : d_tmp;
+        FRZ_TRY(sort_pass(src, dst, n_ptr, 0, (int)kFrzOrderBins, i + 1 == n_shifts ? limit : kFrzNoLimit,
+                          OrderKey{o, shifts[n_shifts - 1 - i]}, ss, stream, st));
+        src = dst;
+    }
+    return FRZ_OK;
 }
 
 // allocates the sort scratch on the current device: counts, totals, digit_base + the pass-completion counter of

@@ -30,6 +30,15 @@ class SortStrategy(enum.IntEnum):
         return self in (SortStrategy.ScoreThenIndexAsc, SortStrategy.ScoreThenIndexDesc)
 
 
+class Order(enum.IntEnum):
+    """How Matcher.match_list_ordered_array orders the matches by an attribute (FRZ_ORDER_*); rows without a value go
+    last in every order."""
+    AttrDesc = 0            # by value, largest first
+    AttrAsc = 1             # by value, smallest first
+    ScoreThenAttrDesc = 2   # by score (with the boost), then by value, largest first
+    ScoreThenAttrAsc = 3    # by score (with the boost), then by value, smallest first
+
+
 class CaseMatching(enum.IntEnum):
     Ignore = 0
     Smart = 1

@@ -415,6 +415,41 @@ FRZ_API void frz_boost_destroy(frz_boost* b);
 FRZ_API frz_status frz_match_list_ranked(frz_matcher* m, const frz_corpus* c, const frz_subset* s, const frz_boost* b,
                                          uint64_t k, frz_match* out, uint64_t* n_out, uint64_t* n_total);
 
+/* ---------------------------------------------------------------- ordered calls
+ *
+ * A shell history lists the most recent matching command first, a log or mail search sorts "newest first", a file picker
+ * sorts by "last modified", and a completion menu breaks score ties by a precomputed sort key.  The reference has no such
+ * method: its callers sort Matcher::match_list's output (src/matcher/mod.rs:212-222) by their own copy of the field.  These
+ * calls order the matches by an attribute (frz_attr above) on the device and return only the first k rows. */
+enum {
+    FRZ_ORDER_ATTR_DESC = 0,              /* by value, largest first (newest first) */
+    FRZ_ORDER_ATTR_ASC = 1,               /* by value, smallest first */
+    FRZ_ORDER_SCORE_THEN_ATTR_DESC = 2,   /* by score (with the boost), then by value, largest first */
+    FRZ_ORDER_SCORE_THEN_ATTR_ASC = 3     /* by score (with the boost), then by value, smallest first */
+};
+/* The reference has no such method (see above).  Let L0 be the rows of frz_match_list_into(m, c, 0), restricted to the
+ * members of s when s is given (as frz_match_list_subset does), and reversed under IndexDesc / ScoreThenIndexDesc.  Let
+ * v(i) be index i's value in a; it is null when it equals FRZ_ATTR_NULL or when i lies past the attribute's values.  Let
+ * r(i) be clamp(score + boost[i], 0, 65535) (32-bit arithmetic, frz_match_list_ranked's key) when b is given, else the
+ * raw score.  L0 is sorted stably by:
+ *   FRZ_ORDER_ATTR_DESC:             non-null rows first, then v descending, then r descending;
+ *   FRZ_ORDER_ATTR_ASC:              non-null rows first, then v ascending, then r descending;
+ *   FRZ_ORDER_SCORE_THEN_ATTR_DESC:  r descending, then non-null rows first, then v descending;
+ *   FRZ_ORDER_SCORE_THEN_ATTR_ASC:   r descending, then non-null rows first, then v ascending.
+ * Rows still tied keep L0's order: index order in the strategy's direction.  Nulls go last in both directions.  Every
+ * strategy orders this way, and so does the empty matcher: it lists the live rows by the attribute ("latest first").  The
+ * rows are those of frz_match_list, bit for bit, raw scores included; only their order differs.  The call writes the first
+ * min(k, total) rows to `out`, their number to *n_out and total to *n_total (may be NULL).
+ *
+ * Same rules as frz_match_list_ranked: `out` is HOST memory with room for k matches (min(k, frz_corpus_len(c)) suffices,
+ * or min(k, frz_subset_len(s)) with a subset), k = 0 only counts, k = UINT64_MAX returns the whole ordered list, and the
+ * call never returns FRZ_ERR_CAPACITY.  Checked before any device work: a NULL matcher, corpus or attribute, or a NULL out
+ * with k > 0, an order above FRZ_ORDER_SCORE_THEN_ATTR_ASC, or a subset, boost or attribute of another corpus is
+ * FRZ_ERR_INVALID_ARG.  s and b may be NULL.  Blocking; it only reads its handles, so several matchers may share them. */
+FRZ_API frz_status frz_match_list_ordered(frz_matcher* m, const frz_corpus* c, const frz_subset* s, const frz_boost* b,
+                                          const frz_attr* a, uint32_t order, uint64_t k, frz_match* out, uint64_t* n_out,
+                                          uint64_t* n_total);
+
 /* ------------------------------------------------ collapsed calls: groups
  *
  * Rows that belong together (every execution of one command in a shell history, every hit of one file in a live grep,
