@@ -370,26 +370,26 @@ class Subset:
             pass
 
 
-class Boost:
-    """A signed 16-bit boost per row of one resident Corpus (frz_boost), kept by index across corpus edits."""
+class _RowValues:
+    """A value per row of one resident Corpus, kept by index across corpus edits: the part Boost, Attr and Groups share."""
+    _dtype, _what, _set_fn, _destroy_fn = None, "values", "", ""
 
     def __init__(self, handle, corpus: Corpus):
         self._h = handle
         self.corpus = corpus
 
-    def set(self, which, values) -> "Boost":
-        """boost[which[j]] = values[j]; any row below len(corpus), appended ones included, each at most once."""
+    def _set(self, which, values):
         which = np.ascontiguousarray(which, dtype=np.uint32)
-        values = np.ascontiguousarray(values, dtype=np.int16)
+        values = np.ascontiguousarray(values, dtype=self._dtype)
         if len(values) != len(which):
-            raise ValueError(f"{len(which)} indices need {len(which)} values, got {len(values)}")
-        _check(lib().frz_boost_set(self._h, which.ctypes.data if which.size else None,
-                                   values.ctypes.data if values.size else None, len(which)))
+            raise ValueError(f"{len(which)} indices need {len(which)} {self._what}, got {len(values)}")
+        _check(getattr(lib(), self._set_fn)(self._h, which.ctypes.data if which.size else None,
+                                            values.ctypes.data if values.size else None, len(which)))
         return self
 
     def close(self):
         if self._h:
-            lib().frz_boost_destroy(self._h)
+            getattr(lib(), self._destroy_fn)(self._h)
             self._h = None
 
     def __del__(self):
@@ -397,6 +397,15 @@ class Boost:
             self.close()
         except Exception:
             pass
+
+
+class Boost(_RowValues):
+    """A signed 16-bit boost per row of one resident Corpus (frz_boost), kept by index across corpus edits."""
+    _dtype, _set_fn, _destroy_fn = np.int16, "frz_boost_set", "frz_boost_destroy"
+
+    def set(self, which, values) -> "Boost":
+        """boost[which[j]] = values[j]; any row below len(corpus), appended ones included, each at most once."""
+        return self._set(which, values)
 
 
 class _CWhereClause(C.Structure):
@@ -416,23 +425,14 @@ class Where:
         return Where(self.attr, self.lo, self.hi, self.values, not self.negate)
 
 
-class Attr:
+class Attr(_RowValues):
     """A signed 64-bit value per row of one resident Corpus (frz_attr), kept by index across corpus edits."""
-
-    def __init__(self, handle, corpus: Corpus):
-        self._h = handle
-        self.corpus = corpus
+    _dtype, _set_fn, _destroy_fn = np.int64, "frz_attr_set", "frz_attr_destroy"
 
     def set(self, which, values) -> "Attr":
         """value[which[j]] = values[j] (ATTR_NULL clears it); any row below len(corpus), appended ones included, each at
         most once."""
-        which = np.ascontiguousarray(which, dtype=np.uint32)
-        values = np.ascontiguousarray(values, dtype=np.int64)
-        if len(values) != len(which):
-            raise ValueError(f"{len(which)} indices need {len(which)} values, got {len(values)}")
-        _check(lib().frz_attr_set(self._h, which.ctypes.data if which.size else None,
-                                  values.ctypes.data if values.size else None, len(which)))
-        return self
+        return self._set(which, values)
 
     def between(self, lo: int, hi: int) -> Where:
         """The clause lo <= v <= hi (it holds for no value when lo > hi)."""
@@ -443,49 +443,30 @@ class Attr:
         values = np.ascontiguousarray(values, dtype=np.int64)
         return Where(self, values=values) if values.size else Where(self, 0, -1)
 
-    def close(self):
-        if self._h:
-            lib().frz_attr_destroy(self._h)
-            self._h = None
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
-
-
-class Groups:
+class Groups(_RowValues):
     """A group id per row of one resident Corpus (frz_groups), kept by index across corpus edits."""
-
-    def __init__(self, handle, corpus: Corpus):
-        self._h = handle
-        self.corpus = corpus
+    _dtype, _what, _set_fn, _destroy_fn = np.uint32, "ids", "frz_groups_set", "frz_groups_destroy"
 
     def set(self, which, ids) -> "Groups":
         """group[which[j]] = ids[j] (an id below len(self), or GROUP_NONE); any row below len(corpus), appended ones
         included, each at most once."""
-        which = np.ascontiguousarray(which, dtype=np.uint32)
-        ids = np.ascontiguousarray(ids, dtype=np.uint32)
-        if len(ids) != len(which):
-            raise ValueError(f"{len(which)} indices need {len(which)} ids, got {len(ids)}")
-        _check(lib().frz_groups_set(self._h, which.ctypes.data if which.size else None, ids.ctypes.data if ids.size else None,
-                                    len(which)))
-        return self
+        return self._set(which, ids)
 
     def __len__(self):
         return lib().frz_groups_count(self._h)
 
-    def close(self):
-        if self._h:
-            lib().frz_groups_destroy(self._h)
-            self._h = None
 
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+def _top_out(out: Optional[np.ndarray], k: Optional[int], n: int, subset: Optional["Subset"], what: str):
+    """(k, out) for a call that returns the first k rows of n (and of the subset's members): k=None is every row; `out`, when
+    given, must hold min(k, n, len(subset)) matches (`what` names the call in the error), else a new array that does."""
+    k = _U64_MAX if k is None else int(k)
+    need = min(k, n, len(subset) if subset is not None else n)
+    if out is None:
+        return k, np.empty(max(1, need), dtype=MATCH_DTYPE)
+    if len(out) < need:
+        raise ValueError(f"out holds {len(out)} matches; {what} needs {need}")
+    return k, out
 
 
 def _to_matches(arr: np.ndarray) -> List[Match]:
@@ -569,13 +550,9 @@ class Matcher:
         `out` (optional) needs room for min(k, len(corpus)) matches: no more rows can match."""
         corpus, owned = self._corpus(haystacks, device)
         try:
-            need = min(int(k), corpus.n)
-            if out is None:
-                out = np.empty(max(1, need), dtype=MATCH_DTYPE)
-            elif len(out) < need:
-                raise ValueError(f"out holds {len(out)} matches; a top-{k} call on {corpus.n} haystacks needs {need}")
+            k, out = _top_out(out, k, corpus.n, None, f"a top-{k} call on {corpus.n} haystacks")
             n, total = C.c_uint64(), C.c_uint64()
-            _check(lib().frz_match_list_top(self._h, corpus._h, int(k), out.ctypes.data, C.byref(n), C.byref(total)))
+            _check(lib().frz_match_list_top(self._h, corpus._h, k, out.ctypes.data, C.byref(n), C.byref(total)))
             return out[: n.value], total.value
         finally:
             if owned:
@@ -591,9 +568,9 @@ class Matcher:
 
     def match_list_subset_top_array(self, corpus: Corpus, subset: Subset, k: int) -> Tuple[np.ndarray, int]:
         """The first k rows of match_list_subset_array (frz_match_list_subset_top): (array of min(k, total) matches, total)."""
-        out = np.empty(max(1, min(int(k), len(subset))), dtype=MATCH_DTYPE)
+        k, out = _top_out(None, k, corpus.n, subset, "")
         n, total = C.c_uint64(), C.c_uint64()
-        _check(lib().frz_match_list_subset_top(self._h, corpus._h, subset._h, int(k), out.ctypes.data, C.byref(n), C.byref(total)))
+        _check(lib().frz_match_list_subset_top(self._h, corpus._h, subset._h, k, out.ctypes.data, C.byref(n), C.byref(total)))
         return out[: n.value], total.value
 
     def match_list_ranked_array(self, corpus: Corpus, boost: Boost, k: Optional[int] = None, subset: Optional[Subset] = None,
@@ -601,12 +578,7 @@ class Matcher:
         """The rows of match_list_array(corpus) (or of its subset), ranked by clamp(score + boost[index], 0, 65535), ties in
         the strategy's index order, truncated to the first k (frz_match_list_ranked): (array of min(k, total) rows, total).
         k=None ranks the whole list.  `out` (optional) needs room for min(k, len(corpus), len(subset)) rows."""
-        k = 0xFFFFFFFFFFFFFFFF if k is None else int(k)
-        need = min(k, corpus.n, len(subset) if subset is not None else corpus.n)
-        if out is None:
-            out = np.empty(max(1, need), dtype=MATCH_DTYPE)
-        elif len(out) < need:
-            raise ValueError(f"out holds {len(out)} matches; this ranked call needs {need}")
+        k, out = _top_out(out, k, corpus.n, subset, "this ranked call")
         n, total = C.c_uint64(), C.c_uint64()
         _check(lib().frz_match_list_ranked(self._h, corpus._h, subset._h if subset is not None else None, boost._h, k,
                                            out.ctypes.data, C.byref(n), C.byref(total)))
@@ -620,12 +592,7 @@ class Matcher:
         (ScoreThenAttrDesc / Asc); rows without a value go last, and remaining ties keep the strategy's index order.
         Truncated to the first k: (array of min(k, total) rows, total).  k=None orders the whole list.  `out` (optional)
         needs room for min(k, len(corpus), len(subset)) rows."""
-        k = _U64_MAX if k is None else int(k)
-        need = min(k, corpus.n, len(subset) if subset is not None else corpus.n)
-        if out is None:
-            out = np.empty(max(1, need), dtype=MATCH_DTYPE)
-        elif len(out) < need:
-            raise ValueError(f"out holds {len(out)} matches; this ordered call needs {need}")
+        k, out = _top_out(out, k, corpus.n, subset, "this ordered call")
         n, total = C.c_uint64(), C.c_uint64()
         _check(lib().frz_match_list_ordered(self._h, corpus._h, subset._h if subset is not None else None,
                                             boost._h if boost is not None else None, attr._h, int(order), k, out.ctypes.data,
@@ -641,13 +608,8 @@ class Matcher:
         (rows, total, counts) with counts=True: the rows of L per group (uint32, len(groups) entries), before collapsing.
         k=None returns every kept row; per_group is 1..32, or None for no cap.  `out` (optional) needs room for
         min(k, len(corpus), len(subset)) rows."""
-        k = _U64_MAX if k is None else int(k)
+        k, out = _top_out(out, k, corpus.n, subset, "this collapsed call")
         per_group = _U64_MAX if per_group is None else int(per_group)
-        need = min(k, corpus.n, len(subset) if subset is not None else corpus.n)
-        if out is None:
-            out = np.empty(max(1, need), dtype=MATCH_DTYPE)
-        elif len(out) < need:
-            raise ValueError(f"out holds {len(out)} matches; this collapsed call needs {need}")
         cnt = np.zeros(len(groups), dtype=np.uint32) if counts else None
         n, total = C.c_uint64(), C.c_uint64()
         _check(lib().frz_match_list_collapsed(self._h, corpus._h, subset._h if subset is not None else None,
@@ -713,17 +675,43 @@ class Matcher:
             pass
 
 
-def match_list_batch_top(matchers, corpus: Corpus, k: int) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
-    """frz_match_list_batch_top: every matcher's match_list_top_array(corpus, k) in one call.  Returns a (q, k) array of
-    MATCH_DTYPE (row j's first n_out[j] entries are matcher j's rows; the rest are zero), n_out and n_total (int64, length q)."""
-    q, k = len(matchers), int(k)
-    handles = (C.c_void_p * max(q, 1))(*[m._h.value for m in matchers])
-    out = np.zeros((q, k), dtype=MATCH_DTYPE)
-    n_out = np.zeros(q, dtype=np.uint64)
-    n_total = np.zeros(q, dtype=np.uint64)
-    _check(lib().frz_match_list_batch_top(handles, q, corpus._h, k, out.ctypes.data if out.size else None, n_out.ctypes.data,
-                                          n_total.ctypes.data))
-    return out, n_out.astype(np.int64), n_total.astype(np.int64)
+class _BatchArgs:
+    """The per-query arrays of a batched call: one handle or NULL per query for subsets / boosts (NULL for None), and the
+    (q, k) rows, n_out and n_total; grouped() adds those of a call that may collapse."""
+
+    def __init__(self, q: int, k: int, subsets=None, boosts=None):
+        self.q = q
+        self.hs, self.hb = _handles(subsets, q, "subsets"), _handles(boosts, q, "boosts")
+        self.counts = None
+        self.out = np.zeros((q, k), dtype=MATCH_DTYPE)
+        self.n_out = np.zeros(q, dtype=np.uint64)
+        self.n_total = np.zeros(q, dtype=np.uint64)
+
+    def grouped(self, groups, per_group, counts: bool, who: str) -> "_BatchArgs":
+        """groups (None, or one Groups / None per query), per_group (an int, None for no cap, or one such value per query) as
+        uint64, and with counts=True a count array per query with groups and their pointers.  who: the queries' name in
+        the errors."""
+        q = self.q
+        groups = list(groups) if groups is not None else [None] * q
+        self.hg = _handles(groups, q, "groups")
+        if per_group is None or isinstance(per_group, (int, np.integer)):
+            per_group = [per_group] * q
+        per_group = list(per_group)
+        if len(per_group) != q:
+            raise ValueError(f"{q} {who} need {q} per_group values, got {len(per_group)}")
+        self.pg = np.array([_U64_MAX if p is None else int(p) for p in per_group] or [1], dtype=np.uint64)
+        self.counts = [np.zeros(len(g), dtype=np.uint32) if g is not None else None for g in groups] if counts else None
+        self.hc = (C.c_void_p * max(q, 1))(*[c.ctypes.data if c is not None else None for c in self.counts]) if counts else None
+        return self
+
+    def outputs(self):
+        """out (NULL when q * k = 0), n_out, n_total."""
+        return self.out.ctypes.data if self.out.size else None, self.n_out.ctypes.data, self.n_total.ctypes.data
+
+    def result(self):
+        """(rows, n_out, n_total), and the counts with counts=True."""
+        r = (self.out, self.n_out.astype(np.int64), self.n_total.astype(np.int64))
+        return r + (self.counts,) if self.counts is not None else r
 
 
 def _handles(xs, q: int, what: str):
@@ -736,20 +724,28 @@ def _handles(xs, q: int, what: str):
     return (C.c_void_p * max(q, 1))(*[x._h.value if x is not None else None for x in xs])
 
 
+def _matcher_array(matchers):
+    return (C.c_void_p * max(len(matchers), 1))(*[m._h.value for m in matchers])
+
+
+def match_list_batch_top(matchers, corpus: Corpus, k: int) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """frz_match_list_batch_top: every matcher's match_list_top_array(corpus, k) in one call.  Returns a (q, k) array of
+    MATCH_DTYPE (row j's first n_out[j] entries are matcher j's rows; the rest are zero), n_out and n_total (int64, length q)."""
+    q, k = len(matchers), int(k)
+    b = _BatchArgs(q, k)
+    _check(lib().frz_match_list_batch_top(_matcher_array(matchers), q, corpus._h, k, *b.outputs()))
+    return b.result()
+
+
 def match_list_batch(matchers, corpus: Corpus, k: int, subsets=None, boosts=None) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
     """frz_match_list_batch: match_list_batch_top where query j may have its own subset and boost.  subsets / boosts: None,
     or one Subset / Boost / None per matcher.  Query j's rows are those of matcher j's match_list_ranked_array(corpus,
     boosts[j], k, subsets[j]) when it has a boost, else of match_list_subset_top_array(corpus, subsets[j], k) when it has
     a subset, else of match_list_top_array(corpus, k).  Returns the (q, k) rows, n_out and n_total as match_list_batch_top."""
     q, k = len(matchers), int(k)
-    hs, hb = _handles(subsets, q, "subsets"), _handles(boosts, q, "boosts")
-    ms = (C.c_void_p * max(q, 1))(*[m._h.value for m in matchers])
-    out = np.zeros((q, k), dtype=MATCH_DTYPE)
-    n_out = np.zeros(q, dtype=np.uint64)
-    n_total = np.zeros(q, dtype=np.uint64)
-    _check(lib().frz_match_list_batch(ms, q, corpus._h, hs, hb, k, out.ctypes.data if out.size else None, n_out.ctypes.data,
-                                      n_total.ctypes.data))
-    return out, n_out.astype(np.int64), n_total.astype(np.int64)
+    b = _BatchArgs(q, k, subsets, boosts)
+    _check(lib().frz_match_list_batch(_matcher_array(matchers), q, corpus._h, b.hs, b.hb, k, *b.outputs()))
+    return b.result()
 
 
 def match_list_batch_collapsed(matchers, corpus: Corpus, k: int, groups, per_group=1, subsets=None, boosts=None, counts: bool = False):
@@ -759,25 +755,10 @@ def match_list_batch_collapsed(matchers, corpus: Corpus, k: int, groups, per_gro
     groups, else those of match_list_batch.  Returns the (q, k) rows, n_out and n_total as match_list_batch_top, and with
     counts=True also a list of each query's rows per group (uint32, len(groups[j]) entries; None for a query without groups)."""
     q, k = len(matchers), int(k)
-    groups = list(groups) if groups is not None else [None] * q
-    hs, hb, hg = _handles(subsets, q, "subsets"), _handles(boosts, q, "boosts"), _handles(groups, q, "groups")
-    if per_group is None or isinstance(per_group, (int, np.integer)):
-        per_group = [per_group] * q
-    per_group = list(per_group)
-    if len(per_group) != q:
-        raise ValueError(f"{q} matchers need {q} per_group values, got {len(per_group)}")
-    pg = np.array([_U64_MAX if p is None else int(p) for p in per_group] or [1], dtype=np.uint64)
-    cnt = [np.zeros(len(g), dtype=np.uint32) if counts and g is not None else None for g in groups]
-    hc = (C.c_void_p * max(q, 1))(*[c.ctypes.data if c is not None else None for c in cnt]) if counts else None
-    ms = (C.c_void_p * max(q, 1))(*[m._h.value for m in matchers])
-    out = np.zeros((q, k), dtype=MATCH_DTYPE)
-    n_out = np.zeros(q, dtype=np.uint64)
-    n_total = np.zeros(q, dtype=np.uint64)
-    _check(lib().frz_match_list_batch_collapsed(ms, q, corpus._h, hs, hb, hg, pg.ctypes.data, k, out.ctypes.data if out.size else None,
-                                                n_out.ctypes.data, n_total.ctypes.data, hc))
-    if counts:
-        return out, n_out.astype(np.int64), n_total.astype(np.int64), cnt
-    return out, n_out.astype(np.int64), n_total.astype(np.int64)
+    b = _BatchArgs(q, k, subsets, boosts).grouped(groups, per_group, counts, "matchers")
+    _check(lib().frz_match_list_batch_collapsed(_matcher_array(matchers), q, corpus._h, b.hs, b.hb, b.hg, b.pg.ctypes.data, k,
+                                                *b.outputs(), b.hc))
+    return b.result()
 
 
 def match_list_columns(matchers, columns, k: Optional[int] = None, sort: SortStrategy = SortStrategy.ScoreThenIndexAsc,
@@ -794,22 +775,15 @@ def match_list_columns(matchers, columns, k: Optional[int] = None, sort: SortStr
     matchers, columns = list(matchers), list(columns)
     if len(matchers) != len(columns):
         raise ValueError(f"{len(matchers)} matchers for {len(columns)} columns")
-    k = _U64_MAX if k is None else int(k)
+    k, out = _top_out(out, k, columns[0].n if columns else 0, subset, "this columns call")
     per_group = _U64_MAX if per_group is None else int(per_group)
-    n = columns[0].n if columns else 0
-    need = min(k, n, len(subset) if subset is not None else n)
-    if out is None:
-        out = np.empty(max(1, need), dtype=MATCH_DTYPE)
-    elif len(out) < need:
-        raise ValueError(f"out holds {len(out)} matches; this columns call needs {need}")
     if counts and groups is None:
         raise ValueError("counts=True needs groups")
     cnt = np.zeros(len(groups), dtype=np.uint32) if counts else None
     q = len(matchers)
-    ms = (C.c_void_p * max(q, 1))(*[m._h.value for m in matchers])
     cs = (C.c_void_p * max(q, 1))(*[c._h.value for c in columns])
     n_out, total = C.c_uint64(), C.c_uint64()
-    _check(lib().frz_match_list_columns(ms, cs, q, int(sort), subset._h if subset is not None else None,
+    _check(lib().frz_match_list_columns(_matcher_array(matchers), cs, q, int(sort), subset._h if subset is not None else None,
                                         boost._h if boost is not None else None, groups._h if groups is not None else None,
                                         per_group, k, out.ctypes.data, C.byref(n_out), C.byref(total),
                                         cnt.ctypes.data if counts else None))
@@ -831,26 +805,11 @@ def match_list_batch_columns(matchers, columns, k: int, sort: SortStrategy = Sor
     for j, mj in enumerate(matchers):
         if len(mj) != n_cols:
             raise ValueError(f"query {j} has {len(mj)} matchers for {n_cols} columns")
-    groups = list(groups) if groups is not None else [None] * q
-    hs, hb, hg = _handles(subsets, q, "subsets"), _handles(boosts, q, "boosts"), _handles(groups, q, "groups")
-    if per_group is None or isinstance(per_group, (int, np.integer)):
-        per_group = [per_group] * q
-    per_group = list(per_group)
-    if len(per_group) != q:
-        raise ValueError(f"{q} queries need {q} per_group values, got {len(per_group)}")
-    pg = np.array([_U64_MAX if p is None else int(p) for p in per_group] or [1], dtype=np.uint64)
-    cnt = [np.zeros(len(g), dtype=np.uint32) if counts and g is not None else None for g in groups]
-    hc = (C.c_void_p * max(q, 1))(*[c.ctypes.data if c is not None else None for c in cnt]) if counts else None
-    ms = (C.c_void_p * max(q * n_cols, 1))(*[m._h.value for mj in matchers for m in mj])
+    b = _BatchArgs(q, k, subsets, boosts).grouped(groups, per_group, counts, "queries")
     cs = (C.c_void_p * max(n_cols, 1))(*[c._h.value for c in columns])
-    out = np.zeros((q, k), dtype=MATCH_DTYPE)
-    n_out = np.zeros(q, dtype=np.uint64)
-    n_total = np.zeros(q, dtype=np.uint64)
-    _check(lib().frz_match_list_batch_columns(ms, q, cs, n_cols, int(sort), hs, hb, hg, pg.ctypes.data, k,
-                                              out.ctypes.data if out.size else None, n_out.ctypes.data, n_total.ctypes.data, hc))
-    if counts:
-        return out, n_out.astype(np.int64), n_total.astype(np.int64), cnt
-    return out, n_out.astype(np.int64), n_total.astype(np.int64)
+    _check(lib().frz_match_list_batch_columns(_matcher_array([m for mj in matchers for m in mj]), q, cs, n_cols, int(sort), b.hs, b.hb,
+                                              b.hg, b.pg.ctypes.data, k, *b.outputs(), b.hc))
+    return b.result()
 
 
 def batch_last() -> dict:

@@ -18,6 +18,7 @@
 #include <atomic>
 #include <memory>
 #include <mutex>
+#include <optional>
 
 #include "batch_collapse_plan.cuh"
 #include "batch_columns_plan.cuh"
@@ -1425,7 +1426,7 @@ struct Collapse {
 // |C|).  order: what the rows' order keys rank by.  The list's length is read back first (a survivor-list overflow
 // returns kRetryOverflow there): the passes and the compaction then cover the list, not the corpus.
 frz_status collapse_list(frz_matcher* m, const FrzCorpusStorage& cs, const Collapse& col, uint8_t order, bool reversed,
-                         const Ranking* rank, FrzMatchDev** d_list, cudaStream_t stream, FrzLaunchStats* st) {
+                         const std::optional<Ranking>& rank, FrzMatchDev** d_list, cudaStream_t stream, FrzLaunchStats* st) {
     FrzWorkspace& ws = m->ws;
     FRZ_TRY(read_counters(m, stream));
     const uint64_t n_list = ws.h_counters.get()->total;
@@ -1522,37 +1523,67 @@ frz_status order_list(frz_matcher* m, const FrzCorpusStorage& cs, const Ordering
     return FRZ_OK;
 }
 
-// `final_out` (optional, device, >= corpus length): where the final list must land.  `limit` (top-K calls): only the first
-// `limit` positions of the final list are written (the sort's last scatter and the final copy drop the rest); the count in
-// ws.counters->total stays the full match count.  scope: as in match_into_device.  rank (optional): sort by the ranking's
-// key instead, under every strategy and for the empty matcher too (the strategy's direction only orders ties).  col
-// (optional, host calls only: final_out == nullptr): collapse the list before its sort (collapse_list).  cols (optional,
-// host calls only): the list is that of a frz_match_list_columns call, whose starting column is cs (match_patterns).  ord
-// (optional, host calls only): order the list by the attribute instead (order_list), under every strategy and for the
-// empty matcher too.
-frz_status match_list_device(frz_matcher* m, const FrzCorpusStorage& cs, uint32_t index_offset, uint8_t sort,
-                             FrzMatchDev** d_result, cudaStream_t stream, FrzLaunchStats* st, FrzMatchDev* final_out = nullptr,
-                             uint32_t limit = kFrzNoLimit, const SubsetScope& scope = SubsetScope(), const Ranking* rank = nullptr,
-                             const Collapse* col = nullptr, const Columns* cols = nullptr, const Ordering* ord = nullptr) {
+// The sort strategies' two halves: the list's index direction, and whether it is sorted by score.
+bool sort_reversed(uint8_t sort) { return sort == FRZ_SORT_INDEX_DESC || sort == FRZ_SORT_SCORE_THEN_INDEX_DESC; }
+bool sort_by_score(uint8_t sort) { return sort == FRZ_SORT_SCORE_THEN_INDEX_ASC || sort == FRZ_SORT_SCORE_THEN_INDEX_DESC; }
+// What a collapse's order keys rank by: the ranking's key, else the score when the list is sorted by score, else the index.
+uint8_t collapse_order(bool ranked, bool by_score) {
+    return ranked ? FRZ_COLLAPSE_BY_KEY : by_score ? FRZ_COLLAPSE_BY_SCORE : FRZ_COLLAPSE_BY_INDEX;
+}
+
+// What a list call asks for (match_list_device, match_list_host): Matcher::match_list in `sort` order, truncated to its
+// first `limit` rows (top-K calls: only those positions of the final list are written, the sort's last scatter and the
+// final copy drop the rest; the count in ws.counters->total stays the full match count).  scope: as in match_into_device.
+// rank: sort by the ranking's key instead, under every strategy and for the empty matcher too (the strategy's direction
+// only orders ties).  col: collapse the list before its sort (collapse_list); group_counts (host, col->n_groups entries)
+// receives the list's rows per group.  cols: the list is that of a frz_match_list_columns call, whose starting column is
+// the call's corpus (match_patterns).  ord: order the list by the attribute instead (order_list), under every strategy and
+// for the empty matcher too.  col, cols and ord are for host calls only; the shard calls set index_offset and final_out
+// (device, >= corpus length: where the final list must land).
+struct ListCall {
+    uint8_t sort = FRZ_SORT_INDEX_ASC;
+    uint64_t limit = UINT64_MAX;
+    uint32_t index_offset = 0;
+    FrzMatchDev* final_out = nullptr;
+    SubsetScope scope;
+    std::optional<Ranking> rank;
+    std::optional<Collapse> col;
+    std::optional<Columns> cols;
+    std::optional<Ordering> ord;
+    uint32_t* group_counts = nullptr;
+
+    // a list never holds more than 2^32 - 1 matches
+    uint32_t dev_limit() const { return (uint32_t)std::min<uint64_t>(limit, kFrzNoLimit); }
+    // `!self.patterns.is_empty() && sort.is_by_score()` (src/matcher/mod.rs:218), and every ranked or ordered call
+    bool will_sort(const frz_matcher& m) const {
+        return rank || ord || (sort_by_score(sort) && (cols ? cols->any_compiled : !m.compiled.empty()));
+    }
+    // the fused histogram counts the scores of every row of the list, so only a plain score sort may use it
+    bool fused_hist(const frz_matcher& m) const { return will_sort(m) && !rank && !col && !ord; }
+    // where the scoring kernels may write the list: final_out when no sort follows them
+    FrzMatchDev* scoring_out(const frz_matcher& m) const { return will_sort(m) ? nullptr : final_out; }
+};
+
+frz_status match_list_device(frz_matcher* m, const FrzCorpusStorage& cs, const ListCall& call, FrzMatchDev** d_result,
+                             cudaStream_t stream, FrzLaunchStats* st) {
     FrzWorkspace& ws = m->ws;
-    const bool reversed = sort == FRZ_SORT_INDEX_DESC || sort == FRZ_SORT_SCORE_THEN_INDEX_DESC;
-    const bool by_score = sort == FRZ_SORT_SCORE_THEN_INDEX_ASC || sort == FRZ_SORT_SCORE_THEN_INDEX_DESC;
-    const bool will_sort = rank || ord || (by_score && (cols ? cols->any_compiled : !m->compiled.empty()));
+    const bool reversed = sort_reversed(call.sort);
+    const bool will_sort = call.will_sort(*m);
+    const uint32_t limit = call.dev_limit();
+    const auto& rank = call.rank;
+    FrzMatchDev* const final_out = call.final_out;
     reset_call_state(m);
     FrzMatchDev* d_list = nullptr;
     uint32_t bound = 0;
-    // the fused histogram counts the scores of every row of the list, so a ranked or collapsed sort never asks for it
     FrzScoreHist hist;
-    if (cols) FRZ_TRY(match_patterns(m, cols->pats, cs, cols->live, index_offset, reversed, &d_list, &bound, stream, st, scope));
-    else FRZ_TRY(match_into_device(m, cs, index_offset, reversed, &d_list, &bound, stream, st, will_sort ? nullptr : final_out,
-                                   will_sort && !rank && !col && !ord ? &hist : nullptr, scope));
-    if (col) {
-        const uint8_t order = rank ? FRZ_COLLAPSE_BY_KEY : will_sort ? FRZ_COLLAPSE_BY_SCORE : FRZ_COLLAPSE_BY_INDEX;
-        FRZ_TRY(collapse_list(m, cs, *col, order, reversed, rank, &d_list, stream, st));
-    }
-    if (ord) {
-        FRZ_TRY(order_list(m, cs, *ord, reversed, limit, &d_list, stream, st));
-    } else if (will_sort) {   // `!self.patterns.is_empty() && sort.is_by_score()` (src/matcher/mod.rs:218)
+    if (call.cols) FRZ_TRY(match_patterns(m, call.cols->pats, cs, call.cols->live, call.index_offset, reversed, &d_list, &bound, stream, st,
+                                          call.scope));
+    else FRZ_TRY(match_into_device(m, cs, call.index_offset, reversed, &d_list, &bound, stream, st, call.scoring_out(*m),
+                                   call.fused_hist(*m) ? &hist : nullptr, call.scope));
+    if (call.col) FRZ_TRY(collapse_list(m, cs, *call.col, collapse_order(rank.has_value(), will_sort), reversed, rank, &d_list, stream, st));
+    if (call.ord) {
+        FRZ_TRY(order_list(m, cs, *call.ord, reversed, limit, &d_list, stream, st));
+    } else if (will_sort) {
         if (rank) bound = (uint32_t)std::min<uint64_t>((uint64_t)bound + rank->max_boost, 0xFFFF);   // the key bound
         FrzMatchDev* other = final_out ? final_out : (d_list == ws.matches_a.get() ? ws.matches_b.get() : ws.matches_a.get());
         // two-pass sort (score bound >= 1024) needs a scratch list of the corpus size: the multi-pattern ping-pong
@@ -1615,35 +1646,29 @@ frz_status copy_out(frz_matcher* m, FrzMatchDev* d_list, uint64_t limit, frz_mat
     return FRZ_OK;
 }
 
-// Matcher::match_list (into, from index_offset, in `sort` order) → host, truncated to its first `limit` rows (top-K calls:
-// the same pipeline with a limit on the final scatter and copy; UINT64_MAX for the whole list).  scope: the rows of a subset
-// call (match_into_device).  rank: a ranked call, col: a collapsed call (match_list_device); group_counts (optional, host,
-// col->n_groups entries) receives the list's rows per group.  cols: a frz_match_list_columns call whose starting column is
-// corpus (match_list_device).  ord: an ordered call (match_list_device).
-frz_status match_list_host(frz_matcher* m, const frz_corpus* corpus, uint32_t index_offset, uint8_t sort, uint64_t limit,
-                           const SubsetScope& scope, frz_match* out, uint64_t cap, uint64_t* n_out, uint64_t* n_total,
-                           const Ranking* rank = nullptr, const Collapse* col = nullptr, uint32_t* group_counts = nullptr,
-                           const Columns* cols = nullptr, const Ordering* ord = nullptr) {
-    if (scope.none) {
+// The call (match_list_device) → host: its first min(call.limit, total) rows (copy_out).
+frz_status match_list_host(frz_matcher* m, const frz_corpus* corpus, const ListCall& call, frz_match* out, uint64_t cap, uint64_t* n_out,
+                           uint64_t* n_total) {
+    const auto& col = call.col;
+    if (call.scope.none) {
         if (n_out) *n_out = 0;
         if (n_total) *n_total = 0;
-        if (col && group_counts) memset(group_counts, 0, col->n_groups * sizeof(uint32_t));
+        if (col && call.group_counts) memset(call.group_counts, 0, col->n_groups * sizeof(uint32_t));
         return FRZ_OK;
     }
     cudaStream_t stream = nullptr;
     FrzLaunchStats st;
     FrzMatchDev* d_list = nullptr;
-    const uint32_t dev_limit = (uint32_t)std::min<uint64_t>(limit, kFrzNoLimit);   // a list never holds more than 2^32 - 1 matches
     frz_status s = FRZ_OK;
     for (int attempt = 0; attempt < 2; attempt++) {
-        s = match_list_device(m, corpus->st, index_offset, sort, &d_list, stream, &st, nullptr, dev_limit, scope, rank, col, cols, ord);
-        if (s == FRZ_OK) s = copy_out(m, d_list, limit, out, cap, n_out, n_total, stream);
+        s = match_list_device(m, corpus->st, call, &d_list, stream, &st);
+        if (s == FRZ_OK) s = copy_out(m, d_list, call.limit, out, cap, n_out, n_total, stream);
         if (s != kRetryOverflow) break;
         FRZ_TRY(ensure_workspace(m, corpus->st, std::max<uint64_t>(corpus->st.n, 1)));  // worst-case lists, then once more
     }
     if (s == kRetryOverflow) s = frz_fail(FRZ_ERR_CUDA, "survivor list overflow persisted");
-    if (s == FRZ_OK && col && group_counts) {
-        FRZ_CUDA_TRY(cudaMemcpyAsync(group_counts, m->ws.collapse_counts.get(), col->n_groups * sizeof(uint32_t), cudaMemcpyDeviceToHost,
+    if (s == FRZ_OK && col && call.group_counts) {
+        FRZ_CUDA_TRY(cudaMemcpyAsync(call.group_counts, m->ws.collapse_counts.get(), col->n_groups * sizeof(uint32_t), cudaMemcpyDeviceToHost,
                                      stream));
         FRZ_CUDA_TRY(cudaStreamSynchronize(stream));
     }
@@ -1652,20 +1677,6 @@ frz_status match_list_host(frz_matcher* m, const frz_corpus* corpus, uint32_t in
 }
 
 }  // namespace
-
-extern "C" frz_status frz_match_list(frz_matcher* m, const frz_corpus* corpus, frz_match* out, uint64_t cap, uint64_t* n_out) {
-    if (!m || !corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
-    FRZ_TRY(frz_ensure_device(corpus->st.device));
-    return match_list_host(m, corpus, 0, m->config.sort, UINT64_MAX, SubsetScope(), out, cap, n_out, nullptr);
-}
-
-extern "C" frz_status frz_match_list_top(frz_matcher* m, const frz_corpus* corpus, uint64_t k, frz_match* out, uint64_t* n_out,
-                                         uint64_t* n_total) {
-    if (!m || !corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
-    if (!out && k > 0) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
-    FRZ_TRY(frz_ensure_device(corpus->st.device));
-    return match_list_host(m, corpus, 0, m->config.sort, k, SubsetScope(), out, k, n_out, n_total);
-}
 
 // ---------------------------------------------------------------------------------- batched top-K
 // frz_match_list_batch_collapsed, frz_match_list_batch and frz_match_list_batch_top (DESIGN.md §4.11), and
@@ -1822,8 +1833,8 @@ frz_status batch_run(frz_matcher* const* ms, const FrzBatchScope* scopes, const 
     for (uint32_t j = 0; j < ns; j++) {
         const uint8_t sort = bc ? bc->sort : ms[which[j]]->config.sort;
         if (!bc) h_pats[j] = ms[which[j]]->compiled[0].dev;
-        h_rev[j] = sort == FRZ_SORT_INDEX_DESC || sort == FRZ_SORT_SCORE_THEN_INDEX_DESC;
-        h_bysc[j] = sort == FRZ_SORT_SCORE_THEN_INDEX_ASC || sort == FRZ_SORT_SCORE_THEN_INDEX_DESC;
+        h_rev[j] = sort_reversed(sort);
+        h_bysc[j] = sort_by_score(sort);
         h_scope[j] = scopes ? scopes[which[j]] : FrzBatchScope();
         scoped |= h_scope[j].scoped || h_scope[j].ranked;
         if (gr.cols && gr.cols[which[j]].ids) {
@@ -2002,12 +2013,6 @@ extern "C" void frz_subset_destroy(frz_subset* s) { delete s; }
 #endif
 
 namespace {
-frz_status check_subset_call(const frz_matcher* m, const frz_corpus* corpus, const frz_subset* s) {
-    if (!m || !corpus || !s) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
-    if (s->corpus != corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "the subset was made on another corpus");
-    return frz_ensure_device(corpus->st.device);
-}
-
 // The rows of a subset call, built in the matcher's workspace on every call, so edits of the corpus between calls need no
 // bookkeeping.  Masked form: the corpus's slot metadata with every non-member an unused slot.  List form: the members
 // whose slots are in use, index-ordered.  An empty corpus keeps the default scope: it has no row.
@@ -2043,60 +2048,156 @@ frz_status subset_scope(frz_matcher* m, const frz_corpus* corpus, const frz_subs
 }
 }  // namespace
 
-extern "C" frz_status frz_match_list_subset(frz_matcher* m, const frz_corpus* corpus, const frz_subset* s, frz_match* out, uint64_t cap,
-                                            uint64_t* n_out) {
-    FRZ_TRY(check_subset_call(m, corpus, s));
-    SubsetScope scope;
-    FRZ_TRY(subset_scope(m, corpus, *s, nullptr, &scope));
-    return match_list_host(m, corpus, 0, m->config.sort, UINT64_MAX, scope, out, cap, n_out, nullptr);
-}
-
-extern "C" frz_status frz_match_list_subset_top(frz_matcher* m, const frz_corpus* corpus, const frz_subset* s, uint64_t k, frz_match* out,
-                                                uint64_t* n_out, uint64_t* n_total) {
-    FRZ_TRY(check_subset_call(m, corpus, s));
-    if (!out && k > 0) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
-    SubsetScope scope;
-    FRZ_TRY(subset_scope(m, corpus, *s, nullptr, &scope));
-    return match_list_host(m, corpus, 0, m->config.sort, k, scope, out, k, n_out, n_total);
-}
-
-// ---------------------------------------------------------------------------------- subsets from attributes
+// ---------------------------------------------------------------------------------- per-row handles
 static_assert(kFrzAttrNull == FRZ_ATTR_NULL && kFrzWhereMaxClauses == FRZ_WHERE_MAX_CLAUSES && kFrzWhereMaxIn == FRZ_WHERE_MAX_IN,
               "where_plan.cuh mirrors frz_cuda.h");
 
-// A signed 64-bit value per index of one corpus, on its device.  Indices at and past `values.cap()` are null.
-struct frz_attr {
-    const frz_corpus* corpus;
-    FrzDevArray<int64_t> values;
+// A value per index of one corpus, on its device, kept by index across corpus edits.  Indices at and past `values.cap()`
+// hold kFill.  The corpus comes first: the argument checks and frz_subset_where read it through any handle.
+template <typename T, T kFill>
+struct RowValues {
+    const frz_corpus* corpus = nullptr;
+    FrzDevArray<T> values;
 };
 
+// A signed 16-bit boost per index (ranked calls); 0 past the values.
+struct frz_boost : RowValues<int16_t, 0> {
+    int32_t max_set = 0;   // the largest value ever set, at least 0: bounds every boost (the sort's key bound)
+};
+// A group id per index (collapsed calls); in no group past the values.
+struct frz_groups : RowValues<uint32_t, FRZ_GROUP_NONE> {
+    uint64_t n_groups = 0;
+};
+// A signed 64-bit value per index (frz_subset_where, ordered calls); null past the values.
+struct frz_attr : RowValues<int64_t, kFrzAttrNull> {};
+
 namespace {
-// (index, value) pairs: x is the index
-__global__ void k_attr_scatter(const longlong2* __restrict__ set, uint64_t n, int64_t* __restrict__ values) {
+template <typename T>
+struct RowSet {   // one (index, value) pair of a *_set call
+    uint32_t index;
+    T value;
+};
+
+template <typename T>
+__global__ void k_row_values_scatter(const RowSet<T>* __restrict__ set, uint64_t n, T* __restrict__ values) {
     for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x)
-        values[set[j].x] = set[j].y;
+        values[set[j].index] = set[j].value;
 }
 
-__global__ void k_attr_fill_null(int64_t* __restrict__ values, uint64_t from, uint64_t to) {
+template <typename T>
+__global__ void k_row_values_fill(T* __restrict__ values, uint64_t from, uint64_t to, T fill) {
     for (uint64_t i = from + (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < to; i += (uint64_t)gridDim.x * blockDim.x)
-        values[i] = kFrzAttrNull;
+        values[i] = fill;
 }
 
-// a->values grows to `n` entries, the old values kept and the new ones null (FrzDevArray drops its contents when it grows,
-// and FRZ_ATTR_NULL is no byte pattern cudaMemset can write)
-frz_status grow_attr(frz_attr* a, uint64_t n) {
-    const uint64_t old = a->values.cap();
-    if (old >= n) return FRZ_OK;
-    FrzDevArray<int64_t> grown;
-    FRZ_TRY(grown.reserve(n));
-    k_attr_fill_null<<<grid_for(n - old, 256), 256>>>(grown.get(), old, n);
-    FRZ_CUDA_TRY(cudaGetLastError());
-    if (old) FRZ_CUDA_TRY(cudaMemcpy(grown.get(), a->values.get(), old * sizeof(int64_t), cudaMemcpyDeviceToDevice));
-    FRZ_CUDA_TRY(cudaStreamSynchronize(nullptr));
-    a->values = std::move(grown);
+frz_status no_check() { return FRZ_OK; }
+
+// frz_*_create: a handle of c holding values[0, n).  what: the values' name in the length message; check: the handle's
+// own checks, after the length.
+template <class H, typename T, class Check>
+frz_status row_values_create(const frz_corpus* c, const T* values, uint64_t n, H** out, const char* what, Check check) {
+    if (!c || !out || (n && !values)) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    if (n > c->st.n)
+        return frz_fail(FRZ_ERR_INVALID_ARG, "%llu %s for a corpus of %llu haystacks", (unsigned long long)n, what, (unsigned long long)c->st.n);
+    FRZ_TRY(check());
+    auto h = std::make_unique<H>();
+    h->corpus = c;
+    if (n) {
+        FRZ_TRY(frz_ensure_device(c->st.device));
+        FRZ_TRY(h->values.reserve(n));
+        FRZ_CUDA_TRY(cudaMemcpy(h->values.get(), values, n * sizeof(T), cudaMemcpyHostToDevice));
+    }
+    *out = h.release();
     return FRZ_OK;
 }
 
+// frz_*_set: values[which[j]] = v[j] for rows below the corpus's length, each at most once.  check: the handle's own checks
+// on v, before the duplicate check.  An index past the values first grows them to the corpus's length, the old values kept
+// and the new ones kFill (FrzDevArray drops its contents when it grows).
+template <typename T, T kFill, class Check>
+frz_status row_values_set(RowValues<T, kFill>* h, const uint32_t* which, const T* v, uint64_t n, Check check) {
+    if (!h || (n && (!which || !v))) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    if (n == 0) return FRZ_OK;
+    FRZ_TRY(check_indices(h->corpus, which, n));
+    FRZ_TRY(check());
+    std::vector<uint32_t> sorted(which, which + n);
+    std::sort(sorted.begin(), sorted.end());
+    for (uint64_t j = 1; j < n; j++)
+        if (sorted[j] == sorted[j - 1]) return frz_fail(FRZ_ERR_INVALID_ARG, "index %u is set twice", sorted[j]);
+    std::vector<RowSet<T>> set(n);
+    for (uint64_t j = 0; j < n; j++) set[j] = RowSet<T>{which[j], v[j]};
+    FRZ_TRY(frz_ensure_device(h->corpus->st.device));
+    if (sorted.back() >= h->values.cap()) {
+        const uint64_t old = h->values.cap(), rows = h->corpus->st.n;
+        FrzDevArray<T> grown;
+        FRZ_TRY(grown.reserve(rows));
+        k_row_values_fill<<<grid_for(rows - old, 256), 256>>>(grown.get(), old, rows, kFill);
+        FRZ_CUDA_TRY(cudaGetLastError());
+        if (old) FRZ_CUDA_TRY(cudaMemcpy(grown.get(), h->values.get(), old * sizeof(T), cudaMemcpyDeviceToDevice));
+        FRZ_CUDA_TRY(cudaStreamSynchronize(nullptr));
+        h->values = std::move(grown);
+    }
+    FrzDevArray<RowSet<T>> d_set;   // one copy, one scatter
+    FRZ_TRY(d_set.reserve(n));
+    FRZ_CUDA_TRY(cudaMemcpy(d_set.get(), set.data(), n * sizeof(RowSet<T>), cudaMemcpyHostToDevice));
+    k_row_values_scatter<<<grid_for(n, 256), 256>>>(d_set.get(), n, h->values.get());
+    FRZ_CUDA_TRY(cudaGetLastError());
+    FRZ_CUDA_TRY(cudaStreamSynchronize(nullptr));
+    return FRZ_OK;
+}
+
+// every id is below n_groups or FRZ_GROUP_NONE
+frz_status check_group_ids(const uint32_t* ids, uint64_t n, uint64_t n_groups) {
+    for (uint64_t j = 0; j < n; j++)
+        if (ids[j] != FRZ_GROUP_NONE && ids[j] >= n_groups)
+            return frz_fail(FRZ_ERR_INVALID_ARG, "group id %u is not below n_groups = %llu", ids[j], (unsigned long long)n_groups);
+    return FRZ_OK;
+}
+}  // namespace
+
+extern "C" frz_status frz_boost_create(const frz_corpus* c, const int16_t* values, uint64_t n, frz_boost** out) {
+    FRZ_TRY(row_values_create(c, values, n, out, "boost values", no_check));
+    if (n) (*out)->max_set = std::max<int32_t>(0, *std::max_element(values, values + n));
+    return FRZ_OK;
+}
+
+extern "C" frz_status frz_boost_set(frz_boost* b, const uint32_t* which, const int16_t* values, uint64_t n) {
+    FRZ_TRY(row_values_set(b, which, values, n, no_check));
+    if (n) b->max_set = std::max<int32_t>(b->max_set, *std::max_element(values, values + n));
+    return FRZ_OK;
+}
+
+extern "C" void frz_boost_destroy(frz_boost* b) { delete b; }
+
+extern "C" frz_status frz_groups_create(const frz_corpus* c, const uint32_t* ids, uint64_t n, uint64_t n_groups, frz_groups** out) {
+    FRZ_TRY(row_values_create(c, ids, n, out, "group ids", [&]() -> frz_status {
+        if (n_groups == 0 || n_groups > FRZ_GROUP_NONE)
+            return frz_fail(FRZ_ERR_INVALID_ARG, "n_groups = %llu is not in 1 .. 2^32 - 1", (unsigned long long)n_groups);
+        return check_group_ids(ids, n, n_groups);
+    }));
+    (*out)->n_groups = n_groups;
+    return FRZ_OK;
+}
+
+extern "C" frz_status frz_groups_set(frz_groups* g, const uint32_t* which, const uint32_t* ids, uint64_t n) {
+    return row_values_set(g, which, ids, n, [&] { return check_group_ids(ids, n, g->n_groups); });
+}
+
+extern "C" uint64_t frz_groups_count(const frz_groups* g) { return g ? g->n_groups : 0; }
+extern "C" void frz_groups_destroy(frz_groups* g) { delete g; }
+
+extern "C" frz_status frz_attr_create(const frz_corpus* c, const int64_t* values, uint64_t n, frz_attr** out) {
+    return row_values_create(c, values, n, out, "attribute values", no_check);
+}
+
+extern "C" frz_status frz_attr_set(frz_attr* a, const uint32_t* which, const int64_t* values, uint64_t n) {
+    return row_values_set(a, which, values, n, no_check);
+}
+
+extern "C" void frz_attr_destroy(frz_attr* a) { delete a; }
+
+// ---------------------------------------------------------------------------------- subsets from attributes
+namespace {
 // The device work of frz_subset_where once every argument has passed: k_where writes the bitmap and the chunk counts,
 // k_scan_blocks scans the counts, one 8-byte read-back gives the member count, and k_where_members writes the list.  The
 // bitmap is written in place unless it must grow; then into a new array, because `base` may be s's old bitmap.
@@ -2140,45 +2241,6 @@ frz_status where_fill(frz_subset* s, FrzWhereDev& w, const std::vector<int64_t>&
 }
 }  // namespace
 
-extern "C" frz_status frz_attr_create(const frz_corpus* c, const int64_t* values, uint64_t n, frz_attr** out) {
-    if (!c || !out || (n && !values)) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
-    if (n > c->st.n)
-        return frz_fail(FRZ_ERR_INVALID_ARG, "%llu attribute values for a corpus of %llu haystacks", (unsigned long long)n,
-                        (unsigned long long)c->st.n);
-    auto a = std::make_unique<frz_attr>();
-    a->corpus = c;
-    if (n) {
-        FRZ_TRY(frz_ensure_device(c->st.device));
-        FRZ_TRY(a->values.reserve(n));
-        FRZ_CUDA_TRY(cudaMemcpy(a->values.get(), values, n * sizeof(int64_t), cudaMemcpyHostToDevice));
-    }
-    *out = a.release();
-    return FRZ_OK;
-}
-
-extern "C" frz_status frz_attr_set(frz_attr* a, const uint32_t* which, const int64_t* values, uint64_t n) {
-    if (!a || (n && (!which || !values))) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
-    if (n == 0) return FRZ_OK;
-    FRZ_TRY(check_indices(a->corpus, which, n));
-    std::vector<uint32_t> sorted(which, which + n);
-    std::sort(sorted.begin(), sorted.end());
-    for (uint64_t j = 1; j < n; j++)
-        if (sorted[j] == sorted[j - 1]) return frz_fail(FRZ_ERR_INVALID_ARG, "index %u is set twice", sorted[j]);
-    std::vector<longlong2> set(n);
-    for (uint64_t j = 0; j < n; j++) set[j] = make_longlong2((long long)which[j], (long long)values[j]);
-    FRZ_TRY(frz_ensure_device(a->corpus->st.device));
-    if (sorted.back() >= a->values.cap()) FRZ_TRY(grow_attr(a, a->corpus->st.n));
-    FrzDevArray<longlong2> d_set;   // (index, value) pairs: one copy, one scatter
-    FRZ_TRY(d_set.reserve(n));
-    FRZ_CUDA_TRY(cudaMemcpy(d_set.get(), set.data(), n * sizeof(longlong2), cudaMemcpyHostToDevice));
-    k_attr_scatter<<<grid_for(n, 256), 256>>>(d_set.get(), n, a->values.get());
-    FRZ_CUDA_TRY(cudaGetLastError());
-    FRZ_CUDA_TRY(cudaStreamSynchronize(nullptr));
-    return FRZ_OK;
-}
-
-extern "C" void frz_attr_destroy(frz_attr* a) { delete a; }
-
 extern "C" frz_status frz_subset_where(frz_subset* s, const frz_where_clause* clauses, uint64_t n_clauses, const frz_subset* base) {
     if (!s || (n_clauses && !clauses)) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
     if (n_clauses > FRZ_WHERE_MAX_CLAUSES)
@@ -2214,96 +2276,118 @@ extern "C" frz_status frz_subset_where(frz_subset* s, const frz_where_clause* cl
     return where_fill(s, w, sets, base);
 }
 
-// ---------------------------------------------------------------------------------- ranked calls
-// A signed 16-bit boost per index of one corpus, on its device.  Indices at and past `values.cap()` have boost 0.
-struct frz_boost {
-    const frz_corpus* corpus;
-    FrzDevArray<int16_t> values;
-    int32_t max_set = 0;   // the largest value ever set, at least 0: bounds every boost (the sort's key bound)
+// ---------------------------------------------------------------------------------- single-query list calls
+namespace {
+constexpr uint64_t kNoQuery = UINT64_MAX;   // the check is of a single call: its message names no query
+
+// The handles of one query: the optional subset, boost, groups with their per-group cap, and attribute with its order.
+struct CallHandles {
+    const frz_subset* s = nullptr;
+    const frz_boost* b = nullptr;
+    const frz_groups* g = nullptr;
+    uint64_t per_group = 1;
+    const frz_attr* a = nullptr;
+    uint32_t order = 0;
 };
 
-namespace {
-__global__ void k_boost_scatter(const uint2* __restrict__ set, uint64_t n, int16_t* __restrict__ values) {
-    for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x)
-        values[set[j].x] = (int16_t)set[j].y;
-}
-
-// b->values grows to `n` entries, the old values kept and the new ones zero (FrzDevArray drops its contents when it grows)
-frz_status grow_boost(frz_boost* b, uint64_t n) {
-    if (b->values.cap() >= n) return FRZ_OK;
-    FrzDevArray<int16_t> grown;
-    FRZ_TRY(grown.reserve(n));
-    FRZ_CUDA_TRY(cudaMemset(grown.get(), 0, n * sizeof(int16_t)));
-    if (b->values.cap())
-        FRZ_CUDA_TRY(cudaMemcpy(grown.get(), b->values.get(), b->values.cap() * sizeof(int16_t), cudaMemcpyDeviceToDevice));
-    b->values = std::move(grown);
+// per_group is 1..kFrzCollapseMaxPerGroup, or UINT64_MAX for no cap
+frz_status check_per_group(uint64_t per_group, uint64_t query = kNoQuery) {
+    char at[32] = "";
+    if (query != kNoQuery) snprintf(at, sizeof at, " at %llu", (unsigned long long)query);
+    if (per_group == 0) return frz_fail(FRZ_ERR_INVALID_ARG, "per_group = 0%s", at);
+    if (per_group > kFrzCollapseMaxPerGroup && per_group != UINT64_MAX)
+        return frz_fail(FRZ_ERR_UNSUPPORTED, "per_group = %llu%s: at most %llu rows per group, or UINT64_MAX for no cap",
+                        (unsigned long long)per_group, at, (unsigned long long)kFrzCollapseMaxPerGroup);
     return FRZ_OK;
 }
 
-Ranking ranking_of(const frz_boost& b) {
-    Ranking rank;
-    rank.boost = b.values.get();
-    rank.n = (uint32_t)b.values.cap();
-    rank.max_boost = (uint32_t)b.max_set;
-    return rank;
+// Every handle of a query was made on one of `mine`: the call's corpus, or for a column call any of its columns
+// (membership, boosts, group ids and values are by index, so a handle of any column serves every column).  The first that
+// was not is reported, in the order subset, boost, groups, attribute; made_on names `mine` in the message.
+constexpr const char* kAnotherCorpus = "another corpus";
+constexpr const char* kNoColumn = "none of the columns";
+frz_status check_handles(const CallHandles& h, const frz_corpus* const* mine, uint64_t n_mine, const char* made_on,
+                         uint64_t query = kNoQuery) {
+    const auto foreign = [&](const auto* handle) { return handle && std::find(mine, mine + n_mine, handle->corpus) == mine + n_mine; };
+    const char* what = foreign(h.s) ? "subset" : foreign(h.b) ? "boost" : foreign(h.g) ? "groups" : foreign(h.a) ? "attribute" : nullptr;
+    if (!what) return FRZ_OK;
+    char of[40] = "";
+    if (query != kNoQuery) snprintf(of, sizeof of, " of query %llu", (unsigned long long)query);
+    return frz_fail(FRZ_ERR_INVALID_ARG, "the %s%s %s made on %s", what, of, strcmp(what, "groups") == 0 ? "were" : "was", made_on);
+}
+
+// The list call of a query whose arguments have passed, on the corpus's device: the matcher's sort strategy, the first k
+// rows, the subset's rows built against `corpus` (subset_scope), the boost as a ranking (with an attribute, as part of the
+// order key instead: order_plan.cuh) and the groups as a collapse.
+frz_status resolve_call(frz_matcher* m, const frz_corpus* corpus, const CallHandles& h, uint64_t k, ListCall* call) {
+    FRZ_TRY(frz_ensure_device(corpus->st.device));
+    call->sort = m->config.sort;
+    call->limit = k;
+    if (h.s) FRZ_TRY(subset_scope(m, corpus, *h.s, nullptr, &call->scope));
+    if (h.a) {
+        FrzOrderDev o{};
+        o.values = h.a->values.get();
+        o.n_values = h.a->values.cap();
+        o.boost = h.b ? h.b->values.get() : nullptr;
+        o.n_boost = h.b ? (uint32_t)h.b->values.cap() : 0;
+        o.order = h.order;
+        call->ord = Ordering{o};
+    } else if (h.b) {
+        call->rank = Ranking{h.b->values.get(), (uint32_t)h.b->values.cap(), (uint32_t)h.b->max_set};
+    }
+    if (h.g) call->col = Collapse{h.g->values.get(), h.g->values.cap(), h.g->n_groups, h.per_group};
+    return FRZ_OK;
+}
+
+// A single-query call whose arguments have passed (and every query of a batched call that runs on its own): its list
+// call, run, the first min(k, total) rows → out.
+frz_status list_call(frz_matcher* m, const frz_corpus* corpus, const CallHandles& h, uint64_t k, frz_match* out, uint64_t cap,
+                     uint64_t* n_out, uint64_t* n_total, uint32_t* group_counts = nullptr) {
+    ListCall call;
+    FRZ_TRY(resolve_call(m, corpus, h, k, &call));
+    call.group_counts = group_counts;
+    return match_list_host(m, corpus, call, out, cap, n_out, n_total);
 }
 }  // namespace
 
-extern "C" frz_status frz_boost_create(const frz_corpus* c, const int16_t* values, uint64_t n, frz_boost** out) {
-    if (!c || !out || (n && !values)) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
-    if (n > c->st.n)
-        return frz_fail(FRZ_ERR_INVALID_ARG, "%llu boost values for a corpus of %llu haystacks", (unsigned long long)n,
-                        (unsigned long long)c->st.n);
-    auto b = std::make_unique<frz_boost>();
-    b->corpus = c;
-    if (n) {
-        FRZ_TRY(frz_ensure_device(c->st.device));
-        FRZ_TRY(b->values.reserve(n));
-        FRZ_CUDA_TRY(cudaMemcpy(b->values.get(), values, n * sizeof(int16_t), cudaMemcpyHostToDevice));
-        b->max_set = std::max<int32_t>(0, *std::max_element(values, values + n));
-    }
-    *out = b.release();
-    return FRZ_OK;
+extern "C" frz_status frz_match_list(frz_matcher* m, const frz_corpus* corpus, frz_match* out, uint64_t cap, uint64_t* n_out) {
+    if (!m || !corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    return list_call(m, corpus, CallHandles(), UINT64_MAX, out, cap, n_out, nullptr);
 }
 
-extern "C" frz_status frz_boost_set(frz_boost* b, const uint32_t* which, const int16_t* values, uint64_t n) {
-    if (!b || (n && (!which || !values))) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
-    if (n == 0) return FRZ_OK;
-    FRZ_TRY(check_indices(b->corpus, which, n));
-    std::vector<uint2> set(n);
-    for (uint64_t j = 0; j < n; j++) set[j] = make_uint2(which[j], (uint32_t)(uint16_t)values[j]);
-    std::vector<uint32_t> sorted(which, which + n);
-    std::sort(sorted.begin(), sorted.end());
-    for (uint64_t j = 1; j < n; j++)
-        if (sorted[j] == sorted[j - 1]) return frz_fail(FRZ_ERR_INVALID_ARG, "index %u is set twice", sorted[j]);
-    FRZ_TRY(frz_ensure_device(b->corpus->st.device));
-    if (sorted.back() >= b->values.cap()) FRZ_TRY(grow_boost(b, b->corpus->st.n));
-    FrzDevArray<uint2> d_set;   // (index, value) pairs: one copy, one scatter
-    FRZ_TRY(d_set.reserve(n));
-    FRZ_CUDA_TRY(cudaMemcpy(d_set.get(), set.data(), n * sizeof(uint2), cudaMemcpyHostToDevice));
-    k_boost_scatter<<<grid_for(n, 256), 256>>>(d_set.get(), n, b->values.get());
-    FRZ_CUDA_TRY(cudaGetLastError());
-    FRZ_CUDA_TRY(cudaStreamSynchronize(nullptr));
-    b->max_set = std::max<int32_t>(b->max_set, *std::max_element(values, values + n));
-    return FRZ_OK;
+extern "C" frz_status frz_match_list_top(frz_matcher* m, const frz_corpus* corpus, uint64_t k, frz_match* out, uint64_t* n_out,
+                                         uint64_t* n_total) {
+    if (!m || !corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    if (!out && k > 0) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
+    return list_call(m, corpus, CallHandles(), k, out, k, n_out, n_total);
 }
 
-extern "C" void frz_boost_destroy(frz_boost* b) { delete b; }
+extern "C" frz_status frz_match_list_subset(frz_matcher* m, const frz_corpus* corpus, const frz_subset* s, frz_match* out, uint64_t cap,
+                                            uint64_t* n_out) {
+    if (!m || !corpus || !s) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    const CallHandles h{s};
+    FRZ_TRY(check_handles(h, &corpus, 1, kAnotherCorpus));
+    return list_call(m, corpus, h, UINT64_MAX, out, cap, n_out, nullptr);
+}
+
+extern "C" frz_status frz_match_list_subset_top(frz_matcher* m, const frz_corpus* corpus, const frz_subset* s, uint64_t k, frz_match* out,
+                                                uint64_t* n_out, uint64_t* n_total) {
+    if (!m || !corpus || !s) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    const CallHandles h{s};
+    FRZ_TRY(check_handles(h, &corpus, 1, kAnotherCorpus));
+    if (!out && k > 0) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
+    return list_call(m, corpus, h, k, out, k, n_out, n_total);
+}
 
 extern "C" frz_status frz_match_list_ranked(frz_matcher* m, const frz_corpus* corpus, const frz_subset* s, const frz_boost* b,
                                             uint64_t k, frz_match* out, uint64_t* n_out, uint64_t* n_total) {
     if (!m || !corpus || !b) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
     if (!out && k > 0) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
-    if (b->corpus != corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "the boost was made on another corpus");
-    if (s) FRZ_TRY(check_subset_call(m, corpus, s));
-    FRZ_TRY(frz_ensure_device(corpus->st.device));
-    SubsetScope scope;
-    if (s) FRZ_TRY(subset_scope(m, corpus, *s, nullptr, &scope));
-    const Ranking rank = ranking_of(*b);
-    return match_list_host(m, corpus, 0, m->config.sort, k, scope, out, k, n_out, n_total, &rank);
+    const CallHandles h{s, b};
+    FRZ_TRY(check_handles(h, &corpus, 1, kAnotherCorpus));
+    return list_call(m, corpus, h, k, out, k, n_out, n_total);
 }
 
-// ---------------------------------------------------------------------------------- ordered calls
 static_assert(FRZ_ORDER_SCORE_THEN_ATTR_DESC == kFrzOrderScoreFirst && FRZ_ORDER_SCORE_THEN_ATTR_ASC + 1 == kFrzOrderCount &&
                   (FRZ_ORDER_ATTR_ASC & 1) && (FRZ_ORDER_SCORE_THEN_ATTR_ASC & 1) && !(FRZ_ORDER_ATTR_DESC & 1),
               "order_plan.cuh mirrors frz_cuda.h");
@@ -2314,143 +2398,44 @@ extern "C" frz_status frz_match_list_ordered(frz_matcher* m, const frz_corpus* c
     if (!m || !corpus || !a) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
     if (!out && k > 0) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
     if (order >= kFrzOrderCount) return frz_fail(FRZ_ERR_INVALID_ARG, "order %u (at most %u)", order, kFrzOrderCount - 1);
-    if (a->corpus != corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "the attribute was made on another corpus");
-    if (b && b->corpus != corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "the boost was made on another corpus");
-    if (s) FRZ_TRY(check_subset_call(m, corpus, s));
-    FRZ_TRY(frz_ensure_device(corpus->st.device));
-    SubsetScope scope;
-    if (s) FRZ_TRY(subset_scope(m, corpus, *s, nullptr, &scope));
-    Ordering ord;
-    ord.dev = FrzOrderDev{};
-    ord.dev.values = a->values.get();
-    ord.dev.n_values = a->values.cap();
-    ord.dev.boost = b ? b->values.get() : nullptr;
-    ord.dev.n_boost = b ? (uint32_t)b->values.cap() : 0;
-    ord.dev.order = order;
-    return match_list_host(m, corpus, 0, m->config.sort, k, scope, out, k, n_out, n_total, nullptr, nullptr, nullptr, nullptr, &ord);
+    const CallHandles h{s, b, nullptr, 1, a, order};
+    FRZ_TRY(check_handles(h, &corpus, 1, kAnotherCorpus));
+    return list_call(m, corpus, h, k, out, k, n_out, n_total);
 }
-
-// ---------------------------------------------------------------------------------- collapsed calls
-// A group id per index of one corpus, on its device.  Indices at and past `ids.cap()` are in no group.
-struct frz_groups {
-    const frz_corpus* corpus;
-    FrzDevArray<uint32_t> ids;
-    uint64_t n_groups;
-};
-
-namespace {
-__global__ void k_groups_scatter(const uint2* __restrict__ set, uint64_t n, uint32_t* __restrict__ ids) {
-    for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x)
-        ids[set[j].x] = set[j].y;
-}
-
-// every id is below n_groups or FRZ_GROUP_NONE
-frz_status check_group_ids(const uint32_t* ids, uint64_t n, uint64_t n_groups) {
-    for (uint64_t j = 0; j < n; j++)
-        if (ids[j] != FRZ_GROUP_NONE && ids[j] >= n_groups)
-            return frz_fail(FRZ_ERR_INVALID_ARG, "group id %u is not below n_groups = %llu", ids[j], (unsigned long long)n_groups);
-    return FRZ_OK;
-}
-
-// g->ids grows to `n` entries, the old ids kept and the new ones FRZ_GROUP_NONE (FrzDevArray drops its contents when it grows)
-frz_status grow_groups(frz_groups* g, uint64_t n) {
-    if (g->ids.cap() >= n) return FRZ_OK;
-    FrzDevArray<uint32_t> grown;
-    FRZ_TRY(grown.reserve(n));
-    FRZ_CUDA_TRY(cudaMemset(grown.get(), 0xFF, n * sizeof(uint32_t)));
-    if (g->ids.cap())
-        FRZ_CUDA_TRY(cudaMemcpy(grown.get(), g->ids.get(), g->ids.cap() * sizeof(uint32_t), cudaMemcpyDeviceToDevice));
-    g->ids = std::move(grown);
-    return FRZ_OK;
-}
-
-Collapse collapse_of(const frz_groups& g, uint64_t per_group) {
-    Collapse col;
-    col.ids = g.ids.get();
-    col.n_ids = g.ids.cap();
-    col.n_groups = g.n_groups;
-    col.per_group = per_group;
-    return col;
-}
-}  // namespace
-
-extern "C" frz_status frz_groups_create(const frz_corpus* c, const uint32_t* ids, uint64_t n, uint64_t n_groups, frz_groups** out) {
-    if (!c || !out || (n && !ids)) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
-    if (n > c->st.n)
-        return frz_fail(FRZ_ERR_INVALID_ARG, "%llu group ids for a corpus of %llu haystacks", (unsigned long long)n,
-                        (unsigned long long)c->st.n);
-    if (n_groups == 0 || n_groups > FRZ_GROUP_NONE)
-        return frz_fail(FRZ_ERR_INVALID_ARG, "n_groups = %llu is not in 1 .. 2^32 - 1", (unsigned long long)n_groups);
-    FRZ_TRY(check_group_ids(ids, n, n_groups));
-    auto g = std::make_unique<frz_groups>();
-    g->corpus = c;
-    g->n_groups = n_groups;
-    if (n) {
-        FRZ_TRY(frz_ensure_device(c->st.device));
-        FRZ_TRY(g->ids.reserve(n));
-        FRZ_CUDA_TRY(cudaMemcpy(g->ids.get(), ids, n * sizeof(uint32_t), cudaMemcpyHostToDevice));
-    }
-    *out = g.release();
-    return FRZ_OK;
-}
-
-extern "C" frz_status frz_groups_set(frz_groups* g, const uint32_t* which, const uint32_t* ids, uint64_t n) {
-    if (!g || (n && (!which || !ids))) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
-    if (n == 0) return FRZ_OK;
-    FRZ_TRY(check_indices(g->corpus, which, n));
-    FRZ_TRY(check_group_ids(ids, n, g->n_groups));
-    std::vector<uint32_t> sorted(which, which + n);
-    std::sort(sorted.begin(), sorted.end());
-    for (uint64_t j = 1; j < n; j++)
-        if (sorted[j] == sorted[j - 1]) return frz_fail(FRZ_ERR_INVALID_ARG, "index %u is set twice", sorted[j]);
-    std::vector<uint2> set(n);
-    for (uint64_t j = 0; j < n; j++) set[j] = make_uint2(which[j], ids[j]);
-    FRZ_TRY(frz_ensure_device(g->corpus->st.device));
-    if (sorted.back() >= g->ids.cap()) FRZ_TRY(grow_groups(g, g->corpus->st.n));
-    FrzDevArray<uint2> d_set;   // (index, id) pairs: one copy, one scatter
-    FRZ_TRY(d_set.reserve(n));
-    FRZ_CUDA_TRY(cudaMemcpy(d_set.get(), set.data(), n * sizeof(uint2), cudaMemcpyHostToDevice));
-    k_groups_scatter<<<grid_for(n, 256), 256>>>(d_set.get(), n, g->ids.get());
-    FRZ_CUDA_TRY(cudaGetLastError());
-    FRZ_CUDA_TRY(cudaStreamSynchronize(nullptr));
-    return FRZ_OK;
-}
-
-extern "C" uint64_t frz_groups_count(const frz_groups* g) { return g ? g->n_groups : 0; }
-extern "C" void frz_groups_destroy(frz_groups* g) { delete g; }
 
 extern "C" frz_status frz_match_list_collapsed(frz_matcher* m, const frz_corpus* corpus, const frz_subset* s, const frz_boost* b,
                                                const frz_groups* g, uint64_t per_group, uint64_t k, frz_match* out, uint64_t* n_out,
                                                uint64_t* n_total, uint32_t* group_counts) {
     if (!m || !corpus || !g) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
-    if (per_group == 0) return frz_fail(FRZ_ERR_INVALID_ARG, "per_group = 0");
-    if (per_group > kFrzCollapseMaxPerGroup && per_group != UINT64_MAX)
-        return frz_fail(FRZ_ERR_UNSUPPORTED, "per_group = %llu: at most %llu rows per group, or UINT64_MAX for no cap",
-                        (unsigned long long)per_group, (unsigned long long)kFrzCollapseMaxPerGroup);
+    FRZ_TRY(check_per_group(per_group));
     if (!out && k > 0) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
-    if (g->corpus != corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "the groups were made on another corpus");
-    if (b && b->corpus != corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "the boost was made on another corpus");
-    if (s && s->corpus != corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "the subset was made on another corpus");
-    FRZ_TRY(frz_ensure_device(corpus->st.device));
-    SubsetScope scope;
-    if (s) FRZ_TRY(subset_scope(m, corpus, *s, nullptr, &scope));
-    Ranking rank;
-    if (b) rank = ranking_of(*b);
-    const Collapse col = collapse_of(*g, per_group);
-    return match_list_host(m, corpus, 0, m->config.sort, k, scope, out, k, n_out, n_total, b ? &rank : nullptr, &col, group_counts);
+    const CallHandles h{s, b, g, per_group};
+    FRZ_TRY(check_handles(h, &corpus, 1, kAnotherCorpus));
+    return list_call(m, corpus, h, k, out, k, n_out, n_total, group_counts);
 }
 
 // ---------------------------------------------------------------------------------- column calls
-// Several text fields of the same rows, one matcher per field (DESIGN.md §4.13): the multi-pattern loop over every
-// column's patterns in column order, each against its own column (match_patterns), then the ranked, collapsed and top-K
-// steps of the single-corpus calls.
-extern "C" frz_status frz_match_list_columns(frz_matcher* const* ms, const frz_corpus* const* cols, uint64_t n_cols, uint8_t sort,
-                                             const frz_subset* s, const frz_boost* b, const frz_groups* g, uint64_t per_group,
-                                             uint64_t k, frz_match* out, uint64_t* n_out, uint64_t* n_total, uint32_t* group_counts) {
+namespace {
+// The column set of a column call: at least one column, no null matcher or corpus, every column on one device and of one
+// length (one index space) within the u32 index range, and `sort` a strategy.  The matchers are ms[c] (frz_match_list_columns,
+// batch_q == nullptr), or *batch_q queries' ms[j * n_cols + c] (frz_match_list_batch_columns).
+frz_status check_columns(frz_matcher* const* ms, const frz_corpus* const* cols, uint64_t n_cols, uint8_t sort, const uint64_t* batch_q) {
     if (n_cols == 0) return frz_fail(FRZ_ERR_INVALID_ARG, "n_cols = 0: a columns call needs at least one column");
     if (!ms || !cols) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
-    for (uint64_t c = 0; c < n_cols; c++)
-        if (!ms[c] || !cols[c]) return frz_fail(FRZ_ERR_INVALID_ARG, "null matcher or corpus of column %llu", (unsigned long long)c);
+    if (!batch_q) {
+        for (uint64_t c = 0; c < n_cols; c++)
+            if (!ms[c] || !cols[c]) return frz_fail(FRZ_ERR_INVALID_ARG, "null matcher or corpus of column %llu", (unsigned long long)c);
+    } else {
+        const uint64_t q = *batch_q;
+        for (uint64_t c = 0; c < n_cols; c++)
+            if (!cols[c]) return frz_fail(FRZ_ERR_INVALID_ARG, "null corpus of column %llu", (unsigned long long)c);
+        if (q > UINT64_MAX / n_cols || q * n_cols > SIZE_MAX / sizeof(frz_matcher*))
+            return frz_fail(FRZ_ERR_INVALID_ARG, "q * n_cols overflows: q = %llu, n_cols = %llu", (unsigned long long)q, (unsigned long long)n_cols);
+        for (uint64_t i = 0; i < q * n_cols; i++)
+            if (!ms[i])
+                return frz_fail(FRZ_ERR_INVALID_ARG, "null matcher of query %llu, column %llu", (unsigned long long)(i / n_cols),
+                                (unsigned long long)(i % n_cols));
+    }
     const FrzCorpusStorage& first = cols[0]->st;
     for (uint64_t c = 1; c < n_cols; c++) {
         if (cols[c]->st.device != first.device)
@@ -2462,17 +2447,22 @@ extern "C" frz_status frz_match_list_columns(frz_matcher* const* ms, const frz_c
     }
     FRZ_TRY(frz_check_index_range(first.n, 0));
     if (sort > FRZ_SORT_INDEX_DESC) return frz_fail(FRZ_ERR_INVALID_ARG, "sort = %u is not a sort strategy", (unsigned)sort);
-    if (g && per_group == 0) return frz_fail(FRZ_ERR_INVALID_ARG, "per_group = 0");
-    if (g && per_group > kFrzCollapseMaxPerGroup && per_group != UINT64_MAX)
-        return frz_fail(FRZ_ERR_UNSUPPORTED, "per_group = %llu: at most %llu rows per group, or UINT64_MAX for no cap",
-                        (unsigned long long)per_group, (unsigned long long)kFrzCollapseMaxPerGroup);
+    return FRZ_OK;
+}
+}  // namespace
+
+// Several text fields of the same rows, one matcher per field (DESIGN.md §4.13): the multi-pattern loop over every
+// column's patterns in column order, each against its own column (match_patterns), then the ranked, collapsed and top-K
+// steps of the single-corpus calls.
+extern "C" frz_status frz_match_list_columns(frz_matcher* const* ms, const frz_corpus* const* cols, uint64_t n_cols, uint8_t sort,
+                                             const frz_subset* s, const frz_boost* b, const frz_groups* g, uint64_t per_group,
+                                             uint64_t k, frz_match* out, uint64_t* n_out, uint64_t* n_total, uint32_t* group_counts) {
+    FRZ_TRY(check_columns(ms, cols, n_cols, sort, nullptr));
+    if (g) FRZ_TRY(check_per_group(per_group));
     if (!out && k > 0) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
-    // membership, boosts and group ids are by index, so a handle of any column serves every column
-    const auto of_a_column = [&](const frz_corpus* h) { return std::find(cols, cols + n_cols, h) != cols + n_cols; };
-    if (s && !of_a_column(s->corpus)) return frz_fail(FRZ_ERR_INVALID_ARG, "the subset was made on none of the columns");
-    if (b && !of_a_column(b->corpus)) return frz_fail(FRZ_ERR_INVALID_ARG, "the boost was made on none of the columns");
-    if (g && !of_a_column(g->corpus)) return frz_fail(FRZ_ERR_INVALID_ARG, "the groups were made on none of the columns");
-    FRZ_TRY(frz_ensure_device(first.device));
+    const CallHandles h{s, b, g, per_group};
+    FRZ_TRY(check_handles(h, cols, n_cols, kNoColumn));
+    FRZ_TRY(frz_ensure_device(cols[0]->st.device));   // (before a matcher is read)
     // the list starts from the column of the first non-negated pattern (its base, scanned in full), else from column 0
     Columns cs;
     uint64_t start = n_cols;
@@ -2489,33 +2479,15 @@ extern "C" frz_status frz_match_list_columns(frz_matcher* const* ms, const frz_c
         if (cols[c] != cols[start] && st->n_removed && std::find(cs.live.begin(), cs.live.end(), st) == cs.live.end())
             cs.live.push_back(st);
     }
-    frz_matcher* m = ms[0];
-    SubsetScope scope;
-    if (s) FRZ_TRY(subset_scope(m, cols[start], *s, nullptr, &scope));
-    Ranking rank;
-    if (b) rank = ranking_of(*b);
-    Collapse col;
-    if (g) col = collapse_of(*g, per_group);
-    return match_list_host(m, cols[start], 0, sort, k, scope, out, k, n_out, n_total, b ? &rank : nullptr, g ? &col : nullptr,
-                           group_counts, &cs);
+    ListCall call;
+    FRZ_TRY(resolve_call(ms[0], cols[start], h, k, &call));
+    call.sort = sort;
+    call.cols = std::move(cs);
+    call.group_counts = group_counts;
+    return match_list_host(ms[0], cols[start], call, out, k, n_out, n_total);
 }
 
 // ---------------------------------------------------------------------------------- batched top-K: entry points
-namespace {
-// query j's single-query call: frz_match_list_collapsed with groups, else frz_match_list_ranked with a boost, else
-// frz_match_list_subset_top with a subset, else frz_match_list_top
-frz_status batch_single(frz_matcher* m, const frz_corpus* c, const frz_subset* s, const frz_boost* b, const frz_groups* g,
-                        uint64_t per_group, uint64_t k, frz_match* out, uint64_t* n_out, uint64_t* n_total, uint32_t* group_counts) {
-    SubsetScope scope;
-    if (s) FRZ_TRY(subset_scope(m, c, *s, nullptr, &scope));
-    Ranking rank;
-    if (b) rank = ranking_of(*b);
-    if (!g) return match_list_host(m, c, 0, m->config.sort, k, scope, out, k, n_out, n_total, b ? &rank : nullptr);
-    const Collapse col = collapse_of(*g, per_group);
-    return match_list_host(m, c, 0, m->config.sort, k, scope, out, k, n_out, n_total, b ? &rank : nullptr, &col, group_counts);
-}
-}  // namespace
-
 extern "C" frz_status frz_match_list_batch(frz_matcher* const* ms, uint64_t q, const frz_corpus* corpus,
                                            const frz_subset* const* subsets, const frz_boost* const* boosts, uint64_t k,
                                            frz_match* out, uint64_t* n_out, uint64_t* n_total) {
@@ -2523,8 +2495,8 @@ extern "C" frz_status frz_match_list_batch(frz_matcher* const* ms, uint64_t q, c
 }
 
 namespace {
-// The arguments of a batched call, checked (frz_match_list_batch_collapsed, frz_match_list_batch_columns).  bc: a column
-// call, whose query j has the matchers ms[j * n_cols ..] and whose corpus is its column 0.
+// The arguments of a batched call (frz_match_list_batch_collapsed, frz_match_list_batch_columns).  bc: a column call,
+// whose query j has the matchers ms[j * n_cols ..] and whose corpus is its column 0.
 struct BatchCall {
     frz_matcher* const* ms;
     uint64_t q;
@@ -2539,10 +2511,16 @@ struct BatchCall {
     uint64_t* n_out;
     uint64_t* n_total;
     uint32_t* const* group_counts;
+
+    CallHandles handles_of(uint64_t j) const {
+        return CallHandles{subsets ? subsets[j] : nullptr, boosts ? boosts[j] : nullptr, groups ? groups[j] : nullptr,
+                           per_group ? per_group[j] : 1};
+    }
 };
 
-// The driver of the batched calls: the queries of the batched class run in sub-batches (batch_run), every other query, and
-// every query of an overflowed sub-batch, its single-query call.
+// The driver of the batched calls once their matchers and columns have passed: every query's per_group (with or without
+// groups) and handles, then the outputs, are checked; the queries of the batched class run in sub-batches (batch_run),
+// every other query, and every query of an overflowed sub-batch, its single-query call.
 frz_status batch_drive(const BatchCall& a) {
     frz_matcher* const* ms = a.ms;
     const uint64_t q = a.q, k = a.k;
@@ -2551,6 +2529,14 @@ frz_status batch_drive(const BatchCall& a) {
     frz_match* out = a.out;
     uint64_t* n_out = a.n_out;
     uint64_t* n_total = a.n_total;
+    for (uint64_t j = 0; a.per_group && j < q; j++) FRZ_TRY(check_per_group(a.per_group[j], j));
+    for (uint64_t j = 0; j < q; j++)
+        FRZ_TRY(bc ? check_handles(a.handles_of(j), bc->cols, bc->n_cols, kNoColumn, j) : check_handles(a.handles_of(j), &corpus, 1, kAnotherCorpus, j));
+    if (q && !n_out) return frz_fail(FRZ_ERR_INVALID_ARG, "null n_out");
+    if (k && (q > UINT64_MAX / k || q * k > SIZE_MAX / sizeof(frz_match)))
+        return frz_fail(FRZ_ERR_INVALID_ARG, "q * k overflows: q = %llu, k = %llu", (unsigned long long)q, (unsigned long long)k);
+    if (q * k > 0 && !out) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
+    if (q == 0) return FRZ_OK;
     int n_dev = 0;
     if (cudaGetDeviceCount(&n_dev) != cudaSuccess || n_dev == 0) {
         cudaGetLastError();
@@ -2560,19 +2546,15 @@ frz_status batch_drive(const BatchCall& a) {
     const FrzCorpusStorage& cs = corpus->st;
     FRZ_TRY(frz_check_index_range(cs.n, 0));
     for (uint64_t& v : g_batch_last) v = 0;
-    auto subset_of = [&](uint64_t j) { return a.subsets ? a.subsets[j] : nullptr; };
-    auto boost_of = [&](uint64_t j) { return a.boosts ? a.boosts[j] : nullptr; };
-    auto groups_of = [&](uint64_t j) { return a.groups ? a.groups[j] : nullptr; };
-    auto per_group_of = [&](uint64_t j) { return a.per_group ? a.per_group[j] : 1; };
     auto counts_of = [&](uint64_t j) { return a.group_counts ? a.group_counts[j] : nullptr; };
-    auto sort_of = [&](uint64_t j) { return bc ? bc->sort : ms[j]->config.sort; };
     auto single = [&](uint64_t j) {
         frz_match* oj = k ? out + j * k : nullptr;
         uint64_t* tj = n_total ? &n_total[j] : nullptr;
+        const CallHandles h = a.handles_of(j);
         if (bc)
-            return frz_match_list_columns(ms + j * bc->n_cols, bc->cols, bc->n_cols, bc->sort, subset_of(j), boost_of(j), groups_of(j),
-                                          per_group_of(j), k, oj, &n_out[j], tj, counts_of(j));
-        return batch_single(ms[j], corpus, subset_of(j), boost_of(j), groups_of(j), per_group_of(j), k, oj, &n_out[j], tj, counts_of(j));
+            return frz_match_list_columns(ms + j * bc->n_cols, bc->cols, bc->n_cols, bc->sort, h.s, h.b, h.g, h.per_group, k, oj,
+                                          &n_out[j], tj, counts_of(j));
+        return list_call(ms[j], corpus, h, k, oj, k, &n_out[j], tj, counts_of(j));
     };
     auto selected = [&](uint64_t j) {
         return bc ? batch_columns_selected(ms + j * bc->n_cols, *bc) : batchable(ms[j], cs) && batch_selected(ms[j], cs);
@@ -2585,7 +2567,7 @@ frz_status batch_drive(const BatchCall& a) {
     const uint64_t qs_max = std::min<uint64_t>(fit, kFrzBatchMaxSub);
     uint64_t n_groups_max = 0;   // the largest n_groups among the batched grouped queries
     for (uint64_t j = 0; j < q; j++) {
-        const frz_groups* g = groups_of(j);
+        const frz_groups* g = a.handles_of(j).g;
         if (qs_max >= 2 && selected(j) &&
             (!g || (frz_batch_collapse_fit(kBatchScratchBytes, base, g->n_groups, list_rows) &&
                     (!counts_of(j) || g->n_groups <= kBatchMaxCountedGroups)))) {
@@ -2602,38 +2584,34 @@ frz_status batch_drive(const BatchCall& a) {
     // every query's subset and boost, as k_batch_top<ScopedKey> reads them (none when no query has either)
     std::vector<FrzBatchScope> scopes;
     for (uint64_t j : batched) {
-        const frz_subset* s = subset_of(j);
-        const frz_boost* b = boost_of(j);
-        if (!s && !b) continue;
+        const CallHandles h = a.handles_of(j);
+        if (!h.s && !h.b) continue;
         if (scopes.empty()) scopes.resize(q);
         FrzBatchScope& r = scopes[j];
-        if (s) {
+        if (h.s) {
             r.scoped = 1;
-            r.bits = s->bits.get();
-            r.n_bits = s->n_bits;
+            r.bits = h.s->bits.get();
+            r.n_bits = h.s->n_bits;
         }
-        if (b) {
+        if (h.b) {
             r.ranked = 1;
-            r.boost = b->values.get();
-            r.n_boost = (uint32_t)b->values.cap();
+            r.boost = h.b->values.get();
+            r.n_boost = (uint32_t)h.b->values.cap();
         }
     }
     // every query's groups, as the batched collapse reads them (none when no batched query has groups)
     std::vector<FrzBatchCollapse> cols;
     std::vector<uint64_t> n_groups;
     for (uint64_t j : batched) {
-        const frz_groups* g = groups_of(j);
-        if (!g) continue;
+        const CallHandles h = a.handles_of(j);
+        if (!h.g) continue;
         if (cols.empty()) { cols.resize(q, FrzBatchCollapse()); n_groups.resize(q, 0); }
-        const uint8_t sort = sort_of(j);
         FrzBatchCollapse& r = cols[j];
-        r.ids = g->ids.get();
-        r.n_ids = g->ids.cap();
-        r.per_group = per_group_of(j) == UINT64_MAX ? 0xFFFFFFFFu : (uint32_t)per_group_of(j);
-        r.order = boost_of(j) ? FRZ_COLLAPSE_BY_KEY
-                : sort == FRZ_SORT_SCORE_THEN_INDEX_ASC || sort == FRZ_SORT_SCORE_THEN_INDEX_DESC ? FRZ_COLLAPSE_BY_SCORE
-                : FRZ_COLLAPSE_BY_INDEX;
-        n_groups[j] = g->n_groups;
+        r.ids = h.g->values.get();
+        r.n_ids = h.g->values.cap();
+        r.per_group = h.per_group == UINT64_MAX ? 0xFFFFFFFFu : (uint32_t)h.per_group;
+        r.order = collapse_order(h.b != nullptr, sort_by_score(bc ? bc->sort : ms[j]->config.sort));
+        n_groups[j] = h.g->n_groups;
     }
     BatchGroups gr;
     if (!cols.empty()) {
@@ -2674,25 +2652,6 @@ extern "C" frz_status frz_match_list_batch_collapsed(frz_matcher* const* ms, uin
     if (!ms || !corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
     for (uint64_t j = 0; j < q; j++)
         if (!ms[j]) return frz_fail(FRZ_ERR_INVALID_ARG, "null matcher at %llu", (unsigned long long)j);
-    for (uint64_t j = 0; per_group && j < q; j++) {
-        if (per_group[j] == 0) return frz_fail(FRZ_ERR_INVALID_ARG, "per_group = 0 at %llu", (unsigned long long)j);
-        if (per_group[j] > kFrzCollapseMaxPerGroup && per_group[j] != UINT64_MAX)
-            return frz_fail(FRZ_ERR_UNSUPPORTED, "per_group = %llu at %llu: at most %llu rows per group, or UINT64_MAX for no cap",
-                            (unsigned long long)per_group[j], (unsigned long long)j, (unsigned long long)kFrzCollapseMaxPerGroup);
-    }
-    for (uint64_t j = 0; j < q; j++) {
-        if (subsets && subsets[j] && subsets[j]->corpus != corpus)
-            return frz_fail(FRZ_ERR_INVALID_ARG, "the subset of query %llu was made on another corpus", (unsigned long long)j);
-        if (boosts && boosts[j] && boosts[j]->corpus != corpus)
-            return frz_fail(FRZ_ERR_INVALID_ARG, "the boost of query %llu was made on another corpus", (unsigned long long)j);
-        if (groups && groups[j] && groups[j]->corpus != corpus)
-            return frz_fail(FRZ_ERR_INVALID_ARG, "the groups of query %llu were made on another corpus", (unsigned long long)j);
-    }
-    if (q && !n_out) return frz_fail(FRZ_ERR_INVALID_ARG, "null n_out");
-    if (k && (q > UINT64_MAX / k || q * k > SIZE_MAX / sizeof(frz_match)))
-        return frz_fail(FRZ_ERR_INVALID_ARG, "q * k overflows: q = %llu, k = %llu", (unsigned long long)q, (unsigned long long)k);
-    if (q * k > 0 && !out) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
-    if (q == 0) return FRZ_OK;
     return batch_drive(BatchCall{ms, q, corpus, nullptr, subsets, boosts, groups, per_group, k, out, n_out, n_total, group_counts});
 }
 
@@ -2702,48 +2661,7 @@ extern "C" frz_status frz_match_list_batch_columns(frz_matcher* const* ms, uint6
                                                    uint8_t sort, const frz_subset* const* subsets, const frz_boost* const* boosts,
                                                    const frz_groups* const* groups, const uint64_t* per_group, uint64_t k,
                                                    frz_match* out, uint64_t* n_out, uint64_t* n_total, uint32_t* const* group_counts) {
-    if (n_cols == 0) return frz_fail(FRZ_ERR_INVALID_ARG, "n_cols = 0: a columns call needs at least one column");
-    if (!ms || !cols) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
-    for (uint64_t c = 0; c < n_cols; c++)
-        if (!cols[c]) return frz_fail(FRZ_ERR_INVALID_ARG, "null corpus of column %llu", (unsigned long long)c);
-    if (q > UINT64_MAX / n_cols || q * n_cols > SIZE_MAX / sizeof(frz_matcher*))
-        return frz_fail(FRZ_ERR_INVALID_ARG, "q * n_cols overflows: q = %llu, n_cols = %llu", (unsigned long long)q, (unsigned long long)n_cols);
-    for (uint64_t i = 0; i < q * n_cols; i++)
-        if (!ms[i])
-            return frz_fail(FRZ_ERR_INVALID_ARG, "null matcher of query %llu, column %llu", (unsigned long long)(i / n_cols),
-                            (unsigned long long)(i % n_cols));
-    const FrzCorpusStorage& first = cols[0]->st;
-    for (uint64_t c = 1; c < n_cols; c++) {
-        if (cols[c]->st.device != first.device)
-            return frz_fail(FRZ_ERR_INVALID_ARG, "column %llu is on device %d, column 0 on device %d", (unsigned long long)c,
-                            cols[c]->st.device, first.device);
-        if (cols[c]->st.n != first.n)
-            return frz_fail(FRZ_ERR_INVALID_ARG, "column %llu holds %llu rows, column 0 holds %llu: the columns must share one index space",
-                            (unsigned long long)c, (unsigned long long)cols[c]->st.n, (unsigned long long)first.n);
-    }
-    FRZ_TRY(frz_check_index_range(first.n, 0));
-    if (sort > FRZ_SORT_INDEX_DESC) return frz_fail(FRZ_ERR_INVALID_ARG, "sort = %u is not a sort strategy", (unsigned)sort);
-    for (uint64_t j = 0; per_group && j < q; j++) {
-        if (per_group[j] == 0) return frz_fail(FRZ_ERR_INVALID_ARG, "per_group = 0 at %llu", (unsigned long long)j);
-        if (per_group[j] > kFrzCollapseMaxPerGroup && per_group[j] != UINT64_MAX)
-            return frz_fail(FRZ_ERR_UNSUPPORTED, "per_group = %llu at %llu: at most %llu rows per group, or UINT64_MAX for no cap",
-                            (unsigned long long)per_group[j], (unsigned long long)j, (unsigned long long)kFrzCollapseMaxPerGroup);
-    }
-    // membership, boosts and group ids are by index, so a handle of any column serves every column
-    const auto of_a_column = [&](const frz_corpus* h) { return std::find(cols, cols + n_cols, h) != cols + n_cols; };
-    for (uint64_t j = 0; j < q; j++) {
-        if (subsets && subsets[j] && !of_a_column(subsets[j]->corpus))
-            return frz_fail(FRZ_ERR_INVALID_ARG, "the subset of query %llu was made on none of the columns", (unsigned long long)j);
-        if (boosts && boosts[j] && !of_a_column(boosts[j]->corpus))
-            return frz_fail(FRZ_ERR_INVALID_ARG, "the boost of query %llu was made on none of the columns", (unsigned long long)j);
-        if (groups && groups[j] && !of_a_column(groups[j]->corpus))
-            return frz_fail(FRZ_ERR_INVALID_ARG, "the groups of query %llu were made on none of the columns", (unsigned long long)j);
-    }
-    if (q && !n_out) return frz_fail(FRZ_ERR_INVALID_ARG, "null n_out");
-    if (k && (q > UINT64_MAX / k || q * k > SIZE_MAX / sizeof(frz_match)))
-        return frz_fail(FRZ_ERR_INVALID_ARG, "q * k overflows: q = %llu, k = %llu", (unsigned long long)q, (unsigned long long)k);
-    if (q * k > 0 && !out) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
-    if (q == 0) return FRZ_OK;
+    FRZ_TRY(check_columns(ms, cols, n_cols, sort, &q));
     const BatchColumns bc{cols, n_cols, sort};
     return batch_drive(BatchCall{ms, q, cols[0], &bc, subsets, boosts, groups, per_group, k, out, n_out, n_total, group_counts});
 }
@@ -2757,7 +2675,9 @@ extern "C" frz_status frz_match_list_into(frz_matcher* m, const frz_corpus* corp
                                           uint64_t cap, uint64_t* n_out) {
     if (!m || !corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
     FRZ_TRY(frz_ensure_device(corpus->st.device));
-    return match_list_host(m, corpus, index_offset, FRZ_SORT_INDEX_ASC, UINT64_MAX, SubsetScope(), out, cap, n_out, nullptr);
+    ListCall call;
+    call.index_offset = index_offset;
+    return match_list_host(m, corpus, call, out, cap, n_out, nullptr);
 }
 
 namespace {   // defined with the shard calls below
@@ -2940,9 +2860,13 @@ frz_status frz_match_shard_device_top(frz_matcher* m, const frz_corpus* shard, u
     if (cap < shard->st.n) return frz_fail(FRZ_ERR_CAPACITY, "d_out must hold the whole shard (%llu)", (unsigned long long)shard->st.n);
     // (the count of a multi-pattern or empty matcher exists only at the end)
     return shard_call(m, d_count, stream, [&](FrzLaunchStats* st) {
+        ListCall call;
+        call.sort = m->config.sort;
+        call.limit = limit;
+        call.index_offset = index_offset;
+        call.final_out = reinterpret_cast<FrzMatchDev*>(d_out);
         FrzMatchDev* d_list = nullptr;
-        return match_list_device(m, shard->st, index_offset, m->config.sort, &d_list, stream, st, reinterpret_cast<FrzMatchDev*>(d_out),
-                                 limit);
+        return match_list_device(m, shard->st, call, &d_list, stream, st);
     });
 }
 
