@@ -119,6 +119,7 @@ def lib():
     L.frz_boost_destroy.restype = None
     L.frz_match_list_ranked.argtypes = [vp, vp, vp, vp, u64, vp, C.POINTER(u64), C.POINTER(u64)]
     L.frz_match_list_ordered.argtypes = [vp, vp, vp, vp, vp, u32, u64, vp, C.POINTER(u64), C.POINTER(u64)]
+    L.frz_match_list_ordered_collapsed.argtypes = [vp, vp, vp, vp, vp, u32, vp, u64, u64, vp, C.POINTER(u64), C.POINTER(u64), vp]
     L.frz_groups_create.argtypes = [vp, vp, u64, u64, C.POINTER(vp)]
     L.frz_groups_set.argtypes = [vp, vp, vp, u64]
     L.frz_groups_count.restype = u64
@@ -127,6 +128,8 @@ def lib():
     L.frz_groups_destroy.restype = None
     L.frz_match_list_collapsed.argtypes = [vp, vp, vp, vp, vp, u64, u64, vp, C.POINTER(u64), C.POINTER(u64), vp]
     L.frz_match_list_columns.argtypes = [vp, vp, u64, C.c_uint8, vp, vp, vp, u64, u64, vp, C.POINTER(u64), C.POINTER(u64), vp]
+    L.frz_match_list_columns_ordered.argtypes = [vp, vp, u64, C.c_uint8, vp, vp, vp, u32, vp, u64, u64, vp, C.POINTER(u64),
+                                                 C.POINTER(u64), vp]
     L.frz_match_list_batch_columns.argtypes = [vp, u64, vp, u64, C.c_uint8, vp, vp, vp, vp, u64, vp, vp, vp, vp]
     L.frz_match_list_into.argtypes = [vp, vp, u32, vp, u64, C.POINTER(u64)]
     L.frz_match_list_host.argtypes = [vp, vp, vp, u64, C.c_int, vp, u64, C.POINTER(u64)]
@@ -586,17 +589,33 @@ class Matcher:
 
     def match_list_ordered_array(self, corpus: Corpus, attr: Attr, order: Order = Order.AttrDesc, k: Optional[int] = None,
                                  subset: Optional[Subset] = None, boost: Optional[Boost] = None,
-                                 out: Optional[np.ndarray] = None) -> Tuple[np.ndarray, int]:
+                                 out: Optional[np.ndarray] = None, groups: Optional[Groups] = None,
+                                 per_group: Optional[int] = 1, counts: bool = False):
         """The rows of match_list_array(corpus) (or of its subset) ordered by attr (frz_match_list_ordered): by value
         (Order.AttrDesc / AttrAsc) or by score, clamp(score + boost[index], 0, 65535) with a boost, then by value
         (ScoreThenAttrDesc / Asc); rows without a value go last, and remaining ties keep the strategy's index order.
         Truncated to the first k: (array of min(k, total) rows, total).  k=None orders the whole list.  `out` (optional)
-        needs room for min(k, len(corpus), len(subset)) rows."""
+        needs room for min(k, len(corpus), len(subset)) rows.
+        With groups, the ordered list is collapsed first (frz_match_list_ordered_collapsed): in its order, the rows in no
+        group and the first per_group rows of each group are kept (per_group 1..32, or None for no cap), so per_group=1
+        gives each group's first row by the attribute, e.g. its newest.  Returns (rows, total), total counting the kept
+        rows, or (rows, total, counts) with counts=True: the ordered list's rows per group, before collapsing."""
         k, out = _top_out(out, k, corpus.n, subset, "this ordered call")
         n, total = C.c_uint64(), C.c_uint64()
-        _check(lib().frz_match_list_ordered(self._h, corpus._h, subset._h if subset is not None else None,
-                                            boost._h if boost is not None else None, attr._h, int(order), k, out.ctypes.data,
-                                            C.byref(n), C.byref(total)))
+        sh, bh = subset._h if subset is not None else None, boost._h if boost is not None else None
+        if groups is None:
+            if counts:
+                raise ValueError("counts=True needs groups")
+            _check(lib().frz_match_list_ordered(self._h, corpus._h, sh, bh, attr._h, int(order), k, out.ctypes.data, C.byref(n),
+                                                C.byref(total)))
+            return out[: n.value], total.value
+        per_group = _U64_MAX if per_group is None else int(per_group)
+        cnt = np.zeros(len(groups), dtype=np.uint32) if counts else None
+        _check(lib().frz_match_list_ordered_collapsed(self._h, corpus._h, sh, bh, attr._h, int(order), groups._h, per_group, k,
+                                                      out.ctypes.data, C.byref(n), C.byref(total),
+                                                      cnt.ctypes.data if counts else None))
+        if counts:
+            return out[: n.value], total.value, cnt
         return out[: n.value], total.value
 
     def match_list_collapsed_array(self, corpus: Corpus, groups: Groups, k: Optional[int] = None,
@@ -763,15 +782,18 @@ def match_list_batch_collapsed(matchers, corpus: Corpus, k: int, groups, per_gro
 
 def match_list_columns(matchers, columns, k: Optional[int] = None, sort: SortStrategy = SortStrategy.ScoreThenIndexAsc,
                        subset: Optional[Subset] = None, boost: Optional[Boost] = None, groups: Optional[Groups] = None,
-                       per_group: Optional[int] = 1, counts: bool = False, out: Optional[np.ndarray] = None):
+                       per_group: Optional[int] = 1, counts: bool = False, out: Optional[np.ndarray] = None,
+                       attr: Optional[Attr] = None, order: Order = Order.AttrDesc):
     """frz_match_list_columns: rows with several text fields, matcher j searching columns[j] (Corpus objects of one length:
     row i is haystack i of every column).  A row matches when it matches in every column; its score is the saturating sum
     of the column scores and its exact flag their OR.  The list is ordered by `sort` (the matchers' own sort settings are
     not read), ranked by boost when one is given, collapsed by groups when they are given (per_group 1..32, or None for no
-    cap), and truncated to the first k rows.  subset / boost / groups may be handles of any of the columns.  Returns
-    (rows, total), or (rows, total, counts) with counts=True (the list's rows per group, before collapsing).  k=None returns
-    every row; `out` (optional) needs room for min(k, len(columns[0]), len(subset)) rows.  Put the most selective column
-    first: the order changes only the speed."""
+    cap), and truncated to the first k rows.  With attr, the list is instead ordered by the attribute as
+    Matcher.match_list_ordered_array orders its list (`order`; the boost, when given, goes into the score), then collapsed
+    in that order when groups are given (frz_match_list_columns_ordered).  subset / boost / groups / attr may be handles of
+    any of the columns.  Returns (rows, total), or (rows, total, counts) with counts=True (the list's rows per group, before
+    collapsing).  k=None returns every row; `out` (optional) needs room for min(k, len(columns[0]), len(subset)) rows.  Put
+    the most selective column first: the order changes only the speed."""
     matchers, columns = list(matchers), list(columns)
     if len(matchers) != len(columns):
         raise ValueError(f"{len(matchers)} matchers for {len(columns)} columns")
@@ -783,10 +805,13 @@ def match_list_columns(matchers, columns, k: Optional[int] = None, sort: SortStr
     q = len(matchers)
     cs = (C.c_void_p * max(q, 1))(*[c._h.value for c in columns])
     n_out, total = C.c_uint64(), C.c_uint64()
-    _check(lib().frz_match_list_columns(_matcher_array(matchers), cs, q, int(sort), subset._h if subset is not None else None,
-                                        boost._h if boost is not None else None, groups._h if groups is not None else None,
-                                        per_group, k, out.ctypes.data, C.byref(n_out), C.byref(total),
-                                        cnt.ctypes.data if counts else None))
+    sh, bh, gh = (h._h if h is not None else None for h in (subset, boost, groups))
+    tail = (per_group, k, out.ctypes.data, C.byref(n_out), C.byref(total), cnt.ctypes.data if counts else None)
+    if attr is None:
+        _check(lib().frz_match_list_columns(_matcher_array(matchers), cs, q, int(sort), sh, bh, gh, *tail))
+    else:
+        _check(lib().frz_match_list_columns_ordered(_matcher_array(matchers), cs, q, int(sort), sh, bh, attr._h, int(order), gh,
+                                                    *tail))
     if counts:
         return out[: n_out.value], total.value, cnt
     return out[: n_out.value], total.value

@@ -1,5 +1,6 @@
-// collapse.cu — the per-group count and the rounds of the collapsed call (frz_match_list_collapsed, DESIGN.md §4.12), and
-// of the batched collapsed call's sub-batches (frz_match_list_batch_collapsed, §4.11).  The row rule is collapse_plan.cuh's;
+// collapse.cu — the per-group count and the rounds of the collapsed call (frz_match_list_collapsed, DESIGN.md §4.12), of
+// the ordered collapsed calls (frz_match_list_ordered_collapsed, frz_match_list_columns_ordered, §4.15.1), and of the
+// batched collapsed call's sub-batches (frz_match_list_batch_collapsed, §4.11).  The row rule is collapse_plan.cuh's;
 // host.cu compacts the kept rows and sorts them, or k_batch_top<CollapsedKey> (batch.cu) cuts them per query.
 #include "batch_collapse_plan.cuh"
 #include "collapse_plan.cuh"
@@ -78,6 +79,86 @@ __global__ void __launch_bounds__(kCollapseBlock) k_collapse_take(FrzCollapseDev
         if (frz_collapse_entry(row_key(c, r)) == __ldcg(&c.best[g])) {
             c.taken[i] = 1;
             c.best[g] = 0;
+        }
+    }
+}
+
+// The rounds on the order key (frz_match_list_ordered_collapsed, the ordered column call): the three steps of
+// collapse_plan.cuh's two-step max, one kernel each.  keys[i] is list row i's FrzOrderKey (k_order_keys, in list order), read
+// as one 16-byte load; c.best is the best_hi table.  The max kernels keep k_collapse_max's warp-uniform register reduction
+// and its skip of an atomic that cannot raise the entry.
+__device__ __forceinline__ FrzOrderKey load_key(const FrzOrderKey* __restrict__ keys, uint64_t i) {
+    const ulonglong2 v = __ldg(reinterpret_cast<const ulonglong2*>(keys) + i);
+    return FrzOrderKey{v.x, v.y};
+}
+
+__device__ __forceinline__ void warp_max_into(unsigned long long* table, uint32_t g, unsigned long long e, uint32_t lane) {
+    const uint32_t peers = __match_any_sync(kFullWarp, g);
+    if (g != kFrzGroupNone && peers == kFullWarp) {   // warp-uniform: every lane contends for g
+#pragma unroll
+        for (int d = 16; d >= 1; d >>= 1) e = max(e, __shfl_xor_sync(kFullWarp, e, d));
+        if (lane == 0 && e > __ldcg(&table[g])) atomicMax(&table[g], e);
+    } else if (g != kFrzGroupNone && e > __ldcg(&table[g])) {
+        atomicMax(&table[g], e);
+    }
+}
+
+// Step 1: best_hi[group] = the largest hi among the group's contenders.
+__global__ void __launch_bounds__(kCollapseBlock) k_collapse_max_hi(FrzCollapseDev c, const FrzMatchDev* __restrict__ list,
+                                                                   const FrzOrderKey* __restrict__ keys,
+                                                                   const unsigned long long* __restrict__ n_ptr) {
+    const unsigned long long n = *n_ptr;
+    const uint32_t lane = threadIdx.x & 31;
+    const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+    for (uint64_t i0 = (uint64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31u); i0 < n; i0 += stride) {
+        const uint64_t i = i0 + lane;
+        uint32_t g = kFrzGroupNone;
+        unsigned long long e = 0;
+        if (i < n) {
+            const uint32_t rg = frz_collapse_group(c.ids, c.n_ids, list[i].index);
+            if (rg != kFrzGroupNone && frz_collapse_contends(rg, c.counts[rg], c.per_group, c.taken[i] != 0)) {
+                g = rg;
+                e = frz_collapse_hi_entry(load_key(keys, i));
+            }
+        }
+        warp_max_into(c.best, g, e, lane);
+    }
+}
+
+// Step 2: best_lo[group] = the largest lo + 1 among the contenders whose hi is best_hi[group].
+__global__ void __launch_bounds__(kCollapseBlock) k_collapse_max_lo(FrzCollapseDev c, const FrzMatchDev* __restrict__ list,
+                                                                   const FrzOrderKey* __restrict__ keys, unsigned long long* best_lo,
+                                                                   const unsigned long long* __restrict__ n_ptr) {
+    const unsigned long long n = *n_ptr;
+    const uint32_t lane = threadIdx.x & 31;
+    const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+    for (uint64_t i0 = (uint64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31u); i0 < n; i0 += stride) {
+        const uint64_t i = i0 + lane;
+        uint32_t g = kFrzGroupNone;
+        unsigned long long e = 0;
+        if (i < n) {
+            const uint32_t rg = frz_collapse_group(c.ids, c.n_ids, list[i].index);
+            if (rg != kFrzGroupNone && frz_collapse_contends(rg, c.counts[rg], c.per_group, c.taken[i] != 0)) {
+                g = rg;
+                e = frz_collapse_lo_entry(load_key(keys, i), __ldcg(&c.best[rg]));
+            }
+        }
+        warp_max_into(best_lo, g, e, lane);
+    }
+}
+
+// Step 3: the contender whose lo + 1 is best_lo[group] is taken, and resets both entries for the next round.
+__global__ void __launch_bounds__(kCollapseBlock) k_collapse_take_key(FrzCollapseDev c, const FrzMatchDev* __restrict__ list,
+                                                                     const FrzOrderKey* __restrict__ keys, unsigned long long* best_lo,
+                                                                     const unsigned long long* __restrict__ n_ptr) {
+    const unsigned long long n = *n_ptr;
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+        const uint32_t g = frz_collapse_group(c.ids, c.n_ids, list[i].index);
+        if (g == kFrzGroupNone || !frz_collapse_contends(g, c.counts[g], c.per_group, c.taken[i] != 0)) continue;
+        if (frz_collapse_key_takes(load_key(keys, i), __ldcg(&best_lo[g]))) {
+            c.taken[i] = 1;
+            c.best[g] = 0;
+            best_lo[g] = 0;
         }
     }
 }
@@ -205,6 +286,22 @@ frz_status frz_launch_collapse(const FrzCollapseDev& c, const FrzMatchDev* list,
         k_collapse_take<<<grid, kCollapseBlock, 0, stream>>>(c, list, n_ptr);
     }
     st->launches += 1 + 2 * (uint64_t)rounds;
+    FRZ_CUDA_TRY(cudaGetLastError());
+    return FRZ_OK;
+}
+
+frz_status frz_launch_collapse_by_key(const FrzCollapseDev& c, unsigned long long* best_lo, const FrzOrderKey* keys,
+                                      const FrzMatchDev* list, const unsigned long long* n_ptr, uint64_t n_cap, uint64_t n_groups,
+                                      uint32_t rounds, cudaStream_t stream, FrzLaunchStats* st) {
+    FRZ_CUDA_TRY(cudaMemsetAsync(c.counts, 0, n_groups * sizeof(uint32_t), stream));
+    const int grid = grid_for(n_cap, kCollapseBlock);
+    k_collapse_count<<<grid, kCollapseBlock, 0, stream>>>(c, list, n_ptr);
+    for (uint32_t r = 0; r < rounds; r++) {
+        k_collapse_max_hi<<<grid, kCollapseBlock, 0, stream>>>(c, list, keys, n_ptr);
+        k_collapse_max_lo<<<grid, kCollapseBlock, 0, stream>>>(c, list, keys, best_lo, n_ptr);
+        k_collapse_take_key<<<grid, kCollapseBlock, 0, stream>>>(c, list, keys, best_lo, n_ptr);
+    }
+    st->launches += 1 + 3 * (uint64_t)rounds;
     FRZ_CUDA_TRY(cudaGetLastError());
     return FRZ_OK;
 }

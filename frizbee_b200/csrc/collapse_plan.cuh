@@ -15,6 +15,7 @@
 #include <stdint.h>
 
 #include "batch_plan.cuh"
+#include "order_plan.cuh"
 
 #if defined(__CUDACC__)
 #define FRZ_CP_HD __host__ __device__ __forceinline__
@@ -58,3 +59,23 @@ FRZ_CP_HD uint64_t frz_collapse_entry(uint64_t key) { return key + 1; }
 FRZ_CP_HD bool frz_collapse_keep(uint32_t group, uint32_t count, uint32_t per_group, bool taken) {
     return group == kFrzGroupNone || count <= per_group || taken;
 }
+
+// Rounds on the order key (frz_match_list_ordered_collapsed and the ordered column call, DESIGN.md §4.15.1).  There L is the
+// ordered call's list, so a row's key is its 112-bit FrzOrderKey (order_plan.cuh): unique, and the first row of a group in L
+// is the one with the largest key.  The count pass and the keep rule above are unchanged; only a round differs.  The key
+// does not fit one 64-bit atomic, and every value of hi is legitimate (INT64_MAX under ATTR_DESC is hi = 2^64 - 1), so
+// hi + 1 could overflow.  A round takes the max in two steps over two tables, best_hi and best_lo, zero between rounds:
+//   1. best_hi[group] = the largest hi among the group's contenders (frz_collapse_hi_entry);
+//   2. best_lo[group] = the largest lo + 1 among the contenders whose hi equals best_hi (frz_collapse_lo_entry; the
+//      others offer 0, which never raises the entry);
+//   3. the contender whose lo + 1 equals best_lo is taken (frz_collapse_key_takes) and resets both entries to 0.
+// Why this is safe:
+//   - lo holds the index part x, so lo is unique within the list: the take test needs only best_lo.
+//   - A contender that reads a reset best_lo cannot mistake itself for the winner: lo + 1 >= 1.
+//   - A reset best_hi of 0 is right for the next round.  In round r < per_group an over-full group still has count - r >
+//     per_group - r >= 1 contenders, so each max is over a non-empty set; a group whose contenders all have hi = 0 (null
+//     attribute values under ATTR_*) keeps best_hi = 0, which step 2 matches.
+//   - Every over-full group has one winner per round, which resets its entries, so both tables are zero after the rounds.
+FRZ_CP_HD uint64_t frz_collapse_hi_entry(const FrzOrderKey& k) { return k.hi; }
+FRZ_CP_HD uint64_t frz_collapse_lo_entry(const FrzOrderKey& k, uint64_t best_hi) { return k.hi == best_hi ? k.lo + 1 : 0; }
+FRZ_CP_HD bool frz_collapse_key_takes(const FrzOrderKey& k, uint64_t best_lo) { return k.lo + 1 == best_lo; }

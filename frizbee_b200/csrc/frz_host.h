@@ -274,6 +274,7 @@ struct FrzWorkspace {
     FrzDevArray<FrzMatchDev> subset_list;   // [2 * members] list-form subset call: member records, then the live ones compacted
     FrzDevArray<uint32_t> collapse_counts;  // [n_groups] collapsed call: the list's rows per group
     FrzDevArray<unsigned long long> collapse_best;  // [n_groups] its round table, all zero between calls
+    FrzDevArray<unsigned long long> collapse_best_lo;  // [n_groups] the second table of rounds on the order key, zero too
     FrzDevArray<uint8_t> collapse_taken;    // [corpus length] its rows taken in a round
     FrzDevArray<FrzOrderKey> order_keys;    // [list rows] ordered call: the order key of each list row
     FrzDevArray<uint32_t> order_cand;       // [2 * list rows] its select's candidate positions (two pass parities)
@@ -448,6 +449,12 @@ struct FrzCollapseDev {
 // rounds (a max pass and a take pass each).  c.best must be zero on entry; it is zero again when the rounds have run.
 frz_status frz_launch_collapse(const FrzCollapseDev& c, const FrzMatchDev* list, const unsigned long long* n_ptr, uint64_t n_cap,
                                uint64_t n_groups, uint32_t rounds, cudaStream_t stream, FrzLaunchStats* st);
+// collapse.cu: frz_launch_collapse with rounds on the order key (collapse_plan.cuh's two-step max): keys[i] is list row i's
+// FrzOrderKey, c.best is the best_hi table and best_lo the second one ([n_groups] each, zero on entry and again after the
+// rounds); c.boost and c.order are not read.  Each round is three passes.
+frz_status frz_launch_collapse_by_key(const FrzCollapseDev& c, unsigned long long* best_lo, const FrzOrderKey* keys,
+                                      const FrzMatchDev* list, const unsigned long long* n_ptr, uint64_t n_cap, uint64_t n_groups,
+                                      uint32_t rounds, cudaStream_t stream, FrzLaunchStats* st);
 
 // The fill of frz_subset_where (host.cu; the rule and FrzWhereDev are where_plan.cuh's).
 struct FrzWhereDev;

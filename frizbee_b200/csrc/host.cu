@@ -1423,10 +1423,14 @@ struct Collapse {
 
 // The collapsed call's steps between the list and its sort (DESIGN.md §4.12): the count pass, per_group rounds, and the
 // stable compaction of the kept rows into the other list buffer (*d_list then points there, and ws.counters->total holds
-// |C|).  order: what the rows' order keys rank by.  The list's length is read back first (a survivor-list overflow
-// returns kRetryOverflow there): the passes and the compaction then cover the list, not the corpus.
+// |C|).  order: what the rows' order keys rank by.  ord (an ordered call's attribute, boost and order; `reversed` is set
+// here): L is the ordered list, so the rounds rank by its 112-bit order key instead and `order` is not read.  The keys
+// are computed into ws.order_keys in list order first (k_order_keys), and each round is collapse_plan.cuh's two-step max
+// over them (DESIGN.md §4.15.1).  The list's length is read back first (a survivor-list overflow returns kRetryOverflow
+// there): the passes and the compaction then cover the list, not the corpus.
 frz_status collapse_list(frz_matcher* m, const FrzCorpusStorage& cs, const Collapse& col, uint8_t order, bool reversed,
-                         const std::optional<Ranking>& rank, FrzMatchDev** d_list, cudaStream_t stream, FrzLaunchStats* st) {
+                         const std::optional<Ranking>& rank, const FrzOrderDev* ord, FrzMatchDev** d_list, cudaStream_t stream,
+                         FrzLaunchStats* st) {
     FrzWorkspace& ws = m->ws;
     FRZ_TRY(read_counters(m, stream));
     const uint64_t n_list = ws.h_counters.get()->total;
@@ -1450,7 +1454,21 @@ frz_status collapse_list(frz_matcher* m, const FrzCorpusStorage& cs, const Colla
     c.order = order;
     c.reversed = reversed;
     const unsigned long long* n_ptr = &ws.counters.get()->total;
-    FRZ_TRY(frz_launch_collapse(c, *d_list, n_ptr, std::max<uint64_t>(n_list, 1), col.n_groups, capped ? c.per_group : 0, stream, st));
+    if (ord && capped && n_list > 0) {
+        if (ws.collapse_best_lo.cap() < col.n_groups) {   // as collapse_best
+            FRZ_TRY(ws.collapse_best_lo.reserve(col.n_groups));
+            FRZ_CUDA_TRY(cudaMemsetAsync(ws.collapse_best_lo.get(), 0, col.n_groups * sizeof(unsigned long long), stream));
+        }
+        FRZ_TRY(ws.order_keys.reserve(n_list));
+        FRZ_TRY(ws.order_state.reserve(1));
+        FrzOrderDev o = *ord;
+        o.reversed = reversed;
+        FRZ_TRY(frz_launch_order_keys(*d_list, n_ptr, n_list, o, ws.order_keys.get(), ws.order_state.get(), stream, st));
+        FRZ_TRY(frz_launch_collapse_by_key(c, ws.collapse_best_lo.get(), ws.order_keys.get(), *d_list, n_ptr, n_list, col.n_groups,
+                                           c.per_group, stream, st));
+    } else {
+        FRZ_TRY(frz_launch_collapse(c, *d_list, n_ptr, std::max<uint64_t>(n_list, 1), col.n_groups, capped ? c.per_group : 0, stream, st));
+    }
     if (!capped || n_list == 0) return FRZ_OK;
     FrzMatchDev* kept = *d_list == ws.matches_a.get() ? ws.matches_b.get() : ws.matches_a.get();
     FRZ_TRY(retain_rows(m, CollapseKeep{c, *d_list}, *d_list, n_list, kept, stream, st));
@@ -1535,7 +1553,8 @@ uint8_t collapse_order(bool ranked, bool by_score) {
 // first `limit` rows (top-K calls: only those positions of the final list are written, the sort's last scatter and the
 // final copy drop the rest; the count in ws.counters->total stays the full match count).  scope: as in match_into_device.
 // rank: sort by the ranking's key instead, under every strategy and for the empty matcher too (the strategy's direction
-// only orders ties).  col: collapse the list before its sort (collapse_list); group_counts (host, col->n_groups entries)
+// only orders ties).  col: collapse the list before its sort (collapse_list; with ord, by the order key, so each group
+// keeps its first rows in the ordered list); group_counts (host, col->n_groups entries)
 // receives the list's rows per group.  cols: the list is that of a frz_match_list_columns call, whose starting column is
 // the call's corpus (match_patterns).  ord: order the list by the attribute instead (order_list), under every strategy and
 // for the empty matcher too.  col, cols and ord are for host calls only; the shard calls set index_offset and final_out
@@ -1580,7 +1599,9 @@ frz_status match_list_device(frz_matcher* m, const FrzCorpusStorage& cs, const L
                                           call.scope));
     else FRZ_TRY(match_into_device(m, cs, call.index_offset, reversed, &d_list, &bound, stream, st, call.scoring_out(*m),
                                    call.fused_hist(*m) ? &hist : nullptr, call.scope));
-    if (call.col) FRZ_TRY(collapse_list(m, cs, *call.col, collapse_order(rank.has_value(), will_sort), reversed, rank, &d_list, stream, st));
+    if (call.col)
+        FRZ_TRY(collapse_list(m, cs, *call.col, collapse_order(rank.has_value(), will_sort), reversed, rank, call.ord ? &call.ord->dev : nullptr,
+                              &d_list, stream, st));
     if (call.ord) {
         FRZ_TRY(order_list(m, cs, *call.ord, reversed, limit, &d_list, stream, st));
     } else if (will_sort) {
@@ -2392,15 +2413,37 @@ static_assert(FRZ_ORDER_SCORE_THEN_ATTR_DESC == kFrzOrderScoreFirst && FRZ_ORDER
                   (FRZ_ORDER_ATTR_ASC & 1) && (FRZ_ORDER_SCORE_THEN_ATTR_ASC & 1) && !(FRZ_ORDER_ATTR_DESC & 1),
               "order_plan.cuh mirrors frz_cuda.h");
 
+namespace {
+frz_status check_order(uint32_t order) {
+    if (order >= kFrzOrderCount) return frz_fail(FRZ_ERR_INVALID_ARG, "order %u (at most %u)", order, kFrzOrderCount - 1);
+    return FRZ_OK;
+}
+}  // namespace
+
 extern "C" frz_status frz_match_list_ordered(frz_matcher* m, const frz_corpus* corpus, const frz_subset* s, const frz_boost* b,
                                              const frz_attr* a, uint32_t order, uint64_t k, frz_match* out, uint64_t* n_out,
                                              uint64_t* n_total) {
     if (!m || !corpus || !a) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
     if (!out && k > 0) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
-    if (order >= kFrzOrderCount) return frz_fail(FRZ_ERR_INVALID_ARG, "order %u (at most %u)", order, kFrzOrderCount - 1);
+    FRZ_TRY(check_order(order));
     const CallHandles h{s, b, nullptr, 1, a, order};
     FRZ_TRY(check_handles(h, &corpus, 1, kAnotherCorpus));
     return list_call(m, corpus, h, k, out, k, n_out, n_total);
+}
+
+// The ordered list collapsed by group (DESIGN.md §4.15.1): resolve_call gives the ListCall both an Ordering and a Collapse,
+// and collapse_list then ranks the rounds by the order key.
+extern "C" frz_status frz_match_list_ordered_collapsed(frz_matcher* m, const frz_corpus* corpus, const frz_subset* s, const frz_boost* b,
+                                                       const frz_attr* a, uint32_t order, const frz_groups* g, uint64_t per_group,
+                                                       uint64_t k, frz_match* out, uint64_t* n_out, uint64_t* n_total,
+                                                       uint32_t* group_counts) {
+    if (!m || !corpus || !a || !g) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    FRZ_TRY(check_per_group(per_group));
+    if (!out && k > 0) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
+    FRZ_TRY(check_order(order));
+    const CallHandles h{s, b, g, per_group, a, order};
+    FRZ_TRY(check_handles(h, &corpus, 1, kAnotherCorpus));
+    return list_call(m, corpus, h, k, out, k, n_out, n_total, group_counts);
 }
 
 extern "C" frz_status frz_match_list_collapsed(frz_matcher* m, const frz_corpus* corpus, const frz_subset* s, const frz_boost* b,
@@ -2449,19 +2492,11 @@ frz_status check_columns(frz_matcher* const* ms, const frz_corpus* const* cols, 
     if (sort > FRZ_SORT_INDEX_DESC) return frz_fail(FRZ_ERR_INVALID_ARG, "sort = %u is not a sort strategy", (unsigned)sort);
     return FRZ_OK;
 }
-}  // namespace
 
-// Several text fields of the same rows, one matcher per field (DESIGN.md §4.13): the multi-pattern loop over every
-// column's patterns in column order, each against its own column (match_patterns), then the ranked, collapsed and top-K
-// steps of the single-corpus calls.
-extern "C" frz_status frz_match_list_columns(frz_matcher* const* ms, const frz_corpus* const* cols, uint64_t n_cols, uint8_t sort,
-                                             const frz_subset* s, const frz_boost* b, const frz_groups* g, uint64_t per_group,
-                                             uint64_t k, frz_match* out, uint64_t* n_out, uint64_t* n_total, uint32_t* group_counts) {
-    FRZ_TRY(check_columns(ms, cols, n_cols, sort, nullptr));
-    if (g) FRZ_TRY(check_per_group(per_group));
-    if (!out && k > 0) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
-    const CallHandles h{s, b, g, per_group};
-    FRZ_TRY(check_handles(h, cols, n_cols, kNoColumn));
+// A column call whose arguments have passed (frz_match_list_columns, frz_match_list_columns_ordered): its Columns, its list
+// call from the handles, run on ms[0]'s workspace, the first min(k, total) rows → out.
+frz_status columns_call(frz_matcher* const* ms, const frz_corpus* const* cols, uint64_t n_cols, uint8_t sort, const CallHandles& h,
+                        uint64_t k, frz_match* out, uint64_t* n_out, uint64_t* n_total, uint32_t* group_counts) {
     FRZ_TRY(frz_ensure_device(cols[0]->st.device));   // (before a matcher is read)
     // the list starts from the column of the first non-negated pattern (its base, scanned in full), else from column 0
     Columns cs;
@@ -2485,6 +2520,36 @@ extern "C" frz_status frz_match_list_columns(frz_matcher* const* ms, const frz_c
     call.cols = std::move(cs);
     call.group_counts = group_counts;
     return match_list_host(ms[0], cols[start], call, out, k, n_out, n_total);
+}
+}  // namespace
+
+// Several text fields of the same rows, one matcher per field (DESIGN.md §4.13): the multi-pattern loop over every
+// column's patterns in column order, each against its own column (match_patterns), then the ranked, collapsed and top-K
+// steps of the single-corpus calls.
+extern "C" frz_status frz_match_list_columns(frz_matcher* const* ms, const frz_corpus* const* cols, uint64_t n_cols, uint8_t sort,
+                                             const frz_subset* s, const frz_boost* b, const frz_groups* g, uint64_t per_group,
+                                             uint64_t k, frz_match* out, uint64_t* n_out, uint64_t* n_total, uint32_t* group_counts) {
+    FRZ_TRY(check_columns(ms, cols, n_cols, sort, nullptr));
+    if (g) FRZ_TRY(check_per_group(per_group));
+    if (!out && k > 0) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
+    const CallHandles h{s, b, g, per_group};
+    FRZ_TRY(check_handles(h, cols, n_cols, kNoColumn));
+    return columns_call(ms, cols, n_cols, sort, h, k, out, n_out, n_total, group_counts);
+}
+
+// frz_match_list_columns' joined list ordered by an attribute, then collapsed when groups are given (DESIGN.md §4.15.1).
+extern "C" frz_status frz_match_list_columns_ordered(frz_matcher* const* ms, const frz_corpus* const* cols, uint64_t n_cols, uint8_t sort,
+                                                     const frz_subset* s, const frz_boost* b, const frz_attr* a, uint32_t order,
+                                                     const frz_groups* g, uint64_t per_group, uint64_t k, frz_match* out,
+                                                     uint64_t* n_out, uint64_t* n_total, uint32_t* group_counts) {
+    FRZ_TRY(check_columns(ms, cols, n_cols, sort, nullptr));
+    if (!a) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    if (g) FRZ_TRY(check_per_group(per_group));
+    if (!out && k > 0) return frz_fail(FRZ_ERR_INVALID_ARG, "null out");
+    FRZ_TRY(check_order(order));
+    const CallHandles h{s, b, g, per_group, a, order};
+    FRZ_TRY(check_handles(h, cols, n_cols, kNoColumn));
+    return columns_call(ms, cols, n_cols, sort, h, k, out, n_out, n_total, group_counts);
 }
 
 // ---------------------------------------------------------------------------------- batched top-K: entry points

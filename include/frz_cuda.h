@@ -533,6 +533,56 @@ FRZ_API frz_status frz_match_list_columns(frz_matcher* const* ms, const frz_corp
                                           uint64_t per_group, uint64_t k, frz_match* out, uint64_t* n_out,
                                           uint64_t* n_total, uint32_t* group_counts);
 
+/* ------------------------------------------------ ordered collapsed and ordered column calls
+ *
+ * The default screen of a shell-history search shows each distinct command once, newest first; a live grep lists the
+ * files with hits, most recently modified first; a launcher shows one entry per app, last used first.  Each needs the
+ * rows grouped and the groups represented by their first rows in an attribute's order, not by their best-scoring rows.
+ * A file picker orders file name + directory matches by modification time.  The reference has no such method: its
+ * callers fetch the whole list and collapse or sort it on the host.  These calls do it on the device. */
+
+/* The reference has no such method (see above).  Let L be the list frz_match_list_ordered(m, c, s, b, a, order,
+ * UINT64_MAX, ...) returns: the rows of frz_match_list_into restricted to the members of s, reversed under the *_DESC
+ * strategies, sorted stably by the order key (with the boost inside r), nulls last, remaining ties in index order.  Let C
+ * be the rows of L, in L's order, that are in no group or that have fewer than per_group earlier rows of L in their group
+ * (frz_match_list_collapsed's rule applied to this L).  The call writes C[0 : min(k, |C|)] to `out`, bit for bit, their
+ * number to *n_out and |C| to *n_total (may be NULL).  group_counts (may be NULL) is a host array of
+ * frz_groups_count(g) entries: entry j receives the rows of L in group j, counted before collapsing.
+ * per_group: 1 .. 32, or UINT64_MAX for no cap (C = L: frz_match_list_ordered plus the counts).  With the empty matcher
+ * the call lists the live rows, so per_group = 1 and FRZ_ORDER_ATTR_DESC over a timestamp gives the latest row of each
+ * group, newest first.
+ *
+ * Every other rule is frz_match_list_ordered's: `out` is HOST memory with room for k matches (min(k, frz_corpus_len(c))
+ * suffices, or min(k, frz_subset_len(s)) with a subset), k = 0 only counts, k = UINT64_MAX returns all of C, and the call
+ * never returns FRZ_ERR_CAPACITY.  Checked in this order before any device work: FRZ_ERR_INVALID_ARG for a NULL matcher,
+ * corpus, attribute or groups; per_group 0 (then FRZ_ERR_UNSUPPORTED for any other per_group out of range); a NULL out
+ * with k > 0; an order above FRZ_ORDER_SCORE_THEN_ATTR_ASC; a subset, boost, groups or attribute handle of another corpus
+ * (the first one reported in that order).  s and b may be NULL.  Blocking; it only reads its handles. */
+FRZ_API frz_status frz_match_list_ordered_collapsed(frz_matcher* m, const frz_corpus* c, const frz_subset* s,
+                                                    const frz_boost* b, const frz_attr* a, uint32_t order,
+                                                    const frz_groups* g, uint64_t per_group, uint64_t k, frz_match* out,
+                                                    uint64_t* n_out, uint64_t* n_total, uint32_t* group_counts);
+
+/* The reference has no such method (see above).  Let L0 be the joined rows of frz_match_list_columns(ms, cols, n_cols,
+ * sort, s, ...) before its ordering step: the rows that match in every column, each with the saturating sum of its
+ * column scores and the OR of its exact flags, in index order, reversed under the *_DESC strategies of `sort`.  L is L0
+ * ordered by the attribute exactly as frz_match_list_ordered orders its L0, with the boost inside r (r is the summed
+ * score, clamped with the boost).  With g, C is L collapsed as frz_match_list_ordered_collapsed collapses its L and
+ * group_counts (may be NULL) receives L's rows per group; without g, C = L and per_group and group_counts are not read.
+ * The call writes C[0 : min(k, |C|)] to `out` (HOST memory), their number to *n_out and |C| to *n_total (may be NULL);
+ * k = 0 only counts, k = UINT64_MAX returns all of C, never FRZ_ERR_CAPACITY.
+ *
+ * Checked in this order before any device work: frz_match_list_columns' column checks (n_cols, NULL matchers or
+ * columns, devices, lengths, the index range, sort); then FRZ_ERR_INVALID_ARG for a NULL attribute; with g, per_group 0
+ * (then FRZ_ERR_UNSUPPORTED for any other per_group out of range); a NULL out with k > 0; an order above
+ * FRZ_ORDER_SCORE_THEN_ATTR_ASC; a subset, boost, groups or attribute handle made on none of the columns.  A handle of
+ * any column serves every column.  Every other rule (scratch, speed, column order, sharing) is frz_match_list_columns'. */
+FRZ_API frz_status frz_match_list_columns_ordered(frz_matcher* const* ms, const frz_corpus* const* cols, uint64_t n_cols,
+                                                  uint8_t sort, const frz_subset* s, const frz_boost* b, const frz_attr* a,
+                                                  uint32_t order, const frz_groups* g, uint64_t per_group, uint64_t k,
+                                                  frz_match* out, uint64_t* n_out, uint64_t* n_total,
+                                                  uint32_t* group_counts);
+
 /* frz_match_list_batch_top (above) where each query may have its own subset and boost, in one call: a service whose users
  * each search their own rows (a subset) ranked by a prior (a boost).  The reference has no such method (see the subset
  * and ranked calls above).  For every j < q, out[j*k .. j*k + n_out[j]), n_out[j] and n_total[j] are bit for bit what the
