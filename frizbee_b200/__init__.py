@@ -97,6 +97,7 @@ def lib():
     L.frz_match_list_batch_top.argtypes = [vp, u64, vp, u64, vp, vp, vp]
     L.frz_match_list_batch.argtypes = [vp, u64, vp, vp, vp, u64, vp, vp, vp]
     L.frz_match_list_batch_collapsed.argtypes = [vp, u64, vp, vp, vp, vp, vp, u64, vp, vp, vp, vp]
+    L.frz_match_list_batch_ordered.argtypes = [vp, u64, vp, vp, vp, vp, vp, vp, vp, u64, vp, vp, vp, vp]
     L.frz_debug_batch_limits.argtypes = [u64, u64]
     L.frz_debug_batch_limits.restype = None
     L.frz_debug_batch_last.argtypes = [vp]
@@ -780,6 +781,30 @@ def match_list_batch_collapsed(matchers, corpus: Corpus, k: int, groups, per_gro
     return b.result()
 
 
+def match_list_batch_ordered(matchers, corpus: Corpus, k: int, attrs, order=Order.AttrDesc, subsets=None, boosts=None, groups=None,
+                             per_group=1, counts: bool = False):
+    """frz_match_list_batch_ordered: match_list_batch_collapsed where query j may also order its rows by attrs[j].  attrs:
+    one Attr for every query, or one Attr or None per matcher; order: one Order, or one per matcher.  Query j's rows are
+    those of matcher j's match_list_ordered_array(corpus, attrs[j], order[j], k, subsets[j], boosts[j], groups=groups[j],
+    per_group=per_group[j]) when it has an attribute, else those of match_list_batch_collapsed.  Returns the (q, k) rows,
+    n_out and n_total as match_list_batch_top, and with counts=True also a list of each query's rows per group (uint32,
+    len(groups[j]) entries; None for a query without groups)."""
+    q, k = len(matchers), int(k)
+    if attrs is None or isinstance(attrs, Attr):
+        attrs = [attrs] * q
+    if isinstance(order, (int, np.integer)):
+        order = [order] * q
+    order = list(order)
+    if len(order) != q:
+        raise ValueError(f"{q} matchers need {q} orders, got {len(order)}")
+    b = _BatchArgs(q, k, subsets, boosts).grouped(groups, per_group, counts, "matchers")
+    ha = _handles(attrs, q, "attrs")
+    orders = np.array([int(o) for o in order] or [0], dtype=np.uint32)
+    _check(lib().frz_match_list_batch_ordered(_matcher_array(matchers), q, corpus._h, b.hs, b.hb, ha, orders.ctypes.data, b.hg,
+                                              b.pg.ctypes.data, k, *b.outputs(), b.hc))
+    return b.result()
+
+
 def match_list_columns(matchers, columns, k: Optional[int] = None, sort: SortStrategy = SortStrategy.ScoreThenIndexAsc,
                        subset: Optional[Subset] = None, boost: Optional[Boost] = None, groups: Optional[Groups] = None,
                        per_group: Optional[int] = 1, counts: bool = False, out: Optional[np.ndarray] = None,
@@ -839,7 +864,7 @@ def match_list_batch_columns(matchers, columns, k: int, sort: SortStrategy = Sor
 
 def batch_last() -> dict:
     """Test aid (frz_debug_batch_last): what this thread's last batched call (match_list_batch_top, match_list_batch,
-    match_list_batch_collapsed or match_list_batch_columns) did."""
+    match_list_batch_collapsed, match_list_batch_ordered or match_list_batch_columns) did."""
     v = np.zeros(4, dtype=np.uint64)
     lib().frz_debug_batch_last(v.ctypes.data)
     return {"batched": int(v[0]), "overflowed": int(v[1]), "sub_batches": int(v[2]), "launches": int(v[3])}

@@ -1,8 +1,11 @@
 // collapse.cu — the per-group count and the rounds of the collapsed call (frz_match_list_collapsed, DESIGN.md §4.12), of
 // the ordered collapsed calls (frz_match_list_ordered_collapsed, frz_match_list_columns_ordered, §4.15.1), and of the
 // batched collapsed call's sub-batches (frz_match_list_batch_collapsed, §4.11).  The row rule is collapse_plan.cuh's;
-// host.cu compacts the kept rows and sorts them, or k_batch_top<CollapsedKey> (batch.cu) cuts them per query.
+// host.cu compacts the kept rows and sorts them, or k_batch_top<CollapsedKey> (batch.cu) cuts them per query, or for the
+// batched ordered call's sub-batches (frz_match_list_batch_ordered) the rounds run on the order key and the batched select
+// (order.cu) orders the kept rows.
 #include "batch_collapse_plan.cuh"
+#include "batch_order_plan.cuh"
 #include "collapse_plan.cuh"
 #include "frz_host.h"
 
@@ -258,6 +261,76 @@ __global__ void __launch_bounds__(kCollapseBlock) k_batch_collapse_take(const Fr
     }
 }
 
+// The batched rounds on the order key (frz_match_list_batch_ordered): k_collapse_max_hi / _max_lo / _take_key per query,
+// over its members, with its keys (k_batch_order_keys), its best table as best_hi and its best_lo table.
+__global__ void __launch_bounds__(kCollapseBlock) k_batch_collapse_max_hi(const FrzBatchDev b, const FrzBatchTables t,
+                                                                         const FrzBatchOrderDev o, uint32_t round) {
+    BatchQuery q;
+    if (!batch_query(b, t, blockIdx.y, &q) || !frz_batch_collapse_in_round(q.c.per_group, round)) return;
+    const uint32_t* counts = t.counts + q.c.table;
+    unsigned long long* best_hi = t.best + q.c.table;
+    const FrzOrderKey* keys = o.keys + frz_batch_order_keys_at(blockIdx.y, b.list_stride);
+    const uint32_t lane = threadIdx.x & 31;
+    const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+    for (uint64_t i0 = (uint64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31u); i0 < q.n; i0 += stride) {
+        const uint64_t i = i0 + lane;
+        uint32_t g = kFrzGroupNone;
+        unsigned long long e = 0;
+        if (i < q.n) {
+            const uint32_t rg = batch_group(q, q.list[i].index);
+            if (rg != kFrzGroupNone && frz_collapse_contends(rg, counts[rg], q.c.per_group, q.taken[i] != 0)) {
+                g = rg;
+                e = frz_collapse_hi_entry(load_key(keys, i));
+            }
+        }
+        warp_max_into(best_hi, g, e, lane);
+    }
+}
+
+__global__ void __launch_bounds__(kCollapseBlock) k_batch_collapse_max_lo(const FrzBatchDev b, const FrzBatchTables t,
+                                                                         const FrzBatchOrderDev o, uint32_t round) {
+    BatchQuery q;
+    if (!batch_query(b, t, blockIdx.y, &q) || !frz_batch_collapse_in_round(q.c.per_group, round)) return;
+    const uint32_t* counts = t.counts + q.c.table;
+    const unsigned long long* best_hi = t.best + q.c.table;
+    unsigned long long* best_lo = o.best_lo + q.c.table;
+    const FrzOrderKey* keys = o.keys + frz_batch_order_keys_at(blockIdx.y, b.list_stride);
+    const uint32_t lane = threadIdx.x & 31;
+    const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+    for (uint64_t i0 = (uint64_t)blockIdx.x * blockDim.x + (threadIdx.x & ~31u); i0 < q.n; i0 += stride) {
+        const uint64_t i = i0 + lane;
+        uint32_t g = kFrzGroupNone;
+        unsigned long long e = 0;
+        if (i < q.n) {
+            const uint32_t rg = batch_group(q, q.list[i].index);
+            if (rg != kFrzGroupNone && frz_collapse_contends(rg, counts[rg], q.c.per_group, q.taken[i] != 0)) {
+                g = rg;
+                e = frz_collapse_lo_entry(load_key(keys, i), __ldcg(&best_hi[rg]));
+            }
+        }
+        warp_max_into(best_lo, g, e, lane);
+    }
+}
+
+__global__ void __launch_bounds__(kCollapseBlock) k_batch_collapse_take_key(const FrzBatchDev b, const FrzBatchTables t,
+                                                                           const FrzBatchOrderDev o, uint32_t round) {
+    BatchQuery q;
+    if (!batch_query(b, t, blockIdx.y, &q) || !frz_batch_collapse_in_round(q.c.per_group, round)) return;
+    const uint32_t* counts = t.counts + q.c.table;
+    unsigned long long* best_hi = t.best + q.c.table;
+    unsigned long long* best_lo = o.best_lo + q.c.table;
+    const FrzOrderKey* keys = o.keys + frz_batch_order_keys_at(blockIdx.y, b.list_stride);
+    for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < q.n; i += (uint64_t)gridDim.x * blockDim.x) {
+        const uint32_t g = batch_group(q, q.list[i].index);
+        if (g == kFrzGroupNone || !frz_collapse_contends(g, counts[g], q.c.per_group, q.taken[i] != 0)) continue;
+        if (frz_collapse_key_takes(load_key(keys, i), __ldcg(&best_lo[g]))) {
+            q.taken[i] = 1;
+            best_hi[g] = 0;
+            best_lo[g] = 0;
+        }
+    }
+}
+
 }  // namespace
 
 frz_status frz_launch_batch_collapse(const FrzBatchDev& b, const FrzBatchTables& t, uint32_t nq, uint32_t rounds, cudaStream_t stream,
@@ -272,6 +345,22 @@ frz_status frz_launch_batch_collapse(const FrzBatchDev& b, const FrzBatchTables&
         k_batch_collapse_take<<<grid, kCollapseBlock, 0, stream>>>(b, t, r);
     }
     st->launches += 1 + 2 * (uint64_t)rounds;
+    FRZ_CUDA_TRY(cudaGetLastError());
+    return FRZ_OK;
+}
+
+frz_status frz_launch_batch_collapse_by_key(const FrzBatchDev& b, const FrzBatchTables& t, const FrzBatchOrderDev& o, uint32_t nq,
+                                            uint32_t rounds, cudaStream_t stream, FrzLaunchStats* st) {
+    if (nq == 0) return FRZ_OK;
+    const uint32_t gx = (uint32_t)std::max<uint64_t>(1, (uint64_t)grid_for(b.list_stride, kCollapseBlock) / nq);
+    const dim3 grid(gx, nq);
+    k_batch_collapse_count<<<grid, kCollapseBlock, 0, stream>>>(b, t);
+    for (uint32_t r = 0; r < rounds; r++) {
+        k_batch_collapse_max_hi<<<grid, kCollapseBlock, 0, stream>>>(b, t, o, r);
+        k_batch_collapse_max_lo<<<grid, kCollapseBlock, 0, stream>>>(b, t, o, r);
+        k_batch_collapse_take_key<<<grid, kCollapseBlock, 0, stream>>>(b, t, o, r);
+    }
+    st->launches += 1 + 3 * (uint64_t)rounds;
     FRZ_CUDA_TRY(cudaGetLastError());
     return FRZ_OK;
 }

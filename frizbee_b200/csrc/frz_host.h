@@ -412,6 +412,28 @@ frz_status frz_launch_batch_collapse(const FrzBatchDev& b, const FrzBatchTables&
 frz_status frz_launch_batch_top_collapsed(const FrzBatchDev& b, const FrzBatchTables& t, uint32_t nq, uint32_t k, FrzMatchDev* rows,
                                           unsigned long long* totals, cudaStream_t stream, FrzLaunchStats* st);
 
+// The ordering of a sub-batch of frz_match_list_batch_ordered (host.cu; the per-query arithmetic is batch_order_plan.cuh's).
+// Every query of such a sub-batch is ordered.
+struct FrzBatchOrderDev {
+    const FrzOrderDev* ords;        // [j] the query's attribute, boost, order and direction, on the device
+    FrzOrderKey* keys;              // [j][list_stride] its list rows' keys
+    uint32_t* cand;                 // [j][2][list_stride] its rows, then the select's candidates
+    uint32_t* sel;                  // [j][kFrzOrderBlockRows] the selection
+    FrzOrderState* st;              // [j] zero before the key kernel
+    uint32_t* hist;                 // [j][kFrzOrderBins] zero
+    unsigned long long* best_lo;    // [slot][n_groups_max] with grouped queries: zero between rounds and calls
+};
+// order.cu: every query's keys (k_batch_order_keys), one launch over the nq queries
+frz_status frz_launch_batch_order_keys(const FrzBatchDev& b, const FrzBatchOrderDev& o, uint32_t nq, cudaStream_t stream, FrzLaunchStats* st);
+// collapse.cu: frz_launch_batch_collapse with rounds on the order keys (collapse_plan.cuh's two-step max, three passes per round)
+frz_status frz_launch_batch_collapse_by_key(const FrzBatchDev& b, const FrzBatchTables& t, const FrzBatchOrderDev& o, uint32_t nq,
+                                            uint32_t rounds, cudaStream_t stream, FrzLaunchStats* st);
+// order.cu: every query's rows (t: the groups, or t.cols == nullptr when no query of the sub-batch has any), their select
+// and their sort: its first min(k, total) rows in order → rows[j * k ...] and its total → totals[j], or kFrzBatchOverflow
+// there when its sticky device error is set (k <= kFrzBatchMaxK)
+frz_status frz_launch_batch_order_top(const FrzBatchDev& b, const FrzBatchTables& t, const FrzBatchOrderDev& o, uint32_t nq, uint32_t k,
+                                      FrzMatchDev* rows, unsigned long long* totals, cudaStream_t stream, FrzLaunchStats* st);
+
 // The join of a sub-batch of frz_match_list_batch_columns (host.cu; the per-row rule is batch_columns_plan.cuh's).
 struct FrzColumnFold;
 struct FrzBatchColumnsDev {

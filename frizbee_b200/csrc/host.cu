@@ -21,6 +21,7 @@
 #include <optional>
 
 #include "batch_collapse_plan.cuh"
+#include "batch_order_plan.cuh"
 #include "batch_columns_plan.cuh"
 #include "batch_plan.cuh"
 #include "collapse_plan.cuh"
@@ -1700,11 +1701,12 @@ frz_status match_list_host(frz_matcher* m, const frz_corpus* corpus, const ListC
 }  // namespace
 
 // ---------------------------------------------------------------------------------- batched top-K
-// frz_match_list_batch_collapsed, frz_match_list_batch and frz_match_list_batch_top (DESIGN.md §4.11), and
-// frz_match_list_batch_columns (§4.13).  Queries of the batched class run in sub-batches whose every stage is one launch
-// (per kernel variant present, and per column) over all of the sub-batch's queries, with one upload, one read-back and one
-// synchronise per sub-batch; every other query, and every query of an overflowed sub-batch, runs its single-query call's
-// pipeline (frz_match_list_top, _subset_top, _ranked, _collapsed or _columns).  The entry points follow the column calls.
+// frz_match_list_batch_ordered, frz_match_list_batch_collapsed, frz_match_list_batch and frz_match_list_batch_top
+// (DESIGN.md §4.11), and frz_match_list_batch_columns (§4.13).  Queries of the batched class run in sub-batches whose
+// every stage is one launch (per kernel variant present, and per column) over all of the sub-batch's queries, with one
+// upload, one read-back and one synchronise per sub-batch; ordered queries run in sub-batches of their own.  Every other
+// query, and every query of an overflowed sub-batch, runs its single-query call's pipeline (frz_match_list_top,
+// _subset_top, _ranked, _collapsed, _ordered, _ordered_collapsed or _columns).  The entry points follow the column calls.
 namespace {
 
 // Device scratch of one sub-batch's queries, in one allocation: a fixed budget, so a batch call holds the same scratch for
@@ -1740,10 +1742,11 @@ struct BatchLayout {
     uint64_t nt = 0, stride = 0, cap = 0, k = 0;
     uint64_t groups = 0;     // entries of each query slot's group tables (0: no query of the call has groups)
     uint64_t n_cols = 0;     // columns of a frz_match_list_batch_columns call (0: a single-corpus call)
-    uint64_t off[21] = {};   // byte offsets of the arrays below, in this order
+    bool ordered = false;    // the call has batched ordered queries (batch_order_plan.cuh's arrays)
+    uint64_t off[28] = {};   // byte offsets of the arrays below, in this order
     uint64_t bytes = 0;
-    enum { CTR, BITMAP, PREFIX, TCOUNT, TBASE, SURV, LISTS, BEST, TAKEN, ACC, JERR, PATS, REV, BYSC, SCOPE, COLS, CMAP, TOTALS, ROWS,
-           COUNTS, END };
+    enum { CTR, BITMAP, PREFIX, TCOUNT, TBASE, SURV, LISTS, BEST, TAKEN, ACC, JERR, PATS, REV, BYSC, SCOPE, COLS, CMAP, ORD, TOTALS, ROWS,
+           COUNTS, KEYS, CAND, SEL, STATE, HIST, BESTLO, END };
     // queries per sub-batch for this corpus and k (0: fewer than two fit the budget)
     static uint64_t per_query(const FrzCorpusStorage& cs, uint64_t k, uint64_t cap) {
         const uint64_t nt = cs.n_tiles;
@@ -1752,23 +1755,34 @@ struct BatchLayout {
                sizeof(FrzBatchScope) + sizeof(unsigned long long) + k * sizeof(FrzMatchDev) + 13 * 256 / 2;
     }
     // n_cols_ > 0 (a column call) adds each query's accumulator and error word, a pattern slot per column and query, and
-    // the fold records (batch_columns_plan.cuh); a single-corpus call gets the layout it had before column calls existed
-    BatchLayout(const FrzCorpusStorage& cs, uint64_t k_, uint64_t cap_, uint64_t qs, uint64_t groups_ = 0, uint64_t n_cols_ = 0)
-        : nt(cs.n_tiles), stride(std::max<uint64_t>(cs.n, 1)), cap(cap_), k(k_), groups(groups_), n_cols(n_cols_) {
+    // the fold records (batch_columns_plan.cuh); a single-corpus call gets the layout it had before column calls existed.
+    // ordered_ adds the ordered sub-batches' arrays (ORD is uploaded with the patterns; the rest follow the read-back and
+    // take no room, not even alignment, without ordered queries: such a call gets the layout it had before them)
+    BatchLayout(const FrzCorpusStorage& cs, uint64_t k_, uint64_t cap_, uint64_t qs, uint64_t groups_ = 0, uint64_t n_cols_ = 0,
+                bool ordered_ = false)
+        : nt(cs.n_tiles), stride(std::max<uint64_t>(cs.n, 1)), cap(cap_), k(k_), groups(groups_), n_cols(n_cols_), ordered(ordered_) {
         const uint64_t g = groups ? qs : 0;   // the group arrays exist only in a call with grouped queries
         const uint64_t c = n_cols ? qs : 0;   // the join arrays only in a column call
+        const uint64_t o = ordered ? qs : 0;  // the ordering arrays only in a call with ordered queries
         const uint64_t size[END] = {qs * sizeof(FrzCounters), qs * nt * 32 * sizeof(uint32_t), qs * nt * 32 * sizeof(uint16_t),
                                     qs * nt * sizeof(uint32_t), qs * nt * sizeof(uint64_t), qs * FRZ_N_CLASSES * cap * sizeof(FrzSurvivor),
                                     qs * stride * sizeof(FrzMatchDev), g * groups * sizeof(unsigned long long), g * stride,
                                     c * stride * sizeof(uint32_t), c * sizeof(uint32_t),
                                     qs * std::max<uint64_t>(n_cols, 1) * sizeof(FrzPatternDev), qs, qs, qs * sizeof(FrzBatchScope),
-                                    g * sizeof(FrzBatchCollapse), c * (n_cols * sizeof(FrzColumnFold) + 1),
-                                    qs * sizeof(unsigned long long), qs * k * sizeof(FrzMatchDev), g * groups * sizeof(uint32_t)};
+                                    g * sizeof(FrzBatchCollapse), c * (n_cols * sizeof(FrzColumnFold) + 1), o * sizeof(FrzOrderDev),
+                                    qs * sizeof(unsigned long long), qs * k * sizeof(FrzMatchDev), g * groups * sizeof(uint32_t),
+                                    o * stride * sizeof(FrzOrderKey), o * 2 * stride * sizeof(uint32_t), o * kFrzOrderBlockRows * sizeof(uint32_t),
+                                    o * sizeof(FrzOrderState), o * kFrzOrderBins * sizeof(uint32_t), (g && o) * g * groups * sizeof(unsigned long long)};
         uint64_t at = 0;
         for (int i = 0; i < END; i++) {
-            // CTR..BITMAP are zeroed as one range, ACC..JERR too, PATS..CMAP uploaded as one, TOTALS..COUNTS read back as one
-            const bool packed = i == BITMAP || i == JERR || i == REV || i == BYSC || i == SCOPE || i == COLS || i == CMAP || i == ROWS ||
-                                i == COUNTS;
+            // CTR..BITMAP are zeroed as one range, ACC..JERR too, PATS..ORD uploaded as one, TOTALS..COUNTS read back as one,
+            // STATE..HIST zeroed as one
+            const bool packed = i == BITMAP || i == JERR || i == REV || i == BYSC || i == SCOPE || i == COLS || i == CMAP || i == ORD ||
+                                i == ROWS || i == COUNTS || i == HIST;
+            if (i > COUNTS && !size[i]) {
+                off[i] = at;
+                continue;
+            }
             if (!packed) at = (at + 255) & ~255ull;
             else at = (at + 7) & ~7ull;
             off[i] = at;
@@ -1833,15 +1847,18 @@ struct BatchGroups {
 // or ranked, else every query's subset and boost (indexed as ms).  gr: the call's groups (L.groups > 0 when it has any).
 // bc: a column call (c is its column 0): each column's stages run for the queries with a pattern in it, in slots of their
 // own, and the join (batch_columns.cu) leaves each query's list where the cut reads it.
+// ords: an ordered sub-batch (frz_match_list_batch_ordered, L.ordered), every query's attribute, boost and order (indexed
+// as ms); its last stage orders each query's rows by its order key (order.cu) in place of the cut.
 // *overflow: a survivor list overflowed, nothing was written to the results (the caller runs the queries one by one).
 frz_status batch_run(frz_matcher* const* ms, const FrzBatchScope* scopes, const BatchGroups& gr, const uint64_t* which, uint32_t ns,
                      const frz_corpus* c, uint64_t k, const BatchLayout& L, uint8_t* d, frz_match* out, uint64_t* n_out,
-                     uint64_t* n_total, bool* overflow, FrzLaunchStats& st, const BatchColumns* bc = nullptr) {
+                     uint64_t* n_total, bool* overflow, FrzLaunchStats& st, const BatchColumns* bc = nullptr,
+                     const FrzOrderDev* ords = nullptr) {
     const FrzCorpusStorage& cs = c->st;
     cudaStream_t stream = nullptr;
     *overflow = false;
     const uint64_t up = L.off[BatchLayout::TOTALS] - L.off[BatchLayout::PATS];
-    FRZ_TRY(c->batch_stage.reserve(std::max(up, L.off[BatchLayout::END] - L.off[BatchLayout::TOTALS])));
+    FRZ_TRY(c->batch_stage.reserve(std::max(up, L.off[BatchLayout::KEYS] - L.off[BatchLayout::TOTALS])));
     uint8_t* h = c->batch_stage.get();
     FrzPatternDev* h_pats = reinterpret_cast<FrzPatternDev*>(h);
     uint8_t* h_rev = h + (L.off[BatchLayout::REV] - L.off[BatchLayout::PATS]);
@@ -1890,6 +1907,12 @@ frz_status batch_run(frz_matcher* const* ms, const FrzBatchScope* scopes, const 
             }
             if (f.slot != kFrzColumnSkip) { h_need[j]++; folded[col] = 1; }
         }
+    }
+    // an ordered sub-batch's attributes, with each query's list direction
+    FrzOrderDev* h_ord = reinterpret_cast<FrzOrderDev*>(h + (L.off[BatchLayout::ORD] - L.off[BatchLayout::PATS]));
+    for (uint32_t j = 0; j < ns && ords; j++) {
+        h_ord[j] = ords[which[j]];
+        h_ord[j].reversed = h_rev[j];
     }
     const uint64_t down = L.off[BatchLayout::COUNTS] + n_back * L.groups * sizeof(uint32_t) - L.off[BatchLayout::TOTALS];
     FrzBatchDev b;
@@ -1940,13 +1963,32 @@ frz_status batch_run(frz_matcher* const* ms, const FrzBatchScope* scopes, const 
         FRZ_TRY(frz_launch_batch_columns_join(b, jd, (uint32_t)L.nt, ns, stream, &st));
     }
     const FrzBatchScope* d_scope = reinterpret_cast<const FrzBatchScope*>(d + L.off[BatchLayout::SCOPE]);
-    if (n_grouped) {   // the collapse, then the kept rows' cut
-        FrzBatchTables t;
+    FrzBatchTables t = {};
+    t.scopes = d_scope;
+    if (L.groups) {
         t.cols = reinterpret_cast<const FrzBatchCollapse*>(d + L.off[BatchLayout::COLS]);
-        t.scopes = d_scope;
         t.counts = reinterpret_cast<uint32_t*>(d + L.off[BatchLayout::COUNTS]);
         t.best = reinterpret_cast<unsigned long long*>(d + L.off[BatchLayout::BEST]);
         t.taken = d + L.off[BatchLayout::TAKEN];
+    }
+    if (ords) {   // the keys, the collapse on them, then each query's rows selected and sorted by key
+        FrzBatchOrderDev od;
+        od.ords = reinterpret_cast<const FrzOrderDev*>(d + L.off[BatchLayout::ORD]);
+        od.keys = reinterpret_cast<FrzOrderKey*>(d + L.off[BatchLayout::KEYS]);
+        od.cand = reinterpret_cast<uint32_t*>(d + L.off[BatchLayout::CAND]);
+        od.sel = reinterpret_cast<uint32_t*>(d + L.off[BatchLayout::SEL]);
+        od.st = reinterpret_cast<FrzOrderState*>(d + L.off[BatchLayout::STATE]);
+        od.hist = reinterpret_cast<uint32_t*>(d + L.off[BatchLayout::HIST]);
+        od.best_lo = reinterpret_cast<unsigned long long*>(d + L.off[BatchLayout::BESTLO]);
+        FRZ_CUDA_TRY(cudaMemsetAsync(od.st, 0, L.off[BatchLayout::HIST] + (uint64_t)ns * kFrzOrderBins * sizeof(uint32_t) - L.off[BatchLayout::STATE],
+                                     stream));
+        FRZ_TRY(frz_launch_batch_order_keys(b, od, ns, stream, &st));
+        if (n_grouped) {
+            FRZ_CUDA_TRY(cudaMemsetAsync(t.counts, 0, n_grouped * L.groups * sizeof(uint32_t), stream));
+            FRZ_TRY(frz_launch_batch_collapse_by_key(b, t, od, ns, rounds, stream, &st));
+        }
+        FRZ_TRY(frz_launch_batch_order_top(b, t, od, ns, (uint32_t)k, rows, totals, stream, &st));
+    } else if (n_grouped) {   // the collapse, then the kept rows' cut
         FRZ_CUDA_TRY(cudaMemsetAsync(t.counts, 0, n_grouped * L.groups * sizeof(uint32_t), stream));
         FRZ_TRY(frz_launch_batch_collapse(b, t, ns, rounds, stream, &st));
         FRZ_TRY(frz_launch_batch_top_collapsed(b, t, ns, (uint32_t)k, rows, totals, stream, &st));
@@ -2414,8 +2456,10 @@ static_assert(FRZ_ORDER_SCORE_THEN_ATTR_DESC == kFrzOrderScoreFirst && FRZ_ORDER
               "order_plan.cuh mirrors frz_cuda.h");
 
 namespace {
-frz_status check_order(uint32_t order) {
-    if (order >= kFrzOrderCount) return frz_fail(FRZ_ERR_INVALID_ARG, "order %u (at most %u)", order, kFrzOrderCount - 1);
+frz_status check_order(uint32_t order, uint64_t query = kNoQuery) {
+    char at[32] = "";
+    if (query != kNoQuery) snprintf(at, sizeof at, " at %llu", (unsigned long long)query);
+    if (order >= kFrzOrderCount) return frz_fail(FRZ_ERR_INVALID_ARG, "order %u%s (at most %u)", order, at, kFrzOrderCount - 1);
     return FRZ_OK;
 }
 }  // namespace
@@ -2559,9 +2603,17 @@ extern "C" frz_status frz_match_list_batch(frz_matcher* const* ms, uint64_t q, c
     return frz_match_list_batch_collapsed(ms, q, corpus, subsets, boosts, nullptr, nullptr, k, out, n_out, n_total, nullptr);
 }
 
+extern "C" frz_status frz_match_list_batch_collapsed(frz_matcher* const* ms, uint64_t q, const frz_corpus* corpus,
+                                                     const frz_subset* const* subsets, const frz_boost* const* boosts,
+                                                     const frz_groups* const* groups, const uint64_t* per_group, uint64_t k,
+                                                     frz_match* out, uint64_t* n_out, uint64_t* n_total, uint32_t* const* group_counts) {
+    return frz_match_list_batch_ordered(ms, q, corpus, subsets, boosts, nullptr, nullptr, groups, per_group, k, out, n_out, n_total,
+                                        group_counts);
+}
+
 namespace {
-// The arguments of a batched call (frz_match_list_batch_collapsed, frz_match_list_batch_columns).  bc: a column call,
-// whose query j has the matchers ms[j * n_cols ..] and whose corpus is its column 0.
+// The arguments of a batched call (frz_match_list_batch_ordered, frz_match_list_batch_columns).  bc: a column call,
+// whose query j has the matchers ms[j * n_cols ..] and whose corpus is its column 0 (it has no attributes).
 struct BatchCall {
     frz_matcher* const* ms;
     uint64_t q;
@@ -2576,16 +2628,19 @@ struct BatchCall {
     uint64_t* n_out;
     uint64_t* n_total;
     uint32_t* const* group_counts;
+    const frz_attr* const* attrs = nullptr;
+    const uint32_t* orders = nullptr;   // nullptr: FRZ_ORDER_ATTR_DESC for every query
 
     CallHandles handles_of(uint64_t j) const {
         return CallHandles{subsets ? subsets[j] : nullptr, boosts ? boosts[j] : nullptr, groups ? groups[j] : nullptr,
-                           per_group ? per_group[j] : 1};
+                           per_group ? per_group[j] : 1, attrs ? attrs[j] : nullptr, orders ? orders[j] : (uint32_t)FRZ_ORDER_ATTR_DESC};
     }
 };
 
 // The driver of the batched calls once their matchers and columns have passed: every query's per_group (with or without
-// groups) and handles, then the outputs, are checked; the queries of the batched class run in sub-batches (batch_run),
-// every other query, and every query of an overflowed sub-batch, its single-query call.
+// groups), every order (with or without an attribute) and the handles, then the outputs, are checked; the queries of the
+// batched class run in sub-batches (batch_run), the ordered ones in sub-batches of their own, every other query, and every
+// query of an overflowed sub-batch, its single-query call.
 frz_status batch_drive(const BatchCall& a) {
     frz_matcher* const* ms = a.ms;
     const uint64_t q = a.q, k = a.k;
@@ -2595,6 +2650,7 @@ frz_status batch_drive(const BatchCall& a) {
     uint64_t* n_out = a.n_out;
     uint64_t* n_total = a.n_total;
     for (uint64_t j = 0; a.per_group && j < q; j++) FRZ_TRY(check_per_group(a.per_group[j], j));
+    for (uint64_t j = 0; a.orders && j < q; j++) FRZ_TRY(check_order(a.orders[j], j));
     for (uint64_t j = 0; j < q; j++)
         FRZ_TRY(bc ? check_handles(a.handles_of(j), bc->cols, bc->n_cols, kNoColumn, j) : check_handles(a.handles_of(j), &corpus, 1, kAnotherCorpus, j));
     if (q && !n_out) return frz_fail(FRZ_ERR_INVALID_ARG, "null n_out");
@@ -2632,12 +2688,14 @@ frz_status batch_drive(const BatchCall& a) {
     const uint64_t qs_max = std::min<uint64_t>(fit, kFrzBatchMaxSub);
     uint64_t n_groups_max = 0;   // the largest n_groups among the batched grouped queries
     for (uint64_t j = 0; j < q; j++) {
-        const frz_groups* g = a.handles_of(j).g;
+        const CallHandles h = a.handles_of(j);
+        const uint64_t n_groups = h.g ? h.g->n_groups : 0;
         if (qs_max >= 2 && selected(j) &&
-            (!g || (frz_batch_collapse_fit(kBatchScratchBytes, base, g->n_groups, list_rows) &&
-                    (!counts_of(j) || g->n_groups <= kBatchMaxCountedGroups)))) {
+            (!h.g || (frz_batch_collapse_fit(kBatchScratchBytes, base, n_groups, list_rows) &&
+                      (!counts_of(j) || n_groups <= kBatchMaxCountedGroups))) &&
+            (!h.a || frz_batch_order_fit(kBatchScratchBytes, base, n_groups, list_rows))) {
             batched.push_back(j);
-            if (g) n_groups_max = std::max(n_groups_max, g->n_groups);
+            n_groups_max = std::max(n_groups_max, n_groups);
         } else {
             FRZ_TRY(single(j));
         }
@@ -2646,7 +2704,16 @@ frz_status batch_drive(const BatchCall& a) {
         for (uint64_t j : batched) FRZ_TRY(single(j));
         return FRZ_OK;
     }
-    // every query's subset and boost, as k_batch_top<ScopedKey> reads them (none when no query has either)
+    // the ordered queries go to sub-batches of their own; when their tables do not fit two to a sub-batch beside the
+    // call's largest group tables, they run their single-query calls
+    std::vector<uint64_t> ordered, unordered;
+    for (uint64_t j : batched) (a.handles_of(j).a ? ordered : unordered).push_back(j);
+    if (!ordered.empty() && !frz_batch_order_fit(kBatchScratchBytes, base, n_groups_max, list_rows)) {
+        for (uint64_t j : ordered) FRZ_TRY(single(j));
+        ordered.clear();
+    }
+    // every query's subset and boost, as k_batch_top<ScopedKey> reads them (none when no query has either); an ordered
+    // query's subset is read by k_batch_order_members, its boost is part of its order key
     std::vector<FrzBatchScope> scopes;
     for (uint64_t j : batched) {
         const CallHandles h = a.handles_of(j);
@@ -2684,40 +2751,63 @@ frz_status batch_drive(const BatchCall& a) {
         gr.n_groups = n_groups.data();
         gr.counts = a.group_counts;
     }
-    const uint64_t qs_fit = n_groups_max ? std::min<uint64_t>(frz_batch_collapse_fit(kBatchScratchBytes, base, n_groups_max, list_rows),
-                                                              kFrzBatchMaxSub)
-                                         : qs_max;
-    const uint64_t qs = std::min<uint64_t>(qs_fit, batched.size());
-    const BatchLayout L(cs, k, cap, qs, n_groups_max, bc ? bc->n_cols : 0);
+    // every ordered query's attribute, boost and order (its direction is set per sub-batch)
+    std::vector<FrzOrderDev> ords;
+    for (uint64_t j : ordered) {
+        const CallHandles h = a.handles_of(j);
+        if (ords.empty()) ords.resize(q, FrzOrderDev());
+        FrzOrderDev& o = ords[j];
+        o.values = h.a->values.get();
+        o.n_values = h.a->values.cap();
+        o.boost = h.b ? h.b->values.get() : nullptr;
+        o.n_boost = h.b ? (uint32_t)h.b->values.cap() : 0;
+        o.order = h.order;
+    }
+    uint64_t qs_fit = n_groups_max ? std::min<uint64_t>(frz_batch_collapse_fit(kBatchScratchBytes, base, n_groups_max, list_rows),
+                                                        kFrzBatchMaxSub)
+                                   : qs_max;
+    if (!ordered.empty()) qs_fit = std::min<uint64_t>(qs_fit, frz_batch_order_fit(kBatchScratchBytes, base, n_groups_max, list_rows));
+    const uint64_t qs = std::min<uint64_t>(qs_fit, std::max(ordered.size(), unordered.size()));
+    const BatchLayout L(cs, k, cap, qs, n_groups_max, bc ? bc->n_cols : 0, !ordered.empty());
     FrzDevArray<uint8_t> scratch;   // released when the call returns
     FRZ_TRY(scratch.reserve(L.bytes));
     if (L.groups)   // the round tables start zero, and every sub-batch's rounds leave them zero
         FRZ_CUDA_TRY(cudaMemsetAsync(scratch.get() + L.off[BatchLayout::BEST], 0, L.off[BatchLayout::TAKEN] - L.off[BatchLayout::BEST]));
-    for (uint64_t s = 0; s < batched.size(); s += qs) {
-        const uint32_t ns = (uint32_t)std::min<uint64_t>(qs, batched.size() - s);
-        bool overflow = false;
-        FrzLaunchStats st;
-        FRZ_TRY(batch_run(ms, scopes.empty() ? nullptr : scopes.data(), gr, batched.data() + s, ns, corpus, k, L, scratch.get(), out,
-                          n_out, n_total, &overflow, st, bc));
-        g_batch_last[overflow ? 1 : 0] += ns;
-        g_batch_last[2]++;
-        g_batch_last[3] += st.launches;
-        if (overflow)   // the single-query pipeline retries with worst-case lists
-            for (uint32_t j = 0; j < ns; j++) FRZ_TRY(single(batched[s + j]));
+    if (L.groups && L.ordered)   // the ordered rounds' second table too
+        FRZ_CUDA_TRY(cudaMemsetAsync(scratch.get() + L.off[BatchLayout::BESTLO], 0, L.off[BatchLayout::END] - L.off[BatchLayout::BESTLO]));
+    for (const std::vector<uint64_t>* part : {&unordered, &ordered}) {
+        const FrzOrderDev* po = part == &ordered ? ords.data() : nullptr;
+        for (uint64_t s = 0; s < part->size(); s += qs) {
+            const uint32_t ns = (uint32_t)std::min<uint64_t>(qs, part->size() - s);
+            bool overflow = false;
+            FrzLaunchStats st;
+            FRZ_TRY(batch_run(ms, scopes.empty() ? nullptr : scopes.data(), gr, part->data() + s, ns, corpus, k, L, scratch.get(), out,
+                              n_out, n_total, &overflow, st, bc, po));
+            g_batch_last[overflow ? 1 : 0] += ns;
+            g_batch_last[2]++;
+            g_batch_last[3] += st.launches;
+            if (overflow)   // the single-query pipeline retries with worst-case lists
+                for (uint32_t j = 0; j < ns; j++) FRZ_TRY(single((*part)[s + j]));
+        }
     }
     return FRZ_OK;
 }
 
 }  // namespace
 
-extern "C" frz_status frz_match_list_batch_collapsed(frz_matcher* const* ms, uint64_t q, const frz_corpus* corpus,
-                                                     const frz_subset* const* subsets, const frz_boost* const* boosts,
-                                                     const frz_groups* const* groups, const uint64_t* per_group, uint64_t k,
-                                                     frz_match* out, uint64_t* n_out, uint64_t* n_total, uint32_t* const* group_counts) {
+// Query j is frz_match_list_ordered_collapsed(ms[j], corpus, subsets[j], boosts[j], attrs[j], orders[j], groups[j],
+// per_group[j], ...) with an attribute and groups, frz_match_list_ordered(...) with an attribute alone, and query j of
+// frz_match_list_batch_collapsed without one.  Its batched class orders its rows on the device (batch_run, order.cu).
+extern "C" frz_status frz_match_list_batch_ordered(frz_matcher* const* ms, uint64_t q, const frz_corpus* corpus,
+                                                   const frz_subset* const* subsets, const frz_boost* const* boosts,
+                                                   const frz_attr* const* attrs, const uint32_t* orders, const frz_groups* const* groups,
+                                                   const uint64_t* per_group, uint64_t k, frz_match* out, uint64_t* n_out,
+                                                   uint64_t* n_total, uint32_t* const* group_counts) {
     if (!ms || !corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
     for (uint64_t j = 0; j < q; j++)
         if (!ms[j]) return frz_fail(FRZ_ERR_INVALID_ARG, "null matcher at %llu", (unsigned long long)j);
-    return batch_drive(BatchCall{ms, q, corpus, nullptr, subsets, boosts, groups, per_group, k, out, n_out, n_total, group_counts});
+    return batch_drive(BatchCall{ms, q, corpus, nullptr, subsets, boosts, groups, per_group, k, out, n_out, n_total, group_counts, attrs,
+                                 orders});
 }
 
 // Query j is frz_match_list_columns(ms + j * n_cols, cols, n_cols, sort, subsets[j], boosts[j], groups[j], per_group[j], ...);

@@ -273,7 +273,8 @@ FRZ_API frz_status frz_match_list_top(frz_matcher* m, const frz_corpus* corpus, 
 FRZ_API frz_status frz_match_list_batch_top(frz_matcher* const* ms, uint64_t q, const frz_corpus* corpus, uint64_t k,
                                             frz_match* out, uint64_t* n_out, uint64_t* n_total);
 /* Test aid: the corpus-size and query-count limits of the batched path of frz_match_list_batch_top,
- * frz_match_list_batch, frz_match_list_batch_collapsed and frz_match_list_batch_columns, process-wide (0 restores
+ * frz_match_list_batch, frz_match_list_batch_collapsed, frz_match_list_batch_ordered and frz_match_list_batch_columns,
+ * process-wide (0 restores
  * a limit's default: 2^18 rows, 32 queries; max_typos = 0 queries batch up to the larger of max_rows and 2^21 rows;
  * fewer than 2 queries never batch).  For frz_match_list_batch_columns, max_rows limits every query, and a query with a
  * typo budget in some column batches only when max_rows is set (by default it runs frz_match_list_columns).  Lets tests reach the batched kernels with
@@ -281,7 +282,7 @@ FRZ_API frz_status frz_match_list_batch_top(frz_matcher* const* ms, uint64_t q, 
  * batch calls. */
 FRZ_API void frz_debug_batch_limits(uint64_t max_rows, uint64_t min_queries);
 /* Test aid: what the calling thread's last frz_match_list_batch_top, frz_match_list_batch,
- * frz_match_list_batch_collapsed or frz_match_list_batch_columns did: [0] queries answered by
+ * frz_match_list_batch_collapsed, frz_match_list_batch_ordered or frz_match_list_batch_columns did: [0] queries answered by
  * the batched kernels, [1] queries of sub-batches whose survivor lists overflowed (answered again by their single-query
  * call's pipeline),
  * [2] sub-batches run, [3] kernel launches of the batched path.  All zero after a call that ran no sub-batch. */
@@ -618,6 +619,36 @@ FRZ_API frz_status frz_match_list_batch_collapsed(frz_matcher* const* ms, uint64
                                                   const frz_subset* const* subsets, const frz_boost* const* boosts,
                                                   const frz_groups* const* groups, const uint64_t* per_group, uint64_t k,
                                                   frz_match* out, uint64_t* n_out, uint64_t* n_total, uint32_t* const* group_counts);
+
+/* frz_match_list_batch_collapsed (above) where each query may also order its rows by its own attribute, in one call: a
+ * shared shell-history server showing each user their distinct commands newest first, or a mail service listing each
+ * user's hits newest first.  For every j < q, out[j*k .. j*k + n_out[j]), n_out[j], n_total[j] and, when given,
+ * group_counts[j] are bit for bit what the matching single-query call returns:
+ *   attrs[j] and groups[j] != NULL: frz_match_list_ordered_collapsed(ms[j], corpus, subsets[j], boosts[j], attrs[j],
+ *                                   orders[j], groups[j], per_group[j], k, ..., group_counts[j]);
+ *   attrs[j] != NULL, no groups:    frz_match_list_ordered(ms[j], corpus, subsets[j], boosts[j], attrs[j], orders[j], k, ...);
+ *   else:                           query j of frz_match_list_batch_collapsed.
+ * attrs, subsets, boosts, groups and group_counts may be NULL, meaning every entry is NULL; orders may be NULL, meaning
+ * FRZ_ORDER_ATTR_DESC for every query; per_group may be NULL, meaning 1 for every query.  Rows out[j*k + n_out[j] ..
+ * (j+1)*k) are not written.  Never FRZ_ERR_CAPACITY.
+ *
+ * Checked in this order before any device work: FRZ_ERR_INVALID_ARG for a NULL ms or corpus, or a NULL ms[j]; every
+ * per_group[j] as frz_match_list_batch_collapsed checks it; FRZ_ERR_INVALID_ARG for an orders[j] above
+ * FRZ_ORDER_SCORE_THEN_ATTR_ASC (every entry is checked, with or without an attribute); a subset, boost, groups or
+ * attribute handle of another corpus (query by query, in that order within a query); a NULL n_out with q > 0; q*k
+ * overflowing uint64_t or size_t; a NULL out with q*k > 0.  q = 0 then returns FRZ_OK without any CUDA call.
+ *
+ * The batched class and its limits are frz_match_list_batch_collapsed's.  Ordered queries run in sub-batches of their own,
+ * whose last stage orders each query's rows by its order key on the device (DESIGN.md §4.11 "Ordered queries"); an ordered
+ * query whose keys and tables do not fit two to a sub-batch, and every query of a sub-batch whose survivor lists
+ * overflowed, runs its single-query call inside the same call.  frz_match_list_batch_collapsed is this call with
+ * attrs == NULL. */
+FRZ_API frz_status frz_match_list_batch_ordered(frz_matcher* const* ms, uint64_t q, const frz_corpus* corpus,
+                                                const frz_subset* const* subsets, const frz_boost* const* boosts,
+                                                const frz_attr* const* attrs, const uint32_t* orders,
+                                                const frz_groups* const* groups, const uint64_t* per_group, uint64_t k,
+                                                frz_match* out, uint64_t* n_out, uint64_t* n_total,
+                                                uint32_t* const* group_counts);
 
 /* frz_match_list_columns (above) for q queries over the same columns in one call: a service answering many users'
  * multi-field searches (file name + directory, command + working directory) over one set of columns.  Query j's matchers
