@@ -16,13 +16,14 @@ import numpy as np
 from .types import (CaseMatching, CConfig, CMatch, Config, CPattern, Match, Matching, Order, Pattern, Scoring,
                     SortStrategy, UnicodeMatching, as_pattern, pattern_array)
 
-__all__ = ["Matcher", "Corpus", "Subset", "Boost", "Groups", "GROUP_NONE", "Attr", "Where", "ATTR_NULL", "Pattern", "Config", "Scoring", "Match", "SortStrategy", "Order", "CaseMatching",
+__all__ = ["Matcher", "Corpus", "Subset", "Boost", "Groups", "GROUP_NONE", "Attr", "Where", "ATTR_NULL", "RankKey", "RANK_MAX_KEYS", "Pattern", "Config", "Scoring", "Match", "SortStrategy", "Order", "CaseMatching",
            "UnicodeMatching", "Matching", "FrizbeeError", "parse_query", "parse_atom", "radix_sort_matches",
            "MATCH_DTYPE", "lib", "lib_path"]
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 GROUP_NONE = 0xFFFFFFFF   # FRZ_GROUP_NONE: a row in no group
 ATTR_NULL = -(2**63)      # FRZ_ATTR_NULL: a row with no value for an attribute
+RANK_MAX_KEYS = 4         # FRZ_RANK_MAX_KEYS: keys of one Corpus.rank / Attr.rank
 _U64_MAX = 0xFFFFFFFFFFFFFFFF   # UINT64_MAX: no k limit / no per-group cap
 MATCH_DTYPE = np.dtype([("index", "<u4"), ("score", "<u2"), ("exact", "u1"), ("_pad", "u1")])
 
@@ -114,6 +115,8 @@ def lib():
     L.frz_attr_destroy.argtypes = [vp]
     L.frz_attr_destroy.restype = None
     L.frz_subset_where.argtypes = [vp, vp, u64, vp]
+    L.frz_attr_rank.argtypes = [vp, vp, u64]
+    L.frz_attr_get.argtypes = [vp, vp, u64]
     L.frz_boost_create.argtypes = [vp, vp, u64, C.POINTER(vp)]
     L.frz_boost_set.argtypes = [vp, vp, vp, u64]
     L.frz_boost_destroy.argtypes = [vp]
@@ -296,6 +299,17 @@ class Corpus:
         the device (frz_subset_where).  Close it before the corpus."""
         return self.subset([]).where(*clauses, base=base)
 
+    def text(self, desc: bool = False, fold_case: bool = False) -> "RankKey":
+        """The rows' haystacks as a key of Corpus.rank / Attr.rank: bytewise (memcmp) order, a proper prefix first; desc
+        reverses it, fold_case compares ASCII A-Z as a-z."""
+        return RankKey(text=self, desc=desc, fold_case=fold_case)
+
+    def rank(self, *keys: "RankKey") -> "Attr":
+        """A new attribute holding each row's dense rank in the lexicographic order of `keys` (at most RANK_MAX_KEYS, each
+        Attr.asc() / Attr.desc() or Corpus.text(...) of a corpus with as many rows), filled on the device
+        (frz_attr_rank).  Rows removed here or in a text key's corpus have no value.  Close it before the corpus."""
+        return self.attr().rank(*keys)
+
     def boost(self, values=None) -> "Boost":
         """A resident per-row boost for Matcher.match_list_ranked_array: values[i] (int16) is the boost of row i, rows
         past len(values) have 0; at most len(self) values.  Close it before the corpus."""
@@ -446,6 +460,43 @@ class Attr(_RowValues):
         """The clause "v is one of values" (any order, duplicates allowed; an empty list holds for no value)."""
         values = np.ascontiguousarray(values, dtype=np.int64)
         return Where(self, values=values) if values.size else Where(self, 0, -1)
+
+    def values(self) -> np.ndarray:
+        """The value of every row below len(corpus), ATTR_NULL where there is none (frz_attr_get)."""
+        out = np.empty(max(1, self.corpus.n), np.int64)
+        _check(lib().frz_attr_get(self._h, out.ctypes.data, self.corpus.n))
+        return out[: self.corpus.n]
+
+    def asc(self) -> "RankKey":
+        """This attribute as a key of Corpus.rank / Attr.rank, smaller values first (a row without a value last)."""
+        return RankKey(attr=self)
+
+    def desc(self) -> "RankKey":
+        """This attribute as a key of Corpus.rank / Attr.rank, larger values first (a row without a value last)."""
+        return RankKey(attr=self, desc=True)
+
+    def rank(self, *keys: "RankKey") -> "Attr":
+        """Refills this attribute with each row's dense rank in the lexicographic order of `keys` (Corpus.rank); it may
+        be one of the keys.  Returns self."""
+        arr = (_CRankKey * max(1, len(keys)))()
+        for j, k in enumerate(keys):
+            arr[j].attr = k.attr._h if k.attr is not None else None
+            arr[j].text = k.text._h if k.text is not None else None
+            arr[j].desc, arr[j].fold_case = int(k.desc), int(k.fold_case)
+        _check(lib().frz_attr_rank(self._h, arr if keys else None, len(keys)))
+        return self
+
+
+class _CRankKey(C.Structure):
+    _fields_ = [("attr", C.c_void_p), ("text", C.c_void_p), ("desc", C.c_uint32), ("fold_case", C.c_uint32)]
+
+
+class RankKey:
+    """One key of Corpus.rank / Attr.rank (frz_rank_key): an attribute (Attr.asc / Attr.desc) or the haystacks of a corpus
+    (Corpus.text)."""
+
+    def __init__(self, attr: Optional["Attr"] = None, text: Optional[Corpus] = None, desc: bool = False, fold_case: bool = False):
+        self.attr, self.text, self.desc, self.fold_case = attr, text, bool(desc), bool(fold_case)
 
 
 class Groups(_RowValues):

@@ -10,7 +10,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libfrz_cuda.so")
 SOURCES = ["pack.cu", "prefilter.cu", "sw.cu", "sort.cu", "unicode.cu", "host.cu", "merge.cu", "parallel.cu", "batch.cu", "collapse.cu",
-           "batch_columns.cu", "where.cu", "order.cu"]
+           "batch_columns.cu", "where.cu", "order.cu", "rank.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr"]
@@ -29,7 +29,7 @@ def _stale(target: str, deps) -> bool:
 def build(force: bool = False, verbose: bool = False, variant: str = "", defines=()) -> str:
     """variant/defines: an A/B build (`libfrz_cuda_<variant>.so`, own object directory) with extra -D flags; load it with
     FRZ_LIB=<path> (frizbee_b200.lib_path).  The default build is untouched."""
-    headers = [os.path.join(CSRC, h) for h in ("frz_device.cuh", "frz_host.h", "unicode_path.cuh", "unicode_needle.h", "unicode_case.inc", "indices_path.cuh", "sw_core.cuh", "sw_generic.cuh", "sw_wave.cuh", "prefilter_masks.cuh", "prefilter_scan.cuh", "merge_plan.cuh", "batch_plan.cuh", "collapse_plan.cuh", "batch_collapse_plan.cuh", "batch_columns_plan.cuh", "where_plan.cuh", "order_plan.cuh", "batch_order_plan.cuh")] + \
+    headers = [os.path.join(CSRC, h) for h in ("frz_device.cuh", "frz_host.h", "unicode_path.cuh", "unicode_needle.h", "unicode_case.inc", "indices_path.cuh", "sw_core.cuh", "sw_generic.cuh", "sw_wave.cuh", "prefilter_masks.cuh", "prefilter_scan.cuh", "merge_plan.cuh", "batch_plan.cuh", "collapse_plan.cuh", "batch_collapse_plan.cuh", "batch_columns_plan.cuh", "where_plan.cuh", "order_plan.cuh", "batch_order_plan.cuh", "rank_plan.cuh")] + \
               [os.path.join(HERE, "..", "include", "frz_cuda.h")]
     objdir = os.path.join(HERE, "build" + ("_" + variant if variant else ""))
     out = OUT if not variant else os.path.join(HERE, f"libfrz_cuda_{variant}.so")

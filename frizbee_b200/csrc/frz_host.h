@@ -509,6 +509,52 @@ frz_status frz_launch_sort_by_order_dev(const FrzMatchDev* d_in, FrzMatchDev* d_
                                         const FrzOrderDev& o, const uint32_t* shifts, uint32_t n_shifts, FrzSortScratch& ss,
                                         cudaStream_t stream, FrzLaunchStats* st, uint32_t limit = kFrzNoLimit);
 
+// The fill of frz_attr_rank (host.cu, DESIGN.md §4.17; the key rules are rank_plan.cuh's).  A segment is a run of rows
+// whose tuples agree so far, named by its first position in the final order.
+struct FrzRankKeyDev {
+    FrzCorpusView text;          // a text key: the corpus whose haystacks are the key
+    const int64_t* values;       // an attribute key: values[i] for i < n_values, null past them
+    uint64_t n_values;
+    uint32_t is_text;
+    uint32_t desc;
+    uint32_t fold;
+    uint32_t pad_;
+};
+struct FrzRankDev {
+    FrzRankKeyDev keys[4];       // FRZ_RANK_MAX_KEYS
+    uint32_t n_keys;
+    uint32_t any_text;
+    uint64_t n;                  // rows of C
+    const uint32_t* slot_meta;   // C's slots: the rows live in C
+    const uint16_t* slot_of;
+    uint32_t* seg_of;            // [n] the row's segment, kFrzRankNone: not ranked
+    uint32_t* at_row;            // [n] the place in the tuple (rank_plan.cuh) of the row's chunk this round
+    FrzOrderKey* keys_row;       // [n] the row's sort key this round (frz_rank_sort_key)
+    uint2* segs;                 // [n] by segment: one of its rows, and the place of its next chunk
+    uint32_t* skip;              // [n] by segment: the bytes its rows share from that place (text keys), kFrzRankNone: unknown
+    uint32_t* heads;             // [ceil(n / 32)] bit p: a finished segment starts at position p
+    unsigned long long* state;   // rows of the list of even rounds, of odd rounds, then the OR of the keys (hi, lo) and of
+                                 // their complements (hi, lo)
+};
+// rank.cu, all asynchronous on `stream`.  init: the ranked rows → list (their number → state[0], which must be zero),
+// seg_of, the first segment.  round: the rows' skips (text keys) and chunks, *n_ptr listed rows (<= n_cap); state[2 ..
+// 6) must be zero.  split: the sorted rows' new segments; the rows still to refine → next, their number → *n_next (zero).
+frz_status frz_launch_rank_init(const FrzRankDev& d, FrzMatchDev* list, cudaStream_t stream);
+frz_status frz_launch_rank_round(const FrzRankDev& d, const FrzMatchDev* list, const unsigned long long* n_ptr, uint64_t n_cap,
+                                 cudaStream_t stream);
+frz_status frz_launch_rank_split(const FrzRankDev& d, const FrzMatchDev* sorted, const unsigned long long* n_ptr, uint64_t n_cap,
+                                 FrzMatchDev* next, unsigned long long* n_next, cudaStream_t stream);
+// rank.cu: per 1024 positions of the m ranked rows, the heads before each bitmap word (word_pref) and their total
+// (chunk_count); then, with chunk_base the exclusive scan of chunk_count, value[i] for the n rows of C
+frz_status frz_launch_rank_heads(const uint32_t* heads, uint64_t m, uint32_t* word_pref, uint32_t* chunk_count, cudaStream_t stream);
+frz_status frz_launch_rank_write(const uint32_t* seg_of, uint64_t n, const uint32_t* heads, const uint32_t* word_pref,
+                                 const uint64_t* chunk_base, int64_t* values, cudaStream_t stream);
+// sort.cu: frz_launch_sort_by_order_dev for a round of frz_attr_rank: the *n_ptr rows at d_in (index = row) sorted by
+// descending keys[row], LSD over shifts[0 .. n_shifts) in reverse (n_shifts >= 1)
+frz_status frz_launch_sort_by_rank_dev(const FrzMatchDev* d_in, FrzMatchDev* d_tmp, FrzMatchDev* d_out, const unsigned long long* n_ptr,
+                                       const FrzOrderKey* keys, const uint32_t* shifts, uint32_t n_shifts, FrzSortScratch& ss,
+                                       cudaStream_t stream, FrzLaunchStats* st);
+
 // k-way merge of per-shard runs (merge.cu) with caller-owned scratch — one per concurrent user (parallel.cu: one per rank)
 #define FRZ_MERGE_MAX_RUNS 64
 struct FrzMergeScratch {

@@ -29,6 +29,7 @@
 #include "frz_host.h"
 #include "unicode_needle.h"
 #include "indices_path.cuh"
+#include "rank_plan.cuh"
 #include "where_plan.cuh"
 
 // ------------------------------------------------------------------------------------ errors
@@ -2131,8 +2132,24 @@ struct frz_boost : RowValues<int16_t, 0> {
 struct frz_groups : RowValues<uint32_t, FRZ_GROUP_NONE> {
     uint64_t n_groups = 0;
 };
+// frz_attr_rank's grow-only scratch (DESIGN.md §4.17), sized by the rows of the attribute's corpus
+struct FrzRankScratch {
+    FrzDevArray<uint32_t> seg_of, at_row, skip;
+    FrzDevArray<FrzOrderKey> keys;
+    FrzDevArray<uint2> segs;
+    FrzDevArray<FrzMatchDev> list[3];       // a round's rows, and the sort's two buffers
+    FrzDevArray<uint32_t> heads, word_pref;
+    FrzDevArray<uint32_t> chunk_count;
+    FrzDevArray<uint64_t> chunk_base;
+    FrzDevArray<unsigned long long> state;  // FrzRankDev::state
+    FrzDevArray<FrzCounters> counters;      // ->total: the head count k_scan_blocks leaves
+    FrzDevArray<int64_t> values;            // the new values, when the attribute's must grow
+    FrzSortScratch sort;
+};
 // A signed 64-bit value per index (frz_subset_where, ordered calls); null past the values.
-struct frz_attr : RowValues<int64_t, kFrzAttrNull> {};
+struct frz_attr : RowValues<int64_t, kFrzAttrNull> {
+    std::unique_ptr<FrzRankScratch> rank;   // created by the first frz_attr_rank
+};
 
 namespace {
 template <typename T>
@@ -2259,6 +2276,18 @@ extern "C" frz_status frz_attr_set(frz_attr* a, const uint32_t* which, const int
 
 extern "C" void frz_attr_destroy(frz_attr* a) { delete a; }
 
+extern "C" frz_status frz_attr_get(const frz_attr* a, int64_t* out, uint64_t n) {
+    if (!a || (n && !out)) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    if (n > a->corpus->st.n)
+        return frz_fail(FRZ_ERR_INVALID_ARG, "%llu values of a corpus of %llu haystacks", (unsigned long long)n, (unsigned long long)a->corpus->st.n);
+    const uint64_t held = std::min<uint64_t>(n, a->values.cap());
+    for (uint64_t i = held; i < n; i++) out[i] = FRZ_ATTR_NULL;
+    if (held == 0) return FRZ_OK;
+    FRZ_TRY(frz_ensure_device(a->corpus->st.device));
+    FRZ_CUDA_TRY(cudaMemcpy(out, a->values.get(), held * sizeof(int64_t), cudaMemcpyDeviceToHost));
+    return FRZ_OK;
+}
+
 // ---------------------------------------------------------------------------------- subsets from attributes
 namespace {
 // The device work of frz_subset_where once every argument has passed: k_where writes the bitmap and the chunk counts,
@@ -2337,6 +2366,121 @@ extern "C" frz_status frz_subset_where(frz_subset* s, const frz_where_clause* cl
     w.n_clauses = (uint32_t)n_clauses;
     FRZ_TRY(frz_ensure_device(s->corpus->st.device));
     return where_fill(s, w, sets, base);
+}
+
+// ---------------------------------------------------------------------------------- ranks from keys
+static_assert(kFrzRankMaxKeys == FRZ_RANK_MAX_KEYS && sizeof(FrzRankDev::keys) / sizeof(FrzRankKeyDev) == FRZ_RANK_MAX_KEYS,
+              "rank_plan.cuh mirrors frz_cuda.h");
+
+namespace {
+// The device work of frz_attr_rank once every argument has passed (DESIGN.md §4.17).  Every buffer is reserved first, so a
+// failed allocation leaves a's values as they were.  One read-back per round: the count of its rows and the masks of
+// their sort keys, which choose the sort's digits.  The values are written last, in place or into a grown array.
+frz_status rank_fill(frz_attr* a, FrzRankDev& d) {
+    const FrzCorpusStorage& cs = a->corpus->st;
+    const uint64_t n = cs.n;
+    if (!a->rank) a->rank = std::make_unique<FrzRankScratch>();
+    FrzRankScratch& r = *a->rank;
+    const uint64_t n_words = (n + 31) / 32, n_chunks = (n + 1023) / 1024;
+    if (n == 0) return FRZ_OK;
+    FRZ_TRY(r.seg_of.reserve(n));
+    FRZ_TRY(r.at_row.reserve(n));
+    FRZ_TRY(r.skip.reserve(n));
+    FRZ_TRY(r.keys.reserve(n));
+    FRZ_TRY(r.segs.reserve(n));
+    for (auto& l : r.list) FRZ_TRY(l.reserve(n));
+    FRZ_TRY(r.heads.reserve(n_words));
+    FRZ_TRY(r.word_pref.reserve(n_words));
+    FRZ_TRY(r.chunk_count.reserve(n_chunks));
+    FRZ_TRY(r.chunk_base.reserve(n_chunks));
+    FRZ_TRY(r.state.reserve(6));
+    FRZ_TRY(r.counters.reserve(1));
+    if (!r.sort.hist.get()) FRZ_TRY(frz_sort_hist_alloc(r.sort.hist));
+    const bool grow = a->values.cap() < n;
+    if (grow) FRZ_TRY(r.values.reserve(n));
+    d.n = n;
+    d.slot_meta = cs.slot_meta.get();
+    d.slot_of = cs.slot_of.get();
+    d.seg_of = r.seg_of.get();
+    d.at_row = r.at_row.get();
+    d.keys_row = r.keys.get();
+    d.segs = r.segs.get();
+    d.skip = r.skip.get();
+    d.heads = r.heads.get();
+    d.state = r.state.get();
+    cudaStream_t stream = nullptr;
+    FRZ_CUDA_TRY(cudaMemsetAsync(d.state, 0, 6 * sizeof(unsigned long long), stream));
+    FRZ_CUDA_TRY(cudaMemsetAsync(d.heads, 0, n_words * sizeof(uint32_t), stream));
+    FRZ_TRY(frz_launch_rank_init(d, r.list[0].get(), stream));
+    unsigned long long h[6];
+    FRZ_CUDA_TRY(cudaMemcpy(h, d.state, sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+    const uint64_t m = h[0];
+    uint32_t cur = 0;
+    for (uint32_t round = 0;; round++) {
+        unsigned long long* n_ptr = d.state + (round & 1);
+        unsigned long long* n_next = d.state + ((round + 1) & 1);
+        FRZ_CUDA_TRY(cudaMemsetAsync(d.state + 2, 0, 4 * sizeof(unsigned long long), stream));
+        FRZ_TRY(frz_launch_rank_round(d, r.list[cur].get(), n_ptr, m, stream));
+        FRZ_CUDA_TRY(cudaMemcpy(h, d.state, sizeof h, cudaMemcpyDeviceToHost));
+        if (h[round & 1] == 0) break;
+        uint32_t shifts[kFrzOrderMaxDigits];
+        const uint32_t n_shifts = frz_order_digits(h[2] & h[4], h[3] & h[5], shifts);
+        const uint32_t tmp = (cur + 1) % 3, out = (cur + 2) % 3;
+        if (n_shifts) FRZ_TRY(frz_launch_sort_by_rank_dev(r.list[cur].get(), r.list[tmp].get(), r.list[out].get(), n_ptr, d.keys_row, shifts,
+                                                          n_shifts, r.sort, stream, nullptr));
+        const uint32_t sorted = n_shifts ? out : cur, next = n_shifts ? cur : tmp;
+        FRZ_CUDA_TRY(cudaMemsetAsync(n_next, 0, sizeof(unsigned long long), stream));
+        FRZ_TRY(frz_launch_rank_split(d, r.list[sorted].get(), n_ptr, h[round & 1], r.list[next].get(), n_next, stream));
+        cur = next;
+    }
+    FRZ_TRY(frz_launch_rank_heads(d.heads, m, r.word_pref.get(), r.chunk_count.get(), stream));
+    if (m) {
+        k_scan_blocks<<<1, 1024, 0, stream>>>(r.chunk_count.get(), r.chunk_base.get(), (uint32_t)((m + 1023) / 1024), r.counters.get());
+        FRZ_CUDA_TRY(cudaGetLastError());
+    }
+    int64_t* values = grow ? r.values.get() : a->values.get();
+    FRZ_TRY(frz_launch_rank_write(d.seg_of, n, d.heads, r.word_pref.get(), r.chunk_base.get(), values, stream));
+    FRZ_CUDA_TRY(cudaStreamSynchronize(stream));
+    if (grow) std::swap(a->values, r.values);   // the old values become the next grow's scratch
+    return FRZ_OK;
+}
+}  // namespace
+
+extern "C" frz_status frz_attr_rank(frz_attr* a, const frz_rank_key* keys, uint64_t n_keys) {
+    if (!a || (n_keys && !keys)) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    if (n_keys == 0) return frz_fail(FRZ_ERR_INVALID_ARG, "n_keys = 0: a rank needs at least one key");
+    if (n_keys > FRZ_RANK_MAX_KEYS)
+        return frz_fail(FRZ_ERR_UNSUPPORTED, "%llu keys (at most %d)", (unsigned long long)n_keys, FRZ_RANK_MAX_KEYS);
+    for (uint64_t j = 0; j < n_keys; j++)
+        if (!keys[j].attr == !keys[j].text)
+            return frz_fail(FRZ_ERR_INVALID_ARG, "key %llu has %s of attr and text", (unsigned long long)j, keys[j].attr ? "both" : "neither");
+    for (uint64_t j = 0; j < n_keys; j++)
+        if (keys[j].attr && keys[j].fold_case) return frz_fail(FRZ_ERR_INVALID_ARG, "fold_case on attribute key %llu", (unsigned long long)j);
+    const FrzCorpusStorage& cs = a->corpus->st;
+    for (uint64_t j = 0; j < n_keys; j++) {
+        const FrzCorpusStorage& ks = keys[j].attr ? keys[j].attr->corpus->st : keys[j].text->st;
+        if (ks.device != cs.device)
+            return frz_fail(FRZ_ERR_INVALID_ARG, "key %llu is on device %d, the attribute on device %d", (unsigned long long)j, ks.device, cs.device);
+        if (ks.n != cs.n)
+            return frz_fail(FRZ_ERR_INVALID_ARG, "key %llu holds %llu rows, the attribute's corpus %llu: the keys must share its index space",
+                            (unsigned long long)j, (unsigned long long)ks.n, (unsigned long long)cs.n);
+    }
+    FrzRankDev d = {};
+    d.n_keys = (uint32_t)n_keys;
+    for (uint64_t j = 0; j < n_keys; j++) {
+        FrzRankKeyDev& k = d.keys[j];
+        k.is_text = keys[j].text != nullptr;
+        k.desc = keys[j].desc != 0;
+        k.fold = keys[j].fold_case != 0;
+        if (k.is_text) k.text = keys[j].text->st.view();
+        else {
+            k.values = keys[j].attr->values.get();
+            k.n_values = keys[j].attr->values.cap();
+        }
+        d.any_text |= k.is_text;
+    }
+    FRZ_TRY(frz_ensure_device(cs.device));
+    return rank_fill(a, d);
 }
 
 // ---------------------------------------------------------------------------------- single-query list calls

@@ -358,6 +358,13 @@ struct OrderKey {
     }
 };
 
+// The digit source of a round of frz_attr_rank (DESIGN.md §4.17): digit `shift` of the row's sort key (rank_plan.cuh)
+struct RankKey {
+    const FrzOrderKey* keys;
+    uint32_t shift;
+    __device__ __forceinline__ uint32_t operator()(const FrzMatchDev& m) const { return frz_order_digit(keys[m.index], shift); }
+};
+
 }  // namespace
 
 frz_status frz_launch_sort_by_score_dev(const FrzMatchDev* d_in, FrzMatchDev* d_tmp, FrzMatchDev* d_out,
@@ -381,6 +388,19 @@ frz_status frz_launch_sort_by_order_dev(const FrzMatchDev* d_in, FrzMatchDev* d_
         FrzMatchDev* dst = (n_shifts - 1 - i) % 2 == 0 ? d_out : d_tmp;
         FRZ_TRY(sort_pass(src, dst, n_ptr, 0, (int)kFrzOrderBins, i + 1 == n_shifts ? limit : kFrzNoLimit,
                           OrderKey{o, shifts[n_shifts - 1 - i]}, ss, stream, st));
+        src = dst;
+    }
+    return FRZ_OK;
+}
+
+frz_status frz_launch_sort_by_rank_dev(const FrzMatchDev* d_in, FrzMatchDev* d_tmp, FrzMatchDev* d_out, const unsigned long long* n_ptr,
+                                       const FrzOrderKey* keys, const uint32_t* shifts, uint32_t n_shifts, FrzSortScratch& ss,
+                                       cudaStream_t stream, FrzLaunchStats* st) {
+    if (n_shifts == 0) return frz_fail(FRZ_ERR_INVALID_ARG, "a rank sort needs a digit");
+    const FrzMatchDev* src = d_in;
+    for (uint32_t i = 0; i < n_shifts; i++) {   // least significant digit first; the last pass lands in d_out
+        FrzMatchDev* dst = (n_shifts - 1 - i) % 2 == 0 ? d_out : d_tmp;
+        FRZ_TRY(sort_pass(src, dst, n_ptr, 0, (int)kFrzOrderBins, kFrzNoLimit, RankKey{keys, shifts[n_shifts - 1 - i]}, ss, stream, st));
         src = dst;
     }
     return FRZ_OK;

@@ -353,6 +353,9 @@ FRZ_API frz_status frz_attr_create(const frz_corpus* c, const int64_t* values, u
  * frz_subset_where reading a. */
 FRZ_API frz_status frz_attr_set(frz_attr* a, const uint32_t* which, const int64_t* values, uint64_t n);
 FRZ_API void frz_attr_destroy(frz_attr* a);
+/* The reference has no such method (see above).  out[i] = value[i] for i < n (FRZ_ATTR_NULL where there is none), e.g.
+ * the ranks frz_attr_rank wrote.  n > frz_corpus_len(c), or NULL out with n > 0, is FRZ_ERR_INVALID_ARG.  Synchronous. */
+FRZ_API frz_status frz_attr_get(const frz_attr* a, int64_t* out, uint64_t n);
 
 /* One clause of frz_subset_where over v, an index's value in `attr`. */
 typedef struct frz_where_clause {
@@ -377,6 +380,34 @@ typedef struct frz_where_clause {
  * to FRZ_ATTR_NULL (FRZ_ERR_INVALID_ARG); an attribute or base of another corpus (FRZ_ERR_INVALID_ARG).  A failure after
  * the checks (out of device memory, for example) leaves s as the empty set, never half-written. */
 FRZ_API frz_status frz_subset_where(frz_subset* s, const frz_where_clause* clauses, uint64_t n_clauses, const frz_subset* base);
+
+/* Ranks from several keys.  An order by name, or by a key and then a name, needs a key the caller does not hold: the
+ * dense rank of each row's text.  frz_attr_rank fills an attribute on the device with each row's place in a lexicographic
+ * order of up to FRZ_RANK_MAX_KEYS keys, each an attribute or the text of a corpus, so that every call that takes an
+ * attribute (the ordered calls, frz_subset_where) orders or filters by it unchanged. */
+#define FRZ_RANK_MAX_KEYS 4
+typedef struct frz_rank_key {
+    const frz_attr* attr;      /* an attribute key, or NULL */
+    const frz_corpus* text;    /* a text key: the haystacks of this corpus, or NULL; exactly one of attr / text */
+    uint32_t desc;             /* nonzero: larger values / later texts first */
+    uint32_t fold_case;        /* text keys only: ASCII A-Z compare as a-z */
+} frz_rank_key;
+/* The reference has no such method (see above).  Let C be a's corpus.  Row i < frz_corpus_len(C) is ranked when it is live
+ * in C and in the corpus of every text key (a removed row has no text).  Afterwards value[i] of a ranked row is the number
+ * of distinct key tuples of ranked rows that come strictly before its own (a dense rank from 0: equal tuples share a
+ * rank), and FRZ_ATTR_NULL for every other row.  Tuples compare key by key: an attribute key by value, reversed by desc,
+ * a null value after every value in both directions; a text key by its bytes as unsigned bytes, a proper prefix first
+ * (memcmp order: code point order for UTF-8), A-Z as a-z under fold_case, reversed by desc.  The values are a snapshot:
+ * rows appended later are null until the next call, and edits of a key do not update them.  a may be one of the keys.
+ * Synchronous; it must not run concurrently with a call that reads a or a key.
+ *
+ * Checked in this order before any device work, leaving a as it was: a NULL a, or NULL keys with n_keys > 0
+ * (FRZ_ERR_INVALID_ARG); n_keys == 0 (FRZ_ERR_INVALID_ARG); more than FRZ_RANK_MAX_KEYS keys (FRZ_ERR_UNSUPPORTED); a key
+ * with both or neither of attr and text (FRZ_ERR_INVALID_ARG); fold_case on an attribute key (FRZ_ERR_INVALID_ARG); a key
+ * whose corpus is on another device or holds another number of rows than C (FRZ_ERR_INVALID_ARG).  A failure after the
+ * checks (out of device memory, for example) leaves a's values as they were.  Scratch stays on a and only grows, so a
+ * refill at the same size allocates nothing. */
+FRZ_API frz_status frz_attr_rank(frz_attr* a, const frz_rank_key* keys, uint64_t n_keys);
 
 /* ---------------------------------------------------------------- ranked calls
  *
