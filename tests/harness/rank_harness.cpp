@@ -22,6 +22,15 @@ extern "C" uint64_t h_rank_attr_chunk(int64_t v, uint32_t desc) { return frz_ran
 extern "C" uint32_t h_rank_chunk_ends(uint64_t chunk, uint32_t text, uint32_t desc) { return frz_rank_chunk_ends(chunk, text != 0, desc != 0); }
 extern "C" uint32_t h_rank_fold4(uint32_t x) { return frz_rank_fold4(x); }
 
+// the sort key of a round as (hi, lo), and the digit shifts the LSD sort visits for the masks of a round's keys
+extern "C" void h_rank_sort_key(uint32_t seg, uint64_t chunk, uint64_t* hi_lo) {
+    const FrzOrderKey k = frz_rank_sort_key(seg, chunk);
+    hi_lo[0] = k.hi;
+    hi_lo[1] = k.lo;
+}
+extern "C" uint32_t h_rank_key_seg(uint64_t hi, uint64_t lo) { return frz_rank_key_seg(FrzOrderKey{hi, lo}); }
+extern "C" uint32_t h_order_digits(uint64_t vary_hi, uint64_t vary_lo, uint32_t* shifts) { return frz_order_digits(vary_hi, vary_lo, shifts); }
+
 // a and b: the texts padded with zeros to whole 16-byte units
 extern "C" uint32_t h_rank_common(const uint8_t* a, uint32_t len_a, const uint8_t* b, uint32_t len_b, uint32_t off, uint32_t fold) {
     const auto unit = [&](int t, uint32_t u, uint32_t* w) { memcpy(w, (t ? b : a) + 16 * u, 16); };

@@ -302,3 +302,59 @@ def test_argument_checks_in_order_and_no_device():
                                                                     (None, corp["c1"], 1, 0), (a["c0"], None, 0, 0)), 4)):
         assert fn(a["c0"], ks, nk) == NO_DEVICE
     assert [b.raw for b in (c0, c1, longer, elsewhere)] + [h.raw for h in handle.values()] == before
+
+
+# ------------------------------------------------------------------------------------------------ the digits of a round
+def _digits(H, keys):
+    """The digit shifts the LSD sort visits for a round's sort keys, from their OR and the OR of their complements as
+    k_rank_chunk accumulates them (the low key word holds 48 bits) and rank_fill combines them."""
+    m48 = (1 << 48) - 1
+    or_hi = or_lo = nor_hi = nor_lo = 0
+    for hi, lo in keys:
+        or_hi, or_lo = or_hi | hi, or_lo | lo
+        nor_hi, nor_lo = nor_hi | (~hi & (2**64 - 1)), nor_lo | (~lo & m48)
+    shifts = np.zeros(14, np.uint32)
+    n = H.h_order_digits(or_hi & nor_hi, or_lo & nor_lo, shifts.ctypes.data)
+    return [int(s) for s in shifts[:n]]
+
+
+@pytest.mark.parametrize("seg_hi", [2**8 - 1, 2**16 - 1, 2**24, 2**32 - 2], ids=["seg8", "seg16", "seg24", "seg32"])
+def test_round_digits_are_the_varying_segment_and_chunk_bytes(H, seg_hi):
+    """Sort keys of rows whose segment ids span [0, seg_hi] and whose chunks vary in chosen bytes: the sort visits exactly
+    the segment bytes (key bits 64-95) and chunk bytes (key bits 0-63) in which the keys differ, most significant first,
+    and never the top 16 bits; the descending key order is the ascending (segment, chunk) order; the segment comes back."""
+    rng = np.random.default_rng(seg_hi % 1000)
+    H.h_rank_sort_key.argtypes = [u32, u64, vp]
+    H.h_rank_key_seg.argtypes = [u64, u64]
+    H.h_rank_key_seg.restype = u32
+    H.h_order_digits.argtypes = [u64, u64, vp]
+    H.h_order_digits.restype = u32
+    out = np.zeros(2, np.uint64)
+    for chunk_bytes in ([], [0], [7], [0, 3, 6], list(range(8))):
+        segs = [0, seg_hi] + [int(x) for x in rng.integers(0, seg_hi + 1, 200, dtype=np.uint64)]
+        base = int(rng.integers(0, 2**64, dtype=np.uint64))
+        chunks = []
+        for _ in segs:
+            c = base
+            for b in chunk_bytes:
+                c = (c & ~(0xFF << 8 * b)) | int(rng.integers(0, 256)) << 8 * b
+            chunks.append(c)
+        if chunk_bytes:   # the first row keeps the base chunk, the second differs in every chosen byte
+            chunks[0] = base
+            chunks[1] = base ^ sum(0x5A << 8 * b for b in chunk_bytes)
+        keys = []
+        for s, c in zip(segs, chunks):
+            H.h_rank_sort_key(s, c, out.ctypes.data)
+            hi, lo = int(out[0]), int(out[1])
+            assert hi >> 48 == 0 and lo >> 48 == 0
+            assert H.h_rank_key_seg(hi, lo) == s
+            keys.append((hi, lo))
+        want = [64 + 8 * b for b in range(3, -1, -1) if len({s >> 8 * b & 0xFF for s in segs}) > 1]
+        want += [8 * b for b in range(7, -1, -1) if len({c >> 8 * b & 0xFF for c in chunks}) > 1]
+        assert _digits(H, keys) == want, (seg_hi, chunk_bytes)
+        assert want[0] == {2**8 - 1: 64, 2**16 - 1: 72, 2**24: 88, 2**32 - 2: 88}[seg_hi]
+        # the key, read as one 112-bit number, descends as (segment, chunk) ascends
+        as_int = [hi << 48 | lo for hi, lo in keys]
+        by_key = sorted(range(len(segs)), key=lambda i: -as_int[i])
+        by_tuple = sorted(range(len(segs)), key=lambda i: (segs[i], chunks[i]))
+        assert [(segs[i], chunks[i]) for i in by_key] == [(segs[i], chunks[i]) for i in by_tuple]
