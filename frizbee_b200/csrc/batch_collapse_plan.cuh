@@ -12,11 +12,7 @@
 
 #include "collapse_plan.cuh"
 
-#if defined(__CUDACC__)
-#define FRZ_BC_HD __host__ __device__ __forceinline__
-#else
-#define FRZ_BC_HD inline
-#endif
+#include "frz_hd.cuh"
 
 // The groups of one query of a sub-batch, uploaded with its pattern (ids == nullptr: the query has no groups).
 struct FrzBatchCollapse {
@@ -29,29 +25,29 @@ struct FrzBatchCollapse {
 };
 
 // The rounds a query takes part in: per_group when capped, none without a cap (every count fits).
-FRZ_BC_HD uint32_t frz_batch_collapse_rounds(uint64_t per_group) {
+FRZ_HD uint32_t frz_batch_collapse_rounds(uint64_t per_group) {
     return per_group <= kFrzCollapseMaxPerGroup ? (uint32_t)per_group : 0u;
 }
-FRZ_BC_HD bool frz_batch_collapse_in_round(uint32_t per_group, uint32_t round) { return round < frz_batch_collapse_rounds(per_group); }
+FRZ_HD bool frz_batch_collapse_in_round(uint32_t per_group, uint32_t round) { return round < frz_batch_collapse_rounds(per_group); }
 
 // The first table entry of slot `slot` when every slot holds n_groups_max entries.
-FRZ_BC_HD uint64_t frz_batch_collapse_table(uint32_t slot, uint64_t n_groups_max) { return (uint64_t)slot * n_groups_max; }
+FRZ_HD uint64_t frz_batch_collapse_table(uint32_t slot, uint64_t n_groups_max) { return (uint64_t)slot * n_groups_max; }
 
 // Device bytes a query slot adds to a sub-batch for tables of n_groups_max entries over lists of list_rows rows: a u32 count
 // and a u64 round entry per group, a taken flag per row, and its record.  0 when no query of the call has groups.
-FRZ_BC_HD uint64_t frz_batch_collapse_bytes(uint64_t n_groups_max, uint64_t list_rows) {
+FRZ_HD uint64_t frz_batch_collapse_bytes(uint64_t n_groups_max, uint64_t list_rows) {
     return n_groups_max ? n_groups_max * (sizeof(uint32_t) + sizeof(unsigned long long)) + list_rows + sizeof(FrzBatchCollapse) : 0;
 }
 // Queries per sub-batch within `budget` bytes, when a query needs base bytes without its groups (0: fewer than two fit, and
 // the grouped queries run the single-query call).
-FRZ_BC_HD uint64_t frz_batch_collapse_fit(uint64_t budget, uint64_t base, uint64_t n_groups_max, uint64_t list_rows) {
+FRZ_HD uint64_t frz_batch_collapse_fit(uint64_t budget, uint64_t base, uint64_t n_groups_max, uint64_t list_rows) {
     const uint64_t q = budget / (base + frz_batch_collapse_bytes(n_groups_max, list_rows));
     return q >= 2 ? q : 0;
 }
 
 // Slots of a sub-batch's ns queries: slot[j] for a grouped query, those with wants[j] first, both in query order; the
 // slot of a query without groups is unused.  Returns the number of slots whose counts are read back.
-FRZ_BC_HD uint32_t frz_batch_collapse_slots(const uint8_t* grouped, const uint8_t* wants, uint32_t ns, uint32_t* slot) {
+FRZ_HD uint32_t frz_batch_collapse_slots(const uint8_t* grouped, const uint8_t* wants, uint32_t ns, uint32_t* slot) {
     uint32_t next = 0;
     for (uint32_t j = 0; j < ns; j++)
         if (grouped[j] && wants[j]) slot[j] = next++;

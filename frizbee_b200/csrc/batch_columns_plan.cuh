@@ -16,11 +16,7 @@
 #pragma once
 #include <stdint.h>
 
-#if defined(__CUDACC__)
-#define FRZ_BK_HD __host__ __device__ __forceinline__
-#else
-#define FRZ_BK_HD inline
-#endif
+#include "frz_hd.cuh"
 
 // Most columns a batched query folds (the matched count is 8 bits); a call with more columns runs the single-query call.
 constexpr uint32_t kFrzBatchMaxColumns = 255;
@@ -34,21 +30,21 @@ struct FrzColumnFold {
 };
 
 // The accumulator of a row after fold `pass` with a record of the column (score, exact).
-FRZ_BK_HD uint32_t frz_columns_fold(uint32_t acc, uint32_t pass, uint32_t score, uint32_t exact) {
+FRZ_HD uint32_t frz_columns_fold(uint32_t acc, uint32_t pass, uint32_t score, uint32_t exact) {
     if ((acc >> 24) != pass) return acc;   // it missed an earlier column
     const uint32_t s = (acc & 0xFFFFu) + score;
     return (pass + 1) << 24 | (acc & 0x10000u) | (exact ? 0x10000u : 0u) | (s > 0xFFFFu ? 0xFFFFu : s);
 }
 // A match of a query that folds `need` columns.
-FRZ_BK_HD bool frz_columns_matched(uint32_t acc, uint32_t need) { return (acc >> 24) == need; }
-FRZ_BK_HD uint32_t frz_columns_score(uint32_t acc) { return acc & 0xFFFFu; }
-FRZ_BK_HD uint32_t frz_columns_exact(uint32_t acc) { return (acc >> 16) & 1u; }
+FRZ_HD bool frz_columns_matched(uint32_t acc, uint32_t need) { return (acc >> 24) == need; }
+FRZ_HD uint32_t frz_columns_score(uint32_t acc) { return acc & 0xFFFFu; }
+FRZ_HD uint32_t frz_columns_exact(uint32_t acc) { return (acc >> 16) & 1u; }
 
 // Position of the p-th match (index order) of a list of `total` matches, reversed under the *_DESC strategies.
-FRZ_BK_HD uint64_t frz_columns_pos(uint64_t p, uint64_t total, bool reversed) { return reversed ? total - 1 - p : p; }
+FRZ_HD uint64_t frz_columns_pos(uint64_t p, uint64_t total, bool reversed) { return reversed ? total - 1 - p : p; }
 
 // Device bytes a query adds to a sub-batch for n_cols columns over lists of list_rows rows: its accumulator, its error
 // word, the patterns of its further columns (pattern_bytes each), its fold records and its column count.
-FRZ_BK_HD uint64_t frz_batch_columns_bytes(uint64_t n_cols, uint64_t list_rows, uint64_t pattern_bytes) {
+FRZ_HD uint64_t frz_batch_columns_bytes(uint64_t n_cols, uint64_t list_rows, uint64_t pattern_bytes) {
     return list_rows * sizeof(uint32_t) + sizeof(uint32_t) + (n_cols - 1) * pattern_bytes + n_cols * sizeof(FrzColumnFold) + 1;
 }

@@ -22,41 +22,37 @@
 #include "batch_collapse_plan.cuh"
 #include "order_plan.cuh"
 
-#if defined(__CUDACC__)
-#define FRZ_BO_HD __host__ __device__ __forceinline__
-#else
-#define FRZ_BO_HD inline
-#endif
+#include "frz_hd.cuh"
 
 // Launches of the select: one per digit a key can have, and the last one that ends every query's selection.
 constexpr uint32_t kFrzBatchOrderPasses = kFrzOrderMaxDigits + 1;
 
 // Slot offsets, in elements of each array
-FRZ_BO_HD uint64_t frz_batch_order_keys_at(uint32_t j, uint64_t list_stride) { return (uint64_t)j * list_stride; }
-FRZ_BO_HD uint64_t frz_batch_order_cand_at(uint32_t j, uint64_t list_stride) { return (uint64_t)j * 2 * list_stride; }
-FRZ_BO_HD uint64_t frz_batch_order_sel_at(uint32_t j) { return (uint64_t)j * kFrzOrderBlockRows; }
-FRZ_BO_HD uint64_t frz_batch_order_hist_at(uint32_t j) { return (uint64_t)j * kFrzOrderBins; }
+FRZ_HD uint64_t frz_batch_order_keys_at(uint32_t j, uint64_t list_stride) { return (uint64_t)j * list_stride; }
+FRZ_HD uint64_t frz_batch_order_cand_at(uint32_t j, uint64_t list_stride) { return (uint64_t)j * 2 * list_stride; }
+FRZ_HD uint64_t frz_batch_order_sel_at(uint32_t j) { return (uint64_t)j * kFrzOrderBlockRows; }
+FRZ_HD uint64_t frz_batch_order_hist_at(uint32_t j) { return (uint64_t)j * kFrzOrderBins; }
 
 // Device bytes an ordered query slot adds to a sub-batch over lists of list_rows rows: its FrzOrderDev record, its keys,
 // its two candidate lists, the selection, the state, the histogram, and with grouped queries (n_groups_max > 0) a best_lo
 // table.
-FRZ_BO_HD uint64_t frz_batch_order_bytes(uint64_t n_groups_max, uint64_t list_rows) {
+FRZ_HD uint64_t frz_batch_order_bytes(uint64_t n_groups_max, uint64_t list_rows) {
     return sizeof(FrzOrderDev) + list_rows * (sizeof(FrzOrderKey) + 2 * sizeof(uint32_t)) + kFrzOrderBlockRows * sizeof(uint32_t) +
            sizeof(FrzOrderState) + kFrzOrderBins * sizeof(uint32_t) + n_groups_max * sizeof(unsigned long long);
 }
 // Queries per ordered sub-batch within `budget` bytes, when a query needs base bytes without its groups and ordering (0:
 // fewer than two fit, and the ordered queries run the single-query call).
-FRZ_BO_HD uint64_t frz_batch_order_fit(uint64_t budget, uint64_t base, uint64_t n_groups_max, uint64_t list_rows) {
+FRZ_HD uint64_t frz_batch_order_fit(uint64_t budget, uint64_t base, uint64_t n_groups_max, uint64_t list_rows) {
     const uint64_t q = budget / (base + frz_batch_collapse_bytes(n_groups_max, list_rows) + frz_batch_order_bytes(n_groups_max, list_rows));
     return q >= 2 ? q : 0;
 }
 
 // The varying bits of a query's rows: set in some key and clear in another (the state's OR masks).
-FRZ_BO_HD FrzOrderKey frz_batch_order_vary(const FrzOrderState& s) { return FrzOrderKey{s.vary_hi & s.flip_hi, s.vary_lo & s.flip_lo}; }
+FRZ_HD FrzOrderKey frz_batch_order_vary(const FrzOrderState& s) { return FrzOrderKey{s.vary_hi & s.flip_hi, s.vary_lo & s.flip_lo}; }
 
 // The p-th varying digit of `vary`, most significant first: true and its shift in *shift when the query has more than p
 // varying digits (frz_order_digits' p-th entry), false otherwise.
-FRZ_BO_HD bool frz_batch_order_shift(const FrzOrderKey& vary, uint32_t p, uint32_t* shift) {
+FRZ_HD bool frz_batch_order_shift(const FrzOrderKey& vary, uint32_t p, uint32_t* shift) {
     uint32_t n = 0;
     for (int32_t s = (int32_t)(kFrzOrderKeyBits - kFrzOrderDigitBits); s >= 0; s -= (int32_t)kFrzOrderDigitBits) {
         if (!frz_order_digit(vary, (uint32_t)s)) continue;
@@ -71,8 +67,8 @@ FRZ_BO_HD bool frz_batch_order_shift(const FrzOrderKey& vary, uint32_t p, uint32
 // The member rule: list row `index` is one of the query's rows when it is a member of its subset (bits == nullptr: no
 // subset) and, for a grouped query (ids != nullptr), kept by its collapse (counts: its count table, taken: the row's flag).
 // Non-members never enter the select: no key value can stand for "not a row", since an all-zero key is a legitimate row.
-FRZ_BO_HD bool frz_batch_order_member(const uint32_t* bits, uint64_t n_bits, const uint32_t* ids, uint64_t n_ids, const uint32_t* counts,
-                                      uint32_t per_group, bool taken, uint32_t index) {
+FRZ_HD bool frz_batch_order_member(const uint32_t* bits, uint64_t n_bits, const uint32_t* ids, uint64_t n_ids, const uint32_t* counts,
+                                   uint32_t per_group, bool taken, uint32_t index) {
     if (bits && !frz_batch_member(bits, n_bits, index)) return false;
     if (!ids) return true;
     const uint32_t g = frz_collapse_group(ids, n_ids, index);
@@ -80,4 +76,4 @@ FRZ_BO_HD bool frz_batch_order_member(const uint32_t* bits, uint64_t n_bits, con
 }
 
 // The rows the block sort reads: every row of the query when they fit it (the select is skipped), else the selection.
-FRZ_BO_HD bool frz_batch_order_whole(uint64_t n_rows) { return n_rows <= kFrzOrderBlockRows; }
+FRZ_HD bool frz_batch_order_whole(uint64_t n_rows) { return n_rows <= kFrzOrderBlockRows; }

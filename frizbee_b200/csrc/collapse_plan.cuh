@@ -17,11 +17,7 @@
 #include "batch_plan.cuh"
 #include "order_plan.cuh"
 
-#if defined(__CUDACC__)
-#define FRZ_CP_HD __host__ __device__ __forceinline__
-#else
-#define FRZ_CP_HD inline
-#endif
+#include "frz_hd.cuh"
 
 constexpr uint32_t kFrzGroupNone = 0xFFFFFFFFu;            // FRZ_GROUP_NONE
 constexpr uint64_t kFrzCollapseMaxPerGroup = 32;           // per_group above this (other than "no cap") is unsupported
@@ -34,29 +30,29 @@ enum FrzCollapseOrder : uint8_t {
 };
 
 // The group of a corpus index: ids[index] for index < n_ids, none past the array (rows appended after the handle).
-FRZ_CP_HD uint32_t frz_collapse_group(const uint32_t* ids, uint64_t n_ids, uint32_t index) {
+FRZ_HD uint32_t frz_collapse_group(const uint32_t* ids, uint64_t n_ids, uint32_t index) {
     return index < n_ids ? ids[index] : kFrzGroupNone;
 }
 
 // The order key of a row; boost is boost[index] (0 past the boost array), read only by FRZ_COLLAPSE_BY_KEY.
-FRZ_CP_HD uint64_t frz_collapse_key(uint8_t order, bool reversed, uint32_t score, int32_t boost, uint32_t index) {
+FRZ_HD uint64_t frz_collapse_key(uint8_t order, bool reversed, uint32_t score, int32_t boost, uint32_t index) {
     const uint32_t primary = order == FRZ_COLLAPSE_BY_KEY ? frz_batch_ranked_value(score, boost)
                            : order == FRZ_COLLAPSE_BY_SCORE ? score : 0u;
     return (uint64_t)primary << 32 | (reversed ? index : ~index);
 }
 
 // A row of an over-full group not yet taken: it takes part in the next round.
-FRZ_CP_HD bool frz_collapse_contends(uint32_t group, uint32_t count, uint32_t per_group, bool taken) {
+FRZ_HD bool frz_collapse_contends(uint32_t group, uint32_t count, uint32_t per_group, bool taken) {
     return group != kFrzGroupNone && count > per_group && !taken;
 }
 
 // The table entry a round's max is taken over: 0 is an empty entry, so a row's entry is its key + 1 (keys are below 2^48).
 // The round's winner is the contender whose entry equals the max; it resets the entry to 0 for the next round, and a
 // contender that reads the reset value cannot mistake itself for the winner.
-FRZ_CP_HD uint64_t frz_collapse_entry(uint64_t key) { return key + 1; }
+FRZ_HD uint64_t frz_collapse_entry(uint64_t key) { return key + 1; }
 
 // The row is in C: no group, a group of at most per_group rows, or taken in a round.
-FRZ_CP_HD bool frz_collapse_keep(uint32_t group, uint32_t count, uint32_t per_group, bool taken) {
+FRZ_HD bool frz_collapse_keep(uint32_t group, uint32_t count, uint32_t per_group, bool taken) {
     return group == kFrzGroupNone || count <= per_group || taken;
 }
 
@@ -76,6 +72,6 @@ FRZ_CP_HD bool frz_collapse_keep(uint32_t group, uint32_t count, uint32_t per_gr
 //     per_group - r >= 1 contenders, so each max is over a non-empty set; a group whose contenders all have hi = 0 (null
 //     attribute values under ATTR_*) keeps best_hi = 0, which step 2 matches.
 //   - Every over-full group has one winner per round, which resets its entries, so both tables are zero after the rounds.
-FRZ_CP_HD uint64_t frz_collapse_hi_entry(const FrzOrderKey& k) { return k.hi; }
-FRZ_CP_HD uint64_t frz_collapse_lo_entry(const FrzOrderKey& k, uint64_t best_hi) { return k.hi == best_hi ? k.lo + 1 : 0; }
-FRZ_CP_HD bool frz_collapse_key_takes(const FrzOrderKey& k, uint64_t best_lo) { return k.lo + 1 == best_lo; }
+FRZ_HD uint64_t frz_collapse_hi_entry(const FrzOrderKey& k) { return k.hi; }
+FRZ_HD uint64_t frz_collapse_lo_entry(const FrzOrderKey& k, uint64_t best_hi) { return k.hi == best_hi ? k.lo + 1 : 0; }
+FRZ_HD bool frz_collapse_key_takes(const FrzOrderKey& k, uint64_t best_lo) { return k.lo + 1 == best_lo; }

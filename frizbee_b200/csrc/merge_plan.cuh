@@ -12,11 +12,7 @@
 #include <stddef.h>
 #include <stdint.h>
 
-#if defined(__CUDACC__)
-#define FRZ_HD __host__ __device__ __forceinline__
-#else
-#define FRZ_HD inline
-#endif
+#include "frz_hd.cuh"
 
 namespace frzmerge {
 

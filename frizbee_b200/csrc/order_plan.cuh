@@ -21,11 +21,7 @@
 
 #include "batch_plan.cuh"
 
-#if defined(__CUDACC__)
-#define FRZ_OP_HD __host__ __device__ __forceinline__
-#else
-#define FRZ_OP_HD inline
-#endif
+#include "frz_hd.cuh"
 
 // Orders (FRZ_ORDER_*): bit 0 set is ascending attribute order, orders from kFrzOrderScoreFirst on rank by r first.
 constexpr uint32_t kFrzOrderScoreFirst = 2;   // FRZ_ORDER_SCORE_THEN_ATTR_DESC
@@ -72,18 +68,18 @@ struct FrzOrderState {
 // The unsigned key of attribute value v: v ascending (asc) or descending maps to descending keys, and null (INT64_MIN)
 // maps to 0 in both directions.  Every other value maps to 1 .. 2^64 - 1: INT64_MIN + 1 is 1 under DESC, INT64_MAX is 1
 // under ASC.
-FRZ_OP_HD uint64_t frz_order_attr_key(int64_t v, bool asc) {
+FRZ_HD uint64_t frz_order_attr_key(int64_t v, bool asc) {
     const uint64_t u = (uint64_t)v;
     return asc ? (1ull << 63) - u : u ^ (1ull << 63);
 }
 
 // i's value in the attribute
-FRZ_OP_HD int64_t frz_order_value(const int64_t* values, uint64_t n_values, uint32_t index) {
+FRZ_HD int64_t frz_order_value(const int64_t* values, uint64_t n_values, uint32_t index) {
     return index < n_values ? values[index] : (int64_t)(1ull << 63);
 }
 
 // The order key of a row from its parts (boost: boost[index], 0 without one; value: the attribute's value)
-FRZ_OP_HD FrzOrderKey frz_order_key(uint32_t order, bool reversed, uint32_t score, int32_t boost, uint32_t index, int64_t value) {
+FRZ_HD FrzOrderKey frz_order_key(uint32_t order, bool reversed, uint32_t score, int32_t boost, uint32_t index, int64_t value) {
     const uint64_t r = frz_batch_ranked_value(score, boost);
     const uint64_t a = frz_order_attr_key(value, (order & 1u) != 0);
     const uint64_t x = reversed ? index : (uint32_t)~index;
@@ -99,22 +95,22 @@ FRZ_OP_HD FrzOrderKey frz_order_key(uint32_t order, bool reversed, uint32_t scor
 }
 
 // The order key of the list row (index, score) under o
-FRZ_OP_HD FrzOrderKey frz_order_row_key(const FrzOrderDev& o, uint32_t index, uint32_t score) {
+FRZ_HD FrzOrderKey frz_order_row_key(const FrzOrderDev& o, uint32_t index, uint32_t score) {
     const int32_t b = index < o.n_boost ? (int32_t)o.boost[index] : 0;
     return frz_order_key(o.order, o.reversed != 0, score, b, index, frz_order_value(o.values, o.n_values, index));
 }
 
 // a is ahead of b in the call's order
-FRZ_OP_HD bool frz_order_ahead(const FrzOrderKey& a, const FrzOrderKey& b) { return a.hi > b.hi || (a.hi == b.hi && a.lo > b.lo); }
+FRZ_HD bool frz_order_ahead(const FrzOrderKey& a, const FrzOrderKey& b) { return a.hi > b.hi || (a.hi == b.hi && a.lo > b.lo); }
 
 // The digit of key bits [shift, shift + 8), shift a multiple of 8 below 112.
-FRZ_OP_HD uint32_t frz_order_digit(const FrzOrderKey& k, uint32_t shift) {
+FRZ_HD uint32_t frz_order_digit(const FrzOrderKey& k, uint32_t shift) {
     return (uint32_t)((shift >= 48 ? k.hi >> (shift - 48) : k.lo >> shift) & (kFrzOrderBins - 1));
 }
 
 // The digit shifts the select visits, most significant first: those where some key bit varies (vary_*: the bits set in
 // some key and clear in another).  Returns their number (<= kFrzOrderMaxDigits).  The LSD sort visits them in reverse.
-FRZ_OP_HD uint32_t frz_order_digits(uint64_t vary_hi, uint64_t vary_lo, uint32_t* shifts) {
+FRZ_HD uint32_t frz_order_digits(uint64_t vary_hi, uint64_t vary_lo, uint32_t* shifts) {
     uint32_t n = 0;
     const FrzOrderKey v = {vary_hi, vary_lo};
     for (int32_t s = (int32_t)(kFrzOrderKeyBits - kFrzOrderDigitBits); s >= 0; s -= (int32_t)kFrzOrderDigitBits)
@@ -134,7 +130,7 @@ struct FrzOrderPick {
 // or the capacity of a later sort that cuts the selection to its first `need` rows itself: the bucket is then taken whole
 // as soon as the whole selection fits in it, so the select may stop above the need-th key.  Without fit the bucket is
 // taken only when it completes the need exactly, and the select ends with exactly the need rows of largest key.
-FRZ_OP_HD FrzOrderPick frz_order_pick(const uint32_t* hist, uint64_t need, uint64_t n_sel, uint64_t fit) {
+FRZ_HD FrzOrderPick frz_order_pick(const uint32_t* hist, uint64_t need, uint64_t n_sel, uint64_t fit) {
     FrzOrderPick p = {kFrzOrderBins, 1u, 0};
     if (need == 0) return p;
     uint32_t b = kFrzOrderBins - 1;

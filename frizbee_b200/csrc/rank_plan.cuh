@@ -23,11 +23,7 @@
 
 #include "order_plan.cuh"
 
-#if defined(__CUDACC__)
-#define FRZ_RK_HD __host__ __device__ __forceinline__
-#else
-#define FRZ_RK_HD inline
-#endif
+#include "frz_hd.cuh"
 
 constexpr uint32_t kFrzRankMaxKeys = 4;           // FRZ_RANK_MAX_KEYS
 constexpr uint32_t kFrzRankChunkBytes = 7;        // text bytes per chunk
@@ -35,15 +31,15 @@ constexpr uint32_t kFrzRankNone = 0xFFFFFFFFu;    // the segment of a row that i
 constexpr uint32_t kFrzRankOffBits = 24;          // a place in the tuple: key << 24 | byte offset (haystacks < 4 MiB)
 constexpr uint32_t kFrzRankOffMask = (1u << kFrzRankOffBits) - 1;
 
-FRZ_RK_HD uint32_t frz_rank_at(uint32_t key, uint32_t off) { return key << kFrzRankOffBits | off; }
-FRZ_RK_HD uint32_t frz_rank_at_key(uint32_t at) { return at >> kFrzRankOffBits; }
-FRZ_RK_HD uint32_t frz_rank_at_off(uint32_t at) { return at & kFrzRankOffMask; }
+FRZ_HD uint32_t frz_rank_at(uint32_t key, uint32_t off) { return key << kFrzRankOffBits | off; }
+FRZ_HD uint32_t frz_rank_at_key(uint32_t at) { return at >> kFrzRankOffBits; }
+FRZ_HD uint32_t frz_rank_at_off(uint32_t at) { return at & kFrzRankOffMask; }
 
 // byte b as fold_case compares it: A-Z as a-z
-FRZ_RK_HD uint32_t frz_rank_fold_byte(uint32_t b) { return b - 'A' < 26u ? b | 0x20u : b; }
+FRZ_HD uint32_t frz_rank_fold_byte(uint32_t b) { return b - 'A' < 26u ? b | 0x20u : b; }
 
 // the four bytes of x folded at once
-FRZ_RK_HD uint32_t frz_rank_fold4(uint32_t x) {
+FRZ_HD uint32_t frz_rank_fold4(uint32_t x) {
     const uint32_t low7 = x & 0x7F7F7F7Fu;
     const uint32_t ge_a = low7 + 0x3F3F3F3Fu;   // high bit: the low 7 bits are >= 'A'
     const uint32_t gt_z = low7 + 0x25252525u;   // high bit: the low 7 bits are > 'Z'
@@ -51,11 +47,11 @@ FRZ_RK_HD uint32_t frz_rank_fold4(uint32_t x) {
 }
 
 // the chunk of an attribute value
-FRZ_RK_HD uint64_t frz_rank_attr_chunk(int64_t v, bool desc) { return ~frz_order_attr_key(v, !desc); }
+FRZ_HD uint64_t frz_rank_attr_chunk(int64_t v, bool desc) { return ~frz_order_attr_key(v, !desc); }
 
 // The chunk of a text of len bytes at byte offset off (<= len); hay(i) is byte i of the text.
 template <class Hay>
-FRZ_RK_HD uint64_t frz_rank_text_chunk(const Hay& hay, uint32_t len, uint32_t off, bool fold, bool desc) {
+FRZ_HD uint64_t frz_rank_text_chunk(const Hay& hay, uint32_t len, uint32_t off, bool fold, bool desc) {
     const uint32_t left = len - off < kFrzRankChunkBytes ? len - off : kFrzRankChunkBytes;
     uint64_t c = 0;
     for (uint32_t j = 0; j < kFrzRankChunkBytes; j++) {
@@ -67,13 +63,13 @@ FRZ_RK_HD uint64_t frz_rank_text_chunk(const Hay& hay, uint32_t len, uint32_t of
 }
 
 // the key ends with this chunk for every row that has it: an attribute key, or a text that ended inside the chunk
-FRZ_RK_HD bool frz_rank_chunk_ends(uint64_t chunk, bool text, bool desc) {
+FRZ_HD bool frz_rank_chunk_ends(uint64_t chunk, bool text, bool desc) {
     return !text || ((desc ? ~chunk : chunk) & 0xFFu) < kFrzRankChunkBytes;
 }
 
 // The place after a chunk of key tuple place `at` (the segment's key and byte offset, the skipped prefix included) that
 // ends or not, with n_keys keys: false when the tuple is used up, else true and the next place in *next.
-FRZ_RK_HD bool frz_rank_next(uint32_t at, bool ends, uint32_t n_keys, uint32_t* next) {
+FRZ_HD bool frz_rank_next(uint32_t at, bool ends, uint32_t n_keys, uint32_t* next) {
     const uint32_t key = frz_rank_at_key(at);
     if (!ends) {
         *next = at + kFrzRankChunkBytes;
@@ -87,17 +83,17 @@ FRZ_RK_HD bool frz_rank_next(uint32_t at, bool ends, uint32_t n_keys, uint32_t* 
 // The sort key of a round, as an order key (order_plan.cuh) whose DESCENDING order is the ascending order of (seg, chunk):
 // bits [64, 96) hold ~seg and [0, 64) ~chunk; the top 16 bits are zero.  The LSD sort of sort.cu visits only the digits in
 // which two keys differ (frz_order_digits).
-FRZ_RK_HD FrzOrderKey frz_rank_sort_key(uint32_t seg, uint64_t chunk) {
+FRZ_HD FrzOrderKey frz_rank_sort_key(uint32_t seg, uint64_t chunk) {
     const uint64_t c = ~chunk;
     FrzOrderKey k;
     k.hi = (uint64_t)(uint32_t)~seg << 16 | c >> 48;
     k.lo = c & ((1ull << 48) - 1);
     return k;
 }
-FRZ_RK_HD uint32_t frz_rank_key_seg(const FrzOrderKey& k) { return ~(uint32_t)(k.hi >> 16); }
-FRZ_RK_HD bool frz_rank_key_eq(const FrzOrderKey& a, const FrzOrderKey& b) { return a.hi == b.hi && a.lo == b.lo; }
+FRZ_HD uint32_t frz_rank_key_seg(const FrzOrderKey& k) { return ~(uint32_t)(k.hi >> 16); }
+FRZ_HD bool frz_rank_key_eq(const FrzOrderKey& a, const FrzOrderKey& b) { return a.hi == b.hi && a.lo == b.lo; }
 
-FRZ_RK_HD uint32_t frz_rank_ctz(uint32_t x) {
+FRZ_HD uint32_t frz_rank_ctz(uint32_t x) {
 #if defined(__CUDA_ARCH__)
     return __ffs(x) - 1;
 #else
@@ -106,7 +102,7 @@ FRZ_RK_HD uint32_t frz_rank_ctz(uint32_t x) {
 }
 
 // The first byte in which two 16-byte units differ (fold: A-Z as a-z), little-endian words; 16 when none does.
-FRZ_RK_HD uint32_t frz_rank_diff16(const uint32_t* a, const uint32_t* b, bool fold) {
+FRZ_HD uint32_t frz_rank_diff16(const uint32_t* a, const uint32_t* b, bool fold) {
     for (uint32_t w = 0; w < 4; w++) {
         const uint32_t x = fold ? frz_rank_fold4(a[w]) ^ frz_rank_fold4(b[w]) : a[w] ^ b[w];
         if (x) return 4 * w + (frz_rank_ctz(x) >> 3);
@@ -117,7 +113,7 @@ FRZ_RK_HD uint32_t frz_rank_diff16(const uint32_t* a, const uint32_t* b, bool fo
 // The common prefix of two texts of len_a and len_b bytes from byte offset off (<= both lengths), bytes compared as
 // fold says, reading whole 16-byte units: unit(t, u) is unit u of text t (0 or 1) as four little-endian words.
 template <class Unit>
-FRZ_RK_HD uint32_t frz_rank_common(const Unit& unit, uint32_t len_a, uint32_t len_b, uint32_t off, bool fold) {
+FRZ_HD uint32_t frz_rank_common(const Unit& unit, uint32_t len_a, uint32_t len_b, uint32_t off, bool fold) {
     const uint32_t lim = len_a < len_b ? len_a : len_b;
     for (uint32_t u = off >> 4; u * 16 < lim; u++) {
         uint32_t a[4], b[4];

@@ -16,11 +16,7 @@
 
 #include "frz_device.cuh"
 
-#if defined(__CUDACC__)
-#define FRZ_WAVE_FN __host__ __device__ __forceinline__
-#else
-#define FRZ_WAVE_FN inline
-#endif
+#include "frz_hd.cuh"
 
 namespace frzwave {
 
@@ -28,7 +24,7 @@ namespace frzwave {
 struct WaveConst {
     uint32_t gex, gopx, mismatch, case_bonus, delim_bonus, cap_bonus, prefix_bonus, match_x;
 };
-FRZ_WAVE_FN WaveConst wave_const(const FrzPatternDev& p) {
+FRZ_HD WaveConst wave_const(const FrzPatternDev& p) {
     return WaveConst{(uint32_t)p.gap_extend, (uint32_t)p.gap_open_x, (uint32_t)p.mismatch, (uint32_t)p.case_bonus,
                      (uint32_t)p.delim_bonus, (uint32_t)p.cap_bonus, (uint32_t)p.prefix_bonus, (uint32_t)p.match_x};
 }
@@ -52,12 +48,12 @@ struct WaveLane {
     uint32_t hlast_prev;  // last cell of the row before it
 };
 
-FRZ_WAVE_FN uint32_t sat_sub(uint32_t a, uint32_t b) { return a > b ? a - b : 0u; }
+FRZ_HD uint32_t sat_sub(uint32_t a, uint32_t b) { return a > b ? a - b : 0u; }
 
 // columns chunk * L .. chunk * L + L - 1 of a window of W bytes (hay(c) = byte c, read for c < W only); per-column bonus as
 // generic_score computes it
 template <int L, class Hay>
-FRZ_WAVE_FN void lane_load(WaveLane<L>& s, const Hay& hay, int chunk, int W, bool include_prefix, const WaveConst& k) {
+FRZ_HD void lane_load(WaveLane<L>& s, const Hay& hay, int chunk, int W, bool include_prefix, const WaveConst& k) {
 #pragma unroll
     for (int q = 0; q < L / 4; q++) s.hb[q] = 0;
 #pragma unroll
@@ -88,7 +84,7 @@ FRZ_WAVE_FN void lane_load(WaveLane<L>& s, const Hay& hay, int chunk, int W, boo
 
 // what this lane hands its right neighbour after its last row
 template <int L>
-FRZ_WAVE_FN WaveLeft<L> lane_out(const WaveLane<L>& s) {
+FRZ_HD WaveLeft<L> lane_out(const WaveLane<L>& s) {
     WaveLeft<L> o;
 #pragma unroll
     for (int q = 0; q < L / 4; q++) o.hp[q] = s.h[L / 2 + 2 * q] | s.h[L / 2 + 2 * q + 1] << 16;
@@ -97,7 +93,7 @@ FRZ_WAVE_FN WaveLeft<L> lane_out(const WaveLane<L>& s) {
     return o;
 }
 template <int L>
-FRZ_WAVE_FN WaveLeft<L> wave_left_zero() {
+FRZ_HD WaveLeft<L> wave_left_zero() {
     WaveLeft<L> o;
 #pragma unroll
     for (int q = 0; q < L / 4; q++) o.hp[q] = 0;
@@ -108,7 +104,7 @@ FRZ_WAVE_FN WaveLeft<L> wave_left_zero() {
 
 // row i of this lane's chunk, needle byte c / its case flip f
 template <int L>
-FRZ_WAVE_FN void lane_row(WaveLane<L>& s, const WaveLeft<L>& left, uint32_t nc, uint32_t nf, const WaveConst& k) {
+FRZ_HD void lane_row(WaveLane<L>& s, const WaveLeft<L>& left, uint32_t nc, uint32_t nf, const WaveConst& k) {
     uint32_t h[L];
     uint32_t m = 0;
 #pragma unroll
@@ -152,7 +148,7 @@ FRZ_WAVE_FN void lane_row(WaveLane<L>& s, const WaveLeft<L>& left, uint32_t nc, 
 }
 
 template <int L>
-FRZ_WAVE_FN uint32_t lane_max(const WaveLane<L>& s) {
+FRZ_HD uint32_t lane_max(const WaveLane<L>& s) {
     uint32_t mx = 0;
 #pragma unroll
     for (int r = 0; r < L; r++) mx = s.h[r] > mx ? s.h[r] : mx;

@@ -13,11 +13,7 @@
 #pragma once
 #include <stdint.h>
 
-#if defined(__CUDACC__)
-#define FRZ_HD __host__ __device__ __forceinline__
-#else
-#define FRZ_HD inline
-#endif
+#include "frz_hd.cuh"
 
 #define FRZ_U_MAX_SCALARS 64   // needle scalars (needle bytes are capped at 64)
 #define FRZ_U_MAX_LANES 64

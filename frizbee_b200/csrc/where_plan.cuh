@@ -11,11 +11,7 @@
 #pragma once
 #include <stdint.h>
 
-#if defined(__CUDACC__)
-#define FRZ_WP_HD __host__ __device__ __forceinline__
-#else
-#define FRZ_WP_HD inline
-#endif
+#include "frz_hd.cuh"
 
 #include <algorithm>
 #include <vector>
@@ -51,7 +47,7 @@ struct FrzWhereDev {
     uint32_t pad_;
 };
 
-FRZ_WP_HD uint32_t frz_where_popc(uint32_t x) {
+FRZ_HD uint32_t frz_where_popc(uint32_t x) {
 #if defined(__CUDA_ARCH__)
     return __popc(x);
 #else
@@ -60,10 +56,10 @@ FRZ_WP_HD uint32_t frz_where_popc(uint32_t x) {
 }
 
 // i's value in the clause's attribute
-FRZ_WP_HD int64_t frz_where_value(const FrzWhereClauseDev& c, uint64_t i) { return i < c.n_values ? c.values[i] : kFrzAttrNull; }
+FRZ_HD int64_t frz_where_value(const FrzWhereClauseDev& c, uint64_t i) { return i < c.n_values ? c.values[i] : kFrzAttrNull; }
 
 // v is one of set[0 .. n) (sorted, distinct)
-FRZ_WP_HD bool frz_where_in(const int64_t* set, uint32_t n, int64_t v) {
+FRZ_HD bool frz_where_in(const int64_t* set, uint32_t n, int64_t v) {
     uint32_t lo = 0, hi = n;   // the first element >= v is in [lo, hi]
     while (lo < hi) {
         const uint32_t mid = (lo + hi) >> 1;
@@ -74,19 +70,19 @@ FRZ_WP_HD bool frz_where_in(const int64_t* set, uint32_t n, int64_t v) {
 }
 
 // the clause holds for value v (sets: the fill's set values)
-FRZ_WP_HD bool frz_where_holds(const FrzWhereClauseDev& c, const int64_t* sets, int64_t v) {
+FRZ_HD bool frz_where_holds(const FrzWhereClauseDev& c, const int64_t* sets, int64_t v) {
     if (v == kFrzAttrNull) return false;
     const bool t = c.n_in ? frz_where_in(sets + c.in_off, c.n_in, v) : (c.lo <= v && v <= c.hi);
     return t != (c.negate != 0);
 }
 
 // i is below n and, with a base, a member of it (base_word: the base's word i / 32, read only below n_base)
-FRZ_WP_HD bool frz_where_in_base(const FrzWhereDev& w, uint32_t base_word, uint64_t i) {
+FRZ_HD bool frz_where_in_base(const FrzWhereDev& w, uint32_t base_word, uint64_t i) {
     return i < w.n && (!w.has_base || (i < w.n_base && ((base_word >> (i & 31)) & 1u)));
 }
 
 // the members of `word` below bit `bit`: the offset of that bit's member within the word's members
-FRZ_WP_HD uint32_t frz_where_rank(uint32_t word, uint32_t bit) { return frz_where_popc(word & ((1u << bit) - 1u)); }
+FRZ_HD uint32_t frz_where_rank(uint32_t word, uint32_t bit) { return frz_where_popc(word & ((1u << bit) - 1u)); }
 
 // (host) Appends in[0 .. n) sorted and de-duplicated to `sets`; returns how many it appended (their offset is the old size).
 inline uint32_t frz_where_pack_set(const int64_t* in, uint64_t n, std::vector<int64_t>& sets) {

@@ -3,22 +3,16 @@ missing-device status, and frizbee_b200/csrc/batch_collapse_plan.cuh built for t
 batch_collapse_harness.cpp): the budget arithmetic against a numpy restatement, and one sub-batch's slots, shared tables,
 count pass, rounds and keep rule against the specification tests/collapsing.py, query by query."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
 import frizbee_b200 as F
 from collapsing import collapse
+from cpu_harness import load
 from frizbee_b200.types import SortStrategy
 from ranking import rank_by_boost
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CSRC = os.path.join(ROOT, "frizbee_b200", "csrc")
-SRC = os.path.join(ROOT, "tests", "harness", "batch_collapse_harness.cpp")
-LIB = os.path.join(ROOT, "tests", "harness", "libbatch_collapse_harness.so")
-DEPS = [SRC] + [os.path.join(CSRC, h) for h in ("batch_collapse_plan.cuh", "collapse_plan.cuh", "batch_plan.cuh")]
 INVALID, UNSUPPORTED, NO_DEVICE = 1, 9, 8
 U64_MAX = 2**64 - 1
 BY_INDEX, BY_SCORE, BY_KEY = 0, 1, 2
@@ -28,9 +22,7 @@ vp, u64, u32 = C.c_void_p, C.c_uint64, C.c_uint32
 
 @pytest.fixture(scope="module")
 def H():
-    if not os.path.exists(LIB) or any(os.path.getmtime(d) > os.path.getmtime(LIB) for d in DEPS):
-        subprocess.run(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-o", LIB, SRC], check=True)
-    L = C.CDLL(LIB)
+    L = load("batch_collapse_harness")
     L.h_record_bytes.restype = u64
     L.h_collapse_bytes.argtypes = [u64, u64]
     L.h_collapse_bytes.restype = u64

@@ -3,20 +3,14 @@ missing-device status, and frizbee_b200/csrc/batch_columns_plan.cuh built for th
 batch_columns_harness.cpp): random per-column lists folded and compacted as the device does it, against the specification
 tests/columns.py (combine), sums that saturate at 65535 included."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
 import frizbee_b200 as F
 from columns import combine
+from cpu_harness import load
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CSRC = os.path.join(ROOT, "frizbee_b200", "csrc")
-SRC = os.path.join(ROOT, "tests", "harness", "batch_columns_harness.cpp")
-LIB = os.path.join(ROOT, "tests", "harness", "libbatch_columns_harness.so")
-DEPS = [SRC, os.path.join(CSRC, "batch_columns_plan.cuh")]
 INVALID, TOO_MANY_ITEMS, UNSUPPORTED, NO_DEVICE = 1, 4, 9, 8
 U64_MAX = 2**64 - 1
 vp, u64, u32 = C.c_void_p, C.c_uint64, C.c_uint32
@@ -126,9 +120,7 @@ def test_argument_checks_in_order_and_no_device():
 
 @pytest.fixture(scope="module")
 def H():
-    if not os.path.exists(LIB) or any(os.path.getmtime(d) > os.path.getmtime(LIB) for d in DEPS):
-        subprocess.run(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-o", LIB, SRC], check=True)
-    L = C.CDLL(LIB)
+    L = load("batch_columns_harness")
     L.h_columns_bytes.argtypes = [u64, u64, u64]
     L.h_columns_bytes.restype = u64
     L.h_fold.argtypes = [u32, u32, u32, u32]

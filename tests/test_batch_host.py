@@ -2,27 +2,20 @@
 per-query position arithmetic (frizbee_b200/csrc/batch_plan.cuh, built for the CPU from tests/harness/batch_plan_harness.cpp)
 against a numpy restatement of frz_match_list_top for every query of a batch."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
 import frizbee_b200 as F
+from cpu_harness import load
 from frizbee_b200.types import Config, SortStrategy
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SRC = os.path.join(ROOT, "tests", "harness", "batch_plan_harness.cpp")
-LIB = os.path.join(ROOT, "tests", "harness", "libbatch_plan_harness.so")
-DEPS = [SRC, os.path.join(ROOT, "frizbee_b200", "csrc", "batch_plan.cuh")]
 INVALID, NO_DEVICE = 1, 8
 
 
 @pytest.fixture(scope="module")
 def H():
-    if not os.path.exists(LIB) or any(os.path.getmtime(d) > os.path.getmtime(LIB) for d in DEPS):
-        subprocess.run(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-o", LIB, SRC], check=True)
-    L = C.CDLL(LIB)
+    L = load("batch_plan_harness")
     L.h_batch_top.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p]
     L.h_batch_top.restype = None
     return L

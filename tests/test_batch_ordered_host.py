@@ -4,23 +4,16 @@ the budget arithmetic against a numpy restatement, each query's digit sequence, 
 tables, the count pass, the rounds on the order key, the member rule, the select's passes and the sort) against the
 specifications tests/ordering.py and tests/collapsing.py, query by query."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
 import frizbee_b200 as F
 from collapsing import collapse
+from cpu_harness import load
 from frizbee_b200.types import SortStrategy
 from ordering import ATTR_NULL, order_by_attr
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CSRC = os.path.join(ROOT, "frizbee_b200", "csrc")
-SRC = os.path.join(ROOT, "tests", "harness", "batch_order_harness.cpp")
-LIB = os.path.join(ROOT, "tests", "harness", "libbatch_order_harness.so")
-DEPS = [SRC] + [os.path.join(CSRC, h) for h in ("batch_order_plan.cuh", "batch_collapse_plan.cuh", "collapse_plan.cuh", "order_plan.cuh",
-                                                 "batch_plan.cuh")]
 INVALID, UNSUPPORTED, NO_DEVICE = 1, 9, 8
 U64_MAX = 2**64 - 1
 I64_MAX = 2**63 - 1
@@ -31,9 +24,7 @@ vp, u64, u32 = C.c_void_p, C.c_uint64, C.c_uint32
 
 @pytest.fixture(scope="module")
 def H():
-    if not os.path.exists(LIB) or any(os.path.getmtime(d) > os.path.getmtime(LIB) for d in DEPS):
-        subprocess.run(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-o", LIB, SRC], check=True)
-    L = C.CDLL(LIB)
+    L = load("batch_order_harness")
     L.h_sizes.argtypes = [u32]
     L.h_sizes.restype = u64
     L.h_order_bytes.argtypes = [u64, u64]

@@ -3,21 +3,16 @@ frz_groups_destroy / frz_match_list_collapsed and the missing-device status, the
 against a literal per-row loop, and frizbee_b200/csrc/collapse_plan.cuh built for the CPU (tests/harness/
 collapse_harness.cpp): its order keys reproduce L's order, and its count pass, rounds and keep rule reproduce collapse."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
 import frizbee_b200 as F
 from collapsing import GROUP_NONE, collapse
+from cpu_harness import load
 from frizbee_b200.types import SortStrategy
 from ranking import rank_by_boost
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SRC = os.path.join(ROOT, "tests", "harness", "collapse_harness.cpp")
-LIB = os.path.join(ROOT, "tests", "harness", "libcollapse_harness.so")
-DEPS = [SRC, os.path.join(ROOT, "frizbee_b200", "csrc", "collapse_plan.cuh"), os.path.join(ROOT, "frizbee_b200", "csrc", "batch_plan.cuh")]
 INVALID, UNSUPPORTED, NO_DEVICE = 1, 9, 8
 U64_MAX = 2**64 - 1
 BY_INDEX, BY_SCORE, BY_KEY = 0, 1, 2
@@ -26,9 +21,7 @@ vp, u64, u32, u8 = C.c_void_p, C.c_uint64, C.c_uint32, C.c_uint8
 
 @pytest.fixture(scope="module")
 def H():
-    if not os.path.exists(LIB) or any(os.path.getmtime(d) > os.path.getmtime(LIB) for d in DEPS):
-        subprocess.run(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-o", LIB, SRC], check=True)
-    L = C.CDLL(LIB)
+    L = load("collapse_harness")
     L.h_collapse_keys.argtypes = [vp, u64, u8, u8, vp, u64, vp]
     L.h_collapse_keys.restype = None
     L.h_collapse.argtypes = [vp, u64, vp, u64, u64, u32, u8, u8, vp, u64, vp, vp]

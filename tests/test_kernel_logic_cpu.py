@@ -5,33 +5,22 @@ otherwise needed for: every emulated lane width, the column-limited classes (CC 
 the u8 wrap emulation and the shift-placement variants, across the scorings of tests/scorings.py.  k_sw_generic's scorers
 (sw_generic.cuh) are built the same way from tests/harness/sw_generic_harness.cpp."""
 import ctypes as C
-import os
 import random
-import subprocess
 
 import numpy as np
 import pytest
 
 import frizbee_b200 as F
+from cpu_harness import load
 from frizbee_b200.types import CaseMatching, Config, Matching, Scoring, UnicodeMatching
 from needles import case_pairs, case_sensitive, n_distinct, plant
 from oracle import pyoracle as O
 from scorings import scorings
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SRC = os.path.join(ROOT, "tests", "harness", "sw_harness.cpp")
-LIB = os.path.join(ROOT, "tests", "harness", "libsw_harness.so")
-DEPS = [SRC] + [os.path.join(ROOT, "frizbee_b200", "csrc", f) for f in ("sw_core.cuh", "frz_device.cuh")]
-CUDA_INC = "/usr/local/cuda/include"
-
 
 @pytest.fixture(scope="module")
 def H():
-    if not os.path.isdir(CUDA_INC):
-        pytest.skip("CUDA headers not found")
-    if not os.path.exists(LIB) or any(os.path.getmtime(d) > os.path.getmtime(LIB) for d in DEPS):
-        subprocess.run(["g++", "-O1", "-std=c++17", "-I" + CUDA_INC, "-fPIC", "-shared", "-o", LIB, SRC], check=True)
-    L = C.CDLL(LIB)
+    L = load("sw_harness", opt="-O1", cuda_include=True)
     L.h_pattern_size.restype = C.c_size_t
     L.h_swcore.argtypes = [C.c_void_p, C.c_char_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                            C.POINTER(C.c_int)]
@@ -254,18 +243,10 @@ def test_swcore_scoring_sweep(H, lanes):
 
 
 # ---------------------------------------------------------------- k_sw_generic's scorers (sw_generic.cuh)
-G_SRC = os.path.join(ROOT, "tests", "harness", "sw_generic_harness.cpp")
-G_LIB = os.path.join(ROOT, "tests", "harness", "libsw_generic_harness.so")
-G_DEPS = [G_SRC] + [os.path.join(ROOT, "frizbee_b200", "csrc", f) for f in ("sw_generic.cuh", "sw_core.cuh", "frz_device.cuh")]
-
 
 @pytest.fixture(scope="module")
 def G():
-    if not os.path.isdir(CUDA_INC):
-        pytest.skip("CUDA headers not found")
-    if not os.path.exists(G_LIB) or any(os.path.getmtime(d) > os.path.getmtime(G_LIB) for d in G_DEPS):
-        subprocess.run(["g++", "-O2", "-std=c++17", "-I" + CUDA_INC, "-fPIC", "-shared", "-o", G_LIB, G_SRC], check=True)
-    L = C.CDLL(G_LIB)
+    L = load("sw_generic_harness", cuda_include=True)
     L.h_pattern_size.restype = C.c_size_t
     L.h_sw_generic.argtypes = [C.c_void_p, C.c_char_p, C.c_int, C.c_int]
     L.h_greedy.argtypes = [C.c_void_p, C.c_char_p, C.c_int, C.c_int]
@@ -333,18 +314,10 @@ def test_greedy_scorer_across_scorings(H, G):
 
 
 # ---------------------------------------------------------------- occurrence-mask prefilter windows (prefilter_masks.cuh)
-PF_SRC = os.path.join(ROOT, "tests", "harness", "pf_harness.cpp")
-PF_LIB = os.path.join(ROOT, "tests", "harness", "libpf_harness.so")
-PF_DEPS = [PF_SRC] + [os.path.join(ROOT, "frizbee_b200", "csrc", f) for f in ("prefilter_masks.cuh", "frz_device.cuh")]
-
 
 @pytest.fixture(scope="module")
 def PF():
-    if not os.path.isdir(CUDA_INC):
-        pytest.skip("CUDA headers not found")
-    if not os.path.exists(PF_LIB) or any(os.path.getmtime(d) > os.path.getmtime(PF_LIB) for d in PF_DEPS):
-        subprocess.run(["g++", "-O1", "-std=c++17", "-I" + CUDA_INC, "-fPIC", "-shared", "-o", PF_LIB, PF_SRC], check=True)
-    L = C.CDLL(PF_LIB)
+    L = load("pf_harness", opt="-O1", cuda_include=True)
     L.h_masks_window.argtypes = [C.c_void_p, C.c_char_p, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]
     L.h_n_distinct.argtypes = [C.c_void_p]
     return L
@@ -622,18 +595,10 @@ def test_swcore_128_column_classes_groundwork(H, lanes):
 
 
 # ---------------------------------------------------------------- scanning prefilter forms and the literal matcher (prefilter_scan.cuh)
-PS_SRC = os.path.join(ROOT, "tests", "harness", "pf_scan_harness.cpp")
-PS_LIB = os.path.join(ROOT, "tests", "harness", "libpf_scan_harness.so")
-PS_DEPS = [PS_SRC] + [os.path.join(ROOT, "frizbee_b200", "csrc", f) for f in ("prefilter_scan.cuh", "prefilter_masks.cuh", "frz_device.cuh")]
-
 
 @pytest.fixture(scope="module")
 def PS():
-    if not os.path.isdir(CUDA_INC):
-        pytest.skip("CUDA headers not found")
-    if not os.path.exists(PS_LIB) or any(os.path.getmtime(d) > os.path.getmtime(PS_LIB) for d in PS_DEPS):
-        subprocess.run(["g++", "-O2", "-std=c++17", "-I" + CUDA_INC, "-fPIC", "-shared", "-o", PS_LIB, PS_SRC], check=True)
-    L = C.CDLL(PS_LIB)
+    L = load("pf_scan_harness", cuda_include=True)
     ip = C.POINTER(C.c_int)
     L.h_scan_window.argtypes = [C.c_void_p, C.c_char_p, C.c_int, ip, ip]
     L.h_scan_window_long.argtypes = [C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_int, ip, ip]

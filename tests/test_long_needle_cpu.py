@@ -3,32 +3,22 @@ tests/harness/sw_wave_harness.cpp (the wavefront arithmetic of k_sw_long, sw_wav
 view of k_sw_long_thread) against the oracle's score_haystack, and the host-side limits of the byte path (which needles
 compile, and the FRZ_ERR_UNSUPPORTED cases that remain)."""
 import ctypes as C
-import os
 import random
-import subprocess
 
 import pytest
 
 import frizbee_b200 as F
+from cpu_harness import load
 from frizbee_b200.types import CaseMatching, Config, Matching, Pattern, Scoring, UnicodeMatching
 from oracle import pyoracle as O
 from scorings import scorings
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SRC = os.path.join(ROOT, "tests", "harness", "sw_wave_harness.cpp")
-LIB = os.path.join(ROOT, "tests", "harness", "libsw_wave_harness.so")
-DEPS = [SRC] + [os.path.join(ROOT, "frizbee_b200", "csrc", f) for f in ("sw_wave.cuh", "sw_generic.cuh", "sw_core.cuh", "frz_device.cuh")]
-CUDA_INC = "/usr/local/cuda/include"
 UNSUPPORTED = 9   # FRZ_ERR_UNSUPPORTED
 
 
 @pytest.fixture(scope="module")
 def W():
-    if not os.path.isdir(CUDA_INC):
-        pytest.skip("CUDA headers not found")
-    if not os.path.exists(LIB) or any(os.path.getmtime(d) > os.path.getmtime(LIB) for d in DEPS):
-        subprocess.run(["g++", "-O2", "-std=c++17", "-I" + CUDA_INC, "-fPIC", "-shared", "-o", LIB, SRC], check=True)
-    L = C.CDLL(LIB)
+    L = load("sw_wave_harness", cuda_include=True)
     L.h_pattern_size.restype = C.c_size_t
     L.h_sw_wave.argtypes = [C.c_void_p, C.c_char_p, C.c_char_p, C.c_int, C.c_char_p, C.c_int, C.c_int]
     L.h_sw_generic_long.argtypes = L.h_sw_wave.argtypes

@@ -5,27 +5,20 @@ scatter kernel does; both must give the host k-way merge (parallel.merge_runs_ho
 host specification's pos0 (parallel.block_bases).  The 2-GPU tests are the only GPU runs of these forms, so this is their
 check on a machine with fewer GPUs."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
+from cpu_harness import load
 from frizbee_b200 import MATCH_DTYPE, parallel
 from frizbee_b200.types import SortStrategy
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SRC = os.path.join(ROOT, "tests", "harness", "merge_plan_harness.cpp")
-LIB = os.path.join(ROOT, "tests", "harness", "libmerge_plan_harness.so")
-DEPS = [SRC, os.path.join(ROOT, "frizbee_b200", "csrc", "merge_plan.cuh")]
 NO_LIMIT = 2**64 - 1
 
 
 @pytest.fixture(scope="module")
 def H():
-    if not os.path.exists(LIB) or any(os.path.getmtime(d) > os.path.getmtime(LIB) for d in DEPS):
-        subprocess.run(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-o", LIB, SRC], check=True)
-    L = C.CDLL(LIB)
+    L = load("merge_plan_harness")
     vp, u64 = C.c_void_p, C.c_uint64
     L.h_tables.argtypes = [vp, vp, C.c_int, C.c_int, C.c_int, vp]
     L.h_tables.restype = None

@@ -4,23 +4,17 @@ over the rows in a random order, and are compared with the specification collaps
 adversarial lists.  The argument checks of frz_match_list_ordered_collapsed and frz_match_list_columns_ordered run on
 zero-filled stand-in handles.  The behaviour on a real corpus is in tests/test_gpu_ordered_collapsed.py."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
 import frizbee_b200 as F
 from collapsing import GROUP_NONE, collapse
+from cpu_harness import load
 from ordering import ATTR_NULL, order_by_attr
 from ranking import MATCH_DTYPE
 from test_columns_host import _field_offset
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CSRC = os.path.join(ROOT, "frizbee_b200", "csrc")
-SRC = os.path.join(ROOT, "tests", "harness", "ordered_collapse_harness.cpp")
-LIB = os.path.join(ROOT, "tests", "harness", "libordered_collapse_harness.so")
-DEPS = [SRC] + [os.path.join(CSRC, h) for h in ("collapse_plan.cuh", "order_plan.cuh", "batch_plan.cuh")]
 INVALID, TOO_MANY_ITEMS, NO_DEVICE, UNSUPPORTED = 1, 4, 8, 9
 U64_MAX = 2**64 - 1
 I64_MAX = 2**63 - 1
@@ -29,9 +23,7 @@ vp, u64, u32, i32 = C.c_void_p, C.c_uint64, C.c_uint32, C.c_int
 
 @pytest.fixture(scope="module")
 def H():
-    if not os.path.exists(LIB) or any(os.path.getmtime(d) > os.path.getmtime(LIB) for d in DEPS):
-        subprocess.run(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-o", LIB, SRC], check=True)
-    L = C.CDLL(LIB)
+    L = load("ordered_collapse_harness")
     L.h_ordered_collapse.argtypes = [vp, u64, vp, u64, vp, u32, u32, i32, vp, u64, u64, u32, u64, vp, vp]
     L.h_ordered_collapse.restype = C.c_int
     return L

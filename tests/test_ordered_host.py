@@ -3,20 +3,15 @@ The key's descending order is checked against tests/ordering.py's np.lexsort spe
 rows, the keys' uniqueness, and the select's pick rule run pass by pass over random key sets.  The argument checks of the
 call run on zero-filled stand-in handles.  The behaviour on a real corpus is in tests/test_gpu_ordered.py."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
 import frizbee_b200 as F
+from cpu_harness import load
 from ordering import ATTR_NULL, order_by_attr
 from ranking import MATCH_DTYPE
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SRC = os.path.join(ROOT, "tests", "harness", "order_harness.cpp")
-LIB = os.path.join(ROOT, "tests", "harness", "liborder_harness.so")
-DEPS = [SRC, os.path.join(ROOT, "frizbee_b200", "csrc", "order_plan.cuh"), os.path.join(ROOT, "frizbee_b200", "csrc", "batch_plan.cuh")]
 INVALID, NO_DEVICE = 1, 8
 I64_MAX = 2**63 - 1
 BLOCK_ROWS = 4096   # kFrzOrderBlockRows
@@ -25,9 +20,7 @@ vp, u64, u32 = C.c_void_p, C.c_uint64, C.c_uint32
 
 @pytest.fixture(scope="module")
 def H():
-    if not os.path.exists(LIB) or any(os.path.getmtime(d) > os.path.getmtime(LIB) for d in DEPS):
-        subprocess.run(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-o", LIB, SRC], check=True)
-    L = C.CDLL(LIB)
+    L = load("order_harness")
     L.h_order_keys.argtypes = [u32, C.c_int, vp, vp, vp, vp, u64, vp]
     L.h_order_keys.restype = None
     L.h_order_digit.argtypes = [u64, u64, u32]

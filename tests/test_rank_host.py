@@ -4,18 +4,13 @@ argument checks of frz_attr_rank and their order on zero-filled stand-in handles
 tests/test_gpu_rank.py."""
 import ctypes as C
 import functools
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
 import frizbee_b200 as F
+from cpu_harness import load
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SRC = os.path.join(ROOT, "tests", "harness", "rank_harness.cpp")
-LIB = os.path.join(ROOT, "tests", "harness", "librank_harness.so")
-DEPS = [SRC] + [os.path.join(ROOT, "frizbee_b200", "csrc", h) for h in ("rank_plan.cuh", "order_plan.cuh", "batch_plan.cuh")]
 INVALID, UNSUPPORTED, NO_DEVICE = 1, 9, 8
 NULL = -(2**63)
 I64_MAX = 2**63 - 1
@@ -25,9 +20,7 @@ FOLD = bytes(range(65)) + bytes(range(97, 123)) + bytes(range(91, 256))   # A-Z 
 
 @pytest.fixture(scope="module")
 def H():
-    if not os.path.exists(LIB) or any(os.path.getmtime(d) > os.path.getmtime(LIB) for d in DEPS):
-        subprocess.run(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-o", LIB, SRC], check=True)
-    L = C.CDLL(LIB)
+    L = load("rank_harness")
     L.h_rank_text_chunk.argtypes = [C.c_char_p, u32, u32, u32, u32]
     L.h_rank_text_chunk.restype = u64
     L.h_rank_attr_chunk.argtypes = [C.c_int64, u32]

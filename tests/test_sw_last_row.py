@@ -3,22 +3,16 @@ a window with the needle only when the window record says it can be exact (sw.cu
 header's g++ build (tests/harness/sw_harness.cpp) against the oracle, at the needle lengths and gap scorings where the
 last row's gap step matters most; the GPU half puts exact windows through frz_match_list."""
 import ctypes as C
-import os
 import random
-import subprocess
 
 import numpy as np
 import pytest
 
 import frizbee_b200 as F
+from cpu_harness import load
 from frizbee_b200.types import CaseMatching, Config, Scoring
 from oracle import pyoracle as O
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SRC = os.path.join(ROOT, "tests", "harness", "sw_harness.cpp")
-LIB = os.path.join(ROOT, "tests", "harness", "libsw_harness.so")
-DEPS = [SRC] + [os.path.join(ROOT, "frizbee_b200", "csrc", f) for f in ("sw_core.cuh", "frz_device.cuh")]
-CUDA_INC = "/usr/local/cuda/include"
 
 NEEDLES = [b"a", b"Q", b"ab", b"aB", b"deadbeef", b"dEad-bEf"]
 
@@ -38,11 +32,7 @@ def gap_scorings(lanes):
 
 @pytest.fixture(scope="module")
 def H():
-    if not os.path.isdir(CUDA_INC):
-        pytest.skip("CUDA headers not found")
-    if not os.path.exists(LIB) or any(os.path.getmtime(d) > os.path.getmtime(LIB) for d in DEPS):
-        subprocess.run(["g++", "-O1", "-std=c++17", "-I" + CUDA_INC, "-fPIC", "-shared", "-o", LIB, SRC], check=True)
-    L = C.CDLL(LIB)
+    L = load("sw_harness", opt="-O1", cuda_include=True)
     L.h_pattern_size.restype = C.c_size_t
     L.h_swcore.argtypes = [C.c_void_p, C.c_char_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                            C.POINTER(C.c_int)]

@@ -3,31 +3,20 @@ for the CPU (tests/harness/unicode_harness.cpp, g++) and checks them against the
 src/prefilter/algo/unicode*.rs, src/smith_waterman/algo/unicode*.rs and src/literal/algo.rs — no GPU needed.  The
 GPU build of the same code is exercised by tests/test_gpu_parity.py::test_unicode_needle_path."""
 import ctypes as C
-import os
 import random
-import subprocess
 
 import numpy as np
 import pytest
 
+from cpu_harness import load
 from frizbee_b200.types import Scoring
 from oracle import pyoracle as O
 from scorings import scorings
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SRC = os.path.join(ROOT, "tests", "harness", "unicode_harness.cpp")
-LIB = os.path.join(ROOT, "tests", "harness", "libunicode_harness.so")
-DEPS = [SRC, os.path.join(ROOT, "frizbee_b200", "csrc", "unicode_path.cuh"),
-        os.path.join(ROOT, "frizbee_b200", "csrc", "indices_path.cuh"),
-        os.path.join(ROOT, "frizbee_b200", "csrc", "unicode_needle.h"),
-        os.path.join(ROOT, "frizbee_b200", "csrc", "unicode_case.inc")]
-
 
 @pytest.fixture(scope="module")
 def H():
-    if not os.path.exists(LIB) or any(os.path.getmtime(d) > os.path.getmtime(LIB) for d in DEPS):
-        subprocess.run(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-o", LIB, SRC], check=True)
-    L = C.CDLL(LIB)
+    L = load("unicode_harness")
     L.h_prefilter.argtypes = [C.c_char_p, C.c_size_t, C.c_int, C.c_char_p, C.c_int, C.c_int, C.c_int,
                               C.POINTER(C.c_int), C.POINTER(C.c_int)]
     L.h_sw_score.argtypes = [C.c_char_p, C.c_size_t, C.c_int, C.c_void_p, C.c_char_p, C.c_int, C.c_int, C.c_int, C.c_int]

@@ -9,28 +9,18 @@ oracle: the traceback (byte and scalar rows, needles of 1-64 bytes, every typo b
 greedy form past them), the unicode Smith-Waterman score for needles of 6-64 bytes, and the unicode and byte literal
 matchers in all four modes, including which occurrence a substring match picks."""
 import ctypes as C
-import os
 import random
-import subprocess
 
 import numpy as np
 import pytest
 
 import frizbee_b200 as F
+from cpu_harness import load
 from frizbee_b200.types import CaseMatching, Config, Matching, Pattern, Scoring, UnicodeMatching
 from needles import case_pairs
 from oracle import pyoracle as O
 from scorings import TIES, literal_scorings, scorings, unicode_scorings
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-CSRC = os.path.join(ROOT, "frizbee_b200", "csrc")
-U_SRC = os.path.join(ROOT, "tests", "harness", "unicode_harness.cpp")
-U_LIB = os.path.join(ROOT, "tests", "harness", "libunicode_harness.so")
-U_DEPS = [U_SRC] + [os.path.join(CSRC, f) for f in ("unicode_path.cuh", "indices_path.cuh", "unicode_needle.h", "unicode_case.inc")]
-PS_SRC = os.path.join(ROOT, "tests", "harness", "pf_scan_harness.cpp")
-PS_LIB = os.path.join(ROOT, "tests", "harness", "libpf_scan_harness.so")
-PS_DEPS = [PS_SRC] + [os.path.join(CSRC, f) for f in ("prefilter_scan.cuh", "prefilter_masks.cuh", "frz_device.cuh")]
-CUDA_INC = "/usr/local/cuda/include"
 
 U_FIELDS = ("gex", "gopx", "match_x", "mismatch", "case_bonus", "cap_bonus", "delim_bonus", "prefix_bonus")
 RAW_FIELDS = ("raw_match", "raw_gap_open", "raw_gap_extend", "raw_prefix", "raw_cap", "raw_case", "raw_delim", "exact_bonus")
@@ -45,15 +35,9 @@ class UScoring(C.Structure):   # unicode_path.cuh: FrzUScoring
     _fields_ = [(f, C.c_int32) for f in U_FIELDS + RAW_FIELDS]
 
 
-def _stale(lib, deps):
-    return not os.path.exists(lib) or any(os.path.getmtime(d) > os.path.getmtime(lib) for d in deps)
-
-
 @pytest.fixture(scope="module")
 def H():
-    if _stale(U_LIB, U_DEPS):
-        subprocess.run(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-o", U_LIB, U_SRC], check=True)
-    L = C.CDLL(U_LIB)
+    L = load("unicode_harness")
     L.h_uneedle_size.restype = L.h_uscoring_size.restype = C.c_size_t
     assert (L.h_uneedle_size(), L.h_uscoring_size()) == (C.sizeof(UNeedle), C.sizeof(UScoring))
     L.h_build_needle.argtypes = [C.c_char_p, C.c_size_t, C.c_int, C.POINTER(UNeedle)]
@@ -71,11 +55,7 @@ def H():
 
 @pytest.fixture(scope="module")
 def PS():
-    if not os.path.isdir(CUDA_INC):
-        pytest.skip("CUDA headers not found")
-    if _stale(PS_LIB, PS_DEPS):
-        subprocess.run(["g++", "-O2", "-std=c++17", "-I" + CUDA_INC, "-fPIC", "-shared", "-o", PS_LIB, PS_SRC], check=True)
-    L = C.CDLL(PS_LIB)
+    L = load("pf_scan_harness", cuda_include=True)
     L.h_pattern_size.restype = C.c_size_t
     L.h_lit_find.argtypes = [C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_uint32)]
     F.lib().frz_matcher_debug_pattern.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]

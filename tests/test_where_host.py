@@ -3,18 +3,13 @@ against a numpy restatement of the clauses, the set packing and the whole fill (
 expansion), and the argument checks of frz_attr_* / frz_subset_where on zero-filled stand-in handles.  The behaviour on a
 real corpus is in tests/test_gpu_where.py."""
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
 import frizbee_b200 as F
+from cpu_harness import load
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SRC = os.path.join(ROOT, "tests", "harness", "where_harness.cpp")
-LIB = os.path.join(ROOT, "tests", "harness", "libwhere_harness.so")
-DEPS = [SRC, os.path.join(ROOT, "frizbee_b200", "csrc", "where_plan.cuh")]
 INVALID, UNSUPPORTED, NO_DEVICE = 1, 9, 8
 NULL = -(2**63)
 I64_MAX = 2**63 - 1
@@ -34,9 +29,7 @@ class Fill(C.Structure):     # FrzWhereDev
 
 @pytest.fixture(scope="module")
 def H():
-    if not os.path.exists(LIB) or any(os.path.getmtime(d) > os.path.getmtime(LIB) for d in DEPS):
-        subprocess.run(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-o", LIB, SRC], check=True)
-    L = C.CDLL(LIB)
+    L = load("where_harness")
     L.h_where_holds.argtypes = [vp, vp, vp, u64, vp]
     L.h_where_holds.restype = None
     L.h_where_pack.argtypes = [vp, u64, vp]
