@@ -16,7 +16,7 @@ import numpy as np
 from .types import (CaseMatching, CConfig, CMatch, Config, CPattern, Match, Matching, Order, Pattern, Scoring,
                     SortStrategy, UnicodeMatching, as_pattern, pattern_array)
 
-__all__ = ["Matcher", "Corpus", "Subset", "Boost", "Groups", "GROUP_NONE", "Attr", "Where", "ATTR_NULL", "RankKey", "RANK_MAX_KEYS", "Pattern", "Config", "Scoring", "Match", "SortStrategy", "Order", "CaseMatching",
+__all__ = ["Matcher", "Corpus", "Subset", "Boost", "Groups", "GROUP_NONE", "Attr", "Where", "where_batch", "ATTR_NULL", "RankKey", "RANK_MAX_KEYS", "Pattern", "Config", "Scoring", "Match", "SortStrategy", "Order", "CaseMatching",
            "UnicodeMatching", "Matching", "FrizbeeError", "parse_query", "parse_atom", "radix_sort_matches",
            "MATCH_DTYPE", "lib", "lib_path"]
 
@@ -115,6 +115,8 @@ def lib():
     L.frz_attr_destroy.argtypes = [vp]
     L.frz_attr_destroy.restype = None
     L.frz_subset_where.argtypes = [vp, vp, u64, vp]
+    L.frz_subset_where_batch.argtypes = [vp, u64, vp, vp, vp]
+    L.frz_debug_where_batch.argtypes = [C.c_int]
     L.frz_attr_rank.argtypes = [vp, vp, u64]
     L.frz_attr_get.argtypes = [vp, vp, u64]
     L.frz_boost_create.argtypes = [vp, vp, u64, C.POINTER(vp)]
@@ -366,14 +368,8 @@ class Subset:
     def where(self, *clauses: "Where", base: Optional["Subset"] = None) -> "Subset":
         """Refills this subset with the rows of its corpus for which every clause holds and which are members of `base`
         (when given; it may be this subset), on the device (frz_subset_where).  Returns self."""
-        arr = (_CWhereClause * max(1, len(clauses)))()
-        for j, w in enumerate(clauses):
-            arr[j].attr = w.attr._h
-            arr[j].lo, arr[j].hi = w.lo, w.hi
-            arr[j].in_ = w.values.ctypes.data if w.values is not None and w.values.size else None
-            arr[j].n_in = 0 if w.values is None else len(w.values)
-            arr[j].negate = int(w.negate)
-        _check(lib().frz_subset_where(self._h, arr if clauses else None, len(clauses), base._h if base is not None else None))
+        _check(lib().frz_subset_where(self._h, _where_clauses(clauses) if clauses else None, len(clauses),
+                                      base._h if base is not None else None))
         return self
 
     def close(self):
@@ -429,6 +425,18 @@ class Boost(_RowValues):
 class _CWhereClause(C.Structure):
     _fields_ = [("attr", C.c_void_p), ("lo", C.c_int64), ("hi", C.c_int64), ("in_", C.c_void_p), ("n_in", C.c_uint64),
                 ("negate", C.c_int32)]
+
+
+def _where_clauses(clauses):
+    """frz_where_clause records of a sequence of Where (their set values stay owned by the Where objects)."""
+    arr = (_CWhereClause * max(1, len(clauses)))()
+    for j, w in enumerate(clauses):
+        arr[j].attr = w.attr._h
+        arr[j].lo, arr[j].hi = w.lo, w.hi
+        arr[j].in_ = w.values.ctypes.data if w.values is not None and w.values.size else None
+        arr[j].n_in = 0 if w.values is None else len(w.values)
+        arr[j].negate = int(w.negate)
+    return arr
 
 
 class Where:
@@ -856,6 +864,29 @@ def match_list_batch_ordered(matchers, corpus: Corpus, k: int, attrs, order=Orde
     return b.result()
 
 
+def where_batch(subsets, clauses, bases=None):
+    """frz_subset_where_batch: subsets[j].where(*clauses[j], base=bases[j]) for every j in one call, each subset bit for
+    bit what its own call leaves.  subsets: distinct Subset objects of one corpus; clauses: one sequence of Where per
+    subset; bases: None, or one Subset or None per subset (a subset's own handle refines it in place; another query's
+    subset is refused).  Returns subsets."""
+    subsets = list(subsets)
+    clauses = [list(c) for c in clauses]
+    q = len(subsets)
+    if len(clauses) != q:
+        raise ValueError(f"{q} subsets need {q} clause lists, got {len(clauses)}")
+    flat = [w for c in clauses for w in c]
+    counts = np.array([len(c) for c in clauses] or [0], dtype=np.uint64)
+    hs = (C.c_void_p * max(q, 1))(*[s._h.value for s in subsets])
+    hb = None
+    if bases is not None:
+        bases = list(bases)
+        if len(bases) != q:
+            raise ValueError(f"{q} subsets need {q} bases, got {len(bases)}")
+        hb = (C.c_void_p * max(q, 1))(*[b._h.value if b is not None else None for b in bases])
+    _check(lib().frz_subset_where_batch(hs, q, _where_clauses(flat) if flat else None, counts.ctypes.data, hb))
+    return subsets
+
+
 def match_list_columns(matchers, columns, k: Optional[int] = None, sort: SortStrategy = SortStrategy.ScoreThenIndexAsc,
                        subset: Optional[Subset] = None, boost: Optional[Boost] = None, groups: Optional[Groups] = None,
                        per_group: Optional[int] = 1, counts: bool = False, out: Optional[np.ndarray] = None,
@@ -924,6 +955,12 @@ def batch_last() -> dict:
 def batch_limits(max_rows: int = 0, min_queries: int = 0):
     """Test aid (frz_debug_batch_limits): the batched path's corpus-size and query-count limits; 0 restores a default."""
     lib().frz_debug_batch_limits(int(max_rows), int(min_queries))
+
+
+def where_batch_debug(force: Optional[bool] = None) -> bool:
+    """Test aid (frz_debug_where_batch): force=True runs where_batch's batched kernels at every shape, False restores the
+    rule, None changes nothing.  Returns whether this thread's last where_batch ran the batched kernels."""
+    return bool(lib().frz_debug_where_batch(-1 if force is None else int(force)))
 
 
 def radix_sort_matches(arr: np.ndarray, device: int = 0) -> np.ndarray:

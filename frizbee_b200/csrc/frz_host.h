@@ -208,6 +208,8 @@ struct frz_corpus {
     std::unique_ptr<FrzCorpusStorage> edit_tiles;
     // pinned staging of frz_match_list_batch (patterns up, rows and counts down), grow-only
     mutable FrzPinnedArray<uint8_t> batch_stage;
+    // device staging of frz_subset_where_batch (attributes, clauses, queries, set values, member counts), grow-only
+    mutable FrzDevArray<uint8_t> where_stage;
 };
 
 // pack.cu
@@ -484,6 +486,14 @@ struct FrzWhereDev;
 frz_status frz_launch_where(const FrzWhereDev& w, cudaStream_t stream);
 // where.cu: the members of bits[0 .. ceil(n / 32)) in ascending order, chunk c's from members[chunk_base[c]] (k_where_members)
 frz_status frz_launch_where_members(const uint32_t* bits, uint64_t n, const uint64_t* chunk_base, uint32_t* members, cudaStream_t stream);
+// frz_subset_where_batch (host.cu; FrzWhereBatchDev is where_plan.cuh's)
+struct FrzWhereBatchDev;
+struct FrzWhereBatchQuery;
+// where.cu: every query's bits and chunk counts (k_where_batch)
+frz_status frz_launch_where_batch(const FrzWhereBatchDev& b, cudaStream_t stream);
+// where.cu: the member list of every query j with totals[j] > 0 (k_where_members_batch)
+frz_status frz_launch_where_members_batch(const FrzWhereBatchQuery* queries, const unsigned long long* totals, uint64_t n, uint32_t q,
+                                          cudaStream_t stream);
 
 // The ordered call (host.cu, DESIGN.md §4.15; the key and the pick are order_plan.cuh's), all asynchronous on `stream`.
 // order.cu: zero *st, then the key of each of the *n_ptr list rows (n_cap bounds it) → keys, and st's n and bit masks

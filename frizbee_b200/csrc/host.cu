@@ -19,6 +19,8 @@
 #include <memory>
 #include <mutex>
 #include <optional>
+#include <string>
+#include <unordered_map>
 
 #include "batch_collapse_plan.cuh"
 #include "batch_order_plan.cuh"
@@ -979,7 +981,8 @@ __global__ void __launch_bounds__(kCompactBlock) k_retain_scatter(const FrzMatch
     for (uint32_t w = 0; w < warp; w++) pre += wc[w];
     if (k) out[block_base[blockIdx.x] + pre + __popc(b & ((1u << lane) - 1))] = cand[i];
 }
-__global__ void __launch_bounds__(1024) k_scan_blocks(const uint32_t* cnt, uint64_t* base, uint32_t n, FrzCounters* ctr) {
+// The exclusive scan of cnt[0 .. n) into base[0 .. n) by one block of 1024 threads; *total = the sum.
+__device__ __forceinline__ void scan_counts(const uint32_t* cnt, uint64_t* base, uint32_t n, unsigned long long* total) {
     __shared__ uint64_t carry;
     __shared__ uint64_t ws[32];
     if (threadIdx.x == 0) carry = 0;
@@ -1002,7 +1005,14 @@ __global__ void __launch_bounds__(1024) k_scan_blocks(const uint32_t* cnt, uint6
         if (threadIdx.x == blockDim.x - 1) carry = incl;
         __syncthreads();
     }
-    if (threadIdx.x == 0) ctr->total = carry;
+    if (threadIdx.x == 0) *total = carry;
+}
+__global__ void __launch_bounds__(1024) k_scan_blocks(const uint32_t* cnt, uint64_t* base, uint32_t n, FrzCounters* ctr) {
+    scan_counts(cnt, base, n, &ctr->total);
+}
+// k_scan_blocks for frz_subset_where_batch: block j scans query j's n chunk counts; totals[j] = its member count.
+__global__ void __launch_bounds__(1024) k_scan_blocks_batch(const FrzWhereBatchQuery* queries, uint32_t n, unsigned long long* totals) {
+    scan_counts(queries[blockIdx.x].chunk_count, queries[blockIdx.x].chunk_base, n, &totals[blockIdx.x]);
 }
 // Slot metadata of a subset call: slot s keeps its metadata when its haystack, index (s & ~1023) + (meta & 1023), is below
 // n_bits with its bit set in `bits`; every other slot becomes FRZ_INVALID_SLOT, which the matching kernels skip.  Four
@@ -2333,7 +2343,9 @@ frz_status where_fill(frz_subset* s, FrzWhereDev& w, const std::vector<int64_t>&
 }
 }  // namespace
 
-extern "C" frz_status frz_subset_where(frz_subset* s, const frz_where_clause* clauses, uint64_t n_clauses, const frz_subset* base) {
+namespace {
+// frz_subset_where's checks of s and its clauses, in its order, up to the corpus checks
+frz_status where_check_clauses(const frz_subset* s, const frz_where_clause* clauses, uint64_t n_clauses) {
     if (!s || (n_clauses && !clauses)) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
     if (n_clauses > FRZ_WHERE_MAX_CLAUSES)
         return frz_fail(FRZ_ERR_UNSUPPORTED, "%llu clauses (at most %d)", (unsigned long long)n_clauses, FRZ_WHERE_MAX_CLAUSES);
@@ -2347,9 +2359,27 @@ extern "C" frz_status frz_subset_where(frz_subset* s, const frz_where_clause* cl
         for (uint64_t v = 0; v < clauses[j].n_in; v++)
             if (clauses[j].in[v] == FRZ_ATTR_NULL)
                 return frz_fail(FRZ_ERR_INVALID_ARG, "set value %llu of clause %llu is FRZ_ATTR_NULL", (unsigned long long)v, (unsigned long long)j);
+    return FRZ_OK;
+}
+
+// frz_subset_where's corpus checks: every attribute and the base belong to c
+frz_status where_check_corpus(const frz_corpus* c, const frz_where_clause* clauses, uint64_t n_clauses, const frz_subset* base) {
     for (uint64_t j = 0; j < n_clauses; j++)
-        if (clauses[j].attr->corpus != s->corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "the attribute was made on another corpus");
-    if (base && base->corpus != s->corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "the base subset was made on another corpus");
+        if (clauses[j].attr->corpus != c) return frz_fail(FRZ_ERR_INVALID_ARG, "the attribute was made on another corpus");
+    if (base && base->corpus != c) return frz_fail(FRZ_ERR_INVALID_ARG, "the base subset was made on another corpus");
+    return FRZ_OK;
+}
+
+// a refusal of query j of a batched call: its single call's message, prefixed with the query
+frz_status where_query_fail(frz_status st, uint64_t j) {
+    const std::string msg = frz_last_error();
+    return frz_fail(st, "query %llu: %s", (unsigned long long)j, msg.c_str());
+}
+}  // namespace
+
+namespace {
+// frz_subset_where once its arguments have passed and its device is current
+frz_status where_fill_clauses(frz_subset* s, const frz_where_clause* clauses, uint64_t n_clauses, const frz_subset* base) {
     FrzWhereDev w = {};
     std::vector<int64_t> sets;
     for (uint64_t j = 0; j < n_clauses; j++) {
@@ -2364,8 +2394,158 @@ extern "C" frz_status frz_subset_where(frz_subset* s, const frz_where_clause* cl
         d.negate = cl.negate != 0;
     }
     w.n_clauses = (uint32_t)n_clauses;
-    FRZ_TRY(frz_ensure_device(s->corpus->st.device));
     return where_fill(s, w, sets, base);
+}
+}  // namespace
+
+extern "C" frz_status frz_subset_where(frz_subset* s, const frz_where_clause* clauses, uint64_t n_clauses, const frz_subset* base) {
+    FRZ_TRY(where_check_clauses(s, clauses, n_clauses));
+    FRZ_TRY(where_check_corpus(s->corpus, clauses, n_clauses, base));
+    FRZ_TRY(frz_ensure_device(s->corpus->st.device));
+    return where_fill_clauses(s, clauses, n_clauses, base);
+}
+
+namespace {
+// Where the batched kernels beat a loop of single fills (tools/bench_where_batch.py on an H100 80GB HBM3 at 700 W, DESIGN.md
+// §4.14 "Batched fills"): from 2 queries, except 2 queries over more than kWhereBatchPairMaxRows rows (at 10 M rows the
+// loop takes 0.23 ms and the batched kernels 0.26 ms).  One query always runs the single fill.
+constexpr uint64_t kWhereBatchPairMaxRows = 1ull << 22;
+thread_local bool g_where_batch_force = false;   // frz_debug_where_batch: the batched kernels at every q
+thread_local bool g_where_batch_last = false;    // this thread's last frz_subset_where_batch ran the batched kernels
+
+bool where_batch_kernels(uint64_t q, uint64_t n) { return g_where_batch_force || (q >= 2 && (q > 2 || n <= kWhereBatchPairMaxRows)); }
+
+template <typename T>
+T* stage_at(uint8_t* stage, uint64_t off) { return reinterpret_cast<T*>(stage + off); }
+
+// The device work of frz_subset_where_batch once every argument has passed (DESIGN.md §4.14, "Batched fills"): one
+// upload of the plan, k_where_batch, k_scan_blocks_batch, one read-back of the q member counts, one upload of the query
+// table with the member lists' addresses, k_where_members_batch and one synchronise.  Every subset is empty until the
+// call completes.  A bitmap that must grow is written into a new array, because the query's base may be its old one.
+frz_status where_fill_batch(frz_subset* const* s, uint64_t q, const frz_subset* const* bases, FrzWhereBatchPlan& p) {
+    const frz_corpus* corpus = s[0]->corpus;
+    const uint64_t n = corpus->st.n;
+    for (uint64_t j = 0; j < q; j++) {   // (read before the subsets are emptied: a base may be its query's subset)
+        const frz_subset* base = bases ? bases[j] : nullptr;
+        FrzWhereBatchQuery& qr = p.queries[j];
+        qr.has_base = base != nullptr;
+        qr.base = base ? base->bits.get() : nullptr;
+        qr.n_base = base ? base->n_bits : 0;
+    }
+    for (uint64_t j = 0; j < q; j++) {
+        s[j]->n_bits = 0;
+        s[j]->n_members = 0;
+    }
+    if (n == 0) return FRZ_OK;
+    const uint64_t n_words = (n + 31) / 32, n_chunks = (n + kFrzWhereChunk - 1) / kFrzWhereChunk;
+    std::vector<FrzDevArray<uint32_t>> grown(q);
+    for (uint64_t j = 0; j < q; j++) {
+        FRZ_TRY(s[j]->chunk_count.reserve(n_chunks));
+        FRZ_TRY(s[j]->chunk_base.reserve(n_chunks));
+        if (s[j]->bits.cap() < n_words) FRZ_TRY(grown[j].reserve(n_words));
+        FrzWhereBatchQuery& qr = p.queries[j];
+        qr.bits = grown[j].get() ? grown[j].get() : s[j]->bits.get();
+        qr.chunk_count = s[j]->chunk_count.get();
+        qr.chunk_base = s[j]->chunk_base.get();
+    }
+    // the staging: attributes, clauses, queries, set values, then the member counts, each 16-byte aligned
+    auto up16 = [](uint64_t x) { return (x + 15) & ~(uint64_t)15; };
+    const uint64_t o_attrs = 0, o_clauses = up16(o_attrs + p.attrs.size() * sizeof(FrzWhereBatchAttr));
+    const uint64_t o_queries = up16(o_clauses + p.clauses.size() * sizeof(FrzWhereBatchClause));
+    const uint64_t o_sets = up16(o_queries + q * sizeof(FrzWhereBatchQuery));
+    const uint64_t o_totals = up16(o_sets + p.sets.size() * sizeof(int64_t));
+    const uint64_t bytes = o_totals + q * sizeof(unsigned long long);
+    FrzDevArray<uint8_t>& stage = corpus->where_stage;
+    if (stage.cap() < bytes) FRZ_TRY(stage.reserve(bytes, std::max<uint64_t>(4096, bytes + bytes / 2)));
+    std::vector<uint8_t> h(o_totals);
+    memcpy(h.data() + o_attrs, p.attrs.data(), p.attrs.size() * sizeof(FrzWhereBatchAttr));
+    memcpy(h.data() + o_clauses, p.clauses.data(), p.clauses.size() * sizeof(FrzWhereBatchClause));
+    memcpy(h.data() + o_queries, p.queries.data(), q * sizeof(FrzWhereBatchQuery));
+    memcpy(h.data() + o_sets, p.sets.data(), p.sets.size() * sizeof(int64_t));
+    FRZ_CUDA_TRY(cudaMemcpy(stage.get(), h.data(), o_totals, cudaMemcpyHostToDevice));
+    FrzWhereBatchDev b = {};
+    b.attrs = stage_at<FrzWhereBatchAttr>(stage.get(), o_attrs);
+    b.clauses = stage_at<FrzWhereBatchClause>(stage.get(), o_clauses);
+    FrzWhereBatchQuery* d_queries = stage_at<FrzWhereBatchQuery>(stage.get(), o_queries);
+    b.queries = d_queries;
+    b.sets = stage_at<int64_t>(stage.get(), o_sets);
+    b.n = n;
+    b.q = (uint32_t)q;
+    b.n_staged = p.n_staged();
+    unsigned long long* d_totals = stage_at<unsigned long long>(stage.get(), o_totals);
+    FRZ_TRY(frz_launch_where_batch(b, nullptr));
+    k_scan_blocks_batch<<<(unsigned)q, 1024>>>(d_queries, (uint32_t)n_chunks, d_totals);
+    FRZ_CUDA_TRY(cudaGetLastError());
+    std::vector<unsigned long long> totals(q);
+    FRZ_CUDA_TRY(cudaMemcpy(totals.data(), d_totals, q * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+    bool any = false;
+    for (uint64_t j = 0; j < q; j++) {
+        if (grown[j].get()) s[j]->bits = std::move(grown[j]);
+        if (totals[j]) FRZ_TRY(s[j]->members.reserve(totals[j]));
+        p.queries[j].members = s[j]->members.get();
+        any = any || totals[j];
+    }
+    if (any) {
+        FRZ_CUDA_TRY(cudaMemcpy(d_queries, p.queries.data(), q * sizeof(FrzWhereBatchQuery), cudaMemcpyHostToDevice));
+        FRZ_TRY(frz_launch_where_members_batch(d_queries, d_totals, n, (uint32_t)q, nullptr));
+        FRZ_CUDA_TRY(cudaStreamSynchronize(nullptr));
+    }
+    for (uint64_t j = 0; j < q; j++) {
+        s[j]->n_bits = n;
+        s[j]->n_members = totals[j];
+    }
+    return FRZ_OK;
+}
+}  // namespace
+
+extern "C" frz_status frz_subset_where_batch(frz_subset* const* s, uint64_t q, const frz_where_clause* clauses, const uint64_t* n_clauses,
+                                             const frz_subset* const* bases) {
+    if (q && (!s || !n_clauses)) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    uint64_t o = 0;
+    for (uint64_t j = 0; j < q; j++) {   // (n_clauses[j] is at most FRZ_WHERE_MAX_CLAUSES before it moves o)
+        if (const frz_status st = where_check_clauses(s[j], clauses ? clauses + o : nullptr, n_clauses[j])) return where_query_fail(st, j);
+        o += n_clauses[j];
+    }
+    o = 0;
+    for (uint64_t j = 0; j < q; j++) {
+        if (s[j]->corpus != s[0]->corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "query %llu: the subset was made on another corpus", (unsigned long long)j);
+        if (const frz_status st = where_check_corpus(s[0]->corpus, clauses ? clauses + o : nullptr, n_clauses[j], bases ? bases[j] : nullptr))
+            return where_query_fail(st, j);
+        o += n_clauses[j];
+    }
+    std::unordered_map<const frz_subset*, uint64_t> query_of;
+    for (uint64_t j = 0; j < q; j++) {
+        const auto at = query_of.emplace(s[j], j);
+        if (!at.second)
+            return frz_fail(FRZ_ERR_INVALID_ARG, "query %llu: the subset is also query %llu's", (unsigned long long)j, (unsigned long long)at.first->second);
+    }
+    for (uint64_t j = 0; bases && j < q; j++) {
+        const auto at = query_of.find(bases[j]);
+        if (at != query_of.end() && at->second != j)
+            return frz_fail(FRZ_ERR_INVALID_ARG, "query %llu: the base is query %llu's subset", (unsigned long long)j, (unsigned long long)at->second);
+    }
+    if (q == 0) return FRZ_OK;
+    FRZ_TRY(frz_ensure_device(s[0]->corpus->st.device));
+    g_where_batch_last = where_batch_kernels(q, s[0]->corpus->st.n);
+    if (!g_where_batch_last) {   // the single fill, query by query; a failure empties every subset, as the kernels' path does
+        o = 0;
+        for (uint64_t j = 0; j < q; j++) {
+            if (const frz_status st = where_fill_clauses(s[j], clauses ? clauses + o : nullptr, n_clauses[j], bases ? bases[j] : nullptr)) {
+                for (uint64_t i = 0; i < q; i++) s[i]->n_bits = s[i]->n_members = 0;
+                return st;
+            }
+            o += n_clauses[j];
+        }
+        return FRZ_OK;
+    }
+    FrzWhereBatchPlan p;
+    frz_where_batch_pack(clauses, n_clauses, q, [](const frz_attr* a) { return FrzWhereBatchAttr{a->values.get(), a->values.cap()}; }, p);
+    return where_fill_batch(s, q, bases, p);
+}
+
+extern "C" int frz_debug_where_batch(int force) {
+    if (force >= 0) g_where_batch_force = force > 0;
+    return g_where_batch_last;
 }
 
 // ---------------------------------------------------------------------------------- ranks from keys

@@ -287,6 +287,10 @@ FRZ_API void frz_debug_batch_limits(uint64_t max_rows, uint64_t min_queries);
  * call's pipeline),
  * [2] sub-batches run, [3] kernel launches of the batched path.  All zero after a call that ran no sub-batch. */
 FRZ_API void frz_debug_batch_last(uint64_t out[4]);
+/* Test aid: force > 0 makes this thread's frz_subset_where_batch run its batched kernels at every q and corpus length,
+ * force == 0 restores its rule (see frz_subset_where_batch), force < 0 changes nothing.  Returns whether this thread's last
+ * frz_subset_where_batch ran the batched kernels. */
+FRZ_API int frz_debug_where_batch(int force);
 
 /* ---------------------------------------------------------------- subsets
  *
@@ -380,6 +384,28 @@ typedef struct frz_where_clause {
  * to FRZ_ATTR_NULL (FRZ_ERR_INVALID_ARG); an attribute or base of another corpus (FRZ_ERR_INVALID_ARG).  A failure after
  * the checks (out of device memory, for example) leaves s as the empty set, never half-written. */
 FRZ_API frz_status frz_subset_where(frz_subset* s, const frz_where_clause* clauses, uint64_t n_clauses, const frz_subset* base);
+/* The reference has no such method (see above).  frz_subset_where for q subsets of one corpus in one call, as a server
+ * answering many filtered requests at once needs before a batched match call: one upload, one pass over the attribute
+ * values in which each chunk of rows is read once for every query, one read-back of the q member counts and one
+ * synchronise.  Query j's clauses are clauses[o_j .. o_j + n_clauses[j]), o_j being the sum of the earlier n_clauses,
+ * and its base is bases[j] (bases == NULL: no query has a base).  Afterwards each s[j] is bit for bit what
+ * frz_subset_where(s[j], clauses + o_j, n_clauses[j], bases[j]) leaves, for every call that takes a subset.  Every s[j],
+ * attribute and base belongs to s[0]'s corpus.  The s[j] are distinct; bases[j] may be s[j] itself (refining it in
+ * place) or any subset that is not another query's s[i], and several queries may share a base.  The per-query limits
+ * are frz_subset_where's (FRZ_WHERE_MAX_CLAUSES clauses, FRZ_WHERE_MAX_IN set values).  The subsets' device buffers and
+ * the call's staging (kept on the corpus) only grow, so steady-state refills at the same q allocate nothing.  The call
+ * runs its batched kernels from q = 2, except for q = 2 on a corpus of more than 2^22 rows; there, and for q = 1, it
+ * runs frz_subset_where query by query, which measured faster (DESIGN.md §4.14, "Batched fills").  Synchronous; it must not run concurrently with a call that reads any s[j] or base, or with
+ * another frz_subset_where_batch on the same corpus.
+ *
+ * Checked in this order before any device work, leaving every subset as it was: NULL s or n_clauses with q > 0
+ * (FRZ_ERR_INVALID_ARG); query by query, frz_subset_where's checks in its order up to the corpus checks (a NULL s[j], or
+ * NULL clauses with n_clauses[j] > 0, ...); query by query, an s[j], attribute or base of another corpus than s[0]'s
+ * (FRZ_ERR_INVALID_ARG); an s[j] given twice (FRZ_ERR_INVALID_ARG); a bases[j] that is s[i] for some i != j
+ * (FRZ_ERR_INVALID_ARG).  The message names the query.  q == 0 makes no CUDA call.  A failure after the checks (out of
+ * device memory, for example) leaves every s[j] as the empty set. */
+FRZ_API frz_status frz_subset_where_batch(frz_subset* const* s, uint64_t q, const frz_where_clause* clauses,
+                                          const uint64_t* n_clauses, const frz_subset* const* bases);
 
 /* Ranks from several keys.  An order by name, or by a key and then a name, needs a key the caller does not hold: the
  * dense rank of each row's text.  frz_attr_rank fills an attribute on the device with each row's place in a lexicographic
