@@ -16,7 +16,7 @@ import numpy as np
 from .types import (CaseMatching, CConfig, CMatch, Config, CPattern, Match, Matching, Order, Pattern, Scoring,
                     SortStrategy, UnicodeMatching, as_pattern, pattern_array)
 
-__all__ = ["Matcher", "Corpus", "Subset", "Boost", "Groups", "GROUP_NONE", "Attr", "Where", "where_batch", "ATTR_NULL", "RankKey", "RANK_MAX_KEYS", "Pattern", "Config", "Scoring", "Match", "SortStrategy", "Order", "CaseMatching",
+__all__ = ["Matcher", "Corpus", "Subset", "Boost", "Groups", "GROUP_NONE", "Attr", "Where", "where_batch", "BoostRule", "boost_where_batch", "BOOST_MAX_RULES", "ATTR_NULL", "RankKey", "RANK_MAX_KEYS", "Pattern", "Config", "Scoring", "Match", "SortStrategy", "Order", "CaseMatching",
            "UnicodeMatching", "Matching", "FrizbeeError", "parse_query", "parse_atom", "radix_sort_matches",
            "MATCH_DTYPE", "lib", "lib_path"]
 
@@ -24,6 +24,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 GROUP_NONE = 0xFFFFFFFF   # FRZ_GROUP_NONE: a row in no group
 ATTR_NULL = -(2**63)      # FRZ_ATTR_NULL: a row with no value for an attribute
 RANK_MAX_KEYS = 4         # FRZ_RANK_MAX_KEYS: keys of one Corpus.rank / Attr.rank
+BOOST_MAX_RULES = 8       # FRZ_BOOST_MAX_RULES: rules of one Boost.where
 _U64_MAX = 0xFFFFFFFFFFFFFFFF   # UINT64_MAX: no k limit / no per-group cap
 MATCH_DTYPE = np.dtype([("index", "<u4"), ("score", "<u2"), ("exact", "u1"), ("_pad", "u1")])
 
@@ -122,6 +123,9 @@ def lib():
     L.frz_boost_create.argtypes = [vp, vp, u64, C.POINTER(vp)]
     L.frz_boost_set.argtypes = [vp, vp, vp, u64]
     L.frz_boost_destroy.argtypes = [vp]
+    L.frz_boost_get.argtypes = [vp, vp, u64]
+    L.frz_boost_where.argtypes = [vp, vp, u64, vp]
+    L.frz_boost_where_batch.argtypes = [vp, u64, vp, vp, vp]
     L.frz_boost_destroy.restype = None
     L.frz_match_list_ranked.argtypes = [vp, vp, vp, vp, u64, vp, C.POINTER(u64), C.POINTER(u64)]
     L.frz_match_list_ordered.argtypes = [vp, vp, vp, vp, vp, u32, u64, vp, C.POINTER(u64), C.POINTER(u64)]
@@ -421,6 +425,20 @@ class Boost(_RowValues):
         """boost[which[j]] = values[j]; any row below len(corpus), appended ones included, each at most once."""
         return self._set(which, values)
 
+    def where(self, *rules: "BoostRule", base: Optional["Boost"] = None) -> "Boost":
+        """Refills this boost on the device (frz_boost_where): row i's boost becomes base's boost of i (0 without a base;
+        it may be this boost) plus the add of every rule whose clause holds for i, clamped to int16.  At most
+        BOOST_MAX_RULES rules.  Returns self."""
+        _check(lib().frz_boost_where(self._h, _boost_rules(rules) if rules else None, len(rules),
+                                     base._h if base is not None else None))
+        return self
+
+    def values(self) -> np.ndarray:
+        """The boost of every row below len(corpus), 0 where there is none (frz_boost_get)."""
+        out = np.empty(max(1, self.corpus.n), np.int16)
+        _check(lib().frz_boost_get(self._h, out.ctypes.data, self.corpus.n))
+        return out[: self.corpus.n]
+
 
 class _CWhereClause(C.Structure):
     _fields_ = [("attr", C.c_void_p), ("lo", C.c_int64), ("hi", C.c_int64), ("in_", C.c_void_p), ("n_in", C.c_uint64),
@@ -449,6 +467,31 @@ class Where:
 
     def __invert__(self) -> "Where":
         return Where(self.attr, self.lo, self.hi, self.values, not self.negate)
+
+    def add(self, n: int) -> "BoostRule":
+        """The rule of Boost.where that adds n (-65535 .. 65535) to the boost of every row for which this clause holds."""
+        return BoostRule(self, n)
+
+
+class BoostRule:
+    """One rule of Boost.where / boost_where_batch (frz_boost_rule): `add` for every row for which `when` holds."""
+
+    def __init__(self, when: Where, add: int):
+        self.when, self.add = when, int(add)
+
+
+class _CBoostRule(C.Structure):
+    _fields_ = [("when", _CWhereClause), ("add", C.c_int32)]
+
+
+def _boost_rules(rules):
+    """frz_boost_rule records of a sequence of BoostRule (their set values stay owned by the Where objects)."""
+    clauses = _where_clauses([r.when for r in rules])
+    arr = (_CBoostRule * max(1, len(rules)))()
+    for j, r in enumerate(rules):
+        arr[j].when = clauses[j]
+        arr[j].add = r.add
+    return arr
 
 
 class Attr(_RowValues):
@@ -885,6 +928,29 @@ def where_batch(subsets, clauses, bases=None):
         hb = (C.c_void_p * max(q, 1))(*[b._h.value if b is not None else None for b in bases])
     _check(lib().frz_subset_where_batch(hs, q, _where_clauses(flat) if flat else None, counts.ctypes.data, hb))
     return subsets
+
+
+def boost_where_batch(boosts, rules, bases=None):
+    """frz_boost_where_batch: boosts[j].where(*rules[j], base=bases[j]) for every j in one call, each boost bit for bit
+    what its own call leaves (values and key bound).  boosts: distinct Boost objects of one corpus; rules: one sequence of
+    BoostRule per boost; bases: None, or one Boost or None per boost (a boost's own handle adds to it in place; another
+    query's boost is refused).  Returns boosts."""
+    boosts = list(boosts)
+    rules = [list(r) for r in rules]
+    q = len(boosts)
+    if len(rules) != q:
+        raise ValueError(f"{q} boosts need {q} rule lists, got {len(rules)}")
+    flat = [r for rs in rules for r in rs]
+    counts = np.array([len(r) for r in rules] or [0], dtype=np.uint64)
+    hs = (C.c_void_p * max(q, 1))(*[b._h.value for b in boosts])
+    hb = None
+    if bases is not None:
+        bases = list(bases)
+        if len(bases) != q:
+            raise ValueError(f"{q} boosts need {q} bases, got {len(bases)}")
+        hb = (C.c_void_p * max(q, 1))(*[b._h.value if b is not None else None for b in bases])
+    _check(lib().frz_boost_where_batch(hs, q, _boost_rules(flat) if flat else None, counts.ctypes.data, hb))
+    return boosts
 
 
 def match_list_columns(matchers, columns, k: Optional[int] = None, sort: SortStrategy = SortStrategy.ScoreThenIndexAsc,

@@ -495,6 +495,11 @@ frz_status frz_launch_where_batch(const FrzWhereBatchDev& b, cudaStream_t stream
 frz_status frz_launch_where_members_batch(const FrzWhereBatchQuery* queries, const unsigned long long* totals, uint64_t n, uint32_t q,
                                           cudaStream_t stream);
 
+// frz_boost_where and frz_boost_where_batch (host.cu; FrzBoostBatchDev is boost_plan.cuh's)
+struct FrzBoostBatchDev;
+// boost_where.cu: every query's values and b.max (k_boost_where)
+frz_status frz_launch_boost_where(const FrzBoostBatchDev& b, cudaStream_t stream);
+
 // The ordered call (host.cu, DESIGN.md §4.15; the key and the pick are order_plan.cuh's), all asynchronous on `stream`.
 // order.cu: zero *st, then the key of each of the *n_ptr list rows (n_cap bounds it) → keys, and st's n and bit masks
 frz_status frz_launch_order_keys(const FrzMatchDev* list, const unsigned long long* n_ptr, uint64_t n_cap, const FrzOrderDev& o,

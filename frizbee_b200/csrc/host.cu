@@ -33,6 +33,7 @@
 #include "indices_path.cuh"
 #include "rank_plan.cuh"
 #include "where_plan.cuh"
+#include "boost_plan.cuh"
 
 // ------------------------------------------------------------------------------------ errors
 
@@ -2137,6 +2138,8 @@ struct RowValues {
 // A signed 16-bit boost per index (ranked calls); 0 past the values.
 struct frz_boost : RowValues<int16_t, 0> {
     int32_t max_set = 0;   // the largest value ever set, at least 0: bounds every boost (the sort's key bound)
+    // frz_boost_where's grow-only scratch: the plan, the set values and the maxima (of every query when b is a batch's first)
+    FrzDevArray<uint8_t> where_stage;
 };
 // A group id per index (collapsed calls); in no group past the values.
 struct frz_groups : RowValues<uint32_t, FRZ_GROUP_NONE> {
@@ -2236,6 +2239,20 @@ frz_status row_values_set(RowValues<T, kFill>* h, const uint32_t* which, const T
     return FRZ_OK;
 }
 
+// frz_*_get: out[i] = the value of index i for i < n, kFill past the values
+template <typename T, T kFill>
+frz_status row_values_get(const RowValues<T, kFill>* h, T* out, uint64_t n) {
+    if (!h || (n && !out)) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    if (n > h->corpus->st.n)
+        return frz_fail(FRZ_ERR_INVALID_ARG, "%llu values of a corpus of %llu haystacks", (unsigned long long)n, (unsigned long long)h->corpus->st.n);
+    const uint64_t held = std::min<uint64_t>(n, h->values.cap());
+    for (uint64_t i = held; i < n; i++) out[i] = kFill;
+    if (held == 0) return FRZ_OK;
+    FRZ_TRY(frz_ensure_device(h->corpus->st.device));
+    FRZ_CUDA_TRY(cudaMemcpy(out, h->values.get(), held * sizeof(T), cudaMemcpyDeviceToHost));
+    return FRZ_OK;
+}
+
 // every id is below n_groups or FRZ_GROUP_NONE
 frz_status check_group_ids(const uint32_t* ids, uint64_t n, uint64_t n_groups) {
     for (uint64_t j = 0; j < n; j++)
@@ -2258,6 +2275,8 @@ extern "C" frz_status frz_boost_set(frz_boost* b, const uint32_t* which, const i
 }
 
 extern "C" void frz_boost_destroy(frz_boost* b) { delete b; }
+
+extern "C" frz_status frz_boost_get(const frz_boost* b, int16_t* out, uint64_t n) { return row_values_get(b, out, n); }
 
 extern "C" frz_status frz_groups_create(const frz_corpus* c, const uint32_t* ids, uint64_t n, uint64_t n_groups, frz_groups** out) {
     FRZ_TRY(row_values_create(c, ids, n, out, "group ids", [&]() -> frz_status {
@@ -2286,17 +2305,7 @@ extern "C" frz_status frz_attr_set(frz_attr* a, const uint32_t* which, const int
 
 extern "C" void frz_attr_destroy(frz_attr* a) { delete a; }
 
-extern "C" frz_status frz_attr_get(const frz_attr* a, int64_t* out, uint64_t n) {
-    if (!a || (n && !out)) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
-    if (n > a->corpus->st.n)
-        return frz_fail(FRZ_ERR_INVALID_ARG, "%llu values of a corpus of %llu haystacks", (unsigned long long)n, (unsigned long long)a->corpus->st.n);
-    const uint64_t held = std::min<uint64_t>(n, a->values.cap());
-    for (uint64_t i = held; i < n; i++) out[i] = FRZ_ATTR_NULL;
-    if (held == 0) return FRZ_OK;
-    FRZ_TRY(frz_ensure_device(a->corpus->st.device));
-    FRZ_CUDA_TRY(cudaMemcpy(out, a->values.get(), held * sizeof(int64_t), cudaMemcpyDeviceToHost));
-    return FRZ_OK;
-}
+extern "C" frz_status frz_attr_get(const frz_attr* a, int64_t* out, uint64_t n) { return row_values_get(a, out, n); }
 
 // ---------------------------------------------------------------------------------- subsets from attributes
 namespace {
@@ -2546,6 +2555,152 @@ extern "C" frz_status frz_subset_where_batch(frz_subset* const* s, uint64_t q, c
 extern "C" int frz_debug_where_batch(int force) {
     if (force >= 0) g_where_batch_force = force > 0;
     return g_where_batch_last;
+}
+
+// ---------------------------------------------------------------------------------- boosts from attributes
+static_assert(kFrzBoostMaxRules == FRZ_BOOST_MAX_RULES, "boost_plan.cuh mirrors frz_cuda.h");
+
+namespace {
+// frz_boost_where's checks of b and its rules, in its order, up to the corpus checks
+frz_status boost_check_rules(const frz_boost* b, const frz_boost_rule* rules, uint64_t n_rules) {
+    if (!b || (n_rules && !rules)) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    if (n_rules > FRZ_BOOST_MAX_RULES)
+        return frz_fail(FRZ_ERR_UNSUPPORTED, "%llu rules (at most %d)", (unsigned long long)n_rules, FRZ_BOOST_MAX_RULES);
+    for (uint64_t j = 0; j < n_rules; j++)
+        if (!rules[j].when.attr || (rules[j].when.n_in && !rules[j].when.in))
+            return frz_fail(FRZ_ERR_INVALID_ARG, "null argument in rule %llu", (unsigned long long)j);
+    for (uint64_t j = 0; j < n_rules; j++)
+        if (rules[j].add < -kFrzBoostMaxAdd || rules[j].add > kFrzBoostMaxAdd)
+            return frz_fail(FRZ_ERR_INVALID_ARG, "rule %llu adds %d (at most %d either way)", (unsigned long long)j, rules[j].add, kFrzBoostMaxAdd);
+    uint64_t n_in = 0;
+    for (uint64_t j = 0; j < n_rules; j++) n_in += std::min<uint64_t>(rules[j].when.n_in, (uint64_t)FRZ_WHERE_MAX_IN + 1);   // (no overflow)
+    if (n_in > FRZ_WHERE_MAX_IN) return frz_fail(FRZ_ERR_UNSUPPORTED, "more than %d set values", FRZ_WHERE_MAX_IN);
+    for (uint64_t j = 0; j < n_rules; j++)
+        for (uint64_t v = 0; v < rules[j].when.n_in; v++)
+            if (rules[j].when.in[v] == FRZ_ATTR_NULL)
+                return frz_fail(FRZ_ERR_INVALID_ARG, "set value %llu of rule %llu is FRZ_ATTR_NULL", (unsigned long long)v, (unsigned long long)j);
+    return FRZ_OK;
+}
+
+// frz_boost_where's corpus checks: every rule's attribute and the base belong to c
+frz_status boost_check_corpus(const frz_corpus* c, const frz_boost_rule* rules, uint64_t n_rules, const frz_boost* base) {
+    for (uint64_t j = 0; j < n_rules; j++)
+        if (rules[j].when.attr->corpus != c)
+            return frz_fail(FRZ_ERR_INVALID_ARG, "the attribute of rule %llu was made on another corpus", (unsigned long long)j);
+    if (base && base->corpus != c) return frz_fail(FRZ_ERR_INVALID_ARG, "the base boost was made on another corpus");
+    return FRZ_OK;
+}
+
+// The device work of frz_boost_where and frz_boost_where_batch once every argument has passed (DESIGN.md §4.18).  Every
+// value array that must grow to the corpus's length is allocated first, so running out of memory leaves every boost as it
+// was.  Then one upload of the plan (rules, set values, zeroed maxima), k_boost_where, and one read-back of the q maxima,
+// the call's one synchronise.  A grown array replaces the old one only after the read-back, because a query's base may be
+// its boost's old array.  A CUDA failure after the allocations leaves the values of a boost filled in place unspecified and
+// its key bound INT16_MAX, which still bounds every value; a boost whose array grew keeps its values and bound.
+frz_status boost_fill(frz_boost* const* b, uint64_t q, const frz_boost* const* bases, FrzBoostPlan& p) {
+    const uint64_t n = b[0]->corpus->st.n;
+    std::vector<FrzDevArray<int16_t>> grown(q);
+    for (uint64_t j = 0; j < q; j++) {
+        const frz_boost* base = bases ? bases[j] : nullptr;
+        FrzBoostQuery& qr = p.queries[j];
+        qr.base = base ? base->values.get() : nullptr;
+        qr.n_base = base ? std::min<uint64_t>(base->values.cap(), n) : 0;
+        if (b[j]->values.cap() < n) FRZ_TRY(grown[j].reserve(n));
+        qr.out = grown[j].get() ? grown[j].get() : b[j]->values.get();
+    }
+    if (n == 0) {   // (no values to fill: every boost is 0)
+        for (uint64_t j = 0; j < q; j++) b[j]->max_set = 0;
+        return FRZ_OK;
+    }
+    // the staging: attributes, clauses, adds, queries, set values, then the maxima, each 16-byte aligned
+    const FrzWhereBatchPlan& w = p.where;
+    auto up16 = [](uint64_t x) { return (x + 15) & ~(uint64_t)15; };
+    const uint64_t o_attrs = 0, o_clauses = up16(o_attrs + w.attrs.size() * sizeof(FrzWhereBatchAttr));
+    const uint64_t o_adds = up16(o_clauses + w.clauses.size() * sizeof(FrzWhereBatchClause));
+    const uint64_t o_queries = up16(o_adds + p.adds.size() * sizeof(int32_t));
+    const uint64_t o_sets = up16(o_queries + q * sizeof(FrzBoostQuery));
+    const uint64_t o_max = up16(o_sets + w.sets.size() * sizeof(int64_t));
+    const uint64_t bytes = o_max + q * sizeof(int32_t);
+    FrzDevArray<uint8_t>& stage = b[0]->where_stage;
+    if (stage.cap() < bytes) FRZ_TRY(stage.reserve(bytes, std::max<uint64_t>(4096, bytes + bytes / 2)));
+    std::vector<uint8_t> h(bytes, 0);
+    memcpy(h.data() + o_attrs, w.attrs.data(), w.attrs.size() * sizeof(FrzWhereBatchAttr));
+    memcpy(h.data() + o_clauses, w.clauses.data(), w.clauses.size() * sizeof(FrzWhereBatchClause));
+    memcpy(h.data() + o_adds, p.adds.data(), p.adds.size() * sizeof(int32_t));
+    memcpy(h.data() + o_queries, p.queries.data(), q * sizeof(FrzBoostQuery));
+    memcpy(h.data() + o_sets, w.sets.data(), w.sets.size() * sizeof(int64_t));
+    FrzBoostBatchDev d = {};
+    d.attrs = stage_at<FrzWhereBatchAttr>(stage.get(), o_attrs);
+    d.clauses = stage_at<FrzWhereBatchClause>(stage.get(), o_clauses);
+    d.adds = stage_at<int32_t>(stage.get(), o_adds);
+    d.queries = stage_at<FrzBoostQuery>(stage.get(), o_queries);
+    d.sets = stage_at<int64_t>(stage.get(), o_sets);
+    d.max = stage_at<int32_t>(stage.get(), o_max);
+    d.n = n;
+    d.q = (uint32_t)q;
+    d.n_staged = w.n_staged();
+    std::vector<int32_t> maxima(q);
+    const frz_status st = [&]() -> frz_status {
+        FRZ_CUDA_TRY(cudaMemcpy(stage.get(), h.data(), bytes, cudaMemcpyHostToDevice));
+        FRZ_TRY(frz_launch_boost_where(d, nullptr));
+        FRZ_CUDA_TRY(cudaMemcpy(maxima.data(), d.max, q * sizeof(int32_t), cudaMemcpyDeviceToHost));
+        return FRZ_OK;
+    }();
+    if (st != FRZ_OK) {
+        for (uint64_t j = 0; j < q; j++)
+            if (!grown[j].get()) b[j]->max_set = INT16_MAX;
+        return st;
+    }
+    for (uint64_t j = 0; j < q; j++) {
+        if (grown[j].get()) b[j]->values = std::move(grown[j]);
+        b[j]->max_set = maxima[j];
+    }
+    return FRZ_OK;
+}
+
+FrzWhereBatchAttr boost_attr_of(const frz_attr* a) { return FrzWhereBatchAttr{a->values.get(), a->values.cap()}; }
+}  // namespace
+
+extern "C" frz_status frz_boost_where(frz_boost* b, const frz_boost_rule* rules, uint64_t n_rules, const frz_boost* base) {
+    FRZ_TRY(boost_check_rules(b, rules, n_rules));
+    FRZ_TRY(boost_check_corpus(b->corpus, rules, n_rules, base));
+    FRZ_TRY(frz_ensure_device(b->corpus->st.device));
+    FrzBoostPlan p;
+    frz_boost_pack(rules, &n_rules, 1, boost_attr_of, p);
+    return boost_fill(&b, 1, &base, p);
+}
+
+extern "C" frz_status frz_boost_where_batch(frz_boost* const* b, uint64_t q, const frz_boost_rule* rules, const uint64_t* n_rules,
+                                            const frz_boost* const* bases) {
+    if (q && (!b || !n_rules)) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    uint64_t o = 0;
+    for (uint64_t j = 0; j < q; j++) {   // (n_rules[j] is at most FRZ_BOOST_MAX_RULES before it moves o)
+        if (const frz_status st = boost_check_rules(b[j], rules ? rules + o : nullptr, n_rules[j])) return where_query_fail(st, j);
+        o += n_rules[j];
+    }
+    o = 0;
+    for (uint64_t j = 0; j < q; j++) {
+        if (b[j]->corpus != b[0]->corpus) return frz_fail(FRZ_ERR_INVALID_ARG, "query %llu: the boost was made on another corpus", (unsigned long long)j);
+        if (const frz_status st = boost_check_corpus(b[0]->corpus, rules ? rules + o : nullptr, n_rules[j], bases ? bases[j] : nullptr))
+            return where_query_fail(st, j);
+        o += n_rules[j];
+    }
+    std::unordered_map<const frz_boost*, uint64_t> query_of;
+    for (uint64_t j = 0; j < q; j++) {
+        const auto at = query_of.emplace(b[j], j);
+        if (!at.second)
+            return frz_fail(FRZ_ERR_INVALID_ARG, "query %llu: the boost is also query %llu's", (unsigned long long)j, (unsigned long long)at.first->second);
+    }
+    for (uint64_t j = 0; bases && j < q; j++) {
+        const auto at = query_of.find(bases[j]);
+        if (at != query_of.end() && at->second != j)
+            return frz_fail(FRZ_ERR_INVALID_ARG, "query %llu: the base is query %llu's boost", (unsigned long long)j, (unsigned long long)at->second);
+    }
+    if (q == 0) return FRZ_OK;
+    FRZ_TRY(frz_ensure_device(b[0]->corpus->st.device));
+    FrzBoostPlan p;
+    frz_boost_pack(rules, n_rules, q, boost_attr_of, p);
+    return boost_fill(b, q, bases, p);
 }
 
 // ---------------------------------------------------------------------------------- ranks from keys

@@ -464,6 +464,56 @@ FRZ_API frz_status frz_boost_create(const frz_corpus* c, const int16_t* values, 
  * boost as it was.  n == 0 does nothing.  Synchronous; it must not run concurrently with a ranked call reading b. */
 FRZ_API frz_status frz_boost_set(frz_boost* b, const uint32_t* which, const int16_t* values, uint64_t n);
 FRZ_API void frz_boost_destroy(frz_boost* b);
+/* The reference has no such method (see above).  out[i] = boost[i] for i < n (0 where there is none).
+ * n > frz_corpus_len(c), or NULL out with n > 0, is FRZ_ERR_INVALID_ARG.  Synchronous. */
+FRZ_API frz_status frz_boost_get(const frz_boost* b, int16_t* out, uint64_t n);
+
+/* Boosts from attribute rules.  Most priors are relative to the request: "modified in the last hour +30, last day +20",
+ * "in the caller's directory +15", "pinned +50".  frz_boost_where fills a boost on the device from rules over the
+ * resident attributes (frz_attr), each a frz_subset_where clause and the amount it adds, so a ranked call's boost follows
+ * every request without a host pass over the rows or an upload of their values.  A rule whose add is a function of the
+ * value (a linear decay) is a ladder of range rules. */
+#define FRZ_BOOST_MAX_RULES 8
+typedef struct frz_boost_rule {
+    frz_where_clause when;   /* the rule applies to an index for which this clause holds (a null value: never, negated or not) */
+    int32_t add;             /* -65535 .. 65535 */
+} frz_boost_rule;
+/* The reference has no such method (see above).  Let C be b's corpus.  Afterwards, for every index i < frz_corpus_len(C),
+ * removed rows included (boosts are kept by index), boost[i] = clamp(base_i + the sum of the adds of the rules whose clause
+ * holds for i, -32768, 32767), the sum in 32-bit arithmetic (it cannot overflow); base_i is base's boost of i, 0 when base
+ * is NULL.  A clause means what it means in frz_subset_where (range or set, negation, a null value never holds).  base may
+ * be b itself (adding to it in place); n_rules == 0 copies base, or zeroes b without one.  Rows appended later have
+ * boost 0 until the next fill or frz_boost_set, which works on a filled boost as on any other.  b's key bound, which
+ * the ranked calls add to the score bound, becomes max(0, the largest value filled), reduced on the device and read
+ * back exactly.  Synchronous: it returns after that read-back, the call's one synchronise.  It must not run concurrently
+ * with a call that reads b or base.  Its device scratch (the uploaded rules, set values and maxima) stays on b and only
+ * grows, and b's values grow once to C's length, so a steady-state refill allocates nothing.
+ *
+ * Checked in this order before any device work, leaving b as it was: a NULL b, or NULL rules with n_rules > 0
+ * (FRZ_ERR_INVALID_ARG); more than FRZ_BOOST_MAX_RULES rules (FRZ_ERR_UNSUPPORTED); a rule with a NULL attr, or NULL in
+ * with n_in > 0 (FRZ_ERR_INVALID_ARG); a rule's add outside -65535 .. 65535 (FRZ_ERR_INVALID_ARG); more than
+ * FRZ_WHERE_MAX_IN set values in all (FRZ_ERR_UNSUPPORTED); a set value equal to FRZ_ATTR_NULL (FRZ_ERR_INVALID_ARG); an
+ * attribute or base of another corpus (FRZ_ERR_INVALID_ARG).  The message names the rule.  Out of device memory while
+ * growing b's values leaves b as it was.  A CUDA failure after that leaves b's values unspecified and its key bound at
+ * 32767, which still bounds every value. */
+FRZ_API frz_status frz_boost_where(frz_boost* b, const frz_boost_rule* rules, uint64_t n_rules, const frz_boost* base);
+/* The reference has no such method (see above).  frz_boost_where for q boosts of one corpus in one call, as a server
+ * answering many users' "my directory and my recent rows first" requests needs before frz_match_list_batch: one upload,
+ * one pass in which each chunk of each distinct attribute is read once for every query, one read-back of the q key
+ * bounds and one synchronise.  Query j's rules are rules[o_j .. o_j + n_rules[j]), o_j being the sum of the earlier
+ * n_rules, and its base is bases[j] (bases == NULL: no query has a base).  Afterwards each b[j] holds, bit for bit, the
+ * values and key bound that frz_boost_where(b[j], rules + o_j, n_rules[j], bases[j]) leaves.  Every b[j], attribute and
+ * base belongs to b[0]'s corpus.  The b[j] are distinct; bases[j] may be b[j] itself or any boost that is not another
+ * query's b[i], and several queries may share a base.  The per-query limits are frz_boost_where's.  The call's scratch
+ * stays on b[0] and only grows.  Synchronous; it must not run concurrently with a call that reads any b[j] or base.
+ *
+ * Checked in this order before any device work, leaving every boost as it was: NULL b or n_rules with q > 0
+ * (FRZ_ERR_INVALID_ARG); query by query, frz_boost_where's checks in its order up to the corpus checks; query by query, a
+ * b[j], attribute or base of another corpus than b[0]'s (FRZ_ERR_INVALID_ARG); a b[j] given twice (FRZ_ERR_INVALID_ARG);
+ * a bases[j] that is b[i] for some i != j (FRZ_ERR_INVALID_ARG).  The message names the query.  q == 0 makes no CUDA
+ * call.  Failures after the checks leave each b[j] as frz_boost_where's would. */
+FRZ_API frz_status frz_boost_where_batch(frz_boost* const* b, uint64_t q, const frz_boost_rule* rules, const uint64_t* n_rules,
+                                         const frz_boost* const* bases);
 /* The reference has no such method (see above).  The first min(k, total) rows ranked by key; *n_total = total (may be
  * NULL).  s: NULL for the whole corpus, or a subset of the same corpus.  Same rules as frz_match_list_top: `out` is HOST
  * memory with room for k matches (min(k, frz_corpus_len(c)) suffices, or min(k, frz_subset_len(s)) with a subset),
