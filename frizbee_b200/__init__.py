@@ -118,6 +118,9 @@ def lib():
     L.frz_subset_where.argtypes = [vp, vp, u64, vp]
     L.frz_subset_where_batch.argtypes = [vp, u64, vp, vp, vp]
     L.frz_debug_where_batch.argtypes = [C.c_int]
+    L.frz_subset_match.argtypes = [vp, vp, vp, vp]
+    L.frz_debug_subset_match.argtypes = [C.c_int]
+    L.frz_debug_subset_match.restype = u32
     L.frz_attr_rank.argtypes = [vp, vp, u64]
     L.frz_attr_get.argtypes = [vp, vp, u64]
     L.frz_boost_create.argtypes = [vp, vp, u64, C.POINTER(vp)]
@@ -305,6 +308,12 @@ class Corpus:
         the device (frz_subset_where).  Close it before the corpus."""
         return self.subset([]).where(*clauses, base=base)
 
+    def matching(self, matcher: "Matcher", text: Optional["Corpus"] = None, base: Optional["Subset"] = None) -> "Subset":
+        """A new subset of the rows of matcher.match_list_into over `text` (this corpus when None; another corpus must have
+        as many rows), restricted to `base` when given, filled on the device from the prefilter stage alone
+        (frz_subset_match).  Close it before the corpus."""
+        return self.subset([]).matching(matcher, text=text, base=base)
+
     def text(self, desc: bool = False, fold_case: bool = False) -> "RankKey":
         """The rows' haystacks as a key of Corpus.rank / Attr.rank: bytewise (memcmp) order, a proper prefix first; desc
         reverses it, fold_case compares ASCII A-Z as a-z."""
@@ -373,6 +382,16 @@ class Subset:
         """Refills this subset with the rows of its corpus for which every clause holds and which are members of `base`
         (when given; it may be this subset), on the device (frz_subset_where).  Returns self."""
         _check(lib().frz_subset_where(self._h, _where_clauses(clauses) if clauses else None, len(clauses),
+                                      base._h if base is not None else None))
+        return self
+
+    def matching(self, matcher: "Matcher", text: Optional[Corpus] = None, base: Optional["Subset"] = None) -> "Subset":
+        """Refills this subset with the indices of the rows of matcher.match_list_into over `text` (its corpus when None;
+        another corpus must have as many rows) that are members of `base` (when given; it may be this subset), on the
+        device from the prefilter stage alone (frz_subset_match).  For example
+        Matcher.from_query("^src/ .rs$ !test", cfg) keeps the Rust files under src/ outside test paths; the matcher's
+        config decides case, unicode and typos.  Returns self."""
+        _check(lib().frz_subset_match(self._h, matcher._h, text._h if text is not None else None,
                                       base._h if base is not None else None))
         return self
 
@@ -1021,6 +1040,14 @@ def batch_last() -> dict:
 def batch_limits(max_rows: int = 0, min_queries: int = 0):
     """Test aid (frz_debug_batch_limits): the batched path's corpus-size and query-count limits; 0 restores a default."""
     lib().frz_debug_batch_limits(int(max_rows), int(min_queries))
+
+
+def subset_match_debug(force: Optional[str] = None) -> int:
+    """Test aid (frz_debug_subset_match): force="masked" prefilters every pattern of Subset.matching after the first (and
+    the first with a base) through slot metadata masked to the members so far, "full" never does, "rule" restores the
+    rule, None changes nothing.  Returns how many patterns this thread's last fill prefiltered masked."""
+    code = {None: -1, "rule": 0, "masked": 1, "full": 2}[force]
+    return int(lib().frz_debug_subset_match(code))
 
 
 def where_batch_debug(force: Optional[bool] = None) -> bool:

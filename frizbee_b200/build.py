@@ -11,7 +11,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libfrz_cuda.so")
 SOURCES = ["pack.cu", "prefilter.cu", "sw.cu", "sort.cu", "unicode.cu", "host.cu", "merge.cu", "parallel.cu", "batch.cu", "collapse.cu",
-           "batch_columns.cu", "where.cu", "order.cu", "rank.cu", "boost_where.cu"]
+           "batch_columns.cu", "where.cu", "order.cu", "rank.cu", "boost_where.cu",
+           "subset_match.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
          "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr"]

@@ -298,9 +298,10 @@ frz_status frz_launch_prefilter(const FrzCorpusView& cv, const FrzPatternDev& pa
                                 FrzLaunchStats* st, const FrzNeedleTab* ntab = nullptr);
 frz_status frz_launch_sig_scan(const FrzCorpusView& cv, const FrzPatternDev& pat, FrzWorkspace& ws, cudaStream_t stream,
                                FrzLaunchStats* st);
+// member_only: only the survivor bitmap (frz_subset_match): no Smith-Waterman, exact check or survivor records
 frz_status frz_launch_unicode(const FrzCorpusView& cv, const FrzPatternDev& pat, const FrzUNeedle& un, const FrzUScoring& usc,
                               const FrzMatchDev* cand, uint64_t n_cand, uint32_t index_offset, FrzWorkspace& ws,
-                              cudaStream_t stream, FrzLaunchStats* st);
+                              cudaStream_t stream, FrzLaunchStats* st, bool member_only = false);
 frz_status frz_launch_match_indices(const FrzCorpusView& cv, const FrzPatternDev& pat, const FrzUNeedle& un, const FrzUScoring& usc,
                                     bool unicode, const uint32_t* d_which, uint64_t n, FrzMatchDev* d_matches, uint32_t* d_idx,
                                     uint32_t stride, uint32_t* d_cnt, uint16_t* d_scratch, uint64_t scratch_stride, uint32_t threads,
@@ -494,6 +495,11 @@ frz_status frz_launch_where_batch(const FrzWhereBatchDev& b, cudaStream_t stream
 // where.cu: the member list of every query j with totals[j] > 0 (k_where_members_batch)
 frz_status frz_launch_where_members_batch(const FrzWhereBatchQuery* queries, const unsigned long long* totals, uint64_t n, uint32_t q,
                                           cudaStream_t stream);
+
+// frz_subset_match (host.cu; FrzSubsetFoldDev is subset_match_plan.cuh's)
+struct FrzSubsetFoldDev;
+// subset_match.cu: one fold step into f.bits, and the chunk counts when f.chunk_count is set (k_subset_fold)
+frz_status frz_launch_subset_fold(const FrzSubsetFoldDev& f, cudaStream_t stream);
 
 // frz_boost_where and frz_boost_where_batch (host.cu; FrzBoostBatchDev is boost_plan.cuh's)
 struct FrzBoostBatchDev;

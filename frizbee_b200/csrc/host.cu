@@ -34,6 +34,7 @@
 #include "rank_plan.cuh"
 #include "where_plan.cuh"
 #include "boost_plan.cuh"
+#include "subset_match_plan.cuh"
 
 // ------------------------------------------------------------------------------------ errors
 
@@ -1163,6 +1164,26 @@ frz_status shard_call(frz_matcher* m, uint64_t* d_count, cudaStream_t stream, Bo
     return FRZ_OK;
 }
 
+// The prefilter stage of pattern c over cv (cs's view, its slot metadata possibly masked), or over cand_list when given:
+// the workspace sized for cs, the counters zeroed, then the kernels that leave one bit per survivor in ws.surv_bitmap and
+// the survivor records in the lists.  member_only (frz_subset_match): a unicode pattern leaves the bitmap alone.  *ntab:
+// the long needle's table (nullptr for other needles).
+frz_status prefilter_pattern(frz_matcher* m, const FrzCorpusStorage& cs, const FrzCorpusView& cv, const Compiled& c,
+                             uint32_t index_offset, cudaStream_t stream, FrzLaunchStats* st, bool record_events,
+                             const FrzMatchDev* cand_list, uint64_t n_cand, frz_matcher* owner, bool member_only,
+                             const FrzNeedleTab** ntab) {
+    FrzWorkspace& ws = m->ws;
+    uint64_t cap = std::max(ws.survivor_cap(), initial_survivor_cap(cs, c.dev));
+    FRZ_TRY(ensure_workspace(m, cs, cap));
+    FRZ_TRY(needle_table(owner ? owner : m, c, ws.device, ntab));
+    FRZ_CUDA_TRY(cudaMemsetAsync(ws.counters.get(), 0, sizeof(FrzCounters), stream));
+    if (record_events) record_ev(ws, 0, stream);
+    if (c.unicode) FRZ_TRY(frz_launch_unicode(cv, c.dev, c.un, c.usc, cand_list, n_cand, index_offset, ws, stream, st, member_only));
+    else if (cand_list) FRZ_TRY(frz_launch_prefilter_list(cv, c.dev, cand_list, n_cand, index_offset, ws, stream, st, *ntab));
+    else FRZ_TRY(frz_launch_prefilter(cv, c.dev, ws, stream, st, *ntab));
+    return FRZ_OK;
+}
+
 // One pattern over the corpus (optionally restricted to a candidate list) → index-ordered matches in d_out (reversed
 // order if `reversed`); the count is left in ws.counters->total (device).  masked_meta (subset calls): slot metadata to
 // read in place of the corpus's own, nullptr = the corpus's.  owner: the matcher whose pattern c is, when it is not m
@@ -1174,15 +1195,8 @@ frz_status run_pattern(frz_matcher* m, const FrzCorpusStorage& cs, const Compile
     FrzWorkspace& ws = m->ws;
     FrzCorpusView cv = cs.view();
     if (masked_meta) cv.slot_meta = masked_meta;
-    uint64_t cap = std::max(ws.survivor_cap(), initial_survivor_cap(cs, c.dev));
-    FRZ_TRY(ensure_workspace(m, cs, cap));
     const FrzNeedleTab* ntab = nullptr;
-    FRZ_TRY(needle_table(owner ? owner : m, c, ws.device, &ntab));
-    FRZ_CUDA_TRY(cudaMemsetAsync(ws.counters.get(), 0, sizeof(FrzCounters), stream));
-    if (record_events) record_ev(ws, 0, stream);
-    if (c.unicode) FRZ_TRY(frz_launch_unicode(cv, c.dev, c.un, c.usc, cand_list, n_cand, index_offset, ws, stream, st));
-    else if (cand_list) FRZ_TRY(frz_launch_prefilter_list(cv, c.dev, cand_list, n_cand, index_offset, ws, stream, st, ntab));
-    else FRZ_TRY(frz_launch_prefilter(cv, c.dev, ws, stream, st, ntab));
+    FRZ_TRY(prefilter_pattern(m, cs, cv, c, index_offset, stream, st, record_events, cand_list, n_cand, owner, false, &ntab));
     FRZ_TRY(frz_launch_tile_scan(cv, ws, stream, st));
     if (record_events) record_ev(ws, 1, stream);
     // single pattern: every survivor becomes exactly one match, so the scan total is the final count
@@ -2309,33 +2323,23 @@ extern "C" frz_status frz_attr_get(const frz_attr* a, int64_t* out, uint64_t n) 
 
 // ---------------------------------------------------------------------------------- subsets from attributes
 namespace {
-// The device work of frz_subset_where once every argument has passed: k_where writes the bitmap and the chunk counts,
-// k_scan_blocks scans the counts, one 8-byte read-back gives the member count, and k_where_members writes the list.  The
-// bitmap is written in place unless it must grow; then into a new array, because `base` may be s's old bitmap.
-frz_status where_fill(frz_subset* s, FrzWhereDev& w, const std::vector<int64_t>& sets, const frz_subset* base) {
-    const uint64_t n = s->corpus->st.n;
-    w.has_base = base != nullptr;   // (read before s is emptied: base may be s)
-    w.base = base ? base->bits.get() : nullptr;
-    w.n_base = base ? base->n_bits : 0;
-    s->n_bits = 0;   // empty until the fill completes
-    s->n_members = 0;
-    if (n == 0) return FRZ_OK;
+// The start of every subset fill (frz_subset_where, frz_subset_match) over a corpus of n >= 1 rows: s's grow-only scratch
+// for n rows, and *bits, where the fill writes the bitmap: s's own, or `grown` when it must grow (a base may be s's old
+// bitmap, so that one is kept until subset_fill_tail).
+frz_status subset_fill_begin(frz_subset* s, uint64_t n, FrzDevArray<uint32_t>& grown, uint32_t** bits) {
     const uint64_t n_words = (n + 31) / 32, n_chunks = (n + kFrzWhereChunk - 1) / kFrzWhereChunk;
     FRZ_TRY(s->chunk_count.reserve(n_chunks));
     FRZ_TRY(s->chunk_base.reserve(n_chunks));
     FRZ_TRY(s->counters.reserve(1));
-    if (!sets.empty()) {
-        FRZ_TRY(s->sets.reserve(sets.size(), std::max<uint64_t>(sets.size(), 64)));
-        FRZ_CUDA_TRY(cudaMemcpy(s->sets.get(), sets.data(), sets.size() * sizeof(int64_t), cudaMemcpyHostToDevice));
-    }
-    FrzDevArray<uint32_t> grown;
     if (s->bits.cap() < n_words) FRZ_TRY(grown.reserve(n_words));
-    w.sets = s->sets.get();
-    w.n_sets = (uint32_t)sets.size();
-    w.bits = grown.get() ? grown.get() : s->bits.get();
-    w.chunk_count = s->chunk_count.get();
-    w.n = n;
-    FRZ_TRY(frz_launch_where(w, nullptr));
+    *bits = grown.get() ? grown.get() : s->bits.get();
+    return FRZ_OK;
+}
+
+// The end of every subset fill, once its bitmap and chunk counts are written: k_scan_blocks scans the counts, one 8-byte
+// read-back gives the member count, k_where_members writes the list, and s takes the new bitmap.
+frz_status subset_fill_tail(frz_subset* s, uint64_t n, FrzDevArray<uint32_t>& grown) {
+    const uint64_t n_chunks = (n + kFrzWhereChunk - 1) / kFrzWhereChunk;
     k_scan_blocks<<<1, 1024>>>(s->chunk_count.get(), s->chunk_base.get(), (uint32_t)n_chunks, s->counters.get());
     FRZ_CUDA_TRY(cudaGetLastError());
     uint64_t total = 0;
@@ -2349,6 +2353,30 @@ frz_status where_fill(frz_subset* s, FrzWhereDev& w, const std::vector<int64_t>&
     s->n_bits = n;
     s->n_members = total;
     return FRZ_OK;
+}
+
+// The device work of frz_subset_where once every argument has passed: k_where writes the bitmap and the chunk counts, then
+// the common tail.
+frz_status where_fill(frz_subset* s, FrzWhereDev& w, const std::vector<int64_t>& sets, const frz_subset* base) {
+    const uint64_t n = s->corpus->st.n;
+    w.has_base = base != nullptr;   // (read before s is emptied: base may be s)
+    w.base = base ? base->bits.get() : nullptr;
+    w.n_base = base ? base->n_bits : 0;
+    s->n_bits = 0;   // empty until the fill completes
+    s->n_members = 0;
+    if (n == 0) return FRZ_OK;
+    FrzDevArray<uint32_t> grown;
+    FRZ_TRY(subset_fill_begin(s, n, grown, &w.bits));
+    if (!sets.empty()) {
+        FRZ_TRY(s->sets.reserve(sets.size(), std::max<uint64_t>(sets.size(), 64)));
+        FRZ_CUDA_TRY(cudaMemcpy(s->sets.get(), sets.data(), sets.size() * sizeof(int64_t), cudaMemcpyHostToDevice));
+    }
+    w.sets = s->sets.get();
+    w.n_sets = (uint32_t)sets.size();
+    w.chunk_count = s->chunk_count.get();
+    w.n = n;
+    FRZ_TRY(frz_launch_where(w, nullptr));
+    return subset_fill_tail(s, n, grown);
 }
 }  // namespace
 
@@ -2555,6 +2583,92 @@ extern "C" frz_status frz_subset_where_batch(frz_subset* const* s, uint64_t q, c
 extern "C" int frz_debug_where_batch(int force) {
     if (force >= 0) g_where_batch_force = force > 0;
     return g_where_batch_last;
+}
+
+// ---------------------------------------------------------------------------------- subsets from text queries
+namespace {
+thread_local int g_subset_match_force = 0;          // frz_debug_subset_match: 0 the rule, 1 every step masked, 2 none
+thread_local uint32_t g_subset_match_masked = 0;    // the steps of this thread's last frz_subset_match that were masked
+
+// The device work of frz_subset_match once every argument has passed (DESIGN.md §4.19): per step of
+// frz_subset_match_steps, the pattern's prefilter over T (its slot metadata masked to the current members when
+// frz_subset_match_masked says so) and k_subset_fold, then the common tail.  No step reads a survivor list, so a list that
+// overflows changes nothing: every prefilter kernel sets a survivor's bit before it stores the survivor's record.
+frz_status subset_match_fill(frz_subset* s, frz_matcher* m, const FrzCorpusStorage& ts, const frz_subset* base) {
+    const uint64_t n = s->corpus->st.n;
+    const uint32_t* base_bits = base ? base->bits.get() : nullptr;   // (read before s is emptied: base may be s)
+    const uint64_t n_base = base ? base->n_bits : 0;
+    const uint64_t base_members = base ? base->n_members : 0;
+    s->n_bits = 0;
+    s->n_members = 0;
+    g_subset_match_masked = 0;
+    if (n == 0) return FRZ_OK;
+    FrzDevArray<uint32_t> grown;
+    uint32_t* bits = nullptr;
+    FRZ_TRY(subset_fill_begin(s, n, grown, &bits));
+    FrzWorkspace& ws = m->ws;
+    FRZ_TRY(ensure_workspace(m, ts, 1));   // (each pattern's prefilter sizes the survivor lists as a match call does)
+    std::vector<bool> negated;
+    for (const Compiled& c : m->compiled) negated.push_back(c.negated);
+    const std::vector<FrzSubsetMatchStep> steps = frz_subset_match_steps(negated);
+    FrzLaunchStats st;
+    for (size_t k = 0; k < steps.size(); k++) {
+        FrzSubsetFoldDev f = {};
+        f.n = n;
+        f.bits = bits;
+        f.op = steps[k].op;
+        f.chunk_count = k + 1 == steps.size() ? s->chunk_count.get() : nullptr;
+        if (k == 0 && base) {
+            f.has_base = 1;
+            f.base = base_bits;
+            f.n_base = n_base;
+        }
+        if (steps[k].pattern < 0) {   // T's live rows
+            f.slot_meta = ts.slot_meta.get();
+            f.slot_of = ts.slot_of.get();
+        } else {
+            FrzCorpusView cv = ts.view();
+            // the rows that can still be members: the base's before the first step, the subset's own after it
+            const uint32_t* mask = k == 0 ? base_bits : bits;
+            const bool masked = mask && (g_subset_match_force ? g_subset_match_force == 1
+                                                              : frz_subset_match_masked((uint32_t)k, base != nullptr, base_members, n));
+            if (masked) {
+                const uint64_t n_slots = (uint64_t)ts.n_tiles * FRZ_TILE;
+                FRZ_TRY(ws.subset_meta.reserve(n_slots));
+                k_subset_meta<<<grid_for(n_slots / 4, 256), 256>>>(reinterpret_cast<const uint4*>(ts.slot_meta.get()), n_slots / 4, mask,
+                                                                   k == 0 ? n_base : n, reinterpret_cast<uint4*>(ws.subset_meta.get()));
+                FRZ_CUDA_TRY(cudaGetLastError());
+                cv.slot_meta = ws.subset_meta.get();
+                g_subset_match_masked++;
+            }
+            const FrzNeedleTab* ntab = nullptr;
+            FRZ_TRY(prefilter_pattern(m, ts, cv, m->compiled[steps[k].pattern], 0, nullptr, &st, false, nullptr, 0, nullptr, true, &ntab));
+            f.surv = ws.surv_bitmap.get();
+        }
+        FRZ_TRY(frz_launch_subset_fold(f, nullptr));
+    }
+    return subset_fill_tail(s, n, grown);
+}
+}  // namespace
+
+extern "C" frz_status frz_subset_match(frz_subset* s, frz_matcher* m, const frz_corpus* text, const frz_subset* base) {
+    if (!s || !m) return frz_fail(FRZ_ERR_INVALID_ARG, "null argument");
+    const frz_corpus* c = s->corpus;
+    const frz_corpus* t = text ? text : c;
+    if (t->st.device != c->st.device)
+        return frz_fail(FRZ_ERR_INVALID_ARG, "the text corpus is on device %d, the subset's corpus on device %d", t->st.device, c->st.device);
+    if (t->st.n != c->st.n)
+        return frz_fail(FRZ_ERR_INVALID_ARG, "the text corpus holds %llu rows, the subset's corpus %llu: they must share one index space",
+                        (unsigned long long)t->st.n, (unsigned long long)c->st.n);
+    if (base && base->corpus != c) return frz_fail(FRZ_ERR_INVALID_ARG, "the base subset was made on another corpus");
+    FRZ_TRY(frz_check_index_range(c->st.n, 0));
+    FRZ_TRY(frz_ensure_device(c->st.device));
+    return subset_match_fill(s, m, t->st, base);
+}
+
+extern "C" uint32_t frz_debug_subset_match(int force) {
+    if (force >= 0) g_subset_match_force = force;
+    return g_subset_match_masked;
 }
 
 // ---------------------------------------------------------------------------------- boosts from attributes

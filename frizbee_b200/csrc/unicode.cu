@@ -22,6 +22,9 @@ constexpr int kUThreads = 128;
 
 using PackedHay = FrzPackedHay;
 
+// MEMBER_ONLY (frz_subset_match): the survivor bitmap alone, so a candidate stops at the prefilter (or the literal
+// search), with no Smith-Waterman, exact check or survivor record.  k_unicode<false> is the match calls' kernel.
+template <bool MEMBER_ONLY>
 __global__ void __launch_bounds__(kUThreads) k_unicode(const FrzCorpusView cv, const __grid_constant__ FrzPatternDev pat,
                                                        const __grid_constant__ FrzUNeedle un, const FrzUScoring usc,
                                                        const FrzMatchDev* __restrict__ cand, unsigned long long n_cand,
@@ -66,7 +69,7 @@ __global__ void __launch_bounds__(kUThreads) k_unicode(const FrzCorpusView cv, c
         } else if (len >= pat.min_hay_len) {
             int start = 0, end = len;
             ok = frzu::prefilter(un, hay, len, pat.pf_lanes, max_typos, &start, &end);
-            if (ok) {
+            if (ok && !MEMBER_ONLY) {
                 start = start > 0 ? start - 1 : 0;   // trim_haystack (src/matcher/algo.rs:331-338)
                 const int W = end - start;
                 const PackedHay win{hay.base, start};
@@ -77,6 +80,10 @@ __global__ void __launch_bounds__(kUThreads) k_unicode(const FrzCorpusView cv, c
             }
         }
         if (!ok) continue;
+        if (MEMBER_ONLY) {
+            atomicOr(&surv_bitmap[(uint64_t)tile * 32 + (li >> 5)], 1u << (li & 31));
+            continue;
+        }
         FrzSurvivor rec;
         rec.tile = tile;
         rec.slot_rank = slot | (li << 10);
@@ -93,7 +100,7 @@ __global__ void __launch_bounds__(kUThreads) k_unicode(const FrzCorpusView cv, c
 
 frz_status frz_launch_unicode(const FrzCorpusView& cv, const FrzPatternDev& pat, const FrzUNeedle& un, const FrzUScoring& usc,
                               const FrzMatchDev* cand, uint64_t n_cand, uint32_t index_offset, FrzWorkspace& ws,
-                              cudaStream_t stream, FrzLaunchStats* st) {
+                              cudaStream_t stream, FrzLaunchStats* st, bool member_only) {
     if (cv.n_tiles == 0) return FRZ_OK;
     FRZ_CUDA_TRY(cudaMemsetAsync(ws.surv_bitmap.get(), 0, (size_t)cv.n_tiles * 32 * sizeof(uint32_t), stream));
     if (cand && n_cand == 0) return FRZ_OK;
@@ -101,13 +108,20 @@ frz_status frz_launch_unicode(const FrzCorpusView& cv, const FrzPatternDev& pat,
     const int sms = frz_sm_count();
     const uint64_t work = cand ? n_cand : (uint64_t)cv.n_tiles * FRZ_TILE;
     const uint32_t grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)sms * 4, (work + kUThreads - 1) / kUThreads));
+    if (member_only) {   // (no scratch: the Smith-Waterman rows are never touched)
+        k_unicode<true><<<grid, kUThreads, 0, stream>>>(cv, pat, un, usc, cand, n_cand, ws.cand_list.get(), ws.cand_list.cap(), index_offset,
+                                                        ws.lists(), ws.survivor_cap(), ws.surv_bitmap.get(), ws.counters.get(), nullptr, 0);
+        FRZ_CUDA_TRY(cudaGetLastError());
+        if (st) st->launches++;
+        return FRZ_OK;
+    }
     // per-thread Smith-Waterman row state: previous-chunk rows + pending-gap-open vectors of every needle scalar
     const uint32_t stride = 2u * (uint32_t)(un.n + 1) * (uint32_t)pat.sw_lanes;
     const uint64_t need = (uint64_t)grid * kUThreads * stride;
     FRZ_TRY(ws.unicode_scratch.reserve(need));
-    k_unicode<<<grid, kUThreads, 0, stream>>>(cv, pat, un, usc, cand, n_cand, ws.cand_list.get(), ws.cand_list.cap(),
-                                              index_offset, ws.lists(), ws.survivor_cap(),
-                                              ws.surv_bitmap.get(), ws.counters.get(), ws.unicode_scratch.get(), stride);
+    k_unicode<false><<<grid, kUThreads, 0, stream>>>(cv, pat, un, usc, cand, n_cand, ws.cand_list.get(), ws.cand_list.cap(),
+                                                     index_offset, ws.lists(), ws.survivor_cap(),
+                                                     ws.surv_bitmap.get(), ws.counters.get(), ws.unicode_scratch.get(), stride);
     FRZ_CUDA_TRY(cudaGetLastError());
     if (st) st->launches++;
     return FRZ_OK;

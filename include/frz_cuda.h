@@ -407,6 +407,40 @@ FRZ_API frz_status frz_subset_where(frz_subset* s, const frz_where_clause* claus
 FRZ_API frz_status frz_subset_where_batch(frz_subset* const* s, uint64_t q, const frz_where_clause* clauses,
                                           const uint64_t* n_clauses, const frz_subset* const* bases);
 
+/* ---------------------------------------------------------------- subsets from text queries
+ *
+ * A scope on the rows' text that changes with every request: a file picker searched "under src/", "only *.rs" or "not in
+ * node_modules", a shell history searched "commands run under this project".  The reference writes such scopes in its
+ * own query syntax (Pattern::parse_query: ^prefix, suffix$, 'exact, !not, several atoms ANDed), and a haystack is in
+ * Matcher::match_list exactly when the prefilter of every non-negated pattern accepts it and that of no negated pattern
+ * does (src/matcher/algo.rs:85-100, src/matcher/multi.rs:84-152).  frz_subset_match fills an ordinary subset with those
+ * rows on the device, from the prefilter stage alone: no scoring, sorting or copy-out. */
+
+/* The reference has no such method (see above).  Let C be s's corpus and T be `text` (NULL: T = C).  Replaces the contents
+ * of s, which keeps its corpus C: afterwards s holds exactly the indices i < frz_corpus_len(C) that are members of `base`
+ * (when base is not NULL; indices at or beyond its bitmap's length are not members) and that are the index of a row of
+ * frz_match_list_into(m, T, 0).  So T's row i is live, passes every non-negated compiled pattern's length gate and
+ * prefilter and no negated pattern's; the empty matcher matches every live row, and an all-negated matcher every live row
+ * that no pattern matches.  T may be another corpus with the same index space (a column of the same rows, as the text
+ * keys of frz_attr_rank may be): for example a subset of a file-name corpus filled from a query over the directory
+ * corpus.  For every call that takes a subset, the filled s behaves bit for bit like frz_subset_create(C, <those
+ * indices>), and frz_subset_len is their number.  base may be s itself (refining in place).  Synchronous: it returns
+ * after the member count is read back, with one read-back and one synchronise.  It must not run concurrently with another
+ * call on m, or with a call that reads s or base.  s's device buffers only grow, and so does m's workspace, which the
+ * fill uses as a match call does, so a steady-state refill allocates nothing.
+ *
+ * Checked in this order before any device work, leaving s as it was: a NULL s or m (FRZ_ERR_INVALID_ARG); T on another
+ * device than C, or with another frz_corpus_len (FRZ_ERR_INVALID_ARG); a base of another corpus than C
+ * (FRZ_ERR_INVALID_ARG); more rows than u32 indices reach (FRZ_ERR_TOO_MANY_ITEMS); no usable device (FRZ_ERR_NO_DEVICE:
+ * there is no CPU fallback).  A failure after the checks (out of device memory, for example) leaves s as the empty set. */
+FRZ_API frz_status frz_subset_match(frz_subset* s, frz_matcher* m, const frz_corpus* text, const frz_subset* base);
+/* Test aid: force 1 makes this thread's frz_subset_match prefilter every pattern after the first, and the first one when a
+ * base is given, through slot metadata masked to the members so far; force 2 never does; force 0 restores its rule (the
+ * masked form for every pattern after the first, and for the first when the base leaves rows out, DESIGN.md §4.19);
+ * force < 0 changes nothing.  Returns how many patterns this thread's last frz_subset_match prefiltered through masked
+ * metadata. */
+FRZ_API uint32_t frz_debug_subset_match(int force);
+
 /* Ranks from several keys.  An order by name, or by a key and then a name, needs a key the caller does not hold: the
  * dense rank of each row's text.  frz_attr_rank fills an attribute on the device with each row's place in a lexicographic
  * order of up to FRZ_RANK_MAX_KEYS keys, each an attribute or the text of a corpus, so that every call that takes an
